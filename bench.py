@@ -1,12 +1,14 @@
-"""bench.py — agent frames/s of the LAV frame path (BASELINE.json metric) on N B200s.
+"""bench.py — agent frames/s of the LAV frame path (BASELINE.json metric) on N H100s.
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--batch B] [--precision f16|fp32] [--impl ours|reference]
+                    [--dump-outputs DIR]
 
 A "step" = one tick of B independent agents per GPU: 3xRGB 288x256 -> ERFNet -> point painting of a
 40k-point sweep -> stack 3 sweeps (120k pts) -> pillars -> BEV backbone + heads -> detection decode ->
 UniPlanner (ego + K=3 vehicles) -> brake model.  `value` = frames/s with inputs resident in HBM;
 `e2e` = the same through FramePipeline.step with pinned-host inputs (H2D + D2H inside the timed region).
 `--impl reference` times the oracle port of the reference's PyTorch path on the host cores.
+`--dump-outputs DIR` writes what the timed path returned in its last timed step as DIR/<name>.npy (see dump_outputs).
 Under torchrun (N>1) every rank runs its own replica (weak scaling, no data-path collective).
 """
 import argparse
@@ -97,17 +99,8 @@ class ClockSampler:
 
 
 def _reference_frame_fn(device, cores=None):
-    """-> (frame(), kind, description): one whole agent frame through the reference's own implementation.  kind "reference" =
-    the UNMODIFIED reference modules staged in baseline/_ref (oracle/ref_runner.py); "port" = the oracle restatement
-    (oracle/lav_ref.py) when the staged sources are absent."""
-    from oracle import ref_runner as RR
+    """-> (frame(), kind, description): one whole agent frame through the oracle restatement of the reference modules."""
     rgbs, tels, lidars, prev, poses = synth_frames(1)
-    if RR.available():
-        rf = RR.ReferenceFrame(device, FIXED_DETS)
-
-        def frame():
-            return rf(rgbs[0], tels[0], lidars[0], prev[0], poses[0][0], poses[0][1], [0.0, -20.0], 3)[:2]
-        return frame, "reference", "unmodified reference modules (baseline/_ref: team_code_v2 InferModel with jit-scripted backbone/heads, RGBSegmentationModel, RGBBrakePredictionModel) + torch_scatter/carla stand-ins"
     from oracle import lav_ref as O
     _, sds = build_models()
     sd_seg, sd_lid, sd_uni, sd_bra = sds
@@ -163,33 +156,27 @@ def run_reference(args, rank, world, return_outputs=False):
         return out
 
 
-def run_gpu_reference(dev, steps=10, warmup=3):
-    """The north_star's denominator: the reference's own PyTorch-CUDA frame path (team_code_v2 InferModel + seg + brake modules,
-    driven like lav_agent_fast.run_step, batch 1, host sensor tensors in, waypoints + brake read back) on the SAME B200."""
-    from oracle import ref_runner as RR
-    if not RR.available():
-        return {"unavailable": "baseline/_ref not staged (run __graft_entry__.build() where /root/reference exists)"}
-    prev_tf32 = (torch.backends.cudnn.allow_tf32, torch.backends.cuda.matmul.allow_tf32)
-    frame, kind, what = _reference_frame_fn(dev)
-    try:
-        for _ in range(warmup):
-            frame()
-        torch.cuda.synchronize()
-        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        t0 = time.perf_counter()
-        e0.record()
-        for _ in range(steps):
-            out = frame()
-        e1.record()
-        torch.cuda.synchronize()
-        wall = time.perf_counter() - t0
-    finally:
-        torch.backends.cudnn.allow_tf32, torch.backends.cuda.matmul.allow_tf32 = prev_tf32
-    ms = e0.elapsed_time(e1) / steps
-    return {"value": 1e3 / ms, "unit": "frames/s", "ms_per_frame": ms, "wall_ms_per_frame": 1e3 * wall / steps, "batch": 1, "steps": steps,
-            "warmup": warmup, "dtype": "fp32 (PyTorch defaults: cuDNN TF32 convs allowed)", "what": what,
-            "driven_like": "team_code_v2/lav_agent_fast.py:run_step model calls (seg -> paint -> stack -> InferModel pieces -> brake), host tensors in, results read back",
-            "outputs": {"plan0": [float(x) for x in out[0][0]], "brake": float(out[1])}}
+def dump_outputs(outs, d, cap=1 << 20):
+    """Write the last step's outputs (agent groups concatenated) as d/<name>.npy, float32.  Above `cap` elements an output is a
+    seeded sample: d/<name>_sample.npy holds its values at the flat indices stored in d/<name>_index.npy (float64)."""
+    os.makedirs(d, exist_ok=True)
+    arrays = {k: [o[k] for o in outs] for k in ("ego_plan_locs", "ego_cast_locs", "ego_embd", "pred_bra", "pred_bev", "features")}
+    arrays["other_cast_locs"] = [t for o in outs for t in o["other_cast_locs"]]
+    arrays["other_cast_cmds"] = [t for o in outs for t in o["other_cast_cmds"]]
+    for name, parts in arrays.items():
+        total = sum(t.numel() for t in parts)
+        if total <= cap:
+            a = torch.cat([t.reshape(-1) for t in parts]).float().cpu().numpy() if parts else np.zeros(0, np.float32)
+            np.save(os.path.join(d, name + ".npy"), a.reshape((-1,) + tuple(parts[0].shape[1:])) if parts else a)
+            continue
+        idx = np.unique(np.random.default_rng(0).integers(0, total, cap))
+        vals, off = [], 0
+        for t in parts:
+            sel = idx[(idx >= off) & (idx < off + t.numel())] - off
+            vals.append(t.reshape(-1)[torch.from_numpy(sel).to(t.device)].float().cpu())
+            off += t.numel()
+        np.save(os.path.join(d, name + "_sample.npy"), torch.cat(vals).numpy())
+        np.save(os.path.join(d, name + "_index.npy"), idx.astype(np.float64))
 
 
 def workload_config(B, precision, P=1):
@@ -197,7 +184,7 @@ def workload_config(B, precision, P=1):
                         "PointPillars -> BEV backbone + 4 heads -> det decode -> UniPlanner (ego + 3 vehicles) -> brake model",
             "frames_per_step_per_gpu": B, "agent_groups_per_gpu": P, "precision": precision, "weights": "seeded random init (released .th files are LFS pointers)",
             "planner_detections": "decode runs on the predicted maps; planner is fed a fixed K=3 list (SURVEY 8d)",
-            "l2": "per-step working set (B x 26 MB canvas + B x 39 MB features + ...) exceeds the 126 MB L2; inputs rotate over 2 sets",
+            "l2": "per-step working set (B x 26 MB canvas + B x 39 MB features + ...) exceeds the 50 MB L2; inputs rotate over 2 sets",
             "parallelism": "replicas (one process per GPU, no data-path collective)",
             "execution": "two CUDA graphs per step (perception+heads+brake; planner), host decode of detections in between; e2e: each step's pinned host inputs go through a copy stream into staging buffers (H2D inside the timed region, overlapping the other agent group's kernels), results read back every step"}
 
@@ -311,7 +298,7 @@ def main():
     ap.add_argument("--pipelines", type=int, default=2, help="agent groups per GPU that overlap host decode with GPU work")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-graphs", action="store_true", help="run the static pipeline eagerly (debug / ncu launch lists)")
-    ap.add_argument("--no-gpu-reference", action="store_true", help="skip the reference-modules-on-this-GPU leg and the batch-1 latency leg")
+    ap.add_argument("--no-gpu-reference", action="store_true", help="skip the batch-1 latency leg")
     ap.add_argument("--vary-k", action="store_true", help="planner fed a different number of vehicles every step (0..15 per frame) instead of the fixed K=3")
     ap.add_argument("--no-train", action="store_true", help="skip the train_lidar leg (BASELINE config 4)")
     ap.add_argument("--train-batch", type=int, default=32, help="train_lidar samples per rank (reference default 32; 8 ranks = 256)")
@@ -319,6 +306,7 @@ def main():
     ap.add_argument("--train-warmup", type=int, default=3)
     ap.add_argument("--train-amp", action="store_true", default=False, help="bf16 autocast for the training leg (opt-in)")
     ap.add_argument("--train-amp-leg", action="store_true", help="also run the training step with bf16 autocast and report it beside the fp32 one")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write the outputs of the last timed step as DIR/<name>.npy")
     args = ap.parse_args()
     rank, world, local = int(os.environ.get("RANK", 0)), int(os.environ.get("WORLD_SIZE", 1)), int(os.environ.get("LOCAL_RANK", 0))
 
@@ -330,7 +318,7 @@ def main():
     from lav_b200 import capi, ops, synth
     from lav_b200.agent import StaticFramePipeline
     capi.lib()
-    torch.backends.cudnn.benchmark = bool(int(os.environ.get("LAVB_CUDNN_BENCHMARK", "0")))   # cuDNN autotune measured slower here (1863 vs 1987 frames/s): off
+    torch.backends.cudnn.benchmark = bool(int(os.environ.get("LAVB_CUDNN_BENCHMARK", "0")))   # cuDNN autotune: off unless asked for
     torch.cuda.set_device(local)
     dev = torch.device("cuda", local)
     if world > 1:
@@ -371,8 +359,11 @@ def main():
 
     vary_k_state = [0]
 
+    last_out = [None]
+
     def step_resident(i):
-        return run(*d_sets[i % 2])
+        last_out[0] = run(*d_sets[i % 2])
+        return last_out[0]
 
     # e2e: host (pinned) inputs in, results out, every step.  The D2H read of step i is queued behind its planner graph
     # on the group's own stream and consumed on the host while step i+1 is already running (one step of latency, every
@@ -444,10 +435,12 @@ def main():
     launches = args.steps * sum(sum(pp._launches[:2]) for pp in pipes)
     _dbg(f"timed resident loop done: {ms / args.steps:.2f} ms/step")
     clocks = sampler.stop(t0, t1) if sampler else None
+    if args.dump_outputs:
+        dump_outputs(last_out[0], args.dump_outputs)
     ms_e2e, _, _ = timed(step_e2e, args.steps, max(3, args.warmup // 2), fin=drain)
 
     _dbg(f"e2e loop done: {ms_e2e / args.steps:.2f} ms/step")
-    # roofline of the dominant kernel (tcgen05 conv), timed per launch with CUDA events on the launch stream.
+    # roofline of the dominant kernel (wgmma conv), timed per launch with CUDA events on the launch stream.
     # Events cannot be recorded inside a captured graph, so this pass runs the same G1 body eagerly.
     ops.PROFILE = []
     for i in range(max(2, args.steps // 4)):
@@ -460,12 +453,7 @@ def main():
         peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
     except OSError:
         pass
-    src = "MEASURED_PEAKS.json" if peaks else "fallback (B200_PROFILING.md)"
-    traffic = {}      # dram__bytes_read+write per launch from committed ncu captures AT THE BENCH BATCH (scripts/ncu_traffic.sh);
-    try:              # used only when the capture's frames-per-launch equals this run's, else `traffic` stays null
-        traffic = json.load(open(os.path.join(ROOT, "profiles", "r02_traffic.json")))
-    except OSError:
-        pass
+    src = "MEASURED_PEAKS.json" if peaks else "fallback (H100 SXM data sheet, dense)"
 
     def entry(rows, bound, unit, peak, scale):
         work, tms = sum(r[0] for r in rows), sum(r[1] for r in rows)
@@ -477,36 +465,22 @@ def main():
         if k.startswith("umma:"):
             umma.setdefault(k[5:], []).append((w, a.elapsed_time(b)))
     if umma:
-        tf_peak = peaks.get("bf16_tflops_sustained", 1400.0)
+        tf_peak = peaks.get("bf16_tflops_sustained", 989.0)
         # headline: conv_umma_kernel over ALL its launches of a tick (ERFNet, backbone, heads: ~110 launches, 9 shapes)
         roof["umma"] = entry([r for v in umma.values() for r in v], "tensor", "TFLOP/s", tf_peak, 1e12)
         roof["umma"]["kernel"] = "conv_umma_kernel (all launches of a tick)"
-        tr_ = traffic.get("umma_tick", {})
-        if tr_.get("frames") == Bp and tr_.get("launches"):       # per launch, like `achieved`: DRAM bytes of the tick's launches / their number
-            roof["umma"]["traffic"] = tr_["dram_bytes"] / tr_["launches"]
-            roof["umma"]["traffic_source"] = tr_.get("source")
-        # its largest single launch, the fused 4-head conv 384->256: DRAM bytes from the committed ncu --set full
-        # capture (profiles/r01_kernels.md §1: 225.5 MB for 8 frames, tensor pipe 83.7 %), scaled to the frames per launch
+        # its largest single launch, the fused 4-head conv 384->256
         hk = [k for k in umma if k.startswith("384->256")]
         if hk:
             # a ~1 ms launch with other kernels between its repeats: the BURST cuBLAS figure is the fair denominator
             # (against the sustained one this launch reads > 1.0); the all-launch aggregate above uses the sustained peak
-            roof["umma_all"] = entry(umma[hk[0]], "tensor", "TFLOP/s", peaks.get("bf16_tflops", 1700.0), 1e12)
+            roof["umma_all"] = entry(umma[hk[0]], "tensor", "TFLOP/s", peaks.get("bf16_tflops", 989.0), 1e12)
             roof["umma_all"]["peak_kind"] = "burst (bf16_tflops)"
             roof["umma_all"]["kernel"] = "conv_umma_kernel " + hk[0]
-            tr_ = traffic.get("heads_conv", {})
-            if tr_.get("frames") == Bp:          # DRAM bytes of THIS launch shape from the stored `ncu --set full` capture
-                roof["umma_all"]["traffic"] = tr_["dram_bytes"]
-                roof["umma_all"]["ncu_tensor_pipe_pct"] = tr_.get("tensor_pipe_pct")
-                roof["umma_all"]["traffic_source"] = tr_.get("source")
     pil = [(w, a.elapsed_time(b)) for k, w, a, b in prof if k == "pillar"]
     if pil:
-        roof["pillar"] = entry(pil, "hbm", "GB/s", peaks.get("hbm_gbs", 6650.0), 1e9)
+        roof["pillar"] = entry(pil, "hbm", "GB/s", peaks.get("hbm_gbs", 3350.0), 1e9)
         roof["pillar"]["kernel"] = "pillar encoder (%s: all its launches)" % ops.PILLAR_ENCODER
-        tr_ = traffic.get("pillar_" + ops.PILLAR_ENCODER, {})
-        if tr_.get("frames") == Bp:
-            roof["pillar"]["traffic"] = tr_["dram_bytes"]
-            roof["pillar"]["traffic_source"] = tr_.get("source")
     train = None
     if not args.no_train:
         for pp in pipes:                      # free the inference graphs' pools before the 22 GB training step
@@ -514,13 +488,12 @@ def main():
         torch.cuda.empty_cache()
         train = run_train_leg(args, dev, rank, world, lid, uni)
         _dbg(f"train leg done: {train['ms_per_step']:.1f} ms/step")
-        if not args.train_amp and args.train_amp_leg:      # opt-in: the same step with bf16 autocast, reported beside it (measured 316 vs 344
-            # samples/s on one B200: the step is launch-bound, not tensor-bound; at 2 ranks cuDNN's bf16 GRU hit an illegal address)
+        if not args.train_amp and args.train_amp_leg:      # opt-in: the same step with bf16 autocast, reported beside it
             a3 = argparse.Namespace(**vars(args))
             a3.train_amp, a3.train_steps, a3.train_warmup = True, max(3, args.train_steps // 2), 2
             amp = run_train_leg(a3, dev, rank, world, lid, uni)
             train["bf16_autocast"] = {k: amp[k] for k in ("value", "unit", "ms_per_step", "precision", "loss", "max_mem_gb")}
-    latency, gpu_ref = None, None
+    latency = None
     if rank == 0 and world == 1 and not args.no_gpu_reference:
         # batch-1 latency of one agent tick (the CARLA agent runs batch 1 at 20 Hz, lav_agent.py:32): host sensors in, waypoints +
         # brake back on the host, synchronised every tick
@@ -546,11 +519,7 @@ def main():
                    "path": "StaticFramePipeline(batch=1): pinned host sensors -> 2 CUDA graphs + host decode -> waypoints + brake on the host"}
         del p1
         torch.cuda.empty_cache()
-        gpu_ref = run_gpu_reference(dev)
-        if "value" in gpu_ref:
-            gpu_ref["ratio_ours_b1_over_reference"] = latency["frames_per_s"] / gpu_ref["value"]
-            gpu_ref["ratio_ours_throughput_over_reference"] = (world * B * args.steps / (ms_e2e * 1e-3)) / gpu_ref["value"]
-        _dbg("latency + gpu reference legs done")
+        _dbg("latency leg done")
     if rank == 0:
         frames = world * B * args.steps
         line = {"metric": "agent_frames_per_s", "value": frames / (ms * 1e-3), "unit": "frames/s", "n_gpus": world, "steps": args.steps,
@@ -561,8 +530,8 @@ def main():
                         "d2h_bytes_per_step": int(B * 20 * 2 * 4 + B * 4)},
                 "gpu_launches": int(launches), "clocks": clocks,
                 "roofline": roof.get("umma"), "roofline_heads_conv": roof.get("umma_all"), "roofline_pillar": roof.get("pillar"),
-                "train": train, "latency_b1": latency, "gpu_reference": gpu_ref}
-        line["dtype"] = "fp16 storage, fp32 accumulate (tcgen05 kind::f16 / mma.sync f16; saturating stores)" if args.precision == "f16" else args.precision
+                "train": train, "latency_b1": latency}
+        line["dtype"] = "fp16 storage, fp32 accumulate (wgmma f16 / mma.sync f16; saturating stores)" if args.precision == "f16" else args.precision
         if not args.no_cpu_baseline and world == 1:      # bounded sample (~10-15 s of host work), rank 0 at N=1 only
             a2 = argparse.Namespace(**vars(args))
             a2.steps, a2.warmup = 16, 2

@@ -1,4 +1,4 @@
-/* lav_b200 — C ABI of the B200-native LAV frame-path kernels (sm_100a).
+/* lav_b200 — C ABI of the H100-native LAV frame-path kernels (sm_90a).
  *
  * The reference (dotchen/LAV) has no FFI: its boundary is Python (torch modules).  A
  * reference-side maintainer binds these entry points with ctypes (see INTEGRATION.md);
@@ -237,21 +237,21 @@ int lavb_crop_bilinear_bwd(const float* d_gout, int b, int h, int w, int c, cons
 int lavb_split_h16(const float* d_src, void* d_dst, long long rows, int c, void* stream);
 int lavb_convert(const void* d_src, int src_dtype, void* d_dst, int dst_dtype, long long count, void* stream);
 
-/* ---------------------------------------------------------------- tcgen05 implicit-GEMM tap-list convolution
+/* ---------------------------------------------------------------- wgmma implicit-GEMM tap-list convolution
  * replaces (h16 path): the Conv2d -> ReLU -> BatchNorm2d layers of ConvBackbone (lidar.py:57-131), the fused 4-head
  *           384->256 conv (lidar.py:152-154) and the 64/128-channel factorised convs of ERFNet (erfnet.py:31-61).
  * Same descriptor and epilogue semantics as lavb_conv_taps, with these differences: input is h16 NHWC, cin % 64 == 0,
  * cout % 32 == 0 and <= 256, channel offsets/strides multiples of 8; d->w points to h16 weights laid out
  * [ntaps][cout][cin] (K contiguous).  Tiles are 8 x 16 output-grid pixels; operands are fetched by TMA
- * (cuTensorMapEncodeTiled through cudaGetDriverEntryPoint), accumulators live in TMEM. */
+ * (cuTensorMapEncodeTiled through cudaGetDriverEntryPoint), accumulators live in registers. */
 int lavb_conv_umma(const lavb_conv_desc* h_desc, void* stream);
 
 /* ---------------------------------------------------------------- fused (3x1 -> 1x3) convolution pair
  * replaces: conv3x1_k -> ReLU -> conv1x3_k -> bn_k [-> + input] -> ReLU of non_bottleneck_1d (lav/models/erfnet.py:37-63) in
- * one tcgen05 kernel; the intermediate activation stays in shared memory.
+ * one wgmma kernel; the intermediate activation stays in shared memory.
  *   mid = relu(conv3x1_dil(in) + bias1);  out = [relu](conv1x3_dil(mid) + shift2 [+ res])
  * The BatchNorm affine (conv + b2) * s + t is folded by the caller: w2 <- w2 * s per output channel, shift2 <- b2 * s + t.
- * bias1 / shift2 (fp32 [c]) are pre-loaded into the TMEM accumulators, so the epilogues only pack, clamp and add the residual
+ * bias1 / shift2 (fp32 [c]) are added to the register accumulators in the epilogues, which then pack, clamp and add the residual
  * (16-bit packed arithmetic: the residual add rounds once more than an fp32 add would).
  * in / out / res: h16 NHWC (n, h, w, c) contiguous, c in {64, 128}, w in {32, 64, 128}; w1 / w2: h16 [3 taps][c out][c in];
  * res may be NULL. */

@@ -1,4 +1,4 @@
-"""lav_b200 — B200-native (sm_100a) kernels and drop-in mirrors for the LAV frame path.
+"""lav_b200 — H100-native (sm_90a) kernels and drop-in mirrors for the LAV frame path.
 
 Layers: ``include/lav_b200.h`` (C ABI) -> ``csrc/*.cu`` built by ``lav_b200.build`` into ``_lib/liblavb200.so`` ->
 ``capi`` (ctypes) -> ``ops`` (tensor front ends) -> mirrors of the reference modules (``erfnet``, ``rgb``, ``point_painting``,

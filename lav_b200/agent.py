@@ -22,8 +22,8 @@ from .model_inference import InferModel
 FUSE_SEG_HEAD = True  # ERFNet's last layer (ConvTranspose2d 16->5, k2 s2) + softmax evaluated inside the painting gather
 FORK_BRAKE = True     # run the brake predictor as a parallel branch of the perception graph
 STEM_U8 = True        # brake-model stem (7x7 s2 on 3 channels) in the lav_b200 kernel, straight from the camera bytes
-UMMA_TRUNKS = os.environ.get("LAVB_UMMA_TRUNKS", "0") == "1"   # ResNet-18 trunks (brake / planner embedder) on the tcgen05 conv kernel: correct (tested) but measured 5-20%
-                      # slower than the BN-folded cuDNN path on these small maps (B200, B=32), so cuDNN stays the default
+UMMA_TRUNKS = os.environ.get("LAVB_UMMA_TRUNKS", "0") == "1"   # ResNet-18 trunks (brake / planner embedder) on the wgmma conv kernel: correct (tested) but measured
+                      # 3 % slower end to end than the BN-folded cuDNN path (H100, bench B = 64), so cuDNN stays the default
 NUM_REPEAT = 4
 GAP = NUM_REPEAT + 1          # lav_agent_fast.py:31-32
 NUM_FRAME_STACK = 2           # team_code_v2/config.yaml: num_frame_stack

@@ -1,4 +1,4 @@
-"""In-tree build of liblavb200.so (sm_100a only) with plain nvcc — no torch headers involved.
+"""In-tree build of liblavb200.so (sm_90a, H100) with plain nvcc — no torch headers involved.
 
     python -m lav_b200.build [--force]
 """
@@ -13,7 +13,8 @@ LIBDIR = os.path.join(HERE, "_lib")
 LIB = os.path.join(LIBDIR, "liblavb200.so")
 SOURCES = ["capi.cu", "paint.cu", "pillar.cu", "conv_taps.cu", "conv_umma.cu", "crop.cu", "deconv_small.cu", "peaks.cu", "stem.cu", "conv_pair_umma.cu", "gru_cluster.cu", "cast_gru.cu", "erf16.cu"]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-std=c++17", "-lineinfo", "-Xcompiler", "-fPIC",
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
+FLAGS = [*ARCH, "-O3", "-std=c++17", "-lineinfo", "-Xcompiler", "-fPIC",
          "--expt-relaxed-constexpr", "-Xptxas", "-v"]
 
 
@@ -51,7 +52,7 @@ def build(force=False, verbose=False):
         with ThreadPoolExecutor(max_workers=min(8, len(jobs))) as ex:
             list(ex.map(cc, jobs))
     if jobs or not os.path.exists(LIB):
-        r = subprocess.run([NVCC, "-shared", "-o", LIB, *objs, "-lcuda", "-gencode", "arch=compute_100a,code=sm_100a"],
+        r = subprocess.run([NVCC, "-shared", "-o", LIB, *objs, "-lcuda", *ARCH],
                            capture_output=True, text=True)
         if r.returncode != 0:
             raise RuntimeError("link failed:\n" + r.stdout + r.stderr)

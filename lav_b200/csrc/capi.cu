@@ -17,16 +17,16 @@ void set_error(const char* fmt, ...) {
 
 // SM count of the current device (cached per ordinal): persistent kernels size their grids from it.
 // LAVB_NUM_SMS (read once) caps it: persistent CTAs with ~200 KB of shared memory leave no room for another stream's small
-// kernels on their SMs, so a cap of e.g. 132 keeps 16 SMs free for the latency-bound chains of a second agent group.
+// kernels on their SMs, so a cap of e.g. 116 keeps 16 SMs free for the latency-bound chains of a second agent group.
 int num_sms() {
   static int cache[64];
   static int cap = -1;
   if (cap < 0) { const char* e = getenv("LAVB_NUM_SMS"); cap = e ? atoi(e) : 0; }
   int dev = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess) { cudaGetLastError(); return kNumSMsB200; }
+  if (cudaGetDevice(&dev) != cudaSuccess) { cudaGetLastError(); return kNumSMsH100; }
   if (dev >= 0 && dev < 64 && cache[dev] > 0) return cache[dev];
   int n = 0;
-  if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) { cudaGetLastError(); return kNumSMsB200; }
+  if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) { cudaGetLastError(); return kNumSMsH100; }
   if (cap > 0 && cap < n) n = cap;
   if (dev >= 0 && dev < 64) cache[dev] = n;
   return n;

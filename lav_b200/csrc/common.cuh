@@ -1,4 +1,4 @@
-// Shared helpers for the lav_b200 kernels (sm_100a only).
+// Shared helpers for the lav_b200 kernels (sm_90a).
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_bf16.h>
@@ -38,7 +38,7 @@ void set_error(const char* fmt, ...);
     }                                                                                        \
   } while (0)
 
-constexpr int kNumSMsB200 = 148;   // fallback only; grids are sized from num_sms()
+constexpr int kNumSMsH100 = 132;   // fallback only; grids are sized from num_sms()
 int num_sms();
 cudaError_t ensure_dyn_smem(const void* kernel, int bytes);
 #define kNumSMs (lavb::num_sms())
@@ -54,7 +54,6 @@ using h162 = __nv_bfloat162;
 #define LAVB_H16_PTX "bf16"
 #define LAVB_H16 LAVB_BF16
 #define LAVB_TMAP_H16 CU_TENSOR_MAP_DATA_TYPE_BFLOAT16
-constexpr uint32_t kH16Fmt = 1;     // tcgen05 instruction-descriptor A/B format field: 0 = f16, 1 = bf16
 __device__ __forceinline__ uint32_t pack_h16(float a, float b) {            // (a -> low half, b -> high half)
   const __nv_bfloat162 v = __floats2bfloat162_rn(a, b);
   return *reinterpret_cast<const uint32_t*>(&v);
@@ -68,7 +67,6 @@ using h162 = __half2;
 #define LAVB_H16_PTX "f16"
 #define LAVB_H16 LAVB_F16
 #define LAVB_TMAP_H16 CU_TENSOR_MAP_DATA_TYPE_FLOAT16
-constexpr uint32_t kH16Fmt = 0;
 __device__ __forceinline__ uint32_t pack_h16(float a, float b) {
   uint32_t r;
   asm("cvt.rn.satfinite.f16x2.f32 %0, %1, %2;" : "=r"(r) : "f"(b), "f"(a));

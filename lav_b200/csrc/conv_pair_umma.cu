@@ -1,27 +1,22 @@
-// Fused ERFNet pair kernel (lav_b200.erfnet.FUSE_PAIRS, on by default; B200: ERFNet of 96 images 2.85 -> 2.72 ms):
+// Fused ERFNet pair kernel (lav_b200.erfnet.FUSE_PAIRS, on by default):
 // one kernel for a (3x1 -> 1x3) convolution pair of ERFNet's non_bottleneck_1d (lav/models/erfnet.py:37-63):
 //     mid = relu(conv3x1(x) + b1)                      (vertical taps, dilation d)
 //     out = [relu]( (conv1x3(mid) + b2) * s + t [+ res] )   (horizontal taps, dilation d; BN affine; residual)
-// Un-fused, each of the two layers is HBM-bound (the 64/128-channel layers run at ~4 TB/s effective, profiles/r01_kernels.md);
+// Un-fused, each of the two layers is HBM-bound;
 // fused, `mid` never leaves the SM.  A tile is 128 pixels made of FULL-WIDTH image rows (W = 64 -> 2 rows, W = 32 -> 4 rows),
 // so the horizontal conv needs no halo: its zero padding is the image border.
-//   stage 1: tcgen05.mma over 3 vertical taps (A = 4-D TMA boxes shifted by the tap, B = W1 blocks) -> TMEM acc1 (2 buffers)
-//   (bias1 / shift2 are PRE-LOADED into the accumulators: the epilogue warps re-arm the TMEM columns they have just drained with
-//    tcgen05.st, every MMA accumulates — so the epilogues carry no per-element fp32 arithmetic at all: pack, clamp, store.
-//    The kernel is bound by the epilogue warps' instruction issue (ncu: tensor pipe 17-19 %, profiles/r02_erf_pair_summary.md):
-//    8.2 -> ~3.8 thread-instructions per output element)
-//   epilogue 1: acc1 -> h16 -> relu -> shared memory, written three times in the SWIZZLE_128B K-major operand layout:
+//   stage 1: wgmma over 3 vertical taps (A = 4-D TMA boxes shifted by the tap, B = W1 blocks) into register accumulators
+//   epilogue 1: acc1 + bias1 -> h16 -> relu -> shared memory, written three times in the SWIZZLE_128B K-major operand layout:
 //               shifted by +d, 0, -d pixels inside each image row (rows that fall off the image border stay zero), i.e. the
 //               three A operands of the horizontal taps
-//   stage 2: tcgen05.mma over the 3 horizontal taps (A = those copies, B = W2 blocks through the same TMA ring) -> TMEM acc2
-//   epilogue 2: acc2 -> h16 -> (+ residual, ReLU as one packed fma.relu) -> NHWC.  The BatchNorm scale is folded into W2 by the caller.
-// Warp roles as conv_umma.cu (warp 0 TMA producer, warp 1 MMA issuer, warps 2-9 epilogue), one CTA per SM, persistent.
-// MMA issue order S1(0), S1(1), S2(0), S1(2), S2(1), ... — the producer feeds the ring in exactly that order — so the
-// stage-1 MMAs of the next tile run while the epilogue warps write `mid` of the current one.
+//   stage 2: wgmma over the 3 horizontal taps (A = those copies, B = W2 blocks through the same TMA ring)
+//   epilogue 2: acc2 + shift2 -> h16 -> (+ residual, ReLU as one packed fma.relu) -> NHWC.  The BatchNorm scale is folded into W2 by the caller.
+// Warp roles: warps 0-3 and 4-7 are two consumer warpgroups (tile pixels 0-63 / 64-127), warp 8 is the TMA producer; persistent
+// over tiles.  With C = 64 two CTAs share an SM, so one CTA's epilogues overlap the other's MMAs.
 #include <cuda.h>
 #include <cudaTypedefs.h>
 #include <stdlib.h>
-#include "common.cuh"
+#include "sm90.cuh"
 
 namespace lavb {
 namespace pair {
@@ -29,19 +24,19 @@ namespace pair {
 constexpr int kBlockM = 128, kBlockK = 64;
 constexpr int kABytes = kBlockM * kBlockK * 2;  // 16 KB: one K-block of an A operand
 constexpr int kMaxStages = 8;
-constexpr int kEpiWarps = 8;
+constexpr int kPairThreads = 288;
 
 struct PairArgs {
-  int n, h, w, c, kchunks, dil, tile_w, tile_h, tiles_per_img, num_tiles, stages, tmem_cols, post_relu;
+  int n, h, w, c, kchunks, dil, tile_w, tile_h, tiles_per_img, num_tiles, stages, post_relu;
   h16* out; const h16* res;
   const float* bias1; const float* shift2;
   long long* trace; int trace_tiles;      // profiling aid (lavb_conv_pair_set_trace): per-CTA, per-tile clock64 stamps, or null
 };
-// stamps of tile iteration i of this CTA: [0..3] epilogue warp 2 (acc1 ready, mid written, acc2 ready, tile stored),
-// [4..7] MMA thread (stage-1 of the next tile issued, mid_full observed, stage-2 issued, -)
+// stamps of tile iteration i of this CTA, taken by thread 0: [0] acc1 ready, [1] mid written, [2] acc2 ready, [3] tile stored
 #define PAIR_STAMP(slot, i)                                                                                         \
   do {                                                                                                              \
-    if (p.trace && (i) < p.trace_tiles) p.trace[((long long)blockIdx.x * p.trace_tiles + (i)) * 8 + (slot)] = clock64(); \
+    if (p.trace && threadIdx.x == 0 && (i) < p.trace_tiles)                                                         \
+      p.trace[((long long)blockIdx.x * p.trace_tiles + (i)) * 8 + (slot)] = clock64();                              \
   } while (0)
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
@@ -74,59 +69,7 @@ __device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* map
       "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
       ::"r"(dst), "l"(reinterpret_cast<uint64_t>(map)), "r"(bar), "r"(c0), "r"(c1) : "memory");
 }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
 __device__ __forceinline__ void proxy_fence_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-// K-major SWIZZLE_128B shared-memory matrix descriptor (same encoding as conv_umma.cu)
-__device__ __forceinline__ uint64_t make_sw128_desc(uint32_t saddr) {
-  const uint32_t lo = (saddr & 0x3FFFFu) >> 4;
-  const uint32_t hi = (1024u >> 4) | (1u << 14) | (2u << 29);
-  return (uint64_t)lo | ((uint64_t)hi << 32);
-}
-__device__ __forceinline__ void umma_h16(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate) : "memory");
-}
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&v)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-        "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]),
-        "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]),
-        "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-      : "r"(taddr) : "memory");
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_st32(uint32_t taddr, const uint32_t (&v)[32]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, "
-      "%17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};"
-      ::"r"(taddr), "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7]), "r"(v[8]),
-        "r"(v[9]), "r"(v[10]), "r"(v[11]), "r"(v[12]), "r"(v[13]), "r"(v[14]), "r"(v[15]), "r"(v[16]),
-        "r"(v[17]), "r"(v[18]), "r"(v[19]), "r"(v[20]), "r"(v[21]), "r"(v[22]), "r"(v[23]), "r"(v[24]),
-        "r"(v[25]), "r"(v[26]), "r"(v[27]), "r"(v[28]), "r"(v[29]), "r"(v[30]), "r"(v[31])
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-// TMEM[this warp's 32 lanes][col0, col0 + 32) <- src[0, 32) (fp32, the same row for every lane): accumulator pre-load
-__device__ __forceinline__ void tmem_fill32(uint32_t taddr, const float* src) {
-  uint32_t b[32];
-#pragma unroll
-  for (int j = 0; j < 8; ++j) {
-    const float4 f = reinterpret_cast<const float4*>(src)[j];
-    b[4 * j] = __float_as_uint(f.x); b[4 * j + 1] = __float_as_uint(f.y); b[4 * j + 2] = __float_as_uint(f.z); b[4 * j + 3] = __float_as_uint(f.w);
-  }
-  tmem_st32(taddr, b);
-}
 __device__ __forceinline__ uint32_t relu2(uint32_t x) {
   const h162 v = __hmax2(*reinterpret_cast<const h162*>(&x), floats2h162(0.f, 0.f));
   return *reinterpret_cast<const uint32_t*>(&v);
@@ -136,297 +79,182 @@ __device__ __forceinline__ uint32_t add2(uint32_t x, uint32_t r, bool relu) {
   const h162 v = relu ? __hfma2_relu(a, floats2h162(1.f, 1.f), b) : __hadd2(a, b);
   return *reinterpret_cast<const uint32_t*>(&v);
 }
-__device__ __forceinline__ uint32_t pack2(float a, float b) {
-  const h162 v = floats2h162(a, b);
-  return *reinterpret_cast<const uint32_t*>(&v);
-}
 
-template <int kMinBlocks>
-__global__ void __launch_bounds__(64 + 32 * kEpiWarps, kMinBlocks) conv_pair_umma_kernel(const __grid_constant__ CUtensorMap tmap_a,
-                                                                               const __grid_constant__ CUtensorMap tmap_w1,
-                                                                               const __grid_constant__ CUtensorMap tmap_w2,
-                                                                               const __grid_constant__ PairArgs p) {
+template <int kC>
+__global__ void __launch_bounds__(kPairThreads, kC == 64 ? 2 : 1) conv_pair_umma_kernel(const __grid_constant__ CUtensorMap tmap_a,
+                                                                                       const __grid_constant__ CUtensorMap tmap_w1,
+                                                                                       const __grid_constant__ CUtensorMap tmap_w2,
+                                                                                       const __grid_constant__ PairArgs p) {
+  constexpr int kNC = kC / 64;                                      // 64-column MMA chunks
+  constexpr int kChunks = kC / kBlockK;                             // K-blocks per tap
+  constexpr int kWBytes = kC * kBlockK * 2;                         // one weight K-block: c rows x 128 B
+  constexpr int kSlotBytes = kABytes + kWBytes;
+  constexpr int kNkb = 3 * kChunks;                                 // K-blocks per stage
+  constexpr int kBpf = kSlotBytes / kWBytes;                        // W2 K-blocks per ring slot in stage 2
+  static_assert(kNkb % kBpf == 0, "stage 2 fills whole ring slots");
   extern __shared__ uint8_t smem_raw[];
   const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;     // SWIZZLE_128B operands need 1024 B alignment
-  const int w_bytes = p.c * kBlockK * 2;                            // one weight K-block: c rows x 128 B
-  const int slot_bytes = kABytes + w_bytes;
-  const uint32_t mid = base + p.stages * slot_bytes;                // [3 taps][kchunks] x 16 KB, K-major SW128
-  const int mid_bytes = 3 * p.kchunks * kABytes;
-  const uint32_t stage_out = mid + mid_bytes;                       // kEpiWarps x 1 KB: per-warp transposition buffer of epilogue 2
-  const uint32_t ctrl = stage_out + kEpiWarps * 1024;
-  const uint32_t full_bar = ctrl, empty_bar = ctrl + 8 * kMaxStages, tfull1 = ctrl + 16 * kMaxStages, tempty1 = tfull1 + 16,
-                 mid_full = tempty1 + 16, tfull2 = mid_full + 8, tmem_slot = tfull2 + 8;
   uint8_t* gen = smem_raw + (base - smem_u32(smem_raw));
-  volatile uint32_t* tmem_slot_p = reinterpret_cast<volatile uint32_t*>(gen + (tmem_slot - base));
-  float* ep_b1 = reinterpret_cast<float*>(gen + (tmem_slot - base) + 16);     // bias of conv A
-  float* ep_t2 = ep_b1 + 128;                                                 // shift of conv B (BatchNorm folded by the caller)
+  const uint32_t mid = base + p.stages * kSlotBytes;                // [3 taps][kchunks] x 16 KB, K-major SW128
+  constexpr int kMidBytes = 3 * kChunks * kABytes;
+  const uint32_t ctrl = mid + kMidBytes;
+  const uint32_t full_bar = ctrl, empty_bar = ctrl + 8 * kMaxStages;
+  float* ep_b1 = reinterpret_cast<float*>(gen + (ctrl - base) + 16 * kMaxStages);   // bias of conv A
+  float* ep_t2 = ep_b1 + 128;                                                       // shift of conv B (BatchNorm folded by the caller)
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   if (threadIdx.x == 0) {
     asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmap_a)) : "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmap_w1)) : "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmap_w2)) : "memory");
-    for (int s = 0; s < p.stages; ++s) { mbar_init(full_bar + 8 * s, 1); mbar_init(empty_bar + 8 * s, 1); }
-    for (int a = 0; a < 2; ++a) { mbar_init(tfull1 + 8 * a, 1); mbar_init(tempty1 + 8 * a, 32 * kEpiWarps); }
-    mbar_init(mid_full, 32 * kEpiWarps);
-    mbar_init(tfull2, 1);
+    for (int s = 0; s < p.stages; ++s) { mbar_init(full_bar + 8 * s, 1); mbar_init(empty_bar + 8 * s, 8); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(tmem_slot), "r"((uint32_t)p.tmem_cols) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  for (int c = threadIdx.x; c < p.c; c += blockDim.x) {
+  for (int c = threadIdx.x; c < kC; c += blockDim.x) {
     ep_b1[c] = __ldg(p.bias1 + c);
     ep_t2[c] = p.shift2 ? __ldg(p.shift2 + c) : 0.f;
   }
   // the shifted copies keep zero rows where a tap falls off the image border: clear `mid` once, data rows are rewritten per tile
-  for (int i = threadIdx.x; i < mid_bytes / 16; i += blockDim.x)
+  for (int i = threadIdx.x; i < kMidBytes / 16; i += blockDim.x)
     *reinterpret_cast<uint4*>(gen + (mid - base) + 16 * i) = make_uint4(0u, 0u, 0u, 0u);
   proxy_fence_async();
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot_p;
-  const int nkb = 3 * p.kchunks;                                    // K-blocks per stage
-  const int bpf = slot_bytes / w_bytes;                             // W2 K-blocks per ring slot in stage 2
-  if (warp >= 2) {
-    // pre-load the three accumulators (acc1[0], acc1[1] <- bias1, acc2 <- shift2): each epilogue warp arms the columns it drains
-    const uint32_t lane_addr = tmem_base + ((uint32_t)((warp & 3) * 32) << 16);
-    for (int c0 = ((warp - 2) >> 2) * 32; c0 < p.c; c0 += 64) {
-      tmem_fill32(lane_addr + (uint32_t)c0, ep_b1 + c0);
-      tmem_fill32(lane_addr + (uint32_t)(p.c + c0), ep_b1 + c0);
-      tmem_fill32(lane_addr + (uint32_t)(2 * p.c + c0), ep_t2 + c0);
-    }
-    tmem_st_wait();
-  }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
 
-  if (warp == 0) {
+  if (warp == 8) {
     if (lane == 0) {
       int slot = 0; uint32_t phase = 0;
-      auto load_stage1 = [&](int tile) {
+      // ring order = consumption order: stage 1 of a tile (A + W1 per K-block), then its stage 2.  Stage 2 needs only weights:
+      // a ring slot (A part + W part) takes kBpf whole W2 K-blocks, so the stage is 1 fill (c = 64) or 3 fills (c = 128)
+      for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
         const int img = tile / p.tiles_per_img, y0 = (tile - img * p.tiles_per_img) * p.tile_h;
         for (int t = 0; t < 3; ++t)
-          for (int kc = 0; kc < p.kchunks; ++kc) {
+          for (int kc = 0; kc < kChunks; ++kc) {
             mbar_wait(empty_bar + 8 * slot, phase ^ 1);
-            const uint32_t sa = base + slot * slot_bytes;
-            mbar_expect_tx(full_bar + 8 * slot, slot_bytes);
+            const uint32_t sa = base + slot * kSlotBytes;
+            mbar_expect_tx(full_bar + 8 * slot, kSlotBytes);
             tma_load_4d(sa, &tmap_a, full_bar + 8 * slot, kc * kBlockK, 0, y0 + (t - 1) * p.dil, img);
-            tma_load_2d(sa + kABytes, &tmap_w1, full_bar + 8 * slot, kc * kBlockK, t * p.c);
+            tma_load_2d(sa + kABytes, &tmap_w1, full_bar + 8 * slot, kc * kBlockK, t * kC);
             if (++slot == p.stages) { slot = 0; phase ^= 1; }
           }
-      };
-      // stage 2 needs only weights: a ring slot (A part + W part) takes bpf = slot_bytes / w_bytes whole W2 K-blocks, so the
-      // stage is 1 fill (c = 64) or 3 fills (c = 128) instead of 3 / 6 — with 2-3 slots in the ring the fills of a stage cannot
-      // all be in flight, and each extra round trip is a TMA latency on the tile's critical path (clock64 trace)
-      auto load_stage2 = [&]() {
-        for (int kb0 = 0; kb0 < nkb; kb0 += bpf) {
+        for (int kb0 = 0; kb0 < kNkb; kb0 += kBpf) {
           mbar_wait(empty_bar + 8 * slot, phase ^ 1);
-          const uint32_t sa = base + slot * slot_bytes;
-          const int nb = min(bpf, nkb - kb0);
-          mbar_expect_tx(full_bar + 8 * slot, nb * w_bytes);
-          for (int b = 0; b < nb; ++b) {
-            const int kb = kb0 + b, t = kb / p.kchunks, kc = kb - t * p.kchunks;
-            tma_load_2d(sa + b * w_bytes, &tmap_w2, full_bar + 8 * slot, kc * kBlockK, t * p.c);
+          const uint32_t sa = base + slot * kSlotBytes;
+          mbar_expect_tx(full_bar + 8 * slot, kBpf * kWBytes);
+          for (int b = 0; b < kBpf; ++b) {
+            const int kb = kb0 + b, t = kb / kChunks, kc = kb - t * kChunks;
+            tma_load_2d(sa + b * kWBytes, &tmap_w2, full_bar + 8 * slot, kc * kBlockK, t * kC);
           }
           if (++slot == p.stages) { slot = 0; phase ^= 1; }
         }
-      };
-      if ((int)blockIdx.x < p.num_tiles) load_stage1(blockIdx.x);
-      for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
-        if (tile + (int)gridDim.x < p.num_tiles) load_stage1(tile + gridDim.x);
-        load_stage2();
       }
     }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      // instruction descriptor: D=f32, A=B=h16, K-major both, N = c, M = 128 (bit layout in conv_umma.cu)
-      const uint32_t idesc = (1u << 4) | (kH16Fmt << 7) | (kH16Fmt << 10) | ((uint32_t)(p.c >> 3) << 17) | ((uint32_t)(kBlockM >> 4) << 24);
-      int slot = 0; uint32_t phase = 0;
-      uint32_t te_phase[2] = {0, 0};                 // parity of tempty1[buf] expected next
-      auto stage1 = [&](int buf) {
-        mbar_wait(tempty1 + 8 * buf, te_phase[buf] ^ 1);
-        te_phase[buf] ^= 1;
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + (uint32_t)(buf * p.c);
-        for (int kb = 0; kb < nkb; ++kb) {
-          mbar_wait(full_bar + 8 * slot, phase);
-          tc_fence_after();
-          const uint32_t sa = base + slot * slot_bytes;
-          const uint64_t a_desc = make_sw128_desc(sa), b_desc = make_sw128_desc(sa + kABytes);
-#pragma unroll
-          for (int k = 0; k < kBlockK / 16; ++k)
-            umma_h16(d_tmem, a_desc + (uint64_t)(2 * k), b_desc + (uint64_t)(2 * k), idesc, 1u);   // onto the pre-loaded bias
-          umma_commit(empty_bar + 8 * slot);
-          if (++slot == p.stages) { slot = 0; phase ^= 1; }
-        }
-        umma_commit(tfull1 + 8 * buf);
-      };
-      if ((int)blockIdx.x < p.num_tiles) stage1(0);
-      int i = 0;
-      for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x, ++i) {
-        if (tile + (int)gridDim.x < p.num_tiles) stage1((i + 1) & 1);
-        PAIR_STAMP(4, i);
-        mbar_wait(mid_full, (uint32_t)(i & 1));      // the epilogue warps have written the three shifted copies of `mid`
-        tc_fence_after();
-        PAIR_STAMP(5, i);
-        const uint32_t d_tmem = tmem_base + (uint32_t)(2 * p.c);
-        for (int kb0 = 0; kb0 < nkb; kb0 += bpf) {
-          mbar_wait(full_bar + 8 * slot, phase);
-          tc_fence_after();
-          const uint32_t sa = base + slot * slot_bytes;
-          const int nb = min(bpf, nkb - kb0);
-          for (int b = 0; b < nb; ++b) {
-            const uint64_t a_desc = make_sw128_desc(mid + (kb0 + b) * kABytes), b_desc = make_sw128_desc(sa + b * w_bytes);   // kb = t*kchunks + kc
-#pragma unroll
-            for (int k = 0; k < kBlockK / 16; ++k)
-              umma_h16(d_tmem, a_desc + (uint64_t)(2 * k), b_desc + (uint64_t)(2 * k), idesc, 1u);   // onto the pre-loaded shift
-          }
-          umma_commit(empty_bar + 8 * slot);
-          if (++slot == p.stages) { slot = 0; phase ^= 1; }
-        }
-        umma_commit(tfull2);                         // acc2 complete; also: `mid` may be rewritten
-        PAIR_STAMP(6, i);
-      }
-    }
-  } else {
-    const int q = warp & 3;                          // TMEM lane quarter this warp may read (warp id % 4)
-    const int half = (warp - 2) >> 2;                // the two warps of a quarter take alternate 32-column chunks
-    const int m = q * 32 + lane;                     // tile row = pixel
-    const int py = m / p.tile_w, px = m - py * p.tile_w;
-    const int d = p.dil;
-    const uint32_t lane_addr = tmem_base + ((uint32_t)(q * 32) << 16);
-    const bool relu_out = p.post_relu != 0;
-    // destination rows of this pixel's data in the three shifted copies (tap t reads x + (t-1) d): row m - (t-1) d
-    const bool ok0 = px + d < p.tile_w, ok2 = px - d >= 0;
-    const int r0 = m + d, r2 = m - d;
-    uint8_t* midp = gen + (mid - base);
-    int i = 0;
-    for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x, ++i) {
-      const int buf = i & 1;
-      const int img = tile / p.tiles_per_img, y = (tile - img * p.tiles_per_img) * p.tile_h + py;
-      const bool valid = y < p.h;
-      const long long pix = ((long long)img * p.h + y) * p.w + px;
-      // ---- epilogue 1: acc1 (bias included) -> h16 -> relu -> three shifted K-major copies in shared memory
-      mbar_wait(tfull1 + 8 * buf, (uint32_t)((i >> 1) & 1));
-      tc_fence_after();
-      if (threadIdx.x == 64) PAIR_STAMP(0, i);
-      for (int c0 = half * 32; c0 < p.c; c0 += 64) {
-        uint32_t w[16];
-        {
-          uint32_t v[32];
-          tmem_ld32(lane_addr + (uint32_t)(buf * p.c + c0), v);
-#pragma unroll
-          for (int j = 0; j < 16; ++j) w[j] = relu2(pack2(__uint_as_float(v[2 * j]), __uint_as_float(v[2 * j + 1])));
-        }
-        tmem_fill32(lane_addr + (uint32_t)(buf * p.c + c0), ep_b1 + c0);      // re-arm these columns for tile i + 2
-        const int kc = c0 >> 6, jj0 = (c0 & 63) >> 3;            // K-block and first 16-byte piece inside the 128-byte row
-        uint8_t* blk = midp + kc * kABytes;
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-          const uint4 val = make_uint4(w[4 * j], w[4 * j + 1], w[4 * j + 2], w[4 * j + 3]);
-          const int jj = jj0 + j;
-          if (ok0) *reinterpret_cast<uint4*>(blk + 0 * p.kchunks * kABytes + r0 * 128 + ((jj ^ (r0 & 7)) << 4)) = val;
-          *reinterpret_cast<uint4*>(blk + 1 * p.kchunks * kABytes + m * 128 + ((jj ^ (m & 7)) << 4)) = val;
-          if (ok2) *reinterpret_cast<uint4*>(blk + 2 * p.kchunks * kABytes + r2 * 128 + ((jj ^ (r2 & 7)) << 4)) = val;
-        }
-      }
-      tmem_st_wait();
-      tc_fence_before();
-      mbar_arrive(tempty1 + 8 * buf);                // acc1[buf] (re-armed) may take the stage-1 MMAs of tile i+2
-      proxy_fence_async();                           // generic-proxy stores -> visible to the tensor core's async-proxy reads
-      mbar_arrive(mid_full);                         // also orders this thread's re-arming of acc2 (previous tile) before stage 2
-      if (threadIdx.x == 64) PAIR_STAMP(1, i);
-      // ---- epilogue 2: acc2 (shift included) -> h16 (+ residual) -> ReLU -> NHWC
-      // residual: loaded with the coalesced mapping (4 lanes per pixel, rr[2 hp + k] = pixel 16 hp + 8 k + lane/4, piece lane%4)
-      // well before the accumulator is ready; transposed to "lane = pixel" through the warp's staging buffer at use
-      uint4 rr[4];
-      const h16* rrow = p.res + (pix - lane) * p.c;
-      auto load_res = [&](int c0) {
-#pragma unroll
-        for (int e = 0; e < 4; ++e)
-          rr[e] = __ldg(reinterpret_cast<const uint4*>(rrow + (long long)((e >> 1) * 16 + 8 * (e & 1) + (lane >> 2)) * p.c + c0 + (lane & 3) * 8));
-      };
-      if (p.res && valid) load_res(half * 32);       // requested before the accumulator wait
-      mbar_wait(tfull2, (uint32_t)(i & 1));
-      tc_fence_after();
-      if (threadIdx.x == 64) PAIR_STAMP(2, i);
-      for (int c0 = half * 32; c0 < p.c; c0 += 64) {
-        uint32_t w[16];
-        {
-          uint32_t v[32];
-          tmem_ld32(lane_addr + (uint32_t)(2 * p.c + c0), v);
-#pragma unroll
-          for (int j = 0; j < 16; ++j) w[j] = pack2(__uint_as_float(v[2 * j]), __uint_as_float(v[2 * j + 1]));
-        }
-        tmem_fill32(lane_addr + (uint32_t)(2 * p.c + c0), ep_t2 + c0);        // re-arm acc2 for the next tile
-        uint8_t* stg = gen + (stage_out - base) + (warp - 2) * 1024;
-        if (valid) {
-          if (p.res) {
-#pragma unroll
-            for (int hp = 0; hp < 2; ++hp) {
-#pragma unroll
-              for (int k = 0; k < 2; ++k) {
-                const int r = 8 * k + (lane >> 2), j = lane & 3;
-                *reinterpret_cast<uint4*>(stg + r * 64 + ((j ^ ((r >> 1) & 3)) << 4)) = rr[2 * hp + k];
-              }
-              __syncwarp();
-              if ((lane >> 4) == hp) {
-                const int r = lane & 15;
-#pragma unroll
-                for (int j = 0; j < 4; ++j) {
-                  const uint4 q4 = *reinterpret_cast<const uint4*>(stg + r * 64 + ((j ^ ((r >> 1) & 3)) << 4));
-                  w[4 * j] = add2(w[4 * j], q4.x, relu_out); w[4 * j + 1] = add2(w[4 * j + 1], q4.y, relu_out);
-                  w[4 * j + 2] = add2(w[4 * j + 2], q4.z, relu_out); w[4 * j + 3] = add2(w[4 * j + 3], q4.w, relu_out);
-                }
-              }
-              __syncwarp();
-            }
-            if (c0 + 64 < p.c) load_res(c0 + 64);
-          } else if (relu_out) {
-#pragma unroll
-            for (int j = 0; j < 16; ++j) w[j] = relu2(w[j]);
-          }
-        }
-        // Store through a per-warp shared-memory transposition: a lane owns 64 contiguous bytes of ITS pixel, so a direct
-        // 16-byte store per lane touches 32 different 128-byte lines (half a sector each) per instruction — measured as the
-        // longest phase of the tile (clock64 trace, scripts/pair_trace.py).  Re-mapped, 4 lanes cover the 64 bytes of one pixel
-        // and an instruction writes 8 pixels x 64 B in full sectors.  16 pixels per pass (1 KB per warp), swizzled so that both
-        // the row-wise writes and the 4-lanes-per-row reads are bank-conflict free.  The warp's 32 pixels are consecutive in x.
-        h16* orow = p.out + (pix - lane) * p.c + c0;              // pixel of lane 0, this chunk's channels
-#pragma unroll
-        for (int hp = 0; hp < 2; ++hp) {
-          if ((lane >> 4) == hp) {
-            const int r = lane & 15;
-#pragma unroll
-            for (int j = 0; j < 4; ++j)
-              *reinterpret_cast<uint4*>(stg + r * 64 + ((j ^ ((r >> 1) & 3)) << 4)) = make_uint4(w[4 * j], w[4 * j + 1], w[4 * j + 2], w[4 * j + 3]);
-          }
-          __syncwarp();
-          if (valid) {
-#pragma unroll
-            for (int k = 0; k < 2; ++k) {
-              const int r = 8 * k + (lane >> 2), j = lane & 3;
-              const uint4 val = *reinterpret_cast<const uint4*>(stg + r * 64 + ((j ^ ((r >> 1) & 3)) << 4));
-              *reinterpret_cast<uint4*>(orow + (long long)(hp * 16 + r) * p.c + j * 8) = val;
-            }
-          }
-          __syncwarp();
-        }
-      }
-      tmem_st_wait();
-      tc_fence_before();                             // acc2 reads and its re-arming are ordered before this thread's next mid_full arrival
-      if (threadIdx.x == 64) PAIR_STAMP(3, i);
-    }
+    return;
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"((uint32_t)p.tmem_cols) : "memory");
+
+  const int wg = warp >> 2;                          // tile pixels [64 wg, 64 wg + 64)
+  const int d = p.dil;
+  const bool relu_out = p.post_relu != 0;
+  uint8_t* midp = gen + (mid - base);
+  int slot = 0; uint32_t phase = 0;
+  int i = 0;
+  for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x, ++i) {
+    const int img = tile / p.tiles_per_img, y0 = (tile - img * p.tiles_per_img) * p.tile_h;
+    // ---- stage 1: acc1 = conv3x1(x)
+    float acc[kNC][32];
+    int prev = -1;
+    for (int kb = 0; kb < kNkb; ++kb) {
+      mbar_wait(full_bar + 8 * slot, phase);
+      const uint32_t sa = base + slot * kSlotBytes;
+      const uint64_t a_desc = sm90::desc_sw128(sa + wg * (kABytes / 2)), b_desc = sm90::desc_sw128(sa + kABytes);
+      sm90::wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < kBlockK / 16; ++k)
+#pragma unroll
+        for (int cc = 0; cc < kNC; ++cc)
+          sm90::wgmma_n64(acc[cc], a_desc + (uint64_t)(2 * k), b_desc + (uint64_t)(cc * 64 * 128 / 16 + 2 * k), (kb | k) ? 1u : 0u);
+      sm90::wgmma_commit();
+      sm90::wgmma_wait<1>();
+      if (prev >= 0 && lane == 0) mbar_arrive(empty_bar + 8 * prev);
+      prev = slot;
+      if (++slot == p.stages) { slot = 0; phase ^= 1; }
+    }
+    sm90::wgmma_wait<0>();
+#pragma unroll
+    for (int cc = 0; cc < kNC; ++cc) sm90::acc_fence(acc[cc]);
+    if (lane == 0) mbar_arrive(empty_bar + 8 * prev);
+    PAIR_STAMP(0, i);
+    // ---- epilogue 1: acc1 + bias1 -> h16 -> relu -> three shifted K-major copies in shared memory.  Both warpgroups' stage-2 MMAs
+    // of the previous tile have completed (each waited for its own before its epilogue 2) once all 256 threads pass here.
+    sm90::bar_sync(1, 256);
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int m = 64 * wg + 16 * (warp & 3) + (lane >> 2) + 8 * h;   // tile row = pixel
+      const int px = m % p.tile_w;
+      // destination rows of this pixel's data in the three shifted copies (tap t reads x + (t-1) d): row m - (t-1) d
+      const bool ok0 = px + d < p.tile_w, ok2 = px - d >= 0;
+      const int r0 = m + d, r2 = m - d;
+#pragma unroll
+      for (int cc = 0; cc < kNC; ++cc)
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+          const int col = 64 * cc + 8 * j + 2 * (lane & 3);
+          const float2 b = *reinterpret_cast<const float2*>(ep_b1 + col);
+          const uint32_t v = relu2(pack_h16(acc[cc][4 * j + 2 * h] + b.x, acc[cc][4 * j + 2 * h + 1] + b.y));
+          uint8_t* blk = midp + cc * kABytes + (col & 7) * 2;              // K-block cc (64 channels), piece j, this pair
+          if (ok0) *reinterpret_cast<uint32_t*>(blk + 0 * kChunks * kABytes + r0 * 128 + ((j ^ (r0 & 7)) << 4)) = v;
+          *reinterpret_cast<uint32_t*>(blk + 1 * kChunks * kABytes + m * 128 + ((j ^ (m & 7)) << 4)) = v;
+          if (ok2) *reinterpret_cast<uint32_t*>(blk + 2 * kChunks * kABytes + r2 * 128 + ((j ^ (r2 & 7)) << 4)) = v;
+        }
+    }
+    proxy_fence_async();                             // generic-proxy stores -> visible to the tensor core's async-proxy reads
+    sm90::bar_sync(1, 256);
+    PAIR_STAMP(1, i);
+    // ---- stage 2: acc2 = conv1x3(mid)
+    prev = -1;
+    for (int kb0 = 0; kb0 < kNkb; kb0 += kBpf) {
+      mbar_wait(full_bar + 8 * slot, phase);
+      const uint32_t sa = base + slot * kSlotBytes;
+      sm90::wgmma_fence();
+#pragma unroll
+      for (int b = 0; b < kBpf; ++b) {
+        const uint64_t a_desc = sm90::desc_sw128(mid + (kb0 + b) * kABytes + wg * (kABytes / 2)), b_desc = sm90::desc_sw128(sa + b * kWBytes);   // kb = t*kchunks + kc
+#pragma unroll
+        for (int k = 0; k < kBlockK / 16; ++k)
+#pragma unroll
+          for (int cc = 0; cc < kNC; ++cc)
+            sm90::wgmma_n64(acc[cc], a_desc + (uint64_t)(2 * k), b_desc + (uint64_t)(cc * 64 * 128 / 16 + 2 * k), (kb0 | b | k) ? 1u : 0u);
+      }
+      sm90::wgmma_commit();
+      sm90::wgmma_wait<1>();
+      if (prev >= 0 && lane == 0) mbar_arrive(empty_bar + 8 * prev);
+      prev = slot;
+      if (++slot == p.stages) { slot = 0; phase ^= 1; }
+    }
+    sm90::wgmma_wait<0>();
+#pragma unroll
+    for (int cc = 0; cc < kNC; ++cc) sm90::acc_fence(acc[cc]);
+    if (lane == 0) mbar_arrive(empty_bar + 8 * prev);
+    PAIR_STAMP(2, i);
+    // ---- epilogue 2: acc2 + shift2 -> h16 (+ residual) -> ReLU -> NHWC
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int m = 64 * wg + 16 * (warp & 3) + (lane >> 2) + 8 * h;
+      const int py = m / p.tile_w, px = m - py * p.tile_w, y = y0 + py;
+      if (y >= p.h) continue;
+      const long long pix = ((long long)img * p.h + y) * p.w + px;
+#pragma unroll
+      for (int cc = 0; cc < kNC; ++cc)
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+          const int col = 64 * cc + 8 * j + 2 * (lane & 3);
+          const float2 t = *reinterpret_cast<const float2*>(ep_t2 + col);
+          uint32_t v = pack_h16(acc[cc][4 * j + 2 * h] + t.x, acc[cc][4 * j + 2 * h + 1] + t.y);
+          if (p.res) v = add2(v, __ldg(reinterpret_cast<const uint32_t*>(p.res + pix * kC + col)), relu_out);
+          else if (relu_out) v = relu2(v);
+          *reinterpret_cast<uint32_t*>(p.out + pix * kC + col) = v;
+        }
+    }
+    PAIR_STAMP(3, i);
   }
 }
 
@@ -477,13 +305,12 @@ extern "C" int lavb_conv_pair_umma(const lavb_conv_pair_desc* d, void* stream) {
   a.trace = g_pair_trace; a.trace_tiles = g_pair_trace_tiles;
   const int slot_bytes = kABytes + d->c * kBlockK * 2;
   const int mid_bytes = 3 * a.kchunks * kABytes;
-  // C = 64: TWO co-resident CTAs per SM (3 x 64 TMEM columns -> 256 each, ~100 KB of shared memory each): two independent tile
-  // pipelines hide the per-tile serial chain (TMA -> MMA -> epilogue 1 -> MMA -> epilogue 2) that bounds this kernel.
-  static int two_mode = -1;
-  if (two_mode < 0) { const char* e = getenv("LAVB_PAIR_TWO"); two_mode = e ? atoi(e) : 1; }
-  const bool two = two_mode && d->c == 64;
-  a.stages = min(kMaxStages, ((two ? 108 : 218) * 1024 - mid_bytes - kEpiWarps * 1024) / slot_bytes);
-  a.tmem_cols = d->c == 64 ? 256 : 512;          // acc1 x 2 + acc2 = 3c columns, power of two
+  const int ctrl_bytes = 1024 /*align*/ + 16 * kMaxStages + 2 * 128 * (int)sizeof(float);
+  // C = 64: TWO co-resident CTAs per SM (~113 KB of shared memory each)
+  const bool two = d->c == 64;
+  const int smem_cap = two ? 113 * 1024 : 227 * 1024;
+  a.stages = min(kMaxStages, (smem_cap - mid_bytes - ctrl_bytes) / slot_bytes);
+  const int smem = a.stages * slot_bytes + mid_bytes + ctrl_bytes;
   CUtensorMap tmap_a, tmap_w1, tmap_w2;
   {
     cuuint64_t dims[4] = {(cuuint64_t)d->c, (cuuint64_t)d->w, (cuuint64_t)d->h, (cuuint64_t)d->n};
@@ -505,13 +332,12 @@ extern "C" int lavb_conv_pair_umma(const lavb_conv_pair_desc* d, void* stream) {
                         CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     LAVB_CHECK_ARG(r == CUDA_SUCCESS, "conv_pair_umma: cuTensorMapEncodeTiled(W%d) failed with %d", which + 1, (int)r);
   }
-  const size_t smem = (size_t)a.stages * slot_bytes + mid_bytes + kEpiWarps * 1024 + 1024 /*align*/ + 16 * kMaxStages + 96 + 3 * 128 * sizeof(float);
   if (two) {
-    LAVB_CUDA_OK(ensure_dyn_smem((const void*)conv_pair_umma_kernel<2>, 113 * 1024));
-    conv_pair_umma_kernel<2><<<min(a.num_tiles, 2 * kNumSMs), 64 + 32 * kEpiWarps, smem, (cudaStream_t)stream>>>(tmap_a, tmap_w1, tmap_w2, a);
+    LAVB_CUDA_OK(ensure_dyn_smem((const void*)conv_pair_umma_kernel<64>, smem_cap));
+    conv_pair_umma_kernel<64><<<min(a.num_tiles, 2 * kNumSMs), kPairThreads, smem, (cudaStream_t)stream>>>(tmap_a, tmap_w1, tmap_w2, a);
   } else {
-    LAVB_CUDA_OK(ensure_dyn_smem((const void*)conv_pair_umma_kernel<1>, 227 * 1024));
-    conv_pair_umma_kernel<1><<<min(a.num_tiles, kNumSMs), 64 + 32 * kEpiWarps, smem, (cudaStream_t)stream>>>(tmap_a, tmap_w1, tmap_w2, a);
+    LAVB_CUDA_OK(ensure_dyn_smem((const void*)conv_pair_umma_kernel<128>, smem_cap));
+    conv_pair_umma_kernel<128><<<min(a.num_tiles, kNumSMs), kPairThreads, smem, (cudaStream_t)stream>>>(tmap_a, tmap_w1, tmap_w2, a);
   }
   LAVB_LAUNCH_OK();
   return 0;

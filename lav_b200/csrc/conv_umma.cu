@@ -1,28 +1,22 @@
-// tcgen05 / TMEM / TMA implicit-GEMM tap-list convolution (h16 in, fp32 accumulate in TMEM).
+// wgmma / TMA implicit-GEMM tap-list convolution (h16 in, fp32 accumulate in registers).
 //
-// GEMM view of one CTA tile: M = 128 output-grid pixels (an 8 x 16 spatial patch), N = cout (<= 256),
+// GEMM view of one CTA tile: M = 128 output-grid pixels (an 8 x 16 spatial patch), N = cout (<= 256, padded to 32),
 // K = ntaps * cin walked in blocks of 64 channels.  No im2col buffer exists anywhere: for tap (dy,dx) the
 // A operand of a K-block is ONE 4-D TMA box {64 ch, 16 px, 8 rows, 1 image} of the NHWC activation tensor whose
 // start coordinate is shifted by the tap offset (out-of-bounds rows/columns are zero-filled by TMA, which IS the
-// conv padding); with SWIZZLE_128B the box lands in shared memory exactly in the K-major layout tcgen05.mma reads
+// conv padding); with SWIZZLE_128B the box lands in shared memory exactly in the K-major layout wgmma reads
 // (128 rows x 128 B).  Strided convs use the tensor map's element strides; a transposed conv is issued per output
 // phase with its own tap list (same host packing as conv_taps.cu).
 //
-// Warp roles (320 threads, 1 CTA/SM, persistent over tiles):
-//   warp 0   : TMA producer (one lane)      — smem ring of `stages` {A 16 KB, B cout*128 B}
-//   warp 1   : TMEM allocator + MMA issuer  — 4 x tcgen05.mma (M128,N=cout,K16) per K-block, commit -> empty barrier
-//   warps 2-9: epilogue (2 per TMEM lane quarter, alternating 32-column chunks) — tcgen05.ld 32x32b.x32,
-//              max/FMA with (scale,shift) pairs broadcast from smem, residual, 16 B global stores; flag-free inner loop
-// Two TMEM accumulator stages let the epilogue of tile i overlap the MMAs of tile i+1.
+// Warp roles (288 threads, persistent over tiles):
+//   warps 0-3, 4-7: two consumer warpgroups, one per 64-pixel half of the tile (tile rows 0-3 / 4-7).  Each issues
+//                   m64 x N x k16 wgmma over its half of the A block and the whole B block, keeps one K-block of MMAs in
+//                   flight, and runs the epilogue (bias / BN affine / ReLU / residual / sigmoid) from its registers.
+//   warp 8         : TMA producer (one lane) — smem ring of `stages` {A 16 KB, B cout*128 B}
+// Layers with cout <= 128 run two CTAs per SM so that one CTA's epilogue overlaps the other's MMAs.
 #include <cuda.h>
-#include <stdlib.h>
-// conv_umma16.cu re-includes this file with these two set to 2 / 8 (8 epilogue warps AND two CTAs per SM for the narrow layers)
-#ifndef LAVB_UMMA_EW8_MINBLOCKS
-#define LAVB_UMMA_EW8_MINBLOCKS 1
-#define LAVB_UMMA_NARROW_EW 4
-#endif
 #include <cudaTypedefs.h>
-#include "common.cuh"
+#include "sm90.cuh"
 
 namespace lavb {
 
@@ -30,14 +24,14 @@ constexpr int kTileH = 8, kTileW = 16, kBlockM = 128, kBlockK = 64;
 constexpr int kABytes = kBlockM * kBlockK * 2;  // 16 KB
 constexpr int kMaxStages = 8;
 constexpr int kMaxTaps = 16;
+constexpr int kConvThreads = 288;
 
-struct UmmaArgs {
+struct ConvArgs {
   int n, hog, wog, tiles_x, tiles_y, num_tiles;
-  int hout, wout, cin, cout, kchunks, ntaps, stages, tmem_cols;
+  int hout, wout, cin, cout, kchunks, ntaps, stages;
   int in_sy, in_sx, out_sy, out_sx, out_oy, out_ox;
   int out_cstride, out_coff, out_is_f32, res_cstride, res_coff;
-  int pre_relu, post_relu, sigmoid, d2s_nout, cout_store;
-  int wres;   // weights-stationary: all ntaps*kchunks B blocks are loaded once per CTA and stay in shared memory
+  int pre_bias, pre_relu, post_relu, sigmoid, d2s_nout, cout_store;
   int dy[kMaxTaps], dx[kMaxTaps];
   void* out; const h16* res;
   const float* bias; const float* scale; const float* shift;
@@ -74,75 +68,31 @@ __device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* map
       "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
       ::"r"(dst), "l"(reinterpret_cast<uint64_t>(map)), "r"(bar), "r"(c0), "r"(c1) : "memory");
 }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-// K-major, SWIZZLE_128B shared-memory matrix descriptor (cute::UMMA::SmemDescriptor bit layout):
-// start>>4 [0,14) | LBO>>4 [16,30) = 0 | SBO>>4 [32,46) = 1024>>4 | version=1 [46,48) | layout=SWIZZLE_128B(2) [61,64)
-__device__ __forceinline__ uint64_t make_sw128_desc(uint32_t saddr) {
-  const uint32_t lo = (saddr & 0x3FFFFu) >> 4;
-  const uint32_t hi = (1024u >> 4) | (1u << 14) | (2u << 29);
-  return (uint64_t)lo | ((uint64_t)hi << 32);
-}
-__device__ __forceinline__ void umma_h16(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate) : "memory");
-}
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&v)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-        "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]),
-        "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]),
-        "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-      : "r"(taddr) : "memory");
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-
-// kEpiWarps = 8: two warps per TMEM lane quarter (they split the column chunks), one CTA per SM — wide layers (cout > 128).
-// kEpiWarps = 4: one warp per quarter and TWO co-resident CTAs per SM (half the smem ring each): two independent tile
-//                pipelines hide the per-tile serial chain (commit -> epilogue -> tmem_empty) of the narrow layers.
-template <bool kOutF32, bool kRes, bool kSigmoid, bool kPreBias, int kEpiWarps, bool kD2S = false>
-__global__ void __launch_bounds__(64 + 32 * kEpiWarps, kEpiWarps == 4 ? 2 : LAVB_UMMA_EW8_MINBLOCKS) conv_umma_kernel(const __grid_constant__ CUtensorMap tmap_a,
-                                                                const __grid_constant__ CUtensorMap tmap_b,
-                                                                const __grid_constant__ UmmaArgs p) {
+// kNC = cout_mma / 32 (the MMA width in 32-column chunks)
+template <int kNC>
+__global__ void __launch_bounds__(kConvThreads, kNC <= 4 ? 2 : 1) conv_umma_kernel(const __grid_constant__ CUtensorMap tmap_a,
+                                                                                 const __grid_constant__ CUtensorMap tmap_b,
+                                                                                 const __grid_constant__ ConvArgs p) {
+  constexpr int kN = 32 * kNC;
+  constexpr int kBBytes = kN * kBlockK * 2;
+  constexpr int kStageBytes = kABytes + kBBytes;
   extern __shared__ uint8_t smem_raw[];
   const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;   // SWIZZLE_128B operands need 1024 B alignment
-  const int b_bytes = p.cout * kBlockK * 2;
-  const bool wres = p.wres != 0;
-  const int stage_bytes = wres ? kABytes : kABytes + b_bytes;     // the ring carries A only when the weights are resident
-  const uint32_t bres = base + p.stages * stage_bytes;            // resident weights: [ntaps*kchunks][cout x 64] (wres)
-  const uint32_t stage_out = bres + (wres ? p.ntaps * p.kchunks * b_bytes : 0);   // kEpiWarps x 1 KB store-transposition buffers
-  const uint32_t ctrl = stage_out + kEpiWarps * 1024;
-  const uint32_t full_bar = ctrl, empty_bar = ctrl + 8 * kMaxStages, tfull_bar = ctrl + 16 * kMaxStages,
-                 tempty_bar = tfull_bar + 16, tmem_slot = tempty_bar + 16, wbar = tmem_slot + 8;
   uint8_t* gen = smem_raw + (base - smem_u32(smem_raw));
-  volatile uint32_t* tmem_slot_p = reinterpret_cast<volatile uint32_t*>(gen + (tmem_slot - base));
-  float* ep_bias = reinterpret_cast<float*>(gen + (tmem_slot - base) + 16);   // only read when kPreBias
-  float* ep_st = ep_bias + 256;                                               // interleaved (scale, shift) per channel
+  const uint32_t ctrl = base + p.stages * kStageBytes;
+  const uint32_t full_bar = ctrl, empty_bar = ctrl + 8 * kMaxStages;
+  float* ep_bias = reinterpret_cast<float*>(gen + (ctrl - base) + 16 * kMaxStages);   // only read when pre_bias
+  float* ep_st = ep_bias + 256;                                                       // interleaved (scale, shift) per channel
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-
   if (threadIdx.x == 0) {
     asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmap_a)) : "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmap_b)) : "memory");
-    for (int s = 0; s < p.stages; ++s) { mbar_init(full_bar + 8 * s, 1); mbar_init(empty_bar + 8 * s, 1); }
-    for (int a = 0; a < 2; ++a) { mbar_init(tfull_bar + 8 * a, 1); mbar_init(tempty_bar + 8 * a, 32 * kEpiWarps); }
-    mbar_init(wbar, 1);
+    // empty: one arrival per consumer warp once its MMAs have read the slot
+    for (int s = 0; s < p.stages; ++s) { mbar_init(full_bar + 8 * s, 1); mbar_init(empty_bar + 8 * s, 8); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(tmem_slot), "r"((uint32_t)p.tmem_cols) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  for (int c = threadIdx.x; c < p.cout; c += blockDim.x) {
+  for (int c = threadIdx.x; c < kN; c += blockDim.x) {
     // epi(a) = max(a + b, lo) * s + t.  Without the pre-ReLU the bias folds into the shift: (a + b) s + t = a s + (b s + t)
     const bool real = c < p.cout_store;      // columns past cout_store are MMA padding (never stored)
     const float b = (p.bias && real) ? __ldg(p.bias + c) : 0.f;
@@ -150,201 +100,106 @@ __global__ void __launch_bounds__(64 + 32 * kEpiWarps, kEpiWarps == 4 ? 2 : LAVB
     const float sh = (p.shift && real) ? __ldg(p.shift + c) : 0.f;
     ep_bias[c] = b;
     ep_st[2 * c] = sc;
-    ep_st[2 * c + 1] = kPreBias ? sh : fmaf(b, sc, sh);
+    ep_st[2 * c + 1] = p.pre_bias ? sh : fmaf(b, sc, sh);
   }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot_p;
   const int nkb = p.ntaps * p.kchunks;
   const int tiles_per_img = p.tiles_x * p.tiles_y;
 
-  if (warp == 0) {
+  if (warp == 8) {
     if (lane == 0) {
       int stage = 0; uint32_t phase = 0;
-      if (wres) {   // narrow layers are bound by L2->SM fill bandwidth: fetch the weights once per CTA, not once per tile
-        mbar_expect_tx(wbar, (uint32_t)(nkb * b_bytes));
-        for (int kb = 0; kb < nkb; ++kb)
-          tma_load_2d(bres + kb * b_bytes, &tmap_b, wbar, (kb % p.kchunks) * kBlockK, (kb / p.kchunks) * p.cout);
-      }
       for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
         const int img = tile / tiles_per_img, r = tile - img * tiles_per_img;
         const int y0 = (r / p.tiles_x) * kTileH * p.in_sy, x0 = (r % p.tiles_x) * kTileW * p.in_sx;
         for (int t = 0; t < p.ntaps; ++t) {
           for (int kc = 0; kc < p.kchunks; ++kc) {
             mbar_wait(empty_bar + 8 * stage, phase ^ 1);
-            const uint32_t sa = base + stage * stage_bytes;
-            mbar_expect_tx(full_bar + 8 * stage, stage_bytes);
+            const uint32_t sa = base + stage * kStageBytes;
+            mbar_expect_tx(full_bar + 8 * stage, kStageBytes);
             tma_load_4d(sa, &tmap_a, full_bar + 8 * stage, kc * kBlockK, x0 + p.dx[t], y0 + p.dy[t], img);
-            if (!wres) tma_load_2d(sa + kABytes, &tmap_b, full_bar + 8 * stage, kc * kBlockK, t * p.cout);
+            tma_load_2d(sa + kABytes, &tmap_b, full_bar + 8 * stage, kc * kBlockK, t * kN);
             if (++stage == p.stages) { stage = 0; phase ^= 1; }
           }
         }
       }
     }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      // instruction descriptor: D=f32 [4,6)=1, A=h16 [7,10)=1, B=h16 [10,13)=1, K-major both, N>>3 [17,23), M>>4 [24,29)
-      const uint32_t idesc = (1u << 4) | (kH16Fmt << 7) | (kH16Fmt << 10) | ((uint32_t)(p.cout >> 3) << 17) | ((uint32_t)(kBlockM >> 4) << 24);
-      int stage = 0; uint32_t phase = 0;
-      int acc = 0; uint32_t acc_phase = 0;
-      if (wres) { mbar_wait(wbar, 0); tc_fence_after(); }
-      for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
-        mbar_wait(tempty_bar + 8 * acc, acc_phase ^ 1);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + (uint32_t)(acc * p.cout);
-        for (int kb = 0; kb < nkb; ++kb) {
-          mbar_wait(full_bar + 8 * stage, phase);
-          tc_fence_after();
-          const uint32_t sa = base + stage * stage_bytes;
-          const uint64_t a_desc = make_sw128_desc(sa), b_desc = make_sw128_desc(wres ? bres + kb * b_bytes : sa + kABytes);
+    return;
+  }
+
+  const int wg = warp >> 2;                        // tile rows [64 wg, 64 wg + 64)
+  const float lo_pre = p.pre_relu ? 0.f : -INFINITY, lo_post = p.post_relu ? 0.f : -INFINITY;
+  int stage = 0; uint32_t phase = 0;
+  float acc[kNC][16];
+  for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
+    int prev_stage = -1;
+    for (int kb = 0; kb < nkb; ++kb) {
+      mbar_wait(full_bar + 8 * stage, phase);
+      const uint32_t sa = base + stage * kStageBytes;
+      const uint64_t a_desc = sm90::desc_sw128(sa + wg * (kABytes / 2)), b_desc = sm90::desc_sw128(sa + kABytes);
+      sm90::wgmma_fence();
 #pragma unroll
-          for (int k = 0; k < kBlockK / 16; ++k)   // +32 B per K16 step inside the 128 B swizzle atom
-            umma_h16(d_tmem, a_desc + (uint64_t)(2 * k), b_desc + (uint64_t)(2 * k), idesc, (kb | k) ? 1u : 0u);
-          umma_commit(empty_bar + 8 * stage);      // frees the smem slot once these MMAs have read it
-          if (++stage == p.stages) { stage = 0; phase ^= 1; }
-        }
-        umma_commit(tfull_bar + 8 * acc);          // accumulator complete -> epilogue
-        if (++acc == 2) { acc = 0; acc_phase ^= 1; }
-      }
+      for (int k = 0; k < kBlockK / 16; ++k)       // +32 B per K16 step inside the 128 B swizzle atom
+#pragma unroll
+        for (int c = 0; c < kNC; ++c)              // 32 B-rows of 128 B per chunk
+          sm90::wgmma_n32(acc[c], a_desc + (uint64_t)(2 * k), b_desc + (uint64_t)(c * 32 * 128 / 16 + 2 * k), (kb | k) ? 1u : 0u);
+      sm90::wgmma_commit();
+      sm90::wgmma_wait<1>();                             // the previous K-block's MMAs are done: its slot may be refilled
+      if (prev_stage >= 0 && lane == 0) mbar_arrive(empty_bar + 8 * prev_stage);
+      prev_stage = stage;
+      if (++stage == p.stages) { stage = 0; phase ^= 1; }
     }
-  } else {
-    const int q = warp & 3;                        // TMEM lane quarter this warp may read (warp id % 4)
-    const int half = (warp - 2) >> 2;              // with 8 warps the two warps of a quarter take alternate 32-column chunks
-    constexpr int kChunkStride = 32 * (kEpiWarps / 4);
-    const int row = q * 32 + lane;
-    const int py = row / kTileW, px = row % kTileW;
-    const float lo_pre = p.pre_relu ? 0.f : -INFINITY, lo_post = p.post_relu ? 0.f : -INFINITY;
-    int acc = 0; uint32_t acc_phase = 0;
-    for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
-      const int img = tile / tiles_per_img, r = tile - img * tiles_per_img;
-      const int ty0 = (r / p.tiles_x) * kTileH, tx0 = (r % p.tiles_x) * kTileW;
-      const int gy = ty0 + py, gx = tx0 + px;
+    sm90::wgmma_wait<0>();
+#pragma unroll
+    for (int c = 0; c < kNC; ++c) sm90::acc_fence(acc[c]);
+    if (prev_stage >= 0 && lane == 0) mbar_arrive(empty_bar + 8 * prev_stage);
+
+    // ---- epilogue: this thread holds rows m and m + 8 of the tile, two adjacent columns per 8-column group
+    const int img = tile / tiles_per_img, r = tile - img * tiles_per_img;
+    const int ty0 = (r / p.tiles_x) * kTileH, tx0 = (r % p.tiles_x) * kTileW;
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int m = 64 * wg + 16 * (warp & 3) + (lane >> 2) + 8 * h;
+      const int gy = ty0 + m / kTileW, gx = tx0 + m % kTileW;
       const int oy = gy * p.out_sy + p.out_oy, ox = gx * p.out_sx + p.out_ox;
-      const bool valid = gy < p.hog && gx < p.wog && oy < p.hout && ox < p.wout;
+      if (!(gy < p.hog && gx < p.wog && oy < p.hout && ox < p.wout)) continue;
       const long long pix = ((long long)img * p.hout + oy) * p.wout + ox;
-      mbar_wait(tfull_bar + 8 * acc, acc_phase);
-      tc_fence_after();
-      for (int c0 = half * 32; c0 < p.cout; c0 += kChunkStride) {
-        uint8_t* stg = gen + (stage_out - base) + (warp - 2) * 1024;
-        // residual, loaded with the coalesced mapping (4 lanes x 16 B per pixel; rr[2 hp + k] = pixel 8k + lane/4 of tile row
-        // 2q + hp, piece lane%4) before the accumulator read, transposed to "lane = pixel" through the staging buffer below
-        uint4 rr[4];
-        if (kRes) {
 #pragma unroll
-          for (int e = 0; e < 4; ++e) {
-            const int gy2 = ty0 + 2 * q + (e >> 1), gx2 = tx0 + 8 * (e & 1) + (lane >> 2);
-            const int oy2 = gy2 * p.out_sy + p.out_oy, ox2 = gx2 * p.out_sx + p.out_ox;
-            rr[e] = make_uint4(0u, 0u, 0u, 0u);
-            if (gy2 < p.hog && gx2 < p.wog && oy2 < p.hout && ox2 < p.wout)
-              rr[e] = __ldg(reinterpret_cast<const uint4*>(p.res + (((long long)img * p.hout + oy2) * p.wout + ox2) * p.res_cstride + p.res_coff + c0 + 8 * (lane & 3)));
+      for (int c = 0; c < kNC; ++c) {
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+          const int col = 32 * c + 8 * i + 2 * (lane & 3);
+          float x0 = acc[c][4 * i + 2 * h], x1 = acc[c][4 * i + 2 * h + 1];
+          if (p.pre_bias) { x0 += ep_bias[col]; x1 += ep_bias[col + 1]; }
+          const float4 st = *reinterpret_cast<const float4*>(ep_st + 2 * col);   // (s0, t0, s1, t1)
+          x0 = fmaf(fmaxf(x0, lo_pre), st.x, st.y);
+          x1 = fmaf(fmaxf(x1, lo_pre), st.z, st.w);
+          if (p.res) {
+            const float2 rv = unpack_h16(__ldg(reinterpret_cast<const uint32_t*>(p.res + pix * p.res_cstride + p.res_coff + col)));
+            x0 += rv.x; x1 += rv.y;
           }
-        }
-        uint32_t v[32];
-        tmem_ld32(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(acc * p.cout + c0), v);
-        float f[32];
-        const float4* st4 = reinterpret_cast<const float4*>(ep_st + 2 * c0);   // (s0,t0,s1,t1): broadcast LDS.128
-#pragma unroll
-        for (int j = 0; j < 16; ++j) {
-          const float4 st = st4[j];
-          float x0 = __uint_as_float(v[2 * j]), x1 = __uint_as_float(v[2 * j + 1]);
-          if (kPreBias) { x0 += ep_bias[c0 + 2 * j]; x1 += ep_bias[c0 + 2 * j + 1]; }
-          f[2 * j] = fmaf(fmaxf(x0, lo_pre), st.x, st.y);
-          f[2 * j + 1] = fmaf(fmaxf(x1, lo_pre), st.z, st.w);
-        }
-        if (kRes) {
-#pragma unroll
-          for (int hp = 0; hp < 2; ++hp) {
-#pragma unroll
-            for (int k = 0; k < 2; ++k) {
-              const int rr_ = 8 * k + (lane >> 2), j = lane & 3;
-              *reinterpret_cast<uint4*>(stg + rr_ * 64 + ((j ^ ((rr_ >> 1) & 3)) << 4)) = rr[2 * hp + k];
-            }
-            __syncwarp();
-            if ((lane >> 4) == hp) {
-              const int rr_ = lane & 15;
-#pragma unroll
-              for (int j = 0; j < 4; ++j) {
-                const uint4 q4 = *reinterpret_cast<const uint4*>(stg + rr_ * 64 + ((j ^ ((rr_ >> 1) & 3)) << 4));
-                const uint32_t w[4] = {q4.x, q4.y, q4.z, q4.w};
-#pragma unroll
-                for (int e = 0; e < 4; ++e) {
-                  const float2 t2 = h1622float2(*reinterpret_cast<const h162*>(&w[e]));
-                  f[j * 8 + e * 2] += t2.x; f[j * 8 + e * 2 + 1] += t2.y;
-                }
-              }
-            }
-            __syncwarp();
-          }
-        }
-        if (valid) {
-#pragma unroll
-          for (int j = 0; j < 32; ++j) {
-            f[j] = fmaxf(f[j], lo_post);
-            if (kSigmoid) f[j] = 1.f / (1.f + expf(-f[j]));
-          }
-          if (kD2S) {   // depth-to-space: column j = pos*nout + k -> pixel (oy + pos/2, ox + pos%2), channel k
+          x0 = fmaxf(x0, lo_post); x1 = fmaxf(x1, lo_post);
+          if (p.sigmoid) { x0 = 1.f / (1.f + expf(-x0)); x1 = 1.f / (1.f + expf(-x1)); }
+          if (p.d2s_nout) {   // depth-to-space: column j = pos*nout + k -> pixel (oy + pos/2, ox + pos%2), channel k
             float* ob = reinterpret_cast<float*>(p.out);
             const int no = p.d2s_nout;
 #pragma unroll
-            for (int j = 0; j < 32; ++j) {
+            for (int e = 0; e < 2; ++e) {
+              const int j = col + e;
               if (j < 4 * no) {
                 const int pos = j / no, k = j - pos * no;
-                ob[(pix + (long long)(pos >> 1) * p.wout + (pos & 1)) * no + k] = f[j];
+                ob[(pix + (long long)(pos >> 1) * p.wout + (pos & 1)) * no + k] = e ? x1 : x0;
               }
             }
-          } else if (kOutF32) {
-            float4* op = reinterpret_cast<float4*>(reinterpret_cast<float*>(p.out) + pix * p.out_cstride + p.out_coff + c0);
-#pragma unroll
-            for (int j = 0; j < 8; ++j)
-              if (c0 + 4 * j < p.cout_store) op[j] = make_float4(f[4 * j], f[4 * j + 1], f[4 * j + 2], f[4 * j + 3]);
-          }
-        }
-        if (!kD2S && !kOutF32) {
-          // h16 NHWC store through a per-warp shared-memory transposition (same scheme as conv_pair_umma.cu): a lane owns 64
-          // contiguous bytes of ITS pixel, so a direct 16-byte store per lane touches 32 different lines per instruction;
-          // re-mapped, 4 lanes cover the 64 bytes of one pixel and an instruction writes 8 pixels in full sectors.  One pass =
-          // the 16 pixels of one spatial row of the 8 x 16 tile (tile row 2q + hp), 1 KB per warp, bank-conflict free both ways.
-          uint32_t w16[16];
-#pragma unroll
-          for (int j = 0; j < 16; ++j) {
-            const h162 b2 = floats2h162(f[2 * j], f[2 * j + 1]);
-            w16[j] = *reinterpret_cast<const uint32_t*>(&b2);
-          }
-#pragma unroll
-          for (int hp = 0; hp < 2; ++hp) {
-            if ((lane >> 4) == hp) {
-              const int rr_ = lane & 15;
-#pragma unroll
-              for (int j = 0; j < 4; ++j)
-                *reinterpret_cast<uint4*>(stg + rr_ * 64 + ((j ^ ((rr_ >> 1) & 3)) << 4)) = make_uint4(w16[4 * j], w16[4 * j + 1], w16[4 * j + 2], w16[4 * j + 3]);
-            }
-            __syncwarp();
-            const int gy2 = ty0 + 2 * q + hp, oy2 = gy2 * p.out_sy + p.out_oy;
-#pragma unroll
-            for (int k = 0; k < 2; ++k) {
-              const int rr_ = 8 * k + (lane >> 2), j = lane & 3;
-              const int gx2 = tx0 + rr_, ox2 = gx2 * p.out_sx + p.out_ox;
-              if (gy2 < p.hog && gx2 < p.wog && oy2 < p.hout && ox2 < p.wout && c0 + 8 * j < p.cout_store) {
-                const uint4 val = *reinterpret_cast<const uint4*>(stg + rr_ * 64 + ((j ^ ((rr_ >> 1) & 3)) << 4));
-                *reinterpret_cast<uint4*>(reinterpret_cast<h16*>(p.out) + (((long long)img * p.hout + oy2) * p.wout + ox2) * p.out_cstride +
-                                          p.out_coff + c0 + 8 * j) = val;
-              }
-            }
-            __syncwarp();
+          } else if (col < p.cout_store) {
+            if (p.out_is_f32)
+              *reinterpret_cast<float2*>(reinterpret_cast<float*>(p.out) + pix * p.out_cstride + p.out_coff + col) = make_float2(x0, x1);
+            else
+              *reinterpret_cast<uint32_t*>(reinterpret_cast<h16*>(p.out) + pix * p.out_cstride + p.out_coff + col) = pack_h16(x0, x1);
           }
         }
       }
-      tc_fence_before();
-      mbar_arrive(tempty_bar + 8 * acc);
-      if (++acc == 2) { acc = 0; acc_phase ^= 1; }
     }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"((uint32_t)p.tmem_cols) : "memory");
   }
 }
 
@@ -403,34 +258,23 @@ extern "C" int lavb_conv_umma(const lavb_conv_desc* d, void* stream) {
                         CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     LAVB_CHECK_ARG(r == CUDA_SUCCESS, "conv_umma: cuTensorMapEncodeTiled(B) failed with %d", (int)r);
   }
-  UmmaArgs a;
+  ConvArgs a;
   memset(&a, 0, sizeof(a));
   a.n = d->n; a.hog = d->hog; a.wog = d->wog;
   a.tiles_x = ceil_div(d->wog, kTileW); a.tiles_y = ceil_div(d->hog, kTileH);
   a.num_tiles = a.n * a.tiles_x * a.tiles_y;
   a.hout = d->hout; a.wout = d->wout; a.cin = d->cin; a.cout = cout_mma; a.cout_store = d->cout; a.kchunks = d->cin / kBlockK;
   a.ntaps = d->ntaps;
-  int stage_bytes = kABytes + cout_mma * kBlockK * 2;
-  bool two_per_sm = cout_mma <= 128;                  // narrow layers: 2 CTAs / SM, each with half the smem ring
-  // weights-stationary mode (LAVB_WRES: 0 off, 1 = layers whose weights fit beside a 2-CTA/SM ring, 2 = also 1-CTA/SM)
-  static int wres_mode = -1;
-  if (wres_mode < 0) { const char* e = getenv("LAVB_WRES"); wres_mode = e ? atoi(e) : 1; }
-  const int res_bytes = d->ntaps * a.kchunks * cout_mma * kBlockK * 2;
-  if (wres_mode >= 1 && two_per_sm && res_bytes <= 48 * 1024) {
-    a.wres = 1; stage_bytes = kABytes;
-    a.stages = min(kMaxStages, (100 * 1024 - res_bytes) / kABytes);
-  } else if (wres_mode >= 2 && two_per_sm && res_bytes <= 96 * 1024) {
-    a.wres = 1; stage_bytes = kABytes; two_per_sm = false;
-    a.stages = min(kMaxStages, (200 * 1024 - res_bytes) / kABytes);
-  } else {
-    a.stages = two_per_sm ? min(kMaxStages, (100 * 1024) / stage_bytes) : min(kMaxStages, (196 * 1024) / stage_bytes);
-  }
-  int cols = 32;
-  while (cols < 2 * cout_mma) cols <<= 1;
-  a.tmem_cols = cols;
+  const int nc = cout_mma / 32;
+  const bool two_per_sm = nc <= 4;                    // narrow layers: 2 CTAs / SM, each with half the shared memory
+  const int stage_bytes = kABytes + cout_mma * kBlockK * 2;
+  const int ctrl_bytes = 1024 /*align*/ + 16 * kMaxStages + 3 * 256 * (int)sizeof(float);
+  const int smem_cap = two_per_sm ? 113 * 1024 : 227 * 1024;
+  a.stages = min(kMaxStages, (smem_cap - ctrl_bytes) / stage_bytes);
   a.in_sy = d->in_sy; a.in_sx = d->in_sx; a.out_sy = d->out_sy; a.out_sx = d->out_sx; a.out_oy = d->out_oy; a.out_ox = d->out_ox;
   a.out_cstride = d->out_cstride; a.out_coff = d->out_coff; a.out_is_f32 = d->out_dtype == LAVB_F32;
   a.res_cstride = d->res_cstride; a.res_coff = d->res_coff;
+  a.pre_bias = d->pre_relu && d->bias != nullptr;
   a.pre_relu = d->pre_relu; a.post_relu = d->post_relu; a.sigmoid = d->sigmoid; a.d2s_nout = d->d2s_nout;
   if (d->d2s_nout) {
     LAVB_CHECK_ARG(d->cout == 32 && d->d2s_nout >= 1 && 4 * d->d2s_nout <= 32 && d->out_dtype == LAVB_F32 && d->out_sy == 2 &&
@@ -440,39 +284,20 @@ extern "C" int lavb_conv_umma(const lavb_conv_desc* d, void* stream) {
   a.out = d->out; a.res = reinterpret_cast<const h16*>(d->res);
   a.bias = d->bias; a.scale = d->scale; a.shift = d->shift;
   if (a.num_tiles == 0) return 0;
-  const size_t smem = (size_t)a.stages * stage_bytes + (a.wres ? res_bytes : 0) + (two_per_sm ? 4 : 8) * 1024 /*store staging: 1 KB per epilogue warp*/ + 1024 /*align*/ + 16 * kMaxStages + 64 + 3 * 256 * sizeof(float);
+  const int smem = a.stages * stage_bytes + ctrl_bytes;
   const int grid = min(a.num_tiles, two_per_sm ? 2 * kNumSMs : kNumSMs);
-  if (a.d2s_nout) {
-#define LAVB_D2S(S)                                                                                                     \
-    {                                                                                                                   \
-      LAVB_CUDA_OK(ensure_dyn_smem((const void*)conv_umma_kernel<true, false, S, false, 4, true>, 112 * 1024));         \
-      conv_umma_kernel<true, false, S, false, 4, true><<<grid, 64 + 32 * 4, smem, (cudaStream_t)stream>>>(tmap_a, tmap_b, a); \
-      LAVB_LAUNCH_OK();                                                                                                 \
-      return 0;                                                                                                         \
-    }
-    if (a.sigmoid) LAVB_D2S(true) else LAVB_D2S(false)
-#undef LAVB_D2S
+#define LAVB_CONV_LAUNCH(NC)                                                                                              \
+  case NC: {                                                                                                              \
+    /* once per (variant, device), never during a later stream capture (callers warm up first) */                         \
+    LAVB_CUDA_OK(ensure_dyn_smem((const void*)conv_umma_kernel<NC>, smem_cap));                                          \
+    conv_umma_kernel<NC><<<grid, kConvThreads, smem, (cudaStream_t)stream>>>(tmap_a, tmap_b, a);                          \
+    break;                                                                                                                \
   }
-  const bool f32 = a.out_is_f32, res = a.res != nullptr, sig = a.sigmoid != 0, pb = a.pre_relu && a.bias != nullptr;
-  // epilogue variants are compiled separately so the inner loop carries no runtime flag tests
-#define LAVB_UMMA_LAUNCH(F, R, S, B, EW)                                                                                \
-  {                                                                                                                     \
-    /* once per (variant, device), never during a later stream capture (callers warm up first) */                       \
-    LAVB_CUDA_OK(ensure_dyn_smem((const void*)conv_umma_kernel<F, R, S, B, EW>, EW == 4 ? 112 * 1024 : 227 * 1024));    \
-    conv_umma_kernel<F, R, S, B, EW><<<grid, 64 + 32 * EW, smem, (cudaStream_t)stream>>>(tmap_a, tmap_b, a);            \
-    LAVB_LAUNCH_OK();                                                                                                   \
-    return 0;                                                                                                           \
+  switch (nc) {
+    LAVB_CONV_LAUNCH(1) LAVB_CONV_LAUNCH(2) LAVB_CONV_LAUNCH(3) LAVB_CONV_LAUNCH(4)
+    LAVB_CONV_LAUNCH(5) LAVB_CONV_LAUNCH(6) LAVB_CONV_LAUNCH(7) LAVB_CONV_LAUNCH(8)
   }
-#define LAVB_UMMA_CASE(F, R, S, B)                                                                                      \
-  if (f32 == F && res == R && sig == S && pb == B) {                                                                    \
-    if (two_per_sm) LAVB_UMMA_LAUNCH(F, R, S, B, LAVB_UMMA_NARROW_EW) else LAVB_UMMA_LAUNCH(F, R, S, B, 8)              \
-  }
-  LAVB_UMMA_CASE(false, false, false, false) LAVB_UMMA_CASE(false, true, false, false)
-  LAVB_UMMA_CASE(true, false, false, false)  LAVB_UMMA_CASE(true, true, false, false)
-  LAVB_UMMA_CASE(false, false, true, false)  LAVB_UMMA_CASE(true, false, true, false)
-  LAVB_UMMA_CASE(false, false, false, true)  LAVB_UMMA_CASE(false, true, false, true)
-  LAVB_UMMA_CASE(true, false, false, true)   LAVB_UMMA_CASE(true, true, false, true)
-#undef LAVB_UMMA_CASE
-#undef LAVB_UMMA_LAUNCH
-  LAVB_CHECK_ARG(false, "conv_umma: this epilogue combination (sigmoid with residual / pre-ReLU bias) is not compiled");
+#undef LAVB_CONV_LAUNCH
+  LAVB_LAUNCH_OK();
+  return 0;
 }

@@ -2,7 +2,7 @@
 // a pillar is addressed directly by (b, xi, yi); pass 1 accumulates the per-pillar centroid sums, pass 2
 // decorates each point, runs the 2-layer point MLP and max-pools into the NHWC canvas.
 #include <stdlib.h>
-#include "common.cuh"
+#include "sm90.cuh"
 
 namespace lavb {
 
@@ -782,55 +782,15 @@ __global__ void __launch_bounds__(256) tile_scatter_kernel(const float* __restri
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
-// tcgen05 version of the tile encoder: the point MLP runs on the 5th-generation tensor cores, one row per thread.
-// A chunk = 128 records of the tile = the 128 rows of an M=128 UMMA:
+// Tensor-core version of the tile encoder: the point MLP runs as warpgroup MMAs (wgmma), the CTA being one warpgroup.
+// A chunk = 128 records of the tile = the 128 rows of two m64 MMAs:
 //   thread r decorates its record and writes row r of the A operand in shared memory (K-major, SWIZZLE_128B, written by hand:
 //   16-byte piece j of row r lives at r*128 + ((j ^ (r & 7)) << 4)) as [hi(16) | lo(16) | hi(16) | 0] h16 — the error-free
 //   split of the fp32 features — against B1 = [W1_hi ; W1_hi ; W1_lo ; 0]: three K16 steps give hi*Wh + lo*Wh + hi*Wl ~ fp32;
-//   D1 (128 x 64 fp32) lands in TMEM; each thread reads ITS row back (tcgen05.ld 32x32b), applies BN1 + ReLU and writes the
-//   h16 hidden row in place as the A operand of layer 2 (K = 64 against B2 = W2); D2 -> BN2; the max-pool is one shared-memory
-//   atomicMax per (row, positive channel) into the fp32 tile.
-// ~450 thread-instructions per point instead of ~1800 with mma.sync fragments.
+//   D1 (128 x 64 fp32) lands in registers; each thread applies BN1 + ReLU to its fragment and writes it back in h16 as the
+//   A operand of layer 2 (K = 64 against B2 = W2); D2 -> BN2; the max-pool is one shared-memory atomicMax per
+//   (row, positive channel) into the fp32 tile.
 // ---------------------------------------------------------------------------------------------------------------------
-namespace tc {
-__device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) { asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count)); }
-__device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
-  uint32_t done;
-  do {
-    asm volatile("{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\tselp.u32 %0, 1, 0, p;\n\t}"
-                 : "=r"(done) : "r"(bar), "r"(parity) : "memory");
-  } while (!done);
-}
-__device__ __forceinline__ void fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void proxy_fence() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ uint64_t sw128_desc(uint32_t saddr) {      // K-major SWIZZLE_128B, SBO = 1024 B, version 1
-  const uint32_t lo = (saddr & 0x3FFFFu) >> 4;
-  const uint32_t hi = (1024u >> 4) | (1u << 14) | (2u << 29);
-  return (uint64_t)lo | ((uint64_t)hi << 32);
-}
-__device__ __forceinline__ void umma(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\ttcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-               ::"r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate) : "memory");
-}
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&v)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-        "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]),
-        "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]),
-        "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-      : "r"(taddr) : "memory");
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-}  // namespace tc
-
 struct TcSmem {                        // byte offsets from the 1024-aligned base
   static constexpr int a = 0;                                   // [128 rows][128 B] A operand of both layers
   static constexpr int b1 = a + 128 * 128;                      // [64 n][128 B]  W1 as [hi | hi | lo | 0]
@@ -839,8 +799,7 @@ struct TcSmem {                        // byte offsets from the 1024-aligned bas
   static constexpr int stats = tile + kTileCells * 64 * 4;      // [(kTileR+1)*(kTileC+1)] float4
   static constexpr int aff = stats + 2560;                      // s1 | t1 | s2 | t2
   static constexpr int cells = aff + 4 * 64 * 4;                // [128] int
-  static constexpr int bars = cells + kRows * 4;                // 2 mbarriers + tmem slot
-  static constexpr int total = bars + 64 + 1024;                // + alignment slack
+  static constexpr int total = cells + kRows * 4 + 1024;        // + alignment slack
 };
 
 // out_mode 0: fp32 [64] per cell; 1: h16 [hi 64 | lo 64]; 2: h16 [64]
@@ -850,28 +809,21 @@ __global__ void __launch_bounds__(kRows, 3) pillar_tile_encode_tc_kernel(
     const __grid_constant__ TileGrid tg, const int* __restrict__ tile_count, const int* __restrict__ tile_off,
     const float* __restrict__ w1, const float* __restrict__ s1, const float* __restrict__ t1, const float* __restrict__ w2,
     const float* __restrict__ s2, const float* __restrict__ t2, void* __restrict__ canvas) {
+  using namespace sm90;
   constexpr int F = D + 5, H = 64;
   static_assert(F == 16, "layer 1 is one k16 block per split term");
+  static_assert(kRows == 128, "one warpgroup, two m64 MMAs per chunk");
   extern __shared__ uint8_t tc_raw[];
-  const uint32_t base = (tc::smem_u32(tc_raw) + 1023u) & ~1023u;
-  uint8_t* gen = tc_raw + (base - tc::smem_u32(tc_raw));
+  const uint32_t base = (smem_u32(tc_raw) + 1023u) & ~1023u;
+  uint8_t* gen = tc_raw + (base - smem_u32(tc_raw));
   uint8_t* As = gen + TcSmem::a;
   float* tile = reinterpret_cast<float*>(gen + TcSmem::tile);
   float* stats = reinterpret_cast<float*>(gen + TcSmem::stats);
   float* aff = reinterpret_cast<float*>(gen + TcSmem::aff);
   int* cells = reinterpret_cast<int*>(gen + TcSmem::cells);
-  const uint32_t bar1 = base + TcSmem::bars, bar2 = bar1 + 8, slot = bar1 + 16;
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
 
-  // ---- one-time set-up: barriers, TMEM (D1 = columns [0,64), D2 = [64,128)), both weight operands, BN affines
-  if (tid == 0) {
-    tc::mbar_init(bar1, 1); tc::mbar_init(bar2, 1);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  if (warp == 0) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(slot), "r"(128u) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
+  // ---- one-time set-up: both weight operands, BN affines
   for (int e = tid; e < 64 * 8; e += kRows) {                  // 16-byte piece jj of weight row n
     const int n = e >> 3, jj = e & 7;
     uint32_t q1[4] = {0u, 0u, 0u, 0u}, q2[4];
@@ -893,15 +845,11 @@ __global__ void __launch_bounds__(kRows, 3) pillar_tile_encode_tc_kernel(
     *reinterpret_cast<uint4*>(gen + TcSmem::b2 + off) = make_uint4(q2[0], q2[1], q2[2], q2[3]);
   }
   for (int i = tid; i < H; i += kRows) { aff[i] = __ldg(s1 + i); aff[H + i] = __ldg(t1 + i); aff[2 * H + i] = __ldg(s2 + i); aff[3 * H + i] = __ldg(t2 + i); }
-  tc::proxy_fence();
-  tc::fence_before();
+  proxy_fence_async();
   __syncthreads();
-  tc::fence_after();
-  const uint32_t tmem = *reinterpret_cast<volatile uint32_t*>(gen + TcSmem::bars + 16);
-  const uint32_t my_tmem = tmem + ((uint32_t)(warp * 32) << 16);
-  const uint64_t a_desc = tc::sw128_desc(base + TcSmem::a), b1_desc = tc::sw128_desc(base + TcSmem::b1), b2_desc = tc::sw128_desc(base + TcSmem::b2);
-  const uint32_t idesc = (1u << 4) | (kH16Fmt << 7) | (kH16Fmt << 10) | ((uint32_t)(64 >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
-  uint32_t phase = 0;
+  const uint64_t b1_desc = desc_sw128(base + TcSmem::b1), b2_desc = desc_sw128(base + TcSmem::b2);
+  // rows of this thread's accumulator fragment: 64 mh + 16 warp + lane / 4 + 8 h; columns 8 j + 2 (lane % 4) (+1)
+  const int frag_row = 16 * warp + (lane >> 2), frag_col = 2 * (lane & 3);
 
   const int total_tiles = clouds.batch * tg.tiles;
   constexpr int kRowBytes = kOutMode == 2 ? 128 : 256;
@@ -972,74 +920,67 @@ __global__ void __launch_bounds__(kRows, 3) pillar_tile_encode_tc_kernel(
         *reinterpret_cast<uint4*>(row + ((5 ^ sw) << 4)) = make_uint4(hi[4], hi[5], hi[6], hi[7]);
       }
       cells[tid] = cell;
-      tc::proxy_fence();                         // generic-proxy stores -> visible to the tensor core's async-proxy reads
-      tc::fence_before();                        // orders this thread's TMEM reads of the previous round before the sync
+      proxy_fence_async();                        // generic-proxy stores -> visible to the tensor core's async-proxy reads
       __syncthreads();
-      if (tid == 0) {
-        tc::fence_after();
+      float acc[2][32];
+      wgmma_fence();
 #pragma unroll
-        for (int k = 0; k < 3; ++k) tc::umma(tmem, a_desc + (uint64_t)(2 * k), b1_desc + (uint64_t)(2 * k), idesc, k ? 1u : 0u);
-        tc::commit(bar1);
+      for (int mh = 0; mh < 2; ++mh) {
+        const uint64_t a_desc = desc_sw128(base + TcSmem::a + mh * 64 * 128);
+#pragma unroll
+        for (int k = 0; k < 3; ++k) wgmma_n64(acc[mh], a_desc + (uint64_t)(2 * k), b1_desc + (uint64_t)(2 * k), k ? 1u : 0u);
       }
-      const bool live_warp = cbeg + warp * 32 < n_t;           // warps whose 32 rows are all past the end skip the epilogues
-      if (live_warp) {
-        tc::mbar_wait(bar1, phase);
-        __syncwarp();
-        tc::fence_after();
-        uint8_t* row = As + tid * 128;
-        const int sw = tid & 7;
+      wgmma_commit();
+      wgmma_wait<0>();
+      acc_fence(acc[0]); acc_fence(acc[1]);
+      __syncthreads();                            // every warp's layer-1 MMAs have read the A rows rewritten below
 #pragma unroll
-        for (int half = 0; half < 2; ++half) {
-          uint32_t v[32];
-          tc::tmem_ld32(my_tmem + (uint32_t)(32 * half), v);
-          uint32_t w[16];
+      for (int mh = 0; mh < 2; ++mh)
 #pragma unroll
-          for (int j = 0; j < 16; ++j) {
-            const int c = 32 * half + 2 * j;
-            w[j] = pack_h16(fmaxf(fmaf(__uint_as_float(v[2 * j]), aff[c], aff[H + c]), 0.f),
-                            fmaxf(fmaf(__uint_as_float(v[2 * j + 1]), aff[c + 1], aff[H + c + 1]), 0.f));
+        for (int h = 0; h < 2; ++h) {
+          const int r = 64 * mh + frag_row + 8 * h;
+          uint8_t* row = As + r * 128;
+#pragma unroll
+          for (int j = 0; j < 8; ++j) {
+            const int c = 8 * j + frag_col;
+            const uint32_t w = pack_h16(fmaxf(fmaf(acc[mh][4 * j + 2 * h], aff[c], aff[H + c]), 0.f),
+                                        fmaxf(fmaf(acc[mh][4 * j + 2 * h + 1], aff[c + 1], aff[H + c + 1]), 0.f));
+            *reinterpret_cast<uint32_t*>(row + ((j ^ (r & 7)) << 4) + 2 * frag_col) = w;
           }
-#pragma unroll
-          for (int q = 0; q < 4; ++q)
-            *reinterpret_cast<uint4*>(row + (((4 * half + q) ^ sw) << 4)) = make_uint4(w[4 * q], w[4 * q + 1], w[4 * q + 2], w[4 * q + 3]);
         }
-      }
-      tc::proxy_fence();
-      tc::fence_before();
+      proxy_fence_async();
       __syncthreads();
-      if (tid == 0) {
-        tc::fence_after();
+      wgmma_fence();
 #pragma unroll
-        for (int k = 0; k < 4; ++k) tc::umma(tmem + 64u, a_desc + (uint64_t)(2 * k), b2_desc + (uint64_t)(2 * k), idesc, k ? 1u : 0u);
-        tc::commit(bar2);
+      for (int mh = 0; mh < 2; ++mh) {
+        const uint64_t a_desc = desc_sw128(base + TcSmem::a + mh * 64 * 128);
+#pragma unroll
+        for (int k = 0; k < 4; ++k) wgmma_n64(acc[mh], a_desc + (uint64_t)(2 * k), b2_desc + (uint64_t)(2 * k), k ? 1u : 0u);
       }
-      if (live_warp) {
-        tc::mbar_wait(bar2, phase);
-        __syncwarp();
-        tc::fence_after();
-        // max-pool: one shared-memory atomicMax per (row, positive channel).  Lanes = 32 different rows; the columns of a cell
-        // are rotated by (cell & 7) * 4 so rows of different cells mostly hit different banks (rows of the SAME cell hit the
-        // same word and are serialised by the LSU — a `__reduce_max_sync` over per-cell lane groups was tried first: with
-        // non-uniform member masks it compiles to a divergent software loop and ran 10x slower).
-        int* trow = reinterpret_cast<int*>(tile) + (cell < 0 ? 0 : cell) * 64;
-        const int sw = (cell & 7) << 2;
+      wgmma_commit();
+      wgmma_wait<0>();
+      acc_fence(acc[0]); acc_fence(acc[1]);
+      // max-pool: one shared-memory atomicMax per (row, positive channel).  The columns of a cell are rotated by (cell & 7) * 4
+      // so rows of different cells mostly hit different banks (rows of the SAME cell hit the same word and are serialised).
 #pragma unroll
-        for (int half = 0; half < 2; ++half) {
-          uint32_t v[32];
-          tc::tmem_ld32(my_tmem + (uint32_t)(64 + 32 * half), v);
-          if (cell >= 0) {
+      for (int mh = 0; mh < 2; ++mh)
 #pragma unroll
-            for (int j = 0; j < 32; ++j) {
-              const int c = 32 * half + j;
-              const float val = fmaf(__uint_as_float(v[j]), aff[2 * H + c], aff[3 * H + c]);
+        for (int h = 0; h < 2; ++h) {
+          const int rcell = cells[64 * mh + frag_row + 8 * h];
+          if (rcell < 0) continue;
+          int* trow = reinterpret_cast<int*>(tile) + rcell * 64;
+          const int sw = (rcell & 7) << 2;
+#pragma unroll
+          for (int j = 0; j < 8; ++j)
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+              const int c = 8 * j + frag_col + e;
+              const float val = fmaf(acc[mh][4 * j + 2 * h + e], aff[2 * H + c], aff[3 * H + c]);
               if (val > 0.f) atomicMax(trow + (c ^ sw), __float_as_int(val));
             }
-          }
         }
-      }
-      phase ^= 1u;
+      __syncthreads();                            // A rows and cells[] are rewritten by the next round
     }
-    tc::fence_before();
     __syncthreads();
     // ---- write-out, zeros included
     for (int e = tid; e < kTileCells * 16; e += kRows) {
@@ -1058,12 +999,6 @@ __global__ void __launch_bounds__(kRows, 3) pillar_tile_encode_tc_kernel(
         }
       }
     }
-  }
-  tc::fence_before();
-  __syncthreads();
-  if (warp == 0) {
-    tc::fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "r"(128u) : "memory");
   }
 }
 

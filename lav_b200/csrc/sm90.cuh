@@ -1,0 +1,64 @@
+// Hopper (sm_90a) warpgroup MMA (wgmma) primitives.  Shared-memory operands are K-major SWIZZLE_128B blocks (piece j of
+// 128-byte row r stored at piece j ^ (r & 7), 1024-byte aligned), as TMA writes them.
+#pragma once
+#include "common.cuh"
+
+namespace lavb {
+namespace sm90 {
+
+__device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
+
+// generic-proxy shared-memory stores -> visible to the async proxy (wgmma operand reads, TMA)
+__device__ __forceinline__ void proxy_fence_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
+// named barrier over `threads` threads (id 0 is __syncthreads)
+__device__ __forceinline__ void bar_sync(int id, int threads) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory"); }
+
+// wgmma shared-memory matrix descriptor of a K-major SWIZZLE_128B operand starting at saddr (1024-byte aligned):
+// start >> 4 in [0,14), leading byte offset >> 4 in [16,30) (unused by swizzled K-major layouts: 1), stride byte offset >> 4
+// in [32,46) = 1024 B between 8-row groups, layout type in [62,64) = 1 (128-byte swizzle).  Within the 128-byte swizzle atom
+// the K16 step k starts 32 k bytes further: descriptor + 2 k.  Rows r0.. of the operand: saddr + 128 r0 (r0 % 8 == 0).
+__device__ __forceinline__ uint64_t desc_sw128(uint32_t saddr) {
+  const uint32_t lo = ((saddr & 0x3FFFFu) >> 4) | (1u << 16);
+  const uint32_t hi = (1024u >> 4) | (1u << 30);
+  return (uint64_t)lo | ((uint64_t)hi << 32);
+}
+
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N> __device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// keeps the compiler from moving accumulator reads/writes across the asynchronous MMAs (fence after wgmma_wait)
+template <int N> __device__ __forceinline__ void acc_fence(float (&d)[N]) {
+#pragma unroll
+  for (int i = 0; i < N; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
+
+// D[64 x 32] (+)= A[64 x 16] * B[32 x 16]^T, both operands K-major in shared memory, fp32 accumulators in registers.
+// Fragment of thread t of the warpgroup: rows 16 (t/32) + (t%32)/4 (+8), columns 8 i + 2 (t%4) (+1):
+//   d[4i] = (row, col), d[4i+1] = (row, col+1), d[4i+2] = (row+8, col), d[4i+3] = (row+8, col+1).
+__device__ __forceinline__ void wgmma_n32(float (&d)[16], uint64_t a, uint64_t b, uint32_t accumulate) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\t"
+      "setp.ne.b32 p, %18, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n32k16.f32." LAVB_H16_PTX "." LAVB_H16_PTX " "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+      : "l"(a), "l"(b), "r"(accumulate));
+}
+// the same with N = 64 (fragment as above, i < 8)
+__device__ __forceinline__ void wgmma_n64(float (&d)[32], uint64_t a, uint64_t b, uint32_t accumulate) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\t"
+      "setp.ne.b32 p, %34, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32." LAVB_H16_PTX "." LAVB_H16_PTX " "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(a), "l"(b), "r"(accumulate));
+}
+
+}  // namespace sm90
+}  // namespace lavb

@@ -2,7 +2,7 @@
 `TemporalLiDARPaintedDataset.__getitem__` (lav/utils/datasets/temporal_lidar_painted_dataset.py:13-179) and
 `LiDARDataset.detections_to_heatmap` (lav/utils/datasets/lidar_dataset.py:92-127).
 
-In the reference these run in 16 numpy / OpenCV DataLoader workers per GPU; at 8 x B200 the loader, not the GPUs, bounds the
+In the reference these run in 16 numpy / OpenCV DataLoader workers per GPU; at 8 x H100 the loader, not the GPUs, bounds the
 training step (SURVEY 8f rank 4).  Here the record reads stay on the host (key-value store, see data_paint.py) and everything that
 touches the points runs on the GPU with the frame path's own kernels:
 

@@ -102,7 +102,7 @@ class _Down:
         return out
 
 
-FUSE_PAIRS = True     # fused (3x1 -> 1x3) tcgen05 kernel (csrc/conv_pair_umma.cu): validated on B200, ERFNet 2.85 -> 2.72 ms @96 images
+FUSE_PAIRS = True     # fused (3x1 -> 1x3) wgmma kernel (csrc/conv_pair_umma.cu)
 
 
 FUSE_STEM = True      # normalize + initial DownsamplerBlock(3,16) as one kernel on the uint8 frames (csrc/erf16.cu: erf_stem_kernel)
@@ -134,7 +134,7 @@ class _NB1D:
         if FUSE_NB16 and self.nb16 is not None and x.dtype == ops.h16() and x.shape[2] % 16 == 0 and x.shape[2] <= 256:
             return ops.erf_nb16(x, *self.nb16)
         if FUSE_PAIRS and x.dtype == ops.h16() and self.a.umma_ok and x.shape[3] in (64, 128) and x.shape[2] in (32, 64, 128):
-            # each (3x1 -> 1x3) pair in one tcgen05 kernel, the intermediate stays in shared memory
+            # each (3x1 -> 1x3) pair in one wgmma kernel, the intermediate stays in shared memory
             if self.pair is None:
                 def folded(t):       # (conv + b) * s + t' = conv_{w*s} + (b*s + t'): scale into the weights (fp32, rounded once)
                     w = t.phases[0]["w"][:, :, :t.cout] * t.scale[None, None, :]

@@ -23,7 +23,7 @@ from . import ops
 
 # ----------------------------------------------------------------------------- ResNet-18
 TRAIN_CROP_KERNEL = True      # UniPlanner.crop_feature with gradients: lav_b200 crop kernel + its gather backward (ops.CropBilinear)
-                              # instead of F.grid_sample (cudnn bilinear_sampler_bw: 7.1 ms of a 94 ms train_lidar step on B200)
+                              # instead of F.grid_sample (cudnn bilinear_sampler_bw)
 
 
 class BasicBlock(nn.Module):
@@ -129,7 +129,7 @@ class ResNet18(nn.Module):
     def _trunk_folded(self, x, f):
         dt = x.dtype
         if getattr(self, "use_umma_trunk", False) and dt == ops.h16():
-            # layer1..4 on the lav_b200 tcgen05 conv kernel (BN / residual / ReLU fused in its epilogue)
+            # layer1..4 on the lav_b200 wgmma conv kernel (BN / residual / ReLU fused in its epilogue)
             key = ("umma", str(x.device))
             cache = self._cache()
             if key not in cache:
@@ -172,11 +172,11 @@ def resnet18(pretrained=False, num_channels=3, **kw):
 # operands, 8e-4 per roll-out, 0.71 ms per tick) ended 1.7e-2 .. 5e-2 from the reference at BASELINE config 3.  This version
 # agrees with nn.GRU to 2e-5 over 20 steps and passes every parity test of both pipelines, but the three products run on the
 # legacy mma.sync path and 64 KB of hidden state cross DSMEM per CTA and step: 1.18 ms per tick of 32 frames against cuDNN's
-# 0.98 ms (B200).  OFF by default for that reason; the tcgen05 form (W_lo as a TMEM A operand) is the open item in DESIGN.md.
+# cuDNN.  OFF by default for that reason.
 GRU_KERNEL = False
 
 # The cast branches (6 x GRU(512, 64) + Linear(64, 2) + cumsum over the repeated embedding) as ONE fp32 kernel (csrc/cast_gru.cu)
-# instead of ~100 dependent cuDNN / ATen launches per call (B200: 0.29 -> 0.05 ms per tick).  Inference only.
+# instead of ~100 dependent cuDNN / ATen launches per call.  Inference only.
 CAST_KERNEL = True
 
 

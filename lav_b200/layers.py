@@ -9,7 +9,7 @@ import torch
 
 from . import ops
 
-USE_UMMA = True   # tests flip this to compare the tcgen05 path with the CUDA-core path
+USE_UMMA = True   # tests flip this to compare the wgmma path with the CUDA-core path
 UMMA_STRIDED = True   # stride-2 convs through the tensor map's element strides
 
 
@@ -76,7 +76,7 @@ class TapConv:
                                             out_o=(oy, ox)))
         for ph in self.phases:
             assert len(ph["taps"]) <= 16, "tap list longer than the kernel's table"
-        # tcgen05 path (f16 activations): weights [ntaps][cout][cin] f16, K contiguous
+        # wgmma path (f16 activations): weights [ntaps][cout][cin] f16, K contiguous
         # (cout that is a multiple of 8 but not of 32 is zero-padded to the MMA width; only the real channels are stored)
         self.umma_ok = USE_UMMA and self.cin_k % 64 == 0 and self.cout % 8 == 0 and self.cout <= 256
         if self.umma_ok:

@@ -64,7 +64,7 @@ class ConvBackbone(PlanMixin, nn.Module):
             plan[name] = crb(seq[0], seq[2])
         if self.precision == "f16":
             # first layer on tensor cores WITHOUT rounding the fp32 canvas to f16: input = [hi | lo] split (2*cin channels),
-            # weights duplicated along cin, so conv(x_hi) + conv(x_lo) accumulate in TMEM (costs 1.9 extra GFLOP / frame)
+            # weights duplicated along cin, so conv(x_hi) + conv(x_lo) accumulate in the MMA accumulators (costs 1.9 extra GFLOP / frame)
             c0, b0 = self.conv1[0], self.conv1[2]
             s, t = bn_affine(b0)
             plan["conv1_split"] = TapConv(torch.cat([c0.weight, c0.weight], 1), False, c0.stride, c0.padding, c0.dilation, 0, None,

@@ -1,7 +1,7 @@
 """Torch-tensor front ends of the C-ABI kernels (device pointers + current stream in, tensors out).
 
 PyTorch is plumbing here: allocation, streams, views.  Every function launches hand-written
-sm_100a kernels through lav_b200.capi; nothing falls back to torch math.
+sm_90a kernels through lav_b200.capi; nothing falls back to torch math.
 """
 import ctypes as C
 
@@ -190,7 +190,7 @@ def conv_taps(x, cin, in_coff, out, cout, out_coff, hog, wog, in_s, out_s, out_o
               res=None, res_coff=0, pre_relu=False, post_relu=False, sigmoid=False, umma=False, d2s_nout=0):
     """x, out, res: contiguous NHWC buffers (N,H,W,Ctot).  taps: list of (dy,dx).
     umma=False: CUDA-core kernel, w (ntaps,cin,cout_pad16) fp32.
-    umma=True : tcgen05 kernel, x f16, w (ntaps,cout,cin) f16."""
+    umma=True : wgmma kernel, x f16, w (ntaps,cout,cin) f16."""
     _need_cuda(x, out, w)
     assert x.is_contiguous() and out.is_contiguous() and w.is_contiguous()
     d = ConvDesc()
@@ -400,9 +400,9 @@ def split_h16(x):
     return out
 
 
-PILLAR_ENCODER = "sorted"    # tensor-core encoders of the 16-bit pipeline, B200 @ 32 frames x 120 000 points:
+PILLAR_ENCODER = "sorted"    # tensor-core encoders of the 16-bit pipeline:
 #   "sorted": counting sort by canvas cell + persistent mma.sync encoder (lavb_pillar_forward_sorted)          23.3 us/frame
-#   "tiled" : points binned by 8x16-cell canvas tile, one CTA per tile, tcgen05 MLP (lavb_pillar_forward_tiled) 29.2 us/frame —
+#   "tiled" : points binned by 8x16-cell canvas tile, one CTA per tile, wgmma MLP (lavb_pillar_forward_tiled) —
 #             fewer launches and 35 % less DRAM traffic (942 vs 1448 MB), but every tile is a serial chain of ~8 dependent steps
 #             (load, centroid atomics, MMA round trips, pooling atomics, store) with 3 CTAs per SM: latency-bound (profiles/)
 

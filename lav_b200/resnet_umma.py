@@ -13,7 +13,7 @@ from .layers import TapConv, bn_affine
 
 
 class _WideTapConv:
-    """TapConv for cout > 256: the tcgen05 kernel holds at most 256 accumulator columns, so wider layers are issued as
+    """TapConv for cout > 256: the wgmma kernel holds at most 256 accumulator columns, so wider layers are issued as
     column chunks that write adjacent channel slices."""
 
     def __init__(self, weight, stride, padding, scale, shift, post_relu, chunk=256):

@@ -299,8 +299,8 @@ class LAVTrainer:
                  cmd_smooth=0.2, perceive_only=False, motion_only=False, bucket_bytes=25 << 20, amp=False, channels_last=True):
         self.lidar_model, self.uniplanner = lidar_model.train(), uniplanner.train()
         if channels_last and next(lidar_model.parameters()).is_cuda:
-            # NHWC convolution weights (values and state_dict unchanged): cuDNN's sm_100 kernels are NHWC — this removes most of
-            # the nchw<->nhwc conversion kernels around them (B200: 75.4 -> 73.8 ms per 32-sample step)
+            # NHWC convolution weights (values and state_dict unchanged): cuDNN's tensor-core kernels are NHWC — this removes most of
+            # the nchw<->nhwc conversion kernels around them
             lidar_model.to(memory_format=torch.channels_last)
             uniplanner.to(memory_format=torch.channels_last)
         uniplanner.bev_planner.eval()
@@ -330,7 +330,7 @@ class LAVTrainer:
         up = self.uniplanner
         bev = bev.float()
         # amp: only the LiDAR model (pillars, backbone, heads — the convolutions) runs under bf16 autocast; the planner (cuDNN
-        # GRUs, crops, embedder) and every loss stay fp32 — cuDNN's bf16 RNN path faulted on these shapes (B200, cuDNN 9)
+        # GRUs, crops, embedder) and every loss stay fp32 — cuDNN's bf16 RNN path faulted on these shapes (cuDNN 9)
         ctx = torch.autocast("cuda", dtype=torch.bfloat16) if self.amp else contextlib.nullcontext()
         with ctx:
             outs = self.lidar_model(lidars, num_points)

@@ -31,6 +31,12 @@ from lav_b200 import synth  # noqa: E402
 from oracle import lav_ref as O  # noqa: E402
 
 GOLD = os.path.join(ROOT, "tests", "golden")
+if "--weights-only" in sys.argv:    # only the real-weight state_dicts of oracle/_ref/; the fixtures go to a scratch directory
+    import atexit
+    import shutil
+    import tempfile
+    GOLD = tempfile.mkdtemp(prefix="lavb_pin_")
+    atexit.register(shutil.rmtree, GOLD, True)
 REFOUT = os.path.join(ROOT, "oracle", "_ref")
 os.makedirs(GOLD, exist_ok=True)
 os.makedirs(REFOUT, exist_ok=True)

@@ -11,7 +11,8 @@ def run(n, h, w, c, dil, use_res, tiles=16):
     w1 = (torch.randn(3, c, c, generator=g) / (3 * c) ** 0.5).to(ops.h16()).cuda()
     w2 = (torch.randn(3, c, c, generator=g) / (3 * c) ** 0.5).to(ops.h16()).cuda()
     b1, t2 = torch.randn(c, generator=g).cuda() * 0.1, torch.randn(c, generator=g).cuda() * 0.1
-    ctas = 296 if c == 64 else 148
+    sms = torch.cuda.get_device_properties(0).multi_processor_count
+    ctas = 2 * sms if c == 64 else sms
     buf = torch.zeros(ctas * tiles * 8, dtype=torch.int64, device="cuda")
     for _ in range(3):
         ops.conv_pair_umma(x, w1, b1, w2, t2, dil, res=x if use_res else None)

@@ -1,4 +1,4 @@
-"""Pillar encoder A/B: sorted vs tile-binned kernels (mma.sync / tcgen05 MLP) on B frames of 120k stacked points (and B x 40k,
+"""Pillar encoder A/B: sorted vs tile-binned kernels (mma.sync / wgmma MLP) on B frames of 120k stacked points (and B x 40k,
 config 2).  python scripts/pillar_ab.py [B]"""
 import os, subprocess, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))

@@ -1,4 +1,4 @@
-"""Run a few representative tcgen05 conv layers once (for ncu --set full) and time them with events."""
+"""Run a few representative wgmma conv layers once and time them with events."""
 import os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
@@ -28,4 +28,4 @@ for name, n, h, w, cin, cout, k, p in cfgs:
     fl = 2.0 * n * h * w * cout * cin * k[0] * k[1]
     by = n * h * w * (cin + cout) * 2
     tiles = n * ((h + 7) // 8) * ((w + 15) // 16)
-    print(f"{name:14s} {t*1e3:8.1f} us  {fl/t/1e9:7.1f} TFLOP/s  {by/t/1e6:7.1f} GB/s(alg)  tiles={tiles} ({tiles/148:.1f}/SM)  {t*1e3/max(1,-(-tiles//148)):.2f} us/tile-round")
+    print(f"{name:14s} {t*1e3:8.1f} us  {fl/t/1e9:7.1f} TFLOP/s  {by/t/1e6:7.1f} GB/s(alg)  tiles={tiles} ({tiles/132:.1f}/SM on 132 SMs)")

@@ -65,7 +65,7 @@ def test_config2_paint_and_voxelise_b32(cuda, precision, monkeypatch):
     """Config 2: point painting + PointPillars voxeliser forward, B = 32 x 40 000 points (time one-hot [1,0,0], D = 11).
     Painted features must be index-equal to the oracle on every frame; the canvas within 1e-3 on sampled frames, with
     identical occupancy.  fp32 = the exact kernel; f16 = the tensor-core encoder the benchmark runs, with its h16 canvas;
-    f16-tiled = the tile-binned tcgen05 encoder (same 1e-3 gate for all three)."""
+    f16-tiled = the tile-binned wgmma encoder (same 1e-3 gate for all three)."""
     if precision == "f16-tiled":
         monkeypatch.setattr(ops, "PILLAR_ENCODER", "tiled")
     from lav_b200 import point_painting as PP

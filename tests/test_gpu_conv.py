@@ -134,7 +134,7 @@ def test_erfnet_matches_oracle(cuda, weights, golden_dir):
     dict(cin=64, cout=128, k=(3, 3), p=(1, 1), d=(1, 1), hw=(40, 36), cs=2),
 ])
 def test_umma_conv_vs_torch(cuda, cfg):
-    """tcgen05 implicit-GEMM conv against fp32 torch on f16-rounded operands (so only accumulation order differs)."""
+    """wgmma implicit-GEMM conv against fp32 torch on f16-rounded operands (so only accumulation order differs)."""
     from lav_b200 import layers
     from lav_b200.layers import TapConv
     g = synth._gen(21, str(cfg))

@@ -266,7 +266,7 @@ def test_static_pipeline_matches_dynamic(cuda, graphs):
 
 
 def test_resnet_trunk_on_umma_matches_cudnn(cuda):
-    """ResNet-18 layer1..4 through the tcgen05 tap-list conv (BN/residual/ReLU fused) vs the folded cuDNN path."""
+    """ResNet-18 layer1..4 through the wgmma tap-list conv (BN/residual/ReLU fused) vs the folded cuDNN path."""
     from lav_b200.heads import resnet18
     m = resnet18(num_channels=3).eval()
     m.load_state_dict(synth.fill_state_dict_(m.state_dict()))

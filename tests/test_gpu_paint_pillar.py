@@ -161,7 +161,7 @@ def test_pillar_full_size_properties(cuda):
 @pytest.mark.parametrize("out", ["fp32", "split", "h16"])
 @pytest.mark.parametrize("mode", ["carla", "uniform", "adversarial", "batch", "empty"])
 def test_pillar_tensor_core_encoders_match_oracle(cuda, mode, out, encoder, monkeypatch):
-    """the two tensor-core encoders of the 16-bit pipeline — cell-sorted + mma.sync, tile-binned + tcgen05 — in their three
+    """the two tensor-core encoders of the 16-bit pipeline — cell-sorted + mma.sync, tile-binned + wgmma — in their three
     canvas formats (fp32, [hi | lo] h16 split, single h16): same occupancy as the oracle, values within 1e-3 (layer 1 runs on
     hi/lo-split operands ~ fp32, layer 2 on h16 operands with fp32 accumulation; the h16 canvas adds one 2^-12 rounding)."""
     monkeypatch.setattr(ops, "PILLAR_ENCODER", encoder)

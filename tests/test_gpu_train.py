@@ -27,7 +27,7 @@ def test_train_forward_backward_matches_reference_golden(cuda, golden_dir):
     loss.backward()
     # Every parameter gradient against the REFERENCE's digest (l2 norm, projection on a seeded vector).  Deep-layer
     # gradients of this untrained, batch-stat-BN network are ill-conditioned: the oracle itself, run on another CPU,
-    # moves by 1e-3..1e-2 of the gradient norm (measured on the B200 host, scripts/train_debug.py), so the gate is
+    # moves by 1e-3..1e-2 of the gradient norm (scripts/train_debug.py), so the gate is
     # statistical for the trunk and tight for the output layers, whose gradients do not pass through the trunk.
     import json
     dig = json.load(open(os.path.join(golden_dir, "lidar_model_train_grad_digest.json")))
