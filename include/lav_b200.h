@@ -246,6 +246,15 @@ int lavb_convert(const void* d_src, int src_dtype, void* d_dst, int dst_dtype, l
  * (cuTensorMapEncodeTiled through cudaGetDriverEntryPoint), accumulators live in registers. */
 int lavb_conv_umma(const lavb_conv_desc* h_desc, void* stream);
 
+/* ---------------------------------------------------------------- planner embedder stem
+ * replaces: conv1 (7x7, s2, p3, cin -> 64) + bn1 + ReLU of UniPlanner's crop embedder resnet18(num_channels=384)
+ * (team_code_v2/models/uniplanner.py:36-40, lav/models/resnet.py:178,235-238) on the h16 path.  d_in: h16 NHWC (n, h, w, cin),
+ * cin % 64 == 0, h, w >= 7; d_w: BatchNorm-folded h16 weights laid out [49 taps (ky*7 + kx)][64 cout][cin]; d_bias: fp32 [64];
+ * d_out: h16 NHWC (n, (h-1)/2+1, (w-1)/2+1, 64) = relu(conv + bias), saturating.  wgmma implicit GEMM with output channels
+ * in M and 16 x 16 output-pixel tiles in N; operands fetched by TMA, whose out-of-bounds zero fill is the padding. */
+int lavb_conv7x7s2_umma(const void* d_in, int n, int h, int w, int cin, const void* d_w, const float* d_bias, void* d_out,
+                        void* stream);
+
 /* ---------------------------------------------------------------- fused (3x1 -> 1x3) convolution pair
  * replaces: conv3x1_k -> ReLU -> conv1x3_k -> bn_k [-> + input] -> ReLU of non_bottleneck_1d (lav/models/erfnet.py:37-63) in
  * one wgmma kernel; the intermediate activation stays in shared memory.

@@ -13,8 +13,6 @@
 //   epilogue 2: acc2 + shift2 -> h16 -> (+ residual, ReLU as one packed fma.relu) -> NHWC.  The BatchNorm scale is folded into W2 by the caller.
 // Warp roles: warps 0-3 and 4-7 are two consumer warpgroups (tile pixels 0-63 / 64-127), warp 8 is the TMA producer; persistent
 // over tiles.  With C = 64 two CTAs share an SM, so one CTA's epilogues overlap the other's MMAs.
-#include <cuda.h>
-#include <cudaTypedefs.h>
 #include <stdlib.h>
 #include "sm90.cuh"
 
@@ -39,37 +37,8 @@ struct PairArgs {
       p.trace[((long long)blockIdx.x * p.trace_tiles + (i)) * 8 + (slot)] = clock64();                              \
   } while (0)
 
-__device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count));
-}
-__device__ __forceinline__ void mbar_expect_tx(uint32_t bar, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_arrive(uint32_t bar) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
-  uint32_t done;
-  do {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-        "selp.u32 %0, 1, 0, p;\n\t}"
-        : "=r"(done) : "r"(bar), "r"(parity) : "memory");
-  } while (!done);
-}
-__device__ __forceinline__ void tma_load_4d(uint32_t dst, const CUtensorMap* map, uint32_t bar, int c0, int c1, int c2, int c3) {
-  asm volatile(
-      "cp.async.bulk.tensor.4d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];"
-      ::"r"(dst), "l"(reinterpret_cast<uint64_t>(map)), "r"(bar), "r"(c0), "r"(c1), "r"(c2), "r"(c3) : "memory");
-}
-__device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* map, uint32_t bar, int c0, int c1) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-      ::"r"(dst), "l"(reinterpret_cast<uint64_t>(map)), "r"(bar), "r"(c0), "r"(c1) : "memory");
-}
-__device__ __forceinline__ void proxy_fence_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
+using namespace sm90;
+
 __device__ __forceinline__ uint32_t relu2(uint32_t x) {
   const h162 v = __hmax2(*reinterpret_cast<const h162*>(&x), floats2h162(0.f, 0.f));
   return *reinterpret_cast<const uint32_t*>(&v);
@@ -256,17 +225,6 @@ __global__ void __launch_bounds__(kPairThreads, kC == 64 ? 2 : 1) conv_pair_umma
     }
     PAIR_STAMP(3, i);
   }
-}
-
-static PFN_cuTensorMapEncodeTiled_v12000 get_encode() {
-  static PFN_cuTensorMapEncodeTiled_v12000 fn = nullptr;
-  if (!fn) {
-    void* p = nullptr;
-    cudaDriverEntryPointQueryResult q;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q) == cudaSuccess && q == cudaDriverEntryPointSuccess)
-      fn = reinterpret_cast<PFN_cuTensorMapEncodeTiled_v12000>(p);
-  }
-  return fn;
 }
 
 }  // namespace pair

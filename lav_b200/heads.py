@@ -9,7 +9,8 @@ keys (tests/golden/keys_uniplanner.json, keys_brake.json):
   RGBBrakePredictionModel, Attention, SegmentationHead
                       team_code_v2/models/rgb.py:48-83, lav/models/attention.py, segmentation.py
 
-Only the crop (bilinear rotated window gather) is a lav_b200 CUDA kernel; convs/GRUs here are cuDNN.
+Only the crop (bilinear rotated window gather) is a lav_b200 CUDA kernel; convs/GRUs here are cuDNN, except the
+flag-selected kernels below (STEM_KERNEL, GRU_KERNEL, CAST_KERNEL) and the brake stem of forward_u8.
 """
 import math
 
@@ -24,6 +25,9 @@ from . import ops
 # ----------------------------------------------------------------------------- ResNet-18
 TRAIN_CROP_KERNEL = True      # UniPlanner.crop_feature with gradients: lav_b200 crop kernel + its gather backward (ops.CropBilinear)
                               # instead of F.grid_sample (cudnn bilinear_sampler_bw)
+# Eval f16 stems with 7x7 / s2 / p3 -> 64 and cin % 64 == 0 (the planner embedder's 384-channel crop stem) run on the lav_b200
+# wgmma kernel (ops.conv7x7s2_umma).  cuDNN gives this shape a generic engine on H100 that is >10x slower.  False: cuDNN.
+STEM_KERNEL = True
 
 
 class BasicBlock(nn.Module):
@@ -106,6 +110,16 @@ class ResNet18(nn.Module):
         dt = self.conv1.weight.dtype
         x = x.to(dt).contiguous(memory_format=torch.channels_last)
         f = self._folded(dt, x.device)
+        c1 = self.conv1
+        if (STEM_KERNEL and dt == ops.h16() and c1.kernel_size == (7, 7) and c1.stride == (2, 2) and c1.padding == (3, 3)
+                and c1.out_channels == 64 and c1.in_channels % 64 == 0):
+            # the planner embedder's 384-channel stem on the lav_b200 wgmma kernel (csrc/stem_umma.cu)
+            if "stem_umma" not in f:
+                w, b = self._folded(torch.float32, x.device)["stem"]                # fold in fp32, round once
+                f["stem_umma"] = (ops.pack_conv7x7s2_weights(w), b.float().contiguous())
+            wk, b = f["stem_umma"]
+            x = ops.conv7x7s2_umma(x.permute(0, 2, 3, 1).contiguous(), wk, b)
+            return self._trunk_folded(ops.maxpool3x3s2_nhwc(x).permute(0, 3, 1, 2), f)
         w, b = f["stem"]
         x = torch.cudnn_convolution_relu(x, w, b, (2, 2), (3, 3), (1, 1), 1)
         if dt == ops.h16():                        # lav_b200 pool kernel on the channels-last memory (ATen's is ~5x slower)

@@ -472,6 +472,31 @@ def pack_stem_weights(w):
     return out.to(h16()).contiguous()
 
 
+def conv7x7s2_umma(x, w_packed, bias):
+    """relu(conv 7x7 / stride 2 / pad 3 + bias) to 64 channels: x contiguous f16 NHWC (n, h, w, cin), cin % 64 == 0;
+    w_packed (49, 64, cin) f16 from pack_conv7x7s2_weights; bias fp32 (64,) -> f16 NHWC (n, (h-1)//2+1, (w-1)//2+1, 64)."""
+    _need_cuda(x, w_packed, bias)
+    assert x.dtype == h16() and x.is_contiguous() and x.dim() == 4
+    n, h, w, cin = x.shape
+    assert cin % 64 == 0 and h >= 7 and w >= 7, x.shape
+    assert w_packed.dtype == h16() and w_packed.is_contiguous() and tuple(w_packed.shape) == (49, 64, cin)
+    assert bias.dtype == torch.float32 and bias.is_contiguous() and bias.numel() == 64
+    ho, wo = (h - 1) // 2 + 1, (w - 1) // 2 + 1
+    out = torch.empty((n, ho, wo, 64), dtype=h16(), device=x.device)
+    e0 = _prof_begin()
+    check(lib().lavb_conv7x7s2_umma(_ptr(x), n, h, w, cin, _ptr(w_packed), _ptr(bias), _ptr(out), _stream()),
+          "lavb_conv7x7s2_umma")
+    _prof_end(f"stem7x7s2:{cin}->64@{h}x{w}", 2.0 * n * ho * wo * 64 * cin * 49, e0)
+    _COUNT[0] += 1
+    return out
+
+
+def pack_conv7x7s2_weights(w):
+    """(64, cin, 7, 7) conv weights -> (49, 64, cin) f16 [tap = ky*7 + kx][cout][cin], the layout conv7x7s2_umma reads."""
+    assert w.dim() == 4 and tuple(w.shape[2:]) == (7, 7) and w.shape[0] == 64
+    return w.permute(2, 3, 0, 1).reshape(49, 64, w.shape[1]).to(h16()).contiguous()
+
+
 def maxpool3x3s2_nhwc(x):
     """MaxPool2d(3, 2, 1) on a contiguous f16 NHWC tensor."""
     _need_cuda(x)
