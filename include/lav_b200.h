@@ -261,7 +261,7 @@ int lavb_conv7x7s2_umma(const void* d_in, int n, int h, int w, int cin, const vo
  *   mid = relu(conv3x1_dil(in) + bias1);  out = [relu](conv1x3_dil(mid) + shift2 [+ res])
  * The BatchNorm affine (conv + b2) * s + t is folded by the caller: w2 <- w2 * s per output channel, shift2 <- b2 * s + t.
  * bias1 / shift2 (fp32 [c]) are added to the register accumulators in the epilogues, which then pack, clamp and add the residual
- * (16-bit packed arithmetic: the residual add rounds once more than an fp32 add would).
+ * (16-bit packed arithmetic: the residual add rounds once more than an fp32 add would, and its sum saturates at +-65504).
  * in / out / res: h16 NHWC (n, h, w, c) contiguous, c in {64, 128}, w in {32, 64, 128}; w1 / w2: h16 [3 taps][c out][c in];
  * res may be NULL. */
 typedef struct lavb_conv_pair_desc {

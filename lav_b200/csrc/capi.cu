@@ -2,7 +2,7 @@
 #include <stdarg.h>
 #include <stdlib.h>
 #include <mutex>
-#include <set>
+#include <map>
 #include <utility>
 #include "common.cuh"
 
@@ -32,18 +32,21 @@ int num_sms() {
   return n;
 }
 
-// cudaFuncAttributeMaxDynamicSharedMemorySize is a per-DEVICE attribute: set it once per (kernel, device ordinal), under a
-// lock (several host threads may drive their own pipelines).  Callers warm up before any stream capture.
+// cudaFuncAttributeMaxDynamicSharedMemorySize is a per-DEVICE attribute: set it per (kernel, device ordinal) whenever a launch
+// needs more than the largest size set so far (erf_nb16's footprint grows with the image width, so a narrow first call must not
+// cap later wide ones), under a lock (several host threads may drive their own pipelines).  Callers warm up before any stream
+// capture.
 cudaError_t ensure_dyn_smem(const void* kernel, int bytes) {
   static std::mutex mu;
-  static std::set<std::pair<const void*, int>> done;
+  static std::map<std::pair<const void*, int>, int> largest;
   int dev = 0;
   cudaError_t e = cudaGetDevice(&dev);
   if (e != cudaSuccess) return e;
   std::lock_guard<std::mutex> lock(mu);
-  if (done.count({kernel, dev})) return cudaSuccess;
+  auto it = largest.find({kernel, dev});
+  if (it != largest.end() && it->second >= bytes) return cudaSuccess;
   e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
-  if (e == cudaSuccess) done.insert({kernel, dev});
+  if (e == cudaSuccess) largest[{kernel, dev}] = bytes;
   return e;
 }
 }  // namespace lavb

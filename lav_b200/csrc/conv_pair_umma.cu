@@ -43,9 +43,16 @@ __device__ __forceinline__ uint32_t relu2(uint32_t x) {
   const h162 v = __hmax2(*reinterpret_cast<const h162*>(&x), floats2h162(0.f, 0.f));
   return *reinterpret_cast<const uint32_t*>(&v);
 }
+// residual add in packed h16 arithmetic.  A packed add rounds a sum past the finite range to inf, so the sum is clamped to
+// +-65504 afterwards: the same saturating store as every cvt.rn.satfinite in the library (in-range sums are unchanged).
 __device__ __forceinline__ uint32_t add2(uint32_t x, uint32_t r, bool relu) {
   const h162 a = *reinterpret_cast<const h162*>(&x), b = *reinterpret_cast<const h162*>(&r);
-  const h162 v = relu ? __hfma2_relu(a, floats2h162(1.f, 1.f), b) : __hadd2(a, b);
+  h162 v = relu ? __hfma2_relu(a, floats2h162(1.f, 1.f), b) : __hadd2(a, b);
+#ifndef LAVB_H16_BF16
+  const uint32_t hi = 0x7BFF7BFFu, lo = 0xFBFFFBFFu;           // +65504 / -65504 in both halves
+  v = __hmin2(v, *reinterpret_cast<const h162*>(&hi));
+  if (!relu) v = __hmax2(v, *reinterpret_cast<const h162*>(&lo));
+#endif
   return *reinterpret_cast<const uint32_t*>(&v);
 }
 

@@ -472,9 +472,10 @@ def pack_stem_weights(w):
     return out.to(h16()).contiguous()
 
 
-def conv7x7s2_umma(x, w_packed, bias):
+def conv7x7s2_umma(x, w_packed, bias, out=None):
     """relu(conv 7x7 / stride 2 / pad 3 + bias) to 64 channels: x contiguous f16 NHWC (n, h, w, cin), cin % 64 == 0;
-    w_packed (49, 64, cin) f16 from pack_conv7x7s2_weights; bias fp32 (64,) -> f16 NHWC (n, (h-1)//2+1, (w-1)//2+1, 64)."""
+    w_packed (49, 64, cin) f16 from pack_conv7x7s2_weights; bias fp32 (64,) -> f16 NHWC (n, (h-1)//2+1, (w-1)//2+1, 64),
+    written into `out` when given (contiguous, that shape)."""
     _need_cuda(x, w_packed, bias)
     assert x.dtype == h16() and x.is_contiguous() and x.dim() == 4
     n, h, w, cin = x.shape
@@ -482,7 +483,9 @@ def conv7x7s2_umma(x, w_packed, bias):
     assert w_packed.dtype == h16() and w_packed.is_contiguous() and tuple(w_packed.shape) == (49, 64, cin)
     assert bias.dtype == torch.float32 and bias.is_contiguous() and bias.numel() == 64
     ho, wo = (h - 1) // 2 + 1, (w - 1) // 2 + 1
-    out = torch.empty((n, ho, wo, 64), dtype=h16(), device=x.device)
+    if out is None:
+        out = torch.empty((n, ho, wo, 64), dtype=h16(), device=x.device)
+    assert out.dtype == h16() and out.is_contiguous() and tuple(out.shape) == (n, ho, wo, 64)
     e0 = _prof_begin()
     check(lib().lavb_conv7x7s2_umma(_ptr(x), n, h, w, cin, _ptr(w_packed), _ptr(bias), _ptr(out), _stream()),
           "lavb_conv7x7s2_umma")
@@ -508,18 +511,20 @@ def maxpool3x3s2_nhwc(x):
     return out
 
 
-def conv_pair_umma(x, w1, bias1, w2, shift2, dil, res=None, post_relu=True):
+def conv_pair_umma(x, w1, bias1, w2, shift2, dil, res=None, post_relu=True, out=None):
     """fused pair: mid = relu(conv3x1_dil(x) + bias1); out = [relu](conv1x3_dil(mid) + shift2 [+ res]).  A BatchNorm affine after
     the second conv is folded by the caller: w2 <- w2 * s (per output channel), shift2 <- b2 * s + t.
     x / res: contiguous f16 NHWC (n, h, w, c), c in {64, 128}, w in {32, 64, 128}; w1 / w2: (3, c, c) f16 [tap][cout][cin];
-    bias1 / shift2: fp32 (c,)."""
+    bias1 / shift2: fp32 (c,).  The result goes to `out` when given (contiguous, the shape of x)."""
     from .capi import ConvPairDesc
     _need_cuda(x, w1, w2, bias1, shift2)
     n, h, w, c = x.shape
     assert x.dtype == h16() and x.is_contiguous() and w1.is_contiguous() and w2.is_contiguous()
     assert tuple(w1.shape) == (3, c, c) and tuple(w2.shape) == (3, c, c) and w1.dtype == w2.dtype == h16()
     assert bias1.dtype == shift2.dtype == torch.float32 and bias1.numel() == shift2.numel() == c
-    out = torch.empty_like(x)
+    if out is None:
+        out = torch.empty_like(x)
+    assert out.dtype == h16() and out.is_contiguous() and out.shape == x.shape
     d = ConvPairDesc()
     d.inp, d.out = x.data_ptr(), out.data_ptr()
     d.n, d.h, d.w, d.c, d.dil, d.post_relu = n, h, w, c, int(dil), int(post_relu)
