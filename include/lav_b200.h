@@ -95,6 +95,18 @@ int lavb_roof_filter(const float* d_src, int frames, int n, int cols, long long 
  * CUDA graph (new poses, new ring-buffer slots) without touching kernel arguments. max_n = largest job. */
 int lavb_stack_jobs(const void* d_jobs, int n_jobs, int max_n, int src_cols, int n_time, int roof_filter, void* stream);
 
+/* ---------------------------------------------------------------- temporal BEV training targets
+ * replaces: TemporalLiDARPaintedDataset.load_bev_channels (lav/utils/datasets/temporal_lidar_painted_dataset.py:182-198) and
+ *           its calls at :110-136: rotate_image (lidar_dataset.py:159-163, cv2.warpAffine INTER_LINEAR, zero border) by the
+ *           ego yaw change, zero-pad by 32, crop shifted by (dx, dy), rotate_image by the sample's jitter, > 0.
+ * One launch builds every (h, w) uint8 plane of a batch.  d_jobs is a DEVICE array of n_jobs 128-byte records
+ *   { long long src; long long dst; double m1[6]; double m2[6]; int dx, dy; int pad[2]; }
+ * src = plane index into d_src (planes of h*w bytes; < 0 writes a zero plane: a frame before the recording's start),
+ * dst = plane index into d_out; m1 / m2 = the inverse affine matrices (row-major 2x3, computed on the host the way
+ * cv::warpAffine inverts getRotationMatrix2D) of the first and second warp; dx shifts rows and dy columns.
+ * The output is bit-identical to OpenCV's fixed-point 8-bit warp chain; every output byte is 0 or 1. */
+int lavb_bev_targets(const void* d_jobs, int n_jobs, const uint8_t* d_src, uint8_t* d_out, int h, int w, void* stream);
+
 /* ---------------------------------------------------------------- PointPillars voxeliser + pillar encoder
  * replaces: PointPillarNet.forward (lav/models/point_pillar.py:92-116) incl. grid_locations :70-79,
  *           pillar_generation/decorate :55-68,81-85, DynamicPointNet.forward :28-35 (torch_scatter

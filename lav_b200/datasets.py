@@ -1,0 +1,279 @@
+"""Training data from recorded trajectories: TemporalLiDARPaintedDataset (lav/utils/datasets/temporal_lidar_painted_dataset.py)
+with its per-sample work on the GPU, and a batch loader for LAVTrainer.train_lidar.
+
+Recording layout: the reference's keys (basic_dataset.py:52-53,82-101; data_paint.py writes lidar_sem_%05d), one key-value
+environment per trajectory directory (LMDB when the `lmdb` package imports and data.mdb exists, else data_paint.DirEnv).
+
+What runs where:
+    record reads, PNG decode (cv2, else torchvision)              host, a background thread of the loader
+    actor filter, ego transform, label padding (a few hundred floats)   host, vectorised numpy
+    LiDAR: roof filter, rotation, FOV re-mask, stacking, shuffle   device, data_pipeline.GpuLidarStacker
+    heat / size / orientation maps                                 device, data_pipeline.detections_to_heatmap
+    the 9-plane temporal BEV target (2 warpAffine per plane)       device, ops.bev_targets: one launch per batch, bit-identical
+                                                                   to the reference's OpenCV chain
+"""
+import glob
+import math
+import os
+from concurrent.futures import ThreadPoolExecutor
+
+import numpy as np
+import torch
+import yaml
+
+from . import data_paint, ops
+from .capi import LavbError
+from .data_pipeline import GpuLidarStacker, detections_to_heatmap
+from .synth import decode_png
+
+TRAIN_TOWNS = ("Town01", "Town03", "Town04", "Town06")          # basic_dataset.py:9
+BEV_SIZE = 320
+
+
+def index_trajectories(data_dir, percentage_data, all_towns, num_plan, seed):
+    """BasicDataset.__init__'s sample list (basic_dataset.py:29-72): one coin toss per entry of ``data_dir`` (seeded like
+    np.random.seed(seed)), entries without a data.mdb (or a directory store) skipped, the TRAIN_TOWNS filter unless all_towns;
+    frame indices 0 .. len - num_plan - 1 of each kept trajectory.  Entries are visited in sorted order (the reference takes
+    the file system's order).  -> (list of trajectory paths, list of (trajectory number, frame index))."""
+    rs = np.random.RandomState(seed)
+    paths, index = [], []
+    for path in sorted(glob.glob(os.path.join(data_dir, "*"))):
+        if rs.random_sample() > percentage_data:
+            continue
+        if not (os.path.exists(os.path.join(path, "data.mdb")) or os.path.isdir(os.path.join(path, "kv"))):
+            continue
+        env = data_paint.open_env(path)
+        n, town = int(env.get("len")), env.get("town").decode()
+        env.close()
+        if not all_towns and town not in TRAIN_TOWNS:
+            continue
+        paths.append(path)
+        index += [(len(paths) - 1, i) for i in range(n - num_plan)]
+    return paths, index
+
+
+def _frame(env, tag, i, dtype=np.float32):
+    return np.frombuffer(env.get(f"{tag}_{i:05d}"), dtype)
+
+
+def ego_pose(env, i):
+    """world pose of the ego (the first id of frame i) as BasicDataset.filter reads it: loc (2,) f64, yaw in radians."""
+    ids = _frame(env, "id", i, np.int32)
+    r = np.nonzero(ids == ids[0])[0][-1]
+    return _frame(env, "loc", i).reshape(-1, 2)[r].astype(np.float64), float(np.deg2rad(_frame(env, "ori", i)[r:r + 1])[0])
+
+
+def actor_tracks(env, index, T, max_pedestrian_radius, max_vehicle_radius):
+    """BasicDataset.filter + transform_ego (basic_dataset.py:103-157, lidar_dataset.py:132-148), vectorised.
+    -> ego_locs (T+1,2), locs (N,T+1,2), oris (N,T+1), bbox (N,T+1,2), typs (N,T+1) in the ego frame of ``index``, actors sorted
+    by id (the ego is one of them)."""
+    ids0 = _frame(env, "id", index, np.int32)
+    ego = ids0[0]
+    uid = np.unique(ids0)
+    n = len(uid)
+    seen = np.zeros((n, T + 1), bool)
+    locs, oris = np.zeros((n, T + 1, 2)), np.zeros((n, T + 1))
+    bbox, typs = np.zeros((n, T + 1, 2)), np.zeros((n, T + 1))
+    for k in range(T + 1):
+        ids = _frame(env, "id", index + k, np.int32)
+        pos = np.clip(np.searchsorted(uid, ids), 0, n - 1)
+        hit = uid[pos] == ids
+        p = pos[hit]
+        seen[p, k] = True
+        locs[p, k] = _frame(env, "loc", index + k).reshape(-1, 2)[hit]
+        oris[p, k] = np.deg2rad(_frame(env, "ori", index + k)[hit])
+        bbox[p, k] = _frame(env, "bbox", index + k).reshape(-1, 2)[hit]
+        typs[p, k] = _frame(env, "type", index + k, np.uint8)[hit]
+    e = int(np.searchsorted(uid, ego))
+    ego_locs, ego_ori = locs[e].copy(), oris[e, 0]
+    r = np.linalg.norm(locs[:, 0] - ego_locs[0], axis=1)
+    keep = seen.all(1) & ~((typs[:, 0] == 0) & (r > max_pedestrian_radius)) & ~((typs[:, 0] == 1) & (r > max_vehicle_radius))
+    R = [[np.sin(ego_ori), np.cos(ego_ori)], [-np.cos(ego_ori), np.sin(ego_ori)]]
+    origin = ego_locs[0]
+    return (ego_locs - origin) @ R, (locs[keep] - origin) @ R, oris[keep] - ego_ori, bbox[keep], typs[keep]
+
+
+def rotate_points(points, angle_deg, center):
+    r = np.deg2rad(angle_deg)
+    return (points - center) @ [[np.cos(r), np.sin(r)], [-np.sin(r), np.cos(r)]] + center
+
+
+class TemporalLiDARPaintedDataset:
+    """TemporalLiDARPaintedDataset (temporal_lidar_painted_dataset.py) over a recording, built on ``device``.
+
+    Same constructor, YAML keys, ``len`` and index mapping as the reference (BasicDataset, with the trajectories in sorted order);
+    ``ds[i]`` returns its 14-tuple as device tensors: lidar (max_lidar_points, 4+C+T) f32, num_points, heatmaps / sizemaps /
+    orimaps (2,320,320) f32, bev (9,320,320) uint8, -ego_locs (T+1,2) f64, cmd, -nxp (2,) f64, bra, -locs (max_objs,T+1,2) f32,
+    oris (max_objs,) f32, typs (max_objs,) int32, num_objs.  ``sample(idx, angle, jitters, generator)`` takes the random draws
+    explicitly; ``ds[i]`` draws them from generators seeded with ``seed``.  The draws have the reference's distributions but not
+    its random streams: the same seed gives other (equally distributed) augmentations than the reference."""
+
+    def __init__(self, config_path, seed=2021, device=torch.device("cuda")):
+        with open(config_path) as f:
+            cfg = yaml.safe_load(f)
+        self.cfg = cfg
+        for k, v in cfg.items():
+            setattr(self, k, v)
+        self.device = torch.device(device)
+        self.margin = ops.BEV_MARGIN
+        self.paths, self.index = index_trajectories(self.data_dir, self.percentage_data, self.all_towns, self.num_plan, seed)
+        self._envs = {}
+        self.stacker = GpuLidarStacker(self.num_frame_stack, len(self.seg_channels), self.max_lidar_points, self.camera_x,
+                                       self.camera_z, device=self.device)
+        self.rng = np.random.RandomState(seed)
+        self.gen = torch.Generator(device="cpu").manual_seed(seed)
+
+    def __len__(self):
+        return len(self.index)
+
+    def env(self, traj):
+        if traj not in self._envs:
+            self._envs[traj] = data_paint.open_env(self.paths[traj])
+        return self._envs[traj]
+
+    def draw(self, rng):
+        """(angle in degrees, stack jitters) with the reference's distributions (temporal_lidar_painted_dataset.py:21,50-51)."""
+        angle = float(rng.uniform(-1, 1)) * self.angle_jitter
+        jit = [(np.zeros(2), 0.0)] + [(rng.uniform(-self.stack_loc_jitter, self.stack_loc_jitter, 2),
+                                       float(rng.uniform(-self.stack_ori_jitter, self.stack_ori_jitter)))
+                                      for _ in range(self.num_frame_stack)]
+        return angle, jit
+
+    # ---- host part: record reads, PNG decode, labels, BEV job rows
+    def prepare(self, idx, angle, jitters):
+        traj, index = self.index[idx]
+        env = self.env(traj)
+        T, nseg = self.num_plan, len(self.seg_channels)
+        radii = (self.max_pedestrian_radius, self.max_vehicle_radius)
+        frames = [i for i in range(index, index - self.num_frame_stack - 1, -1) if i >= 0]
+        ego_locs, locs, oris, bbox, typs = actor_tracks(env, index, T, *radii)
+        poses = {i: ego_pose(env, i) for i in frames}
+        loc0, ori0 = poses[index]
+        sweeps = [(_frame(env, "lidar", i).reshape(-1, 4), _frame(env, "lidar_sem", i).reshape(-1, nseg), poses[i][0], poses[i][1])
+                  for i in frames]
+        planes = [decode_png(env.get(f"map_{c}_{index:05d}")) for c in (0, 9, 10)]
+        rows = [(c, c, 0.0, angle, 0, 0) for c in range(3)]                                   # load_bev_channels(angle=0, loc=0)
+        ppm = self.pixels_per_meter
+        for t, i in enumerate(frames):
+            loc, ori = poses[i]
+            dl = (loc - loc0) @ [[np.cos(ori0), -np.sin(ori0)], [np.sin(ori0), np.cos(ori0)]] * ppm
+            dx, dy = map(int, dl)
+            if abs(dx) > self.margin or abs(dy) > self.margin:
+                raise LavbError(f"frame {i} of {self.paths[traj]}: BEV shift ({dx}, {dy}) px exceeds the {self.margin}-pixel margin")
+            for c in (1, 2):
+                rows.append((len(planes), 3 + 2 * t + c - 1, -(ori - ori0) * 180 / math.pi, angle, dx, dy))
+                planes.append(decode_png(env.get(f"map_{c}_{i:05d}")))
+        rows += [(-1, 3 + 2 * t + c, 0.0, 0.0, 0, 0) for t in range(len(frames), self.num_frame_stack + 1) for c in (0, 1)]
+
+        locs = rotate_points(locs, -angle, ego_locs[0])
+        oris[1:] = oris[1:] - np.deg2rad(angle)
+        n_obj = min(len(locs), self.max_objs)
+        p_locs = np.zeros((self.max_objs, T + 1, 2), np.float32)
+        p_oris = np.zeros((self.max_objs,), np.float32)
+        p_typs = np.zeros((self.max_objs,), np.int32)
+        p_locs[:n_obj], p_oris[:n_obj], p_typs[:n_obj] = locs[:n_obj], oris[:n_obj, 0], typs[:n_obj, 0]
+        ego_rot = rotate_points(ego_locs, -angle, ego_locs[0])
+        nxp = rotate_points(_frame(env, "nxp", index).reshape(2), -angle, ego_rot[0])
+        return dict(sweeps=sweeps, angle=angle, jitters=jitters, planes=np.stack(planes), rows=rows,
+                    det=(locs[:, 0], oris[:, 0], bbox[:, 0], typs[:, 0]), ego_locs=-ego_rot, nxp=-nxp,
+                    cmd=int(_frame(env, "cmd", index, np.uint8)[0]), bra=int(_frame(env, "bra", index, np.uint8)[0]),
+                    locs=-p_locs, oris=p_oris, typs=p_typs, num_objs=n_obj)
+
+    # ---- device part
+    def lidar_and_maps(self, h, generator=None):
+        lidar, num = self.stacker(h["sweeps"], h["angle"], h["jitters"], generator=generator)
+        grid = dict(min_x=self.min_x, max_x=self.max_x, min_y=self.min_y, max_y=self.max_y, pixels_per_meter=self.pixels_per_meter)
+        heat, size, orim = detections_to_heatmap(*h["det"], device=self.device, **grid)
+        return lidar, num, heat, size, orim
+
+    def bev_batch(self, hs, planes=None):
+        """one bev_targets launch for the samples ``hs`` -> (len(hs), 9, 320, 320) uint8 on the device."""
+        n_bev = 3 + 2 * (self.num_frame_stack + 1)
+        rows, base = [], 0
+        for b, h in enumerate(hs):
+            rows += [(s + base if s >= 0 else -1, b * n_bev + d, a1, a2, dx, dy) for s, d, a1, a2, dx, dy in h["rows"]]
+            base += len(h["planes"])
+        if planes is None:
+            planes = torch.from_numpy(np.concatenate([h["planes"] for h in hs])).to(self.device)
+        out = torch.empty((len(hs), n_bev, BEV_SIZE, BEV_SIZE), dtype=torch.uint8, device=self.device)
+        return ops.bev_targets(planes, ops.bev_jobs(rows), out)
+
+    def sample(self, idx, angle, jitters, generator=None):
+        """the 14-tuple of sample ``idx`` for the given draws: angle (degrees), jitters[i] = (loc (2,), ori) of stacked frame i
+        (index - i; entry 0 is unused), generator = torch generator of the LiDAR row shuffle."""
+        h = self.prepare(idx, angle, jitters)
+        lidar, num, heat, size, orim = self.lidar_and_maps(h, generator)
+        bev = self.bev_batch([h])[0]
+        dev = self.device
+        return (lidar, num, heat, size, orim, bev, torch.as_tensor(h["ego_locs"], device=dev), h["cmd"],
+                torch.as_tensor(h["nxp"], device=dev), h["bra"], torch.as_tensor(h["locs"], device=dev),
+                torch.as_tensor(h["oris"], device=dev), torch.as_tensor(h["typs"], device=dev), h["num_objs"])
+
+    def __getitem__(self, idx):
+        angle, jit = self.draw(self.rng)
+        return self.sample(idx, angle, jit, self.gen)
+
+
+class TemporalBatchLoader:
+    """Batches of ``dataset`` for LAVTrainer.train_lidar, one rank of ``world``.
+
+    Each epoch shuffles the sample list with a permutation seeded by (seed, epoch) — the same on every rank — and rank r takes
+    every world-th entry; every rank yields the same number of batches (len // world // batch_size with drop_last).  While
+    batch k is on the GPU, one background thread reads the records and decodes the PNGs of batch k+1.  A batch is the 14-tuple
+    lidars (B,P,4+C+T) f32, num_points (B,) int64 (host), heatmaps / sizemaps / orimaps (B,2,320,320) f32, bev (B,9,320,320)
+    uint8, ego_locs (B,T+1,2) f32, cmds (B,) int64, nxps (B,2) f32, bras (B,) int64, locs (B,max_objs,T+1,2) f32, oris
+    (B,max_objs) f32, typs (B,max_objs) int32, num_objs (B,) int64; train_lidar takes the first 13."""
+
+    def __init__(self, dataset, batch_size, seed=2021, rank=0, world=1, drop_last=True):
+        self.ds, self.B, self.seed, self.rank, self.world, self.drop_last = dataset, batch_size, seed, rank, world, drop_last
+        self.epoch = 0
+
+    def shard(self, epoch):
+        perm = np.random.RandomState([self.seed, epoch]).permutation(len(self.ds))
+        return perm[self.rank::self.world][:len(self.ds) // self.world]
+
+    def __len__(self):
+        n = len(self.ds) // self.world
+        return n // self.B if self.drop_last else -(-n // self.B)
+
+    def _host(self, idxs, rng):
+        hs = [self.ds.prepare(int(i), *self.ds.draw(rng)) for i in idxs]
+        planes = torch.from_numpy(np.concatenate([h["planes"] for h in hs]))
+        return hs, planes.pin_memory() if self.ds.device.type == "cuda" else planes
+
+    def __iter__(self):
+        epoch, self.epoch = self.epoch, self.epoch + 1
+        order = self.shard(epoch)
+        batches = [order[k * self.B:(k + 1) * self.B] for k in range(len(self))]
+        rng = np.random.RandomState([self.seed, epoch, self.rank])
+        gen = torch.Generator(device="cpu").manual_seed(self.seed * 1000003 + epoch * 1009 + self.rank)
+        if not batches:
+            return
+        with ThreadPoolExecutor(1) as pool:
+            nxt = pool.submit(self._host, batches[0], rng)
+            for k in range(len(batches)):
+                hs, planes = nxt.result()
+                if k + 1 < len(batches):
+                    nxt = pool.submit(self._host, batches[k + 1], rng)
+                yield self._device(hs, planes, gen)
+
+    def _device(self, hs, planes, gen):
+        ds, dev = self.ds, self.ds.device
+        parts = [ds.lidar_and_maps(h, gen) for h in hs]
+        bev = ds.bev_batch(hs, planes.to(dev, non_blocking=True))
+        st = lambda i: torch.stack([p[i] for p in parts])
+        f32 = lambda key: torch.as_tensor(np.stack([h[key] for h in hs]), dtype=torch.float32).to(dev, non_blocking=False)
+        ints = lambda key, dt=torch.int64: torch.tensor([h[key] for h in hs], dtype=dt)
+        return (st(0), torch.tensor([p[1] for p in parts], dtype=torch.int64), st(2), st(3), st(4), bev, f32("ego_locs"),
+                ints("cmd").to(dev), f32("nxp"), ints("bra").to(dev), f32("locs"), f32("oris"),
+                torch.as_tensor(np.stack([h["typs"] for h in hs])).to(dev), ints("num_objs"))
+
+
+def get_data_loader(data_type, args):
+    """lav.utils.datasets.get_data_loader for 'temporal_lidar_painted' (args: config_path, seed, batch_size; optional rank,
+    world_size, device).  The other dataset types are not provided."""
+    if data_type != "temporal_lidar_painted":
+        raise NotImplementedError(f"data type {data_type!r}: only 'temporal_lidar_painted' is provided")
+    dev = getattr(args, "device", None) or torch.device("cuda", torch.cuda.current_device())
+    ds = TemporalLiDARPaintedDataset(args.config_path, seed=args.seed, device=dev)
+    return TemporalBatchLoader(ds, args.batch_size, args.seed, getattr(args, "rank", 0), getattr(args, "world_size", 1))

@@ -4,6 +4,7 @@ PyTorch is plumbing here: allocation, streams, views.  Every function launches h
 sm_90a kernels through lav_b200.capi; nothing falls back to torch math.
 """
 import ctypes as C
+import math
 
 import numpy as np
 import torch
@@ -387,6 +388,62 @@ def stack_jobs(d_jobs, n_jobs, max_n, src_cols, n_time, roof_filter=False):
     _need_cuda(d_jobs)
     check(lib().lavb_stack_jobs(_ptr(d_jobs), n_jobs, max_n, src_cols, n_time, int(roof_filter), _stream()), "lavb_stack_jobs")
     _COUNT[0] += 1
+
+
+# ----------------------------------------------------------------------------- temporal BEV targets
+BEV_JOB_DTYPE = np.dtype([("src", np.int64), ("dst", np.int64), ("m1", np.float64, 6), ("m2", np.float64, 6), ("dx", np.int32),
+                          ("dy", np.int32), ("pad", np.int32, 2)])
+assert BEV_JOB_DTYPE.itemsize == 128
+BEV_MARGIN = 32                  # TemporalLiDARPaintedDataset.margin (lidar_painted_dataset.py:19)
+
+
+def _inverse_rotation(angle_deg, center):
+    """inverse of cv2.getRotationMatrix2D(center, angle, 1.0), computed as cv::warpAffine inverts it (same operation order, so
+    the same fp64 roundings; math.cos / math.sin are the C library's, as OpenCV's)."""
+    a = angle_deg * (math.pi / 180)
+    c, s = math.cos(a), math.sin(a)
+    cx, cy = center
+    m = ((c, s, (1 - c) * cx - s * cy), (-s, c, s * cx + (1 - c) * cy))
+    det = m[0][0] * m[1][1] - m[0][1] * m[1][0]
+    d = 1.0 / det if det != 0 else 0.0
+    a11, a22, a12, a21 = m[1][1] * d, m[0][0] * d, -m[0][1] * d, -m[1][0] * d
+    return (a11, a12, -a11 * m[0][2] - a12 * m[1][2], a21, a22, -a21 * m[0][2] - a22 * m[1][2])
+
+
+def bev_jobs(rows, center=(160, 280)):
+    """rows of (src plane or -1, dst plane, first angle (deg), second angle (deg), dx, dy) -> BEV_JOB_DTYPE records for
+    bev_targets: each output plane is rotate(src, angle1) -> shift by (dx rows, dy columns) -> rotate(., angle2) -> > 0."""
+    jobs = np.zeros(len(rows), BEV_JOB_DTYPE)
+    for k, (src, dst, a1, a2, dx, dy) in enumerate(rows):
+        jobs[k] = (src, dst, _inverse_rotation(a1, center), _inverse_rotation(a2, center), dx, dy, (0, 0))
+    return jobs
+
+
+def bev_targets(src_planes, jobs, out=None):
+    """The temporal BEV target planes (load_bev_channels, temporal_lidar_painted_dataset.py:182-198) in one launch.
+    src_planes (P, h, w) uint8 CUDA; jobs: BEV_JOB_DTYPE records (see bev_jobs); out: uint8 CUDA tensor of (..., h, w) planes
+    (default (max dst + 1, h, w)).  Every plane a job names is overwritten with 0/1; a missing source (src < 0) gives zeros.
+    Raises LavbError for a shift beyond the 32-pixel margin, where the reference's crop fails."""
+    _need_cuda(src_planes)
+    assert src_planes.dtype == torch.uint8 and src_planes.dim() == 3 and src_planes.is_contiguous()
+    jobs = np.ascontiguousarray(jobs, dtype=BEV_JOB_DTYPE)
+    P, h, w = src_planes.shape
+    if len(jobs) and (np.abs(jobs["dx"]).max() > BEV_MARGIN or np.abs(jobs["dy"]).max() > BEV_MARGIN):
+        raise capi.LavbError(f"bev_targets: shift beyond the {BEV_MARGIN}-pixel margin "
+                             f"(dx {jobs['dx'].tolist()}, dy {jobs['dy'].tolist()})")
+    if out is None:
+        out = torch.empty((int(jobs["dst"].max()) + 1 if len(jobs) else 0, h, w), dtype=torch.uint8, device=src_planes.device)
+    _need_cuda(out)
+    assert out.dtype == torch.uint8 and out.is_contiguous() and tuple(out.shape[-2:]) == (h, w)
+    n_out = out.numel() // (h * w)
+    if len(jobs) and (jobs["src"].max() >= P or jobs["dst"].min() < 0 or jobs["dst"].max() >= n_out):
+        raise capi.LavbError(f"bev_targets: job plane index out of range ({P} source planes, {n_out} output planes)")
+    if len(jobs) == 0:
+        return out
+    d_jobs = torch.from_numpy(jobs.view(np.uint8)).to(src_planes.device)
+    check(lib().lavb_bev_targets(_ptr(d_jobs), len(jobs), _ptr(src_planes), _ptr(out), h, w, _stream()), "lavb_bev_targets")
+    _COUNT[0] += 1
+    return out
 
 
 def split_h16(x):

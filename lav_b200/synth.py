@@ -191,3 +191,111 @@ def loss_block_inputs(B=4, K=5, seed=SEED, num_cmds=6, num_plan=20, num_plan_ite
                    bev=(u(B, 9, 320, 320) > 0.7).to(torch.uint8), ego_locs=r(B, num_plan + 1, 2),
                    cmds=torch.randint(0, num_cmds, (B,), generator=g), bras=torch.tensor([0, 1, 0, 0][:B] + [0] * max(0, B - 4)))
     return outs, planner, targets
+
+
+# --------------------------------------------------------------------------- recorded trajectories
+def encode_png(gray):
+    """(h, w) uint8 -> grayscale PNG bytes (cv2 when it imports, else a stored-filter zlib writer; both lossless)."""
+    gray = np.ascontiguousarray(gray, dtype=np.uint8)
+    try:
+        import cv2
+    except ImportError:
+        cv2 = None
+    if cv2 is not None:
+        return cv2.imencode(".png", gray)[1].tobytes()
+    import struct
+    import zlib
+    h, w = gray.shape
+
+    def chunk(tag, data):
+        return struct.pack(">I", len(data)) + tag + data + struct.pack(">I", zlib.crc32(tag + data) & 0xFFFFFFFF)
+    raw = b"".join(b"\x00" + gray[r].tobytes() for r in range(h))
+    return (b"\x89PNG\r\n\x1a\n" + chunk(b"IHDR", struct.pack(">IIBBBBB", w, h, 8, 0, 0, 0, 0)) +
+            chunk(b"IDAT", zlib.compress(raw, 6)) + chunk(b"IEND", b""))
+
+
+def decode_png(data):
+    """grayscale PNG bytes -> (h, w) uint8, as cv2.imdecode(..., IMREAD_GRAYSCALE) (torchvision when cv2 is missing)."""
+    try:
+        import cv2
+    except ImportError:
+        cv2 = None
+    buf = np.frombuffer(data, np.uint8)
+    if cv2 is not None:
+        return cv2.imdecode(buf, cv2.IMREAD_GRAYSCALE)
+    from torchvision.io import ImageReadMode, decode_png as tv_decode
+    return tv_decode(torch.from_numpy(buf.copy()), ImageReadMode.GRAY)[0].numpy()
+
+
+def _road_planes(rs, h=320, w=320):
+    """12 binary (0/255) map planes of one frame: a road band, lane lines, a crossing and a few boxes."""
+    yy, xx = np.mgrid[:h, :w].astype(np.float64)
+    planes = np.zeros((12, h, w), np.uint8)
+    th = rs.uniform(-0.4, 0.4)
+    off = rs.uniform(-30, 30)
+    u = (xx - 160 - off) * np.cos(th) - (yy - 280) * np.sin(th)              # distance across the road
+    v = (xx - 160 - off) * np.sin(th) + (yy - 280) * np.cos(th)              # along it
+    cross = np.abs(v + rs.uniform(80, 200)) < rs.uniform(18, 30)
+    road = (np.abs(u) < rs.uniform(25, 40)) | cross
+    planes[0] = road * 255
+    planes[1] = (road & (np.abs(np.abs(u) - 12) < 1.5)) * 255                # lane lines
+    planes[2] = (road & (np.abs(u) < 1.2) & (np.mod(v, 24) < 12)) * 255       # dashed centre line
+    for c in range(3, 12):
+        for _ in range(rs.randint(0, 4)):
+            cx, cy, a, b = rs.uniform(40, 280), rs.uniform(40, 300), rs.uniform(3, 9), rs.uniform(2, 5)
+            planes[c] |= ((np.abs(xx - cx) < a) & (np.abs(yy - cy) < b)).astype(np.uint8) * 255
+    return planes
+
+
+def record_trajectories(root, n_traj=2, n_frames=30, seed=SEED, n_points=600, n_actors=12, seg_channels=4,
+                        towns=("Town01", "Town03", "Town02", "Town04", "Town05", "Town06")):
+    """Write ``n_traj`` seeded synthetic trajectories of ``n_frames`` frames under ``root`` in the reference's record layout
+    (basic_dataset.py:52-53,82-157, temporal_lidar_painted_dataset.py:29-30), through data_paint.DirEnv (one file per key):
+      len, town; lidar_%05d (n,4) f32; lidar_sem_%05d (n,C) f32; map_{0..11}_%05d grayscale PNG (0/255);
+      id (int32, ego first), loc (f32 (n,2) metres), ori (f32 degrees), bbox (f32 (n,2)), type (uint8), cmd / bra (uint8),
+      nxp (f32 (2,)) per frame.
+    The ego drives a smooth arc; the other actors move smoothly, some leave before the last frame, some are out of range.
+    Returns the trajectory directories."""
+    import os
+    from .data_paint import DirEnv
+    paths = []
+    for k in range(n_traj):
+        rs = np.random.RandomState(int.from_bytes(hashlib.sha256(f"{seed}:traj{k}".encode()).digest()[:4], "little"))
+        path = os.path.join(root, f"traj_{k:03d}")
+        env = DirEnv(path)
+        env.put("len", str(n_frames).encode())
+        env.put("town", towns[k % len(towns)].encode())
+        speed, yaw0, yaw_rate = rs.uniform(6, 12) / 20, rs.uniform(-180, 180), rs.uniform(-3, 3)
+        start = rs.uniform(-100, 100, 2)
+        ego_id = int(rs.randint(1, 100))
+        ids = ego_id + 1 + rs.choice(5000, n_actors, replace=False)
+        a_typ = (rs.rand(n_actors) > 0.35).astype(np.uint8)                  # 1 vehicle, 0 pedestrian
+        a_off = rs.uniform(-25, 25, (n_actors, 2))
+        a_off[-2:] *= 3                                                       # two actors beyond the radius cuts
+        a_vel = rs.uniform(-0.4, 0.4, (n_actors, 2))
+        a_ori = rs.uniform(-180, 180, n_actors)
+        a_box = np.where(a_typ[:, None] == 1, rs.uniform(1.8, 2.6, (n_actors, 2)), rs.uniform(0.3, 0.5, (n_actors, 2)))
+        a_last = np.where(rs.rand(n_actors) < 0.3, rs.randint(n_frames // 3, n_frames, n_actors), n_frames)   # leaves after a_last
+        for f in range(n_frames):
+            yaw = yaw0 + yaw_rate * f
+            heading = np.deg2rad(yaw0 + yaw_rate * f / 2)
+            ego_loc = start + speed * f * np.array([np.cos(heading), np.sin(heading)])
+            here = np.nonzero(f < a_last)[0]
+            locs = np.concatenate([ego_loc[None], ego_loc + a_off[here] + a_vel[here] * f])
+            env.put(f"id_{f:05d}", np.concatenate([[ego_id], ids[here]]).astype(np.int32).tobytes())
+            env.put(f"loc_{f:05d}", locs.astype(np.float32).tobytes())
+            env.put(f"ori_{f:05d}", np.concatenate([[yaw], a_ori[here] + 2 * f]).astype(np.float32).tobytes())
+            env.put(f"bbox_{f:05d}", np.concatenate([[[2.4, 1.1]], a_box[here]]).astype(np.float32).tobytes())
+            env.put(f"type_{f:05d}", np.concatenate([[1], a_typ[here]]).astype(np.uint8).tobytes())
+            env.put(f"cmd_{f:05d}", np.array([rs.randint(0, 6)], np.uint8).tobytes())
+            env.put(f"bra_{f:05d}", np.array([rs.rand() < 0.2], np.uint8).tobytes())
+            env.put(f"nxp_{f:05d}", (ego_loc + rs.uniform(-20, 20, 2)).astype(np.float32).tobytes())
+            pts = lidar_sweep(n_points, seed, f"rec{k}_{f}").numpy()
+            pts[:25, :3] = np.array([-1.2, 0.0, -1.25]) + rs.uniform(-0.3, 0.3, (25, 3)) * [1, 1, 0.5]   # ego-roof returns
+            sem = rs.rand(n_points, seg_channels) * (rs.rand(n_points, 1) > 0.4)
+            env.put(f"lidar_{f:05d}", pts.astype(np.float32).tobytes())
+            env.put(f"lidar_sem_{f:05d}", sem.astype(np.float32).tobytes())
+            for c, plane in enumerate(_road_planes(rs)):
+                env.put(f"map_{c}_{f:05d}", encode_png(plane))
+        paths.append(path)
+    return paths
