@@ -237,7 +237,15 @@ int lavb_det_peaks(const float* d_center, const float* d_box, const float* d_ori
  * [k][crop][crop][c] in the feature dtype. */
 int lavb_crop_bilinear(const void* d_feat, int dtype, int b, int h, int w, int c, const int* d_frame_idx,
                        const float* d_theta, int k, int crop, void* d_out, void* stream);
-/* gradient of the above with respect to d_feat (fp32 NHWC; training, lav/models/uniplanner.py:56-151 through F.grid_sample):
+/* the same crop from a uint8 PLANAR map (the ground-truth BEV): d_map [b][c][h][w] uint8 -> d_out NCHW [k][c][crop][crop] fp32.
+ * replaces: BEVPlanner.forward's `bev.float()`, `bev.expand(N,...).permute(...).contiguous()[typs]`, F.affine_grid and
+ *           F.grid_sample (lav/models/bev_planner_v2.py:92,104,146,222-264).
+ * Bit-identical to lavb_crop_bilinear (fp32) on the float copy of the map.  Frame indices outside [0, b) are clamped to the
+ * nearest frame, as in lavb_crop_bilinear.  Every output element is written (zeros where a sample leaves the map).
+ * c >= 1, crop >= 2, k <= 65535; no backward (the map is data). */
+int lavb_crop_bilinear_u8(const uint8_t* d_map, int b, int c, int h, int w, const int* d_frame_idx, const float* d_theta,
+                          int k, int crop, float* d_out, void* stream);
+/* gradient of lavb_crop_bilinear with respect to d_feat (fp32 NHWC; training, lav/models/uniplanner.py:56-151 through F.grid_sample):
  * replaces cudnn_grid_sampler_backward + the index_put of `features[frame]`.  A gather over the crops of each frame — no
  * atomics, fixed summation order, EVERY element of d_gfeat [b][h][w][c] is written (zeros where no crop samples). */
 int lavb_crop_bilinear_bwd(const float* d_gout, int b, int h, int w, int c, const int* d_frame_idx, const float* d_theta,

@@ -102,6 +102,8 @@ _SIGS = {
                                  C.c_void_p, C.c_void_p, C.c_void_p]),
     "lavb_crop_bilinear": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_int,
                                      C.c_int, C.c_void_p, C.c_void_p]),
+    "lavb_crop_bilinear_u8": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_int,
+                                        C.c_void_p, C.c_void_p]),
     "lavb_cast_gru": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int,
                                 C.c_int, C.c_void_p, C.c_void_p]),
     "lavb_conv_pair_set_trace": (C.c_int, [C.c_void_p, C.c_int]),

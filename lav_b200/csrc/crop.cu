@@ -94,6 +94,51 @@ __global__ void __launch_bounds__(256) crop_kernel(const T* __restrict__ feat, i
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
+// The same crop read straight from a uint8 PLANAR map (b, c, h, w) — the ground-truth BEV of the dataset and of bev_targets —
+// into an fp32 NCHW crop (k, c, S, S), the layout F.grid_sample returns and the 9-channel embedder's conv1 consumes.  It replaces
+// `bev.float()` + the per-crop gather + affine_grid + grid_sample of BEVPlanner's training forward.  HBM-write-bound (4 B per
+// output element, the u8 taps are re-read from L1 / L2), so a thread owns one output pixel and walks the channels: its sample
+// position and weights are computed once, and a warp stores 32 consecutive floats of one output row (128 B) per channel.
+// block = 32 x 8 output pixels (rows overlap in L1); grid = (patches per crop, crops).  Per channel, the four taps accumulate
+// in crop_kernel's order with its fmaf chain, so the result is bit-identical to crop_kernel<float> on the float copy of the map.
+// ---------------------------------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(256) crop_u8_kernel(const uint8_t* __restrict__ map, int B, int C, int H, int W,
+                                                      const int* __restrict__ frame_idx, const float* __restrict__ theta,
+                                                      int S, float* __restrict__ out) {
+  const int pw = (S + 31) >> 5;
+  const int pj = blockIdx.x / pw, pi = blockIdx.x - pj * pw;
+  const int k = blockIdx.y;
+  const int i = pi * 32 + (threadIdx.x & 31), j = pj * 8 + (threadIdx.x >> 5);
+  if (i >= S || j >= S) return;
+  float th[6];
+#pragma unroll
+  for (int e = 0; e < 6; ++e) th[e] = __ldg(theta + k * 6 + e);
+  float ix, iy;
+  crop_sample_pos(i, j, S, th, H, W, ix, iy);
+  const float fx = floorf(ix), fy = floorf(iy);
+  const int x0 = (int)fx, y0 = (int)fy;
+  const float ax = ix - fx, ay = iy - fy;
+  const float w00 = (1.f - ax) * (1.f - ay), w01 = ax * (1.f - ay), w10 = (1.f - ax) * ay, w11 = ax * ay;
+  const bool vx0 = x0 >= 0 && x0 < W, vx1 = x0 + 1 >= 0 && x0 + 1 < W, vy0 = y0 >= 0 && y0 < H, vy1 = y0 + 1 >= 0 && y0 + 1 < H;
+  const bool v00 = vx0 && vy0, v01 = vx1 && vy0, v10 = vx0 && vy1, v11 = vx1 && vy1;
+  int b = __ldg(frame_idx + k);
+  b = b < 0 ? 0 : (b >= B ? B - 1 : b);
+  const long long plane = (long long)H * W;
+  // offsets of the taps inside a plane, formed only for taps that lie on the map
+  const long long o00 = (long long)y0 * W + x0;
+  const uint8_t* src = map + (long long)b * C * plane;
+  float* dst = out + (long long)k * C * S * S + (long long)j * S + i;
+  for (int c = 0; c < C; ++c, src += plane, dst += (long long)S * S) {
+    float acc = 0.f;
+    if (v00) acc = fmaf(w00, (float)__ldg(src + o00), acc);
+    if (v01) acc = fmaf(w01, (float)__ldg(src + o00 + 1), acc);
+    if (v10) acc = fmaf(w10, (float)__ldg(src + o00 + W), acc);
+    if (v11) acc = fmaf(w11, (float)__ldg(src + o00 + W + 1), acc);
+    *dst = acc;
+  }
+}
+
+// ---------------------------------------------------------------------------------------------------------------------
 // Backward of the crop with respect to the feature map, as a GATHER (no atomics, every feature pixel written exactly once,
 // zeros included, fixed summation order): cudnn's bilinear_sampler_bw scatters 4 atomics per crop pixel and channel.
 //   gfeat[b, y, x, :] = sum over crops k of frame b, crop pixels (i, j) whose 2x2 footprint contains (x, y):  w * gout[k, j, i, :]
@@ -250,6 +295,22 @@ extern "C" int lavb_crop_bilinear(const void* d_feat, int dtype, int b, int h, i
     crop_kernel<h16><<<blocks, 256, 0, st>>>((const h16*)d_feat, b, h, w, c, d_frame_idx, d_theta, k, crop,
                                                            (h16*)d_out);
   else LAVB_CHECK_ARG(false, "crop_bilinear: bad dtype");
+  LAVB_LAUNCH_OK();
+  return 0;
+}
+
+// uint8 planar (b, c, h, w) map -> fp32 NCHW crops (k, c, crop, crop); frame indices are clamped to [0, b-1] as in
+// lavb_crop_bilinear.  Every output element is written (zeros where the sample falls off the map).
+extern "C" int lavb_crop_bilinear_u8(const uint8_t* d_map, int b, int c, int h, int w, const int* d_frame_idx, const float* d_theta,
+                                     int k, int crop, float* d_out, void* stream) {
+  LAVB_CHECK_ARG(c >= 1, "crop_bilinear_u8: need at least one channel (got %d)", c);
+  LAVB_CHECK_ARG(crop >= 2, "crop_bilinear_u8: crop size must be >= 2 (got %d)", crop);
+  LAVB_CHECK_ARG(b >= 1 && h >= 1 && w >= 1, "crop_bilinear_u8: empty map (%d x %d x %d)", b, h, w);
+  LAVB_CHECK_ARG(k >= 0, "crop_bilinear_u8: negative crop count");
+  if (k == 0) return 0;
+  LAVB_CHECK_ARG(k <= 65535, "crop_bilinear_u8: at most 65535 crops per call");
+  const dim3 blocks(((crop + 31) / 32) * ((crop + 7) / 8), k);
+  crop_u8_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(d_map, b, c, h, w, d_frame_idx, d_theta, crop, d_out);
   LAVB_LAUNCH_OK();
   return 0;
 }

@@ -1,5 +1,6 @@
 """Training data from recorded trajectories: TemporalLiDARPaintedDataset (lav/utils/datasets/temporal_lidar_painted_dataset.py)
-with its per-sample work on the GPU, and a batch loader for LAVTrainer.train_lidar.
+with its per-sample work on the GPU and a batch loader for LAVTrainer.train_lidar; TemporalBEVDataset
+(lav/utils/datasets/temporal_bev_dataset.py) and its loader for BEVTrainer.train_bev.
 
 Recording layout: the reference's keys (basic_dataset.py:52-53,82-101; data_paint.py writes lidar_sem_%05d), one key-value
 environment per trajectory directory (LMDB when the `lmdb` package imports and data.mdb exists, else data_paint.DirEnv).
@@ -15,6 +16,7 @@ What runs where:
 import glob
 import math
 import os
+import threading
 from concurrent.futures import ThreadPoolExecutor
 
 import numpy as np
@@ -269,11 +271,145 @@ class TemporalBatchLoader:
                 torch.as_tensor(np.stack([h["typs"] for h in hs])).to(dev), ints("num_objs"))
 
 
+class TemporalBEVDataset:
+    """TemporalBEVDataset (lav/utils/datasets/temporal_bev_dataset.py), the data of the privileged planner, over a recording.
+
+    Same constructor, YAML keys, ``len`` and index mapping as the reference (BasicDataset, trajectories in sorted order).
+    ``ds[i]`` returns its 9-tuple: bev (3+2*(num_frame_stack+1), 320, 320) uint8 on ``device`` (one bev_targets launch),
+    -ego_locs (T+1,2) f64, cmd, -nxp (2,) f64, bra, -locs (max_objs,T+1,2) f32, oris (max_objs,) f32, typs (max_objs,) int32,
+    num_objs.  ``sample(idx, offset, angle)`` takes the draws explicitly: the column shift ``offset`` in pixels and the rotation
+    ``angle`` in degrees.  ``ds[i]`` draws them from ``self.gen``, a torch CPU generator seeded with ``seed``, exactly as the
+    reference draws them from torch's global generator (temporal_bev_dataset.py:28-30), so a seeded stream replays."""
+
+    def __init__(self, config_path, seed=2021, device=torch.device("cuda")):
+        with open(config_path) as f:
+            cfg = yaml.safe_load(f)
+        self.cfg = cfg
+        for k, v in cfg.items():
+            setattr(self, k, v)
+        self.device = torch.device(device)
+        self.margin = ops.BEV_MARGIN
+        self.paths, self.index = index_trajectories(self.data_dir, self.percentage_data, self.all_towns, self.num_plan, seed)
+        self._envs, self._env_lock = {}, threading.Lock()
+        self.gen = torch.Generator(device="cpu").manual_seed(seed)
+
+    __len__ = TemporalLiDARPaintedDataset.__len__
+    bev_batch = TemporalLiDARPaintedDataset.bev_batch
+
+    def env(self, traj):
+        with self._env_lock:                        # the loader's threads share it: open each environment once per process
+            if traj not in self._envs:
+                self._envs[traj] = data_paint.open_env(self.paths[traj])
+            return self._envs[traj]
+
+    def draw(self, gen):
+        """(offset in pixels, angle in degrees): int of the fp32 draw clipped to the margin, then the angle — the reference's
+        expressions and order (temporal_bev_dataset.py:28-30)."""
+        offset = int((torch.rand(1, generator=gen) * 2 - 1) * self.x_jitter)
+        offset = int(np.clip(offset, -self.margin, self.margin))
+        angle = float(torch.rand(1, generator=gen) * 2 - 1) * self.angle_jitter
+        return offset, angle
+
+    # ---- host part: record reads, PNG decode, labels, BEV job rows
+    def prepare(self, idx, offset, angle):
+        traj, index = self.index[idx]
+        env = self.env(traj)
+        T = self.num_plan
+        ego_locs, locs, oris, _, typs = actor_tracks(env, index, T, self.max_pedestrian_radius, self.max_vehicle_radius)
+        frames = [i for i in range(index, index - self.num_frame_stack - 1, -1) if i >= 0]
+        poses = {i: ego_pose(env, i) for i in frames}
+        loc0, ori0 = poses[index]
+        planes = [decode_png(env.get(f"map_{c}_{index:05d}")) for c in (0, 9, 10)]
+        rows = [(c, c, 0.0, angle, 0, offset) for c in range(3)]                          # load_bev_channels(y_offset=offset)
+        ppm = self.pixels_per_meter
+        for t, i in enumerate(frames):
+            loc, ori = poses[i]
+            dl = (loc - loc0) @ [[np.cos(ori0), -np.sin(ori0)], [np.sin(ori0), np.cos(ori0)]] * ppm
+            dx, dy = map(int, dl)
+            if abs(dx) > self.margin or abs(dy + offset) > self.margin:
+                raise LavbError(f"frame {i} of {self.paths[traj]}: BEV shift ({dx}, {dy + offset}) px exceeds the "
+                                f"{self.margin}-pixel margin")
+            for c in (1, 2):
+                rows.append((len(planes), 3 + 2 * t + c - 1, -(ori - ori0) * 180 / math.pi, angle, dx, dy + offset))
+                planes.append(decode_png(env.get(f"map_{c}_{i:05d}")))
+        rows += [(-1, 3 + 2 * t + c, 0.0, 0.0, 0, 0) for t in range(len(frames), self.num_frame_stack + 1) for c in (0, 1)]
+
+        shift = [offset / ppm, 0]
+        locs = rotate_points(locs, -angle, ego_locs[0]) + shift                           # about the unshifted ego origin
+        oris[1:] = oris[1:] - np.deg2rad(angle)
+        ego = rotate_points(ego_locs, -angle, ego_locs[0]) + shift
+        nxp = rotate_points(_frame(env, "nxp", index).reshape(2), -angle, ego[0]) + shift  # about the SHIFTED ego origin
+        n_obj = min(len(locs), self.max_objs)
+        p_locs = np.zeros((self.max_objs, T + 1, 2), np.float32)
+        p_oris = np.zeros((self.max_objs,), np.float32)
+        p_typs = np.zeros((self.max_objs,), np.int32)
+        p_locs[:n_obj], p_oris[:n_obj], p_typs[:n_obj] = locs[:n_obj], oris[:n_obj, 0], typs[:n_obj, 0]
+        return dict(planes=np.stack(planes), rows=rows, ego_locs=-ego, nxp=-nxp, cmd=int(_frame(env, "cmd", index, np.uint8)[0]),
+                    bra=int(_frame(env, "bra", index, np.uint8)[0]), locs=-p_locs, oris=p_oris, typs=p_typs, num_objs=n_obj)
+
+    def sample(self, idx, offset, angle):
+        """the 9-tuple of sample ``idx`` for the given draws (offset in pixels, angle in degrees)."""
+        h = self.prepare(idx, offset, angle)
+        dev = self.device
+        return (self.bev_batch([h])[0], torch.as_tensor(h["ego_locs"], device=dev), h["cmd"], torch.as_tensor(h["nxp"], device=dev),
+                h["bra"], torch.as_tensor(h["locs"], device=dev), torch.as_tensor(h["oris"], device=dev),
+                torch.as_tensor(h["typs"], device=dev), h["num_objs"])
+
+    def __getitem__(self, idx):
+        return self.sample(idx, *self.draw(self.gen))
+
+
+class TemporalBEVBatchLoader(TemporalBatchLoader):
+    """Batches of a TemporalBEVDataset for BEVTrainer.train_bev, one rank of ``world``: the shuffle and sharding of
+    TemporalBatchLoader.  The draws of a batch come from one torch CPU generator seeded by (seed, epoch, rank), in sample
+    order; record reads and PNG decodes run on ``num_workers`` threads (a batch of 256 is about 2,300 decodes), one batch ahead
+    of the GPU.  A batch is the 9-tuple bev (B,9,320,320) uint8, ego_locs (B,T+1,2) f32, cmds (B,) int64, nxps (B,2) f32,
+    bras (B,) int64, locs (B,max_objs,T+1,2) f32, oris (B,max_objs) f32, typs (B,max_objs) int32, num_objs (B,) int64 (host),
+    with one bev_targets launch per batch."""
+
+    def __init__(self, dataset, batch_size, seed=2021, rank=0, world=1, drop_last=True, num_workers=8):
+        super().__init__(dataset, batch_size, seed, rank, world, drop_last)
+        self.num_workers = max(1, int(num_workers))
+
+    def _host_bev(self, idxs, draws, pool):
+        hs = list(pool.map(lambda a: self.ds.prepare(int(a[0]), *a[1]), zip(idxs, draws)))
+        planes = torch.from_numpy(np.concatenate([h["planes"] for h in hs]))
+        return hs, planes.pin_memory() if self.ds.device.type == "cuda" else planes
+
+    def __iter__(self):
+        epoch, self.epoch = self.epoch, self.epoch + 1
+        order = self.shard(epoch)
+        batches = [order[k * self.B:(k + 1) * self.B] for k in range(len(self))]
+        gen = torch.Generator(device="cpu").manual_seed(self.seed * 1000003 + epoch * 1009 + self.rank)
+        if not batches:
+            return
+        draws = lambda idxs: [self.ds.draw(gen) for _ in idxs]                  # on this thread, in sample order
+        with ThreadPoolExecutor(1) as ahead, ThreadPoolExecutor(self.num_workers) as pool:
+            nxt = ahead.submit(self._host_bev, batches[0], draws(batches[0]), pool)
+            for k in range(len(batches)):
+                hs, planes = nxt.result()
+                if k + 1 < len(batches):
+                    nxt = ahead.submit(self._host_bev, batches[k + 1], draws(batches[k + 1]), pool)
+                yield self._device_bev(hs, planes)
+
+    def _device_bev(self, hs, planes):
+        ds, dev = self.ds, self.ds.device
+        bev = ds.bev_batch(hs, planes.to(dev, non_blocking=True))
+        f32 = lambda key: torch.as_tensor(np.stack([h[key] for h in hs]), dtype=torch.float32).to(dev)
+        ints = lambda key: torch.tensor([h[key] for h in hs], dtype=torch.int64)
+        return (bev, f32("ego_locs"), ints("cmd").to(dev), f32("nxp"), ints("bra").to(dev), f32("locs"), f32("oris"),
+                torch.as_tensor(np.stack([h["typs"] for h in hs])).to(dev), ints("num_objs"))
+
+
 def get_data_loader(data_type, args):
-    """lav.utils.datasets.get_data_loader for 'temporal_lidar_painted' (args: config_path, seed, batch_size; optional rank,
-    world_size, device).  The other dataset types are not provided."""
-    if data_type != "temporal_lidar_painted":
-        raise NotImplementedError(f"data type {data_type!r}: only 'temporal_lidar_painted' is provided")
+    """lav.utils.datasets.get_data_loader for 'temporal_lidar_painted' and 'temporal_bev' (args: config_path, seed, batch_size;
+    optional rank, world_size, device, and num_workers for 'temporal_bev').  The other dataset types are not provided."""
+    if data_type not in ("temporal_lidar_painted", "temporal_bev"):
+        raise NotImplementedError(f"data type {data_type!r}: only 'temporal_lidar_painted' and 'temporal_bev' are provided")
     dev = getattr(args, "device", None) or torch.device("cuda", torch.cuda.current_device())
+    rank, world = getattr(args, "rank", 0), getattr(args, "world_size", 1)
+    if data_type == "temporal_bev":
+        ds = TemporalBEVDataset(args.config_path, seed=args.seed, device=dev)
+        return TemporalBEVBatchLoader(ds, args.batch_size, args.seed, rank, world, num_workers=getattr(args, "num_workers", 8))
     ds = TemporalLiDARPaintedDataset(args.config_path, seed=args.seed, device=dev)
-    return TemporalBatchLoader(ds, args.batch_size, args.seed, getattr(args, "rank", 0), getattr(args, "world_size", 1))
+    return TemporalBatchLoader(ds, args.batch_size, args.seed, rank, world)

@@ -5,7 +5,7 @@ keys (tests/golden/keys_uniplanner.json, keys_brake.json):
 
   resnet18            lav/models/resnet.py:144-283 (num_channels stem, returns the layer4 map)
   UniPlanner          team_code_v2/models/uniplanner.py (infer path) — crop -> embed -> cast/plan GRUs
-  BEVPlanner          team_code_v2/models/bev_planner.py (parameters only; teacher is used in training)
+  BEVPlanner          lav/models/bev_planner_v2.py (training forward; the frozen teacher of UniPlanner's distillation)
   RGBBrakePredictionModel, Attention, SegmentationHead
                       team_code_v2/models/rgb.py:48-83, lav/models/attention.py, segmentation.py
 
@@ -236,14 +236,43 @@ def crop_theta(rel_locs, rel_oris, H, W, pixels_per_meter, crop_size, offset_x, 
                         torch.stack([k * sin, k * cos, rot_y_offset + rel_y], dim=-1)], dim=-2)
 
 
+def _pose_jitter(n, x_jitter, angle_jitter, device):
+    """augmentation of a crop's pose: lateral offset U(-x_jitter, x_jitter) metres (no longitudinal part) and heading
+    U(-angle_jitter, angle_jitter) radians.  Drawn on the CPU generator as rand(n,2) then rand(n): the reference's stream order
+    (uniplanner.py:83-86,118-121, bev_planner_v2.py:100-102)."""
+    shift = (torch.rand(n, 2) * 2 - 1) * x_jitter
+    shift[:, 1] = 0
+    turn = (torch.rand(n) * 2 - 1) * angle_jitter
+    return shift.to(device), turn.to(device)
+
+
+def _cap_rows_host(mask, limit):
+    """cap_per_sample(mask, limit) with ONE device->host copy of the mask instead of one synchronisation per row: the same
+    multinomial draws in the same row order, so the same actors are kept.  -> (frame, slot) index tensors on the mask's device,
+    in row-major order (the order of a boolean-mask gather)."""
+    m = mask.cpu()
+    for b in range(m.shape[0]):
+        on = m[b].nonzero().flatten()
+        if on.numel() > limit:
+            keep = on[torch.multinomial(torch.ones(on.numel()), limit)]
+            m[b] = False
+            m[b, keep] = True
+    frame, slot = m.nonzero(as_tuple=True)
+    return frame.to(mask.device), slot.to(mask.device)
+
+
 class BEVPlanner(nn.Module):
-    """Weight container for the privileged teacher nested in the UniPlanner checkpoint (bev_planner.*)."""
+    """The privileged planner (lav/models/bev_planner_v2.py): the teacher nested in the UniPlanner checkpoint (bev_planner.*),
+    and trained on its own from ground-truth BEV maps by ``forward`` (stage 1 of the v2 recipe, lav_b200.train_bev)."""
 
     def __init__(self, pixels_per_meter=2, crop_size=64, x_offset=0, y_offset=0.75, feature_x_jitter=1, feature_angle_jitter=10,
                  num_plan=10, k=16, num_out_feature=64, num_cmds=6, max_num_cars=5, num_plan_iter=1, num_frame_stack=0):
         super().__init__()
-        self.num_cmds, self.num_plan, self.num_plan_iter = num_cmds, num_plan, num_plan_iter
+        self.num_cmds, self.num_plan, self.num_plan_iter, self.max_num_cars = num_cmds, num_plan, num_plan_iter, max_num_cars
+        self.num_out_feature = num_out_feature
         self.pixels_per_meter, self.crop_size = pixels_per_meter, crop_size
+        self.feature_x_jitter = feature_x_jitter
+        self.feature_angle_jitter = np.deg2rad(feature_angle_jitter)
         self.offset_x = nn.Parameter(torch.tensor(x_offset).float(), requires_grad=False)
         self.offset_y = nn.Parameter(torch.tensor(y_offset).float(), requires_grad=False)
         self.bev_conv_emb = nn.Sequential(resnet18(num_channels=3 + 2 * (num_frame_stack + 1)), nn.AdaptiveAvgPool2d((1, 1)), nn.Flatten())
@@ -253,12 +282,60 @@ class BEVPlanner(nn.Module):
         self.cast_mlps = nn.ModuleList([nn.Linear(64, 2) for _ in range(num_cmds)])
         self.cast_cmd_pred = nn.Sequential(nn.Linear(512, num_cmds), nn.Sigmoid())
 
-    # the frozen teacher of the distillation step (lav/models/bev_planner_v2.py:176-262); PyTorch, no grad needed
-    def crop_feature(self, features, rel_locs, rel_oris, pixels_per_meter=4, crop_size=96):
+    def crop_feature(self, features, rel_locs, rel_oris, pixels_per_meter=4, crop_size=96, frame_idx=None):
+        """BEVPlanner.crop_feature (bev_planner_v2.py:222-264).  A uint8 CUDA map (B,C,H,W) goes through the lav_b200 kernel
+        (ops.crop_bilinear_u8): crop k reads frame ``frame_idx[k]`` (default k) straight from the bytes, -> fp32 NCHW crops.
+        Every other input takes F.affine_grid + F.grid_sample (the frozen teacher of train_lidar passes fp32 maps), after
+        gathering ``features[frame_idx]`` when frame indices are given."""
         B, C, H, W = features.size()
         theta = crop_theta(rel_locs, rel_oris, H, W, pixels_per_meter, crop_size, self.offset_x, self.offset_y)
+        if features.is_cuda and features.dtype == torch.uint8:
+            if frame_idx is None:
+                frame_idx = torch.arange(theta.shape[0], device=features.device, dtype=torch.int32)
+            return ops.crop_bilinear_u8(features.contiguous(), frame_idx, theta.detach(), crop_size)
+        if frame_idx is not None:
+            features = features[frame_idx.long()]
+            B = features.shape[0]
         grids = F.affine_grid(theta, torch.Size((B, C, crop_size, crop_size)), align_corners=True)
         return F.grid_sample(features, grids, align_corners=True)
+
+    def forward(self, bev, ego_locs, locs, oris, nxps, typs):
+        """Training forward of the privileged planner (bev_planner_v2.py:72-174): from crops of the ground-truth BEV ``bev``
+        (B,C,H,W) — uint8 on the GPU takes the lav_b200 crop kernel, anything else is cast to fp32 and takes grid_sample —
+        forecast the vehicles ahead of each ego (at most max_num_cars per sample, pose jittered) and plan for the ego (no jitter).
+        locs / oris / typs slot 0 is the ego.  Returns the reference's 6-tuple
+            (other_locs, other_cast_locs, other_cast_cmds, ego_plan_locs, ego_cast_locs, ego_cast_cmds).
+        Random draws keep the reference's order on the CPU generator: the per-row multinomial cap, then rand(K,2), rand(K).
+        Others and egos go through the embedder in two calls, so BatchNorm sees the reference's two batches."""
+        if not (bev.is_cuda and bev.dtype == torch.uint8):
+            bev = bev.float()
+        dev = bev.device
+        dt = torch.float32 if bev.dtype == torch.uint8 else bev.dtype
+        ppm, crop = self.pixels_per_meter, 2 * self.crop_size
+        ego_heading = oris[:, :1]
+        act_locs, act_oris = locs[:, 1:], oris[:, 1:]
+        slots = act_locs.shape[1]
+        chosen = vehicles_ahead(ego_locs, act_locs, typs[:, 1:] == 1)
+        if bool(chosen.any()):
+            frame, slot = _cap_rows_host(chosen, self.max_num_cars)
+            future = act_locs[frame, slot, 1:] - act_locs[frame, slot, :1]
+            start = act_locs[frame, slot, 0] - ego_locs[frame, 0]
+            heading = act_oris[frame, slot] - ego_heading[frame, 0]
+            shift, turn = _pose_jitter(frame.numel(), self.feature_x_jitter, self.feature_angle_jitter, dev)
+            crops = self.crop_feature(bev, start + shift, heading + turn, pixels_per_meter=ppm, crop_size=crop, frame_idx=frame)
+            other_locs = transform_points(future - shift[:, None], -heading - turn)
+            other_embd = self.bev_conv_emb(crops)
+            other_cast, other_cmds = self.cast(other_embd), self.cast_cmd_pred(other_embd)
+        else:                                                               # no vehicle ahead: zero placeholders, one per slot
+            other_locs = torch.zeros((slots, self.num_plan, 2), dtype=dt, device=dev)
+            other_cast = torch.zeros((slots, self.num_cmds, self.num_plan, 2), dtype=dt, device=dev)
+            other_cmds = torch.zeros((slots, self.num_cmds), dtype=dt, device=dev)
+        B = bev.shape[0]
+        zero = torch.zeros((B, 2), dtype=dt, device=dev)
+        ego_embd = self.bev_conv_emb(self.crop_feature(bev, zero, zero[:, 0], pixels_per_meter=ppm, crop_size=crop))
+        ego_cast = self.cast(ego_embd)
+        ego_plan = self.plan(ego_embd, nxps, cast_locs=ego_cast, pixels_per_meter=ppm, crop_size=crop)
+        return other_locs, other_cast, other_cmds, ego_plan, ego_cast, self.cast_cmd_pred(ego_embd)
 
     def cast(self, embd):
         return _cast_branches(self, self.cast_grus, self.cast_mlps, embd, self.num_plan)
@@ -368,10 +445,7 @@ class UniPlanner(nn.Module):
     def _jitter(self, n, device):
         """augmentation of a crop's pose: lateral offset U(-jx, jx) metres (no longitudinal part) and heading U(-ja, ja).
         Drawn on the CPU generator as rand(n,2) then rand(n): the reference's stream order (uniplanner.py:83-86,118-121)."""
-        shift = (torch.rand(n, 2) * 2 - 1) * self.feature_x_jitter
-        shift[:, 1] = 0
-        turn = (torch.rand(n) * 2 - 1) * self.feature_angle_jitter
-        return shift.to(device), turn.to(device)
+        return _pose_jitter(n, self.feature_x_jitter, self.feature_angle_jitter, device)
 
     def _student(self, crops):
         """crops (n,C,crop,crop) -> (embedding, cast (n,cmds,T,2), command scores (n,cmds)); one call = one BatchNorm batch."""

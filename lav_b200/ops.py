@@ -289,6 +289,31 @@ def crop_bilinear(feats_nhwc, frame_idx, theta, crop_size):
     return out
 
 
+def crop_bilinear_u8(bev_u8, frame_idx, theta, crop_size, out=None):
+    """bev_u8 (B,C,H,W) contiguous uint8; frame_idx (K,) int32; theta (K,2,3) fp32 -> fp32 NCHW (K,C,crop,crop): the crops of
+    crop_bilinear read straight from a uint8 planar map (bit-identical to crop_bilinear on its float copy).  Frame indices
+    outside [0, B) are clamped to the nearest frame.  ``out`` (K,C,crop,crop) fp32 contiguous is written in full if given."""
+    _need_cuda(bev_u8, frame_idx, theta)
+    if bev_u8.dtype != torch.uint8 or bev_u8.dim() != 4:
+        raise capi.LavbError(f"crop_bilinear_u8: need a 4-d uint8 map, got {bev_u8.dtype} {tuple(bev_u8.shape)}")
+    if not bev_u8.is_contiguous():
+        raise capi.LavbError("crop_bilinear_u8: the map must be contiguous (B,C,H,W)")
+    b, c, h, w = bev_u8.shape
+    k = theta.shape[0]
+    if tuple(theta.shape) != (k, 2, 3) or frame_idx.numel() != k:
+        raise capi.LavbError(f"crop_bilinear_u8: theta {tuple(theta.shape)} / frame_idx {tuple(frame_idx.shape)} do not describe K crops")
+    theta = theta.float().contiguous()
+    frame_idx = frame_idx.to(torch.int32).contiguous()
+    if out is None:
+        out = torch.empty((k, c, crop_size, crop_size), dtype=torch.float32, device=bev_u8.device)
+    elif tuple(out.shape) != (k, c, crop_size, crop_size) or out.dtype != torch.float32 or not out.is_contiguous():
+        raise capi.LavbError(f"crop_bilinear_u8: out must be a contiguous fp32 ({k}, {c}, {crop_size}, {crop_size}) tensor")
+    check(lib().lavb_crop_bilinear_u8(_ptr(bev_u8), b, c, h, w, _ptr(frame_idx), _ptr(theta), k, crop_size, _ptr(out), _stream()),
+          "lavb_crop_bilinear_u8")
+    _COUNT[0] += 1
+    return out
+
+
 def crop_bilinear_bwd(gout_nhwc, frame_idx, theta, feat_shape):
     """gout_nhwc (K,crop,crop,C) fp32 contiguous -> gradient of crop_bilinear w.r.t. the (B,H,W,C) fp32 feature map."""
     _need_cuda(gout_nhwc, frame_idx, theta)

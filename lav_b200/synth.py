@@ -169,6 +169,29 @@ def _is_transposed_key(k):
     return k.endswith("_head.net.3.weight") or ("decoder.layers.0.conv" in k) or ("decoder.layers.3.conv" in k)
 
 
+def bev_planner_batch(seed=SEED, B=3, n_actors=8, T=21, no_vehicles=False):
+    """Seeded train_bev batch for the privileged planner: bev (B,9,320,320) uint8 0/1, ego_locs (B,T,2), cmds (B,), nxps (B,2),
+    bras (B,), locs (B,n_actors,T,2) with slot 0 = the ego, oris (B,n_actors), typs (B,n_actors) int64.  Sample 0 has every actor
+    a vehicle ahead (more than max_num_cars = 5: the multinomial path), sample 1 a mix, the last none.  ``no_vehicles``: no
+    actor is a vehicle (the zero-placeholder path).  Used by oracle/pin_bev.py and the tests."""
+    g = _gen(seed, f"bevbatch{B}{n_actors}{int(no_vehicles)}")
+    bev = (torch.rand(B, 9, 320, 320, generator=g) > 0.7).to(torch.uint8)
+    ego_locs = torch.cumsum(torch.rand(B, T, 2, generator=g) * torch.tensor([0.2, -1.0]), dim=1)
+    locs = torch.randn(B, n_actors, T, 2, generator=g) * torch.tensor([5.0, 4.0]) + torch.tensor([0.0, -12.0])
+    locs[:, 0] = ego_locs
+    locs[-1, 1:, :, 1] = locs[-1, 1:, :, 1].abs() + 2.0                      # last sample: every actor behind the ego
+    oris = torch.rand(B, n_actors, generator=g) * 0.6 - 0.3
+    typs = torch.ones(B, n_actors, dtype=torch.int64)
+    typs[1, 1::2] = 0
+    if no_vehicles:
+        typs[:] = 0
+    cmds = torch.randint(0, 6, (B,), generator=g)
+    nxps = torch.tensor([[0.0, -20.0]]).repeat(B, 1) + torch.randn(B, 2, generator=g)
+    bras = torch.zeros(B, dtype=torch.int64)
+    bras[1] = 1
+    return bev, ego_locs, cmds, nxps, bras, locs, oris, typs
+
+
 def loss_block_inputs(B=4, K=5, seed=SEED, num_cmds=6, num_plan=20, num_plan_iter=5):
     """Seeded stand-ins for everything the loss block of LAV.train_lidar consumes (lav/lav_final_v2.py:177-225): the five
     LiDARModel outputs, the eleven UniPlanner outputs and the targets.  Used by oracle/pin_against_reference.py (which feeds

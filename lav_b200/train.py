@@ -352,6 +352,74 @@ class LAVTrainer:
         return loss.detach(), parts
 
 
+# --------------------------------------------------------------------------- privileged planner (stage 1 of the v2 recipe)
+def bev_losses(planner_out, ego_locs, cmds, bras, branch_weights, other_weight=0.0, cmd_weight=0.1, cmd_smooth=0.2):
+    """LAV.train_bev's losses (lav/lav_privileged_v2.py:131-142) term for term -> (total loss, dict of the 4 terms).
+    planner_out = the 6 BEVPlanner.forward outputs; ego_locs (B,T+1,2), cmds (B,), bras (B,) 0/1.
+      plan_loss      L1 of every iteration and command branch of the plan against the ego's future, mean per sample over the
+                     samples WITHOUT a brake label only, weighted by the branch weight of the command (NaN when all brake)
+      ego_cast_loss  L1 of the commanded cast branch against the ego's future, over all samples
+      other_cast_loss L1 of the best command branch per forecast vehicle, scaled by ``other_weight`` in the total
+      cmd_loss       BCE of the command scores against smoothed one-hot targets, scaled by ``cmd_weight`` in the total"""
+    other_next, other_cast, _other_cmds, ego_plan, ego_cast, ego_cmds = planner_out
+    cmds = cmds.long()
+    moving = (1 - bras).bool().to(cmds.device)
+    n_iter, n_cmds, T = ego_plan.shape[1], ego_plan.shape[2], ego_plan.shape[3]
+    future = ego_locs[:, 1:]
+    plan = torch.mean(F.l1_loss(ego_plan, future[:, None, None].repeat(1, n_iter, n_cmds, 1, 1), reduction="none")
+                      .mean(dim=[1, 2, 3, 4])[moving] * branch_weights[cmds[moving]])
+    commanded = ego_cast.gather(1, cmds.expand(T, 2, 1, -1).permute(3, 2, 0, 1)).squeeze(1)
+    ego_c = F.l1_loss(commanded, future, reduction="none").mean(dim=[1, 2]).mean()
+    other_c = F.l1_loss(other_cast, other_next.unsqueeze(1).repeat(1, n_cmds, 1, 1), reduction="none").mean(dim=[2, 3]).min(1)[0].mean()
+    cmd = F.binary_cross_entropy(ego_cmds, (1.0 - cmd_smooth) * F.one_hot(cmds, n_cmds) + cmd_smooth / n_cmds)
+    total = plan + ego_c + other_c * other_weight + cmd * cmd_weight
+    return total, dict(plan_loss=plan, ego_cast_loss=ego_c, other_cast_loss=other_c, cmd_loss=cmd)
+
+
+def other_weight_schedule(it, beta=0.8):
+    """weight of the other-vehicle forecast loss at global step ``it`` (lav/train_bev_v2.py:36-37): 0 at the start, -> 1."""
+    return 1 - beta ** (it / 4000)
+
+
+class BEVTrainer:
+    """LAV.train_bev (lav/lav_privileged_v2.py:110-160) as one process per GPU: Adam at ``lr`` over every BEVPlanner parameter,
+    StepLR(32, 0.5) stepped once per epoch by the caller (``sched``), gradients averaged across ranks by GradAllReducer.
+    Precision as LAVTrainer: fp32 tensors under PyTorch's defaults (cuDNN convolutions may use TF32, as in the reference).
+    The map may stay uint8 on the GPU: BEVPlanner.forward crops it with the lav_b200 kernel instead of a float copy."""
+
+    def __init__(self, bev_planner, lr=3e-4, device=None, branch_weights=(5, 5, 5, 1, 1, 1), cmd_weight=0.1, cmd_smooth=0.2,
+                 use_others_to_train=True, bucket_bytes=25 << 20):
+        self.model = bev_planner.train()
+        self.device = device or next(bev_planner.parameters()).device
+        self.optim = torch.optim.Adam(self.model.parameters(), lr=lr)
+        self.sched = torch.optim.lr_scheduler.StepLR(self.optim, step_size=32, gamma=0.5)
+        self.reducer = GradAllReducer(self.model.parameters(), bucket_bytes)
+        self.branch_weights = torch.tensor(branch_weights).float().to(self.device)
+        self.cmd_weight, self.cmd_smooth, self.use_others_to_train = cmd_weight, cmd_smooth, bool(use_others_to_train)
+
+    def other_weight(self, it):
+        return other_weight_schedule(it) if self.use_others_to_train else 0.0
+
+    def losses(self, bev, ego_locs, cmds, nxps, bras, locs, oris, typs, other_weight=0.0):
+        dev = self.device
+        if not self.use_others_to_train:
+            other_weight = 0.0
+        ego_locs = ego_locs.float().to(dev)
+        out = self.model(bev.to(dev), ego_locs, locs.float().to(dev), oris.float().to(dev), nxps.float().to(dev), typs.to(dev))
+        loss, parts = bev_losses(out, ego_locs, cmds.to(dev), bras.to(dev), self.branch_weights, other_weight, self.cmd_weight,
+                                 self.cmd_smooth)
+        return loss, {k: v.detach() for k, v in parts.items()}
+
+    def train_bev(self, bev, ego_locs, cmds, nxps, bras, locs, oris, typs, num_objs=None, other_weight=0.0):
+        """one step on this rank's sub-batch: the 9-tuple of TemporalBEVDataset (num_objs unused, as in the reference)."""
+        loss, parts = self.losses(bev, ego_locs, cmds, nxps, bras, locs, oris, typs, other_weight)
+        self.optim.zero_grad(set_to_none=True)
+        loss.backward()
+        self.reducer.finish()
+        self.optim.step()
+        return loss.detach(), parts
+
+
 def synthetic_train_batch(B, device, seed=2021, n_points=(60000, 120000), n_obj=6):
     """seeded batch with the shapes of SURVEY 8(a) a18: lidar (B,120000,11), maps (B,2,320,320), bev (B,9,320,320) ..."""
     from . import synth
