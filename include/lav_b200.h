@@ -152,8 +152,20 @@ int lavb_pillar_forward_tiled(const float* d_pts, int pt_stride, int d,
 /* training-mode pieces (BatchNorm1d batch statistics over all in-window points, arg-routed backward).
  * stage 0: voxelise + decorate -> d_feat [M][d+5] (M = number of in-window points, returned in *h_m),
  *          d_cell [M] int32 canvas cell id (b*ny*nx + row*nx + col), -1 never appears.
+ *          Rows come in input order: clouds in batch order, points in their order within the cloud (an order-preserving
+ *          compaction of the in-window points).  A pillar is (b, xi, yi) before any clamp, so a y that rounds to yi == nx
+ *          (SURVEY App. C.5) forms its own pillar for the centroid and cell-origin columns, while its cell clamps onto
+ *          col nx-1 (an x that rounds up to the last index likewise clamps onto row 0).  pt_stride >= d, 1 <= batch <= 128,
+ *          d == 11.
  * The Linear/BN1d/ReLU stack then runs on d_feat with autograd; stage 1 max-pools rows into the canvas and
- * records the arg-max row per (cell, channel) for the backward. */
+ * records the arg-max row per (cell, channel) for the backward:
+ *   precondition: d_h >= 0 (post-ReLU) and 0 <= d_cell[r] < n_cells; m >= 0, c >= 1, n_cells >= 0.
+ *   canvas[cell, ch] = max over the rows r of that cell of h[r, ch]; an empty cell holds 0.  When two pillars share a
+ *   cell (the clamp above), the cell holds the per-channel max over the rows of both.
+ *   argmax[cell, ch] = the SMALLEST row r of that cell with h[r, ch] == canvas[cell, ch] (ties, including channels
+ *   whose rows are all 0, go to the smallest row); an empty cell holds 0x7f7f7f7f.  d_argmax may be null.
+ * backward: gh[r, ch] = gcanvas[cell[r], ch] if argmax[cell[r], ch] == r else 0, so each (cell, channel) gradient
+ *   reaches exactly one row. */
 int lavb_pillar_decorate(const float* d_pts, int pt_stride, int d,
                          const long long* h_cloud_start, const int* h_cloud_count, int batch,
                          float min_x, float max_x, float min_y, float max_y, float ppm, int nx, int ny,

@@ -1063,6 +1063,7 @@ extern "C" int lavb_pillar_decorate(const float* d_pts, int pt_stride, int d, co
   Clouds clouds;
   if (fill_clouds(clouds, h_cloud_start, h_cloud_count, batch)) return 1;
   LAVB_CHECK_ARG(d == 11, "pillar_decorate: only D=11 is built (got %d)", d);
+  LAVB_CHECK_ARG(pt_stride >= d, "pillar_decorate: pt_stride < d");
   cudaStream_t st = (cudaStream_t)stream;
   Grid g{min_x, max_x, min_y, max_y, ppm, nx, ny};
   float4* stats = reinterpret_cast<float4*>(d_workspace);
@@ -1091,6 +1092,7 @@ extern "C" int lavb_pillar_decorate(const float* d_pts, int pt_stride, int d, co
 
 extern "C" int lavb_pillar_scatter_max(const float* d_h, const int* d_cell, int m, int c, long long n_cells, float* d_canvas,
                                        int* d_argmax, void* stream) {
+  LAVB_CHECK_ARG(m >= 0 && c >= 1 && n_cells >= 0, "pillar_scatter_max: bad shape (m=%d, c=%d, n_cells=%lld)", m, c, n_cells);
   cudaStream_t st = (cudaStream_t)stream;
   LAVB_CUDA_OK(cudaMemsetAsync(d_canvas, 0, (size_t)n_cells * c * sizeof(float), st));
   if (d_argmax) LAVB_CUDA_OK(cudaMemsetAsync(d_argmax, 0x7f, (size_t)n_cells * c * sizeof(int), st));
@@ -1107,6 +1109,7 @@ extern "C" int lavb_pillar_scatter_max(const float* d_h, const int* d_cell, int 
 
 extern "C" int lavb_pillar_scatter_max_bwd(const float* d_gcanvas, const int* d_argmax, const int* d_cell, int m, int c,
                                                  float* d_gh, void* stream) {
+  LAVB_CHECK_ARG(m >= 0 && c >= 1, "pillar_scatter_max_bwd: bad shape (m=%d, c=%d)", m, c);
   const long long mc = (long long)m * c;
   if (mc == 0) return 0;
   scatter_bwd_kernel<<<ceil_div(mc, 256), 256, 0, (cudaStream_t)stream>>>(d_gcanvas, d_argmax, d_cell, mc, c, d_gh);

@@ -149,8 +149,9 @@ def pillar_forward(pts, starts, counts, grid, w1, s1, t1, w2, s2, t2):
 
 
 def pillar_decorate(pts, starts, counts, grid, d):
-    """training stage 0: returns (feat (M,d+5) fp32, cell (M,) int32)."""
+    """training stage 0: returns (feat (M,d+5) fp32, cell (M,) int32), rows in input order (clouds in batch order)."""
     _need_cuda(pts)
+    assert pts.dtype == torch.float32 and pts.dim() == 2 and pts.stride(1) == 1
     min_x, max_x, min_y, max_y, ppm, nx, ny = grid
     b, st, ct = _clouds(starts, counts)
     ws = _workspace(pts.device, lib().lavb_pillar_workspace_bytes(b, nx, ny))
@@ -165,7 +166,12 @@ def pillar_decorate(pts, starts, counts, grid, d):
 
 
 def pillar_scatter_max(h, cell, n_cells, want_argmax=True):
+    """training stage 1: h (M,C) fp32 >= 0, cell (M,) int32 in [0, n_cells) -> (canvas (n_cells,C) fp32, arg (n_cells,C) int32
+    or None).  See lavb_pillar_scatter_max in include/lav_b200.h for the tie rule and the empty-cell values."""
     _need_cuda(h, cell)
+    assert h.dtype == torch.float32 and h.dim() == 2, "h must be (M, C) fp32"
+    assert cell.dtype == torch.int32 and cell.shape == (h.shape[0],) and cell.is_contiguous(), "cell must be (M,) int32"
+    assert cell.device == h.device and int(n_cells) >= 0
     h = h.contiguous()
     m, c = h.shape
     canvas = torch.empty((n_cells, c), dtype=torch.float32, device=h.device)
@@ -177,6 +183,12 @@ def pillar_scatter_max(h, cell, n_cells, want_argmax=True):
 
 
 def pillar_scatter_max_bwd(gcanvas, arg, cell, m):
+    """gh (m,C) fp32: gh[r, c] = gcanvas[cell[r], c] where arg[cell[r], c] == r, else 0.  gcanvas may have any strides."""
+    _need_cuda(gcanvas, arg, cell)
+    assert gcanvas.dtype == torch.float32 and gcanvas.dim() == 2, "gcanvas must be (n_cells, C) fp32"
+    assert arg.dtype == torch.int32 and arg.shape == gcanvas.shape and arg.is_contiguous(), "arg must be (n_cells, C) int32"
+    assert cell.dtype == torch.int32 and cell.shape == (m,) and cell.is_contiguous(), "cell must be (m,) int32"
+    assert gcanvas.device == arg.device == cell.device
     gcanvas = gcanvas.contiguous()
     c = gcanvas.shape[-1]
     gh = torch.empty((m, c), dtype=torch.float32, device=gcanvas.device)

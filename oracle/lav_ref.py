@@ -226,7 +226,7 @@ def pillar_net(sd, lidar_list, num_points, prefix="point_pillar_net.", min_x=-10
     canvas = torch.zeros(B, fmax.shape[1], ny, nx, dtype=fmax.dtype)
     canvas[uniq[:, 0], :, torch.clamp(ny - 1 - uniq[:, 1], 0, ny - 1), torch.clamp(uniq[:, 2], 0, nx - 1)] = fmax
     if return_aux:
-        return canvas, dict(decorated=feat, coords=coords, uniq=uniq, inv=inv, points=pts)
+        return canvas, dict(decorated=feat, coords=coords, uniq=uniq, inv=inv, points=pts, point_feats=h)
     return canvas
 
 
