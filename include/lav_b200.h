@@ -107,6 +107,39 @@ int lavb_stack_jobs(const void* d_jobs, int n_jobs, int max_n, int src_cols, int
  * The output is bit-identical to OpenCV's fixed-point 8-bit warp chain; every output byte is 0 or 1. */
 int lavb_bev_targets(const void* d_jobs, int n_jobs, const uint8_t* d_src, uint8_t* d_out, int h, int w, void* stream);
 
+/* ---------------------------------------------------------------- LiDAR rows of a training batch
+ * replaces: one GpuLidarStacker call per sample (lav_b200/data_pipeline.py; TemporalLiDARPaintedDataset.__getitem__,
+ *           temporal_lidar_painted_dataset.py:13-91): roof filter, rotate_lidar(-angle), the camera-FOV re-mask of the painted
+ *           columns, move_lidar_points + time one-hot, shuffle, truncation to max_lidar_points and zero padding.
+ * d_raw: n_raw rows of 4 + c floats [x y z r | painted c], every sweep of the batch; sweep s owns rows [row0(s), row0(s+1)).
+ * d_rows: DEVICE int32[n_rows], one entry per output row: the raw row it copies, or -1 for a zero row.  The host does the roof
+ *   filter (the fp32 predicate of lavb_roof_filter), the per-sample permutation, the truncation and the padding on these
+ *   indices, so output row b*P + i of sample b (P rows per sample) is kept row perm_b[i] of the sample's sweeps taken newest
+ *   first, each in its recorded order — the row order of GpuLidarStacker for the same permutation.
+ * d_sweeps: DEVICE array of n_sweeps 88-byte records, sorted by row0,
+ *   { float R_aug[9]; float R_mv[9]; float dx, dy; int time_idx; int row0; }
+ *   (3x3 row-major matrices).  Each output row = [xyz' @ R_mv + (dx, dy, 0) | r | painted * vis | one_hot(time_idx, n_time)] with
+ *   xyz' = xyz @ R_aug + (0, 0, 0) (a real fp32 add: -0 becomes +0) and vis = 1 if lavb_paint's projection through the ncam
+ *   cameras of h_cams (host, as lavb_paint) lands inside an h x w image, else 0, multiplied in as one fp32 multiply (NaN * 0 stays
+ *   NaN).  Bit-identical to lavb_roof_filter + lavb_stack_sweep + lavb_paint (mode 0, a ones map) + multiply + lavb_stack_sweep.
+ *   A row index outside [0, n_raw) or below the first row0 gives a zero row.
+ * d_out: n_rows x (4 + c + n_time) fp32, every element written.  4 + c + n_time <= 16, ncam 1..4. */
+int lavb_lidar_batch(const float* d_raw, long long n_raw, int c, const int* d_rows, long long n_rows, const void* d_sweeps,
+                     int n_sweeps, const float* h_cams, int ncam, int h, int w, int n_time, float* d_out, void* stream);
+
+/* ---------------------------------------------------------------- detection targets of a training batch
+ * replaces: LiDARDataset.detections_to_heatmap (lav/utils/datasets/lidar_dataset.py:92-127), once per sample.
+ * d_actors: DEVICE array of 24-byte records { float x, y, ori, bx, by, typ; } (ego-frame metres, radians, box extents, class:
+ *   0 pedestrian, 1 vehicle, anything else ignored); sample i owns records [d_offsets[i], d_offsets[i+1]) (DEVICE int32[b+1]).
+ * Output planes (b, 2, h, w) fp32 each, every element written: d_heat = per class the maximum over its actors of
+ *   exp(-((x - cx) / r)^2) * exp(-((y - cy) / r)^2), cx = -x * ppm + cx0, cy = (-y * ppm + cy0) + cy1, the division done as a
+ *   multiply by inv_radius; ties go to the first actor, a NaN wins.  Where class 0's value is > 0, and then where class 1's
+ *   value is > class 0's (or > 0 without pedestrians), d_size = (bx, by) * ppm and d_ori = (cos, sin)(ori) of that winning
+ *   actor; elsewhere 0.  A class without actors leaves its heat plane 0.  Every operation is the fp32 operation torch performs
+ *   in lav_b200.data_pipeline.detections_to_heatmap, in its order.  b <= 65535. */
+int lavb_det_heatmaps(const void* d_actors, const int* d_offsets, int b, int h, int w, float ppm, float cx0, float cy0, float cy1,
+                      float inv_radius, float* d_heat, float* d_size, float* d_ori, void* stream);
+
 /* ---------------------------------------------------------------- PointPillars voxeliser + pillar encoder
  * replaces: PointPillarNet.forward (lav/models/point_pillar.py:92-116) incl. grid_locations :70-79,
  *           pillar_generation/decorate :55-68,81-85, DynamicPointNet.forward :28-35 (torch_scatter

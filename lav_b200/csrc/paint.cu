@@ -35,6 +35,34 @@ __device__ __forceinline__ long long trunc_i64(float v) {
   return (long long)v;  // cvt.rzi
 }
 
+// The camera that sees (x, y, z): the last of cams.ncam whose truncated projection (u, v) lies inside the W x H image, or -1;
+// (hit_u, hit_v) = its pixel.  The one projection every painting kernel uses, so their visibility decisions agree bit for bit.
+__device__ __forceinline__ int project_hit(const CamSet& cams, float x, float y, float z, int H, int W, int& hit_u, int& hit_v) {
+  int hit_cam = -1;
+#pragma unroll 1
+  for (int c = 0; c < cams.ncam; ++c) {
+    const float* K = cams.m[c];
+    const float* L = cams.m[c] + 9;
+    const float* Wc = cams.m[c] + 25;
+    // world = lidar_to_world @ [x,y,z,1]
+    const float w0 = dot4(L + 0, x, y, z, 1.f), w1 = dot4(L + 4, x, y, z, 1.f), w2 = dot4(L + 8, x, y, z, 1.f),
+                w3 = dot4(L + 12, x, y, z, 1.f);
+    // cam = world_to_cam @ world ; re-axis (cam_y, -cam_z, cam_x)
+    const float c0 = dot4(Wc + 0, w0, w1, w2, w3), c1 = dot4(Wc + 4, w0, w1, w2, w3), c2 = dot4(Wc + 8, w0, w1, w2, w3);
+    const float a0 = c1, a1 = -c2, a2 = c0;
+    // cam_2d = K @ cam
+    const float q0 = dot3(K + 0, a0, a1, a2), q1 = dot3(K + 3, a0, a1, a2), q2 = dot3(K + 6, a0, a1, a2);
+    const float den = __fadd_rn(1e-5f, q2);
+    const long long u = trunc_i64(__fdiv_rn(q0, den));
+    const long long v = trunc_i64(__fdiv_rn(q1, den));
+    const long long zi = trunc_i64(q2);
+    if (zi >= 0 && u >= 0 && u < W && v >= 0 && v < H) {
+      hit_cam = c; hit_u = (int)u; hit_v = (int)v;
+    }
+  }
+  return hit_cam;
+}
+
 template <int MODE>
 __global__ void __launch_bounds__(256) paint_kernel(const float* __restrict__ pts, int n, int pt_stride,
                                                     const float* __restrict__ sem, int c_in, int H, int W,
@@ -59,28 +87,8 @@ __global__ void __launch_bounds__(256) paint_kernel(const float* __restrict__ pt
   } else {
     x = __ldg(p); y = __ldg(p + 1); z = __ldg(p + 2);
   }
-  int hit_cam = -1, hit_u = 0, hit_v = 0;
-#pragma unroll 1
-  for (int c = 0; c < cams.ncam; ++c) {
-    const float* K = cams.m[c];
-    const float* L = cams.m[c] + 9;
-    const float* Wc = cams.m[c] + 25;
-    // world = lidar_to_world @ [x,y,z,1]
-    const float w0 = dot4(L + 0, x, y, z, 1.f), w1 = dot4(L + 4, x, y, z, 1.f), w2 = dot4(L + 8, x, y, z, 1.f),
-                w3 = dot4(L + 12, x, y, z, 1.f);
-    // cam = world_to_cam @ world ; re-axis (cam_y, -cam_z, cam_x)
-    const float c0 = dot4(Wc + 0, w0, w1, w2, w3), c1 = dot4(Wc + 4, w0, w1, w2, w3), c2 = dot4(Wc + 8, w0, w1, w2, w3);
-    const float a0 = c1, a1 = -c2, a2 = c0;
-    // cam_2d = K @ cam
-    const float q0 = dot3(K + 0, a0, a1, a2), q1 = dot3(K + 3, a0, a1, a2), q2 = dot3(K + 6, a0, a1, a2);
-    const float den = __fadd_rn(1e-5f, q2);
-    const long long u = trunc_i64(__fdiv_rn(q0, den));
-    const long long v = trunc_i64(__fdiv_rn(q1, den));
-    const long long zi = trunc_i64(q2);
-    if (zi >= 0 && u >= 0 && u < W && v >= 0 && v < H) {
-      hit_cam = c; hit_u = (int)u; hit_v = (int)v;
-    }
-  }
+  int hit_u = 0, hit_v = 0;
+  const int hit_cam = project_hit(cams, x, y, z, H, W, hit_u, hit_v);
   float* o = out + (size_t)i * out_stride;
   if (copy_cols == 4 && vec && out_col0 >= 4 && (out_stride % 4) == 0) {
     *reinterpret_cast<float4*>(o) = p4;
@@ -118,6 +126,15 @@ __global__ void __launch_bounds__(256) paint_kernel(const float* __restrict__ pt
 
 struct StackParams { float R[9]; float dx, dy; };
 
+// [x y z] @ R (row vector times the row-major 3x3 R, k-sequential _rn FMAs), then x += dx, y += dy: lav_agent_fast.py:555-563.
+// The adds are real fp32 adds even when dx = dy = 0 (-0 + 0 = +0), as in the reference's rotate-then-translate.
+__device__ __forceinline__ void move_point(const float* R, float dx, float dy, float x, float y, float z, float& nx, float& ny,
+                                           float& nz) {
+  nx = __fadd_rn(__fmaf_rn(z, R[6], __fmaf_rn(y, R[3], __fmul_rn(x, R[0]))), dx);
+  ny = __fadd_rn(__fmaf_rn(z, R[7], __fmaf_rn(y, R[4], __fmul_rn(x, R[1]))), dy);
+  nz = __fmaf_rn(z, R[8], __fmaf_rn(y, R[5], __fmul_rn(x, R[2])));
+}
+
 __global__ void __launch_bounds__(256) stack_kernel(const float* __restrict__ src, int n, int src_cols,
                                                     const __grid_constant__ StackParams P, int time_idx, int n_time,
                                                     int roof_filter, float* __restrict__ dst) {
@@ -127,12 +144,8 @@ __global__ void __launch_bounds__(256) stack_kernel(const float* __restrict__ sr
   const int dcols = src_cols + n_time;
   float* d = dst + (size_t)i * dcols;
   const float x = __ldg(s), y = __ldg(s + 1), z = __ldg(s + 2);
-  // lidar @ R  (row vector times matrix, k-sequential), then += dloc: lav_agent_fast.py:555-563
-  float nx = __fmaf_rn(z, P.R[6], __fmaf_rn(y, P.R[3], __fmul_rn(x, P.R[0])));
-  float ny = __fmaf_rn(z, P.R[7], __fmaf_rn(y, P.R[4], __fmul_rn(x, P.R[1])));
-  float nz = __fmaf_rn(z, P.R[8], __fmaf_rn(y, P.R[5], __fmul_rn(x, P.R[2])));
-  nx = __fadd_rn(nx, P.dx);
-  ny = __fadd_rn(ny, P.dy);
+  float nx, ny, nz;
+  move_point(P.R, P.dx, P.dy, x, y, z, nx, ny, nz);
   if (roof_filter) {  // LAVAgent.preprocess, lav_agent.py:450 — on the sensor-frame coordinates
     if (x > -2.4f && x < 0.f && y > -0.8f && y < 0.8f && z > -1.5f && z < -1.f) nx = __int_as_float(0x7fc00000);
   }
@@ -277,23 +290,8 @@ __global__ void __launch_bounds__(256) paint_deconv_kernel(const float* __restri
   const bool vec = (pt_stride == 4);
   if (vec) { p4 = __ldg(reinterpret_cast<const float4*>(p)); x = p4.x; y = p4.y; z = p4.z; }
   else { x = __ldg(p); y = __ldg(p + 1); z = __ldg(p + 2); }
-  int hit_cam = -1, hit_u = 0, hit_v = 0;
-#pragma unroll 1
-  for (int c = 0; c < cams.ncam; ++c) {       // identical projection arithmetic to paint_kernel
-    const float* K = cams.m[c];
-    const float* L = cams.m[c] + 9;
-    const float* Wc = cams.m[c] + 25;
-    const float w0 = dot4(L + 0, x, y, z, 1.f), w1 = dot4(L + 4, x, y, z, 1.f), w2 = dot4(L + 8, x, y, z, 1.f),
-                w3 = dot4(L + 12, x, y, z, 1.f);
-    const float c0 = dot4(Wc + 0, w0, w1, w2, w3), c1 = dot4(Wc + 4, w0, w1, w2, w3), c2 = dot4(Wc + 8, w0, w1, w2, w3);
-    const float a0 = c1, a1 = -c2, a2 = c0;
-    const float q0 = dot3(K + 0, a0, a1, a2), q1 = dot3(K + 3, a0, a1, a2), q2 = dot3(K + 6, a0, a1, a2);
-    const float den = __fadd_rn(1e-5f, q2);
-    const long long u = trunc_i64(__fdiv_rn(q0, den));
-    const long long v = trunc_i64(__fdiv_rn(q1, den));
-    const long long zi = trunc_i64(q2);
-    if (zi >= 0 && u >= 0 && u < W && v >= 0 && v < H) { hit_cam = c; hit_u = (int)u; hit_v = (int)v; }
-  }
+  int hit_u = 0, hit_v = 0;
+  const int hit_cam = project_hit(cams, x, y, z, H, W, hit_u, hit_v);
   float* o = out + (size_t)i * out_stride;
   if (copy_cols == 4 && vec && out_col0 >= 4 && (out_stride % 4) == 0) *reinterpret_cast<float4*>(o) = p4;
   else for (int k = 0; k < copy_cols; ++k) o[k] = __ldg(p + k);
@@ -386,11 +384,8 @@ __global__ void __launch_bounds__(256) stack_jobs_kernel(const StackJob* __restr
         x = __ldg(s); y = __ldg(s + 1); z = __ldg(s + 2);
         for (int k = 3; k < src_cols; ++k) d[k] = __ldg(s + k);
       }
-      float nx = __fmaf_rn(z, j.R[6], __fmaf_rn(y, j.R[3], __fmul_rn(x, j.R[0])));
-      float ny = __fmaf_rn(z, j.R[7], __fmaf_rn(y, j.R[4], __fmul_rn(x, j.R[1])));
-      const float nz = __fmaf_rn(z, j.R[8], __fmaf_rn(y, j.R[5], __fmul_rn(x, j.R[2])));
-      nx = __fadd_rn(nx, j.dx);
-      ny = __fadd_rn(ny, j.dy);
+      float nx, ny, nz;
+      move_point(j.R, j.dx, j.dy, x, y, z, nx, ny, nz);
       if (roof_filter && x > -2.4f && x < 0.f && y > -0.8f && y < 0.8f && z > -1.5f && z < -1.f) nx = __int_as_float(0x7fc00000);
       d[0] = nx; d[1] = ny; d[2] = nz;
       for (int k = 0; k < n_time; ++k) d[src_cols + k] = (k == j.time_idx) ? 1.f : 0.f;
@@ -409,6 +404,77 @@ extern "C" int lavb_stack_jobs(const void* d_jobs, int n_jobs, int max_n, int sr
   if (n_jobs == 0 || max_n == 0) return 0;
   dim3 grid(min(ceil_div(max_n, 256), 64), n_jobs);
   stack_jobs_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(reinterpret_cast<const StackJob*>(d_jobs), src_cols, n_time, roof_filter);
+  LAVB_LAUNCH_OK();
+  return 0;
+}
+
+// ---- the LiDAR rows of a whole training batch in one launch: GpuLidarStacker (data_pipeline.py) for every sample at once.
+// The host has already applied the roof filter, the shuffle, the truncation and the zero padding to row INDICES (rows[r] = raw
+// row of output row r, or -1); this kernel gathers and restates the stacker's per-row arithmetic: stack_sweep with R_aug and a
+// zero shift, paint (mode 0) on a ones map, the in-place multiply of the painted columns by that 0/1, stack_sweep with R_mv.
+struct LidarSweep {          // 88 bytes
+  float R_aug[9]; float R_mv[9]; float dx, dy; int time_idx; int row0;
+};
+static_assert(sizeof(LidarSweep) == 88, "LidarSweep layout is part of the ABI (lav_b200.h)");
+
+__global__ void __launch_bounds__(256) lidar_batch_kernel(const float* __restrict__ raw, long long n_raw, int src_cols,
+                                                          const int* __restrict__ rows, long long n_rows,
+                                                          const LidarSweep* __restrict__ sweeps, int n_sweeps,
+                                                          const __grid_constant__ CamSet cams, int H, int W, int n_time,
+                                                          float* __restrict__ out) {
+  __shared__ float tile[256 * kStackMaxCols];
+  const int dcols = src_cols + n_time;
+  const long long r0 = (long long)blockIdx.x * 256, r = r0 + threadIdx.x;
+  if (r < n_rows) {
+    float* d = tile + threadIdx.x * dcols;
+    const int src = __ldg(rows + r);
+    int s = -1;
+    if (src >= 0 && src < n_raw) {   // the sweep holding raw row src: the last one with row0 <= src
+      int lo = 0, hi = n_sweeps;
+      while (lo < hi) {
+        const int mid = (lo + hi) >> 1;
+        if (__ldg(&sweeps[mid].row0) <= src) lo = mid + 1; else hi = mid;
+      }
+      s = lo - 1;
+    }
+    if (s < 0) {
+      for (int k = 0; k < dcols; ++k) d[k] = 0.f;
+    } else {
+      const LidarSweep& sw = sweeps[s];
+      const float* p = raw + (size_t)src * src_cols;
+      float ax, ay, az;
+      move_point(sw.R_aug, 0.f, 0.f, __ldg(p), __ldg(p + 1), __ldg(p + 2), ax, ay, az);
+      int u = 0, v = 0;
+      const float vis = project_hit(cams, ax, ay, az, H, W, u, v) >= 0 ? 1.f : 0.f;
+      move_point(sw.R_mv, sw.dx, sw.dy, ax, ay, az, d[0], d[1], d[2]);
+      d[3] = __ldg(p + 3);
+      for (int k = 4; k < src_cols; ++k) d[k] = __fmul_rn(__ldg(p + k), vis);   // NaN * 0 stays NaN, -x * 0 = -0, as in torch
+      for (int k = 0; k < n_time; ++k) d[src_cols + k] = (k == sw.time_idx) ? 1.f : 0.f;
+    }
+  }
+  __syncthreads();
+  const int nrow = (int)min(256LL, n_rows - r0);
+  float* o = out + r0 * dcols;
+  for (int e = threadIdx.x; e < nrow * dcols; e += 256) o[e] = tile[e];
+}
+
+extern "C" int lavb_lidar_batch(const float* d_raw, long long n_raw, int c, const int* d_rows, long long n_rows,
+                                const void* d_sweeps, int n_sweeps, const float* h_cams, int ncam, int h, int w, int n_time,
+                                float* d_out, void* stream) {
+  LAVB_CHECK_ARG(n_raw >= 0 && n_raw <= 0x7fffffffLL && n_rows >= 0 && n_sweeps >= 0 && c >= 0 && n_time >= 0,
+                 "lidar_batch: bad sizes (n_raw %lld, n_rows %lld, n_sweeps %d, c %d, n_time %d)", n_raw, n_rows, n_sweeps, c,
+                 n_time);
+  LAVB_CHECK_ARG(4 + c + n_time <= kStackMaxCols, "lidar_batch: rows wider than %d floats", kStackMaxCols);
+  LAVB_CHECK_ARG(h_cams != nullptr && ncam >= 1 && ncam <= 4 && h > 0 && w > 0, "lidar_batch: bad cameras (ncam %d, %d x %d)",
+                 ncam, h, w);
+  LAVB_CHECK_ARG(n_rows == 0 || (d_rows != nullptr && d_out != nullptr), "lidar_batch: null row table or output");
+  LAVB_CHECK_ARG(n_raw == 0 || (d_raw != nullptr && d_sweeps != nullptr && n_sweeps > 0), "lidar_batch: null raw rows or sweeps");
+  if (n_rows == 0) return 0;
+  CamSet cs;
+  memcpy(cs.m, h_cams, sizeof(float) * 41 * ncam);
+  cs.ncam = ncam;
+  lidar_batch_kernel<<<(unsigned)((n_rows + 255) / 256), 256, 0, (cudaStream_t)stream>>>(
+      d_raw, n_raw, 4 + c, d_rows, n_rows, reinterpret_cast<const LidarSweep*>(d_sweeps), n_sweeps, cs, h, w, n_time, d_out);
   LAVB_LAUNCH_OK();
   return 0;
 }

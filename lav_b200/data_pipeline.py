@@ -12,6 +12,10 @@ touches the points runs on the GPU with the frame path's own kernels:
     ego-motion + jitter + time one-hot     move_lidar_points, :159-177 / :62-66,80-87                lavb_stack_sweep
     shuffle, truncate to max_lidar_points, zero-pad  :89-91,131-133                                  torch.randperm + copies
     heat / size / orientation maps         detections_to_heatmap                                    vectorised torch on the device
+A training batch takes the batched path instead: GpuLidarStacker.batch_tables does the roof filter, the shuffle, the truncation
+and the padding on row indices on the host, and one lavb_lidar_batch launch builds every LiDAR row of the batch; one
+lavb_det_heatmaps launch builds every sample's maps.  Both are bit-identical to the per-sample path above, which stays as their
+reference.
 Not here (host, as in the reference): LMDB reads, the actor filter, BEV image loading and its cv2 rotation.
 """
 import math
@@ -28,7 +32,7 @@ class GpuLidarStacker:
 
     def __init__(self, num_frame_stack=2, seg_channels=4, max_lidar_points=120000, camera_x=1.5, camera_z=2.4, rgb_hw=(288, 256),
                  device=torch.device("cuda")):
-        self.T, self.C, self.max_points, self.device = num_frame_stack + 1, seg_channels, max_lidar_points, device
+        self.T, self.C, self.max_points, self.device, self.rgb_hw = num_frame_stack + 1, seg_channels, max_lidar_points, device, rgb_hw
         self.cams = np.stack([c.packed() for c in PP.make_converters(camera_x, camera_z, rgb_hw[0], rgb_hw[1])])
         self.ones = torch.ones((len(self.cams), 1, rgb_hw[0], rgb_hw[1]), device=device)       # `self.dummy` of the reference
 
@@ -38,9 +42,7 @@ class GpuLidarStacker:
         angle_deg: the sample's rotation jitter; jitters[i] = (loc_jitter (2,), ori_jitter) of sweep i (zeros for i = 0).
         Returns (lidar (max_points, 4+C+T) fp32 zero-padded, num_points)."""
         dev = self.device
-        loc0, ori0 = np.asarray(sweeps[0][2], dtype=np.float64), float(sweeps[0][3])
-        rad = math.radians(-angle_deg)
-        R_aug = np.array([[math.cos(rad), math.sin(rad), 0], [-math.sin(rad), math.cos(rad), 0], [0, 0, 1]], dtype=np.float32)
+        R_aug, moves = sweep_transforms(sweeps, angle_deg, jitters)
         rows = []
         for i, (xyzr, painted, loc, ori) in enumerate(sweeps):
             raw = torch.cat([torch.as_tensor(xyzr, dtype=torch.float32), torch.as_tensor(painted, dtype=torch.float32)], 1).to(dev).contiguous()
@@ -51,10 +53,7 @@ class GpuLidarStacker:
             ops.stack_sweep(kept, R_aug, 0.0, 0.0, 0, 0, rot)                                # rotate_lidar(xyzr, -angle)
             vis = ops.paint(rot, self.ones, self.cams, mode=0)                               # 1 where some camera still sees the point
             rot[:, 4:] *= vis
-            lj, oj = (np.zeros(2), 0.0) if (jitters is None or i == 0) else jitters[i]
-            dloc = (np.asarray(loc, dtype=np.float64) - loc0 + np.asarray(lj)) @ np.array([[math.cos(ori0), -math.sin(ori0)], [math.sin(ori0), math.cos(ori0)]])
-            d = float(ori) + float(oj) - ori0
-            R_mv = np.array([[math.cos(d), math.sin(d), 0], [-math.sin(d), math.cos(d), 0], [0, 0, 1]], dtype=np.float32)
+            R_mv, dloc = moves[i]
             out = torch.empty((n, 4 + self.C + self.T), device=dev)
             ops.stack_sweep(rot, R_mv, dloc[0], dloc[1], i, self.T, out)                     # move_lidar_points + one-hot(t)
             rows.append(out)
@@ -66,6 +65,76 @@ class GpuLidarStacker:
         num = min(self.max_points, total)
         padded[:num] = lidar[:num]
         return padded, num
+
+    def batch_tables(self, samples, generator=None):
+        """The host half of a batch: samples = [(sweeps, angle_deg, jitters)] as __call__ takes them, sweeps numpy.  Draws each
+        sample's permutation from ``generator`` (a CPU torch.Generator; None = torch's default CPU generator) with the sizes and in
+        the order of one __call__ per sample, and composes it with the kept rows of the roof filter.  No device work.
+        -> dict(raw (N, 4+C) fp32, rows (B, P) int32, sweeps LIDAR_SWEEP_DTYPE records, nums list): raw and rows are pinned
+        CPU tensors when the stacker's device is CUDA."""
+        pin = torch.device(self.device).type == "cuda"
+        n_raw = sum(len(sw[0]) for sweeps, _, _ in samples for sw in sweeps)
+        raw = torch.empty((n_raw, 4 + self.C), dtype=torch.float32, pin_memory=pin)
+        rows = torch.full((len(samples), self.max_points), -1, dtype=torch.int32, pin_memory=pin)
+        a, r = raw.numpy(), rows.numpy()
+        table = np.zeros(sum(len(sweeps) for sweeps, _, _ in samples), ops.LIDAR_SWEEP_DTYPE)
+        r0, s, nums = 0, 0, []
+        for b, (sweeps, angle_deg, jitters) in enumerate(samples):
+            R_aug, moves = sweep_transforms(sweeps, angle_deg, jitters)
+            kept = []
+            for i, (xyzr, painted, _, _) in enumerate(sweeps):
+                n = len(xyzr)
+                a[r0:r0 + n, :4], a[r0:r0 + n, 4:] = xyzr, painted
+                kept.append(r0 + np.flatnonzero(roof_keep(a[r0:r0 + n])))
+                R_mv, dloc = moves[i]
+                table[s] = (R_aug.ravel(), R_mv.ravel(), dloc[0], dloc[1], i, r0)
+                r0, s = r0 + n, s + 1
+            kept = np.concatenate(kept)
+            perm = torch.randperm(len(kept), generator=generator, device="cpu").numpy()
+            num = min(self.max_points, len(kept))
+            r[b, :num] = kept[perm[:num]]
+            nums.append(num)
+        return dict(raw=raw, rows=rows, sweeps=table, nums=nums)
+
+    @torch.no_grad()
+    def batch_launch(self, t):
+        """The device half: H2D copies of the tables and one lavb_lidar_batch launch -> (B, P, 4+C+T) fp32."""
+        dev = self.device
+        raw, rows = t["raw"].to(dev, non_blocking=True), t["rows"].to(dev, non_blocking=True)
+        sweeps = ops._to_device(t["sweeps"].view(np.uint8), dev)
+        return ops.lidar_batch(raw, rows, sweeps, self.cams, self.rgb_hw, self.T)
+
+    def batch(self, samples, generator=None):
+        """__call__ for every sample of a batch, in one launch: -> (lidar (B, P, 4+C+T) fp32, nums list), bit-identical to
+        stacking one __call__ per sample in order with the same generator."""
+        t = self.batch_tables(samples, generator)
+        return self.batch_launch(t), t["nums"]
+
+
+def sweep_transforms(sweeps, angle_deg, jitters):
+    """GpuLidarStacker's per-sample rotation R_aug (rotate_lidar(-angle)) and per-sweep (R_mv, dloc) (move_lidar_points to the
+    newest sweep's ego frame, with the stack jitters): 3x3 fp32 matrices, dloc (2,) fp64."""
+    loc0, ori0 = np.asarray(sweeps[0][2], dtype=np.float64), float(sweeps[0][3])
+    rad = math.radians(-angle_deg)
+    R_aug = np.array([[math.cos(rad), math.sin(rad), 0], [-math.sin(rad), math.cos(rad), 0], [0, 0, 1]], dtype=np.float32)
+    moves = []
+    for i, (_, _, loc, ori) in enumerate(sweeps):
+        lj, oj = (np.zeros(2), 0.0) if (jitters is None or i == 0) else jitters[i]
+        dloc = (np.asarray(loc, dtype=np.float64) - loc0 + np.asarray(lj)) @ np.array([[math.cos(ori0), -math.sin(ori0)], [math.sin(ori0), math.cos(ori0)]])
+        d = float(ori) + float(oj) - ori0
+        R_mv = np.array([[math.cos(d), math.sin(d), 0], [-math.sin(d), math.cos(d), 0], [0, 0, 1]], dtype=np.float32)
+        moves.append((R_mv, dloc))
+    return R_aug, moves
+
+
+_ROOF = tuple(np.float32(v) for v in (-2.4, 0, -0.8, 0.8, -1.5, -1))
+
+
+def roof_keep(rows):
+    """LAVAgent.preprocess's keep mask on (n, >=3) fp32 rows: lavb_roof_filter's fp32 predicate (NaN rows are kept)."""
+    x, y, z = rows[:, 0], rows[:, 1], rows[:, 2]
+    x0, x1, y0, y1, z0, z1 = _ROOF
+    return ~((x > x0) & (x < x1) & (y > y0) & (y < y1) & (z > z0) & (z < z1))
 
 
 @torch.no_grad()

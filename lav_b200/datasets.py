@@ -8,8 +8,10 @@ environment per trajectory directory (LMDB when the `lmdb` package imports and d
 What runs where:
     record reads, PNG decode (cv2, else torchvision)              host, a background thread of the loader
     actor filter, ego transform, label padding (a few hundred floats)   host, vectorised numpy
-    LiDAR: roof filter, rotation, FOV re-mask, stacking, shuffle   device, data_pipeline.GpuLidarStacker
-    heat / size / orientation maps                                 device, data_pipeline.detections_to_heatmap
+    LiDAR: roof filter, rotation, FOV re-mask, stacking, shuffle   device, data_pipeline.GpuLidarStacker (per sample), or for a
+                                                                   batch its index tables on the host and one ops.lidar_batch
+    heat / size / orientation maps                                 device, data_pipeline.detections_to_heatmap (per sample), or
+                                                                   one ops.det_heatmaps launch per batch
     the 9-plane temporal BEV target (2 warpAffine per plane)       device, ops.bev_targets: one launch per batch, bit-identical
                                                                    to the reference's OpenCV chain
 """
@@ -119,7 +121,7 @@ class TemporalLiDARPaintedDataset:
         self.device = torch.device(device)
         self.margin = ops.BEV_MARGIN
         self.paths, self.index = index_trajectories(self.data_dir, self.percentage_data, self.all_towns, self.num_plan, seed)
-        self._envs = {}
+        self._envs, self._env_lock = {}, threading.Lock()
         self.stacker = GpuLidarStacker(self.num_frame_stack, len(self.seg_channels), self.max_lidar_points, self.camera_x,
                                        self.camera_z, device=self.device)
         self.rng = np.random.RandomState(seed)
@@ -129,9 +131,10 @@ class TemporalLiDARPaintedDataset:
         return len(self.index)
 
     def env(self, traj):
-        if traj not in self._envs:
-            self._envs[traj] = data_paint.open_env(self.paths[traj])
-        return self._envs[traj]
+        with self._env_lock:                        # the loaders' threads share it: open each environment once per process
+            if traj not in self._envs:
+                self._envs[traj] = data_paint.open_env(self.paths[traj])
+            return self._envs[traj]
 
     def draw(self, rng):
         """(angle in degrees, stack jitters) with the reference's distributions (temporal_lidar_painted_dataset.py:21,50-51)."""
@@ -191,14 +194,10 @@ class TemporalLiDARPaintedDataset:
     def bev_batch(self, hs, planes=None):
         """one bev_targets launch for the samples ``hs`` -> (len(hs), 9, 320, 320) uint8 on the device."""
         n_bev = 3 + 2 * (self.num_frame_stack + 1)
-        rows, base = [], 0
-        for b, h in enumerate(hs):
-            rows += [(s + base if s >= 0 else -1, b * n_bev + d, a1, a2, dx, dy) for s, d, a1, a2, dx, dy in h["rows"]]
-            base += len(h["planes"])
         if planes is None:
             planes = torch.from_numpy(np.concatenate([h["planes"] for h in hs])).to(self.device)
         out = torch.empty((len(hs), n_bev, BEV_SIZE, BEV_SIZE), dtype=torch.uint8, device=self.device)
-        return ops.bev_targets(planes, ops.bev_jobs(rows), out)
+        return ops.bev_targets(planes, bev_job_table(hs, n_bev), out)
 
     def sample(self, idx, angle, jitters, generator=None):
         """the 14-tuple of sample ``idx`` for the given draws: angle (degrees), jitters[i] = (loc (2,), ori) of stacked frame i
@@ -215,19 +214,74 @@ class TemporalLiDARPaintedDataset:
         angle, jit = self.draw(self.rng)
         return self.sample(idx, angle, jit, self.gen)
 
+    # ---- a whole batch: host tables (any thread), then a fixed number of launches and H2D copies (the caller's thread)
+    def stage_batch(self, hs, generator=None):
+        """the host tables of a batch of prepared samples ``hs``, in pinned memory on a CUDA dataset.  Draws the LiDAR
+        shuffles from ``generator`` (CPU) in sample order, as one sample() per entry of ``hs`` would."""
+        pin = self.device.type == "cuda"
+        pinned = lambda a: torch.from_numpy(np.ascontiguousarray(a)).pin_memory() if pin else torch.from_numpy(np.ascontiguousarray(a))
+        lidar = self.stacker.batch_tables([(h["sweeps"], h["angle"], h["jitters"]) for h in hs], generator)
+        dets = [np.column_stack([np.reshape(locs, (-1, 2)), oris, np.reshape(bbox, (-1, 2)), typs]) for locs, oris, bbox, typs in
+                (h["det"] for h in hs)]
+        offsets = np.concatenate([[0], np.cumsum([len(d) for d in dets])]).astype(np.int32)
+        f32 = lambda key: np.stack([h[key] for h in hs]).astype(np.float32)
+        labels = dict(ego_locs=f32("ego_locs"), nxp=f32("nxp"), locs=f32("locs"), oris=f32("oris"),
+                      typs=np.stack([h["typs"] for h in hs]).astype(np.int32),
+                      cmd=np.array([h["cmd"] for h in hs], np.int64), bra=np.array([h["bra"] for h in hs], np.int64))
+        return dict(lidar=lidar, actors=pinned(np.concatenate(dets + [np.zeros((0, 6))]).astype(np.float32)),
+                    offsets=pinned(offsets), planes=pinned(np.concatenate([h["planes"] for h in hs])),
+                    bev_jobs=bev_job_table(hs, 3 + 2 * (self.num_frame_stack + 1)),
+                    labels={k: pinned(v) for k, v in labels.items()}, num_objs=[h["num_objs"] for h in hs])
+
+    @torch.no_grad()
+    def launch_batch(self, st):
+        """the device half of a batch staged by stage_batch: lidar_batch, det_heatmaps and bev_targets, and the H2D copies, with no
+        device-to-host read -> the loader's 14-tuple."""
+        dev = self.device
+        to = lambda t: t.to(dev, non_blocking=True)
+        lidar = self.stacker.batch_launch(st["lidar"])
+        grid = dict(min_x=self.min_x, max_x=self.max_x, min_y=self.min_y, max_y=self.max_y, pixels_per_meter=self.pixels_per_meter)
+        heat, size, orim = ops.det_heatmaps(to(st["actors"]), to(st["offsets"]), grid)
+        bev = torch.empty((len(st["num_objs"]), 3 + 2 * (self.num_frame_stack + 1), BEV_SIZE, BEV_SIZE), dtype=torch.uint8, device=dev)
+        ops.bev_targets(to(st["planes"]), st["bev_jobs"], bev)
+        lab = {k: to(v) for k, v in st["labels"].items()}
+        return (lidar, torch.tensor(st["lidar"]["nums"], dtype=torch.int64), heat, size, orim, bev, lab["ego_locs"], lab["cmd"],
+                lab["nxp"], lab["bra"], lab["locs"], lab["oris"], lab["typs"], torch.tensor(st["num_objs"], dtype=torch.int64))
+
+    def sample_batch(self, idxs, draws, generator=None):
+        """the loader's 14-tuple for the samples ``idxs`` with the draws ``draws[i] = (angle, jitters)``; the LiDAR shuffles come
+        from ``generator`` (CPU) in sample order.  Equal, tensor for tensor, to stacking sample(idxs[i], *draws[i], generator) in
+        order, with the device work in a fixed number of launches."""
+        hs = [self.prepare(int(i), *d) for i, d in zip(idxs, draws)]
+        return self.launch_batch(self.stage_batch(hs, generator))
+
+
+def bev_job_table(hs, n_bev):
+    """BEV_JOB_DTYPE records of the prepared samples ``hs``, their planes concatenated in order, sample b's output planes at
+    b * n_bev + d."""
+    rows, base = [], 0
+    for b, h in enumerate(hs):
+        rows += [(s + base if s >= 0 else -1, b * n_bev + d, a1, a2, dx, dy) for s, d, a1, a2, dx, dy in h["rows"]]
+        base += len(h["planes"])
+    return ops.bev_jobs(rows)
+
 
 class TemporalBatchLoader:
     """Batches of ``dataset`` for LAVTrainer.train_lidar, one rank of ``world``.
 
     Each epoch shuffles the sample list with a permutation seeded by (seed, epoch) — the same on every rank — and rank r takes
-    every world-th entry; every rank yields the same number of batches (len // world // batch_size with drop_last).  While
-    batch k is on the GPU, one background thread reads the records and decodes the PNGs of batch k+1.  A batch is the 14-tuple
+    every world-th entry; every rank yields the same number of batches (len // world // batch_size with drop_last).  The draws
+    of an epoch come from a RandomState (angle and jitters, on the caller's thread) and a torch CPU generator (the LiDAR
+    shuffles), both seeded by (seed, epoch, rank) and taken in sample order.  While batch k is on the GPU, a background thread
+    builds batch k+1 on the host: record reads, PNG decodes and labels on ``num_workers`` threads, then the tables of
+    TemporalLiDARPaintedDataset.stage_batch; the device part is launch_batch.  A batch is the 14-tuple
     lidars (B,P,4+C+T) f32, num_points (B,) int64 (host), heatmaps / sizemaps / orimaps (B,2,320,320) f32, bev (B,9,320,320)
     uint8, ego_locs (B,T+1,2) f32, cmds (B,) int64, nxps (B,2) f32, bras (B,) int64, locs (B,max_objs,T+1,2) f32, oris
     (B,max_objs) f32, typs (B,max_objs) int32, num_objs (B,) int64; train_lidar takes the first 13."""
 
-    def __init__(self, dataset, batch_size, seed=2021, rank=0, world=1, drop_last=True):
+    def __init__(self, dataset, batch_size, seed=2021, rank=0, world=1, drop_last=True, num_workers=8):
         self.ds, self.B, self.seed, self.rank, self.world, self.drop_last = dataset, batch_size, seed, rank, world, drop_last
+        self.num_workers = max(1, int(num_workers))
         self.epoch = 0
 
     def shard(self, epoch):
@@ -238,37 +292,30 @@ class TemporalBatchLoader:
         n = len(self.ds) // self.world
         return n // self.B if self.drop_last else -(-n // self.B)
 
-    def _host(self, idxs, rng):
-        hs = [self.ds.prepare(int(i), *self.ds.draw(rng)) for i in idxs]
-        planes = torch.from_numpy(np.concatenate([h["planes"] for h in hs]))
-        return hs, planes.pin_memory() if self.ds.device.type == "cuda" else planes
+    def generators(self, epoch):
+        """(RandomState of the angle and jitter draws, torch CPU generator of the LiDAR shuffles) of ``epoch`` on this rank."""
+        return (np.random.RandomState([self.seed, epoch, self.rank]),
+                torch.Generator(device="cpu").manual_seed(self.seed * 1000003 + epoch * 1009 + self.rank))
+
+    def _host(self, idxs, draws, gen, pool):
+        hs = list(pool.map(lambda a: self.ds.prepare(int(a[0]), *a[1]), zip(idxs, draws)))
+        return self.ds.stage_batch(hs, gen)
 
     def __iter__(self):
         epoch, self.epoch = self.epoch, self.epoch + 1
         order = self.shard(epoch)
         batches = [order[k * self.B:(k + 1) * self.B] for k in range(len(self))]
-        rng = np.random.RandomState([self.seed, epoch, self.rank])
-        gen = torch.Generator(device="cpu").manual_seed(self.seed * 1000003 + epoch * 1009 + self.rank)
+        rng, gen = self.generators(epoch)
         if not batches:
             return
-        with ThreadPoolExecutor(1) as pool:
-            nxt = pool.submit(self._host, batches[0], rng)
+        draws = lambda idxs: [self.ds.draw(rng) for _ in idxs]                  # on this thread, in sample order
+        with ThreadPoolExecutor(1) as ahead, ThreadPoolExecutor(self.num_workers) as pool:
+            nxt = ahead.submit(self._host, batches[0], draws(batches[0]), gen, pool)
             for k in range(len(batches)):
-                hs, planes = nxt.result()
+                staged = nxt.result()
                 if k + 1 < len(batches):
-                    nxt = pool.submit(self._host, batches[k + 1], rng)
-                yield self._device(hs, planes, gen)
-
-    def _device(self, hs, planes, gen):
-        ds, dev = self.ds, self.ds.device
-        parts = [ds.lidar_and_maps(h, gen) for h in hs]
-        bev = ds.bev_batch(hs, planes.to(dev, non_blocking=True))
-        st = lambda i: torch.stack([p[i] for p in parts])
-        f32 = lambda key: torch.as_tensor(np.stack([h[key] for h in hs]), dtype=torch.float32).to(dev, non_blocking=False)
-        ints = lambda key, dt=torch.int64: torch.tensor([h[key] for h in hs], dtype=dt)
-        return (st(0), torch.tensor([p[1] for p in parts], dtype=torch.int64), st(2), st(3), st(4), bev, f32("ego_locs"),
-                ints("cmd").to(dev), f32("nxp"), ints("bra").to(dev), f32("locs"), f32("oris"),
-                torch.as_tensor(np.stack([h["typs"] for h in hs])).to(dev), ints("num_objs"))
+                    nxt = ahead.submit(self._host, batches[k + 1], draws(batches[k + 1]), gen, pool)
+                yield self.ds.launch_batch(staged)
 
 
 class TemporalBEVDataset:
@@ -295,12 +342,7 @@ class TemporalBEVDataset:
 
     __len__ = TemporalLiDARPaintedDataset.__len__
     bev_batch = TemporalLiDARPaintedDataset.bev_batch
-
-    def env(self, traj):
-        with self._env_lock:                        # the loader's threads share it: open each environment once per process
-            if traj not in self._envs:
-                self._envs[traj] = data_paint.open_env(self.paths[traj])
-            return self._envs[traj]
+    env = TemporalLiDARPaintedDataset.env
 
     def draw(self, gen):
         """(offset in pixels, angle in degrees): int of the fp32 draw clipped to the margin, then the angle — the reference's
@@ -367,10 +409,6 @@ class TemporalBEVBatchLoader(TemporalBatchLoader):
     bras (B,) int64, locs (B,max_objs,T+1,2) f32, oris (B,max_objs) f32, typs (B,max_objs) int32, num_objs (B,) int64 (host),
     with one bev_targets launch per batch."""
 
-    def __init__(self, dataset, batch_size, seed=2021, rank=0, world=1, drop_last=True, num_workers=8):
-        super().__init__(dataset, batch_size, seed, rank, world, drop_last)
-        self.num_workers = max(1, int(num_workers))
-
     def _host_bev(self, idxs, draws, pool):
         hs = list(pool.map(lambda a: self.ds.prepare(int(a[0]), *a[1]), zip(idxs, draws)))
         planes = torch.from_numpy(np.concatenate([h["planes"] for h in hs]))
@@ -403,7 +441,7 @@ class TemporalBEVBatchLoader(TemporalBatchLoader):
 
 def get_data_loader(data_type, args):
     """lav.utils.datasets.get_data_loader for 'temporal_lidar_painted' and 'temporal_bev' (args: config_path, seed, batch_size;
-    optional rank, world_size, device, and num_workers for 'temporal_bev').  The other dataset types are not provided."""
+    optional rank, world_size, device, num_workers).  The other dataset types are not provided."""
     if data_type not in ("temporal_lidar_painted", "temporal_bev"):
         raise NotImplementedError(f"data type {data_type!r}: only 'temporal_lidar_painted' and 'temporal_bev' are provided")
     dev = getattr(args, "device", None) or torch.device("cuda", torch.cuda.current_device())
@@ -412,4 +450,4 @@ def get_data_loader(data_type, args):
         ds = TemporalBEVDataset(args.config_path, seed=args.seed, device=dev)
         return TemporalBEVBatchLoader(ds, args.batch_size, args.seed, rank, world, num_workers=getattr(args, "num_workers", 8))
     ds = TemporalLiDARPaintedDataset(args.config_path, seed=args.seed, device=dev)
-    return TemporalBatchLoader(ds, args.batch_size, args.seed, rank, world)
+    return TemporalBatchLoader(ds, args.batch_size, args.seed, rank, world, num_workers=getattr(args, "num_workers", 8))

@@ -477,10 +477,86 @@ def bev_targets(src_planes, jobs, out=None):
         raise capi.LavbError(f"bev_targets: job plane index out of range ({P} source planes, {n_out} output planes)")
     if len(jobs) == 0:
         return out
-    d_jobs = torch.from_numpy(jobs.view(np.uint8)).to(src_planes.device)
+    d_jobs = _to_device(jobs.view(np.uint8), src_planes.device)
     check(lib().lavb_bev_targets(_ptr(d_jobs), len(jobs), _ptr(src_planes), _ptr(out), h, w, _stream()), "lavb_bev_targets")
     _COUNT[0] += 1
     return out
+
+
+def _to_device(a, device):
+    """host array -> device tensor through pinned staging, without a host synchronisation (the pinned block is not reused
+    before the copy has run: the caching host allocator records the copy's stream)."""
+    return torch.from_numpy(np.ascontiguousarray(a)).pin_memory().to(device, non_blocking=True)
+
+
+# ----------------------------------------------------------------------------- training batches
+LIDAR_SWEEP_DTYPE = np.dtype([("R_aug", np.float32, 9), ("R_mv", np.float32, 9), ("dx", np.float32), ("dy", np.float32),
+                              ("time_idx", np.int32), ("row0", np.int32)])
+assert LIDAR_SWEEP_DTYPE.itemsize == 88
+
+
+def lidar_batch(raw, rows, sweeps, cams, image_hw, n_time, out=None):
+    """The LiDAR input of a training batch in one launch (see lavb_lidar_batch in include/lav_b200.h).  raw (N, 4+C) fp32: every
+    sweep's rows [xyzr | painted]; rows (B, P) int32: the raw row of each output row, -1 for a zero row; sweeps: uint8 CUDA tensor
+    of LIDAR_SWEEP_DTYPE records sorted by row0; cams (ncam, 41) float32 numpy; image_hw = the camera image size.
+    -> (B, P, 4+C+n_time) fp32, bit-identical to GpuLidarStacker on each sample for the same shuffle."""
+    _need_cuda(raw, rows, sweeps)
+    if raw.dtype != torch.float32 or raw.dim() != 2 or not raw.is_contiguous() or raw.shape[1] < 4:
+        raise capi.LavbError(f"lidar_batch: raw must be a contiguous (N, 4+C) fp32 tensor, got {raw.dtype} {tuple(raw.shape)}")
+    if rows.dtype != torch.int32 or rows.dim() != 2 or not rows.is_contiguous():
+        raise capi.LavbError(f"lidar_batch: rows must be a contiguous (B, P) int32 tensor, got {rows.dtype} {tuple(rows.shape)}")
+    if sweeps.dtype != torch.uint8 or not sweeps.is_contiguous() or sweeps.numel() % LIDAR_SWEEP_DTYPE.itemsize:
+        raise capi.LavbError("lidar_batch: sweeps must be a contiguous uint8 tensor of 88-byte LIDAR_SWEEP_DTYPE records")
+    if not raw.device == rows.device == sweeps.device:
+        raise capi.LavbError("lidar_batch: raw, rows and sweeps must be on one device")
+    cams = np.ascontiguousarray(cams, dtype=np.float32)
+    if cams.ndim != 2 or cams.shape[1] != 41:
+        raise capi.LavbError(f"lidar_batch: cams must be (ncam, 41), got {cams.shape}")
+    b, p = rows.shape
+    c = raw.shape[1] - 4
+    if out is None:
+        out = torch.empty((b, p, 4 + c + n_time), dtype=torch.float32, device=raw.device)
+    elif out.dtype != torch.float32 or tuple(out.shape) != (b, p, 4 + c + n_time) or not out.is_contiguous() \
+            or out.device != raw.device:
+        raise capi.LavbError(f"lidar_batch: out must be a contiguous fp32 ({b}, {p}, {4 + c + n_time}) tensor on {raw.device}")
+    check(lib().lavb_lidar_batch(_ptr(raw), raw.shape[0], c, _ptr(rows), b * p, _ptr(sweeps),
+                                 sweeps.numel() // LIDAR_SWEEP_DTYPE.itemsize, cams.ctypes.data_as(C.c_void_p), cams.shape[0],
+                                 image_hw[0], image_hw[1], n_time, _ptr(out), _stream()), "lavb_lidar_batch")
+    _COUNT[0] += 1
+    return out
+
+
+def det_grid(min_x=-10, max_x=70, min_y=-40, max_y=40, pixels_per_meter=4, radius=1):
+    """(h, w, scalars) of the heat-map grid, each scalar computed as detections_to_heatmap's torch ops see it."""
+    h, w = (max_y - min_y) * pixels_per_meter, (max_x - min_x) * pixels_per_meter
+    inv_r = float(np.float32(1) / np.float32(radius))                  # torch divides by a scalar as a multiply by its reciprocal
+    return int(h), int(w), (pixels_per_meter, (max_y - min_y) * pixels_per_meter / 2, h, min_x * pixels_per_meter, inv_r)
+
+
+def det_heatmaps(actors, offsets, grid=None, out=None):
+    """Heat, size and orientation maps of a batch in one launch (see lavb_det_heatmaps in include/lav_b200.h).  actors (A, 6)
+    fp32 rows [x, y, ori, bx, by, typ]; offsets (B+1,) int32: sample i owns actors[offsets[i]:offsets[i+1]]; grid: the
+    keyword arguments of det_grid.  -> (heat, size, orim), each (B, 2, h, w) fp32, bit-identical to detections_to_heatmap."""
+    _need_cuda(actors, offsets)
+    if actors.dtype != torch.float32 or actors.dim() != 2 or actors.shape[1] != 6 or not actors.is_contiguous():
+        raise capi.LavbError(f"det_heatmaps: actors must be a contiguous (A, 6) fp32 tensor, got {actors.dtype} {tuple(actors.shape)}")
+    if offsets.dtype != torch.int32 or offsets.dim() != 1 or offsets.numel() < 1 or not offsets.is_contiguous():
+        raise capi.LavbError(f"det_heatmaps: offsets must be a contiguous (B+1,) int32 tensor, got {offsets.dtype} "
+                             f"{tuple(offsets.shape)}")
+    if actors.device != offsets.device:
+        raise capi.LavbError("det_heatmaps: actors and offsets must be on one device")
+    h, w, (ppm, cx0, cy0, cy1, inv_r) = det_grid(**(grid or {}))
+    b = offsets.numel() - 1
+    if out is None:
+        out = tuple(torch.empty((b, 2, h, w), dtype=torch.float32, device=actors.device) for _ in range(3))
+    elif any(t.dtype != torch.float32 or tuple(t.shape) != (b, 2, h, w) or not t.is_contiguous() or t.device != actors.device
+             for t in out):
+        raise capi.LavbError(f"det_heatmaps: out must be three contiguous fp32 ({b}, 2, {h}, {w}) tensors on {actors.device}")
+    heat, size, orim = out
+    check(lib().lavb_det_heatmaps(_ptr(actors), _ptr(offsets), b, h, w, ppm, cx0, cy0, cy1, inv_r, _ptr(heat), _ptr(size),
+                                  _ptr(orim), _stream()), "lavb_det_heatmaps")
+    _COUNT[0] += 1
+    return heat, size, orim
 
 
 def split_h16(x):

@@ -35,6 +35,7 @@ def parse_args(argv=None):
     ap.add_argument("--seed", type=int, default=2021)
     ap.add_argument("--save-dir", default=".", help="directory of the checkpoints")
     ap.add_argument("--max-steps", type=int, default=0, help="stop after this many steps (0 = run every epoch)")
+    ap.add_argument("--num-workers", type=int, default=16, help="host threads of the loader (record reads, PNG decodes)")
     args = ap.parse_args(argv)
     if args.perceive_only and args.motion_only:
         ap.error("--perceive-only and --motion-only exclude each other")
@@ -81,7 +82,7 @@ def main(argv=None):
                     perceive_only=args.perceive_only, motion_only=args.motion_only, **weights)
     loader = get_data_loader("temporal_lidar_painted", SimpleNamespace(config_path=args.config_path, seed=args.seed,
                                                                       batch_size=args.batch_size, rank=rank, world_size=world,
-                                                                      device=dev))
+                                                                      device=dev, num_workers=args.num_workers))
     if rank == 0:
         print(f"{len(loader.ds)} samples, {len(loader)} steps per epoch per rank, {world} rank(s) x {args.batch_size}")
         os.makedirs(args.save_dir, exist_ok=True)

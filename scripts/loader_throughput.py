@@ -8,7 +8,11 @@ Writes a seeded recording to a temporary directory and measures, with the GPU na
      read + written) over it;
   3. one sample of the CPU path (numpy / OpenCV restatement of __getitem__, oracle/dataset_ref.py) on one host core — what one
      of the reference's DataLoader workers does per sample;
-  4. LAVTrainer.train_lidar samples/s with the loader in the loop, against the same trainer on one pre-staged batch.
+  4. LAVTrainer.train_lidar samples/s with the loader in the loop, against the same trainer on one pre-staged batch;
+  5. a breakdown per batch at B = 32 and 64: host `prepare` on 1 and on --num-workers threads, the host tables of the batched
+     path (stage_batch), and the device build of the per-sample path (one GpuLidarStacker and detections_to_heatmap call per
+     sample, as the loader did before the batched kernels) against the batched path (launch_batch), both ending in a
+     synchronize, alternating on the same prepared batch.
 Results go to OUT/loader_throughput.json.
 """
 import argparse
@@ -34,12 +38,61 @@ def gpu_info():
     return q.stdout.strip().splitlines()[0] if q.returncode == 0 and q.stdout.strip() else torch.cuda.get_device_name()
 
 
+def per_sample_device(ds, hs, planes, gen):
+    """the device part of a batch as the loader built it before the batched kernels: per sample GpuLidarStacker and
+    detections_to_heatmap, one bev_targets launch, and the label copies."""
+    dev = ds.device
+    parts = [ds.lidar_and_maps(h, gen) for h in hs]
+    bev = ds.bev_batch(hs, planes.to(dev, non_blocking=True))
+    st = lambda i: torch.stack([p[i] for p in parts])
+    f32 = lambda key: torch.as_tensor(np.stack([h[key] for h in hs]), dtype=torch.float32).to(dev)
+    ints = lambda key: torch.tensor([h[key] for h in hs], dtype=torch.int64)
+    return (st(0), torch.tensor([p[1] for p in parts]), st(2), st(3), st(4), bev, f32("ego_locs"), ints("cmd").to(dev), f32("nxp"),
+            ints("bra").to(dev), f32("locs"), f32("oris"), torch.as_tensor(np.stack([h["typs"] for h in hs])).to(dev),
+            ints("num_objs"))
+
+
+def breakdown(ds, B, workers, reps):
+    """seconds per batch of B samples: host prepare (1 and `workers` threads), host tables, the two device paths."""
+    from concurrent.futures import ThreadPoolExecutor
+    rng = np.random.RandomState(B)
+    idxs = list(range(B))
+    draws = [ds.draw(rng) for _ in idxs]
+    out = {k: [] for k in ("prepare_1_thread_s", "prepare_workers_s", "stage_batch_s", "device_per_sample_s", "device_batched_s")}
+    with ThreadPoolExecutor(workers) as pool:
+        for r in range(reps + 1):                                      # the first round warms up and is not kept
+            t0 = time.perf_counter()
+            hs = [ds.prepare(i, *d) for i, d in zip(idxs, draws)]
+            t1 = time.perf_counter()
+            list(pool.map(lambda a: ds.prepare(a[0], *a[1]), zip(idxs, draws)))
+            t2 = time.perf_counter()
+            st = ds.stage_batch(hs, torch.Generator().manual_seed(r))
+            t3 = time.perf_counter()
+            planes = torch.from_numpy(np.concatenate([h["planes"] for h in hs])).pin_memory()
+            torch.cuda.synchronize()
+            t4 = time.perf_counter()
+            old = per_sample_device(ds, hs, planes, torch.Generator().manual_seed(r))
+            torch.cuda.synchronize()
+            t5 = time.perf_counter()
+            new = ds.launch_batch(st)
+            torch.cuda.synchronize()
+            t6 = time.perf_counter()
+            if r == 0:
+                assert all(torch.equal(a.cpu(), b.cpu()) for a, b in zip(old, new))
+                continue
+            for k, v in zip(out, (t1 - t0, t2 - t1, t3 - t2, t5 - t4, t6 - t5)):
+                out[k].append(v)
+    return {k: float(np.median(v)) for k, v in out.items()}
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--out-dir", required=True)
     ap.add_argument("--batch", type=int, default=32)
     ap.add_argument("--batches", type=int, default=6)
     ap.add_argument("--train-steps", type=int, default=4)
+    ap.add_argument("--num-workers", type=int, default=16)
+    ap.add_argument("--breakdown-reps", type=int, default=3)
     args = ap.parse_args()
     os.makedirs(args.out_dir, exist_ok=True)
     if not torch.cuda.is_available():
@@ -51,10 +104,10 @@ def main():
     from oracle import dataset_ref as D
     from oracle import lav_ref as O
     dev = torch.device("cuda:0")
-    res = dict(gpu=gpu_info(), batch=args.batch)
+    res = dict(gpu=gpu_info(), batch=args.batch, num_workers=args.num_workers)
     tmp = tempfile.mkdtemp(prefix="lavb_loader_")                      # the recording (~1 MB per frame) stays out of --out-dir
     rec = os.path.join(tmp, "recording")
-    n_traj, n_frames = 4, 21 + args.batch * (args.batches + 1) // 4 + 1
+    n_traj, n_frames = 4, 21 + max(args.batch * (args.batches + 1), 64) // 4 + 1
     t0 = time.time()
     synth.record_trajectories(rec, n_traj, n_frames, seed=2021, n_points=30000)
     res["record_s"] = time.time() - t0
@@ -68,7 +121,7 @@ def main():
     res["samples"] = len(ds)
 
     # 1. loader batches/s
-    loader = TemporalBatchLoader(ds, args.batch, seed=1)
+    loader = TemporalBatchLoader(ds, args.batch, seed=1, num_workers=args.num_workers)
     it = iter(loader)
     staged = next(it)                                                  # warm-up (and the trainer's pre-staged batch below)
     torch.cuda.synchronize()
@@ -134,7 +187,7 @@ def main():
         tr.train_lidar(*staged)
     torch.cuda.synchronize()
     res["train_staged_samples_per_s"] = args.train_steps * args.batch / (time.time() - t0)
-    loader = TemporalBatchLoader(ds, args.batch, seed=2)
+    loader = TemporalBatchLoader(ds, args.batch, seed=2, num_workers=args.num_workers)
     it = iter(loader)
     tr.train_lidar(*next(it))
     torch.cuda.synchronize()
@@ -143,6 +196,7 @@ def main():
         tr.train_lidar(*next(it))
     torch.cuda.synchronize()
     res["train_loader_samples_per_s"] = args.train_steps * args.batch / (time.time() - t0)
+    res["breakdown"] = {B: breakdown(ds, B, args.num_workers, args.breakdown_reps) for B in (32, 64)}
     shutil.rmtree(tmp, True)
     os.makedirs(args.out_dir, exist_ok=True)
     with open(os.path.join(args.out_dir, "loader_throughput.json"), "w") as f:
