@@ -136,7 +136,7 @@ __global__ void __launch_bounds__(kPairThreads, kC == 64 ? 2 : 1) conv_pair_umma
   for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x, ++i) {
     const int img = tile / p.tiles_per_img, y0 = (tile - img * p.tiles_per_img) * p.tile_h;
     // ---- stage 1: acc1 = conv3x1(x)
-    float acc[kNC][32];
+    float acc[kC / 2];                               // 64-column chunk cc: acc[32cc .. 32cc+31]
     int prev = -1;
     for (int kb = 0; kb < kNkb; ++kb) {
       mbar_wait(full_bar + 8 * slot, phase);
@@ -144,10 +144,8 @@ __global__ void __launch_bounds__(kPairThreads, kC == 64 ? 2 : 1) conv_pair_umma
       const uint64_t a_desc = sm90::desc_sw128(sa + wg * (kABytes / 2)), b_desc = sm90::desc_sw128(sa + kABytes);
       sm90::wgmma_fence();
 #pragma unroll
-      for (int k = 0; k < kBlockK / 16; ++k)
-#pragma unroll
-        for (int cc = 0; cc < kNC; ++cc)
-          sm90::wgmma_n64(acc[cc], a_desc + (uint64_t)(2 * k), b_desc + (uint64_t)(cc * 64 * 128 / 16 + 2 * k), (kb | k) ? 1u : 0u);
+      for (int k = 0; k < kBlockK / 16; ++k)         // one MMA over all kC columns per K16 step
+        sm90::wgmma<kC>(acc, a_desc + (uint64_t)(2 * k), b_desc + (uint64_t)(2 * k), (kb | k) ? 1u : 0u);
       sm90::wgmma_commit();
       sm90::wgmma_wait<1>();
       if (prev >= 0 && lane == 0) mbar_arrive(empty_bar + 8 * prev);
@@ -155,8 +153,7 @@ __global__ void __launch_bounds__(kPairThreads, kC == 64 ? 2 : 1) conv_pair_umma
       if (++slot == p.stages) { slot = 0; phase ^= 1; }
     }
     sm90::wgmma_wait<0>();
-#pragma unroll
-    for (int cc = 0; cc < kNC; ++cc) sm90::acc_fence(acc[cc]);
+    sm90::acc_fence(acc);
     if (lane == 0) mbar_arrive(empty_bar + 8 * prev);
     PAIR_STAMP(0, i);
     // ---- epilogue 1: acc1 + bias1 -> h16 -> relu -> three shifted K-major copies in shared memory.  Both warpgroups' stage-2 MMAs
@@ -175,7 +172,7 @@ __global__ void __launch_bounds__(kPairThreads, kC == 64 ? 2 : 1) conv_pair_umma
         for (int j = 0; j < 8; ++j) {
           const int col = 64 * cc + 8 * j + 2 * (lane & 3);
           const float2 b = *reinterpret_cast<const float2*>(ep_b1 + col);
-          const uint32_t v = relu2(pack_h16(acc[cc][4 * j + 2 * h] + b.x, acc[cc][4 * j + 2 * h + 1] + b.y));
+          const uint32_t v = relu2(pack_h16(acc[32 * cc + 4 * j + 2 * h] + b.x, acc[32 * cc + 4 * j + 2 * h + 1] + b.y));
           uint8_t* blk = midp + cc * kABytes + (col & 7) * 2;              // K-block cc (64 channels), piece j, this pair
           if (ok0) *reinterpret_cast<uint32_t*>(blk + 0 * kChunks * kABytes + r0 * 128 + ((j ^ (r0 & 7)) << 4)) = v;
           *reinterpret_cast<uint32_t*>(blk + 1 * kChunks * kABytes + m * 128 + ((j ^ (m & 7)) << 4)) = v;
@@ -196,9 +193,7 @@ __global__ void __launch_bounds__(kPairThreads, kC == 64 ? 2 : 1) conv_pair_umma
         const uint64_t a_desc = sm90::desc_sw128(mid + (kb0 + b) * kABytes + wg * (kABytes / 2)), b_desc = sm90::desc_sw128(sa + b * kWBytes);   // kb = t*kchunks + kc
 #pragma unroll
         for (int k = 0; k < kBlockK / 16; ++k)
-#pragma unroll
-          for (int cc = 0; cc < kNC; ++cc)
-            sm90::wgmma_n64(acc[cc], a_desc + (uint64_t)(2 * k), b_desc + (uint64_t)(cc * 64 * 128 / 16 + 2 * k), (kb0 | b | k) ? 1u : 0u);
+          sm90::wgmma<kC>(acc, a_desc + (uint64_t)(2 * k), b_desc + (uint64_t)(2 * k), (kb0 | b | k) ? 1u : 0u);
       }
       sm90::wgmma_commit();
       sm90::wgmma_wait<1>();
@@ -207,8 +202,7 @@ __global__ void __launch_bounds__(kPairThreads, kC == 64 ? 2 : 1) conv_pair_umma
       if (++slot == p.stages) { slot = 0; phase ^= 1; }
     }
     sm90::wgmma_wait<0>();
-#pragma unroll
-    for (int cc = 0; cc < kNC; ++cc) sm90::acc_fence(acc[cc]);
+    sm90::acc_fence(acc);
     if (lane == 0) mbar_arrive(empty_bar + 8 * prev);
     PAIR_STAMP(2, i);
     // ---- epilogue 2: acc2 + shift2 -> h16 (+ residual) -> ReLU -> NHWC
@@ -224,7 +218,7 @@ __global__ void __launch_bounds__(kPairThreads, kC == 64 ? 2 : 1) conv_pair_umma
         for (int j = 0; j < 8; ++j) {
           const int col = 64 * cc + 8 * j + 2 * (lane & 3);
           const float2 t = *reinterpret_cast<const float2*>(ep_t2 + col);
-          uint32_t v = pack_h16(acc[cc][4 * j + 2 * h] + t.x, acc[cc][4 * j + 2 * h + 1] + t.y);
+          uint32_t v = pack_h16(acc[32 * cc + 4 * j + 2 * h] + t.x, acc[32 * cc + 4 * j + 2 * h + 1] + t.y);
           if (p.res) v = add2(v, __ldg(reinterpret_cast<const uint32_t*>(p.res + pix * kC + col)), relu_out);
           else if (relu_out) v = relu2(v);
           *reinterpret_cast<uint32_t*>(p.out + pix * kC + col) = v;

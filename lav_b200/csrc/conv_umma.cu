@@ -9,9 +9,10 @@
 // phase with its own tap list (same host packing as conv_taps.cu).
 //
 // Warp roles (288 threads, persistent over tiles):
-//   warps 0-3, 4-7: two consumer warpgroups, one per 64-pixel half of the tile (tile rows 0-3 / 4-7).  Each issues
-//                   m64 x N x k16 wgmma over its half of the A block and the whole B block, keeps one K-block of MMAs in
-//                   flight, and runs the epilogue (bias / BN affine / ReLU / residual / sigmoid) from its registers.
+//   warps 0-3, 4-7: two consumer warpgroups, one per 64-pixel half of the tile (tile rows 0-3 / 4-7).  Each issues ONE
+//                   m64 x N x k16 wgmma per K16 step over its half of the A block and the whole B block (N = cout_mma, so
+//                   the A fragment is read from shared memory once per step, not once per 32 columns), keeps one K-block
+//                   of MMAs in flight, and runs the epilogue (bias / BN affine / ReLU / residual / sigmoid) from its registers.
 //   warp 8         : TMA producer (one lane) — smem ring of `stages` {A 16 KB, B cout*128 B}
 // Layers with cout <= 128 run two CTAs per SM so that one CTA's epilogue overlaps the other's MMAs.
 #include "sm90.cuh"
@@ -99,7 +100,7 @@ __global__ void __launch_bounds__(kConvThreads, kNC <= 4 ? 2 : 1) conv_umma_kern
   const int wg = warp >> 2;                        // tile rows [64 wg, 64 wg + 64)
   const float lo_pre = p.pre_relu ? 0.f : -INFINITY, lo_post = p.post_relu ? 0.f : -INFINITY;
   int stage = 0; uint32_t phase = 0;
-  float acc[kNC][16];
+  float acc[16 * kNC];                             // 32-column chunk c: acc[16c .. 16c+15]
   for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
     int prev_stage = -1;
     for (int kb = 0; kb < nkb; ++kb) {
@@ -108,10 +109,8 @@ __global__ void __launch_bounds__(kConvThreads, kNC <= 4 ? 2 : 1) conv_umma_kern
       const uint64_t a_desc = sm90::desc_sw128(sa + wg * (kABytes / 2)), b_desc = sm90::desc_sw128(sa + kABytes);
       sm90::wgmma_fence();
 #pragma unroll
-      for (int k = 0; k < kBlockK / 16; ++k)       // +32 B per K16 step inside the 128 B swizzle atom
-#pragma unroll
-        for (int c = 0; c < kNC; ++c)              // 32 B-rows of 128 B per chunk
-          sm90::wgmma_n32(acc[c], a_desc + (uint64_t)(2 * k), b_desc + (uint64_t)(c * 32 * 128 / 16 + 2 * k), (kb | k) ? 1u : 0u);
+      for (int k = 0; k < kBlockK / 16; ++k)       // +32 B per K16 step inside the 128 B swizzle atom; one MMA over all kN columns
+        sm90::wgmma<kN>(acc, a_desc + (uint64_t)(2 * k), b_desc + (uint64_t)(2 * k), (kb | k) ? 1u : 0u);
       sm90::wgmma_commit();
       sm90::wgmma_wait<1>();                             // the previous K-block's MMAs are done: its slot may be refilled
       if (prev_stage >= 0 && lane == 0) mbar_arrive(empty_bar + 8 * prev_stage);
@@ -119,53 +118,56 @@ __global__ void __launch_bounds__(kConvThreads, kNC <= 4 ? 2 : 1) conv_umma_kern
       if (++stage == p.stages) { stage = 0; phase ^= 1; }
     }
     sm90::wgmma_wait<0>();
-#pragma unroll
-    for (int c = 0; c < kNC; ++c) sm90::acc_fence(acc[c]);
+    sm90::acc_fence(acc);
     if (prev_stage >= 0 && lane == 0) mbar_arrive(empty_bar + 8 * prev_stage);
 
-    // ---- epilogue: this thread holds rows m and m + 8 of the tile, two adjacent columns per 8-column group
+    // ---- epilogue: this thread holds rows m and m + 8 of the tile, columns 8 j + c0 (+1) of every 8-column group j.
+    // Every per-column offset below is the compile-time 8 j on top of a per-thread base, so no column index is kept live
+    // in registers across tiles next to the 16 kNC accumulators.
+    const int c0 = 2 * (lane & 3), store_lim = p.cout_store - c0;
     const int img = tile / tiles_per_img, r = tile - img * tiles_per_img;
-    const int ty0 = (r / p.tiles_x) * kTileH, tx0 = (r % p.tiles_x) * kTileW;
+    // tile row m = 64 wg + 16 (warp & 3) + (lane >> 2) + 8 h is grid pixel (row 4 wg + (warp & 3), column (lane >> 2) + 8 h)
+    const int gy = (r / p.tiles_x) * kTileH + 4 * wg + (warp & 3), oy = gy * p.out_sy + p.out_oy;
+    if (!(gy < p.hog && oy < p.hout)) continue;
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
-      const int m = 64 * wg + 16 * (warp & 3) + (lane >> 2) + 8 * h;
-      const int gy = ty0 + m / kTileW, gx = tx0 + m % kTileW;
-      const int oy = gy * p.out_sy + p.out_oy, ox = gx * p.out_sx + p.out_ox;
-      if (!(gy < p.hog && gx < p.wog && oy < p.hout && ox < p.wout)) continue;
+      const int gx = (r % p.tiles_x) * kTileW + (lane >> 2) + 8 * h, ox = gx * p.out_sx + p.out_ox;
+      if (!(gx < p.wog && ox < p.wout)) continue;
       const long long pix = ((long long)img * p.hout + oy) * p.wout + ox;
+      uint8_t* out_at = reinterpret_cast<uint8_t*>(p.out) + (pix * p.out_cstride + p.out_coff + c0) * (p.out_is_f32 ? 4 : 2);
+      const h16* res_at = p.res ? p.res + pix * p.res_cstride + p.res_coff + c0 : nullptr;
+      const float* bias_at = ep_bias + c0;
+      const float* st_at = ep_st + 2 * c0;
 #pragma unroll
-      for (int c = 0; c < kNC; ++c) {
+      for (int j = 0; j < 4 * kNC; ++j) {
+        const int g = 8 * j;                         // column = g + c0
+        float x0 = acc[4 * j + 2 * h], x1 = acc[4 * j + 2 * h + 1];
+        if (p.pre_bias) { x0 += bias_at[g]; x1 += bias_at[g + 1]; }
+        const float4 st = *reinterpret_cast<const float4*>(st_at + 2 * g);   // (s0, t0, s1, t1)
+        x0 = fmaf(fmaxf(x0, lo_pre), st.x, st.y);
+        x1 = fmaf(fmaxf(x1, lo_pre), st.z, st.w);
+        if (res_at) {
+          const float2 rv = unpack_h16(__ldg(reinterpret_cast<const uint32_t*>(res_at + g)));
+          x0 += rv.x; x1 += rv.y;
+        }
+        x0 = fmaxf(x0, lo_post); x1 = fmaxf(x1, lo_post);
+        if (p.sigmoid) { x0 = 1.f / (1.f + expf(-x0)); x1 = 1.f / (1.f + expf(-x1)); }
+        if (kNC == 1 && p.d2s_nout) {   // depth-to-space (cout 32 only): column q = pos*nout + k -> pixel (oy + pos/2, ox + pos%2), channel k
+          float* ob = reinterpret_cast<float*>(p.out);
+          const int no = p.d2s_nout;
 #pragma unroll
-        for (int i = 0; i < 4; ++i) {
-          const int col = 32 * c + 8 * i + 2 * (lane & 3);
-          float x0 = acc[c][4 * i + 2 * h], x1 = acc[c][4 * i + 2 * h + 1];
-          if (p.pre_bias) { x0 += ep_bias[col]; x1 += ep_bias[col + 1]; }
-          const float4 st = *reinterpret_cast<const float4*>(ep_st + 2 * col);   // (s0, t0, s1, t1)
-          x0 = fmaf(fmaxf(x0, lo_pre), st.x, st.y);
-          x1 = fmaf(fmaxf(x1, lo_pre), st.z, st.w);
-          if (p.res) {
-            const float2 rv = unpack_h16(__ldg(reinterpret_cast<const uint32_t*>(p.res + pix * p.res_cstride + p.res_coff + col)));
-            x0 += rv.x; x1 += rv.y;
-          }
-          x0 = fmaxf(x0, lo_post); x1 = fmaxf(x1, lo_post);
-          if (p.sigmoid) { x0 = 1.f / (1.f + expf(-x0)); x1 = 1.f / (1.f + expf(-x1)); }
-          if (p.d2s_nout) {   // depth-to-space: column j = pos*nout + k -> pixel (oy + pos/2, ox + pos%2), channel k
-            float* ob = reinterpret_cast<float*>(p.out);
-            const int no = p.d2s_nout;
-#pragma unroll
-            for (int e = 0; e < 2; ++e) {
-              const int j = col + e;
-              if (j < 4 * no) {
-                const int pos = j / no, k = j - pos * no;
-                ob[(pix + (long long)(pos >> 1) * p.wout + (pos & 1)) * no + k] = e ? x1 : x0;
-              }
+          for (int e = 0; e < 2; ++e) {
+            const int q = g + c0 + e;
+            if (q < 4 * no) {
+              const int pos = q / no, k = q - pos * no;
+              ob[(pix + (long long)(pos >> 1) * p.wout + (pos & 1)) * no + k] = e ? x1 : x0;
             }
-          } else if (col < p.cout_store) {
-            if (p.out_is_f32)
-              *reinterpret_cast<float2*>(reinterpret_cast<float*>(p.out) + pix * p.out_cstride + p.out_coff + col) = make_float2(x0, x1);
-            else
-              *reinterpret_cast<uint32_t*>(reinterpret_cast<h16*>(p.out) + pix * p.out_cstride + p.out_coff + col) = pack_h16(x0, x1);
           }
+        } else if (g < store_lim) {                  // g + c0 < cout_store
+          if (p.out_is_f32)
+            *reinterpret_cast<float2*>(out_at + 4 * g) = make_float2(x0, x1);
+          else
+            *reinterpret_cast<uint32_t*>(out_at + 2 * g) = pack_h16(x0, x1);
         }
       }
     }

@@ -928,7 +928,7 @@ __global__ void __launch_bounds__(kRows, 3) pillar_tile_encode_tc_kernel(
       for (int mh = 0; mh < 2; ++mh) {
         const uint64_t a_desc = desc_sw128(base + TcSmem::a + mh * 64 * 128);
 #pragma unroll
-        for (int k = 0; k < 3; ++k) wgmma_n64(acc[mh], a_desc + (uint64_t)(2 * k), b1_desc + (uint64_t)(2 * k), k ? 1u : 0u);
+        for (int k = 0; k < 3; ++k) wgmma<64>(acc[mh], a_desc + (uint64_t)(2 * k), b1_desc + (uint64_t)(2 * k), k ? 1u : 0u);
       }
       wgmma_commit();
       wgmma_wait<0>();
@@ -955,7 +955,7 @@ __global__ void __launch_bounds__(kRows, 3) pillar_tile_encode_tc_kernel(
       for (int mh = 0; mh < 2; ++mh) {
         const uint64_t a_desc = desc_sw128(base + TcSmem::a + mh * 64 * 128);
 #pragma unroll
-        for (int k = 0; k < 4; ++k) wgmma_n64(acc[mh], a_desc + (uint64_t)(2 * k), b2_desc + (uint64_t)(2 * k), k ? 1u : 0u);
+        for (int k = 0; k < 4; ++k) wgmma<64>(acc[mh], a_desc + (uint64_t)(2 * k), b2_desc + (uint64_t)(2 * k), k ? 1u : 0u);
       }
       wgmma_commit();
       wgmma_wait<0>();

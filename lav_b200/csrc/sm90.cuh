@@ -77,54 +77,62 @@ template <int N> __device__ __forceinline__ void acc_fence(float (&d)[N]) {
   for (int i = 0; i < N; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
 
-// D[64 x 32] (+)= A[64 x 16] * B[32 x 16]^T, both operands K-major in shared memory, fp32 accumulators in registers.
-// Fragment of thread t of the warpgroup: rows 16 (t/32) + (t%32)/4 (+8), columns 8 i + 2 (t%4) (+1):
+// D[64 x N] (+)= A[64 x 16] * B[N x 16]^T for N = 32, 64, ..., 256: both operands K-major in shared memory, fp32
+// accumulators in registers.  Fragment of thread t of the warpgroup: rows 16 (t/32) + (t%32)/4 (+8), columns 8 i + 2 (t%4)
+// (+1) for 8-column group i < N/8:
 //   d[4i] = (row, col), d[4i+1] = (row, col+1), d[4i+2] = (row+8, col), d[4i+3] = (row+8, col+1).
-__device__ __forceinline__ void wgmma_n32(float (&d)[16], uint64_t a, uint64_t b, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %18, 0;\n\t"
-      "wgmma.mma_async.sync.aligned.m64n32k16.f32." LAVB_H16_PTX "." LAVB_H16_PTX " "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1, 0, 0;\n\t}"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
-        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
-      : "l"(a), "l"(b), "r"(accumulate));
-}
-// the same with N = 64 (fragment as above, i < 8)
-__device__ __forceinline__ void wgmma_n64(float (&d)[32], uint64_t a, uint64_t b, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %34, 0;\n\t"
-      "wgmma.mma_async.sync.aligned.m64n64k16.f32." LAVB_H16_PTX "." LAVB_H16_PTX " "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, 0, 0;\n\t}"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
-        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
-        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
-        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
-      : "l"(a), "l"(b), "r"(accumulate));
-}
+// So the fragment of one m64nNk16 is the column-wise concatenation of N/32 m64n32k16 fragments: 32-column chunk c is
+// d[16c .. 16c+15].  B rows r0.. of a K-major SWIZZLE_128B operand start at descriptor + 8 r0 (128 B rows, r0 % 8 == 0).
+template <int N> __device__ void wgmma(float (&d)[N / 2], uint64_t a, uint64_t b, uint32_t accumulate);
 
-// the same with N = 128 (fragment as above, i < 16)
-__device__ __forceinline__ void wgmma_n128(float (&d)[64], uint64_t a, uint64_t b, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %66, 0;\n\t"
-      "wgmma.mma_async.sync.aligned.m64n128k16.f32." LAVB_H16_PTX "." LAVB_H16_PTX " "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
-      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
-      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, 0, 0;\n\t}"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
-        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
-        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
-        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
-        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
-        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
-        "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
-        "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
-      : "l"(a), "l"(b), "r"(accumulate));
-}
+// operand text of accumulator registers 16c .. 16c + 15 (one 32-column chunk)
+#define LAVB_WG_R0 "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15"
+#define LAVB_WG_R1 "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31"
+#define LAVB_WG_R2 "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47"
+#define LAVB_WG_R3 "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63"
+#define LAVB_WG_R4 "%64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79"
+#define LAVB_WG_R5 "%80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95"
+#define LAVB_WG_R6 "%96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111"
+#define LAVB_WG_R7 "%112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127"
+#define LAVB_WG_D4(i) "+f"(d[i]), "+f"(d[i + 1]), "+f"(d[i + 2]), "+f"(d[i + 3])
+#define LAVB_WG_D16(i) LAVB_WG_D4(i), LAVB_WG_D4(i + 4), LAVB_WG_D4(i + 8), LAVB_WG_D4(i + 12)
+// N, the accumulator register list, the operand numbers of a, b and accumulate (N/2, N/2 + 1, N/2 + 2), the "+f" operands
+#define LAVB_WGMMA(N, REGS, IA, IB, IP, ...)                                                                         \
+  template <> __device__ __forceinline__ void wgmma<N>(float (&d)[N / 2], uint64_t a, uint64_t b, uint32_t accumulate) { \
+    asm volatile(                                                                                                      \
+        "{\n\t.reg .pred p;\n\t"                                                                                       \
+        "setp.ne.b32 p, %" #IP ", 0;\n\t"                                                                              \
+        "wgmma.mma_async.sync.aligned.m64n" #N "k16.f32." LAVB_H16_PTX "." LAVB_H16_PTX " "                            \
+        "{" REGS "}, %" #IA ", %" #IB ", p, 1, 1, 0, 0;\n\t}"                                                          \
+        : __VA_ARGS__                                                                                                  \
+        : "l"(a), "l"(b), "r"(accumulate));                                                                            \
+  }
+LAVB_WGMMA(32, LAVB_WG_R0, 16, 17, 18, LAVB_WG_D16(0))
+LAVB_WGMMA(64, LAVB_WG_R0 ", " LAVB_WG_R1, 32, 33, 34, LAVB_WG_D16(0), LAVB_WG_D16(16))
+LAVB_WGMMA(96, LAVB_WG_R0 ", " LAVB_WG_R1 ", " LAVB_WG_R2, 48, 49, 50, LAVB_WG_D16(0), LAVB_WG_D16(16), LAVB_WG_D16(32))
+LAVB_WGMMA(128, LAVB_WG_R0 ", " LAVB_WG_R1 ", " LAVB_WG_R2 ", " LAVB_WG_R3, 64, 65, 66,
+           LAVB_WG_D16(0), LAVB_WG_D16(16), LAVB_WG_D16(32), LAVB_WG_D16(48))
+LAVB_WGMMA(160, LAVB_WG_R0 ", " LAVB_WG_R1 ", " LAVB_WG_R2 ", " LAVB_WG_R3 ", " LAVB_WG_R4, 80, 81, 82,
+           LAVB_WG_D16(0), LAVB_WG_D16(16), LAVB_WG_D16(32), LAVB_WG_D16(48), LAVB_WG_D16(64))
+LAVB_WGMMA(192, LAVB_WG_R0 ", " LAVB_WG_R1 ", " LAVB_WG_R2 ", " LAVB_WG_R3 ", " LAVB_WG_R4 ", " LAVB_WG_R5, 96, 97, 98,
+           LAVB_WG_D16(0), LAVB_WG_D16(16), LAVB_WG_D16(32), LAVB_WG_D16(48), LAVB_WG_D16(64), LAVB_WG_D16(80))
+LAVB_WGMMA(224, LAVB_WG_R0 ", " LAVB_WG_R1 ", " LAVB_WG_R2 ", " LAVB_WG_R3 ", " LAVB_WG_R4 ", " LAVB_WG_R5 ", " LAVB_WG_R6,
+           112, 113, 114, LAVB_WG_D16(0), LAVB_WG_D16(16), LAVB_WG_D16(32), LAVB_WG_D16(48), LAVB_WG_D16(64), LAVB_WG_D16(80),
+           LAVB_WG_D16(96))
+LAVB_WGMMA(256, LAVB_WG_R0 ", " LAVB_WG_R1 ", " LAVB_WG_R2 ", " LAVB_WG_R3 ", " LAVB_WG_R4 ", " LAVB_WG_R5 ", " LAVB_WG_R6 ", " LAVB_WG_R7,
+           128, 129, 130, LAVB_WG_D16(0), LAVB_WG_D16(16), LAVB_WG_D16(32), LAVB_WG_D16(48), LAVB_WG_D16(64), LAVB_WG_D16(80),
+           LAVB_WG_D16(96), LAVB_WG_D16(112))
+#undef LAVB_WGMMA
+#undef LAVB_WG_D16
+#undef LAVB_WG_D4
+#undef LAVB_WG_R0
+#undef LAVB_WG_R1
+#undef LAVB_WG_R2
+#undef LAVB_WG_R3
+#undef LAVB_WG_R4
+#undef LAVB_WG_R5
+#undef LAVB_WG_R6
+#undef LAVB_WG_R7
 
 }  // namespace sm90
 }  // namespace lavb

@@ -103,7 +103,7 @@ __global__ void __launch_bounds__(kThreads, 1) conv7x7s2_umma_kernel(const __gri
       wgmma_fence();
 #pragma unroll
       for (int k = 0; k < kBlockK / 16; ++k)      // +32 B per K16 step inside the 128 B swizzle atom
-        wgmma_n128(acc, a_desc + (uint64_t)(2 * k), b_desc + (uint64_t)(2 * k), (kb | k) ? 1u : 0u);
+        wgmma<128>(acc, a_desc + (uint64_t)(2 * k), b_desc + (uint64_t)(2 * k), (kb | k) ? 1u : 0u);
       wgmma_commit();
       wgmma_wait<1>();                             // the previous K-block's MMAs are done: its slot may be refilled
       if (prev_stage >= 0 && lane == 0) mbar_arrive(empty_bar + 8 * prev_stage);

@@ -1,0 +1,157 @@
+"""A/B timing of the product's conv_umma layers (and the fused ERFNet pairs of conv_pair_umma) at bench shapes (B = 32 frames
+per agent group) for two builds of liblavb200.so.
+
+    python scripts/conv_umma_ab.py --base-lib OTHER/liblavb200.so [--rounds 5] [--reps 10]
+
+Both libraries are loaded into one process; the rounds alternate base / this tree's build on the same inputs and weights.
+For every layer it prints the median kernel time (CUDA events over `reps` back-to-back launches), the GEMM rate and its
+fraction of the 989 TFLOP/s dense fp16 peak, whether the two builds' outputs are bit-identical, and two byte counts derived
+from the shapes for one 64-deep K-block of one CTA (128 pixels x cout_mma):
+  smem/KB : shared-memory operand bytes the MMAs read (A once per wgmma, B once per warpgroup), base -> this tree
+  L2/KB   : bytes the TMA moves from L2 into shared memory (A box + B box)
+The card name, power limit and SM clocks are read in the same run.
+"""
+import argparse
+import os
+import subprocess
+import sys
+
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+import torch
+from lav_b200 import capi, ops
+from lav_b200.layers import TapConv
+
+PEAK = 989e12
+
+
+def load(path):
+    capi._lib, capi.LIB_PATH = None, path
+    return capi.lib()
+
+
+def layers(dev, B):
+    """(name, run() -> output, GEMM flop, cout_mma, [(cin, ntaps) per launch])"""
+    g = torch.Generator(device=dev).manual_seed(0)
+    rn = lambda *s: torch.randn(*s, device=dev, generator=g)
+    h16 = ops.h16()
+    out = []
+
+    def tap(name, n, hin, win, cin, cout, k, stride=1, pad=1, transposed=False, opad=0, **kw):
+        wshape = (cin, cout, k, k) if transposed else (cout, cin, k, k)
+        layer = TapConv(rn(*wshape) * (2.0 / (cin * k * k)) ** 0.5, transposed, stride, pad, 1, opad, **kw)
+        x = rn(n, hin, win, cin).to(h16)
+        ho, wo = layer.out_size(hin, win)
+        y = torch.empty(n, ho, wo, cout, device=dev, dtype=h16)
+        fl = 0
+        for ph in layer.phases:
+            (osy, osx), (ooy, oox) = ph["out_s"], ph["out_o"]
+            fl += 2 * n * ((ho - ooy + osy - 1) // osy) * ((wo - oox + osx - 1) // osx) * cin * len(ph["taps"]) * layer.cout
+        out.append((name, lambda: layer(x, out=y), fl, (cout + 31) // 32 * 32, [(cin, len(ph["taps"])) for ph in layer.phases]))
+
+    bn = lambda c: dict(pre_relu=True, scale=rn(c).abs() + 0.5, shift=rn(c) * 0.1)
+    tap("heads 384->256 160x160", B, 160, 160, 384, 256, 3, **bn(256))
+    tap("bb 64->64 s1 160x160", B, 160, 160, 64, 64, 3, **bn(64))
+    tap("bb 64->64 s2 320->160", B, 320, 320, 64, 64, 3, stride=2, **bn(64))
+    tap("bb 128->128 s1 80x80", B, 80, 80, 128, 128, 3, **bn(128))
+    tap("erf down 64->64 s2 72x64", 3 * B, 72, 64, 64, 64, 3, stride=2, bias=rn(64) * 0.1, scale=rn(64).abs() + 0.5,
+        shift=rn(64) * 0.1, post_relu=True)
+    tap("erf up 128->64 36x32", 3 * B, 36, 32, 128, 64, 3, stride=2, transposed=True, opad=1, bias=rn(64) * 0.1,
+        scale=rn(64).abs() + 0.5, shift=rn(64) * 0.1, post_relu=True)
+    tap("erf up 64->16 72x64", 3 * B, 72, 64, 64, 16, 3, stride=2, transposed=True, opad=1, bias=rn(16) * 0.1,
+        scale=rn(16).abs() + 0.5, shift=rn(16) * 0.1, post_relu=True)
+
+    # the four head output layers: 2x2-tap GEMMs over the 64-channel slices of the heads conv output, depth-to-space epilogue
+    hid = rn(B, 160, 160, 256).to(h16)
+    heads = []
+    for gi, no in enumerate((2, 2, 2, 3)):
+        wu = (rn(4, 32, 64) * 0.1).to(h16).contiguous()
+        b32 = torch.zeros(32, device=dev)
+        b32[:4 * no] = rn(no).repeat(4) * 0.1
+        heads.append((gi, no, wu, b32, torch.empty(B, 320, 320, no, device=dev)))
+
+    def d2s():
+        for gi, no, wu, b32, o in heads:
+            ops.conv_taps(hid, 64, 64 * gi, o, 32, 0, 160, 160, (1, 1), (2, 2), (0, 0), [(0, 0), (0, 1), (1, 0), (1, 1)], wu,
+                          bias=b32, sigmoid=gi == 3, umma=True, d2s_nout=no)
+        return torch.cat([h[4].flatten() for h in heads])
+
+    out.append(("head outputs 4x(64->32 2x2 d2s)", d2s, 4 * 2 * B * 160 * 160 * 64 * 4 * 32, 32, [(64, 4)] * 4))
+
+    # the fused ERFNet (3x1 -> 1x3) pairs (conv_pair_umma_kernel): 64 channels at 72 x 64, 128 channels at 36 x 32 (dilation 2)
+    def pair(name, n, h, w, c, dil):
+        x = rn(n, h, w, c).to(h16)
+        w1, w2 = ((rn(3, c, c) / (3 * c) ** 0.5).to(h16).contiguous() for _ in range(2))
+        b1, t2 = rn(c) * 0.1, rn(c) * 0.1
+        y = torch.empty(n, h, w, c, device=dev, dtype=h16)
+        out.append((name, lambda: ops.conv_pair_umma(x, w1, b1, w2, t2, dil, res=x, out=y), 2 * 2 * n * h * w * c * c * 3, c, None))
+
+    pair("erf pair 64 72x64 (fused 3x1,1x3)", 3 * B, 72, 64, 64, 1)
+    pair("erf pair 128 36x32 d2 (fused)", 3 * B, 36, 32, 128, 2)
+    return out
+
+
+def kblock_bytes(cout_mma, old_width=32):
+    """(smem operand bytes per K-block with one wgmma per `old_width` columns, with one full-width wgmma, L2 -> SM bytes)"""
+    a_per_wgmma = 64 * 16 * 2                      # one warpgroup's 64 x 16 A fragment
+    b = 2 * 4 * cout_mma * 16 * 2                  # 2 warpgroups x 4 K16 steps x the whole B slice
+    old = 2 * 4 * max(1, cout_mma // old_width) * a_per_wgmma + b
+    return old, 2 * 4 * a_per_wgmma + b, 128 * 128 + cout_mma * 128
+
+
+def time_ms(fn, reps):
+    a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    a.record()
+    for _ in range(reps):
+        fn()
+    b.record()
+    torch.cuda.synchronize()
+    return a.elapsed_time(b) / reps
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--base-lib", required=True, help="liblavb200.so of the tree to compare against")
+    ap.add_argument("--batch", type=int, default=32)
+    ap.add_argument("--rounds", type=int, default=5)
+    ap.add_argument("--reps", type=int, default=10)
+    args = ap.parse_args()
+    if not torch.cuda.is_available():
+        sys.exit("conv_umma_ab.py needs a CUDA device")
+    dev = torch.device("cuda:0")
+    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.sm,clocks.max.sm", "--format=csv,noheader"],
+                       capture_output=True, text=True).stdout.strip()
+    print(f"device: {torch.cuda.get_device_name(dev)} | nvidia-smi name, power limit, SM clock, max SM clock: {q}")
+    new_path = capi.LIB_PATH
+    libs = {"base": load(os.path.abspath(args.base_lib)), "this": load(new_path)}
+    ls = layers(dev, args.batch)
+    times = {(n, k): [] for n, *_ in ls for k in libs}
+    same = {}
+    for name, run, *_ in ls:                      # warm up both builds on every shape; compare their outputs
+        res = {}
+        for k, h in libs.items():
+            capi._lib = h
+            for _ in range(2):
+                y = run()
+            torch.cuda.synchronize()
+            res[k] = y.clone()
+        same[name] = bool(torch.equal(res["base"], res["this"])), float((res["base"].float() - res["this"].float()).abs().max())
+    for _ in range(args.rounds):
+        for name, run, *_ in ls:
+            for k, h in libs.items():
+                capi._lib = h
+                times[(name, k)].append(time_ms(run, args.reps))
+    capi._lib = libs["this"]
+    med = lambda v: sorted(v)[len(v) // 2]
+    span = lambda v: f"{med(v):.3f} [{min(v):.3f}-{max(v):.3f}]"
+    print(f"{'layer':34s} {'base ms [min-max]':>24s} {'this ms [min-max]':>24s} {'base TF/s':>9s} {'this TF/s':>9s} {'/989':>5s} "
+          f"{'speedup':>7s} {'bitwise':>8s} {'smem KB':>9s} {'L2 KB':>6s}")
+    for name, run, fl, cm, launches in ls:
+        tb, tt = times[(name, "base")], times[(name, "this")]
+        s_old, s_new, l2 = kblock_bytes(cm, 32 if launches else 64)   # the pair kernel issued 64-column MMAs before
+        diff = "same" if same[name][0] else f"{same[name][1]:.1e}"
+        print(f"{name:34s} {span(tb):>24s} {span(tt):>24s} {fl / med(tb) / 1e9:9.1f} {fl / med(tt) / 1e9:9.1f} "
+              f"{fl / (med(tt) * 1e-3) / PEAK:5.2f} {med(tb) / med(tt):7.3f} {diff:>8s} {f'{s_old // 1024}->{s_new // 1024}':>9s} {l2 // 1024:6d}")
+
+
+if __name__ == "__main__":
+    main()
