@@ -5,10 +5,13 @@ per agent group) for two builds of liblavb200.so.
 
 Both libraries are loaded into one process; the rounds alternate base / this tree's build on the same inputs and weights.
 For every layer it prints the median kernel time (CUDA events over `reps` back-to-back launches), the GEMM rate and its
-fraction of the 989 TFLOP/s dense fp16 peak, whether the two builds' outputs are bit-identical, and two byte counts derived
-from the shapes for one 64-deep K-block of one CTA (128 pixels x cout_mma):
-  smem/KB : shared-memory operand bytes the MMAs read (A once per wgmma, B once per warpgroup), base -> this tree
-  L2/KB   : bytes the TMA moves from L2 into shared memory (A box + B box)
+fraction of the 989 TFLOP/s dense fp16 peak, whether the two builds' outputs are bit-identical (else the largest difference
+relative to the output's scale), and byte counts derived from the shapes:
+  smem KB  : shared-memory operand bytes the MMAs read per 64-deep K-block of one CTA (conv_umma: 128 pixels x cout_mma)
+  fill KB  : bytes the TMA moves from L2 into shared memory per tile (conv_umma: one A and one B box per tap and chunk;
+             stem: one pixel box per tap (base) -> one per kernel row and kx parity (this tree))
+  fill TB/s: all tiles' fill bytes of this tree over its median time
+The planner stem (conv7x7s2_umma, 128 and 9 crops of 96 x 96 x 384) is timed the same way.
 The card name, power limit and SM clocks are read in the same run.
 """
 import argparse
@@ -30,7 +33,8 @@ def load(path):
 
 
 def layers(dev, B):
-    """(name, run() -> output, GEMM flop, cout_mma, [(cin, ntaps) per launch])"""
+    """(name, run() -> output, GEMM flop, cout_mma, [(cin, ntaps, tiles) per launch] or None for the pair kernel,
+    or ("stem", crops, cin, tiles))"""
     g = torch.Generator(device=dev).manual_seed(0)
     rn = lambda *s: torch.randn(*s, device=dev, generator=g)
     h16 = ops.h16()
@@ -46,7 +50,10 @@ def layers(dev, B):
         for ph in layer.phases:
             (osy, osx), (ooy, oox) = ph["out_s"], ph["out_o"]
             fl += 2 * n * ((ho - ooy + osy - 1) // osy) * ((wo - oox + osx - 1) // osx) * cin * len(ph["taps"]) * layer.cout
-        out.append((name, lambda: layer(x, out=y), fl, (cout + 31) // 32 * 32, [(cin, len(ph["taps"])) for ph in layer.phases]))
+        tiles = lambda ph: n * -(-((ho - ph["out_o"][0] + ph["out_s"][0] - 1) // ph["out_s"][0]) // 8) * \
+            -(-((wo - ph["out_o"][1] + ph["out_s"][1] - 1) // ph["out_s"][1]) // 16)
+        out.append((name, lambda: layer(x, out=y), fl, (cout + 31) // 32 * 32,
+                    [(cin, len(ph["taps"]), tiles(ph)) for ph in layer.phases]))
 
     bn = lambda c: dict(pre_relu=True, scale=rn(c).abs() + 0.5, shift=rn(c) * 0.1)
     tap("heads 384->256 160x160", B, 160, 160, 384, 256, 3, **bn(256))
@@ -75,7 +82,20 @@ def layers(dev, B):
                           bias=b32, sigmoid=gi == 3, umma=True, d2s_nout=no)
         return torch.cat([h[4].flatten() for h in heads])
 
-    out.append(("head outputs 4x(64->32 2x2 d2s)", d2s, 4 * 2 * B * 160 * 160 * 64 * 4 * 32, 32, [(64, 4)] * 4))
+    out.append(("head outputs 4x(64->32 2x2 d2s)", d2s, 4 * 2 * B * 160 * 160 * 64 * 4 * 32, 32,
+                [(64, 4, B * 20 * 10)] * 4))
+
+    # the planner embedder's 7x7 / s2 stem: 4 crops per agent (ego + K = 3 vehicles) -> 128 crops, and the batch-1 leg's 9
+    def stem(name, crops):
+        x = rn(crops, 96, 96, 384).to(h16)
+        wp = ops.pack_conv7x7s2_weights(rn(64, 384, 7, 7) / (49 * 384) ** 0.5)
+        b = rn(64) * 0.1
+        y = torch.empty(crops, 48, 48, 64, device=dev, dtype=h16)
+        out.append((name, lambda: ops.conv7x7s2_umma(x, wp, b, out=y), 2 * crops * 48 * 48 * 64 * 384 * 49, 64,
+                    ("stem", crops, 384, crops * 9)))
+
+    stem(f"planner stem {4 * B} crops 96x96x384", 4 * B)
+    stem("planner stem 9 crops 96x96x384", 9)
 
     # the fused ERFNet (3x1 -> 1x3) pairs (conv_pair_umma_kernel): 64 channels at 72 x 64, 128 channels at 36 x 32 (dilation 2)
     def pair(name, n, h, w, c, dil):
@@ -88,6 +108,18 @@ def layers(dev, B):
     pair("erf pair 64 72x64 (fused 3x1,1x3)", 3 * B, 72, 64, 64, 1)
     pair("erf pair 128 36x32 d2 (fused)", 3 * B, 36, 32, 128, 2)
     return out
+
+
+def fill_bytes_per_tile(cin, ntaps, cout_mma):
+    """TMA bytes from L2 into shared memory for one 8 x 16 tile of conv_umma: per 64-channel chunk and tap one A box of
+    8 x 16 pixels x 128 B and one B box of cout_mma x 128 B"""
+    return cin // 64 * ntaps * (8 * 16 * 128 + cout_mma * 128)
+
+
+def stem_fill_bytes_per_tile(cin, grouped):
+    """the same for one 16 x 16 tile of conv7x7s2_umma: 49 weight boxes of 8 KB plus 49 pixel boxes of 16 x 16 x 128 B
+    (one per tap) or 14 of 19 x 16 x 128 B (one per kernel row and kx parity)"""
+    return cin // 64 * (49 * 8192 + (14 * 19 if grouped else 49 * 16) * 16 * 128)
 
 
 def kblock_bytes(cout_mma, old_width=32):
@@ -134,7 +166,8 @@ def main():
                 y = run()
             torch.cuda.synchronize()
             res[k] = y.clone()
-        same[name] = bool(torch.equal(res["base"], res["this"])), float((res["base"].float() - res["this"].float()).abs().max())
+        same[name] = (bool(torch.equal(res["base"], res["this"])),
+                      float((res["base"].float() - res["this"].float()).abs().max() / res["base"].float().abs().max()))
     for _ in range(args.rounds):
         for name, run, *_ in ls:
             for k, h in libs.items():
@@ -144,13 +177,24 @@ def main():
     med = lambda v: sorted(v)[len(v) // 2]
     span = lambda v: f"{med(v):.3f} [{min(v):.3f}-{max(v):.3f}]"
     print(f"{'layer':34s} {'base ms [min-max]':>24s} {'this ms [min-max]':>24s} {'base TF/s':>9s} {'this TF/s':>9s} {'/989':>5s} "
-          f"{'speedup':>7s} {'bitwise':>8s} {'smem KB':>9s} {'L2 KB':>6s}")
+          f"{'speedup':>7s} {'bitwise':>8s} {'smem KB':>7s} {'fill KB/tile':>13s} {'fill TB/s':>9s}")
     for name, run, fl, cm, launches in ls:
         tb, tt = times[(name, "base")], times[(name, "this")]
-        s_old, s_new, l2 = kblock_bytes(cm, 32 if launches else 64)   # the pair kernel issued 64-column MMAs before
         diff = "same" if same[name][0] else f"{same[name][1]:.1e}"
+        if launches is None:                       # fused pair kernel: no tap boxes
+            s_new, fill, rate = kblock_bytes(cm, 64)[1] // 1024, "-", "-"
+        elif launches[0] == "stem":
+            _, crops, cin, tiles = launches
+            f0, f1 = stem_fill_bytes_per_tile(cin, False), stem_fill_bytes_per_tile(cin, True)
+            s_new, fill, rate = (8192 + 16384) * 2 // 1024, f"{f0 // 1024}->{f1 // 1024}", f"{tiles * f1 / (med(tt) * 1e-3) / 1e12:.2f}"
+        else:
+            s_new = kblock_bytes(cm)[1] // 1024
+            f1 = [fill_bytes_per_tile(ci, nt, cm) for ci, nt, _ in launches]
+            total = sum(f * t for f, (*_, t) in zip(f1, launches))
+            fill = f"{f1[0] // 1024}" + ("" if len(set(f1)) == 1 else f" ({len(f1)} launches)")
+            rate = f"{total / (med(tt) * 1e-3) / 1e12:.2f}"
         print(f"{name:34s} {span(tb):>24s} {span(tt):>24s} {fl / med(tb) / 1e9:9.1f} {fl / med(tt) / 1e9:9.1f} "
-              f"{fl / (med(tt) * 1e-3) / PEAK:5.2f} {med(tb) / med(tt):7.3f} {diff:>8s} {f'{s_old // 1024}->{s_new // 1024}':>9s} {l2 // 1024:6d}")
+              f"{fl / (med(tt) * 1e-3) / PEAK:5.2f} {med(tb) / med(tt):7.3f} {diff:>8s} {s_new:7d} {fill:>13s} {rate:>9s}")
 
 
 if __name__ == "__main__":
