@@ -328,7 +328,8 @@ int lavb_conv7x7s2_umma(const void* d_in, int n, int h, int w, int cin, const vo
  * bias1 / shift2 (fp32 [c]) are added to the register accumulators in the epilogues, which then pack, clamp and add the residual
  * (16-bit packed arithmetic: the residual add rounds once more than an fp32 add would, and its sum saturates at +-65504).
  * in / out / res: h16 NHWC (n, h, w, c) contiguous, c in {64, 128}, w in {32, 64, 128}; w1 / w2: h16 [3 taps][c out][c in];
- * res may be NULL. */
+ * res may be NULL.  out must not overlap in or res (rejected): the kernel reads a tile's residual while earlier tiles are
+ * still being stored. */
 typedef struct lavb_conv_pair_desc {
   const void* in; void* out; const void* res;
   int n, h, w, c, dil, post_relu;

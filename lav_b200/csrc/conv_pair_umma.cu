@@ -10,9 +10,13 @@
 //               shifted by +d, 0, -d pixels inside each image row (rows that fall off the image border stay zero), i.e. the
 //               three A operands of the horizontal taps
 //   stage 2: wgmma over the 3 horizontal taps (A = those copies, B = W2 blocks through the same TMA ring)
-//   epilogue 2: acc2 + shift2 -> h16 -> (+ residual, ReLU as one packed fma.relu) -> NHWC.  The BatchNorm scale is folded into W2 by the caller.
+//   epilogue 2: acc2 + shift2 -> h16 (+ residual, ReLU as one packed fma.relu), written in place over the residual tile in a
+//               ring slot and stored to NHWC by one TMA store per 64 channels.  The BatchNorm scale is folded into W2 by the caller.
 // Warp roles: warps 0-3 and 4-7 are two consumer warpgroups (tile pixels 0-63 / 64-127), warp 8 is the TMA producer; persistent
-// over tiles.  With C = 64 two CTAs share an SM, so one CTA's epilogues overlap the other's MMAs.
+// over tiles.  Ring order per tile: stage-1 fills (A + W1), stage-2 fills (W2 only), then the tile's output slot, which the
+// producer fills with the residual tile (rows past the image zero-filled) ahead of stage 2, so epilogue 2 reads it from shared
+// memory; the slot is released once the TMA store has read it, and the store clips rows past the image.  With C = 64 two
+// CTAs share an SM, so one CTA's epilogues overlap the other's MMAs.
 #include <stdlib.h>
 #include "sm90.cuh"
 
@@ -26,7 +30,7 @@ constexpr int kPairThreads = 288;
 
 struct PairArgs {
   int n, h, w, c, kchunks, dil, tile_w, tile_h, tiles_per_img, num_tiles, stages, post_relu;
-  h16* out; const h16* res;
+  const h16* res;                          // only tested for null: the residual tile arrives by TMA
   const float* bias1; const float* shift2;
   long long* trace; int trace_tiles;      // profiling aid (lavb_conv_pair_set_trace): per-CTA, per-tile clock64 stamps, or null
 };
@@ -60,6 +64,8 @@ template <int kC>
 __global__ void __launch_bounds__(kPairThreads, kC == 64 ? 2 : 1) conv_pair_umma_kernel(const __grid_constant__ CUtensorMap tmap_a,
                                                                                        const __grid_constant__ CUtensorMap tmap_w1,
                                                                                        const __grid_constant__ CUtensorMap tmap_w2,
+                                                                                       const __grid_constant__ CUtensorMap tmap_r,
+                                                                                       const __grid_constant__ CUtensorMap tmap_o,
                                                                                        const __grid_constant__ PairArgs p) {
   constexpr int kNC = kC / 64;                                      // 64-column MMA chunks
   constexpr int kChunks = kC / kBlockK;                             // K-blocks per tap
@@ -67,7 +73,9 @@ __global__ void __launch_bounds__(kPairThreads, kC == 64 ? 2 : 1) conv_pair_umma
   constexpr int kSlotBytes = kABytes + kWBytes;
   constexpr int kNkb = 3 * kChunks;                                 // K-blocks per stage
   constexpr int kBpf = kSlotBytes / kWBytes;                        // W2 K-blocks per ring slot in stage 2
+  constexpr int kOutBytes = kChunks * kABytes;                      // one tile of the residual / output: 128 px x c x 2 B
   static_assert(kNkb % kBpf == 0, "stage 2 fills whole ring slots");
+  static_assert(kOutBytes <= kSlotBytes, "the residual / output tile fits one ring slot");
   extern __shared__ uint8_t smem_raw[];
   const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;     // SWIZZLE_128B operands need 1024 B alignment
   uint8_t* gen = smem_raw + (base - smem_u32(smem_raw));
@@ -83,6 +91,8 @@ __global__ void __launch_bounds__(kPairThreads, kC == 64 ? 2 : 1) conv_pair_umma
     asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmap_a)) : "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmap_w1)) : "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmap_w2)) : "memory");
+    asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmap_r)) : "memory");
+    asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmap_o)) : "memory");
     for (int s = 0; s < p.stages; ++s) { mbar_init(full_bar + 8 * s, 1); mbar_init(empty_bar + 8 * s, 8); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
@@ -99,8 +109,9 @@ __global__ void __launch_bounds__(kPairThreads, kC == 64 ? 2 : 1) conv_pair_umma
   if (warp == 8) {
     if (lane == 0) {
       int slot = 0; uint32_t phase = 0;
-      // ring order = consumption order: stage 1 of a tile (A + W1 per K-block), then its stage 2.  Stage 2 needs only weights:
-      // a ring slot (A part + W part) takes kBpf whole W2 K-blocks, so the stage is 1 fill (c = 64) or 3 fills (c = 128)
+      // ring order = consumption order, per tile: stage 1 (A + W1 per K-block); stage 2, which needs only weights: a ring slot
+      // (A part + W part) takes kBpf whole W2 K-blocks, so the stage is 1 fill (c = 64) or 3 fills (c = 128); then the tile's
+      // output slot, filled with the residual tile (or, without a residual, just marked full), where epilogue 2 stages the output
       for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
         const int img = tile / p.tiles_per_img, y0 = (tile - img * p.tiles_per_img) * p.tile_h;
         for (int t = 0; t < 3; ++t)
@@ -122,6 +133,15 @@ __global__ void __launch_bounds__(kPairThreads, kC == 64 ? 2 : 1) conv_pair_umma
           }
           if (++slot == p.stages) { slot = 0; phase ^= 1; }
         }
+        mbar_wait(empty_bar + 8 * slot, phase ^ 1);
+        if (p.res) {                                 // rows past the image are zero-filled (and never stored)
+          mbar_expect_tx(full_bar + 8 * slot, kOutBytes);
+          for (int kc = 0; kc < kChunks; ++kc)
+            tma_load_4d(base + slot * kSlotBytes + kc * kABytes, &tmap_r, full_bar + 8 * slot, kc * kBlockK, 0, y0, img);
+        } else {
+          mbar_arrive(full_bar + 8 * slot);
+        }
+        if (++slot == p.stages) { slot = 0; phase ^= 1; }
       }
     }
     return;
@@ -205,27 +225,38 @@ __global__ void __launch_bounds__(kPairThreads, kC == 64 ? 2 : 1) conv_pair_umma
     sm90::acc_fence(acc);
     if (lane == 0) mbar_arrive(empty_bar + 8 * prev);
     PAIR_STAMP(2, i);
-    // ---- epilogue 2: acc2 + shift2 -> h16 (+ residual) -> ReLU -> NHWC
+    const int out_slot = slot; const uint32_t out_phase = phase;
+    if (++slot == p.stages) { slot = 0; phase ^= 1; }
+    // ---- epilogue 2: acc2 + shift2 -> h16 (+ residual) -> ReLU, staged in the output slot in the input's layout, one TMA store
+    mbar_wait(full_bar + 8 * out_slot, out_phase);
+    uint8_t* outp = gen + out_slot * kSlotBytes;
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
       const int m = 64 * wg + 16 * (warp & 3) + (lane >> 2) + 8 * h;
-      const int py = m / p.tile_w, px = m - py * p.tile_w, y = y0 + py;
-      if (y >= p.h) continue;
-      const long long pix = ((long long)img * p.h + y) * p.w + px;
 #pragma unroll
       for (int cc = 0; cc < kNC; ++cc)
 #pragma unroll
         for (int j = 0; j < 8; ++j) {
           const int col = 64 * cc + 8 * j + 2 * (lane & 3);
           const float2 t = *reinterpret_cast<const float2*>(ep_t2 + col);
+          uint32_t* o = reinterpret_cast<uint32_t*>(outp + cc * kABytes + m * 128 + ((j ^ (m & 7)) << 4) + (col & 7) * 2);
           uint32_t v = pack_h16(acc[32 * cc + 4 * j + 2 * h] + t.x, acc[32 * cc + 4 * j + 2 * h + 1] + t.y);
-          if (p.res) v = add2(v, __ldg(reinterpret_cast<const uint32_t*>(p.res + pix * kC + col)), relu_out);
+          if (p.res) v = add2(v, *o, relu_out);
           else if (relu_out) v = relu2(v);
-          *reinterpret_cast<uint32_t*>(p.out + pix * kC + col) = v;
+          *o = v;
         }
+    }
+    proxy_fence_async();                             // the TMA store reads what these threads wrote
+    sm90::bar_sync(1, 256);
+    if (threadIdx.x == 0) {                          // rows past the image are clipped by the tensor map
+      for (int kc = 0; kc < kChunks; ++kc) tma_store_4d(&tmap_o, base + out_slot * kSlotBytes + kc * kABytes, kc * kBlockK, 0, y0, img);
+      bulk_commit();
+      bulk_wait_read<0>();
+      mbar_arrive(empty_bar + 8 * out_slot, 8);      // the slot is free once the store has read it
     }
     PAIR_STAMP(3, i);
   }
+  if (threadIdx.x == 0) bulk_wait<0>();              // the last stores have landed before the CTA retires
 }
 
 }  // namespace pair
@@ -249,6 +280,14 @@ extern "C" int lavb_conv_pair_umma(const lavb_conv_pair_desc* d, void* stream) {
   LAVB_CHECK_ARG(d->dil >= 1 && d->dil < d->w, "conv_pair_umma: dilation must be in [1, width)");
   LAVB_CHECK_ARG(d->n >= 0 && d->h >= 1, "conv_pair_umma: bad shape");
   LAVB_CHECK_ARG(d->w1 && d->w2 && d->bias1 && d->in && d->out, "conv_pair_umma: null operand");
+  {  // the residual tile is prefetched while earlier tiles are stored: `out` must not overlap `in` or `res`
+    const size_t bytes = (size_t)d->n * d->h * d->w * d->c * 2;
+    const auto overlap = [&](const void* x) {
+      const char *o = static_cast<const char*>(d->out), *q = static_cast<const char*>(x);
+      return x && o < q + bytes && q < o + bytes;
+    };
+    LAVB_CHECK_ARG(!overlap(d->in) && !overlap(d->res), "conv_pair_umma: out must not overlap in or res");
+  }
   if (d->n == 0) return 0;
   auto encode = get_encode();
   LAVB_CHECK_ARG(encode != nullptr, "conv_pair_umma: cuTensorMapEncodeTiled not available from the driver");
@@ -259,7 +298,7 @@ extern "C" int lavb_conv_pair_umma(const lavb_conv_pair_desc* d, void* stream) {
   a.tiles_per_img = ceil_div(d->h, a.tile_h);
   a.num_tiles = d->n * a.tiles_per_img;
   a.post_relu = d->post_relu;
-  a.out = reinterpret_cast<h16*>(d->out); a.res = reinterpret_cast<const h16*>(d->res);
+  a.res = reinterpret_cast<const h16*>(d->res);
   a.bias1 = d->bias1; a.shift2 = d->shift2;
   a.trace = g_pair_trace; a.trace_tiles = g_pair_trace_tiles;
   const int slot_bytes = kABytes + d->c * kBlockK * 2;
@@ -270,17 +309,22 @@ extern "C" int lavb_conv_pair_umma(const lavb_conv_pair_desc* d, void* stream) {
   const int smem_cap = two ? 113 * 1024 : 227 * 1024;
   a.stages = min(kMaxStages, (smem_cap - mid_bytes - ctrl_bytes) / slot_bytes);
   const int smem = a.stages * slot_bytes + mid_bytes + ctrl_bytes;
-  CUtensorMap tmap_a, tmap_w1, tmap_w2;
-  {
+  CUtensorMap tmap_a, tmap_w1, tmap_w2, tmap_r, tmap_o;
+  // input, residual and output: one geometry, boxes of 64 channels x one tile of full rows
+  const auto encode_act = [&](CUtensorMap* m, const void* ptr) {
     cuuint64_t dims[4] = {(cuuint64_t)d->c, (cuuint64_t)d->w, (cuuint64_t)d->h, (cuuint64_t)d->n};
     cuuint64_t strides[3] = {(cuuint64_t)d->c * 2, (cuuint64_t)d->w * d->c * 2, (cuuint64_t)d->h * d->w * d->c * 2};
     cuuint32_t box[4] = {(cuuint32_t)kBlockK, (cuuint32_t)a.tile_w, (cuuint32_t)a.tile_h, 1};
     cuuint32_t estr[4] = {1, 1, 1, 1};
-    CUresult r = encode(&tmap_a, LAVB_TMAP_H16, 4, const_cast<void*>(d->in), dims, strides, box, estr,
-                        CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                        CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    LAVB_CHECK_ARG(r == CUDA_SUCCESS, "conv_pair_umma: cuTensorMapEncodeTiled(A) failed with %d", (int)r);
-  }
+    return encode(m, LAVB_TMAP_H16, 4, const_cast<void*>(ptr), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                  CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  };
+  CUresult r = encode_act(&tmap_a, d->in);
+  LAVB_CHECK_ARG(r == CUDA_SUCCESS, "conv_pair_umma: cuTensorMapEncodeTiled(in) failed with %d", (int)r);
+  r = encode_act(&tmap_r, d->res ? d->res : d->in);           // without a residual the map is never read
+  LAVB_CHECK_ARG(r == CUDA_SUCCESS, "conv_pair_umma: cuTensorMapEncodeTiled(res) failed with %d", (int)r);
+  r = encode_act(&tmap_o, d->out);
+  LAVB_CHECK_ARG(r == CUDA_SUCCESS, "conv_pair_umma: cuTensorMapEncodeTiled(out) failed with %d", (int)r);
   for (int which = 0; which < 2; ++which) {
     cuuint64_t dims[2] = {(cuuint64_t)d->c, (cuuint64_t)3 * d->c};
     cuuint64_t strides[1] = {(cuuint64_t)d->c * 2};
@@ -293,10 +337,10 @@ extern "C" int lavb_conv_pair_umma(const lavb_conv_pair_desc* d, void* stream) {
   }
   if (two) {
     LAVB_CUDA_OK(ensure_dyn_smem((const void*)conv_pair_umma_kernel<64>, smem_cap));
-    conv_pair_umma_kernel<64><<<min(a.num_tiles, 2 * kNumSMs), kPairThreads, smem, (cudaStream_t)stream>>>(tmap_a, tmap_w1, tmap_w2, a);
+    conv_pair_umma_kernel<64><<<min(a.num_tiles, 2 * kNumSMs), kPairThreads, smem, (cudaStream_t)stream>>>(tmap_a, tmap_w1, tmap_w2, tmap_r, tmap_o, a);
   } else {
     LAVB_CUDA_OK(ensure_dyn_smem((const void*)conv_pair_umma_kernel<128>, smem_cap));
-    conv_pair_umma_kernel<128><<<min(a.num_tiles, kNumSMs), kPairThreads, smem, (cudaStream_t)stream>>>(tmap_a, tmap_w1, tmap_w2, a);
+    conv_pair_umma_kernel<128><<<min(a.num_tiles, kNumSMs), kPairThreads, smem, (cudaStream_t)stream>>>(tmap_a, tmap_w1, tmap_w2, tmap_r, tmap_o, a);
   }
   LAVB_LAUNCH_OK();
   return 0;

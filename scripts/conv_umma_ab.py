@@ -11,7 +11,8 @@ relative to the output's scale), and byte counts derived from the shapes:
   fill KB  : bytes the TMA moves from L2 into shared memory per tile (conv_umma: one A and one B box per tap and chunk;
              stem: one pixel box per tap (base) -> one per kernel row and kx parity (this tree))
   fill TB/s: all tiles' fill bytes of this tree over its median time
-The planner stem (conv7x7s2_umma, 128 and 9 crops of 96 x 96 x 384) is timed the same way.
+The planner stem (conv7x7s2_umma, 128 and 9 crops of 96 x 96 x 384) is timed the same way, and so is every shape of the fused
+ERFNet pair a tick runs; the last line sums the pair times at their launch counts per tick.
 The card name, power limit and SM clocks are read in the same run.
 """
 import argparse
@@ -97,17 +98,27 @@ def layers(dev, B):
     stem(f"planner stem {4 * B} crops 96x96x384", 4 * B)
     stem("planner stem 9 crops 96x96x384", 9)
 
-    # the fused ERFNet (3x1 -> 1x3) pairs (conv_pair_umma_kernel): 64 channels at 72 x 64, 128 channels at 36 x 32 (dilation 2)
-    def pair(name, n, h, w, c, dil):
-        x = rn(n, h, w, c).to(h16)
+    # the fused ERFNet (3x1 -> 1x3) pairs (conv_pair_umma_kernel), every shape a tick runs, with its launch count per tick:
+    # each non_bottleneck_1d block is a dilation-1 pair without the residual, then a dilation-d pair with it
+    for c, h, w, dil, res, count in PAIR_SHAPES:
+        x = rn(3 * B, h, w, c).to(h16)
+        r = rn(3 * B, h, w, c).to(h16) if res else None
         w1, w2 = ((rn(3, c, c) / (3 * c) ** 0.5).to(h16).contiguous() for _ in range(2))
         b1, t2 = rn(c) * 0.1, rn(c) * 0.1
-        y = torch.empty(n, h, w, c, device=dev, dtype=h16)
-        out.append((name, lambda: ops.conv_pair_umma(x, w1, b1, w2, t2, dil, res=x, out=y), 2 * 2 * n * h * w * c * c * 3, c, None))
-
-    pair("erf pair 64 72x64 (fused 3x1,1x3)", 3 * B, 72, 64, 64, 1)
-    pair("erf pair 128 36x32 d2 (fused)", 3 * B, 36, 32, 128, 2)
+        y = torch.empty(3 * B, h, w, c, device=dev, dtype=h16)
+        out.append((pair_name(c, h, w, dil, res, count),
+                    lambda x=x, r=r, w1=w1, w2=w2, b1=b1, t2=t2, y=y, dil=dil: ops.conv_pair_umma(x, w1, b1, w2, t2, dil, res=r, out=y),
+                    2 * 2 * 3 * B * h * w * c * c * 3, c, None))
     return out
+
+
+# (c, h, w, dilation, residual, launches per tick): 7 blocks of 64 channels at 72 x 64, 8 of 128 channels at 36 x 32
+PAIR_SHAPES = [(64, 72, 64, 1, False, 7), (64, 72, 64, 1, True, 7), (128, 36, 32, 1, False, 8),
+               (128, 36, 32, 2, True, 2), (128, 36, 32, 4, True, 2), (128, 36, 32, 8, True, 2), (128, 36, 32, 16, True, 2)]
+
+
+def pair_name(c, h, w, dil, res, count):
+    return f"erf pair {c} {h}x{w} d{dil}{' +res' if res else ''} x{count}"
 
 
 def fill_bytes_per_tile(cin, ntaps, cout_mma):
@@ -195,6 +206,10 @@ def main():
             rate = f"{total / (med(tt) * 1e-3) / 1e12:.2f}"
         print(f"{name:34s} {span(tb):>24s} {span(tt):>24s} {fl / med(tb) / 1e9:9.1f} {fl / med(tt) / 1e9:9.1f} "
               f"{fl / (med(tt) * 1e-3) / PEAK:5.2f} {med(tb) / med(tt):7.3f} {diff:>8s} {s_new:7d} {fill:>13s} {rate:>9s}")
+    # all pair launches of one tick: each round's per-shape times weighted by the launch counts, median over rounds
+    tick = {k: [sum(s[5] * times[(pair_name(*s), k)][r] for s in PAIR_SHAPES) for r in range(args.rounds)] for k in libs}
+    print(f"{'erf pairs, one tick (' + str(sum(s[5] for s in PAIR_SHAPES)) + ' launches)':34s} {span(tick['base']):>24s} "
+          f"{span(tick['this']):>24s} {'':9s} {'':9s} {'':5s} {med(tick['base']) / med(tick['this']):7.3f}")
 
 
 if __name__ == "__main__":
