@@ -159,9 +159,8 @@ int lavb_pillar_forward(const float* d_pts, int pt_stride, int d,
 
 /* Sorted, atomic-free variant for the tensor-core pipeline (the product encoder): counting sort of the points by canvas cell,
  * layer 1 on hi/lo-split h16 operands (~ fp32), layer 2 on h16 operands with fp32 accumulation (mma.sync), one canvas row written
- * per pillar and the rows of empty cells zero-filled by the scan pass.  out_mode 0: fp32 canvas [B][ny][nx][h2]; 1: h16 canvas
- * [B][ny][nx][hi(h2) | lo(h2)] (the error-free split lavb_split_h16 produces); 2: h16 canvas [B][ny][nx][h2].  Same semantics
- * otherwise. */
+ * per pillar and the rows of empty cells zero-filled by the scan pass.  out_mode 0: fp32 canvas [B][ny][nx][h2]; 2: h16 canvas
+ * [B][ny][nx][h2], saturating; any other out_mode is rejected.  Same semantics otherwise. */
 size_t lavb_pillar_sorted_workspace_bytes(int batch, int nx, int ny, long long total_points);
 int lavb_pillar_forward_sorted(const float* d_pts, int pt_stride, int d,
                                const long long* h_cloud_start, const int* h_cloud_count, int batch,
@@ -169,18 +168,6 @@ int lavb_pillar_forward_sorted(const float* d_pts, int pt_stride, int d,
                                const float* d_w1, const float* d_s1, const float* d_t1, int h1,
                                const float* d_w2, const float* d_s2, const float* d_t2, int h2,
                                void* d_canvas, int out_mode, void* d_workspace, void* stream);
-
-/* Tile-binned variant (the 16-bit pipeline's encoder): the points are binned by canvas tile (8 x 16 cells) into 48-byte records and
- * one CTA produces each tile start to finish in shared memory — per-pillar centroids, decorate, layer 1 (hi/lo-split MMAs ~ fp32),
- * layer 2 (h16 MMAs), max-pool by shared-memory atomics — and writes it, zeros included, as full 256-byte cell rows.  Same
- * arguments, semantics and out_mode as lavb_pillar_forward_sorted; no per-cell global arrays, no canvas zero-fill pass. */
-size_t lavb_pillar_tiled_workspace_bytes(int batch, int nx, int ny, long long total_points);
-int lavb_pillar_forward_tiled(const float* d_pts, int pt_stride, int d,
-                              const long long* h_cloud_start, const int* h_cloud_count, int batch,
-                              float min_x, float max_x, float min_y, float max_y, float ppm, int nx, int ny,
-                              const float* d_w1, const float* d_s1, const float* d_t1, int h1,
-                              const float* d_w2, const float* d_s2, const float* d_t2, int h2,
-                              void* d_canvas, int out_mode, void* d_workspace, void* stream);
 
 /* training-mode pieces (BatchNorm1d batch statistics over all in-window points, arg-routed backward).
  * stage 0: voxelise + decorate -> d_feat [M][d+5] (M = number of in-window points, returned in *h_m),
@@ -297,9 +284,6 @@ int lavb_crop_bilinear_bwd(const float* d_gout, int b, int h, int w, int c, cons
                            int k, int crop, float* d_gfeat, void* stream);
 
 /* dtype / layout helpers */
-/* fp32 [rows][c] -> h16 [rows][hi(c) | lo(c)] with hi = h16(x), lo = h16(x - hi) (error-free split of the canvas so the
- * first tensor-core conv sees ~fp32 input precision; its weights are duplicated along cin by the host). */
-int lavb_split_h16(const float* d_src, void* d_dst, long long rows, int c, void* stream);
 int lavb_convert(const void* d_src, int src_dtype, void* d_dst, int dst_dtype, long long count, void* stream);
 
 /* ---------------------------------------------------------------- wgmma implicit-GEMM tap-list convolution
@@ -364,15 +348,6 @@ int lavb_erf_down16(const void* d_in, void* d_out, int n, int h, int w, const fl
  * [4 convs][3 taps][16 cin][16 cout]; d_st: fp32 [4 convs][16 cout][2] = (scale, shift) with epi(a) = relu(a * scale + shift)
  * (conv bias folded into shift; scale = 1 for the two convs that have no BatchNorm). */
 int lavb_erf_nb16(const void* d_in, void* d_out, int n, int h, int w, const float* d_w4, const float* d_st, void* stream);
-
-/* ---------------------------------------------------------------- cluster-persistent GRU roll-out
- * replaces: one call of plan_gru = nn.GRU(4, 512, batch_first=True) (team_code_v2/models/uniplanner.py:45,247-259;
- * lav/models/bev_planner_v2.py) over `steps` time steps for `nseq` sequences.
- * d_u (nseq, steps, 4) fp32; d_h0 (nseq, 512) fp32; d_whh = weight_hh_l0 (1536, 512) fp32; d_wih = weight_ih_l0
- * (1536, 4), d_bih / d_bhh (1536,) fp32; d_out (nseq, steps, 512) fp32 = the GRU's output sequence.
- * fp32-class arithmetic: the recurrent product runs on the 16-bit tensor cores with both operands split into hi + lo parts. */
-int lavb_gru_h512(const float* d_u, const float* d_h0, const float* d_whh, const float* d_wih, const float* d_bih,
-                  const float* d_bhh, float* d_out, int nseq, int steps, void* stream);
 
 /* ---------------------------------------------------------------- motion-forecast ("cast") heads in one launch
  * replaces: UniPlanner.cast / BEVPlanner.cast (team_code_v2/models/uniplanner.py:286-301, lav/models/bev_planner_v2.py:226-236):

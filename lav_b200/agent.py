@@ -22,8 +22,6 @@ from .model_inference import InferModel
 FUSE_SEG_HEAD = True  # ERFNet's last layer (ConvTranspose2d 16->5, k2 s2) + softmax evaluated inside the painting gather
 FORK_BRAKE = True     # run the brake predictor as a parallel branch of the perception graph
 STEM_U8 = True        # brake-model stem (7x7 s2 on 3 channels) in the lav_b200 kernel, straight from the camera bytes
-UMMA_TRUNKS = os.environ.get("LAVB_UMMA_TRUNKS", "0") == "1"   # ResNet-18 trunks (brake / planner embedder) on the wgmma conv kernel: correct (tested) but measured
-                      # 3 % slower end to end than the BN-folded cuDNN path (H100, bench B = 64), so cuDNN stays the default
 NUM_REPEAT = 4
 GAP = NUM_REPEAT + 1          # lav_agent_fast.py:31-32
 NUM_FRAME_STACK = 2           # team_code_v2/config.yaml: num_frame_stack
@@ -87,13 +85,11 @@ class FramePipeline:
         dt = ops.h16() if precision == "f16" else torch.float32
         up = copy.deepcopy(self._src_uniplanner)
         up.lidar_conv_emb.to(dt).to(memory_format=torch.channels_last)
-        up.lidar_conv_emb[0].use_umma_trunk = (precision == "f16") and UMMA_TRUNKS
         self.infer_model = InferModel(self._lidar_model, up, self._cam[0], self._cam[1], self.device)
         if self._src_bra is not None:
             bra = copy.deepcopy(self._src_bra)
             bra.conv_backbone.to(dt).to(memory_format=torch.channels_last)
             bra.attn1.to(dt); bra.attn2.to(dt)
-            bra.conv_backbone.use_umma_trunk = (precision == "f16") and UMMA_TRUNKS
             self.bra_model = bra
         return self
 

@@ -75,11 +75,6 @@ _SIGS = {
                                              C.c_float, C.c_float, C.c_float, C.c_float, C.c_float, C.c_int, C.c_int,
                                              C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int,
                                              C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
-    "lavb_pillar_tiled_workspace_bytes": (C.c_size_t, [C.c_int, C.c_int, C.c_int, C.c_longlong]),
-    "lavb_pillar_forward_tiled": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_int,
-                                            C.c_float, C.c_float, C.c_float, C.c_float, C.c_float, C.c_int, C.c_int,
-                                            C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int,
-                                            C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
     "lavb_pillar_decorate": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_int,
                                        C.c_float, C.c_float, C.c_float, C.c_float, C.c_float, C.c_int, C.c_int,
                                        C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
@@ -90,12 +85,9 @@ _SIGS = {
     "lavb_pool2_affine_relu": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
                                          C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p]),
     "lavb_rgb_normalize": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_int, C.c_void_p]),
-    "lavb_split_h16": (C.c_int, [C.c_void_p, C.c_void_p, C.c_longlong, C.c_int, C.c_void_p]),
     "lavb_convert": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_longlong, C.c_void_p]),
     "lavb_stem7x7s2_u8": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                     C.c_void_p, C.c_void_p]),
-    "lavb_gru_h512": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int,
-                                C.c_void_p]),
     "lavb_erf_stem": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]),
     "lavb_erf_down16": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),
     "lavb_erf_nb16": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),

@@ -189,38 +189,9 @@ __global__ void __launch_bounds__(256) convert_kernel(const TS* __restrict__ s, 
   }
 }
 
-// fp32 -> (hi, lo) h16 pair per element, laid out [row][hi(C) | lo(C)]: hi = h16(x), lo = h16(x - hi).  Feeding both
-// halves to a tensor-core conv whose weights are duplicated along cin recovers ~16 mantissa bits of the input.
-__global__ void __launch_bounds__(256) split_h16_kernel(const float* __restrict__ src, h16* __restrict__ dst,
-                                                         long long rows, int c) {
-  const long long i4 = ((long long)blockIdx.x * blockDim.x + threadIdx.x) * 4;
-  if (i4 >= rows * c) return;
-  const long long r = i4 / c;
-  const int ch = (int)(i4 - r * c);
-  const float4 v = __ldg(reinterpret_cast<const float4*>(src + i4));
-  const float x[4] = {v.x, v.y, v.z, v.w};
-  float hi[4], lo[4];
-#pragma unroll
-  for (int e = 0; e < 4; ++e) {
-    hi[e] = h162float(float2h16(x[e]));
-    lo[e] = x[e] - hi[e];
-  }
-  h16* d = dst + r * 2 * c + ch;
-  store4<h16>(d, make_float4(hi[0], hi[1], hi[2], hi[3]));
-  store4<h16>(d + c, make_float4(lo[0], lo[1], lo[2], lo[3]));
-}
-
 }  // namespace lavb
 
 using namespace lavb;
-
-extern "C" int lavb_split_h16(const float* d_src, void* d_dst, long long rows, int c, void* stream) {
-  LAVB_CHECK_ARG(c % 4 == 0 && c > 0, "split_h16: channels must be a multiple of 4");
-  if (rows == 0) return 0;
-  split_h16_kernel<<<ceil_div(rows * c / 4, 256), 256, 0, (cudaStream_t)stream>>>(d_src, (h16*)d_dst, rows, c);
-  LAVB_LAUNCH_OK();
-  return 0;
-}
 
 static int paint_impl(const float* d_pts, int n, int pt_stride, const float* d_sem, int ncam, int c_in, int h, int w,
                       long long s_cam, long long s_c, long long s_y, long long s_x, const float* h_cams, int mode,

@@ -2,7 +2,7 @@
 // a pillar is addressed directly by (b, xi, yi); pass 1 accumulates the per-pillar centroid sums, pass 2
 // decorates each point, runs the 2-layer point MLP and max-pools into the NHWC canvas.
 #include <stdlib.h>
-#include "sm90.cuh"
+#include "common.cuh"
 
 namespace lavb {
 
@@ -290,7 +290,7 @@ static size_t stats_bytes(int batch, int nx, int ny) { return (size_t)batch * (n
 //                decorate + layer 1 (fp32 FFMA) -> h16 hidden tile in swizzled smem -> layer 2 on the tensor cores
 //                (mma.sync m16n8k16 h16, fp32 accumulate; the 64x64 weight fragments live in registers) ->
 //                BN affine + ReLU -> fp32 tile in smem -> 64 channel-threads walk the rows and emit one canvas row per
-//                pillar (running max), as fp32 or as the [hi | lo] h16 split conv1 consumes.
+//                pillar (running max), as fp32 or as h16.
 // The first layer stays fp32 because its inputs are raw metric coordinates (h16 would quantise x to 0.25 m).
 // =====================================================================================================================
 constexpr int kCellsPerBlock = 1024;
@@ -414,17 +414,10 @@ struct EncSmem {                      // shared-memory plan of pillar_encode_sor
   static constexpr int total = pcell + 2 * 4 * 4 * 4;
 };
 
-template <int kOutMode>      // 0: fp32 [64]; 1: h16 [hi 64 | lo 64]; 2: h16 [64]
+template <int kOutMode>      // 0: fp32 [64]; 2: h16 [64]
 __device__ __forceinline__ void emit_pair(void* canvas, int cell, int c, float m0, float m1) {     // channels c, c+1 (c even)
   if (kOutMode == 2) {
     *reinterpret_cast<uint32_t*>(reinterpret_cast<h16*>(canvas) + (long long)cell * 64 + c) = pack_h16(m0, m1);
-  } else if (kOutMode == 1) {
-    h16* o = reinterpret_cast<h16*>(canvas) + (long long)cell * 128;
-    const h162 hi = floats2h162(m0, m1);
-    const float2 hf = h1622float2(hi);
-    const h162 lo = floats2h162(m0 - hf.x, m1 - hf.y);
-    *reinterpret_cast<h162*>(o + c) = hi;
-    *reinterpret_cast<h162*>(o + 64 + c) = lo;
   } else {
     *reinterpret_cast<float2*>(reinterpret_cast<float*>(canvas) + (long long)cell * 64 + c) = make_float2(m0, m1);
   }
@@ -433,10 +426,6 @@ template <int kOutMode>
 __device__ __forceinline__ void emit_one(void* canvas, int cell, int c, float m) {
   if (kOutMode == 2) {
     reinterpret_cast<h16*>(canvas)[(long long)cell * 64 + c] = float2h16(m);
-  } else if (kOutMode == 1) {
-    h16* o = reinterpret_cast<h16*>(canvas) + (long long)cell * 128;
-    const h16 hi = float2h16(m);
-    o[c] = hi; o[64 + c] = float2h16(m - h162float(hi));
   } else {
     reinterpret_cast<float*>(canvas)[(long long)cell * 64 + c] = m;
   }
@@ -646,380 +635,6 @@ static SortedWs carve_sorted(void* base, int batch, int nx, int ny, long long to
   return w;
 }
 
-
-// =====================================================================================================================
-// Tile-binned pillar encoder (the 16-bit pipeline's encoder): the canvas is cut into tiles of kTileR x kTileC cells and
-// every tile is produced start to finish by one CTA, in shared memory:
-//   K1 tile_count   : per point -> canvas tile id; per-block shared-memory histogram -> one global atomic per (block, tile)
-//   K2 tile_scatter : every block re-derives its frame's exclusive tile offsets from the counts (800 entries: cheaper than a
-//                     launch), ranks its points inside the block through shared-memory atomics, reserves one range per
-//                     (block, tile) and writes the in-window points as 48-byte records [pt(11) | packed local cell] in tile
-//                     order — out-of-window points stop here
-//   K3 tile_encode  : CTA = one tile at a time (static interleave over the grid): per-pillar centroid sums in shared memory
-//                     (pass A over the tile's records), then decorate + layer 1 (hi/lo-split MMAs ~ fp32) + layer 2 (h16 MMAs)
-//                     exactly as the sorted kernel did, and the max-pool as shared-memory atomicMax on the fp32 tile
-//                     (post-ReLU values are >= +0: int max on the bit pattern, zero = identity = empty cell); the finished
-//                     tile — zeros included — leaves as full 256-byte cell rows, kTileC cells (4 KB) contiguous.
-// No per-cell global arrays (stats / count / offsets / cursor), no canvas memset or zero-fill pass, no index indirection:
-// global traffic = points read twice (K1 touches x,y), records written + read once, canvas written once.
-// =====================================================================================================================
-constexpr int kTileR = 8, kTileC = 16, kTileCells = kTileR * kTileC;     // 128 cells: a 2 m x 4 m patch at 4 px/m
-constexpr int kRecF = 12;                                                // floats per binned record (48 B)
-constexpr int kBinPts = 2048;                                            // points per block in K1 / K2
-constexpr int kMaxTiles = 2048;                                          // tiles per frame the shared-memory histograms cover
-
-struct TileGrid { int tiles_r, tiles_c, tiles; };
-
-// canvas row / col BEFORE the clamp of scatter_points: row in [-1, ny-1], col in [0, nx] (index == n can occur by rounding)
-__device__ __forceinline__ void raw_row_col(const Grid& g, int xi, int yi, int& row, int& col) { row = g.ny - 1 - xi; col = yi; }
-
-__device__ __forceinline__ int tile_of(const Grid& g, const TileGrid& tg, int xi, int yi, int& packed) {
-  int row, col;
-  raw_row_col(g, xi, yi, row, col);
-  const int crow = row < 0 ? 0 : row, ccol = col > g.nx - 1 ? g.nx - 1 : col;
-  const int tr = crow / kTileR, tc = ccol / kTileC;
-  // local pillar slot: (row - r0 + 1) in [0, kTileR], (col - c0) in [0, kTileC] — the overflow row/col keeps its own centroid
-  packed = ((row - tr * kTileR + 1) << 8) | (col - tc * kTileC);
-  return tr * tg.tiles_c + tc;
-}
-
-__global__ void __launch_bounds__(256) tile_count_kernel(const float* __restrict__ pts, int pt_stride,
-                                                         const __grid_constant__ Clouds clouds, const __grid_constant__ Grid g,
-                                                         const __grid_constant__ TileGrid tg, int* __restrict__ tile_count) {
-  __shared__ int hist[kMaxTiles];
-  const int b = blockIdx.y;
-  const int n = clouds.cum[b + 1] - clouds.cum[b];
-  const int i0 = blockIdx.x * kBinPts;
-  if (i0 >= n) return;
-  for (int t = threadIdx.x; t < tg.tiles; t += 256) hist[t] = 0;
-  __syncthreads();
-  const float* base = pts + clouds.start[b] * pt_stride;
-  for (int i = i0 + threadIdx.x; i < min(n, i0 + kBinPts); i += 256) {
-    const float* p = base + (size_t)i * pt_stride;
-    int xi, yi, packed;
-    if (!locate(g, __ldg(p), __ldg(p + 1), xi, yi)) continue;
-    atomicAdd(&hist[tile_of(g, tg, xi, yi, packed)], 1);
-  }
-  __syncthreads();
-  for (int t = threadIdx.x; t < tg.tiles; t += 256)
-    if (hist[t]) atomicAdd(&tile_count[b * tg.tiles + t], hist[t]);
-}
-
-template <int D>
-__global__ void __launch_bounds__(256) tile_scatter_kernel(const float* __restrict__ pts, int pt_stride,
-                                                           const __grid_constant__ Clouds clouds, const __grid_constant__ Grid g,
-                                                           const __grid_constant__ TileGrid tg, const int* __restrict__ tile_count,
-                                                           int* __restrict__ tile_cursor, int* __restrict__ tile_off,
-                                                           float4* __restrict__ recs) {
-  __shared__ int off[kMaxTiles];      // exclusive offsets of this frame's tiles (relative to the frame's first record)
-  __shared__ int hist[kMaxTiles];     // per-block count -> then the block's base slot per tile
-  __shared__ int wsum[8];
-  const int b = blockIdx.y;
-  const int n = clouds.cum[b + 1] - clouds.cum[b];
-  const int i0 = blockIdx.x * kBinPts;
-  if (i0 >= n && blockIdx.x != 0) return;
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  // block-wide exclusive scan of the frame's tile counts, 256 entries per round
-  int carry = 0;
-  for (int t0 = 0; t0 < tg.tiles; t0 += 256) {
-    const int t = t0 + threadIdx.x;
-    const int c = t < tg.tiles ? __ldg(tile_count + b * tg.tiles + t) : 0;
-    int x = c;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) { const int y = __shfl_up_sync(0xffffffffu, x, o); if (lane >= o) x += y; }
-    if (lane == 31) wsum[warp] = x;
-    __syncthreads();
-    int woff = 0, tot = 0;
-#pragma unroll
-    for (int w = 0; w < 8; ++w) { const int v = wsum[w]; if (w < warp) woff += v; tot += v; }
-    if (t < tg.tiles) { off[t] = carry + woff + x - c; hist[t] = 0; }
-    carry += tot;
-    __syncthreads();
-  }
-  if (blockIdx.x == 0) {   // one block per frame publishes the offsets for the encode kernel
-    for (int t = threadIdx.x; t < tg.tiles; t += 256) tile_off[b * tg.tiles + t] = off[t];
-    if (threadIdx.x == 0) tile_off[clouds.batch * tg.tiles + b] = carry;      // records of frame b (tail of the table)
-  }
-  if (i0 >= n) return;
-  // rank inside the block
-  const float* base = pts + clouds.start[b] * pt_stride;
-  int my_tile[kBinPts / 256], my_rank[kBinPts / 256], my_packed[kBinPts / 256];
-#pragma unroll
-  for (int k = 0; k < kBinPts / 256; ++k) {
-    const int i = i0 + k * 256 + threadIdx.x;
-    my_tile[k] = -1;
-    if (i < n) {
-      const float* p = base + (size_t)i * pt_stride;
-      int xi, yi;
-      if (locate(g, __ldg(p), __ldg(p + 1), xi, yi)) {
-        my_tile[k] = tile_of(g, tg, xi, yi, my_packed[k]);
-        my_rank[k] = atomicAdd(&hist[my_tile[k]], 1);
-      }
-    }
-  }
-  __syncthreads();
-  for (int t = threadIdx.x; t < tg.tiles; t += 256) {
-    const int c = hist[t];
-    if (c) hist[t] = clouds.cum[b] + off[t] + atomicAdd(&tile_cursor[b * tg.tiles + t], c);
-  }
-  __syncthreads();
-#pragma unroll
-  for (int k = 0; k < kBinPts / 256; ++k) {
-    if (my_tile[k] < 0) continue;
-    const int i = i0 + k * 256 + threadIdx.x;
-    const float* p = base + (size_t)i * pt_stride;
-    float f[kRecF];
-#pragma unroll
-    for (int e = 0; e < D; ++e) f[e] = __ldg(p + e);
-#pragma unroll
-    for (int e = D; e < kRecF - 1; ++e) f[e] = 0.f;
-    f[kRecF - 1] = __int_as_float(my_packed[k]);
-    float4* r = recs + (size_t)(hist[my_tile[k]] + my_rank[k]) * (kRecF / 4);
-    r[0] = make_float4(f[0], f[1], f[2], f[3]);
-    r[1] = make_float4(f[4], f[5], f[6], f[7]);
-    r[2] = make_float4(f[8], f[9], f[10], f[11]);
-  }
-}
-
-// ---------------------------------------------------------------------------------------------------------------------
-// Tensor-core version of the tile encoder: the point MLP runs as warpgroup MMAs (wgmma), the CTA being one warpgroup.
-// A chunk = 128 records of the tile = the 128 rows of two m64 MMAs:
-//   thread r decorates its record and writes row r of the A operand in shared memory (K-major, SWIZZLE_128B, written by hand:
-//   16-byte piece j of row r lives at r*128 + ((j ^ (r & 7)) << 4)) as [hi(16) | lo(16) | hi(16) | 0] h16 — the error-free
-//   split of the fp32 features — against B1 = [W1_hi ; W1_hi ; W1_lo ; 0]: three K16 steps give hi*Wh + lo*Wh + hi*Wl ~ fp32;
-//   D1 (128 x 64 fp32) lands in registers; each thread applies BN1 + ReLU to its fragment and writes it back in h16 as the
-//   A operand of layer 2 (K = 64 against B2 = W2); D2 -> BN2; the max-pool is one shared-memory atomicMax per
-//   (row, positive channel) into the fp32 tile.
-// ---------------------------------------------------------------------------------------------------------------------
-struct TcSmem {                        // byte offsets from the 1024-aligned base
-  static constexpr int a = 0;                                   // [128 rows][128 B] A operand of both layers
-  static constexpr int b1 = a + 128 * 128;                      // [64 n][128 B]  W1 as [hi | hi | lo | 0]
-  static constexpr int b2 = b1 + 64 * 128;                      // [64 n][128 B]  W2
-  static constexpr int tile = b2 + 64 * 128;                    // [128 cells][64] fp32, columns XOR (cell & 7) << 2
-  static constexpr int stats = tile + kTileCells * 64 * 4;      // [(kTileR+1)*(kTileC+1)] float4
-  static constexpr int aff = stats + 2560;                      // s1 | t1 | s2 | t2
-  static constexpr int cells = aff + 4 * 64 * 4;                // [128] int
-  static constexpr int total = cells + kRows * 4 + 1024;        // + alignment slack
-};
-
-// out_mode 0: fp32 [64] per cell; 1: h16 [hi 64 | lo 64]; 2: h16 [64]
-template <int D, int kOutMode>
-__global__ void __launch_bounds__(kRows, 3) pillar_tile_encode_tc_kernel(
-    const float4* __restrict__ recs, const __grid_constant__ Clouds clouds, const __grid_constant__ Grid g,
-    const __grid_constant__ TileGrid tg, const int* __restrict__ tile_count, const int* __restrict__ tile_off,
-    const float* __restrict__ w1, const float* __restrict__ s1, const float* __restrict__ t1, const float* __restrict__ w2,
-    const float* __restrict__ s2, const float* __restrict__ t2, void* __restrict__ canvas) {
-  using namespace sm90;
-  constexpr int F = D + 5, H = 64;
-  static_assert(F == 16, "layer 1 is one k16 block per split term");
-  static_assert(kRows == 128, "one warpgroup, two m64 MMAs per chunk");
-  extern __shared__ uint8_t tc_raw[];
-  const uint32_t base = (smem_u32(tc_raw) + 1023u) & ~1023u;
-  uint8_t* gen = tc_raw + (base - smem_u32(tc_raw));
-  uint8_t* As = gen + TcSmem::a;
-  float* tile = reinterpret_cast<float*>(gen + TcSmem::tile);
-  float* stats = reinterpret_cast<float*>(gen + TcSmem::stats);
-  float* aff = reinterpret_cast<float*>(gen + TcSmem::aff);
-  int* cells = reinterpret_cast<int*>(gen + TcSmem::cells);
-  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-
-  // ---- one-time set-up: both weight operands, BN affines
-  for (int e = tid; e < 64 * 8; e += kRows) {                  // 16-byte piece jj of weight row n
-    const int n = e >> 3, jj = e & 7;
-    uint32_t q1[4] = {0u, 0u, 0u, 0u}, q2[4];
-    if (jj < 6) {
-      const float* src = w1 + n * F + (jj & 1) * 8;            // w1 is [64 n][16 k]
-#pragma unroll
-      for (int h = 0; h < 4; ++h) {
-        const float va = __ldg(src + 2 * h), vb = __ldg(src + 2 * h + 1);
-        const uint32_t hi = pack_h16(va, vb);
-        if (jj < 4) q1[h] = hi;
-        else { const float2 hf = unpack_h16(hi); q1[h] = pack_h16(va - hf.x, vb - hf.y); }
-      }
-    }
-    const float* s2p = w2 + n * H + jj * 8;                     // w2 is [64 n][64 k]
-#pragma unroll
-    for (int h = 0; h < 4; ++h) q2[h] = pack_h16(__ldg(s2p + 2 * h), __ldg(s2p + 2 * h + 1));
-    const int off = n * 128 + ((jj ^ (n & 7)) << 4);
-    *reinterpret_cast<uint4*>(gen + TcSmem::b1 + off) = make_uint4(q1[0], q1[1], q1[2], q1[3]);
-    *reinterpret_cast<uint4*>(gen + TcSmem::b2 + off) = make_uint4(q2[0], q2[1], q2[2], q2[3]);
-  }
-  for (int i = tid; i < H; i += kRows) { aff[i] = __ldg(s1 + i); aff[H + i] = __ldg(t1 + i); aff[2 * H + i] = __ldg(s2 + i); aff[3 * H + i] = __ldg(t2 + i); }
-  proxy_fence_async();
-  __syncthreads();
-  const uint64_t b1_desc = desc_sw128(base + TcSmem::b1), b2_desc = desc_sw128(base + TcSmem::b2);
-  // rows of this thread's accumulator fragment: 64 mh + 16 warp + lane / 4 + 8 h; columns 8 j + 2 (lane % 4) (+1)
-  const int frag_row = 16 * warp + (lane >> 2), frag_col = 2 * (lane & 3);
-
-  const int total_tiles = clouds.batch * tg.tiles;
-  constexpr int kRowBytes = kOutMode == 2 ? 128 : 256;
-  for (int work = blockIdx.x; work < total_tiles; work += gridDim.x) {
-    const int b = work / tg.tiles, t = work - b * tg.tiles;
-    const int tr = t / tg.tiles_c, tcx = t - tr * tg.tiles_c;
-    const int r0 = tr * kTileR, c0 = tcx * kTileC;
-    const int n_t = __ldg(tile_count + work);
-    uint8_t* cbase = reinterpret_cast<uint8_t*>(canvas) + ((size_t)b * g.ny * g.nx) * kRowBytes;
-    constexpr int kVecPerCell = kRowBytes / 16;
-    if (n_t == 0) {
-      for (int e = tid; e < kTileCells * kVecPerCell; e += kRows) {
-        const int cell = e / kVecPerCell, lr = cell / kTileC, lc = cell - lr * kTileC;
-        if (r0 + lr < g.ny && c0 + lc < g.nx)
-          __stcs(reinterpret_cast<uint4*>(cbase + ((size_t)(r0 + lr) * g.nx + c0 + lc) * kRowBytes) + (e % kVecPerCell), make_uint4(0u, 0u, 0u, 0u));
-      }
-      continue;
-    }
-    __syncthreads();
-    for (int e = tid; e < kTileCells * 16; e += kRows) reinterpret_cast<float4*>(tile)[e] = make_float4(0.f, 0.f, 0.f, 0.f);
-    for (int e = tid; e < (kTileR + 1) * (kTileC + 1); e += kRows) reinterpret_cast<float4*>(stats)[e] = make_float4(0.f, 0.f, 0.f, 0.f);
-    __syncthreads();
-    const float4* rec = recs + ((size_t)clouds.cum[b] + __ldg(tile_off + work)) * (kRecF / 4);
-    for (int i = tid; i < n_t; i += kRows) {                   // pass A: per-pillar centroid sums
-      const float4 p0 = __ldg(rec + (size_t)i * 3);
-      const int packed = __float_as_int(__ldg(reinterpret_cast<const float*>(rec + (size_t)i * 3 + 2) + 3));
-      float* st = stats + ((packed >> 8) * (kTileC + 1) + (packed & 255)) * 4;
-      atomicAdd(st, p0.x); atomicAdd(st + 1, p0.y); atomicAdd(st + 2, p0.z); atomicAdd(st + 3, 1.f);
-    }
-    __syncthreads();
-    for (int cbeg = 0; cbeg < n_t; cbeg += kRows) {            // pass B: 128 records per round
-      const int i = cbeg + tid;
-      int cell = -1;
-      {
-        float f[F];
-#pragma unroll
-        for (int k = 0; k < F; ++k) f[k] = 0.f;
-        if (i < n_t) {
-          const float4 p0 = __ldg(rec + (size_t)i * 3), p1 = __ldg(rec + (size_t)i * 3 + 1), p2 = __ldg(rec + (size_t)i * 3 + 2);
-          const int packed = __float_as_int(p2.w);
-          const int lr1 = packed >> 8, lc = packed & 255;
-          const float4 st = *reinterpret_cast<const float4*>(stats + (lr1 * (kTileC + 1) + lc) * 4);
-          const int xi = g.ny - 1 - (r0 + lr1 - 1), yi = c0 + lc;
-          f[0] = p0.x; f[1] = p0.y; f[2] = p0.z; f[3] = p0.w; f[4] = p1.x; f[5] = p1.y; f[6] = p1.z; f[7] = p1.w;
-          f[8] = p2.x; f[9] = p2.y; f[10] = p2.z;
-          f[D + 0] = __fsub_rn(f[0], __fdiv_rn(st.x, st.w));
-          f[D + 1] = __fsub_rn(f[1], __fdiv_rn(st.y, st.w));
-          f[D + 2] = __fsub_rn(f[2], __fdiv_rn(st.z, st.w));
-          f[D + 3] = __fsub_rn(f[0], __fadd_rn(__fdiv_rn((float)yi, g.ppm), g.min_x));
-          f[D + 4] = __fsub_rn(f[1], __fadd_rn(__fdiv_rn((float)xi, g.ppm), g.min_y));
-          const int lr = lr1 > 0 ? lr1 - 1 : 0, lcc = lc < kTileC ? lc : kTileC - 1;
-          cell = lr * kTileC + (c0 + lcc > g.nx - 1 ? g.nx - 1 - c0 : lcc);
-        }
-        uint32_t hi[8], lo[8];
-#pragma unroll
-        for (int h = 0; h < 8; ++h) {
-          hi[h] = pack_h16(f[2 * h], f[2 * h + 1]);
-          const float2 hf = unpack_h16(hi[h]);
-          lo[h] = pack_h16(f[2 * h] - hf.x, f[2 * h + 1] - hf.y);
-        }
-        uint8_t* row = As + tid * 128;
-        const int sw = tid & 7;
-        *reinterpret_cast<uint4*>(row + ((0 ^ sw) << 4)) = make_uint4(hi[0], hi[1], hi[2], hi[3]);
-        *reinterpret_cast<uint4*>(row + ((1 ^ sw) << 4)) = make_uint4(hi[4], hi[5], hi[6], hi[7]);
-        *reinterpret_cast<uint4*>(row + ((2 ^ sw) << 4)) = make_uint4(lo[0], lo[1], lo[2], lo[3]);
-        *reinterpret_cast<uint4*>(row + ((3 ^ sw) << 4)) = make_uint4(lo[4], lo[5], lo[6], lo[7]);
-        *reinterpret_cast<uint4*>(row + ((4 ^ sw) << 4)) = make_uint4(hi[0], hi[1], hi[2], hi[3]);
-        *reinterpret_cast<uint4*>(row + ((5 ^ sw) << 4)) = make_uint4(hi[4], hi[5], hi[6], hi[7]);
-      }
-      cells[tid] = cell;
-      proxy_fence_async();                        // generic-proxy stores -> visible to the tensor core's async-proxy reads
-      __syncthreads();
-      float acc[2][32];
-      wgmma_fence();
-#pragma unroll
-      for (int mh = 0; mh < 2; ++mh) {
-        const uint64_t a_desc = desc_sw128(base + TcSmem::a + mh * 64 * 128);
-#pragma unroll
-        for (int k = 0; k < 3; ++k) wgmma<64>(acc[mh], a_desc + (uint64_t)(2 * k), b1_desc + (uint64_t)(2 * k), k ? 1u : 0u);
-      }
-      wgmma_commit();
-      wgmma_wait<0>();
-      acc_fence(acc[0]); acc_fence(acc[1]);
-      __syncthreads();                            // every warp's layer-1 MMAs have read the A rows rewritten below
-#pragma unroll
-      for (int mh = 0; mh < 2; ++mh)
-#pragma unroll
-        for (int h = 0; h < 2; ++h) {
-          const int r = 64 * mh + frag_row + 8 * h;
-          uint8_t* row = As + r * 128;
-#pragma unroll
-          for (int j = 0; j < 8; ++j) {
-            const int c = 8 * j + frag_col;
-            const uint32_t w = pack_h16(fmaxf(fmaf(acc[mh][4 * j + 2 * h], aff[c], aff[H + c]), 0.f),
-                                        fmaxf(fmaf(acc[mh][4 * j + 2 * h + 1], aff[c + 1], aff[H + c + 1]), 0.f));
-            *reinterpret_cast<uint32_t*>(row + ((j ^ (r & 7)) << 4) + 2 * frag_col) = w;
-          }
-        }
-      proxy_fence_async();
-      __syncthreads();
-      wgmma_fence();
-#pragma unroll
-      for (int mh = 0; mh < 2; ++mh) {
-        const uint64_t a_desc = desc_sw128(base + TcSmem::a + mh * 64 * 128);
-#pragma unroll
-        for (int k = 0; k < 4; ++k) wgmma<64>(acc[mh], a_desc + (uint64_t)(2 * k), b2_desc + (uint64_t)(2 * k), k ? 1u : 0u);
-      }
-      wgmma_commit();
-      wgmma_wait<0>();
-      acc_fence(acc[0]); acc_fence(acc[1]);
-      // max-pool: one shared-memory atomicMax per (row, positive channel).  The columns of a cell are rotated by (cell & 7) * 4
-      // so rows of different cells mostly hit different banks (rows of the SAME cell hit the same word and are serialised).
-#pragma unroll
-      for (int mh = 0; mh < 2; ++mh)
-#pragma unroll
-        for (int h = 0; h < 2; ++h) {
-          const int rcell = cells[64 * mh + frag_row + 8 * h];
-          if (rcell < 0) continue;
-          int* trow = reinterpret_cast<int*>(tile) + rcell * 64;
-          const int sw = (rcell & 7) << 2;
-#pragma unroll
-          for (int j = 0; j < 8; ++j)
-#pragma unroll
-            for (int e = 0; e < 2; ++e) {
-              const int c = 8 * j + frag_col + e;
-              const float val = fmaf(acc[mh][4 * j + 2 * h + e], aff[2 * H + c], aff[3 * H + c]);
-              if (val > 0.f) atomicMax(trow + (c ^ sw), __float_as_int(val));
-            }
-        }
-      __syncthreads();                            // A rows and cells[] are rewritten by the next round
-    }
-    __syncthreads();
-    // ---- write-out, zeros included
-    for (int e = tid; e < kTileCells * 16; e += kRows) {
-      const int cell = e >> 4, q = e & 15, lr = cell / kTileC, lc = cell - lr * kTileC;
-      if (r0 + lr >= g.ny || c0 + lc >= g.nx) continue;
-      const float4 v = *reinterpret_cast<const float4*>(tile + cell * 64 + ((4 * q) ^ ((cell & 7) << 2)));
-      uint8_t* row = cbase + ((size_t)(r0 + lr) * g.nx + c0 + lc) * kRowBytes;
-      if (kOutMode == 0) {
-        __stcs(reinterpret_cast<float4*>(row) + q, v);
-      } else {
-        const uint32_t h0 = pack_h16(v.x, v.y), h1 = pack_h16(v.z, v.w);
-        __stcs(reinterpret_cast<uint2*>(row) + q, make_uint2(h0, h1));
-        if (kOutMode == 1) {
-          const float2 f0 = unpack_h16(h0), f1 = unpack_h16(h1);
-          __stcs(reinterpret_cast<uint2*>(row + 128) + q, make_uint2(pack_h16(v.x - f0.x, v.y - f0.y), pack_h16(v.z - f1.x, v.w - f1.y)));
-        }
-      }
-    }
-  }
-}
-
-struct TiledWs { int* tile_count; int* tile_cursor; int* tile_off; float4* recs; size_t bytes; };
-static TiledWs carve_tiled(void* base, int batch, int tiles, long long total_pts) {
-  TiledWs w;
-  char* p = reinterpret_cast<char*>(base);
-  auto take = [&](size_t n) { char* r = p; p += (n + 255) / 256 * 256; return r; };
-  w.tile_count = reinterpret_cast<int*>(take((size_t)batch * tiles * 4));
-  w.tile_cursor = reinterpret_cast<int*>(take((size_t)batch * tiles * 4));      // adjacent to tile_count: one memset
-  w.tile_off = reinterpret_cast<int*>(take(((size_t)batch * tiles + batch) * 4));
-  w.recs = reinterpret_cast<float4*>(take((size_t)total_pts * kRecF * 4));
-  w.bytes = (size_t)(p - reinterpret_cast<char*>(base));
-  return w;
-}
-static TileGrid make_tile_grid(int nx, int ny) {
-  TileGrid tg;
-  tg.tiles_r = ceil_div(ny, kTileR); tg.tiles_c = ceil_div(nx, kTileC); tg.tiles = tg.tiles_r * tg.tiles_c;
-  return tg;
-}
-
 }  // namespace lavb
 
 using namespace lavb;
@@ -1129,7 +744,7 @@ extern "C" int lavb_pillar_forward_sorted(const float* d_pts, int pt_stride, int
   Clouds clouds;
   if (fill_clouds(clouds, h_cloud_start, h_cloud_count, batch)) return 1;
   LAVB_CHECK_ARG(d == 11 && h1 == 64 && h2 == 64, "pillar_forward_sorted: only the v2 configuration (D=11, features [64,64]) is built");
-  LAVB_CHECK_ARG(out_mode >= 0 && out_mode <= 2, "pillar_forward_sorted: out_mode 0 (fp32), 1 (h16 hi|lo split) or 2 (h16)");
+  LAVB_CHECK_ARG(out_mode == 0 || out_mode == 2, "pillar_forward_sorted: out_mode must be 0 (fp32) or 2 (h16) (got %d)", out_mode);
   LAVB_CHECK_ARG(pt_stride >= d, "pillar_forward_sorted: pt_stride < d");
   cudaStream_t st = (cudaStream_t)stream;
   Grid g{min_x, max_x, min_y, max_y, ppm, nx, ny};
@@ -1137,7 +752,7 @@ extern "C" int lavb_pillar_forward_sorted(const float* d_pts, int pt_stride, int
   const long long ncells = (long long)batch * nx * ny;
   LAVB_CHECK_ARG(ncells < (1LL << 31), "pillar_forward_sorted: too many cells");
   const SortedWs w = carve_sorted(d_workspace, batch, nx, ny, total);
-  const int row_bytes = h2 * (out_mode == 2 ? 2 : 4);        // fp32: 64*4; split: 128*2; h16: 64*2
+  const int row_bytes = h2 * (out_mode == 2 ? 2 : 4);        // fp32: 64*4; h16: 64*2
   LAVB_CUDA_OK(cudaMemsetAsync(w.stats, 0, stats_bytes(batch, nx, ny), st));
   LAVB_CUDA_OK(cudaMemsetAsync(w.count, 0, (size_t)ncells * 8 + 512, st));       // count + cursor (adjacent, 256 B padded)
   LAVB_CUDA_OK(cudaMemsetAsync(w.tile_start, 0, ((size_t)total / kRows + 2) * 4, st));
@@ -1159,60 +774,13 @@ extern "C" int lavb_pillar_forward_sorted(const float* d_pts, int pt_stride, int
   LAVB_LAUNCH_OK();
   const size_t smem = EncSmem::total;
   LAVB_CUDA_OK(ensure_dyn_smem((const void*)pillar_encode_sorted_kernel<11, 0>, 72 * 1024));
-  LAVB_CUDA_OK(ensure_dyn_smem((const void*)pillar_encode_sorted_kernel<11, 1>, 72 * 1024));
   LAVB_CUDA_OK(ensure_dyn_smem((const void*)pillar_encode_sorted_kernel<11, 2>, 72 * 1024));
   const int ntiles = min(ceil_div(total, kRows), kNumSMs * 3);     // persistent: 3 resident blocks per SM
 #define LAVB_SORTED_LAUNCH(M)                                                                                                        \
   pillar_encode_sorted_kernel<11, M><<<ntiles, kRows, smem, st>>>(d_pts, pt_stride, clouds, g, w.stats, w.order, w.ocell, w.tile_start, \
                                                                   w.total, d_w1, d_s1, d_t1, d_w2, d_s2, d_t2, d_canvas)
-  if (out_mode == 0) LAVB_SORTED_LAUNCH(0); else if (out_mode == 1) LAVB_SORTED_LAUNCH(1); else LAVB_SORTED_LAUNCH(2);
+  if (out_mode == 0) LAVB_SORTED_LAUNCH(0); else LAVB_SORTED_LAUNCH(2);
 #undef LAVB_SORTED_LAUNCH
-  LAVB_LAUNCH_OK();
-  return 0;
-}
-
-extern "C" size_t lavb_pillar_tiled_workspace_bytes(int batch, int nx, int ny, long long total_points) {
-  return carve_tiled(nullptr, batch, make_tile_grid(nx, ny).tiles, total_points).bytes;
-}
-
-extern "C" int lavb_pillar_forward_tiled(const float* d_pts, int pt_stride, int d, const long long* h_cloud_start,
-                                         const int* h_cloud_count, int batch, float min_x, float max_x, float min_y,
-                                         float max_y, float ppm, int nx, int ny, const float* d_w1, const float* d_s1,
-                                         const float* d_t1, int h1, const float* d_w2, const float* d_s2, const float* d_t2,
-                                         int h2, void* d_canvas, int out_mode, void* d_workspace, void* stream) {
-  Clouds clouds;
-  if (fill_clouds(clouds, h_cloud_start, h_cloud_count, batch)) return 1;
-  LAVB_CHECK_ARG(d == 11 && h1 == 64 && h2 == 64, "pillar_forward_tiled: only the v2 configuration (D=11, features [64,64]) is built");
-  LAVB_CHECK_ARG(out_mode >= 0 && out_mode <= 2, "pillar_forward_tiled: out_mode 0 (fp32), 1 (h16 hi|lo split) or 2 (h16)");
-  LAVB_CHECK_ARG(pt_stride >= d, "pillar_forward_tiled: pt_stride < d");
-  const TileGrid tg = make_tile_grid(nx, ny);
-  LAVB_CHECK_ARG(tg.tiles <= kMaxTiles, "pillar_forward_tiled: grid of %d x %d cells has more than %d tiles", nx, ny, kMaxTiles);
-  LAVB_CHECK_ARG((long long)batch * tg.tiles < (1LL << 31), "pillar_forward_tiled: too many tiles");
-  cudaStream_t st = (cudaStream_t)stream;
-  Grid g{min_x, max_x, min_y, max_y, ppm, nx, ny};
-  const int total = clouds.cum[batch];
-  const TiledWs w = carve_tiled(d_workspace, batch, tg.tiles, total);
-  LAVB_CUDA_OK(cudaMemsetAsync(w.tile_count, 0, (size_t)(reinterpret_cast<char*>(w.tile_off) - reinterpret_cast<char*>(w.tile_count)), st));
-  int max_n = 0;
-  for (int b = 0; b < batch; ++b) max_n = max(max_n, h_cloud_count[b]);
-  if (max_n > 0) {
-    dim3 grid(ceil_div(max_n, kBinPts), batch);
-    tile_count_kernel<<<grid, 256, 0, st>>>(d_pts, pt_stride, clouds, g, tg, w.tile_count);
-    LAVB_LAUNCH_OK();
-    tile_scatter_kernel<11><<<grid, 256, 0, st>>>(d_pts, pt_stride, clouds, g, tg, w.tile_count, w.tile_cursor, w.tile_off, w.recs);
-    LAVB_LAUNCH_OK();
-  } else {
-    LAVB_CUDA_OK(cudaMemsetAsync(w.tile_off, 0, ((size_t)batch * tg.tiles + batch) * 4, st));
-  }
-  const int grid4 = min(batch * tg.tiles, kNumSMs * 3);              // persistent: 3 resident CTAs per SM
-#define LAVB_TC_LAUNCH(M)                                                                                                          \
-  {                                                                                                                               \
-    LAVB_CUDA_OK(ensure_dyn_smem((const void*)pillar_tile_encode_tc_kernel<11, M>, TcSmem::total));                               \
-    pillar_tile_encode_tc_kernel<11, M><<<grid4, kRows, TcSmem::total, st>>>(w.recs, clouds, g, tg, w.tile_count, w.tile_off, d_w1,  \
-                                                                             d_s1, d_t1, d_w2, d_s2, d_t2, d_canvas);             \
-  }
-  if (out_mode == 0) LAVB_TC_LAUNCH(0) else if (out_mode == 1) LAVB_TC_LAUNCH(1) else LAVB_TC_LAUNCH(2)
-#undef LAVB_TC_LAUNCH
   LAVB_LAUNCH_OK();
   return 0;
 }

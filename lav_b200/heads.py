@@ -10,7 +10,7 @@ keys (tests/golden/keys_uniplanner.json, keys_brake.json):
                       team_code_v2/models/rgb.py:48-83, lav/models/attention.py, segmentation.py
 
 Only the crop (bilinear rotated window gather) is a lav_b200 CUDA kernel; convs/GRUs here are cuDNN, except the
-flag-selected kernels below (STEM_KERNEL, GRU_KERNEL, CAST_KERNEL) and the brake stem of forward_u8.
+flag-selected kernels below (STEM_KERNEL, CAST_KERNEL) and the brake stem of forward_u8.
 """
 import math
 
@@ -141,15 +141,6 @@ class ResNet18(nn.Module):
         return self._trunk_folded(x.permute(0, 3, 1, 2), f)                            # NCHW view of channels-last memory
 
     def _trunk_folded(self, x, f):
-        dt = x.dtype
-        if getattr(self, "use_umma_trunk", False) and dt == ops.h16():
-            # layer1..4 on the lav_b200 wgmma conv kernel (BN / residual / ReLU fused in its epilogue)
-            key = ("umma", str(x.device))
-            cache = self._cache()
-            if key not in cache:
-                from .resnet_umma import ResNetTrunkUMMA
-                cache[key] = ResNetTrunkUMMA(self)
-            return cache[key](x.permute(0, 2, 3, 1).contiguous()).permute(0, 3, 1, 2)
         for li in range(1, 5):
             for bi, blk in enumerate(getattr(self, f"layer{li}")):
                 st = blk.conv1.stride
@@ -179,15 +170,6 @@ class ResNet18(nn.Module):
 def resnet18(pretrained=False, num_channels=3, **kw):
     return ResNet18(num_channels=num_channels)
 
-
-# Cluster-persistent plan GRU (csrc/gru_cluster.cu): one launch per 20-step roll-out instead of cuDNN's 20 GEMM + cell launch
-# pairs.  fp32-class arithmetic — both operands of the recurrent product are split into h16 hi + lo parts (3 mma.sync products) —
-# because the 5 x 20-step plan roll-out is not contractive on untrained weights: the first version of the kernel (plain h16
-# operands, 8e-4 per roll-out, 0.71 ms per tick) ended 1.7e-2 .. 5e-2 from the reference at BASELINE config 3.  This version
-# agrees with nn.GRU to 2e-5 over 20 steps and passes every parity test of both pipelines, but the three products run on the
-# legacy mma.sync path and 64 KB of hidden state cross DSMEM per CTA and step: 1.18 ms per tick of 32 frames against cuDNN's
-# cuDNN.  OFF by default for that reason.
-GRU_KERNEL = False
 
 # The cast branches (6 x GRU(512, 64) + Linear(64, 2) + cumsum over the repeated embedding) as ONE fp32 kernel (csrc/cast_gru.cu)
 # instead of ~100 dependent cuDNN / ATen launches per call.  Inference only.
@@ -354,14 +336,7 @@ def _plan_rollout(plan_gru, plan_mlp, num_cmds, num_plan, num_plan_iter, embd, n
     outs = []
     for _ in range(num_plan_iter):
         u = torch.cat([u0[:, None, None].expand(B, num_cmds, num_plan, 2), plan_loc], dim=3)
-        if (GRU_KERNEL and u.is_cuda and not torch.is_grad_enabled() and plan_gru.hidden_size == 512 and plan_gru.input_size == 4
-                and plan_gru.weight_hh_l0.dtype == torch.float32):
-            # the whole 20-step roll-out in one cluster-persistent kernel (csrc/gru_cluster.cu); fp32-class arithmetic (split
-            # operands on the tensor cores), so it serves the fp32 and the 16-bit pipeline alike
-            out = ops.gru_h512(u.reshape(B * num_cmds, num_plan, 4).float(), h0[0].float(), plan_gru.weight_hh_l0.detach(),
-                               plan_gru.weight_ih_l0.detach(), plan_gru.bias_ih_l0.detach(), plan_gru.bias_hh_l0.detach())
-        else:
-            out, _ = plan_gru(u.reshape(B * num_cmds, num_plan, 4), h0)
+        out, _ = plan_gru(u.reshape(B * num_cmds, num_plan, 4), h0)
         plan_loc = torch.cumsum(plan_mlp(out), dim=1).view(B, num_cmds, num_plan, 2) + plan_loc
         outs.append(plan_loc)
     return torch.stack(outs, dim=1)

@@ -14,9 +14,6 @@ from .layers import PlanMixin, TapConv, bn_affine
 from .point_pillar import PointPillarNet
 
 
-CANVAS16 = True       # 16-bit path: single h16 canvas (tile-binned encoder, out_mode 2) instead of the [hi | lo] split
-
-
 def _dt(precision):
     return torch.float32 if precision == "fp32" else ops.h16()
 
@@ -62,13 +59,6 @@ class ConvBackbone(PlanMixin, nn.Module):
         for name in ("upconv1", "upconv2", "upconv3"):
             seq = getattr(self, name)
             plan[name] = crb(seq[0], seq[2])
-        if self.precision == "f16":
-            # first layer on tensor cores WITHOUT rounding the fp32 canvas to f16: input = [hi | lo] split (2*cin channels),
-            # weights duplicated along cin, so conv(x_hi) + conv(x_lo) accumulate in the MMA accumulators (costs 1.9 extra GFLOP / frame)
-            c0, b0 = self.conv1[0], self.conv1[2]
-            s, t = bn_affine(b0)
-            plan["conv1_split"] = TapConv(torch.cat([c0.weight, c0.weight], 1), False, c0.stride, c0.padding, c0.dilation, 0, None,
-                                          pre_relu=True, scale=s, shift=t)
         return plan
 
     def forward_nhwc(self, x):
@@ -77,15 +67,13 @@ class ConvBackbone(PlanMixin, nn.Module):
             raise LavbError("ConvBackbone: training-mode forward goes through lav_b200.train (autograd path)")
         plan = self._plan_get(x.device, self._build)
         dt = _dt(self.precision)
-        first = None
         if dt == ops.h16() and x.dtype == torch.float32:
-            first = plan["conv1_split"](ops.split_h16(x), out_dtype=dt)
-        elif dt == ops.h16() and x.shape[-1] == 2 * self.conv1[0].in_channels:
-            first = plan["conv1_split"](x, out_dtype=dt)       # canvas already arrives as the [hi | lo] f16 split
+            # an fp32 canvas gets the saturating round-to-nearest the encoder's h16 canvas (out_mode 2) applies
+            x = ops.convert(x, dt)
         xs = []
         for name in ("conv1", "conv2", "conv3"):
-            for li, layer in enumerate(plan[name]):
-                x = first if (name == "conv1" and li == 0 and first is not None) else layer(x, out_dtype=dt)
+            for layer in plan[name]:
+                x = layer(x, out_dtype=dt)
             xs.append(x)
         n, h, w, _ = xs[0].shape
         ctot = plan["upconv1"].cout + plan["upconv2"].cout + plan["upconv3"].cout
@@ -224,11 +212,9 @@ class LiDARModel(PlanMixin, nn.Module):
         return ops.deconv3x3s2_small(hid, 4, nh, wd, bd, n_outs, sig)
 
     def forward_nhwc(self, lidars, num_points):
-        f16 = self.precision == "f16"
         # 16-bit path: the canvas is an h16 activation like every other layer's input (64 ch, 128 B per cell).  With half storage
-        # its rounding (2^-12) is the same as everywhere else in the stack; the [hi | lo] split canvas (CANVAS16 = False) is the
-        # legacy form that kept the first conv at fp32 input precision when the storage type was bfloat16.
-        canvas = self.point_pillar_net.forward_nhwc(lidars, num_points, split_out=f16 and not CANVAS16, canvas16=f16 and CANVAS16)
+        # its rounding (2^-12) is the same as everywhere else in the stack.
+        canvas = self.point_pillar_net.forward_nhwc(lidars, num_points, canvas16=self.precision == "f16")
         feats = self.backbone.forward_nhwc(canvas)
         return (feats, *self.heads_nhwc(feats))
 

@@ -559,28 +559,13 @@ def det_heatmaps(actors, offsets, grid=None, out=None):
     return heat, size, orim
 
 
-def split_h16(x):
-    """fp32 (..., C) contiguous -> f16 (..., 2C) = [hi | lo] error-free split (see lavb_split_h16)."""
-    _need_cuda(x)
-    assert x.is_contiguous() and x.dtype == torch.float32
-    c = x.shape[-1]
-    out = torch.empty((*x.shape[:-1], 2 * c), dtype=h16(), device=x.device)
-    check(lib().lavb_split_h16(_ptr(x), _ptr(out), x.numel() // c, c, _stream()), "lavb_split_h16")
-    _COUNT[0] += 1
-    return out
+PILLAR_ENCODER = "sorted"    # name of the 16-bit pipeline's pillar encoder, reported by bench.py; it selects nothing
 
 
-PILLAR_ENCODER = "sorted"    # tensor-core encoders of the 16-bit pipeline:
-#   "sorted": counting sort by canvas cell + persistent mma.sync encoder (lavb_pillar_forward_sorted)          23.3 us/frame
-#   "tiled" : points binned by 8x16-cell canvas tile, one CTA per tile, wgmma MLP (lavb_pillar_forward_tiled) —
-#             fewer launches and 35 % less DRAM traffic (942 vs 1448 MB), but every tile is a serial chain of ~8 dependent steps
-#             (load, centroid atomics, MMA round trips, pooling atomics, store) with 3 CTAs per SM: latency-bound (profiles/)
-
-
-def pillar_forward_sorted(pts, starts, counts, grid, w1, s1, t1, w2, s2, t2, split_out=False, canvas16=False):
-    """tensor-core pillar encoder of the 16-bit pipeline (tile-binned or sorted kernel, see PILLAR_ENCODER).  Returns the NHWC
-    canvas: fp32 (B,ny,nx,H2); with split_out, h16 (B,ny,nx,2*H2) = [hi | lo]; with canvas16, h16 (B,ny,nx,H2) — what the 16-bit
-    pipeline feeds the backbone."""
+def pillar_forward_sorted(pts, starts, counts, grid, w1, s1, t1, w2, s2, t2, canvas16=False):
+    """tensor-core pillar encoder of the 16-bit pipeline: counting sort by canvas cell + persistent mma.sync encoder
+    (lavb_pillar_forward_sorted).  Returns the NHWC canvas: fp32 (B,ny,nx,H2); with canvas16, h16 (B,ny,nx,H2), saturating —
+    what the 16-bit pipeline feeds the backbone."""
     _need_cuda(pts, w1, w2)
     assert pts.dtype == torch.float32 and pts.dim() == 2 and pts.stride(1) == 1
     min_x, max_x, min_y, max_y, ppm, nx, ny = grid
@@ -588,19 +573,14 @@ def pillar_forward_sorted(pts, starts, counts, grid, w1, s1, t1, w2, s2, t2, spl
     b, st, ct = _clouds(starts, counts)
     total = int(sum(int(c) for c in counts))
     h2 = w2.shape[0]
-    assert not (split_out and canvas16)
-    canvas = torch.empty((b, ny, nx, 2 * h2 if split_out else h2), dtype=h16() if (split_out or canvas16) else torch.float32, device=pts.device)
-    tiled = PILLAR_ENCODER == "tiled"
-    if tiled:      # every frame's records start at its exclusive point offset: size the record buffer for the clouds as given
-        total = int(sum(int(c) for c in counts))
-    ws = _workspace(pts.device, (lib().lavb_pillar_tiled_workspace_bytes if tiled else lib().lavb_pillar_sorted_workspace_bytes)(b, nx, ny, total))
+    canvas = torch.empty((b, ny, nx, h2), dtype=h16() if canvas16 else torch.float32, device=pts.device)
+    ws = _workspace(pts.device, lib().lavb_pillar_sorted_workspace_bytes(b, nx, ny, total))
     e0 = _prof_begin()
-    fn, name = (lib().lavb_pillar_forward_tiled, "lavb_pillar_forward_tiled") if tiled else (lib().lavb_pillar_forward_sorted, "lavb_pillar_forward_sorted")
-    check(fn(_ptr(pts), pts.stride(0), d, st, ct, b, min_x, max_x, min_y, max_y, ppm, nx, ny,
+    check(lib().lavb_pillar_forward_sorted(_ptr(pts), pts.stride(0), d, st, ct, b, min_x, max_x, min_y, max_y, ppm, nx, ny,
                                            _ptr(w1), _ptr(s1), _ptr(t1), w1.shape[0], _ptr(w2), _ptr(s2), _ptr(t2), h2,
-                                           _ptr(canvas), 2 if canvas16 else int(split_out), _ptr(ws), _stream()), name)
+                                           _ptr(canvas), 2 if canvas16 else 0, _ptr(ws), _stream()), "lavb_pillar_forward_sorted")
     _prof_end("pillar", float(total) * d * 4 + float(b) * ny * nx * h2 * (2 if canvas16 else 4), e0)
-    _COUNT[0] += 3 if tiled else 6
+    _COUNT[0] += 6
     return canvas
 
 
@@ -764,22 +744,5 @@ def cast_gru(embd, wih_t, whh_t, bih, bhh, wmlp, bmlp, steps):
     out = torch.empty((n, ncmd, steps, 2), dtype=torch.float32, device=embd.device)
     check(lib().lavb_cast_gru(_ptr(embd), n, _ptr(wih_t), _ptr(whh_t), _ptr(bih), _ptr(bhh), _ptr(wmlp), _ptr(bmlp), ncmd, steps,
                               _ptr(out), _stream()), "lavb_cast_gru")
-    _COUNT[0] += 1
-    return out
-
-
-def gru_h512(u, h0, whh, wih, bih, bhh):
-    """cluster-persistent GRU(4 -> 512) roll-out (csrc/gru_cluster.cu), fp32-class arithmetic.  u (N, T, 4), h0 (N, 512),
-    whh (1536, 512), wih (1536, 4), bih / bhh (1536,), all fp32 -> out (N, T, 512) fp32 (the output sequence of
-    nn.GRU(batch_first=True))."""
-    _need_cuda(u, h0, whh)
-    n, t, k = u.shape
-    assert k == 4 and tuple(h0.shape) == (n, 512) and tuple(whh.shape) == (1536, 512)
-    assert u.dtype == h0.dtype == whh.dtype == wih.dtype == bih.dtype == bhh.dtype == torch.float32
-    u, h0 = u.contiguous(), h0.contiguous()
-    assert whh.is_contiguous() and wih.is_contiguous()
-    out = torch.empty((n, t, 512), dtype=torch.float32, device=u.device)
-    check(lib().lavb_gru_h512(_ptr(u), _ptr(h0), _ptr(whh), _ptr(wih), _ptr(bih), _ptr(bhh), _ptr(out), n, t, _stream()),
-          "lavb_gru_h512")
     _COUNT[0] += 1
     return out

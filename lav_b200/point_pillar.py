@@ -112,14 +112,14 @@ class PointPillarNet(PlanMixin, nn.Module):
             return canvas.view(B, self.ny, self.nx, -1).permute(0, 3, 1, 2)
         return self.forward_nhwc(lidar_list, num_points, _buf=(buf, starts, counts)).permute(0, 3, 1, 2)
 
-    def forward_nhwc(self, lidar_list, num_points, split_out=False, _buf=None, canvas16=False):
+    def forward_nhwc(self, lidar_list, num_points, _buf=None, canvas16=False):
         """eval forward returning the raw NHWC canvas buffer.  fp32 precision: exact kernel (fp32 FFMA + atomicMax).
-        f16 precision: sorted / tensor-core kernel; with split_out the canvas comes as f16 [hi | lo] (B,ny,nx,2C),
-        which is what ConvBackbone's first tensor-core conv consumes."""
+        f16 precision: sorted / tensor-core kernel; the canvas comes as fp32 (B,ny,nx,C), or with canvas16 as the saturating
+        h16 (B,ny,nx,C) that ConvBackbone's first tensor-core conv consumes."""
         buf, starts, counts = _buf if _buf is not None else self._as_buffer(lidar_list, num_points)
         if not buf.is_cuda:
             raise LavbError("lav_b200.PointPillarNet needs CUDA tensors (no CPU fallback)")
         w1, s1, t1, w2, s2, t2 = self._plan_get(buf.device, self._build)
         if self.precision == "f16":
-            return ops.pillar_forward_sorted(buf, starts, counts, self._grid(), w1, s1, t1, w2, s2, t2, split_out=split_out, canvas16=canvas16)
+            return ops.pillar_forward_sorted(buf, starts, counts, self._grid(), w1, s1, t1, w2, s2, t2, canvas16=canvas16)
         return ops.pillar_forward(buf, starts, counts, self._grid(), w1, s1, t1, w2, s2, t2)

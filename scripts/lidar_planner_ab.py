@@ -15,7 +15,6 @@ import torch
 from lav_b200 import capi, ops, synth
 from tests import util
 from tests.test_heads_cpu import uniplanner
-from lav_b200 import lidar as L
 
 
 def load(path):
@@ -50,7 +49,7 @@ cmds = torch.full((B,), 3, dtype=torch.long, device=cuda)
 
 
 def canvas():
-    return m.point_pillar_net.forward_nhwc(batch, [3 * N] * B, split_out=not L.CANVAS16, canvas16=L.CANVAS16).clone()
+    return m.point_pillar_net.forward_nhwc(batch, [3 * N] * B, canvas16=True).clone()
 
 with torch.no_grad():
     for k, h in libs.items():

@@ -2,10 +2,9 @@
 import os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
-from lav_b200 import ops, synth
+from lav_b200 import synth
 from tests import util
 B = int(sys.argv[1]) if len(sys.argv) > 1 else 16
-ops.PILLAR_ENCODER = os.environ.get("LAVB_PILLAR_ENCODER", ops.PILLAR_ENCODER)
 KW = dict(canvas16=True)
 dev = torch.device("cuda:0")
 m, _ = util.lidar_model(dev)

@@ -60,14 +60,12 @@ def _config2_inputs(B):
     return lidars, sems
 
 
-@pytest.mark.parametrize("precision", ["fp32", "f16", "f16-tiled"])
-def test_config2_paint_and_voxelise_b32(cuda, precision, monkeypatch):
+@pytest.mark.parametrize("precision", ["fp32", "f16"])
+def test_config2_paint_and_voxelise_b32(cuda, precision):
     """Config 2: point painting + PointPillars voxeliser forward, B = 32 x 40 000 points (time one-hot [1,0,0], D = 11).
     Painted features must be index-equal to the oracle on every frame; the canvas within 1e-3 on sampled frames, with
-    identical occupancy.  fp32 = the exact kernel; f16 = the tensor-core encoder the benchmark runs, with its h16 canvas;
-    f16-tiled = the tile-binned wgmma encoder (same 1e-3 gate for all three)."""
-    if precision == "f16-tiled":
-        monkeypatch.setattr(ops, "PILLAR_ENCODER", "tiled")
+    identical occupancy.  fp32 = the exact kernel; f16 = the tensor-core encoder the benchmark runs, with its h16 canvas
+    (same 1e-3 gate for both)."""
     from lav_b200 import point_painting as PP
     B = 32
     lidars, sems = _config2_inputs(B)
@@ -84,7 +82,7 @@ def test_config2_paint_and_voxelise_b32(cuda, precision, monkeypatch):
     assert n_bad <= B * N_SWEEP // 5000, f"{n_bad} painted rows differ over the batch"           # pixel-boundary flips only
     pts = torch.cat([fused, torch.tensor([1.0, 0.0, 0.0], device=cuda).expand(B, N_SWEEP, 3)], 2).contiguous()
     m, sd = util.lidar_model(cuda)
-    m.set_precision(precision.split("-")[0])
+    m.set_precision(precision)
     with torch.no_grad():
         canvas = m.point_pillar_net.forward_nhwc(pts, [N_SWEEP] * B, canvas16=(precision != "fp32")).float()
     assert canvas.shape == (B, 320, 320, 64)
@@ -96,13 +94,10 @@ def test_config2_paint_and_voxelise_b32(cuda, precision, monkeypatch):
         assert util.rel_err(got, want) < 1e-3, (b, util.rel_err(got, want))
 
 
-@pytest.mark.parametrize("gru_kernel", [True, False])     # the cluster-persistent plan GRU (product default) and cuDNN's
-def test_config3_backbone_heads_planner_b64_f16(cuda, gru_kernel, monkeypatch):
-    """Config 3: B = 64 frames of 120 000 stacked points through the 16-bit tensor-core path — pillar encoder (split canvas),
-    BEV backbone, the four heads and UniPlanner with K = 3 fixed vehicles per frame — vs the fp32 oracle on sampled frames of the
-    batch: north_star tolerance 1e-2 (max-norm and rms of every output)."""
-    from lav_b200 import heads
-    monkeypatch.setattr(heads, "GRU_KERNEL", gru_kernel)
+def test_config3_backbone_heads_planner_b64_f16(cuda):
+    """Config 3: B = 64 frames of 120 000 stacked points through the 16-bit tensor-core path — pillar encoder (h16 canvas),
+    BEV backbone, the four heads and UniPlanner (cuDNN's plan GRU) with K = 3 fixed vehicles per frame — vs the fp32 oracle on
+    sampled frames of the batch: north_star tolerance 1e-2 (max-norm and rms of every output)."""
     B, K = 64, 3
     dets = [(150.0, 200.0, 8.0, 4.0, 0.9, 0.3), (170.0, 240.0, 8.0, 4.0, -0.2, 0.95), (120.0, 150.0, 8., 4., 1., 0.)]
     clouds = [synth.stacked_lidar(N_SWEEP, tag=f"c3{b % 8}") for b in range(8)]

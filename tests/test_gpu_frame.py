@@ -265,23 +265,6 @@ def test_static_pipeline_matches_dynamic(cuda, graphs):
             assert [d[:2] for d in o_s["det"][b][0]] == [d[:2] for d in o_d["det"][b][0]]     # class 1 was overridden with DETS
 
 
-def test_resnet_trunk_on_umma_matches_cudnn(cuda):
-    """ResNet-18 layer1..4 through the wgmma tap-list conv (BN/residual/ReLU fused) vs the folded cuDNN path."""
-    from lav_b200.heads import resnet18
-    m = resnet18(num_channels=3).eval()
-    m.load_state_dict(synth.fill_state_dict_(m.state_dict()))
-    m = m.to(cuda).to(ops.h16()).to(memory_format=torch.channels_last)
-    x = synth.rgb_frames(smooth=True, tag="rt", n_cam=2, h=192, w=480).permute(0, 3, 1, 2).float().to(cuda) / 255.
-    with torch.no_grad():
-        m.use_umma_trunk = False
-        want = m(x).float()
-        m.use_umma_trunk = True
-        got = m(x).float()
-    assert got.shape == want.shape == (2, 512, 6, 15)
-    rms = float(((got - want) ** 2).mean().sqrt() / (want ** 2).mean().sqrt())
-    assert rms < 5e-3, rms            # both paths are f16 with different rounding points (cuDNN keeps BN folded in the weights)
-
-
 @pytest.mark.parametrize("kind", ["blobs", "noise", "flat"])
 def test_det_peaks_kernel_matches_reference_decode(cuda, kind):
     """CUDA decode (sigmoid + 7x7 NMS + top-15 + map reads) vs the torch restatement of extract_peak / det_inference."""

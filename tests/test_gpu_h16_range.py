@@ -279,12 +279,8 @@ def test_pool2_affine_relu_h16_saturates(cuda):
 
 
 # ------------------------------------------------------------------------------------------------------------ pillar encoders
-@pytest.mark.parametrize("encoder", ["sorted", "tiled"])
-@pytest.mark.parametrize("out_mode", [1, 2])
-def test_pillar_encoders_h16_canvas_saturates(cuda, encoder, out_mode, monkeypatch):
-    """the tensor-core pillar encoders with the second layer's BatchNorm affine enlarged.  out_mode 2: h16 canvas, saturating;
-    out_mode 1: [hi | lo] split, hi saturating and hi + lo the fp32 value up to 2 x 65504."""
-    monkeypatch.setattr(ops, "PILLAR_ENCODER", encoder)
+def test_pillar_encoders_h16_canvas_saturates(cuda):
+    """the tensor-core pillar encoder with the second layer's BatchNorm affine enlarged: the h16 canvas (out_mode 2) saturates."""
     m, sd = util.lidar_model(cuda)
     m.set_precision("f16")
     pp = m.point_pillar_net
@@ -299,42 +295,20 @@ def test_pillar_encoders_h16_canvas_saturates(cuda, encoder, out_mode, monkeypat
     buf, starts, counts = pp._as_buffer([c.to(cuda) for c in clouds], npts)
     with torch.no_grad():
         got = ops.pillar_forward_sorted(buf, starts, counts, pp._grid(), w1, s1, t1, w2, (s2 * k).contiguous(), (t2 * k).contiguous(),
-                                        split_out=out_mode == 1, canvas16=out_mode == 2).double().cpu()
+                                        canvas16=True).double().cpu()
     # layer 2 on h16 operands: the existing parity test allows 1e-3 of the canvas scale, here that of the unsaturated canvas
-    scale = float(raw.abs().max())
-    if out_mode == 2:
-        check(got, raw, store(raw), 1e-3, both_signs=False, live=live, scale=scale)
-        return
-    hi, lo = got[..., :64], got[..., 64:]
-    assert bool(torch.isfinite(got).all())
-    check(hi, raw, store(raw), 1e-3, both_signs=False, live=live, scale=scale)
-    hi_ref = store(raw)
-    sum_ref = hi_ref + store(raw - hi_ref)          # lo saturates too: the split holds at most 2 x 65504
-    assert float((hi + lo - sum_ref).abs().max()) / scale < 1e-3
+    check(got, raw, store(raw), 1e-3, both_signs=False, live=live, scale=float(raw.abs().max()))
 
 
 # ------------------------------------------------------------------------------------------------------------- dtype helpers
 def test_convert_f32_to_h16_saturates_at_the_boundaries(cuda):
-    """65504 is the largest half; 65519.99 rounds to it; from 65520 on, round-to-nearest gives inf and the contract 65504"""
+    """65504 is the largest half; 65519.99 rounds to it; from 65520 on, round-to-nearest gives inf and the contract 65504.
+    This is the conversion ConvBackbone applies to an fp32 canvas on the 16-bit path."""
     edge = [65504.0, 65505.0, 65519.0, 65519.99, 65520.0, 65536.0, 1e5, 3.0e38, 65503.0, 65488.0, 1.0, 0.0]
     x = torch.tensor(edge + [-v for v in edge], dtype=torch.float32)
     got = ops.convert(x.to(cuda), torch.float16).cpu()
     want = x.double().clamp(-H, H).to(torch.float16)
     assert torch.equal(got, want), (x[got != want].tolist(), got[got != want].tolist())
-
-
-def test_split_h16_saturates_hi_and_keeps_the_sum(cuda):
-    """lavb_split_h16 for |x| up to 131000: hi = sat(x) rounded, lo = h16(x - hi), hi + lo within one h16 rounding of x"""
-    g = gen("split")
-    x = ((torch.rand(2048, 32, generator=g) * 2 - 1) * 131000).float()
-    x[0, :8] = torch.tensor([65504., 65519.99, 65520., 131000., -65504., -65520., -131000., 1e-3])
-    out = ops.split_h16(x.to(cuda)).cpu()
-    hi, lo = out[:, :32], out[:, 32:]
-    assert bool(torch.isfinite(out).all())
-    assert torch.equal(hi, x.double().clamp(-H, H).to(torch.float16))
-    d = x.double() - hi.double()                                    # exact
-    assert torch.equal(lo, d.to(torch.float16))
-    assert bool(((hi.double() + lo.double() - x.double()).abs() <= d.abs() * 2.0 ** -11 + 2.0 ** -25).all())
 
 
 def test_crop_bilinear_h16_full_range_stays_finite(cuda):
