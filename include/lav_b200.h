@@ -107,6 +107,21 @@ int lavb_stack_jobs(const void* d_jobs, int n_jobs, int max_n, int src_cols, int
  * The output is bit-identical to OpenCV's fixed-point 8-bit warp chain; every output byte is 0 or 1. */
 int lavb_bev_targets(const void* d_jobs, int n_jobs, const uint8_t* d_src, uint8_t* d_out, int h, int w, void* stream);
 
+/* ---------------------------------------------------------------- grayscale PNG maps of a recording
+ * replaces: BasicDataset.load_bev's cv2.imdecode(..., cv2.IMREAD_GRAYSCALE) of each map_%d_%05d plane
+ *           (lav/utils/datasets/basic_dataset.py:94,99).
+ * One launch decodes n_jobs 8-bit grayscale, non-interlaced PNG images into (n_planes, h, w) uint8 planes at d_out.  The host
+ * walks the chunks; d_src (src_bytes bytes) holds each image's IDAT payloads concatenated, i.e. its zlib stream.  d_jobs is a
+ * DEVICE array of n_jobs 32-byte records
+ *   { long long off, len; int dst, h, w, pad; }
+ * stream = bytes [off, off + len) of d_src, dst = output plane, h / w = the IHDR size (must equal the launch's h / w).
+ * d_status: DEVICE int32[n_jobs], 0 = decoded, bit-identical to libpng; otherwise the job's stream is malformed (zlib header,
+ * deflate block, code lengths, symbol, distance, inflated size != h * (w + 1), Adler-32, filter byte > 4: the codes of
+ * lavb_png::PngStatus in png_inflate.cuh).  Every read stays inside the job's stream and every write inside its plane, so a
+ * malformed job leaves all other bytes, and the other jobs, untouched.  Jobs must name distinct planes. */
+int lavb_png_decode_gray8(const uint8_t* d_src, long long src_bytes, const void* d_jobs, int n_jobs, uint8_t* d_out,
+                          int n_planes, int h, int w, int* d_status, void* stream);
+
 /* ---------------------------------------------------------------- LiDAR rows of a training batch
  * replaces: one GpuLidarStacker call per sample (lav_b200/data_pipeline.py; TemporalLiDARPaintedDataset.__getitem__,
  *           temporal_lidar_painted_dataset.py:13-91): roof filter, rotate_lidar(-angle), the camera-FOV re-mask of the painted

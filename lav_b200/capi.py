@@ -57,6 +57,8 @@ _SIGS = {
                                             C.c_void_p]),
     "lavb_stack_jobs": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p]),
     "lavb_bev_targets": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p]),
+    "lavb_png_decode_gray8": (C.c_int, [C.c_void_p, C.c_longlong, C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_int,
+                                        C.c_void_p, C.c_void_p]),
     "lavb_lidar_batch": (C.c_int, [C.c_void_p, C.c_longlong, C.c_int, C.c_void_p, C.c_longlong, C.c_void_p, C.c_int, C.c_void_p,
                                    C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
     "lavb_det_heatmaps": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_float, C.c_float, C.c_float, C.c_float,

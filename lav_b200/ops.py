@@ -483,6 +483,45 @@ def bev_targets(src_planes, jobs, out=None):
     return out
 
 
+PNG_JOB_DTYPE = np.dtype([("off", np.int64), ("len", np.int64), ("dst", np.int32), ("h", np.int32), ("w", np.int32),
+                          ("pad", np.int32)])
+assert PNG_JOB_DTYPE.itemsize == 32
+
+
+def png_decode_gray8(src, jobs, out, status=None):
+    """8-bit grayscale PNG images -> uint8 planes in one launch (see lavb_png_decode_gray8 in include/lav_b200.h), as
+    cv2.imdecode(..., IMREAD_GRAYSCALE).  src: 1-D uint8 CUDA tensor of the images' zlib streams (their IDAT payloads,
+    concatenated); jobs: PNG_JOB_DTYPE records (off, len, dst, h, w); out: contiguous (P, h, w) uint8 CUDA tensor, every job's (h, w)
+    equal to its planes'.  -> status (n_jobs,) int32 on the device, 0 where the image decoded; a nonzero entry marks a malformed
+    stream whose plane holds garbage.  The other planes of out are not written."""
+    _need_cuda(src, out, status)
+    if src.dtype != torch.uint8 or src.dim() != 1 or not src.is_contiguous():
+        raise capi.LavbError(f"png_decode_gray8: src must be a contiguous 1-D uint8 tensor, got {src.dtype} {tuple(src.shape)}")
+    if out.dtype != torch.uint8 or out.dim() != 3 or not out.is_contiguous() or out.device != src.device:
+        raise capi.LavbError(f"png_decode_gray8: out must be a contiguous (P, h, w) uint8 tensor on {src.device}")
+    jobs = np.ascontiguousarray(jobs, dtype=PNG_JOB_DTYPE)
+    P, h, w = out.shape
+    if not (0 < h <= 4096 and 0 < w <= 4096):
+        raise capi.LavbError(f"png_decode_gray8: plane size {h}x{w} outside 1..4096")
+    if len(jobs) and ((jobs["h"] != h).any() or (jobs["w"] != w).any()):
+        raise capi.LavbError(f"png_decode_gray8: a job's size differs from the {h}x{w} planes")
+    if len(jobs) and ((jobs["dst"] < 0).any() or (jobs["dst"] >= P).any() or len(np.unique(jobs["dst"])) != len(jobs)):
+        raise capi.LavbError(f"png_decode_gray8: job planes must be distinct and in 0..{P - 1}")
+    if len(jobs) and ((jobs["off"] < 0).any() or (jobs["len"] < 0).any() or (jobs["off"] + jobs["len"] > src.numel()).any()):
+        raise capi.LavbError(f"png_decode_gray8: a job's stream lies outside the {src.numel()}-byte source")
+    if status is None:
+        status = torch.empty(len(jobs), dtype=torch.int32, device=src.device)
+    elif status.dtype != torch.int32 or status.numel() != len(jobs) or not status.is_contiguous() or status.device != src.device:
+        raise capi.LavbError(f"png_decode_gray8: status must be a contiguous ({len(jobs)},) int32 tensor on {src.device}")
+    if len(jobs) == 0:
+        return status
+    d_jobs = _to_device(jobs.view(np.uint8), src.device)
+    check(lib().lavb_png_decode_gray8(_ptr(src), src.numel(), _ptr(d_jobs), len(jobs), _ptr(out), P, h, w, _ptr(status), _stream()),
+          "lavb_png_decode_gray8")
+    _COUNT[0] += 1
+    return status
+
+
 def _to_device(a, device):
     """host array -> device tensor through pinned staging, without a host synchronisation (the pinned block is not reused
     before the copy has run: the caching host allocator records the copy's stream)."""

@@ -38,12 +38,12 @@ def gpu_info():
     return q.stdout.strip().splitlines()[0] if q.returncode == 0 and q.stdout.strip() else torch.cuda.get_device_name()
 
 
-def per_sample_device(ds, hs, planes, gen):
+def per_sample_device(ds, hs, decoded, gen):
     """the device part of a batch as the loader built it before the batched kernels: per sample GpuLidarStacker and
     detections_to_heatmap, one bev_targets launch, and the label copies."""
     dev = ds.device
     parts = [ds.lidar_and_maps(h, gen) for h in hs]
-    bev = ds.bev_batch(hs, planes.to(dev, non_blocking=True))
+    bev = ds.bev_batch(hs, decoded)
     st = lambda i: torch.stack([p[i] for p in parts])
     f32 = lambda key: torch.as_tensor(np.stack([h[key] for h in hs]), dtype=torch.float32).to(dev)
     ints = lambda key: torch.tensor([h[key] for h in hs], dtype=torch.int64)
@@ -55,6 +55,7 @@ def per_sample_device(ds, hs, planes, gen):
 def breakdown(ds, B, workers, reps):
     """seconds per batch of B samples: host prepare (1 and `workers` threads), host tables, the two device paths."""
     from concurrent.futures import ThreadPoolExecutor
+    from lav_b200.datasets import stage_maps
     rng = np.random.RandomState(B)
     idxs = list(range(B))
     draws = [ds.draw(rng) for _ in idxs]
@@ -68,10 +69,10 @@ def breakdown(ds, B, workers, reps):
             t2 = time.perf_counter()
             st = ds.stage_batch(hs, torch.Generator().manual_seed(r))
             t3 = time.perf_counter()
-            planes = torch.from_numpy(np.concatenate([h["planes"] for h in hs])).pin_memory()
+            decoded = ds.decode_maps(stage_maps(hs, True))
             torch.cuda.synchronize()
             t4 = time.perf_counter()
-            old = per_sample_device(ds, hs, planes, torch.Generator().manual_seed(r))
+            old = per_sample_device(ds, hs, decoded, torch.Generator().manual_seed(r))
             torch.cuda.synchronize()
             t5 = time.perf_counter()
             new = ds.launch_batch(st)
@@ -139,12 +140,13 @@ def main():
 
     # 2. bev_targets alone
     hs = [ds.prepare(i, *ds.draw(ds.rng)) for i in range(args.batch)]
-    planes = torch.from_numpy(np.concatenate([h["planes"] for h in hs])).to(dev)
+    from lav_b200.datasets import stage_maps
+    planes = ds.planes_on_stream(ds.decode_maps(stage_maps(hs, True)))
     n_bev = 3 + 2 * (ds.num_frame_stack + 1)
-    jobs = ops.bev_jobs([(s + sum(len(x["planes"]) for x in hs[:b]) if s >= 0 else -1, b * n_bev + d, a1, a2, dx, dy)
+    jobs = ops.bev_jobs([(s + sum(len(x["pngs"]) for x in hs[:b]) if s >= 0 else -1, b * n_bev + d, a1, a2, dx, dy)
                          for b, h in enumerate(hs) for s, d, a1, a2, dx, dy in h["rows"]])
     out = torch.empty((len(hs), n_bev, 320, 320), dtype=torch.uint8, device=dev)
-    assert torch.equal(ops.bev_targets(planes, jobs, out), ds.bev_batch(hs, planes))
+    assert torch.equal(ops.bev_targets(planes, jobs, out), ds.bev_batch(hs))
     torch.cuda.synchronize()
     reps = 50
     e0.record()
