@@ -155,6 +155,29 @@ int lavb_lidar_batch(const float* d_raw, long long n_raw, int c, const int* d_ro
 int lavb_det_heatmaps(const void* d_actors, const int* d_offsets, int b, int h, int w, float ppm, float cx0, float cy0, float cy1,
                       float inv_radius, float* d_heat, float* d_size, float* d_ori, void* stream);
 
+/* ---------------------------------------------------------------- scores of an evaluation batch
+ * replaces: the comparisons LAV.train_lidar draws for wandb (lav/lav_final_v2.py:226-258): predicted detections against gt_det,
+ *           ego_plan_locs against the expert's ego_locs, pred_bev against the GT bev — as counts over every sample of a batch.
+ * One block per sample (batches of more than 256 samples take one launch per 256).
+ * BEV: d_seg (b, h, w, 3) NHWC sigmoid probabilities, fp32 or h16 (seg_dtype); d_gt (b, gt_planes, h, w) uint8, planes 0..2 the
+ *   targets.  d_iou (b, 3, 2) int64 = per channel (|pred > 0.5 and gt != 0|, |pred > 0.5 or gt != 0|).  h * w % 4 == 0.
+ * Detections: d_packed (b, 7, 2 * n_det) fp32 = lavb_det_peaks' output (class c in columns [c * n_det, (c + 1) * n_det)), the
+ *   peak pixel (flat % w, flat / w).  A peak survives InferModel.decode_packed's filters: score > min_score, not (class 1 and both
+ *   box sides < float32(0.1 * ppm)), and 2 < d < 30 * ppm pixels from (cx0, cy0 + cy1).  d_actors: lavb_det_heatmaps' table
+ *   (24-byte records, n_actors rows), sample i owning rows [h_offsets[i], h_offsets[i+1]) (HOST int32[b+1], monotone, at most
+ *   1024 rows per sample); an actor of class typ (0 / 1, others ignored) counts when its centre, placed as lavb_det_heatmaps
+ *   places it, lies in the same window.  Per class and threshold t in {0.5, 1, 2, 4} m, the survivors in descending score (ties:
+ *   lower flat index, then lower column) each take the nearest untaken actor of their class with squared pixel distance
+ *   <= (t * ppm)^2 (fp64, ties: lower row).  d_ngt (b, 2) int32 = actors counted per class; d_score (b, 2 * n_det) fp32 = the
+ *   packed scores; d_flags (b, 2 * n_det) int32 = bit 4 set for a survivor, bit k for a match at threshold k.
+ * Plan: d_plan (b, n_plan, 2) fp32, d_ego_locs (b, n_plan + 1, 2) fp32 with entry 0 the origin; d_plan_err (b, 2) fp64 = (mean
+ *   over the steps of |plan[t] - ego_locs[t+1]|, the error at the last step).  n_plan <= 32.
+ * Every output element of the b samples is written; a rejected call writes nothing. */
+int lavb_eval_batch(const void* d_seg, int seg_dtype, const uint8_t* d_gt, int gt_planes, int b, int h, int w, const float* d_packed,
+                    int n_det, const void* d_actors, int n_actors, const int* h_offsets, float ppm, float cx0, float cy0, float cy1,
+                    double min_score, const float* d_plan, const float* d_ego_locs, int n_plan, long long* d_iou, int* d_ngt,
+                    float* d_score, int* d_flags, double* d_plan_err, void* stream);
+
 /* ---------------------------------------------------------------- PointPillars voxeliser + pillar encoder
  * replaces: PointPillarNet.forward (lav/models/point_pillar.py:92-116) incl. grid_locations :70-79,
  *           pillar_generation/decorate :55-68,81-85, DynamicPointNet.forward :28-35 (torch_scatter

@@ -64,6 +64,33 @@ def stack_into(dst, sweeps, roof_filter=False):
     return row
 
 
+def infer_model(lidar_model, uniplanner, precision, camera_x, camera_z, device):
+    """The InferModel of the agent at ``precision``: ``lidar_model`` switched to it in place; the UniPlanner's embedder cast on a
+    PRIVATE copy of ``uniplanner``, so a model object shared with a trainer / checkpoint writer / fp32 parity check keeps its fp32
+    master weights."""
+    lidar_model.set_precision(precision)
+    dt = ops.h16() if precision == "f16" else torch.float32
+    up = copy.deepcopy(uniplanner)
+    up.lidar_conv_emb.to(dt).to(memory_format=torch.channels_last)
+    return InferModel(lidar_model, up, camera_x, camera_z, device)
+
+
+@contextlib.contextmanager
+def math_mode(precision):
+    """exact path: the cuDNN / cuBLAS heads must not drop to TF32 — scoped to the caller's block, the process-wide flags are
+    restored afterwards."""
+    if precision != "fp32":
+        yield
+        return
+    prev = (torch.backends.cudnn.allow_tf32, torch.backends.cuda.matmul.allow_tf32)
+    torch.backends.cudnn.allow_tf32 = False
+    torch.backends.cuda.matmul.allow_tf32 = False
+    try:
+        yield
+    finally:
+        torch.backends.cudnn.allow_tf32, torch.backends.cuda.matmul.allow_tf32 = prev
+
+
 class FramePipeline:
     def __init__(self, seg_model, lidar_model, uniplanner, bra_model, camera_x=1.5, camera_z=2.4, device=torch.device("cuda"),
                  precision="f16"):
@@ -81,11 +108,8 @@ class FramePipeline:
         assert precision in ("fp32", "f16"), precision
         self.precision = precision
         self.seg_model.set_precision(precision)
-        self._lidar_model.set_precision(precision)
+        self.infer_model = infer_model(self._lidar_model, self._src_uniplanner, precision, self._cam[0], self._cam[1], self.device)
         dt = ops.h16() if precision == "f16" else torch.float32
-        up = copy.deepcopy(self._src_uniplanner)
-        up.lidar_conv_emb.to(dt).to(memory_format=torch.channels_last)
-        self.infer_model = InferModel(self._lidar_model, up, self._cam[0], self._cam[1], self.device)
         if self._src_bra is not None:
             bra = copy.deepcopy(self._src_bra)
             bra.conv_backbone.to(dt).to(memory_format=torch.channels_last)
@@ -93,20 +117,8 @@ class FramePipeline:
             self.bra_model = bra
         return self
 
-    @contextlib.contextmanager
     def _math_mode(self):
-        """exact path: the cuDNN / cuBLAS heads must not drop to TF32 — scoped to the pipeline's own calls, the process-wide
-        flags are restored afterwards."""
-        if self.precision != "fp32":
-            yield
-            return
-        prev = (torch.backends.cudnn.allow_tf32, torch.backends.cuda.matmul.allow_tf32)
-        torch.backends.cudnn.allow_tf32 = False
-        torch.backends.cuda.matmul.allow_tf32 = False
-        try:
-            yield
-        finally:
-            torch.backends.cudnn.allow_tf32, torch.backends.cuda.matmul.allow_tf32 = prev
+        return math_mode(self.precision)
 
     @torch.no_grad()
     def step(self, rgbs_u8, tel_u8, lidars, histories, nxps, cmds, poses=None):

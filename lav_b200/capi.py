@@ -63,6 +63,10 @@ _SIGS = {
                                    C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
     "lavb_det_heatmaps": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_float, C.c_float, C.c_float, C.c_float,
                                     C.c_float, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "lavb_eval_batch": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_int,
+                                  C.c_void_p, C.c_int, C.c_void_p, C.c_float, C.c_float, C.c_float, C.c_float, C.c_double,
+                                  C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                  C.c_void_p]),
     "lavb_roof_filter": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_longlong, C.c_void_p, C.c_longlong, C.c_void_p, C.c_int,
                                    C.c_void_p]),
     "lavb_stack_sweep": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_float, C.c_float, C.c_int, C.c_int, C.c_int,

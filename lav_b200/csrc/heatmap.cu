@@ -1,25 +1,23 @@
 // Detection targets of a training batch in one launch: the heat, size and orientation maps of LiDARDataset.detections_to_heatmap
 // (lidar_dataset.py:92-127) for every sample, restating data_pipeline.detections_to_heatmap (the same computation in torch ops)
 // operation for operation so that the maps are bit-identical to it.
-#include "common.cuh"
+#include "det_grid.cuh"
 
 namespace {
 
-struct DetActor { float x, y, ori, bx, by, typ; };   // 24 bytes: ego-frame metres, radians, box extents, class (0 / 1)
-static_assert(sizeof(DetActor) == 24, "DetActor layout is part of the ABI (lav_b200.h)");
-
-struct DetGrid { float ppm, cx0, cy0, cy1, inv_r; };
+using lavb::DetActor;
+using lavb::DetGrid;
 
 // torch's arg-max over a reduced dimension (GreaterOrNan in ATen's SharedReduceOps.h): a NaN beats everything, the larger value
 // wins, and a tie keeps the lower index.  Actors are visited in index order, so "take" means strictly better.
 __device__ __forceinline__ bool better(float best, float v) { return !isnan(best) && (isnan(v) || v > best); }
 
-// gx * gy of one actor at pixel (px, py): torch computes cx = -x * ppm + cx0 and cy = (-y * ppm + cy0) + cy1 as separate fp32 ops,
-// (p - c) / radius as (p - c) * (1 / radius), ** 2 as d * d, then exp of the negation, then the product of the two separable
-// factors.  The _rn intrinsics keep nvcc from contracting any of it into an FMA.
+// gx * gy of one actor at pixel (px, py): the centre as lavb::det_centre, then torch's (p - c) / radius as (p - c) * (1 / radius),
+// ** 2 as d * d, then exp of the negation, then the product of the two separable factors.  The _rn intrinsics keep nvcc from
+// contracting any of it into an FMA.
 __device__ __forceinline__ float gauss(const DetActor& a, const DetGrid& g, float px, float py) {
-  const float cx = __fadd_rn(__fmul_rn(-a.x, g.ppm), g.cx0);
-  const float cy = __fadd_rn(__fadd_rn(__fmul_rn(-a.y, g.ppm), g.cy0), g.cy1);
+  const float2 c = lavb::det_centre(a, g);
+  const float cx = c.x, cy = c.y;
   const float dx = __fmul_rn(__fsub_rn(px, cx), g.inv_r), dy = __fmul_rn(__fsub_rn(py, cy), g.inv_r);
   return __fmul_rn(expf(-__fmul_rn(dx, dx)), expf(-__fmul_rn(dy, dy)));
 }

@@ -111,11 +111,13 @@ class TemporalLiDARPaintedDataset:
     orimaps (2,320,320) f32, bev (9,320,320) uint8, -ego_locs (T+1,2) f64, cmd, -nxp (2,) f64, bra, -locs (max_objs,T+1,2) f32,
     oris (max_objs,) f32, typs (max_objs,) int32, num_objs.  ``sample(idx, angle, jitters, generator)`` takes the random draws
     explicitly; ``ds[i]`` draws them from generators seeded with ``seed``.  The draws have the reference's distributions but not
-    its random streams: the same seed gives other (equally distributed) augmentations than the reference."""
+    its random streams: the same seed gives other (equally distributed) augmentations than the reference.  ``overrides``
+    replaces keys of the YAML (the evaluator's --data-dir)."""
 
-    def __init__(self, config_path, seed=2021, device=torch.device("cuda")):
+    def __init__(self, config_path, seed=2021, device=torch.device("cuda"), overrides=None):
         with open(config_path) as f:
             cfg = yaml.safe_load(f)
+        cfg.update(overrides or {})
         self.cfg = cfg
         for k, v in cfg.items():
             setattr(self, k, v)
@@ -145,6 +147,10 @@ class TemporalLiDARPaintedDataset:
                                        float(rng.uniform(-self.stack_ori_jitter, self.stack_ori_jitter)))
                                       for _ in range(self.num_frame_stack)]
         return angle, jit
+
+    def no_draw(self):
+        """the draws of an unaugmented sample: angle 0 and zero stack jitters."""
+        return 0.0, [(np.zeros(2), 0.0)] * (self.num_frame_stack + 1)
 
     # ---- host part: record reads, PNG chunk walks, labels, BEV job rows
     def prepare(self, idx, angle, jitters):
@@ -332,15 +338,19 @@ class TemporalBatchLoader:
     a malformed map is yielded); the rest of the device part is launch_batch.  A batch is the 14-tuple
     lidars (B,P,4+C+T) f32, num_points (B,) int64 (host), heatmaps / sizemaps / orimaps (B,2,320,320) f32, bev (B,9,320,320)
     uint8, ego_locs (B,T+1,2) f32, cmds (B,) int64, nxps (B,2) f32, bras (B,) int64, locs (B,max_objs,T+1,2) f32, oris
-    (B,max_objs) f32, typs (B,max_objs) int32, num_objs (B,) int64; train_lidar takes the first 13."""
+    (B,max_objs) f32, typs (B,max_objs) int32, num_objs (B,) int64; train_lidar takes the first 13.
 
-    def __init__(self, dataset, batch_size, seed=2021, rank=0, world=1, drop_last=True, num_workers=8):
+    With ``ordered`` (evaluation) the samples come in index order with no augmentation: every draw is dataset.no_draw(), and the
+    LiDAR shuffles still come from the generator of (seed, epoch, rank)."""
+
+    def __init__(self, dataset, batch_size, seed=2021, rank=0, world=1, drop_last=True, num_workers=8, ordered=False):
         self.ds, self.B, self.seed, self.rank, self.world, self.drop_last = dataset, batch_size, seed, rank, world, drop_last
         self.num_workers = max(1, int(num_workers))
+        self.ordered = ordered
         self.epoch = 0
 
     def shard(self, epoch):
-        perm = np.random.RandomState([self.seed, epoch]).permutation(len(self.ds))
+        perm = np.arange(len(self.ds)) if self.ordered else np.random.RandomState([self.seed, epoch]).permutation(len(self.ds))
         return perm[self.rank::self.world][:len(self.ds) // self.world]
 
     def __len__(self):
@@ -359,20 +369,27 @@ class TemporalBatchLoader:
         return st
 
     def __iter__(self):
+        for batch, _ in self.staged_batches():
+            yield batch
+
+    def staged_batches(self):
+        """the batches of the next epoch as (14-tuple, the host tables stage_batch made for it): the evaluator reads the actor
+        table ("actors", "offsets") that the tuple does not carry."""
         epoch, self.epoch = self.epoch, self.epoch + 1
         order = self.shard(epoch)
         batches = [order[k * self.B:(k + 1) * self.B] for k in range(len(self))]
         rng, gen = self.generators(epoch)
         if not batches:
             return
-        draws = lambda idxs: [self.ds.draw(rng) for _ in idxs]                  # on this thread, in sample order
+        draw = self.ds.no_draw if self.ordered else lambda: self.ds.draw(rng)
+        draws = lambda idxs: [draw() for _ in idxs]                             # on this thread, in sample order
         with ThreadPoolExecutor(1) as ahead, ThreadPoolExecutor(self.num_workers) as pool:
             nxt = ahead.submit(self._host, batches[0], draws(batches[0]), gen, pool)
             for k in range(len(batches)):
                 staged = nxt.result()
                 if k + 1 < len(batches):
                     nxt = ahead.submit(self._host, batches[k + 1], draws(batches[k + 1]), gen, pool)
-                yield self.ds.launch_batch(staged)
+                yield self.ds.launch_batch(staged), staged
 
 
 class TemporalBEVDataset:

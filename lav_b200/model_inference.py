@@ -107,13 +107,15 @@ class InferModel(nn.Module):
     @torch.no_grad()
     def forward_batch(self, lidars, num_points, nxps, cmd_values):
         """B independent frames.  lidars: list of (P_b,11) tensors or (B,P,11); nxps (B,2); cmd_values (B,).
-        Returns dict of batched outputs; 'det' is the per-frame detection list of the reference."""
+        Returns dict of batched outputs; 'det' is the per-frame detection list of the reference, 'packed' the device peaks it
+        was decoded from (ops.det_peaks)."""
         from . import ops
         feats, center, box, ori, seg = self.lidar_model.forward_nhwc(lidars, num_points)
-        dets = self.decode_packed(ops.det_peaks(center, box, ori))
+        packed = ops.det_peaks(center, box, ori)
+        dets = self.decode_packed(packed)
         ee, epl, ecl, ocl, occ = self.uniplanner.infer_batch(feats.permute(0, 3, 1, 2), [d[1] for d in dets], cmd_values, nxps)
         return dict(ego_embd=ee, ego_plan_locs=epl, ego_cast_locs=ecl, other_cast_locs=ocl, other_cast_cmds=occ,
-                    pred_bev=seg.permute(0, 3, 1, 2), det=dets, features=feats)
+                    pred_bev=seg.permute(0, 3, 1, 2), det=dets, features=feats, packed=packed)
 
     @torch.no_grad()
     def forward(self, lidar_points, nxps, cmd_value):

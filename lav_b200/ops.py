@@ -598,6 +598,72 @@ def det_heatmaps(actors, offsets, grid=None, out=None):
     return heat, size, orim
 
 
+def _eval_layout(b, ncols):
+    """(name, dtype, shape, byte offset) of the parts of eval_batch's result buffer, 8-byte parts first, and its size."""
+    parts = [("iou", torch.int64, (b, 3, 2)), ("plan_err", torch.float64, (b, 2)), ("ngt", torch.int32, (b, 2)),
+             ("score", torch.float32, (b, ncols)), ("flags", torch.int32, (b, ncols))]
+    out, pos = [], 0
+    for name, dt, shape in parts:
+        out.append((name, dt, shape, pos))
+        pos += int(np.prod(shape)) * torch.empty((), dtype=dt).element_size()
+    return out, pos
+
+
+def eval_views(buf, b, ncols):
+    """the named parts of an eval_batch result buffer (on the device or a host copy of it): iou (b,3,2) int64 = per BEV channel
+    (intersection, union); plan_err (b,2) fp64 = (ADE, FDE); ngt (b,2) int32 = actors per class in the window; score / flags
+    (b, ncols) = the packed scores and, per column, bit 4 for a surviving peak and bit k for a match at EVAL_THRESHOLDS_M[k]."""
+    layout, _ = _eval_layout(b, ncols)
+    return {name: buf[pos:pos + int(np.prod(shape)) * torch.empty((), dtype=dt).element_size()].view(dt).view(shape)
+            for name, dt, shape, pos in layout}
+
+
+EVAL_THRESHOLDS_M = (0.5, 1.0, 2.0, 4.0)      # centre-distance thresholds of the detection matching (evaluate.cu)
+
+
+def eval_batch(seg, gt, packed, actors, offsets, plan, ego_locs, grid=None, min_score=0.2, out=None):
+    """The scores of one evaluation batch in one launch (see lavb_eval_batch in include/lav_b200.h).  seg (B,H,W,3) NHWC sigmoid
+    probabilities, fp32 or h16; gt (B,P>=3,H,W) uint8; packed (B,7,2*n_det) fp32 from det_peaks; actors (A,6) fp32 (the
+    det_heatmaps table, on the device); offsets (B+1,) int32 on the HOST; plan (B,T,2) and ego_locs (B,T+1,2) fp32; grid: the
+    keyword arguments of det_grid.  -> the uint8 result buffer (written into ``out`` when given), to be read through eval_views,
+    usually after one copy to the host."""
+    _need_cuda(seg, gt, packed, actors, plan, ego_locs)
+    if seg.dim() != 4 or seg.shape[3] != 3 or seg.dtype not in (torch.float32, h16()) or not seg.is_contiguous():
+        raise capi.LavbError(f"eval_batch: seg must be a contiguous (B,H,W,3) fp32 or {h16()} tensor, got {seg.dtype} {tuple(seg.shape)}")
+    b, h, w, _ = seg.shape
+    if gt.dtype != torch.uint8 or gt.dim() != 4 or gt.shape[0] != b or tuple(gt.shape[2:]) != (h, w) or not gt.is_contiguous():
+        raise capi.LavbError(f"eval_batch: gt must be a contiguous ({b}, P, {h}, {w}) uint8 tensor, got {gt.dtype} {tuple(gt.shape)}")
+    if packed.dtype != torch.float32 or packed.dim() != 3 or packed.shape[:2] != (b, 7) or packed.shape[2] % 2 \
+            or not packed.is_contiguous():
+        raise capi.LavbError(f"eval_batch: packed must be a contiguous ({b}, 7, 2*n_det) fp32 tensor, got {tuple(packed.shape)}")
+    if actors.dtype != torch.float32 or actors.dim() != 2 or actors.shape[1] != 6 or not actors.is_contiguous():
+        raise capi.LavbError(f"eval_batch: actors must be a contiguous (A, 6) fp32 tensor, got {actors.dtype} {tuple(actors.shape)}")
+    offsets = np.ascontiguousarray(offsets.numpy() if torch.is_tensor(offsets) else offsets)
+    if offsets.dtype != np.int32 or offsets.shape != (b + 1,):
+        raise capi.LavbError(f"eval_batch: offsets must be a host ({b + 1},) int32 array, got {offsets.dtype} {offsets.shape}")
+    t = plan.shape[1] if plan.dim() == 3 else -1
+    if plan.dtype != torch.float32 or tuple(plan.shape) != (b, t, 2) or not plan.is_contiguous() or ego_locs.dtype != torch.float32 \
+            or tuple(ego_locs.shape) != (b, t + 1, 2) or not ego_locs.is_contiguous():
+        raise capi.LavbError(f"eval_batch: plan ({b}, T, 2) and ego_locs ({b}, T+1, 2) must be contiguous fp32, got "
+                             f"{plan.dtype} {tuple(plan.shape)} / {ego_locs.dtype} {tuple(ego_locs.shape)}")
+    if len({seg.device, gt.device, packed.device, actors.device, plan.device, ego_locs.device}) != 1:
+        raise capi.LavbError("eval_batch: the inputs must be on one device")
+    ncols = packed.shape[2]
+    _, nbytes = _eval_layout(b, ncols)
+    if out is None:
+        out = torch.empty((nbytes,), dtype=torch.uint8, device=seg.device)
+    elif out.dtype != torch.uint8 or tuple(out.shape) != (nbytes,) or out.device != seg.device:
+        raise capi.LavbError(f"eval_batch: out must be a ({nbytes},) uint8 tensor on {seg.device}")
+    v = eval_views(out, b, ncols)
+    _, _, (ppm, cx0, cy0, cy1, _) = det_grid(**(grid or {}))
+    check(lib().lavb_eval_batch(_ptr(seg), _DT[seg.dtype], _ptr(gt), gt.shape[1], b, h, w, _ptr(packed), ncols // 2, _ptr(actors),
+                                actors.shape[0], offsets.ctypes.data_as(C.c_void_p), ppm, cx0, cy0, cy1, float(min_score), _ptr(plan),
+                                _ptr(ego_locs), t, _ptr(v["iou"]), _ptr(v["ngt"]), _ptr(v["score"]), _ptr(v["flags"]),
+                                _ptr(v["plan_err"]), _stream()), "lavb_eval_batch")
+    _COUNT[0] += -(-b // 256)
+    return out
+
+
 PILLAR_ENCODER = "sorted"    # name of the 16-bit pipeline's pillar encoder, reported by bench.py; it selects nothing
 
 

@@ -42,24 +42,29 @@ def parse_args(argv=None):
     return args
 
 
-def build_models(cfg, perceive_only=False, motion_only=False):
-    """LAV.__init__'s models (lav_final_v2.py:31-72): LiDARModel, the frozen BEVPlanner teacher and the UniPlanner student, with
-    lidar_model_dir / bev_model_dir / uniplanner_dir loaded as the reference loads them."""
+def make_models(cfg):
+    """LAV.__init__'s models (lav_final_v2.py:31-72), freshly initialised: (LiDARModel, BEVPlanner teacher, UniPlanner student
+    holding that teacher)."""
     if not cfg.get("point_painting", True):
         raise NotImplementedError("only the point-painted LiDAR model (point_painting: True) is provided")
     lid = LiDARModel(num_input=len(cfg["seg_channels"]) + cfg["num_frame_stack"] + 10, num_features=cfg["num_features"],
                      backbone=cfg["backbone"], min_x=cfg["min_x"], max_x=cfg["max_x"], min_y=cfg["min_y"], max_y=cfg["max_y"],
                      pixels_per_meter=cfg["pixels_per_meter"])
-    if not perceive_only:
-        lid.load_state_dict(torch.load(cfg["lidar_model_dir"], map_location="cpu"))
     kw = dict(pixels_per_meter=cfg["pixels_per_meter"], crop_size=cfg["crop_size"], feature_x_jitter=cfg["feature_x_jitter"],
               feature_angle_jitter=cfg["feature_angle_jitter"], x_offset=0,
               y_offset=1 + cfg["min_x"] / ((cfg["max_x"] - cfg["min_x"]) / 2), num_cmds=cfg["num_cmds"], num_plan=cfg["num_plan"],
               num_plan_iter=cfg["num_plan_iter"])
     bev = BEVPlanner(num_frame_stack=cfg["num_frame_stack"], **kw)
+    return lid, bev, UniPlanner(bev, num_input_feature=cfg["num_features"][-1] * 6, **kw)
+
+
+def build_models(cfg, perceive_only=False, motion_only=False):
+    """make_models with lidar_model_dir / bev_model_dir / uniplanner_dir loaded as the reference loads them."""
+    lid, bev, uni = make_models(cfg)
+    if not perceive_only:
+        lid.load_state_dict(torch.load(cfg["lidar_model_dir"], map_location="cpu"))
     bev.load_state_dict(torch.load(cfg["bev_model_dir"], map_location="cpu"))
     bev.eval()
-    uni = UniPlanner(bev, num_input_feature=cfg["num_features"][-1] * 6, **kw)
     if not perceive_only and not motion_only:
         uni.load_state_dict(torch.load(cfg["uniplanner_dir"], map_location="cpu"))
     return lid, uni
