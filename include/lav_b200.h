@@ -178,6 +178,21 @@ int lavb_eval_batch(const void* d_seg, int seg_dtype, const uint8_t* d_gt, int g
                     double min_score, const float* d_plan, const float* d_ego_locs, int n_plan, long long* d_iou, int* d_ngt,
                     float* d_score, int* d_flags, double* d_plan_err, void* stream);
 
+/* ---------------------------------------------------------------- scores of the planners' motion forecasts
+ * replaces: the forecast terms of the planners' training losses (other_cast_loss, ego_cast_loss, cmd_loss in lav_b200.train) as
+ *           displacement errors and branch choices per forecast row, for an evaluation over a recording.
+ * One warp per row, one lane per command branch (batches of any k in one launch).
+ * d_cast (k, c, t, 2) fp32 = the c command branches of each row's forecast; d_score (k, c) fp32 = the command scores;
+ * d_target (k, t, 2) fp32 = the recorded future in the same frame; d_cmd (k,) int32 = the recorded command, or -1 for none.
+ * Per branch j: ADE_j = (sum over steps i in ascending order of |cast[j, i] - target[i]|) / t, FDE_j = the error at step t - 1,
+ * every error in fp64 with no contraction.  d_err (k, 6) fp64 = (min_j ADE_j, min_j FDE_j, ADE and FDE of the top branch,
+ * ADE and FDE of branch cmd, NaN where cmd is outside [0, c)); d_branch (k, 2) int32 = (argmin_j ADE_j, top branch).  The
+ * minima are taken independently, ties go to the lower branch and a NaN error never wins; the top branch has the highest
+ * score, ties to the lower branch, a NaN score counting as lowest.  1 <= c <= 32, 1 <= t <= 32, k >= 0 (k = 0 does nothing).
+ * cast / target / err 8-byte aligned.  Every output element of the k rows is written; a rejected call writes nothing. */
+int lavb_forecast_eval(const float* d_cast, const float* d_score, const float* d_target, const int* d_cmd, int k, int c, int t,
+                       double* d_err, int* d_branch, void* stream);
+
 /* ---------------------------------------------------------------- PointPillars voxeliser + pillar encoder
  * replaces: PointPillarNet.forward (lav/models/point_pillar.py:92-116) incl. grid_locations :70-79,
  *           pillar_generation/decorate :55-68,81-85, DynamicPointNet.forward :28-35 (torch_scatter

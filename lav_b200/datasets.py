@@ -400,11 +400,13 @@ class TemporalBEVDataset:
     -ego_locs (T+1,2) f64, cmd, -nxp (2,) f64, bra, -locs (max_objs,T+1,2) f32, oris (max_objs,) f32, typs (max_objs,) int32,
     num_objs.  ``sample(idx, offset, angle)`` takes the draws explicitly: the column shift ``offset`` in pixels and the rotation
     ``angle`` in degrees.  ``ds[i]`` draws them from ``self.gen``, a torch CPU generator seeded with ``seed``, exactly as the
-    reference draws them from torch's global generator (temporal_bev_dataset.py:28-30), so a seeded stream replays."""
+    reference draws them from torch's global generator (temporal_bev_dataset.py:28-30), so a seeded stream replays.  ``overrides``
+    replaces keys of the YAML (the evaluator's --data-dir)."""
 
-    def __init__(self, config_path, seed=2021, device=torch.device("cuda")):
+    def __init__(self, config_path, seed=2021, device=torch.device("cuda"), overrides=None):
         with open(config_path) as f:
             cfg = yaml.safe_load(f)
+        cfg.update(overrides or {})
         self.cfg = cfg
         for k, v in cfg.items():
             setattr(self, k, v)
@@ -429,6 +431,10 @@ class TemporalBEVDataset:
         offset = int(np.clip(offset, -self.margin, self.margin))
         angle = float(torch.rand(1, generator=gen) * 2 - 1) * self.angle_jitter
         return offset, angle
+
+    def no_draw(self):
+        """the draws of an unaugmented sample: no shift, no rotation."""
+        return 0, 0.0
 
     # ---- host part: record reads, PNG chunk walks, labels, BEV job rows
     def prepare(self, idx, offset, angle):
@@ -485,27 +491,31 @@ class TemporalBEVBatchLoader(TemporalBatchLoader):
     order; record reads and PNG chunk walks run on ``num_workers`` threads and the batch's maps (about 2,300 planes at 256) are
     decoded in one launch on a side stream, one batch ahead of the GPU.  A batch is the 9-tuple bev (B,9,320,320) uint8, ego_locs (B,T+1,2) f32, cmds (B,) int64, nxps (B,2) f32,
     bras (B,) int64, locs (B,max_objs,T+1,2) f32, oris (B,max_objs) f32, typs (B,max_objs) int32, num_objs (B,) int64 (host),
-    with one bev_targets launch per batch."""
+    with one bev_targets launch per batch.  With ``ordered`` (evaluation) the samples come in index order and every draw is
+    dataset.no_draw()."""
 
     def _host_bev(self, idxs, draws, pool):
         hs = list(pool.map(lambda a: self.ds.prepare(int(a[0]), *a[1]), zip(idxs, draws)))
         return hs, self.ds.decode_maps(stage_maps(hs, self.ds.device.type == "cuda"))
 
-    def __iter__(self):
+    def staged_batches(self):
+        """the batches of the next epoch as (9-tuple, the host records dataset.prepare made for it): the evaluator reads the
+        recorded commands there without a copy back from the device."""
         epoch, self.epoch = self.epoch, self.epoch + 1
         order = self.shard(epoch)
         batches = [order[k * self.B:(k + 1) * self.B] for k in range(len(self))]
         gen = torch.Generator(device="cpu").manual_seed(self.seed * 1000003 + epoch * 1009 + self.rank)
         if not batches:
             return
-        draws = lambda idxs: [self.ds.draw(gen) for _ in idxs]                  # on this thread, in sample order
+        draw = self.ds.no_draw if self.ordered else lambda: self.ds.draw(gen)
+        draws = lambda idxs: [draw() for _ in idxs]                             # on this thread, in sample order
         with ThreadPoolExecutor(1) as ahead, ThreadPoolExecutor(self.num_workers) as pool:
             nxt = ahead.submit(self._host_bev, batches[0], draws(batches[0]), pool)
             for k in range(len(batches)):
                 hs, decoded = nxt.result()
                 if k + 1 < len(batches):
                     nxt = ahead.submit(self._host_bev, batches[k + 1], draws(batches[k + 1]), pool)
-                yield self._device_bev(hs, decoded)
+                yield self._device_bev(hs, decoded), hs
 
     def _device_bev(self, hs, decoded):
         ds, dev = self.ds, self.ds.device

@@ -3,7 +3,8 @@
 against the expert's future — as numbers over every sample of the recording, through the agent's eval-mode inference path.
 
     python -m lav_b200.evaluate --config-path config_v2.yaml --data-dir VALDIR --lidar-weights lidar_7.th \
-        --uniplanner-weights uniplanner_7.th [--batch-size 32] [--precision f16|fp32] [--num-workers 16] [--json out.json]
+        --uniplanner-weights uniplanner_7.th [--batch-size 32] [--precision f16|fp32] [--num-workers 16] [--json out.json] \
+        [--forecast]
 
 Every sample is taken once, in index order, unaugmented (TemporalBatchLoader's ordered mode); the last batch may be short.  Per
 batch, InferModel.forward_batch runs the models and one ops.eval_batch launch scores its outputs; the one device-to-host copy
@@ -17,6 +18,37 @@ Metrics:
                   mean over the thresholds
   plan            ADE (mean over the steps of the Euclidean error) and FDE (error at the last step) in metres, over all samples
                   and per recorded command
+
+With --forecast (``forecast=True``) the result also holds ``forecast``: the UniPlanner's motion forecasts scored by
+ops.forecast_eval, one launch and one result copy per batch, from the LiDAR features forward_batch already computed.  The
+protocol, shared with lav_b200.evaluate_bev (the privileged BEV planner):
+
+  The forecasts are made from the recorded poses, which is what the training forward of both planners does with the jitter set
+  to zero.
+  Rows.  A row is an actor of a sample that the training selection rule accepts, heads.vehicles_ahead(ego_locs, locs[:, 1:],
+    typs[:, 1:] == 1), in slot order.  The max_num_cars cap and its multinomial draw are not applied: every such actor is
+    scored.  actor_tracks keeps only actors seen in all T + 1 frames, so every row has a full recorded future; padded slots have
+    typ 0 and are never rows.
+  Pose and target.  For a row at sample f and slot s >= 1 (slot 0 is the ego): start = locs[f, s, 0] - ego_locs[f, 0],
+    heading = oris[f, s] - oris[f, 0], target = transform_points(locs[f, s, 1:] - locs[f, s, :1], -heading), in the actor's
+    crop frame, the frame the loss compares in.  Ego rows use pose (0, 0) and target ego_locs[:, 1:].
+  Models, in eval mode.  UniPlanner: crop of the LiDAR features at (start, heading), lidar_conv_emb at the agent's precision
+    (the private copy agent.infer_model makes), then cast and cast_cmd_pred: infer_device's chain without its transform to the
+    ego frame.  BEVPlanner: crop_u8_kernel crop of the uint8 ground-truth BEV at pixels_per_meter and 2 * crop_size, then
+    bev_conv_emb, cast and cast_cmd_pred, in fp32 under math_mode("fp32"); its ego plan is
+    plan(ego_embd, nxp, cast_locs=ego_cast)[:, -1].
+  Metrics per row, with C branches and T steps; distances are fp64 Euclidean with no contraction.  ADE_j is the mean over t of
+    |cast[j, t] - target[t]|, summed in ascending t and then divided by T; FDE_j is the error at t = T - 1.  minADE and minFDE
+    are each minimised over j independently, ties to the lower j.  top is the branch with the highest command score, ties to
+    the lower j, NaN counting as lowest; the row reports its ADE / FDE.  A row with a recorded command (ego rows) reports the
+    ADE / FDE of that branch; rows without one (other vehicles, cmd = -1) get NaN there.
+  Host reduction over the recording.  other: row count, mean minADE, mean minFDE, mean top-1 ADE and FDE, and miss rate
+    (minFDE > 2 m).  ego_cast: ADE / FDE under the recorded command, minADE / minFDE, command accuracy (top == cmd), and the
+    same per recorded command.  ego_plan (BEV planner only): the plan's ADE / FDE under the recorded command, overall and per
+    command; the UniPlanner's plan is scored by ``plan`` above.  A mean over no row is null.
+
+Not scored: forecasts made on detected vehicles (that needs a detection-to-track match feeding the rows), pedestrians (the planners
+forecast vehicles only).
 """
 import argparse
 import json
@@ -84,10 +116,82 @@ class Scores:
                     bev_counts=self.iou.tolist(), det=det, plan=plan)
 
 
+FORECAST_MISS_M = 2.0       # a vehicle row whose minFDE exceeds this counts as a miss
+
+
+def score_forecasts(fc, cmds, plan=False):
+    """one ops.forecast_eval launch over a forecast_recorded result: its K vehicle rows (no command), its B ego casts and, with
+    ``plan``, its B ego plans (those two under the recorded commands ``cmds``, a (B,) device tensor).  -> the result buffer."""
+    K = fc["cast"].shape[0]
+    parts = [(fc["cast"], fc["score"], fc["target"]), (fc["ego_cast"], fc["ego_score"], fc["ego_target"])]
+    if plan:
+        parts.append((fc["ego_plan"], fc["ego_score"], fc["ego_target"]))
+    cat = lambda i: torch.cat([p[i].float() for p in parts]).contiguous()
+    cmd = torch.cat([torch.full((K,), -1, dtype=torch.int32, device=cmds.device)] + [cmds.to(torch.int32)] * (len(parts) - 1))
+    return ops.forecast_eval(cat(0), cat(1), cat(2), cmd)
+
+
+class ForecastScores:
+    """host accumulation of score_forecasts results over a recording."""
+
+    def __init__(self, plan=False):
+        self.plan = plan
+        self.other, self.ego, self.top, self.ego_plan, self.cmd = [], [], [], [], []
+
+    def add(self, v, n_other, cmds):
+        """v = ops.forecast_views of a host copy of one batch's result buffer; n_other its vehicle rows; cmds (B,) the recorded
+        commands, on the host."""
+        err, branch = v["err"].numpy(), v["branch"].numpy()
+        b = len(cmds)
+        self.other.append(err[:n_other])
+        self.ego.append(err[n_other:n_other + b])
+        self.top.append(branch[n_other:n_other + b, 1])
+        if self.plan:
+            self.ego_plan.append(err[n_other + b:n_other + 2 * b])
+        self.cmd.append(np.asarray(cmds, np.int64))
+
+    def summary(self):
+        mean = lambda a: float(np.mean(a)) if len(a) else None
+        rows = lambda parts: np.concatenate(parts) if parts else np.zeros((0, 6))
+        o, e, cmd = rows(self.other), rows(self.ego), np.concatenate(self.cmd) if self.cmd else np.zeros(0, np.int64)
+        top = np.concatenate(self.top) if self.top else np.zeros(0, np.int32)
+
+        def ego(m):
+            return dict(samples=int(m.sum()), ade=mean(e[m, 4]), fde=mean(e[m, 5]), min_ade=mean(e[m, 0]), min_fde=mean(e[m, 1]),
+                        cmd_accuracy=mean(top[m] == cmd[m]))
+        cmds, every = sorted(set(cmd.tolist())), np.ones(len(cmd), bool)
+        r = dict(other=dict(rows=len(o), min_ade=mean(o[:, 0]), min_fde=mean(o[:, 1]), top_ade=mean(o[:, 2]), top_fde=mean(o[:, 3]),
+                            miss_rate=mean(o[:, 1] > FORECAST_MISS_M)),
+                 ego_cast=dict(ego(every), per_cmd={str(c): ego(cmd == c) for c in cmds}))
+        if self.plan:
+            p = rows(self.ego_plan)
+            plan = lambda m: dict(samples=int(m.sum()), ade=mean(p[m, 4]), fde=mean(p[m, 5]))
+            r["ego_plan"] = dict(plan(every), per_cmd={str(c): plan(cmd == c) for c in cmds})
+        return r
+
+
+def format_forecast(f):
+    """the printout lines of a ForecastScores summary."""
+    fmt = lambda v: "n/a" if v is None else f"{v:.4f}"
+    o, e = f["other"], f["ego_cast"]
+    lines = [f"forecast, other vehicles ({o['rows']} rows): minADE {fmt(o['min_ade'])} m, minFDE {fmt(o['min_fde'])} m, "
+             f"top-1 ADE {fmt(o['top_ade'])} m, FDE {fmt(o['top_fde'])} m, miss rate {fmt(o['miss_rate'])}",
+             f"forecast, ego cast: ADE {fmt(e['ade'])} m, FDE {fmt(e['fde'])} m, minADE {fmt(e['min_ade'])} m, "
+             f"minFDE {fmt(e['min_fde'])} m, command accuracy {fmt(e['cmd_accuracy'])}"]
+    lines += [f"  cmd {c}: {d['samples']} samples, ADE {fmt(d['ade'])} m, FDE {fmt(d['fde'])} m, minADE {fmt(d['min_ade'])} m, "
+              f"minFDE {fmt(d['min_fde'])} m, accuracy {fmt(d['cmd_accuracy'])}" for c, d in e["per_cmd"].items()]
+    if "ego_plan" in f:
+        p = f["ego_plan"]
+        lines.append(f"ego plan: ADE {fmt(p['ade'])} m, FDE {fmt(p['fde'])} m")
+        lines += [f"  cmd {c}: {d['samples']} samples, ADE {fmt(d['ade'])} m, FDE {fmt(d['fde'])} m" for c, d in p["per_cmd"].items()]
+    return lines
+
+
 @torch.no_grad()
-def evaluate(lidar_model, uniplanner, dataset, batch_size=32, precision="f16", num_workers=16):
+def evaluate(lidar_model, uniplanner, dataset, batch_size=32, precision="f16", num_workers=16, forecast=False):
     """Scores of ``lidar_model`` and ``uniplanner`` over every sample of ``dataset`` (a TemporalLiDARPaintedDataset), the models
-    run as the agent runs them at ``precision``.  -> dict (see the module docstring)."""
+    run as the agent runs them at ``precision``; with ``forecast`` also the UniPlanner's forecast scores.  -> dict (see the
+    module docstring)."""
     dev = dataset.device
     lidar_model.to(dev).eval()
     uniplanner.to(dev).eval()
@@ -95,16 +199,23 @@ def evaluate(lidar_model, uniplanner, dataset, batch_size=32, precision="f16", n
     grid = dict(min_x=dataset.min_x, max_x=dataset.max_x, min_y=dataset.min_y, max_y=dataset.max_y,
                 pixels_per_meter=dataset.pixels_per_meter)
     loader = TemporalBatchLoader(dataset, batch_size, drop_last=False, num_workers=num_workers, ordered=True)
-    scores = Scores()
+    scores, forecasts = Scores(), ForecastScores()
     with math_mode(precision):
         for batch, staged in loader.staged_batches():
             lidars, num_points, bev, ego_locs, cmds, nxps = batch[0], batch[1], batch[5], batch[6], batch[7], batch[8]
             out = im.forward_batch(lidars, num_points, nxps, cmds)
             res = ops.eval_batch(out["pred_bev"].permute(0, 2, 3, 1), bev, out["packed"], staged["actors"].to(dev, non_blocking=True),
                                  staged["offsets"], out["ego_plan_locs"].float().contiguous(), ego_locs, grid)
-            scores.add(ops.eval_views(res.cpu(), len(num_points), out["packed"].shape[2]), staged["labels"]["cmd"].numpy())
+            host_cmds = staged["labels"]["cmd"].numpy()
+            scores.add(ops.eval_views(res.cpu(), len(num_points), out["packed"].shape[2]), host_cmds)
+            if forecast:
+                fc = im.uniplanner.forecast_recorded(out["features"].permute(0, 3, 1, 2), ego_locs, batch[10], batch[11], batch[12])
+                k = fc["cast"].shape[0]
+                forecasts.add(ops.forecast_views(score_forecasts(fc, cmds).cpu(), k + len(num_points)), k, host_cmds)
     result = scores.summary()
     result["precision"] = precision
+    if forecast:
+        result["forecast"] = forecasts.summary()
     return result
 
 
@@ -118,6 +229,7 @@ def parse_args(argv=None):
     ap.add_argument("--precision", default="f16", choices=["f16", "fp32"])
     ap.add_argument("--num-workers", type=int, default=16, help="host threads of the loader (record reads, PNG chunk walks)")
     ap.add_argument("--json", default=None, help="also write the result here")
+    ap.add_argument("--forecast", action="store_true", help="also score the UniPlanner's forecasts of the recorded vehicles")
     return ap.parse_args(argv)
 
 
@@ -130,6 +242,8 @@ def format_result(r):
     p = r["plan"]
     lines.append(f"plan ADE {fmt(p['ade'])} m, FDE {fmt(p['fde'])} m")
     lines += [f"  cmd {c}: {d['samples']} samples, ADE {fmt(d['ade'])} m, FDE {fmt(d['fde'])} m" for c, d in p["per_cmd"].items()]
+    if "forecast" in r:
+        lines += format_forecast(r["forecast"])
     return "\n".join(lines)
 
 
@@ -145,7 +259,7 @@ def main(argv=None):
     lid.load_state_dict(torch.load(args.lidar_weights, map_location="cpu"))
     uni.load_state_dict(torch.load(args.uniplanner_weights, map_location="cpu"))
     ds = TemporalLiDARPaintedDataset(args.config_path, device=dev, overrides=dict(data_dir=args.data_dir))
-    result = evaluate(lid, uni, ds, args.batch_size, args.precision, args.num_workers)
+    result = evaluate(lid, uni, ds, args.batch_size, args.precision, args.num_workers, args.forecast)
     print(format_result(result))
     if args.json:
         with open(args.json, "w") as f:

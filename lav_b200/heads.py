@@ -319,6 +319,25 @@ class BEVPlanner(nn.Module):
         ego_plan = self.plan(ego_embd, nxps, cast_locs=ego_cast, pixels_per_meter=ppm, crop_size=crop)
         return other_locs, other_cast, other_cmds, ego_plan, ego_cast, self.cast_cmd_pred(ego_embd)
 
+    @torch.no_grad()
+    def forecast_recorded(self, bev, ego_locs, locs, oris, typs, nxps):
+        """Forecasts of every recorded_rows row and of each ego, from crops of the ground-truth BEV ``bev`` at the recorded poses
+        (forward's crops at zero jitter; a uint8 map on the GPU takes the lav_b200 crop kernel), all through one embedder call.
+        -> dict: frame, slot, cast (K,C,T,2), score (K,C), target (K,T,2) of the rows; ego_cast (B,C,T,2), ego_score (B,C),
+        ego_target (B,T,2) = ego_locs[:, 1:]; ego_plan (B,C,T,2) = the last plan iteration from the ego's cast and ``nxps``."""
+        if not (bev.is_cuda and bev.dtype == torch.uint8):
+            bev = bev.float()
+        B, dev = bev.shape[0], bev.device
+        ppm, crop = self.pixels_per_meter, 2 * self.crop_size
+        rows = recorded_rows(ego_locs, locs, oris, typs)
+        at, facing, fidx = _forecast_poses(rows, B, dev)
+        embd = self.bev_conv_emb(self.crop_feature(bev, at, facing, pixels_per_meter=ppm, crop_size=crop, frame_idx=fidx))
+        cast, score = self.cast(embd), self.cast_cmd_pred(embd)
+        out = _forecast_result(rows, cast, score, ego_locs)
+        K = rows["frame"].numel()
+        out["ego_plan"] = self.plan(embd[K:], nxps, cast_locs=cast[K:], pixels_per_meter=ppm, crop_size=crop)[:, -1]
+        return out
+
     def cast(self, embd):
         return _cast_branches(self, self.cast_grus, self.cast_mlps, embd, self.num_plan)
 
@@ -347,6 +366,33 @@ def vehicles_ahead(ego_locs, locs, is_vehicle):
     frame) — the selection rule of lav/models/uniplanner.py:329-333.  ego_locs (B,T,2), locs (B,N,T,2), is_vehicle (B,N) bool."""
     ahead = (locs[:, :, 0, 1] - ego_locs[:, None, 0, 1]) < 0
     return is_vehicle & ahead
+
+
+def recorded_rows(ego_locs, locs, oris, typs):
+    """the forecast rows of an evaluation over recorded poses: every actor the training selection accepts
+    (vehicles_ahead(ego_locs, locs[:, 1:], typs[:, 1:] == 1), slot order, no max_num_cars cap) with the training forward's pose
+    and target at zero jitter.  locs (B,N,T+1,2), oris (B,N), typs (B,N), slot 0 the ego.  -> dict: frame, slot (K,) int64 with
+    slot >= 1 the index into locs; start (K,2) = locs[f, s, 0] - ego_locs[f, 0]; heading (K,) = oris[f, s] - oris[f, 0]; target
+    (K,T,2) = the actor's recorded future in its crop frame, transform_points(locs[f, s, 1:] - locs[f, s, :1], -heading)."""
+    frame, slot = vehicles_ahead(ego_locs, locs[:, 1:], typs[:, 1:] == 1).nonzero(as_tuple=True)
+    slot = slot + 1
+    heading = oris[frame, slot] - oris[frame, 0]
+    return dict(frame=frame, slot=slot, start=locs[frame, slot, 0] - ego_locs[frame, 0], heading=heading,
+                target=transform_points(locs[frame, slot, 1:] - locs[frame, slot, :1], -heading))
+
+
+def _forecast_poses(rows, B, device):
+    """(locations, headings, frame indices) of the crops of forecast_recorded: the K rows, then the B egos at the origin."""
+    at = torch.cat([rows["start"], torch.zeros((B, 2), dtype=rows["start"].dtype, device=device)])
+    facing = torch.cat([rows["heading"], torch.zeros((B,), dtype=rows["heading"].dtype, device=device)])
+    fidx = torch.cat([rows["frame"], torch.arange(B, device=device)]).to(torch.int32)
+    return at, facing, fidx
+
+
+def _forecast_result(rows, cast, score, ego_locs):
+    K = rows["frame"].numel()
+    return dict(frame=rows["frame"], slot=rows["slot"], cast=cast[:K], score=score[:K], target=rows["target"], ego_cast=cast[K:],
+                ego_score=score[K:], ego_target=ego_locs[:, 1:])
 
 
 def cap_per_sample(mask, limit):
@@ -533,6 +579,19 @@ class UniPlanner(nn.Module):
             o_cast = torch.zeros((0, self.num_cmds, self.num_plan, 2), device=dev)
             o_cmds = torch.zeros((0, self.num_cmds), device=dev)
         return ego_embd, ego_plan_locs, ego_cast_locs, o_cast, o_cmds
+
+    @torch.no_grad()
+    def forecast_recorded(self, features, ego_locs, locs, oris, typs):
+        """Forecasts of every recorded_rows row and of each ego from crops of the LiDAR ``features`` (logical (B,C,h,w)) at the
+        recorded poses: infer_device's crop -> embed (at the embedder's dtype) -> cast / cast_cmd_pred chain, without its
+        transform to the ego frame, all rows through one embedder call.  -> dict: frame, slot, cast (K,C,T,2), score (K,C), target
+        (K,T,2) of the rows; ego_cast (B,C,T,2), ego_score (B,C), ego_target (B,T,2) = ego_locs[:, 1:]."""
+        rows = recorded_rows(ego_locs, locs, oris, typs)
+        at, facing, fidx = _forecast_poses(rows, features.shape[0], features.device)
+        crops = self.crop_feature(features, at, facing, pixels_per_meter=self.pixels_per_meter / 2, crop_size=self.crop_size,
+                                  frame_idx=fidx)
+        embd = self.lidar_conv_emb(crops.to(self.lidar_conv_emb[0].conv1.weight.dtype)).float()
+        return _forecast_result(rows, self.cast(embd), self.cast_cmd_pred(embd), ego_locs)
 
     @torch.no_grad()
     def infer(self, features, det, cmd, nxp):

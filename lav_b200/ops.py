@@ -664,6 +664,41 @@ def eval_batch(seg, gt, packed, actors, offsets, plan, ego_locs, grid=None, min_
     return out
 
 
+def forecast_views(buf, k):
+    """the named parts of a forecast_eval result buffer (on the device or a host copy of it): err (k,6) fp64 = (min ADE, min FDE,
+    top-branch ADE, top-branch FDE, ADE and FDE under the recorded command or NaN); branch (k,2) int32 = (argmin-ADE branch, top
+    branch)."""
+    return dict(err=buf[:k * 48].view(torch.float64).view(k, 6), branch=buf[k * 48:k * 56].view(torch.int32).view(k, 2))
+
+
+def forecast_eval(cast, score, target, cmd, out=None):
+    """The forecast scores of k rows in one launch (see lavb_forecast_eval in include/lav_b200.h).  cast (k,C,T,2), score (k,C)
+    and target (k,T,2) fp32; cmd (k,) int32, -1 where the row has no recorded command.  -> the uint8 result buffer (written into
+    ``out`` when given), to be read through forecast_views, usually after one copy to the host."""
+    _need_cuda(cast, score, target, cmd)
+    if cast.dtype != torch.float32 or cast.dim() != 4 or cast.shape[3] != 2 or not cast.is_contiguous():
+        raise capi.LavbError(f"forecast_eval: cast must be a contiguous (k, C, T, 2) fp32 tensor, got {cast.dtype} {tuple(cast.shape)}")
+    k, c, t, _ = cast.shape
+    if score.dtype != torch.float32 or tuple(score.shape) != (k, c) or not score.is_contiguous():
+        raise capi.LavbError(f"forecast_eval: score must be a contiguous ({k}, {c}) fp32 tensor, got {score.dtype} {tuple(score.shape)}")
+    if target.dtype != torch.float32 or tuple(target.shape) != (k, t, 2) or not target.is_contiguous():
+        raise capi.LavbError(f"forecast_eval: target must be a contiguous ({k}, {t}, 2) fp32 tensor, got {target.dtype} "
+                             f"{tuple(target.shape)}")
+    if cmd.dtype != torch.int32 or tuple(cmd.shape) != (k,) or not cmd.is_contiguous():
+        raise capi.LavbError(f"forecast_eval: cmd must be a contiguous ({k},) int32 tensor, got {cmd.dtype} {tuple(cmd.shape)}")
+    if len({cast.device, score.device, target.device, cmd.device}) != 1:
+        raise capi.LavbError("forecast_eval: the inputs must be on one device")
+    if out is None:
+        out = torch.empty((k * 56,), dtype=torch.uint8, device=cast.device)
+    elif out.dtype != torch.uint8 or tuple(out.shape) != (k * 56,) or out.device != cast.device:
+        raise capi.LavbError(f"forecast_eval: out must be a ({k * 56},) uint8 tensor on {cast.device}")
+    v = forecast_views(out, k)
+    check(lib().lavb_forecast_eval(_ptr(cast), _ptr(score), _ptr(target), _ptr(cmd), k, c, t, _ptr(v["err"]), _ptr(v["branch"]),
+                                   _stream()), "lavb_forecast_eval")
+    _COUNT[0] += k > 0
+    return out
+
+
 PILLAR_ENCODER = "sorted"    # name of the 16-bit pipeline's pillar encoder, reported by bench.py; it selects nothing
 
 
