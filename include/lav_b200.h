@@ -193,6 +193,31 @@ int lavb_eval_batch(const void* d_seg, int seg_dtype, const uint8_t* d_gt, int g
 int lavb_forecast_eval(const float* d_cast, const float* d_score, const float* d_target, const int* d_cmd, int k, int c, int t,
                        double* d_err, int* d_branch, void* stream);
 
+/* ---------------------------------------------------------------- match of the forecast detections to the recorded tracks
+ * stands behind: the vehicles UniPlanner.infer forecasts (team_code_v2/models/uniplanner.py:186-247, the detections of
+ *           InferModel.det_inference that lie more than 4 px from the crop centre) and that lav_agent_fast.py:plan_collide brakes
+ *           on; the reference has no evaluation of them.  Pairs each such row with the recorded actor it forecasts, so
+ *           lavb_forecast_eval can score the row's forecast against that actor's recorded future.
+ * One block per sample.  Rows: sample i owns rows [h_row_offsets[i], h_row_offsets[i+1]) (HOST int32[b+1], h_row_offsets[0] = 0,
+ *   monotone, at most n_det rows per sample); h_cols (HOST int32, one per row) = the row's column of d_packed (b, 7, 2 * n_det)
+ *   fp32 (lavb_det_peaks' layout, flat index read as lavb_eval_batch reads it on a map of width w), ascending within a sample
+ *   and in the class-1 half [n_det, 2 * n_det).  d_actors / h_actor_offsets: lavb_eval_batch's actor table (at most 1024 rows
+ *   per sample); actor row a of sample i has a recorded track when a < h_num_objs[i] (HOST int32[b], 0..max_objs): its label
+ *   slot a of d_locs (b, max_objs, t + 1, 2) fp32, with d_ego_locs (b, t + 1, 2) fp32.
+ * Match, per sample: the actors of class 1 whose centre lies in lavb_eval_batch's window (tracked or not) are the candidates;
+ *   the rows in descending score (ties: lower flat index, then lower column; a NaN score last) each take the nearest candidate
+ *   not yet taken with squared pixel distance <= (match_m * ppm)^2 (fp64, no contraction, ties: lower actor row) - the search
+ *   of lavb_eval_batch.  Per row: d_actor int32 = the actor row or -1; d_flag int32 = bit 0 matched, bit 1 matched to a tracked
+ *   actor; d_dist fp64 = the match distance in metres (sqrt(d2) / ppm) or NaN; d_target (t, 2) fp32 = locs[i, a, 1 + s] -
+ *   ego_locs[i, 0] for a row matched to a tracked actor a (the frame of UniPlanner.infer's other_cast_locs), NaN otherwise.
+ *   d_ngt (b, 2) int32 = the candidates with and without a track.  1 <= n_det <= 64, 1 <= t <= 32; dist and target 8-byte
+ *   aligned.  Every output element of the b samples is written; a rejected call writes nothing. */
+int lavb_det_forecast_match(const float* d_packed, int b, int w, int n_det, const void* d_actors, int n_actors,
+                            const int* h_actor_offsets, const int* h_row_offsets, const int* h_cols, const int* h_num_objs,
+                            const float* d_locs, const float* d_ego_locs, int max_objs, int t, float ppm, float cx0, float cy0,
+                            float cy1, double match_m, int* d_actor, int* d_flag, double* d_dist, float* d_target, int* d_ngt,
+                            void* stream);
+
 /* ---------------------------------------------------------------- PointPillars voxeliser + pillar encoder
  * replaces: PointPillarNet.forward (lav/models/point_pillar.py:92-116) incl. grid_locations :70-79,
  *           pillar_generation/decorate :55-68,81-85, DynamicPointNet.forward :28-35 (torch_scatter

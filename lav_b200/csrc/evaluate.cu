@@ -1,7 +1,7 @@
 // Scores of one evaluation batch in one launch, one block per sample: the BEV intersection / union counts, the detections matched
 // to the recorded actors at four centre-distance thresholds, and the plan's displacement errors.  Everything per pixel and per
 // (prediction, actor) pair happens here; the host only sums the counts and ranks the matched flags of a whole recording (AP).
-#include "det_grid.cuh"
+#include "det_match.cuh"
 
 namespace {
 
@@ -27,8 +27,7 @@ struct EvalArgs {
   long long* iou; int* ngt; float* score; int* flags; double* plan_err;
 };
 
-// Squared distance in double with no contraction, so the host's numpy statement gets the same bits.
-__device__ __forceinline__ double dist2(double dx, double dy) { return __dadd_rn(__dmul_rn(dx, dx), __dmul_rn(dy, dy)); }
+using lavb::dist2;
 
 template <typename T> __device__ __forceinline__ void load12(const T* p, float (&v)[12]);
 template <> __device__ __forceinline__ void load12<float>(const float* p, float (&v)[12]) {
@@ -102,11 +101,9 @@ __global__ void __launch_bounds__(kThreads) eval_batch_kernel(const EvalArgs p, 
   if (tid < ncols) {
     const float* pk = p.packed + (long long)b * 7 * ncols + tid;
     const float sc = pk[0], bw = pk[2 * ncols], bh = pk[3 * ncols];
-    const long long loc = (long long)pk[ncols];                   // numpy's astype(int64): truncation
-    long long x = loc % p.w;
-    if (x < 0) x += p.w;                                          // Python's floor % and //
-    const long long y = (loc - x) / p.w;
-    const double d = sqrt(dist2((double)x - (double)p.g.cx0, (double)y - (double)__fadd_rn(p.g.cy0, p.g.cy1)));
+    long long loc, x, y;
+    lavb::peak_pixel(pk[ncols], p.w, loc, x, y);
+    const double d = lavb::window_dist((double)x, (double)y, p.g);
     const int cls = tid / p.n_det;
     const bool keep = (double)sc > p.min_score && !(cls == 1 && bw < p.size_thr && bh < p.size_thr) && d > p.win_lo && d < p.win_hi;
     s_score[tid] = sc; s_loc[tid] = loc; s_x[tid] = (int)x; s_y[tid] = (int)y; s_keep[tid] = keep; s_flags[tid] = keep ? 16 : 0;
@@ -116,7 +113,7 @@ __global__ void __launch_bounds__(kThreads) eval_batch_kernel(const EvalArgs p, 
     const DetActor A = p.actors[a0 + i];
     const int cls = A.typ == 0.f ? 0 : A.typ == 1.f ? 1 : -1;    // det_heatmaps ignores any other class
     const float2 c = lavb::det_centre(A, p.g);
-    const double d = sqrt(dist2((double)c.x - (double)p.g.cx0, (double)c.y - (double)__fadd_rn(p.g.cy0, p.g.cy1)));
+    const double d = lavb::window_dist((double)c.x, (double)c.y, p.g);
     const bool keep = cls >= 0 && d > p.win_lo && d < p.win_hi;
     s_gx[i] = c.x; s_gy[i] = c.y; s_gcls[i] = keep ? cls : -1;
 #pragma unroll
@@ -130,7 +127,7 @@ __global__ void __launch_bounds__(kThreads) eval_batch_kernel(const EvalArgs p, 
     const long long loc = s_loc[tid];
     int r = 0;
     for (int i = j0; i < j0 + p.n_det; ++i)
-      r += s_keep[i] && (s_score[i] > sc || (s_score[i] == sc && (s_loc[i] < loc || (s_loc[i] == loc && i < tid))));
+      r += s_keep[i] && lavb::ranks_before(s_score[i], s_loc[i], i, sc, loc, tid);
     s_order[cls][r] = tid;
     atomicAdd(&s_nsurv[cls], 1);
   }
@@ -144,20 +141,10 @@ __global__ void __launch_bounds__(kThreads) eval_batch_kernel(const EvalArgs p, 
     for (int r = 0; r < s_nsurv[cls]; ++r) {
       const int j = s_order[cls][r];
       const double px = (double)s_x[j], py = (double)s_y[j];
-      double best = INFINITY;
-      int who = 0x7fffffff;
-      for (int i = lane; i < n_gt; i += 32) {
-        if (s_gcls[i] != cls || s_used[k][i]) continue;
-        const double d2 = dist2(px - (double)s_gx[i], py - (double)s_gy[i]);
-        if (d2 <= thr2 && d2 < best) { best = d2; who = i; }    // lanes visit rows in ascending order: the first equal stays
-      }
-#pragma unroll
-      for (int o = 16; o > 0; o >>= 1) {
-        const double ob = __shfl_xor_sync(0xffffffffu, best, o);
-        const int ow = __shfl_xor_sync(0xffffffffu, who, o);
-        if (ob < best || (ob == best && ow < who)) { best = ob; who = ow; }
-      }
-      if (who != 0x7fffffff) {
+      double d2;
+      const int who = lavb::nearest_unmatched(px, py, s_gx, s_gy, n_gt, thr2,
+                                              [&](int i) { return s_gcls[i] == cls && !s_used[k][i]; }, &d2);
+      if (who >= 0) {
         if (lane == 0) { s_used[k][who] = 1; atomicOr(&s_flags[j], 1 << k); }
         __syncwarp();
       }

@@ -4,7 +4,7 @@ against the expert's future — as numbers over every sample of the recording, t
 
     python -m lav_b200.evaluate --config-path config_v2.yaml --data-dir VALDIR --lidar-weights lidar_7.th \
         --uniplanner-weights uniplanner_7.th [--batch-size 32] [--precision f16|fp32] [--num-workers 16] [--json out.json] \
-        [--forecast]
+        [--forecast] [--forecast-detected]
 
 Every sample is taken once, in index order, unaugmented (TemporalBatchLoader's ordered mode); the last batch may be short.  Per
 batch, InferModel.forward_batch runs the models and one ops.eval_batch launch scores its outputs; the one device-to-host copy
@@ -47,8 +47,36 @@ protocol, shared with lav_b200.evaluate_bev (the privileged BEV planner):
     same per recorded command.  ego_plan (BEV planner only): the plan's ADE / FDE under the recorded command, overall and per
     command; the UniPlanner's plan is scored by ``plan`` above.  A mean over no row is null.
 
-Not scored: forecasts made on detected vehicles (that needs a detection-to-track match feeding the rows), pedestrians (the planners
-forecast vehicles only).
+With --forecast-detected (``forecast_detected=True``) the result also holds ``forecast_detected``: the forecasts the agent acts
+on, the ones UniPlanner.infer_batch makes for the vehicles the LiDAR model detects (other_cast_locs / other_cast_cmds of
+forward_batch, the rows lav_agent_fast.plan_collide brakes on), matched to the recorded tracks and scored.  Per batch: one
+ops.det_forecast_match launch and one ops.forecast_eval launch into the same buffer, that buffer copied to the host once, plus
+one copy of the packed peaks (B x 7 x 30 floats) that the row table is built from; no extra model call.  The protocol:
+
+  Rows.  A row is a detection infer_batch forecasts: a class-1 packed peak that passes decode_packed's filters
+    (model_inference.peak_filter: score > 0.2, the size filter, 2 px < d < 30 m) and det_to_locs' centre test
+    (heads.off_centre: more than 4 px from the crop centre), in frame order, then packed-column order: the order of the
+    concatenated other_cast_locs, whose per-frame lengths must equal the row counts.  The row table (frame, column) is built on
+    the host (detected_rows) from a copy of the packed peaks.
+  Ground truth.  eval_batch's vehicle class and window: the actor rows of the sample with typ == 1 whose centre (det_grid.cuh's
+    det_centre) lies 2 px < d < 30 m from the ego.  Actor row a of a sample is label slot a (actor_tracks emits both in one id
+    order, the labels capped at max_objs), so an actor has a recorded track when a < num_objs.
+  Match.  Greedy per sample, the rows in eval_batch's order (descending score, then lower flat index, then lower column): each
+    takes the nearest GT vehicle not yet taken whose centre is within match_m = 2 m (fp64 pixel distance, no contraction; equal
+    distances to the lower actor row), the search eval_batch runs.  Vehicles without a track take part, so a detection of a
+    capped actor never takes a tracked neighbour; rows matched to them are counted and not scored.
+  Target.  For a row matched to a tracked actor a of sample f: locs[f, a, 1:] - ego_locs[f, 0] (the label tensors), the ego frame
+    of other_cast_locs: det_to_locs maps a peak at (X, Y) to ((X - 160) / ppm, (Y - 280) / ppm), det_centre places an actor at
+    X = -x * ppm + 160, and the labels are the negated actor positions.
+  Metrics per row: ops.forecast_eval(other_cast_locs, other_cast_cmds, target, cmd = -1) as above (minADE, minFDE, the
+    top-scored branch's ADE and FDE).
+  Host reduction (DetectedForecastScores): rows; matched (to a tracked actor); matched_untracked; gt (tracked vehicles in the
+    window); recall = matched / gt; over the matched rows the mean minADE, minFDE, top-1 ADE and FDE and the miss rate (minFDE >
+    2 m); ap = average_precision over every row but the matched-untracked ones, ranked by detection score (ties keep sample, then
+    column order), a row a true positive when matched to a tracked actor with minFDE <= 2 m, against gt; match_m.  A mean over
+    no row, and recall and ap with gt = 0, are null.
+
+Not scored: pedestrians (the planners forecast vehicles only).
 """
 import argparse
 import json
@@ -58,7 +86,10 @@ import torch
 
 from . import ops
 from .agent import infer_model, math_mode
+from .capi import LavbError
 from .datasets import TemporalBatchLoader, TemporalLiDARPaintedDataset
+from .heads import off_centre
+from .model_inference import peak_filter
 
 CLASSES = ("pedestrian", "vehicle")
 
@@ -187,11 +218,71 @@ def format_forecast(f):
     return lines
 
 
+def detected_rows(packed, pixels_per_meter, centre, min_score=0.2):
+    """The row table of the forecasts on detected vehicles: the class-1 peaks of host ``packed`` (B, 7, 2 * n_det) that
+    decode_packed keeps and det_to_locs forecasts (``centre`` = UniPlanner.crop_centre), in frame, then column order.  -> dict:
+    frame (K,) int64, col (K,) int32 = the packed column, score (K,) fp32, locs (K, 2) fp32 = det_to_locs' ego metres, counts (B,)."""
+    keep, x, y, cls = peak_filter(packed, pixels_per_meter, 2, min_score)
+    keep = keep & (cls[None] == 1) & off_centre(x, y, *centre)
+    frame, col = np.nonzero(keep)
+    X, Y = x[frame, col], y[frame, col]
+    locs = np.stack([(X - centre[0]) / pixels_per_meter, (Y - centre[1]) / pixels_per_meter], 1).astype(np.float32).reshape(-1, 2)
+    return dict(frame=frame, col=col.astype(np.int32), score=packed[frame, 0, col].astype(np.float32), locs=locs,
+                counts=keep.sum(1))
+
+
+def score_detected(out, rows, actors, offsets, locs, ego_locs, num_objs, grid):
+    """one ops.det_forecast_match launch and one ops.forecast_eval launch into its buffer: forward_batch's output ``out``, its
+    detected_rows ``rows``, eval_batch's actor table and the labels locs / ego_locs / num_objs (host).  -> the result buffer."""
+    counts = [len(c) for c in out["other_cast_locs"]]
+    if rows["counts"].tolist() != counts:
+        raise LavbError(f"forecast rows per frame {rows['counts'].tolist()} differ from the forecasts infer_batch made {counts}")
+    b, k = len(counts), len(rows["col"])
+    row_offsets = np.concatenate([[0], np.cumsum(counts)]).astype(np.int32)
+    buf = ops.det_forecast_match(out["packed"], actors, offsets, row_offsets, rows["col"], num_objs, locs, ego_locs, grid)
+    cast = torch.cat(out["other_cast_locs"]).float().contiguous()
+    score = torch.cat(out["other_cast_cmds"]).float().contiguous()
+    target = ops.det_match_views(buf, b, k, locs.shape[2] - 1)["target"]
+    ops.forecast_eval(cast, score, target, torch.full((k,), -1, dtype=torch.int32, device=cast.device), out=buf[:56 * k])
+    return buf
+
+
+class DetectedForecastScores:
+    """host accumulation of score_detected results over a recording."""
+
+    def __init__(self, match_m=ops.DET_MATCH_M):
+        self.match_m = match_m
+        self.score, self.flag, self.err = [], [], []
+        self.gt = 0
+
+    def add(self, v, scores):
+        """v = ops.det_match_views of a host copy of one batch's result buffer; scores (K,) the rows' detection scores."""
+        self.score.append(np.asarray(scores, np.float32))
+        self.flag.append(v["flag"].numpy().copy())
+        self.err.append(v["err"].numpy()[:, :4].copy())
+        self.gt += int(v["ngt"].numpy()[:, 0].sum())
+
+    def summary(self):
+        mean = lambda a: float(np.mean(a)) if len(a) else None
+        s = np.concatenate(self.score) if self.score else np.zeros(0, np.float32)
+        f = np.concatenate(self.flag) if self.flag else np.zeros(0, np.int32)
+        e = np.concatenate(self.err) if self.err else np.zeros((0, 4))
+        tracked, untracked = (f & 2) != 0, ((f & 1) != 0) & ((f & 2) == 0)
+        m = e[tracked]
+        tp = tracked & (e[:, 1] <= FORECAST_MISS_M)
+        n = int(tracked.sum())
+        return dict(rows=len(f), matched=n, matched_untracked=int(untracked.sum()), gt=self.gt,
+                    recall=n / self.gt if self.gt else None, min_ade=mean(m[:, 0]), min_fde=mean(m[:, 1]), top_ade=mean(m[:, 2]),
+                    top_fde=mean(m[:, 3]), miss_rate=mean(m[:, 1] > FORECAST_MISS_M),
+                    ap=average_precision(s[~untracked], tp[~untracked], self.gt), match_m=self.match_m)
+
+
 @torch.no_grad()
-def evaluate(lidar_model, uniplanner, dataset, batch_size=32, precision="f16", num_workers=16, forecast=False):
+def evaluate(lidar_model, uniplanner, dataset, batch_size=32, precision="f16", num_workers=16, forecast=False,
+             forecast_detected=False):
     """Scores of ``lidar_model`` and ``uniplanner`` over every sample of ``dataset`` (a TemporalLiDARPaintedDataset), the models
-    run as the agent runs them at ``precision``; with ``forecast`` also the UniPlanner's forecast scores.  -> dict (see the
-    module docstring)."""
+    run as the agent runs them at ``precision``; with ``forecast`` also the UniPlanner's forecast scores on the recorded poses,
+    with ``forecast_detected`` those on the detected vehicles.  -> dict (see the module docstring)."""
     dev = dataset.device
     lidar_model.to(dev).eval()
     uniplanner.to(dev).eval()
@@ -199,7 +290,7 @@ def evaluate(lidar_model, uniplanner, dataset, batch_size=32, precision="f16", n
     grid = dict(min_x=dataset.min_x, max_x=dataset.max_x, min_y=dataset.min_y, max_y=dataset.max_y,
                 pixels_per_meter=dataset.pixels_per_meter)
     loader = TemporalBatchLoader(dataset, batch_size, drop_last=False, num_workers=num_workers, ordered=True)
-    scores, forecasts = Scores(), ForecastScores()
+    scores, forecasts, detected = Scores(), ForecastScores(), DetectedForecastScores()
     with math_mode(precision):
         for batch, staged in loader.staged_batches():
             lidars, num_points, bev, ego_locs, cmds, nxps = batch[0], batch[1], batch[5], batch[6], batch[7], batch[8]
@@ -212,10 +303,18 @@ def evaluate(lidar_model, uniplanner, dataset, batch_size=32, precision="f16", n
                 fc = im.uniplanner.forecast_recorded(out["features"].permute(0, 3, 1, 2), ego_locs, batch[10], batch[11], batch[12])
                 k = fc["cast"].shape[0]
                 forecasts.add(ops.forecast_views(score_forecasts(fc, cmds).cpu(), k + len(num_points)), k, host_cmds)
+            if forecast_detected:
+                h, w = out["features"].shape[1:3]                   # forward_batch's features are NHWC at half the map size
+                rows = detected_rows(out["packed"].cpu().numpy(), im.pixels_per_meter, im.uniplanner.crop_centre(2 * h, 2 * w))
+                res = score_detected(out, rows, staged["actors"].to(dev, non_blocking=True), staged["offsets"], batch[10], ego_locs,
+                                     batch[13], grid)
+                detected.add(ops.det_match_views(res.cpu(), len(num_points), len(rows["col"]), batch[10].shape[2] - 1), rows["score"])
     result = scores.summary()
     result["precision"] = precision
     if forecast:
         result["forecast"] = forecasts.summary()
+    if forecast_detected:
+        result["forecast_detected"] = detected.summary()
     return result
 
 
@@ -230,6 +329,8 @@ def parse_args(argv=None):
     ap.add_argument("--num-workers", type=int, default=16, help="host threads of the loader (record reads, PNG chunk walks)")
     ap.add_argument("--json", default=None, help="also write the result here")
     ap.add_argument("--forecast", action="store_true", help="also score the UniPlanner's forecasts of the recorded vehicles")
+    ap.add_argument("--forecast-detected", action="store_true",
+                    help="also score the forecasts the agent makes for the vehicles it detects, matched to the recorded tracks")
     return ap.parse_args(argv)
 
 
@@ -244,6 +345,12 @@ def format_result(r):
     lines += [f"  cmd {c}: {d['samples']} samples, ADE {fmt(d['ade'])} m, FDE {fmt(d['fde'])} m" for c, d in p["per_cmd"].items()]
     if "forecast" in r:
         lines += format_forecast(r["forecast"])
+    if "forecast_detected" in r:
+        d = r["forecast_detected"]
+        lines.append(f"forecast, detected vehicles ({d['rows']} rows, {d['matched']} matched of {d['gt']} tracked, "
+                     f"{d['matched_untracked']} untracked, within {d['match_m']:g} m): recall {fmt(d['recall'])}, "
+                     f"minADE {fmt(d['min_ade'])} m, minFDE {fmt(d['min_fde'])} m, top-1 ADE {fmt(d['top_ade'])} m, "
+                     f"FDE {fmt(d['top_fde'])} m, miss rate {fmt(d['miss_rate'])}, AP {fmt(d['ap'])}")
     return "\n".join(lines)
 
 
@@ -259,7 +366,7 @@ def main(argv=None):
     lid.load_state_dict(torch.load(args.lidar_weights, map_location="cpu"))
     uni.load_state_dict(torch.load(args.uniplanner_weights, map_location="cpu"))
     ds = TemporalLiDARPaintedDataset(args.config_path, device=dev, overrides=dict(data_dir=args.data_dir))
-    result = evaluate(lid, uni, ds, args.batch_size, args.precision, args.num_workers, args.forecast)
+    result = evaluate(lid, uni, ds, args.batch_size, args.precision, args.num_workers, args.forecast, args.forecast_detected)
     print(format_result(result))
     if args.json:
         with open(args.json, "w") as f:

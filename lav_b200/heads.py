@@ -395,6 +395,13 @@ def _forecast_result(rows, cast, score, ego_locs):
                 ego_score=score[K:], ego_target=ego_locs[:, 1:])
 
 
+def off_centre(x, y, center_x, center_y):
+    """det_to_locs' centre test (uniplanner.py:203-204): a detection at pixel (x, y) (scalars or arrays) is forecast when it lies
+    more than 4 px from the crop centre."""
+    dx, dy = np.asarray(x, np.float64) - center_x, np.asarray(y, np.float64) - center_y
+    return np.sqrt(dx * dx + dy * dy) > 4
+
+
 def cap_per_sample(mask, limit):
     """at most `limit` True entries per row of a (B,N) bool mask; rows over the limit keep a uniformly random subset.  One
     torch.multinomial draw per over-full row, in row order — the random stream consumption of uniplanner.py:336-347, so a
@@ -521,13 +528,16 @@ class UniPlanner(nn.Module):
         return (other_locs, other_cast, other_cmds, other_cast_t, other_cmds_t,
                 ego_future, ego_plan, ego_cast, ego_cmds, ego_cast_t, ego_plan_t)
 
+    def crop_centre(self, H, W):
+        """(center_x, center_y) in map pixels of the agent's crop frame, for features of logical size (H/2, W/2)."""
+        return float(W / 2 + self.offset_x * W / 2), float(H / 2 + self.offset_y * H / 2)
+
     def det_to_locs(self, det, H, W):
         """detections -> (locs list, oris list) in ego metres (uniplanner.py:195-214)."""
-        center_x = float(W / 2 + self.offset_x * W / 2)
-        center_y = float(H / 2 + self.offset_y * H / 2)
+        center_x, center_y = self.crop_centre(H, W)
         locs, oris = [], []
         for X, Y, h, w, cos, sin in det:
-            if np.linalg.norm([X - center_x, Y - center_y]) <= 4:
+            if not off_centre(X, Y, center_x, center_y):
                 continue
             locs.append([(X - center_x) / self.pixels_per_meter, (Y - center_y) / self.pixels_per_meter])
             oris.append(float(np.arctan2(sin, cos)))

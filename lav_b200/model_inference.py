@@ -23,6 +23,21 @@ def extract_peak_batch(heat, max_pool_ks=7, max_det=15):
     return torch.topk(possible.flatten(1), min(max_det, possible[0].numel()), dim=1)
 
 
+def peak_filter(packed, pixels_per_meter, ncls=2, min_score=0.2):
+    """decode_packed's filters on host packed peaks (B, 7, ncls * n) (det_inference, model_inference.py:98-121): score threshold,
+    the class-1 size filter, the ego-distance window.  -> keep (B, cols) bool, x, y (B, cols) int64 pixel, cls (cols,)."""
+    W = int(packed[0, 6, 0])
+    nd = packed.shape[2] // ncls
+    score, loc = packed[:, 0].astype(np.float64), packed[:, 1].astype(np.int64)
+    x, y = loc % W, loc // W
+    w, h = packed[:, 2], packed[:, 3]
+    cls = np.arange(packed.shape[2]) // nd
+    dist = np.sqrt(((x - 160) ** 2 + (y - 280) ** 2).astype(np.float64))     # TODO hard-code of the reference kept
+    keep = (score > min_score) & ~((cls[None] == 1) & (np.maximum(w, h) < 0.1 * pixels_per_meter))
+    keep &= ~((dist <= 2) | (dist >= 30 * pixels_per_meter))
+    return keep, x, y, cls
+
+
 class InferModel(nn.Module):
     def __init__(self, lidar_model, uniplanner, camera_x, camera_z, device=torch.device("cuda")):
         super().__init__()
@@ -75,15 +90,7 @@ class InferModel(nn.Module):
         B = packed.shape[0]
         if B == 0:
             return []
-        W = int(packed[0, 6, 0])
-        nd = packed.shape[2] // ncls
-        score, loc = packed[:, 0].astype(np.float64), packed[:, 1].astype(np.int64)
-        x, y = loc % W, loc // W
-        w, h = packed[:, 2], packed[:, 3]
-        cls = np.arange(packed.shape[2]) // nd
-        dist = np.sqrt(((x - 160) ** 2 + (y - 280) ** 2).astype(np.float64))     # TODO hard-code of the reference kept
-        keep = (score > min_score) & ~((cls[None] == 1) & (np.maximum(w, h) < 0.1 * self.pixels_per_meter))
-        keep &= ~((dist <= 2) | (dist >= 30 * self.pixels_per_meter))
+        keep, x, y, cls = peak_filter(packed, self.pixels_per_meter, ncls, min_score)
         out = []
         for b in range(B):
             dets = [[] for _ in range(ncls)]

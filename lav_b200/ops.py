@@ -699,7 +699,83 @@ def forecast_eval(cast, score, target, cmd, out=None):
     return out
 
 
-PILLAR_ENCODER = "sorted"    # name of the 16-bit pipeline's pillar encoder, reported by bench.py; it selects nothing
+DET_MATCH_M = 2.0       # centre-distance radius of the detected-forecast match (det_forecast.cu)
+
+
+def _det_match_layout(b, k, t):
+    """(name, dtype, shape, byte offset) of the parts of det_forecast_match's result buffer and its size: forecast_eval's result
+    of the k rows first (err, branch: its ``out`` is buf[:56 * k]), then the match's."""
+    parts = [("err", torch.float64, (k, 6)), ("branch", torch.int32, (k, 2)), ("dist", torch.float64, (k,)),
+             ("target", torch.float32, (k, t, 2)), ("actor", torch.int32, (k,)), ("flag", torch.int32, (k,)),
+             ("ngt", torch.int32, (b, 2))]
+    out, pos = [], 0
+    for name, dt, shape in parts:
+        out.append((name, dt, shape, pos))
+        pos += int(np.prod(shape)) * torch.empty((), dtype=dt).element_size()
+    return out, pos
+
+
+def det_match_views(buf, b, k, t):
+    """the named parts of a det_forecast_match result buffer of b samples, k rows and t steps (on the device or a host copy):
+    err (k,6) fp64 / branch (k,2) int32 = forecast_views of the rows, once forecast_eval has written buf[:56 * k]; dist (k,) fp64 =
+    match distance in metres, NaN when unmatched; target (k,t,2) fp32 = the matched track's future in the ego frame, NaN unless
+    matched to a tracked actor; actor (k,) int32 = the actor row within its sample, or -1; flag (k,) int32 = bit 0 matched, bit 1
+    matched to a tracked actor; ngt (b,2) int32 = vehicles in the window with and without a track."""
+    layout, _ = _det_match_layout(b, k, t)
+    return {name: buf[pos:pos + int(np.prod(shape)) * torch.empty((), dtype=dt).element_size()].view(dt).view(shape)
+            for name, dt, shape, pos in layout}
+
+
+def det_forecast_match(packed, actors, offsets, row_offsets, cols, num_objs, locs, ego_locs, grid=None, match_m=DET_MATCH_M,
+                       out=None):
+    """The match of one batch's forecast rows to the recorded actors in one launch (see lavb_det_forecast_match in
+    include/lav_b200.h).  packed (B,7,2*n_det) fp32 from det_peaks; actors (A,6) fp32 on the device and offsets (B+1,) int32 on the
+    HOST (eval_batch's actor table); row_offsets (B+1,) and cols (K,) int32 on the HOST = each sample's rows and their packed
+    columns; num_objs (B,) on the HOST = the recorded tracks; locs (B,max_objs,T+1,2) and ego_locs (B,T+1,2) fp32 = the labels;
+    grid: the keyword arguments of det_grid.  -> the uint8 result buffer (written into ``out`` when given), read through
+    det_match_views; forecast_eval(..., out=buf[:56 * K]) puts the rows' scores in the same buffer."""
+    _need_cuda(packed, actors, locs, ego_locs)
+    if packed.dtype != torch.float32 or packed.dim() != 3 or packed.shape[1] != 7 or packed.shape[2] % 2 or not packed.is_contiguous():
+        raise capi.LavbError(f"det_forecast_match: packed must be a contiguous (B, 7, 2*n_det) fp32 tensor, got {packed.dtype} "
+                             f"{tuple(packed.shape)}")
+    b = packed.shape[0]
+    if actors.dtype != torch.float32 or actors.dim() != 2 or actors.shape[1] != 6 or not actors.is_contiguous():
+        raise capi.LavbError(f"det_forecast_match: actors must be a contiguous (A, 6) fp32 tensor, got {actors.dtype} "
+                             f"{tuple(actors.shape)}")
+    host = lambda a: np.ascontiguousarray(a.numpy() if torch.is_tensor(a) else a)
+    offsets, row_offsets, cols, num_objs = host(offsets), host(row_offsets), host(cols), host(num_objs).astype(np.int32)
+    for name, a, shape in (("offsets", offsets, (b + 1,)), ("row_offsets", row_offsets, (b + 1,)), ("num_objs", num_objs, (b,))):
+        if a.dtype != np.int32 or a.shape != shape:
+            raise capi.LavbError(f"det_forecast_match: {name} must be a host {shape} int32 array, got {a.dtype} {a.shape}")
+    k = int(row_offsets[-1])
+    if cols.dtype != np.int32 or cols.shape != (k,):
+        raise capi.LavbError(f"det_forecast_match: cols must be a host ({k},) int32 array, got {cols.dtype} {cols.shape}")
+    if locs.dtype != torch.float32 or locs.dim() != 4 or locs.shape[0] != b or locs.shape[3] != 2 or not locs.is_contiguous():
+        raise capi.LavbError(f"det_forecast_match: locs must be a contiguous ({b}, max_objs, T+1, 2) fp32 tensor, got {locs.dtype} "
+                             f"{tuple(locs.shape)}")
+    t = locs.shape[2] - 1
+    if ego_locs.dtype != torch.float32 or tuple(ego_locs.shape) != (b, t + 1, 2) or not ego_locs.is_contiguous():
+        raise capi.LavbError(f"det_forecast_match: ego_locs must be a contiguous ({b}, {t + 1}, 2) fp32 tensor, got {ego_locs.dtype} "
+                             f"{tuple(ego_locs.shape)}")
+    if len({packed.device, actors.device, locs.device, ego_locs.device}) != 1:
+        raise capi.LavbError("det_forecast_match: the inputs must be on one device")
+    _, nbytes = _det_match_layout(b, k, t)
+    if out is None:
+        out = torch.empty((nbytes,), dtype=torch.uint8, device=packed.device)
+    elif out.dtype != torch.uint8 or tuple(out.shape) != (nbytes,) or out.device != packed.device:
+        raise capi.LavbError(f"det_forecast_match: out must be a ({nbytes},) uint8 tensor on {packed.device}")
+    v = det_match_views(out, b, k, t)
+    h, w, (ppm, cx0, cy0, cy1, _) = det_grid(**(grid or {}))
+    ip = lambda a: a.ctypes.data_as(C.c_void_p)
+    check(lib().lavb_det_forecast_match(_ptr(packed), b, w, packed.shape[2] // 2, _ptr(actors), actors.shape[0], ip(offsets),
+                                        ip(row_offsets), ip(cols), ip(num_objs), _ptr(locs), _ptr(ego_locs), locs.shape[1], t, ppm,
+                                        cx0, cy0, cy1, float(match_m), _ptr(v["actor"]), _ptr(v["flag"]), _ptr(v["dist"]),
+                                        _ptr(v["target"]), _ptr(v["ngt"]), _stream()), "lavb_det_forecast_match")
+    _COUNT[0] += -(-b // 128)
+    return out
+
+
+PILLAR_ENCODER ="sorted"    # name of the 16-bit pipeline's pillar encoder, reported by bench.py; it selects nothing
 
 
 def pillar_forward_sorted(pts, starts, counts, grid, w1, s1, t1, w2, s2, t2, canvas16=False):
