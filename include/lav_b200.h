@@ -218,6 +218,32 @@ int lavb_det_forecast_match(const float* d_packed, int b, int w, int n_det, cons
                             float cy1, double match_m, int* d_actor, int* d_flag, double* d_dist, float* d_target, int* d_ngt,
                             void* stream);
 
+/* ---------------------------------------------------------------- collisions and road departures of planned ego trajectories
+ * stands behind: the check lav_agent_fast.py:plan_collide makes before the agent drives a plan; the reference has no open-loop
+ *           evaluation of the plan against the recorded traffic or the road.
+ * One block per sample (batches of more than 512 samples take one launch per 512).  d_traj (b, n, t, 2) fp32 = n trajectories of t
+ *   steps per sample in the label frame (entry 0 of ego_locs, the origin, precedes step 1).  Ego box at step s (1..t): centre
+ *   p_s; heading d / sqrt(d . d) with d = p_s - p_{s-1} (fp64, correctly rounded), the previous heading kept when
+ *   sqrt(d . d) < 0.1 m, (0, -1) before step 1; half extents d_ego_ext (b, 2) fp64 = the ego's (half length, half width).
+ *   A step whose centre or heading is not finite is invalid: counted, never a collision or off-road.
+ * Actors: d_actors is a DEVICE array of 56-byte records
+ *   { double x, y, cos, sin, e1, e2; int typ, present; }
+ *   sample i owning actor rows [h_offsets[i], h_offsets[i+1]) (HOST int32[b+1], monotone, any number of rows per sample), row a's
+ *   record of step s at index a * t + s - 1: label-frame centre, cos / sin of the yaw relative to the ego (heading (sin, -cos),
+ *   perpendicular (cos, sin)), half extents, class (1 vehicle, 0 pedestrian, others ignored), present != 0 when recorded.
+ * Collision: a separating-axis test over both boxes' headings and perpendiculars n, separated when |(c_B - c_A) . n| >=
+ *   r_A(n) + r_B(n), r(n) = e1 |u1 . n| + e2 |u2 . n|, in fp64 with no contraction; touching boxes do not collide.
+ * Road: the four corners of a valid box go to map pixels (floor(x * ppm + cx0), floor((y * ppm + cy0) + cy1)) in fp64 (column,
+ *   row; lavb_det_heatmaps' grid for label-frame, i.e. negated, coordinates); a corner outside the h x w plane is off the map,
+ *   an in-map corner on a 0 byte of d_map (plane of sample i at d_map + i * map_stride bytes, row-major) is off the road.
+ * d_out (b, n, 8) int32 per trajectory: first step colliding with a vehicle and its actor row (the lowest row at that step),
+ *   first step colliding with a pedestrian and its row, first off-road step, steps with a corner off the map, invalid steps,
+ *   first step colliding with either class; -1 for none.  1 <= n <= 8, 1 <= t <= 32; traj, actors and ego_ext 8-byte aligned.
+ *   Every output element of the b samples is written; a rejected call writes nothing. */
+int lavb_plan_safety(const float* d_traj, int b, int n, int t, const void* d_actors, int n_actors, const int* h_offsets,
+                     const double* d_ego_ext, const uint8_t* d_map, long long map_stride, int h, int w, float ppm, float cx0,
+                     float cy0, float cy1, int* d_out, void* stream);
+
 /* ---------------------------------------------------------------- PointPillars voxeliser + pillar encoder
  * replaces: PointPillarNet.forward (lav/models/point_pillar.py:92-116) incl. grid_locations :70-79,
  *           pillar_generation/decorate :55-68,81-85, DynamicPointNet.forward :28-35 (torch_scatter

@@ -68,10 +68,9 @@ def ego_pose(env, i):
     return _frame(env, "loc", i).reshape(-1, 2)[r].astype(np.float64), float(np.deg2rad(_frame(env, "ori", i)[r:r + 1])[0])
 
 
-def actor_tracks(env, index, T, max_pedestrian_radius, max_vehicle_radius):
-    """BasicDataset.filter + transform_ego (basic_dataset.py:103-157, lidar_dataset.py:132-148), vectorised.
-    -> ego_locs (T+1,2), locs (N,T+1,2), oris (N,T+1), bbox (N,T+1,2), typs (N,T+1) in the ego frame of ``index``, actors sorted
-    by id (the ego is one of them)."""
+def _read_tracks(env, index, T):
+    """the records of frames index .. index + T for the actors of frame ``index``, sorted by id: seen (N,T+1), world locs
+    (N,T+1,2), oris (N,T+1) in radians, bbox (N,T+1,2), typs (N,T+1), zero where unseen; and the ego's row."""
     ids0 = _frame(env, "id", index, np.int32)
     ego = ids0[0]
     uid = np.unique(ids0)
@@ -89,13 +88,77 @@ def actor_tracks(env, index, T, max_pedestrian_radius, max_vehicle_radius):
         oris[p, k] = np.deg2rad(_frame(env, "ori", index + k)[hit])
         bbox[p, k] = _frame(env, "bbox", index + k).reshape(-1, 2)[hit]
         typs[p, k] = _frame(env, "type", index + k, np.uint8)[hit]
-    e = int(np.searchsorted(uid, ego))
-    ego_locs, ego_ori = locs[e].copy(), oris[e, 0]
+    return seen, locs, oris, bbox, typs, int(np.searchsorted(uid, ego))
+
+
+def _ego_transform(locs, oris, e):
+    """(origin, R, ego yaw) of transform_ego: ego-frame points are (p - origin) @ R."""
+    ego_ori = oris[e, 0]
+    return locs[e, 0].copy(), [[np.sin(ego_ori), np.cos(ego_ori)], [-np.cos(ego_ori), np.sin(ego_ori)]], ego_ori
+
+
+def _label_tracks(tracks, max_pedestrian_radius, max_vehicle_radius):
+    seen, locs, oris, bbox, typs, e = tracks
+    ego_locs = locs[e].copy()
     r = np.linalg.norm(locs[:, 0] - ego_locs[0], axis=1)
     keep = seen.all(1) & ~((typs[:, 0] == 0) & (r > max_pedestrian_radius)) & ~((typs[:, 0] == 1) & (r > max_vehicle_radius))
-    R = [[np.sin(ego_ori), np.cos(ego_ori)], [-np.cos(ego_ori), np.sin(ego_ori)]]
-    origin = ego_locs[0]
+    origin, R, ego_ori = _ego_transform(locs, oris, e)
     return (ego_locs - origin) @ R, (locs[keep] - origin) @ R, oris[keep] - ego_ori, bbox[keep], typs[keep]
+
+
+def actor_tracks(env, index, T, max_pedestrian_radius, max_vehicle_radius):
+    """BasicDataset.filter + transform_ego (basic_dataset.py:103-157, lidar_dataset.py:132-148), vectorised.
+    -> ego_locs (T+1,2), locs (N,T+1,2), oris (N,T+1), bbox (N,T+1,2), typs (N,T+1) in the ego frame of ``index``, actors sorted
+    by id (the ego is one of them)."""
+    return _label_tracks(_read_tracks(env, index, T), max_pedestrian_radius, max_vehicle_radius)
+
+
+def _safety_table(tracks):
+    seen, locs, oris, bbox, typs, e = tracks
+    origin, R, ego_ori = _ego_transform(locs, oris, e)
+    others = np.arange(len(seen)) != e
+    present = seen[others, 1:]
+    yaw = oris[others, 1:] - ego_ori
+    only = lambda a: np.where(present.reshape(present.shape + (1,) * (a.ndim - 2)), a, 0)
+    return dict(locs=only(-((locs[others, 1:] - origin) @ R)), cos=only(np.cos(yaw)), sin=only(np.sin(yaw)),
+                bbox=only(bbox[others, 1:]), typ=only(typs[others, 1:]).astype(np.int32), present=present,
+                ego_bbox=bbox[e, 0].copy())
+
+
+def plan_safety_table(env, index, T):
+    """The actors an ego plan of sample ``index`` is checked against (lav_b200.evaluate, --plan-safety): every actor of frame
+    ``index`` but the ego, with no radius filter, at steps 1..T (frames index + 1 .. index + T), in actor_tracks' id order.
+    -> dict: locs (N,T,2) fp64 in the label frame (actor_tracks' ego frame, negated as the labels are), cos / sin (N,T) fp64 of
+    the yaw relative to the ego (the actor heads along (sin, -cos) there), bbox (N,T,2) = the recorded half extents, typ (N,T)
+    int32, present (N,T) bool (the id appears in that frame; the other entries are zero); ego_bbox (2,) = the ego's bbox at
+    frame ``index``."""
+    return _safety_table(_read_tracks(env, index, T))
+
+
+def _plan_safety_of(tracks, wanted, augmented):
+    """the plan_safety_table of a prepared sample when ``wanted``; its label frame is the unaugmented one."""
+    if not wanted:
+        return None
+    if augmented:
+        raise LavbError("plan_safety_table: the table is in the unaugmented label frame; the sample is rotated or shifted")
+    return _safety_table(tracks)
+
+
+def stage_plan_safety(tables, pin):
+    """the plan_safety_table of each sample of a batch packed for ops.plan_safety: actors = PLAN_SAFETY_ACTOR_DTYPE records as a
+    1-D uint8 tensor (sample i's rows, then within a row its steps), offsets (B+1,) int32 = the actor rows of each sample, ego_ext
+    (B,2) fp64; pinned on ``pin``."""
+    T = tables[0]["locs"].shape[1] if tables else 0
+    rec = np.zeros((sum(len(s["locs"]) for s in tables), T), ops.PLAN_SAFETY_ACTOR_DTYPE)
+    offsets = np.concatenate([[0], np.cumsum([len(s["locs"]) for s in tables])]).astype(np.int32)
+    for s, a0, a1 in zip(tables, offsets[:-1], offsets[1:]):
+        r = rec[a0:a1]
+        r["x"], r["y"], r["cos"], r["sin"] = s["locs"][..., 0], s["locs"][..., 1], s["cos"], s["sin"]
+        r["e1"], r["e2"], r["typ"], r["present"] = s["bbox"][..., 0], s["bbox"][..., 1], s["typ"], s["present"]
+    ego = np.array([s["ego_bbox"] for s in tables], np.float64).reshape(-1, 2)
+    tensor = lambda a: torch.from_numpy(np.ascontiguousarray(a))
+    out = dict(actors=tensor(rec.reshape(-1).view(np.uint8)), offsets=tensor(offsets), ego_ext=tensor(ego))
+    return {k: v.pin_memory() for k, v in out.items()} if pin else out
 
 
 def rotate_points(points, angle_deg, center):
@@ -153,13 +216,17 @@ class TemporalLiDARPaintedDataset:
         return 0.0, [(np.zeros(2), 0.0)] * (self.num_frame_stack + 1)
 
     # ---- host part: record reads, PNG chunk walks, labels, BEV job rows
-    def prepare(self, idx, angle, jitters):
+    def prepare(self, idx, angle, jitters, plan_safety=False):
+        """the host record of sample ``idx``; with ``plan_safety`` (unaugmented samples only) it also holds the sample's
+        plan_safety_table, from the same record reads."""
         traj, index = self.index[idx]
         env = self.env(traj)
         T, nseg = self.num_plan, len(self.seg_channels)
         radii = (self.max_pedestrian_radius, self.max_vehicle_radius)
         frames = [i for i in range(index, index - self.num_frame_stack - 1, -1) if i >= 0]
-        ego_locs, locs, oris, bbox, typs = actor_tracks(env, index, T, *radii)
+        tracks = _read_tracks(env, index, T)
+        table = _plan_safety_of(tracks, plan_safety, angle != 0)
+        ego_locs, locs, oris, bbox, typs = _label_tracks(tracks, *radii)
         poses = {i: ego_pose(env, i) for i in frames}
         loc0, ori0 = poses[index]
         sweeps = [(_frame(env, "lidar", i).reshape(-1, 4), _frame(env, "lidar_sem", i).reshape(-1, nseg), poses[i][0], poses[i][1])
@@ -187,10 +254,13 @@ class TemporalLiDARPaintedDataset:
         p_locs[:n_obj], p_oris[:n_obj], p_typs[:n_obj] = locs[:n_obj], oris[:n_obj, 0], typs[:n_obj, 0]
         ego_rot = rotate_points(ego_locs, -angle, ego_locs[0])
         nxp = rotate_points(_frame(env, "nxp", index).reshape(2), -angle, ego_rot[0])
-        return dict(sweeps=sweeps, angle=angle, jitters=jitters, pngs=pngs, rows=rows,
-                    det=(locs[:, 0], oris[:, 0], bbox[:, 0], typs[:, 0]), ego_locs=-ego_rot, nxp=-nxp,
-                    cmd=int(_frame(env, "cmd", index, np.uint8)[0]), bra=int(_frame(env, "bra", index, np.uint8)[0]),
-                    locs=-p_locs, oris=p_oris, typs=p_typs, num_objs=n_obj)
+        h = dict(sweeps=sweeps, angle=angle, jitters=jitters, pngs=pngs, rows=rows,
+                 det=(locs[:, 0], oris[:, 0], bbox[:, 0], typs[:, 0]), ego_locs=-ego_rot, nxp=-nxp,
+                 cmd=int(_frame(env, "cmd", index, np.uint8)[0]), bra=int(_frame(env, "bra", index, np.uint8)[0]),
+                 locs=-p_locs, oris=p_oris, typs=p_typs, num_objs=n_obj)
+        if table is not None:
+            h["plan_safety"] = table
+        return h
 
     # ---- device part
     def lidar_and_maps(self, h, generator=None):
@@ -274,10 +344,13 @@ class TemporalLiDARPaintedDataset:
         labels = dict(ego_locs=f32("ego_locs"), nxp=f32("nxp"), locs=f32("locs"), oris=f32("oris"),
                       typs=np.stack([h["typs"] for h in hs]).astype(np.int32),
                       cmd=np.array([h["cmd"] for h in hs], np.int64), bra=np.array([h["bra"] for h in hs], np.int64))
-        return dict(lidar=lidar, actors=pinned(np.concatenate(dets + [np.zeros((0, 6))]).astype(np.float32)),
-                    offsets=pinned(offsets), maps=stage_maps(hs, pin),
-                    bev_jobs=bev_job_table(hs, 3 + 2 * (self.num_frame_stack + 1)),
-                    labels={k: pinned(v) for k, v in labels.items()}, num_objs=[h["num_objs"] for h in hs])
+        st = dict(lidar=lidar, actors=pinned(np.concatenate(dets + [np.zeros((0, 6))]).astype(np.float32)),
+                  offsets=pinned(offsets), maps=stage_maps(hs, pin),
+                  bev_jobs=bev_job_table(hs, 3 + 2 * (self.num_frame_stack + 1)),
+                  labels={k: pinned(v) for k, v in labels.items()}, num_objs=[h["num_objs"] for h in hs])
+        if hs and "plan_safety" in hs[0]:                                       # prepared with plan_safety (the evaluator)
+            st["plan_safety"] = stage_plan_safety([h["plan_safety"] for h in hs], pin)
+        return st
 
     @torch.no_grad()
     def launch_batch(self, st):
@@ -341,13 +414,22 @@ class TemporalBatchLoader:
     (B,max_objs) f32, typs (B,max_objs) int32, num_objs (B,) int64; train_lidar takes the first 13.
 
     With ``ordered`` (evaluation) the samples come in index order with no augmentation: every draw is dataset.no_draw(), and the
-    LiDAR shuffles still come from the generator of (seed, epoch, rank)."""
+    LiDAR shuffles still come from the generator of (seed, epoch, rank).  With ``plan_safety`` (ordered only) every sample is
+    prepared with its plan_safety_table, and the staged tables carry them packed under "plan_safety" (stage_plan_safety)."""
 
-    def __init__(self, dataset, batch_size, seed=2021, rank=0, world=1, drop_last=True, num_workers=8, ordered=False):
+    def __init__(self, dataset, batch_size, seed=2021, rank=0, world=1, drop_last=True, num_workers=8, ordered=False,
+                 plan_safety=False):
         self.ds, self.B, self.seed, self.rank, self.world, self.drop_last = dataset, batch_size, seed, rank, world, drop_last
         self.num_workers = max(1, int(num_workers))
         self.ordered = ordered
+        self.plan_safety = plan_safety
+        if plan_safety and not ordered:
+            raise LavbError("plan_safety tables need the ordered, unaugmented loader")
         self.epoch = 0
+
+    def _prepare(self, pool, idxs, draws):
+        kw = dict(plan_safety=True) if self.plan_safety else {}
+        return list(pool.map(lambda a: self.ds.prepare(int(a[0]), *a[1], **kw), zip(idxs, draws)))
 
     def shard(self, epoch):
         perm = np.arange(len(self.ds)) if self.ordered else np.random.RandomState([self.seed, epoch]).permutation(len(self.ds))
@@ -363,7 +445,7 @@ class TemporalBatchLoader:
                 torch.Generator(device="cpu").manual_seed(self.seed * 1000003 + epoch * 1009 + self.rank))
 
     def _host(self, idxs, draws, gen, pool):
-        hs = list(pool.map(lambda a: self.ds.prepare(int(a[0]), *a[1]), zip(idxs, draws)))
+        hs = self._prepare(pool, idxs, draws)
         st = self.ds.stage_batch(hs, gen)
         st["decoded"] = self.ds.decode_maps(st["maps"])
         return st
@@ -437,11 +519,15 @@ class TemporalBEVDataset:
         return 0, 0.0
 
     # ---- host part: record reads, PNG chunk walks, labels, BEV job rows
-    def prepare(self, idx, offset, angle):
+    def prepare(self, idx, offset, angle, plan_safety=False):
+        """the host record of sample ``idx``; with ``plan_safety`` (unaugmented samples only) it also holds the sample's
+        plan_safety_table, from the same record reads."""
         traj, index = self.index[idx]
         env = self.env(traj)
         T = self.num_plan
-        ego_locs, locs, oris, _, typs = actor_tracks(env, index, T, self.max_pedestrian_radius, self.max_vehicle_radius)
+        tracks = _read_tracks(env, index, T)
+        table = _plan_safety_of(tracks, plan_safety, offset != 0 or angle != 0)
+        ego_locs, locs, oris, _, typs = _label_tracks(tracks, self.max_pedestrian_radius, self.max_vehicle_radius)
         frames = [i for i in range(index, index - self.num_frame_stack - 1, -1) if i >= 0]
         poses = {i: ego_pose(env, i) for i in frames}
         loc0, ori0 = poses[index]
@@ -470,8 +556,11 @@ class TemporalBEVDataset:
         p_oris = np.zeros((self.max_objs,), np.float32)
         p_typs = np.zeros((self.max_objs,), np.int32)
         p_locs[:n_obj], p_oris[:n_obj], p_typs[:n_obj] = locs[:n_obj], oris[:n_obj, 0], typs[:n_obj, 0]
-        return dict(pngs=pngs, rows=rows, ego_locs=-ego, nxp=-nxp, cmd=int(_frame(env, "cmd", index, np.uint8)[0]),
-                    bra=int(_frame(env, "bra", index, np.uint8)[0]), locs=-p_locs, oris=p_oris, typs=p_typs, num_objs=n_obj)
+        h = dict(pngs=pngs, rows=rows, ego_locs=-ego, nxp=-nxp, cmd=int(_frame(env, "cmd", index, np.uint8)[0]),
+                 bra=int(_frame(env, "bra", index, np.uint8)[0]), locs=-p_locs, oris=p_oris, typs=p_typs, num_objs=n_obj)
+        if table is not None:
+            h["plan_safety"] = table
+        return h
 
     def sample(self, idx, offset, angle):
         """the 9-tuple of sample ``idx`` for the given draws (offset in pixels, angle in degrees)."""
@@ -492,10 +581,10 @@ class TemporalBEVBatchLoader(TemporalBatchLoader):
     decoded in one launch on a side stream, one batch ahead of the GPU.  A batch is the 9-tuple bev (B,9,320,320) uint8, ego_locs (B,T+1,2) f32, cmds (B,) int64, nxps (B,2) f32,
     bras (B,) int64, locs (B,max_objs,T+1,2) f32, oris (B,max_objs) f32, typs (B,max_objs) int32, num_objs (B,) int64 (host),
     with one bev_targets launch per batch.  With ``ordered`` (evaluation) the samples come in index order and every draw is
-    dataset.no_draw()."""
+    dataset.no_draw(); with ``plan_safety`` as well, every host record holds its plan_safety_table under "plan_safety"."""
 
     def _host_bev(self, idxs, draws, pool):
-        hs = list(pool.map(lambda a: self.ds.prepare(int(a[0]), *a[1]), zip(idxs, draws)))
+        hs = self._prepare(pool, idxs, draws)
         return hs, self.ds.decode_maps(stage_maps(hs, self.ds.device.type == "cuda"))
 
     def staged_batches(self):

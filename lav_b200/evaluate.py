@@ -4,7 +4,7 @@ against the expert's future — as numbers over every sample of the recording, t
 
     python -m lav_b200.evaluate --config-path config_v2.yaml --data-dir VALDIR --lidar-weights lidar_7.th \
         --uniplanner-weights uniplanner_7.th [--batch-size 32] [--precision f16|fp32] [--num-workers 16] [--json out.json] \
-        [--forecast] [--forecast-detected]
+        [--forecast] [--forecast-detected] [--plan-safety]
 
 Every sample is taken once, in index order, unaugmented (TemporalBatchLoader's ordered mode); the last batch may be short.  Per
 batch, InferModel.forward_batch runs the models and one ops.eval_batch launch scores its outputs; the one device-to-host copy
@@ -77,6 +77,45 @@ one copy of the packed peaks (B x 7 x 30 floats) that the row table is built fro
     no row, and recall and ap with gt = 0, are null.
 
 Not scored: pedestrians (the planners forecast vehicles only).
+
+With --plan-safety (``plan_safety=True``, also lav_b200.evaluate_bev) the result also holds ``plan_safety``: the open-loop
+collision rate of the ego plan against the recorded (non-reactive) traffic and the share of plans that leave the road, the check
+lav_agent_fast.plan_collide makes before the agent drives a plan.  Per batch: one ops.plan_safety launch and one copy of its
+(B, 2, 8) int32 result; the actor table comes from the loader (datasets.plan_safety_table, built only when asked), the road from
+the batch's bev; no extra model call.  The protocol:
+
+  Trajectories.  n = 2 per sample, T steps in the label frame (that of ego_locs and ego_plan_locs, entry 0 of ego_locs the
+    origin): the plan under the recorded command (evaluate: forward_batch's ego_plan_locs; evaluate_bev: the recorded command's
+    branch of forecast_recorded's ego_plan, NaN when the command has no branch) and the expert, ego_locs[:, 1:].  The expert is
+    scored by the same rules: it is the metric's floor on the recording and is always reported next to the plan.
+  Ego box at step t = 1..T.  Centre p_t = traj[t - 1], p_0 the origin.  Heading d / sqrt(d . d), d = p_t - p_{t-1}, in fp64 with
+    correctly rounded sqrt and divide (no trig); a step of less than 0.1 m keeps the previous heading, and the heading before
+    step 1 is the ego's forward direction (0, -1) ("ahead" is negative y, heads.vehicles_ahead).  Half extents: the ego's
+    recorded bbox at the sample's frame, read as CARLA's bounding_box.extent (half length along the heading, half width), the
+    reading detections_to_heatmap's scaling of bbox by ppm implies; the synthetic ego's (2.4, 1.1) is a 4.8 x 2.2 m car.
+  Actors.  Every actor of the sample's frame but the ego, with no radius filter and no max_objs cap.  It is present at step t
+    when its id appears in frame index + t, with that frame's loc, ori, bbox and type; type 1 is a vehicle, 0 a pedestrian,
+    others are ignored.  Positions go into the label frame as actor_tracks transforms them, then negated as the labels are.  A
+    yaw psi relative to the ego heads along (sin psi, -cos psi) there: actor_tracks maps a world direction (cos phi, sin phi)
+    through R = [[sin e, cos e], [-cos e, sin e]] (e the ego yaw) to (-sin psi, cos psi) with psi = phi - e, negated to
+    (sin psi, -cos psi); psi = 0 gives the ego's own (0, -1).  cos psi and sin psi are computed on the host in fp64 and travel in the table.
+  Collision.  A separating-axis test of the two rectangles over both boxes' headings and their perpendiculars (u2 = (-u1y,
+    u1x)): on axis n the separation |(c_B - c_A) . n| against the reach r_A(n) + r_B(n), r(n) = e1 |u1 . n| + e2 |u2 . n|, in
+    fp64 with no contraction, evaluated in the order written; separated when separation >= reach, so touching does not collide.
+    A step collides with a class when any present actor of that class overlaps the ego box.
+  Leaving the road.  The four corners of the ego box go to map pixels as det_centre places label-frame coordinates: column =
+    floor(x * ppm + cx0), row = floor((y * ppm + cy0) + cy1), in fp64, i.e. (160 + 4x, 280 + 4y) on the v2 grid.  A corner
+    outside the 320 x 320 map is off the map; a step is off-road when any in-map corner lands on a 0 pixel of bev[:, 0] (the road
+    plane; in the ordered, unaugmented loaders it is in the label frame).  A step with a corner off the map counts in
+    off_map_steps; its in-map corners still decide whether it is off-road.
+  Invalid steps.  A step whose centre or heading is not finite (a NaN point also spoils the next step's heading) is counted in
+    invalid_steps and is never a collision or off-road.
+  Per sample and trajectory (ops.plan_safety_views): the first vehicle-collision step and the actor row it hit, the same for
+    pedestrians, the first off-road step, off_map_steps and invalid_steps; steps are numbered 1..T, -1 for none.
+  Host reduction (PlanSafetyScores), for plan and for expert, overall and per recorded command: samples, collision_rate (either
+    class), vehicle_collision_rate, pedestrian_collision_rate, off_road_rate, collision_rate_by_step (T values: the share of
+    samples whose first collision is at or before that step), and the summed off_map_steps and invalid_steps.  A rate over no
+    sample is null.
 """
 import argparse
 import json
@@ -277,20 +316,80 @@ class DetectedForecastScores:
                     ap=average_precision(s[~untracked], tp[~untracked], self.gt), match_m=self.match_m)
 
 
+PLAN_SAFETY_TRAJECTORIES = ("plan", "expert")
+
+
+def score_plan_safety(plan, ego_locs, table, bev, grid):
+    """one ops.plan_safety launch over a batch's ego plans ``plan`` (B,T,2) and experts ego_locs[:, 1:], against the batch's
+    packed plan_safety tables (stage_plan_safety, on the host) and the road plane of its ``bev``.  -> (B, 2, 8) int32 on the
+    device, trajectory 0 the plan, 1 the expert."""
+    dev = bev.device
+    traj = torch.stack([plan.float(), ego_locs[:, 1:].float()], 1).contiguous()
+    return ops.plan_safety(traj, table["actors"].to(dev, non_blocking=True), table["offsets"],
+                           table["ego_ext"].to(dev, non_blocking=True), bev, grid)
+
+
+class PlanSafetyScores:
+    """host accumulation of score_plan_safety results over a recording."""
+
+    def __init__(self, names=PLAN_SAFETY_TRAJECTORIES):
+        self.names = names
+        self.res, self.cmd = [], []
+
+    def add(self, res, cmds):
+        """res (B, n, 8) int32, a host copy of one batch's result; cmds (B,) the recorded commands."""
+        self.res.append(np.asarray(res, np.int32).copy())
+        self.cmd.append(np.asarray(cmds, np.int64))
+
+    def summary(self, t):
+        """per trajectory: the rates over all samples and per recorded command (``t`` steps per trajectory)."""
+        res = np.concatenate(self.res) if self.res else np.zeros((0, len(self.names), 8), np.int32)
+        cmd = np.concatenate(self.cmd) if self.cmd else np.zeros(0, np.int64)
+
+        def rates(r):
+            n = len(r)
+            rate = lambda hit: float(hit.mean()) if n else None
+            first = r[:, 7]
+            return dict(samples=n, collision_rate=rate(first > 0), vehicle_collision_rate=rate(r[:, 0] > 0),
+                        pedestrian_collision_rate=rate(r[:, 2] > 0), off_road_rate=rate(r[:, 4] > 0),
+                        collision_rate_by_step=[rate((first > 0) & (first <= s)) for s in range(1, t + 1)],
+                        off_map_steps=int(r[:, 5].sum()), invalid_steps=int(r[:, 6].sum()))
+
+        out = {}
+        for j, name in enumerate(self.names):
+            r = res[:, j]
+            out[name] = dict(rates(r), per_cmd={str(c): rates(r[cmd == c]) for c in sorted(set(cmd.tolist()))})
+        return out
+
+
+def format_plan_safety(s):
+    """the printout lines of a PlanSafetyScores summary."""
+    fmt = lambda v: "n/a" if v is None else f"{v:.4f}"
+    line = lambda d: (f"{d['samples']} samples, collision rate {fmt(d['collision_rate'])} (vehicles "
+                      f"{fmt(d['vehicle_collision_rate'])}, pedestrians {fmt(d['pedestrian_collision_rate'])}), off-road rate "
+                      f"{fmt(d['off_road_rate'])}, {d['off_map_steps']} off-map steps, {d['invalid_steps']} invalid steps")
+    lines = []
+    for name, d in s.items():
+        lines.append(f"plan safety, {name}: " + line(d))
+        lines += [f"  cmd {c}: " + line(e) for c, e in d["per_cmd"].items()]
+    return lines
+
+
 @torch.no_grad()
 def evaluate(lidar_model, uniplanner, dataset, batch_size=32, precision="f16", num_workers=16, forecast=False,
-             forecast_detected=False):
+             forecast_detected=False, plan_safety=False):
     """Scores of ``lidar_model`` and ``uniplanner`` over every sample of ``dataset`` (a TemporalLiDARPaintedDataset), the models
     run as the agent runs them at ``precision``; with ``forecast`` also the UniPlanner's forecast scores on the recorded poses,
-    with ``forecast_detected`` those on the detected vehicles.  -> dict (see the module docstring)."""
+    with ``forecast_detected`` those on the detected vehicles, with ``plan_safety`` the collision and off-road rates of the ego
+    plan and of the expert.  -> dict (see the module docstring)."""
     dev = dataset.device
     lidar_model.to(dev).eval()
     uniplanner.to(dev).eval()
     im = infer_model(lidar_model, uniplanner, precision, dataset.camera_x, dataset.camera_z, dev)
     grid = dict(min_x=dataset.min_x, max_x=dataset.max_x, min_y=dataset.min_y, max_y=dataset.max_y,
                 pixels_per_meter=dataset.pixels_per_meter)
-    loader = TemporalBatchLoader(dataset, batch_size, drop_last=False, num_workers=num_workers, ordered=True)
-    scores, forecasts, detected = Scores(), ForecastScores(), DetectedForecastScores()
+    loader = TemporalBatchLoader(dataset, batch_size, drop_last=False, num_workers=num_workers, ordered=True, plan_safety=plan_safety)
+    scores, forecasts, detected, safety = Scores(), ForecastScores(), DetectedForecastScores(), PlanSafetyScores()
     with math_mode(precision):
         for batch, staged in loader.staged_batches():
             lidars, num_points, bev, ego_locs, cmds, nxps = batch[0], batch[1], batch[5], batch[6], batch[7], batch[8]
@@ -309,12 +408,17 @@ def evaluate(lidar_model, uniplanner, dataset, batch_size=32, precision="f16", n
                 res = score_detected(out, rows, staged["actors"].to(dev, non_blocking=True), staged["offsets"], batch[10], ego_locs,
                                      batch[13], grid)
                 detected.add(ops.det_match_views(res.cpu(), len(num_points), len(rows["col"]), batch[10].shape[2] - 1), rows["score"])
+            if plan_safety:
+                res = score_plan_safety(out["ego_plan_locs"], ego_locs, staged["plan_safety"], bev, grid)
+                safety.add(res.cpu().numpy(), host_cmds)
     result = scores.summary()
     result["precision"] = precision
     if forecast:
         result["forecast"] = forecasts.summary()
     if forecast_detected:
         result["forecast_detected"] = detected.summary()
+    if plan_safety:
+        result["plan_safety"] = safety.summary(dataset.num_plan)
     return result
 
 
@@ -331,6 +435,8 @@ def parse_args(argv=None):
     ap.add_argument("--forecast", action="store_true", help="also score the UniPlanner's forecasts of the recorded vehicles")
     ap.add_argument("--forecast-detected", action="store_true",
                     help="also score the forecasts the agent makes for the vehicles it detects, matched to the recorded tracks")
+    ap.add_argument("--plan-safety", action="store_true",
+                    help="also score the ego plan and the expert for collisions with the recorded traffic and for leaving the road")
     return ap.parse_args(argv)
 
 
@@ -351,6 +457,8 @@ def format_result(r):
                      f"{d['matched_untracked']} untracked, within {d['match_m']:g} m): recall {fmt(d['recall'])}, "
                      f"minADE {fmt(d['min_ade'])} m, minFDE {fmt(d['min_fde'])} m, top-1 ADE {fmt(d['top_ade'])} m, "
                      f"FDE {fmt(d['top_fde'])} m, miss rate {fmt(d['miss_rate'])}, AP {fmt(d['ap'])}")
+    if "plan_safety" in r:
+        lines += format_plan_safety(r["plan_safety"])
     return "\n".join(lines)
 
 
@@ -366,7 +474,8 @@ def main(argv=None):
     lid.load_state_dict(torch.load(args.lidar_weights, map_location="cpu"))
     uni.load_state_dict(torch.load(args.uniplanner_weights, map_location="cpu"))
     ds = TemporalLiDARPaintedDataset(args.config_path, device=dev, overrides=dict(data_dir=args.data_dir))
-    result = evaluate(lid, uni, ds, args.batch_size, args.precision, args.num_workers, args.forecast, args.forecast_detected)
+    result = evaluate(lid, uni, ds, args.batch_size, args.precision, args.num_workers, args.forecast, args.forecast_detected,
+                      args.plan_safety)
     print(format_result(result))
     if args.json:
         with open(args.json, "w") as f:

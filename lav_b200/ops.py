@@ -775,6 +775,57 @@ def det_forecast_match(packed, actors, offsets, row_offsets, cols, num_objs, loc
     return out
 
 
+# one (actor, step) record of plan_safety's actor table (lavb_plan_safety in include/lav_b200.h)
+PLAN_SAFETY_ACTOR_DTYPE = np.dtype([("x", np.float64), ("y", np.float64), ("cos", np.float64), ("sin", np.float64),
+                                    ("e1", np.float64), ("e2", np.float64), ("typ", np.int32), ("present", np.int32)])
+assert PLAN_SAFETY_ACTOR_DTYPE.itemsize == 56
+PLAN_SAFETY_FIELDS = ("veh_step", "veh_row", "ped_step", "ped_row", "off_road_step", "off_map_steps", "invalid_steps", "first_step")
+
+
+def plan_safety_views(res):
+    """the named columns of a plan_safety result (B, n, 8) int32 (on the device or a host copy), each (B, n): veh_step / veh_row
+    = the first step (1..T) whose ego box overlaps a vehicle and that vehicle's actor row, ped_step / ped_row the same for
+    pedestrians, off_road_step = the first step with a corner on a 0 pixel of the road plane, off_map_steps / invalid_steps =
+    step counts, first_step = the first collision of either class; -1 for none."""
+    return {name: res[..., i] for i, name in enumerate(PLAN_SAFETY_FIELDS)}
+
+
+def plan_safety(traj, actors, offsets, ego_ext, bev, grid=None, out=None):
+    """Collisions and road departures of n ego trajectories per sample in one launch (see lavb_plan_safety in include/lav_b200.h).
+    traj (B,n,T,2) fp32 in the label frame; actors = PLAN_SAFETY_ACTOR_DTYPE records of every actor row and step as a 1-D uint8
+    tensor on the device, sample i owning rows [offsets[i], offsets[i+1]) (offsets (B+1,) int32 on the HOST), row a's step s at
+    record a * T + s - 1; ego_ext (B,2) fp64 = the ego's half extents; bev (B,P,H,W) uint8, plane 0 the road; grid: the keyword
+    arguments of det_grid.  -> (B,n,8) int32, read through plan_safety_views (written into ``out`` when given)."""
+    _need_cuda(traj, actors, ego_ext, bev)
+    if traj.dtype != torch.float32 or traj.dim() != 4 or traj.shape[3] != 2 or not traj.is_contiguous():
+        raise capi.LavbError(f"plan_safety: traj must be a contiguous (B, n, T, 2) fp32 tensor, got {traj.dtype} {tuple(traj.shape)}")
+    b, n, t, _ = traj.shape
+    offsets = np.ascontiguousarray(offsets.numpy() if torch.is_tensor(offsets) else offsets)
+    if offsets.dtype != np.int32 or offsets.shape != (b + 1,):
+        raise capi.LavbError(f"plan_safety: offsets must be a host ({b + 1},) int32 array, got {offsets.dtype} {offsets.shape}")
+    rec = PLAN_SAFETY_ACTOR_DTYPE.itemsize
+    if actors.dtype != torch.uint8 or actors.dim() != 1 or actors.numel() % (rec * t) or not actors.is_contiguous():
+        raise capi.LavbError(f"plan_safety: actors must be a contiguous 1-D uint8 tensor of {rec}-byte records, {t} per actor row, "
+                             f"got {actors.dtype} {tuple(actors.shape)}")
+    if ego_ext.dtype != torch.float64 or tuple(ego_ext.shape) != (b, 2) or not ego_ext.is_contiguous():
+        raise capi.LavbError(f"plan_safety: ego_ext must be a contiguous ({b}, 2) fp64 tensor, got {ego_ext.dtype} {tuple(ego_ext.shape)}")
+    if bev.dtype != torch.uint8 or bev.dim() != 4 or bev.shape[0] != b or not bev.is_contiguous():
+        raise capi.LavbError(f"plan_safety: bev must be a contiguous ({b}, P, H, W) uint8 tensor, got {bev.dtype} {tuple(bev.shape)}")
+    if len({traj.device, actors.device, ego_ext.device, bev.device}) != 1:
+        raise capi.LavbError("plan_safety: the inputs must be on one device")
+    if out is None:
+        out = torch.empty((b, n, 8), dtype=torch.int32, device=traj.device)
+    elif out.dtype != torch.int32 or tuple(out.shape) != (b, n, 8) or not out.is_contiguous() or out.device != traj.device:
+        raise capi.LavbError(f"plan_safety: out must be a contiguous ({b}, {n}, 8) int32 tensor on {traj.device}")
+    _, _, h, w = bev.shape
+    _, _, (ppm, cx0, cy0, cy1, _) = det_grid(**(grid or {}))
+    check(lib().lavb_plan_safety(_ptr(traj), b, n, t, _ptr(actors), actors.numel() // (rec * t), offsets.ctypes.data_as(C.c_void_p),
+                                 _ptr(ego_ext), _ptr(bev), bev[0].numel() if b else h * w, h, w, ppm, cx0, cy0, cy1, _ptr(out),
+                                 _stream()), "lavb_plan_safety")
+    _COUNT[0] += -(-b // 512)
+    return out
+
+
 PILLAR_ENCODER ="sorted"    # name of the 16-bit pipeline's pillar encoder, reported by bench.py; it selects nothing
 
 
