@@ -244,6 +244,56 @@ int lavb_plan_safety(const float* d_traj, int b, int n, int t, const void* d_act
                      const double* d_ego_ext, const uint8_t* d_map, long long map_stride, int h, int w, float ppm, float cx0,
                      float cy0, float cy1, int* d_out, void* stream);
 
+/* ---------------------------------------------------------------- the agent's controls: collision brake, PIDs, brake rules
+ * stands behind: lav_agent_fast.py:228-231 and 325-352 (the stop counter, the 4/5 plan swap, pid_control called twice, the
+ *           brake model, plan_collide, the speed cap and the creep), pid_control :404-426, plan_collide :385-401 and
+ *           team_code_v2/pid.py, for b agents in one launch per 512 agents (one warp per agent).
+ * Per agent i, in the reference's order:
+ *   stop counter += 1 when (double)speed < 0.1, else 0.  plan = d_cast when h_cmd[i] is 4 or 5, else d_plan (both (b, t, 2)
+ *   fp32).  If the plan has no NaN, pid_control: w = plan * (float)ppm with y negated (fp32); desired = fp32 mean of the t-1
+ *   step lengths |w[s+1] - w[s]| (fp32 norms, numpy's pairwise summation order); angle = degrees(pi/2 - atan2f(w_a.y, w_a.x))
+ *   / 90 in fp64 with atan2f correctly rounded, a = aim_point[cmd]; delta = clip(desired * speed_ratio[cmd] - speed, 0,
+ *   clip_delta) in fp64.  Each PID window (n values, starting as n zeros) receives its error twice; its output is
+ *   kp * e + ki * mean(window) + kd * (w[-1] - w[-2]) in fp64 (mean in numpy's pairwise order; 0 and 0 when n == 1).
+ *   steer = clip(turn, -1, 1); brake = desired < brake_speed * ppm; throttle = brake ? 0 : clip(speed pid, 0, max_throttle).
+ *   A plan with a NaN gives (0, 0, 0) and steps no PID.
+ *   plan_collide: a forecast row whose first point has y > 0.5 * ppm is skipped, a branch scoring < cmd_thresh is skipped;
+ *   otherwise the branch collides when min_s |row[s] - plan[s]| < (its fp32 mean step length < brake_speed ? 1.0 : 2.5).  All
+ *   norms fp32, every comparison in fp64; a NaN anywhere in the branch or the plan means no collision.
+ *   Brake rules: (double)pred_bra > 0.1 or a collision -> throttle 0, brake 1; speed * 3.6 > max_speed -> throttle 0; stop
+ *   counter >= 600 -> creep counter = 20; creep counter > 0 -> throttle = max(0.4, throttle), brake 0, creep counter -= 1.
+ * Inputs: forecast rows d_other_locs (k, c, t, 2) fp32 and their scores d_other_cmds (k, c) fp32, agent i owning rows
+ *   [h_offsets[i], h_offsets[i+1]) (HOST int32[b+1], monotone, within 0..k, any number per agent); d_pred_bra, d_speed (b,)
+ *   fp32 (m/s); h_cmd (b,) HOST int32 in 0..c-1; *h_config read during the call.  2 <= t <= 32, 1 <= c <= 8, 1 <= turn_n,
+ *   speed_n <= 64, 0 <= aim_point[j] < t.
+ * State: d_state holds b records of lavb_agent_control_state_bytes(turn_n, speed_n) bytes (8-byte aligned):
+ *   { int stop_counter, creep_counter, turn_head, speed_head; double turn_window[turn_n], speed_window[speed_n]; }
+ *   a window's oldest value at index head, the others following cyclically.  All-zero bytes are the state of a new route.
+ * Outputs: d_control (b, 3) fp32 = steer, throttle, brake; d_flags (b,) int32, LAVB_CTL_* bits.  Every output of the b agents
+ *   is written; a rejected call writes nothing. */
+#define LAVB_CTL_PLAN_INVALID 1  /* the plan has a NaN: no PID step, controls (0, 0, 0) before the brake rules */
+#define LAVB_CTL_PID_BRAKE 2     /* pid_control's brake: the desired speed is below brake_speed * ppm */
+#define LAVB_CTL_BRAKE_MODEL 4   /* pred_bra > 0.1 */
+#define LAVB_CTL_COLLIDE 8       /* plan_collide, evaluated for every agent */
+#define LAVB_CTL_SPEED_CAP 16    /* speed * 3.6 > max_speed */
+#define LAVB_CTL_CREEP 32        /* the creep after 600 stopped ticks forced the throttle */
+#define LAVB_CTL_MAX_CMDS 8
+
+typedef struct lavb_control_config {
+  int aim_point[LAVB_CTL_MAX_CMDS];
+  double speed_ratio[LAVB_CTL_MAX_CMDS];
+  double turn_kp, turn_ki, turn_kd;
+  double speed_kp, speed_ki, speed_kd;
+  int turn_n, speed_n;
+  double brake_speed, clip_delta, max_throttle, max_speed, cmd_thresh, pixels_per_meter;
+} lavb_control_config;
+
+size_t lavb_agent_control_state_bytes(int turn_n, int speed_n);
+int lavb_agent_control(const float* d_plan, const float* d_cast, int b, int t, int c, const float* d_other_locs,
+                       const float* d_other_cmds, int k, const int* h_offsets, const float* d_pred_bra, const float* d_speed,
+                       const int* h_cmd, const lavb_control_config* h_config, void* d_state, float* d_control, int* d_flags,
+                       void* stream);
+
 /* ---------------------------------------------------------------- PointPillars voxeliser + pillar encoder
  * replaces: PointPillarNet.forward (lav/models/point_pillar.py:92-116) incl. grid_locations :70-79,
  *           pillar_generation/decorate :55-68,81-85, DynamicPointNet.forward :28-35 (torch_scatter

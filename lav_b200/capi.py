@@ -41,6 +41,18 @@ class ConvPairDesc(C.Structure):
     ]
 
 
+class ControlConfig(C.Structure):
+    """mirror of lavb_control_config"""
+    _fields_ = [
+        ("aim_point", C.c_int * 8), ("speed_ratio", C.c_double * 8),
+        ("turn_kp", C.c_double), ("turn_ki", C.c_double), ("turn_kd", C.c_double),
+        ("speed_kp", C.c_double), ("speed_ki", C.c_double), ("speed_kd", C.c_double),
+        ("turn_n", C.c_int), ("speed_n", C.c_int),
+        ("brake_speed", C.c_double), ("clip_delta", C.c_double), ("max_throttle", C.c_double), ("max_speed", C.c_double),
+        ("cmd_thresh", C.c_double), ("pixels_per_meter", C.c_double),
+    ]
+
+
 _SIGS = {
     "lavb_abi_version": (C.c_int, []),
     "lavb_last_error": (C.c_char_p, []),
@@ -76,6 +88,10 @@ _SIGS = {
     "lavb_plan_safety": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
                                    C.c_longlong, C.c_int, C.c_int, C.c_float, C.c_float, C.c_float, C.c_float, C.c_void_p,
                                    C.c_void_p]),
+    "lavb_agent_control_state_bytes": (C.c_size_t, [C.c_int, C.c_int]),
+    "lavb_agent_control": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p,
+                                     C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(ControlConfig), C.c_void_p, C.c_void_p,
+                                     C.c_void_p, C.c_void_p]),
     "lavb_roof_filter": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_longlong, C.c_void_p, C.c_longlong, C.c_void_p, C.c_int,
                                    C.c_void_p]),
     "lavb_stack_sweep": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_float, C.c_float, C.c_int, C.c_int, C.c_int,

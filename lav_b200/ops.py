@@ -826,6 +826,80 @@ def plan_safety(traj, actors, offsets, ego_ext, bev, grid=None, out=None):
     return out
 
 
+def agent_control_state_bytes(turn_n, speed_n):
+    """bytes of one agent's controller state (lavb_agent_control_state_bytes); all-zero bytes are a new route."""
+    n = int(lib().lavb_agent_control_state_bytes(int(turn_n), int(speed_n)))
+    if n == 0:
+        raise capi.LavbError(f"agent_control: PID windows {turn_n}, {speed_n} outside 1..64")
+    return n
+
+
+def agent_control_state_views(state, turn_n, speed_n):
+    """the named fields of a HOST copy of agent_control's state (a uint8 array of B records): stop (B,) and creep (B,) int32,
+    turn (B, turn_n) and speed (B, speed_n) fp64 = the PID windows, oldest value first."""
+    rec = np.dtype([("stop", np.int32), ("creep", np.int32), ("turn_head", np.int32), ("speed_head", np.int32),
+                    ("turn", np.float64, (turn_n,)), ("speed", np.float64, (speed_n,))])
+    s = np.ascontiguousarray(state).view(rec)
+    roll = lambda w, h: np.take_along_axis(w, (h[:, None] + np.arange(w.shape[1])[None]) % w.shape[1], axis=1)
+    return dict(stop=s["stop"].copy(), creep=s["creep"].copy(), turn=roll(s["turn"], s["turn_head"]),
+                speed=roll(s["speed"], s["speed_head"]))
+
+
+def agent_control(plan, cast, other_locs, other_cmds, offsets, pred_bra, speed, cmds, config, state, control=None, flags=None):
+    """The agent's controls for B agents in one launch (see lavb_agent_control in include/lav_b200.h): plan / cast (B,T,2) fp32 =
+    ego plan and ego cast under the command; other_locs (K,C,T,2) / other_cmds (K,C) fp32 = the forecast rows of all agents,
+    agent i owning rows [offsets[i], offsets[i+1]) (offsets (B+1,) int32 on the HOST); pred_bra, speed (B,) fp32; cmds (B,)
+    int32 on the HOST; config a capi.ControlConfig; state the agents' controller state, a contiguous uint8 device tensor of
+    B * agent_control_state_bytes(config.turn_n, config.speed_n) bytes, updated in place.
+    -> (control (B,3) fp32 = steer, throttle, brake; flags (B,) int32 of LAVB_CTL_* bits), written into ``control`` / ``flags``
+    when given."""
+    _need_cuda(plan, cast, other_locs, other_cmds, pred_bra, speed, state)
+    f32 = lambda x, shape: x.dtype == torch.float32 and tuple(x.shape) == shape and x.is_contiguous()
+    if plan.dtype != torch.float32 or plan.dim() != 3 or plan.shape[2] != 2 or not plan.is_contiguous():
+        raise capi.LavbError(f"agent_control: plan must be a contiguous (B, T, 2) fp32 tensor, got {plan.dtype} {tuple(plan.shape)}")
+    b, t, _ = plan.shape
+    if not f32(cast, (b, t, 2)):
+        raise capi.LavbError(f"agent_control: cast must be a contiguous ({b}, {t}, 2) fp32 tensor, got {cast.dtype} {tuple(cast.shape)}")
+    if other_locs.dim() != 4 or not f32(other_locs, (other_locs.shape[0], other_locs.shape[1], t, 2)):
+        raise capi.LavbError(f"agent_control: other_locs must be a contiguous (K, C, {t}, 2) fp32 tensor, got {other_locs.dtype} "
+                             f"{tuple(other_locs.shape)}")
+    k, c = other_locs.shape[:2]
+    if not f32(other_cmds, (k, c)):
+        raise capi.LavbError(f"agent_control: other_cmds must be a contiguous ({k}, {c}) fp32 tensor, got {other_cmds.dtype} "
+                             f"{tuple(other_cmds.shape)}")
+    if not f32(pred_bra, (b,)) or not f32(speed, (b,)):
+        raise capi.LavbError(f"agent_control: pred_bra and speed must be contiguous ({b},) fp32 tensors, got "
+                             f"{tuple(pred_bra.shape)} and {tuple(speed.shape)}")
+    offsets = np.ascontiguousarray(offsets.numpy() if torch.is_tensor(offsets) else offsets)
+    if offsets.dtype != np.int32 or offsets.shape != (b + 1,):
+        raise capi.LavbError(f"agent_control: offsets must be a host ({b + 1},) int32 array, got {offsets.dtype} {offsets.shape}")
+    cmds = np.ascontiguousarray(cmds.numpy() if torch.is_tensor(cmds) else cmds)
+    if cmds.dtype != np.int32 or cmds.shape != (b,):
+        raise capi.LavbError(f"agent_control: cmds must be a host ({b},) int32 array, got {cmds.dtype} {cmds.shape}")
+    if not isinstance(config, capi.ControlConfig):
+        raise capi.LavbError("agent_control: config must be a capi.ControlConfig")
+    nbytes = b * agent_control_state_bytes(config.turn_n, config.speed_n)
+    if state.dtype != torch.uint8 or tuple(state.shape) != (nbytes,) or not state.is_contiguous():
+        raise capi.LavbError(f"agent_control: state must be a contiguous ({nbytes},) uint8 tensor, got {state.dtype} {tuple(state.shape)}")
+    dev = plan.device
+    if len({dev, cast.device, other_locs.device, other_cmds.device, pred_bra.device, speed.device, state.device}) != 1:
+        raise capi.LavbError("agent_control: the inputs must be on one device")
+    if control is None:
+        control = torch.empty((b, 3), dtype=torch.float32, device=dev)
+    elif not f32(control, (b, 3)) or control.device != dev:
+        raise capi.LavbError(f"agent_control: control must be a contiguous ({b}, 3) fp32 tensor on {dev}")
+    if flags is None:
+        flags = torch.empty((b,), dtype=torch.int32, device=dev)
+    elif flags.dtype != torch.int32 or tuple(flags.shape) != (b,) or not flags.is_contiguous() or flags.device != dev:
+        raise capi.LavbError(f"agent_control: flags must be a contiguous ({b},) int32 tensor on {dev}")
+    ip = lambda a: a.ctypes.data_as(C.c_void_p)
+    check(lib().lavb_agent_control(_ptr(plan), _ptr(cast), b, t, c, _ptr(other_locs), _ptr(other_cmds), k, ip(offsets),
+                                   _ptr(pred_bra), _ptr(speed), ip(cmds), C.byref(config), _ptr(state), _ptr(control),
+                                   _ptr(flags), _stream()), "lavb_agent_control")
+    _COUNT[0] += -(-b // 512)
+    return control, flags
+
+
 PILLAR_ENCODER ="sorted"    # name of the 16-bit pipeline's pillar encoder, reported by bench.py; it selects nothing
 
 
