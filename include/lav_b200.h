@@ -162,7 +162,8 @@ int lavb_det_heatmaps(const void* d_actors, const int* d_offsets, int b, int h, 
  * BEV: d_seg (b, h, w, 3) NHWC sigmoid probabilities, fp32 or h16 (seg_dtype); d_gt (b, gt_planes, h, w) uint8, planes 0..2 the
  *   targets.  d_iou (b, 3, 2) int64 = per channel (|pred > 0.5 and gt != 0|, |pred > 0.5 or gt != 0|).  h * w % 4 == 0.
  * Detections: d_packed (b, 7, 2 * n_det) fp32 = lavb_det_peaks' output (class c in columns [c * n_det, (c + 1) * n_det)), the
- *   peak pixel (flat % w, flat / w).  A peak survives InferModel.decode_packed's filters: score > min_score, not (class 1 and both
+ *   peak pixel (flat % w, flat / w).  A peak survives InferModel.decode_packed's filters: score > float32(min_score) compared
+ *   in fp32 (as the reference's `s > min_score` on an fp32 tensor; a NaN score never survives), not (class 1 and both
  *   box sides < float32(0.1 * ppm)), and 2 < d < 30 * ppm pixels from (cx0, cy0 + cy1).  d_actors: lavb_det_heatmaps' table
  *   (24-byte records, n_actors rows), sample i owning rows [h_offsets[i], h_offsets[i+1]) (HOST int32[b+1], monotone, at most
  *   1024 rows per sample); an actor of class typ (0 / 1, others ignored) counts when its centre, placed as lavb_det_heatmaps
@@ -408,10 +409,18 @@ int lavb_maxpool3x3s2_nhwc(const void* d_in, int n, int h, int w, int c, void* d
 
 /* ---------------------------------------------------------------- detection decode (device part)
  * replaces: extract_peak (team_code_v2/model_inference.py:189-202: sigmoid, 7x7 max-pool NMS, top-k) and the per-peak
- * map reads of det_inference (:100-112).  d_center: heat-map LOGITS, d_box / d_ori: size / orientation maps, all fp32
- * NHWC [batch][h][w][2] (ncls = 2 classes in d_center).  Only local maxima with sigmoid > min_score are kept (anything
- * else is dropped by the reference's host filter anyway); per (frame, class) the max_det best go to
- * d_packed [batch][7][ncls*max_det] = score | flat index | w | h | cos | sin | W, -1e5 scores padding the rest. */
+ * map reads of det_inference (:100-112).  d_center: heat-map LOGITS fp32 NHWC [batch][h][w][ncls]; d_box / d_ori: size /
+ * orientation maps fp32 NHWC [batch][h][w][2], shared by the classes.  Score s = 1 / (1 + expf(-logit)) in fp32, bit for bit
+ * torch.sigmoid on the device.  A pixel is a peak when nothing in its 7x7 window (pixels off the map ignored) is larger
+ * (equal neighbours are all peaks); a NaN in the window never suppresses, as in max_pool2d.  Candidates: the peaks with
+ * s > min_score compared in fp32, plus every NaN pixel (torch.topk ranks NaN first, so a NaN takes one of the reference's
+ * max_det slots; the host filter then drops it).  Anything else is dropped by the reference's host filter anyway.  Per
+ * (frame, class) the max_det first candidates — NaN first, then descending s, ties (and NaNs among themselves) to the
+ * lower flat index y * w + x — fill d_packed [batch][7][ncls*max_det] = s | flat index | w | h | cos | sin | W with the
+ * box and orientation values at the peak; the columns past the last candidate are (-1e5, 0, 0, 0, 0, 0, W).  The output
+ * depends on the maps alone: however many candidates a class has, the selection is exact.  1 <= ncls <= 8,
+ * 1 <= max_det <= 64, h, w >= 1, h * w <= 2^24 (the flat index is stored as fp32); batch = 0 writes nothing.  A rejected
+ * call writes nothing.  d_workspace: lavb_det_peaks_workspace_bytes(batch, ncls) bytes. */
 size_t lavb_det_peaks_workspace_bytes(int batch, int ncls);
 int lavb_det_peaks(const float* d_center, const float* d_box, const float* d_ori, int batch, int h, int w, int ncls,
                    float min_score, int max_det, float* d_packed, void* d_workspace, void* stream);

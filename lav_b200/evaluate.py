@@ -54,7 +54,7 @@ ops.det_forecast_match launch and one ops.forecast_eval launch into the same buf
 one copy of the packed peaks (B x 7 x 30 floats) that the row table is built from; no extra model call.  The protocol:
 
   Rows.  A row is a detection infer_batch forecasts: a class-1 packed peak that passes decode_packed's filters
-    (model_inference.peak_filter: score > 0.2, the size filter, 2 px < d < 30 m) and det_to_locs' centre test
+    (model_inference.peak_filter: score > float32(0.2) in fp32, the size filter, 2 px < d < 30 m) and det_to_locs' centre test
     (heads.off_centre: more than 4 px from the crop centre), in frame order, then packed-column order: the order of the
     concatenated other_cast_locs, whose per-frame lengths must equal the row counts.  The row table (frame, column) is built on
     the host (detected_rows) from a copy of the packed peaks.

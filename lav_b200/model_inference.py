@@ -23,17 +23,24 @@ def extract_peak_batch(heat, max_pool_ks=7, max_det=15):
     return torch.topk(possible.flatten(1), min(max_det, possible[0].numel()), dim=1)
 
 
+def score_kept(score, min_score=0.2):
+    """det_inference's score test (model_inference.py:101-103): the reference compares each fp32 score, a 0-d tensor, with the
+    Python float min_score, and torch does that in fp32.  So a score of exactly float32(min_score) is dropped, and so is NaN."""
+    return np.asarray(score, np.float32) > np.float32(min_score)
+
+
 def peak_filter(packed, pixels_per_meter, ncls=2, min_score=0.2):
-    """decode_packed's filters on host packed peaks (B, 7, ncls * n) (det_inference, model_inference.py:98-121): score threshold,
-    the class-1 size filter, the ego-distance window.  -> keep (B, cols) bool, x, y (B, cols) int64 pixel, cls (cols,)."""
+    """decode_packed's filters on host packed peaks (B, 7, ncls * n) (det_inference, model_inference.py:98-121): score threshold
+    (score_kept), the class-1 size filter, the ego-distance window.  -> keep (B, cols) bool, x, y (B, cols) int64 pixel, cls
+    (cols,)."""
     W = int(packed[0, 6, 0])
     nd = packed.shape[2] // ncls
-    score, loc = packed[:, 0].astype(np.float64), packed[:, 1].astype(np.int64)
+    loc = packed[:, 1].astype(np.int64)
     x, y = loc % W, loc // W
     w, h = packed[:, 2], packed[:, 3]
     cls = np.arange(packed.shape[2]) // nd
     dist = np.sqrt(((x - 160) ** 2 + (y - 280) ** 2).astype(np.float64))     # TODO hard-code of the reference kept
-    keep = (score > min_score) & ~((cls[None] == 1) & (np.maximum(w, h) < 0.1 * pixels_per_meter))
+    keep = score_kept(packed[:, 0], min_score) & ~((cls[None] == 1) & (np.maximum(w, h) < 0.1 * pixels_per_meter))
     keep &= ~((dist <= 2) | (dist >= 30 * pixels_per_meter))
     return keep, x, y, cls
 

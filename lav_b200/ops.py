@@ -926,10 +926,12 @@ def pillar_forward_sorted(pts, starts, counts, grid, w1, s1, t1, w2, s2, t2, can
 
 
 def det_peaks(center, box, ori, min_score=0.2, max_det=15):
-    """center (LOGITS), box, ori: fp32 NHWC (B,H,W,2) contiguous -> packed (B,7,2*max_det) (see lavb_det_peaks)."""
+    """center (LOGITS) fp32 NHWC (B,H,W,ncls), box, ori: fp32 NHWC (B,H,W,2), all contiguous -> packed (B,7,ncls*max_det)
+    (see lavb_det_peaks)."""
     _need_cuda(center, box, ori)
-    assert center.is_contiguous() and box.is_contiguous() and ori.is_contiguous() and center.dtype == torch.float32
+    assert center.dim() == 4 and all(t.is_contiguous() and t.dtype == torch.float32 for t in (center, box, ori))
     b, h, w, ncls = center.shape
+    assert tuple(box.shape) == tuple(ori.shape) == (b, h, w, 2), "det_peaks: box and ori must be (B, H, W, 2)"
     packed = torch.empty((b, 7, ncls * max_det), dtype=torch.float32, device=center.device)
     ws = _workspace(center.device, lib().lavb_det_peaks_workspace_bytes(b, ncls))
     check(lib().lavb_det_peaks(_ptr(center), _ptr(box), _ptr(ori), b, h, w, ncls, min_score, max_det, _ptr(packed), _ptr(ws), _stream()),

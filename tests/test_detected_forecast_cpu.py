@@ -6,6 +6,7 @@ import math
 import numpy as np
 import torch
 
+from lav_b200.model_inference import score_kept
 from tests import test_evaluate_cpu as E
 from tests import test_forecast_eval_cpu as F
 
@@ -28,7 +29,7 @@ def row_table_ref(packed, ppm=4, centre=CENTRE, min_score=0.2):
             x, y = loc % W, loc // W
             d = math.sqrt((x - 160) ** 2 + (y - 280) ** 2)
             small = np.float32(max(packed[b, 2, j], packed[b, 3, j])) < np.float32(0.1 * ppm)
-            if not float(packed[b, 0, j]) > min_score or small or d <= 2 or d >= 30 * ppm:
+            if not score_kept(packed[b, 0, j], min_score) or small or d <= 2 or d >= 30 * ppm:
                 continue
             if math.sqrt((x - centre[0]) ** 2 + (y - centre[1]) ** 2) <= 4:
                 continue
@@ -114,11 +115,11 @@ def agent_rows(packed, ppm=4):
     return [Planner().det_to_locs(d[1], 320, 320)[0] for d in dets]
 
 
-def test_row_table_equals_decode_packed_and_det_to_locs():
+def test_row_table_equals_decode_packed_and_det_to_locs_in_fp32():
     from lav_b200.evaluate import detected_rows
     below = float(np.nextafter(np.float32(0.2), np.float32(0)))
     frames = [
-        [(1, 0.9, 100, 200, 5, 5), (1, below, 110, 200, 5, 5), (1, 0.2, 120, 200, 5, 5),   # just below 0.2 / float32(0.2) > 0.2
+        [(1, 0.9, 100, 200, 5, 5), (1, below, 110, 200, 5, 5), (1, 0.2, 120, 200, 5, 5),   # below / exactly float32(0.2): both dropped
          (0, 0.9, 130, 200, 5, 5), (0, 0.5, 90, 90, 0, 0),                                 # class 0: decoded, never a row
          (1, 0.8, 163, 280, 5, 5), (1, 0.8, 164, 280, 5, 5), (1, 0.8, 160, 276, 5, 5),     # within 4 px of the crop centre
          (1, 0.8, 165, 280, 5, 5), (1, 0.7, 160, 281, 5, 5), (1, 0.7, 160, 160, 5, 5),     # 5 px: kept; outside the window
@@ -130,19 +131,21 @@ def test_row_table_equals_decode_packed_and_det_to_locs():
     packed = np.concatenate([E.packed_of(p) for p in frames])
     want = agent_rows(packed)
     frame, col, locs = row_table_ref(packed)
-    assert [int((frame == b).sum()) for b in range(3)] == [len(w) for w in want] == [6, 0, 2]
+    assert [int((frame == b).sum()) for b in range(3)] == [len(w) for w in want] == [5, 0, 2]
     assert np.array_equal(locs, np.array([x for w in want for x in w], np.float32).reshape(-1, 2))
-    assert col.tolist() == [15, 17, 21, 25, 26, 27, 15, 16]
+    assert col.tolist() == [15, 21, 25, 26, 27, 15, 16]
     got = detected_rows(packed, 4, CENTRE)
     assert np.array_equal(got["frame"], frame) and np.array_equal(got["col"], col) and np.array_equal(got["locs"], locs)
-    assert got["counts"].tolist() == [6, 0, 2] and np.array_equal(got["score"], packed[frame, 0, col])
+    assert got["counts"].tolist() == [5, 0, 2] and np.array_equal(got["score"], packed[frame, 0, col])
 
 
-def test_row_table_on_random_peaks():
+def test_row_table_on_random_peaks_in_fp32():
+    """Scores rounded to two decimals, so float32(0.2) occurs: those columns are never rows (the reference compares in fp32)."""
     from lav_b200.evaluate import detected_rows
     rs = np.random.RandomState(5)
     packed = np.zeros((40, 7, 30), np.float32)
     packed[:, 0] = np.round(rs.rand(40, 30) * 0.5, 2)
+    assert (packed[:, 0] == np.float32(0.2)).any()
     packed[:, 1] = np.where(rs.rand(40, 30) < 0.3, 280 * 320 + 160 + rs.randint(-6, 7, (40, 30)) + 320 * rs.randint(-6, 7, (40, 30)),
                             rs.randint(0, 320 * 320, (40, 30)))
     packed[:, 2:4] = rs.uniform(0, 1, (40, 2, 30))
@@ -153,6 +156,7 @@ def test_row_table_on_random_peaks():
     assert np.array_equal(locs, np.array([x for w in want for x in w], np.float32).reshape(-1, 2))
     got = detected_rows(packed, 4, CENTRE)
     assert np.array_equal(got["frame"], frame) and np.array_equal(got["col"], col) and np.array_equal(got["locs"], locs)
+    assert not (packed[frame, 0, col] <= np.float32(0.2)).any()
 
 
 # ---------------------------------------------------------------------------------------------------- the match

@@ -5,6 +5,8 @@ import numpy as np
 import pytest
 import torch
 
+from lav_b200.model_inference import score_kept
+
 THRESHOLDS = (0.5, 1.0, 2.0, 4.0)
 GRID = dict(ppm=4, cx0=160.0, cy0=320.0, cy1=-40.0)          # ops.det_grid() of the default map
 
@@ -36,12 +38,12 @@ def survivors(packed, w=320, min_score=0.2, grid=GRID):
     """decode_packed's filters on packed peaks (B,7,2*n_det) -> keep (B,cols) bool, x, y (int64), loc (int64)."""
     packed = np.asarray(packed, np.float32)
     ppm = grid["ppm"]
-    score, loc = packed[:, 0].astype(np.float64), packed[:, 1].astype(np.int64)
+    loc = packed[:, 1].astype(np.int64)
     x, y = loc % w, loc // w
     bw, bh = packed[:, 2], packed[:, 3]
     cls = np.arange(packed.shape[2]) // (packed.shape[2] // 2)
     dist = window_dist(x, y, grid)
-    keep = (score > min_score) & ~((cls[None] == 1) & (np.maximum(bw, bh) < 0.1 * ppm))
+    keep = score_kept(packed[:, 0], min_score) & ~((cls[None] == 1) & (np.maximum(bw, bh) < 0.1 * ppm))
     keep &= ~((dist <= 2) | (dist >= 30 * ppm))
     return keep, x, y, loc
 

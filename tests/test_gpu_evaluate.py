@@ -62,7 +62,9 @@ def check_equal(got, want):
 
 @pytest.mark.parametrize("B", [1, 7, 64])
 @pytest.mark.parametrize("half", [False, True])
-def test_eval_batch_equals_the_numpy_statement(cuda, B, half):
+def test_eval_batch_equals_the_fp32_threshold_statement(cuda, B, half):
+    """The kernel equals the numpy statement, whose score threshold is model_inference.score_kept: a packed score of exactly
+    float32(0.2) (random_batch rounds scores to one decimal) is not a survivor, as in the reference."""
     seg, gt, packed, actors, offsets, plan, ego = random_batch(B, B + 100 * half, cuda)
     if half:
         seg = seg.to(ops.h16())
@@ -71,6 +73,8 @@ def test_eval_batch_equals_the_numpy_statement(cuda, B, half):
                             plan.cpu().numpy(), ego.cpu().numpy())
     check_equal(v, want)
     f = v["flags"].numpy()
+    at = packed.cpu().numpy()[:, 0] == np.float32(0.2)
+    assert at.any() and not (f[at] & 16).any()
     if B > 1:
         assert (f & 1).any() and ((f & 16) & ~(f & 1)).any()              # matches and misses both occur
         assert not (f[1] & 16).any() and v["ngt"].numpy()[0].sum() == 0
