@@ -429,7 +429,12 @@ int lavb_det_peaks(const float* d_center, const float* d_box, const float* d_ori
  * replaces: UniPlanner.crop_feature (team_code_v2/models/uniplanner.py:303-340; model_inference.py:204-238) =
  *           F.affine_grid(theta, align_corners=True) + F.grid_sample(bilinear, zeros padding, align_corners=True).
  * d_feat NHWC [b][h][w][c]; crop k samples frame d_frame_idx[k] with the 2x3 affine d_theta[k]; out NHWC
- * [k][crop][crop][c] in the feature dtype. */
+ * [k][crop][crop][c] in the feature dtype.  d_frame_idx: int32 [k]; d_theta: fp32 [k][2][3].
+ * dtype LAVB_F32 (c a positive multiple of 4) or the library's 16-bit type (c a positive multiple of 8): a thread moves
+ * 16 bytes of channels, so d_feat and d_out must be 16-byte aligned.  b, h, w >= 1 (maps one pixel wide or high included),
+ * crop >= 2, 0 <= k <= 65535; k = 0 launches nothing and writes nothing.  Frame indices outside [0, b) are clamped to the
+ * nearest frame.  Every element of d_out is written (zeros where a sample leaves the map).  Accumulation is fp32 in the same
+ * fmaf order for both dtypes; the 16-bit output is the fp32 result rounded once to nearest. */
 int lavb_crop_bilinear(const void* d_feat, int dtype, int b, int h, int w, int c, const int* d_frame_idx,
                        const float* d_theta, int k, int crop, void* d_out, void* stream);
 /* the same crop from a uint8 PLANAR map (the ground-truth BEV): d_map [b][c][h][w] uint8 -> d_out NCHW [k][c][crop][crop] fp32.
@@ -442,7 +447,11 @@ int lavb_crop_bilinear_u8(const uint8_t* d_map, int b, int c, int h, int w, cons
                           int k, int crop, float* d_out, void* stream);
 /* gradient of lavb_crop_bilinear with respect to d_feat (fp32 NHWC; training, lav/models/uniplanner.py:56-151 through F.grid_sample):
  * replaces cudnn_grid_sampler_backward + the index_put of `features[frame]`.  A gather over the crops of each frame — no
- * atomics, fixed summation order, EVERY element of d_gfeat [b][h][w][c] is written (zeros where no crop samples). */
+ * atomics, fixed summation order, EVERY element of d_gfeat [b][h][w][c] is written (zeros where no crop samples, and for
+ * every frame when k = 0).  d_gout fp32 NHWC [k][crop][crop][c]; d_frame_idx, d_theta as in lavb_crop_bilinear, frame
+ * indices clamped the same way.  c a positive multiple of 4, d_gout and d_gfeat 16-byte aligned, 1 <= b <= 65535,
+ * h, w >= 1, crop >= 2, k >= 0.  Any theta is accepted; one with no usable inverse (a map one pixel wide or high, a
+ * rank-deficient theta) is handled exactly, at the cost of visiting every crop pixel for each feature pixel. */
 int lavb_crop_bilinear_bwd(const float* d_gout, int b, int h, int w, int c, const int* d_frame_idx, const float* d_theta,
                            int k, int crop, float* d_gfeat, void* stream);
 

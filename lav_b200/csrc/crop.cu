@@ -144,11 +144,13 @@ __global__ void __launch_bounds__(256) crop_u8_kernel(const uint8_t* __restrict_
 //   gfeat[b, y, x, :] = sum over crops k of frame b, crop pixels (i, j) whose 2x2 footprint contains (x, y):  w * gout[k, j, i, :]
 // The sample position is affine in (i, j); its inverse gives the (at most ~4x4) candidate crop pixels of a feature pixel, and
 // each candidate's weight is then recomputed with the forward's own arithmetic, so forward and backward agree exactly on
-// which corner a sample touches.  block = 8x8 feature pixels of one frame, one warp per patch row; the crops of the frame
-// whose footprint meets the patch are listed once per block (in k order) in shared memory.
+// which corner a sample touches.  A crop whose sample position has no usable inverse (a map one pixel wide or high, a
+// rank-deficient theta) takes every crop pixel as a candidate: correct, and slow only for inputs the planners never build.
+// block = 8x8 feature pixels of one frame, one warp per patch row; the crops of the frame whose footprint meets the patch
+// are listed once per block (in k order) in shared memory.
 // ---------------------------------------------------------------------------------------------------------------------
 constexpr int kBwdList = 32;                       // crops per pass of the shared-memory list
-struct BwdCrop { float th[6]; float inv[4]; float c0, c1; int k; };
+struct BwdCrop { float th[6]; float inv[4]; float c0, c1, pad; int k; };
 
 __global__ void __launch_bounds__(256) crop_bwd_kernel(const float* __restrict__ gout, int B, int H, int W, int C,
                                                        const int* __restrict__ frame_idx, const float* __restrict__ theta,
@@ -201,6 +203,15 @@ __global__ void __launch_bounds__(256) crop_bwd_kernel(const float* __restrict__
             c.inv[0] = a11 * r; c.inv[1] = -a01 * r; c.inv[2] = -a10 * r; c.inv[3] = a00 * r;
             c.c0 = sx * (th[2] + 1.f - th[0] - th[1]); c.c1 = sy * (th[5] + 1.f - th[3] - th[4]);
             c.k = k;
+            c.pad = 1e-3f;                         // margin of the candidate window around the inverse image
+            // det 0 (sx or sy is 0 on a one-pixel map), lost to cancellation (rank-1 theta) or not finite: no inverse, so
+            // the window is centred on crop pixel 0 with a margin of S, i.e. the whole crop
+            const bool finite = isfinite(c.inv[0]) && isfinite(c.inv[1]) && isfinite(c.inv[2]) && isfinite(c.inv[3]);
+            if (!(fabsf(det) > 1e-5f * (fabsf(a00 * a11) + fabsf(a01 * a10))) || !finite) {
+              c.inv[0] = c.inv[1] = c.inv[2] = c.inv[3] = 0.f;
+              c.c0 = c.c1 = 0.f;
+              c.pad = (float)S;
+            }
           }
           const int total = n + __popc(m);
           if (total > kBwdList) {                  // list full inside this chunk: resume at the first crop that did not fit
@@ -227,7 +238,7 @@ __global__ void __launch_bounds__(256) crop_bwd_kernel(const float* __restrict__
             const BwdCrop& c = list[ci];
             const float dx = (float)x - c.c0, dy = (float)y - c.c1;
             const float is = c.inv[0] * dx + c.inv[1] * dy, js = c.inv[2] * dx + c.inv[3] * dy;
-            const float ri = fabsf(c.inv[0]) + fabsf(c.inv[1]) + 1e-3f, rj = fabsf(c.inv[2]) + fabsf(c.inv[3]) + 1e-3f;
+            const float ri = fabsf(c.inv[0]) + fabsf(c.inv[1]) + c.pad, rj = fabsf(c.inv[2]) + fabsf(c.inv[3]) + c.pad;
             const int i_lo = max(0, (int)ceilf(is - ri)), i_hi = min(S - 1, (int)floorf(is + ri));
             const int j_lo = max(0, (int)ceilf(js - rj)), j_hi = min(S - 1, (int)floorf(js + rj));
             const int ni = i_hi - i_lo + 1, nj = j_hi - j_lo + 1;
@@ -282,19 +293,22 @@ using namespace lavb;
 
 extern "C" int lavb_crop_bilinear(const void* d_feat, int dtype, int b, int h, int w, int c, const int* d_frame_idx,
                                   const float* d_theta, int k, int crop, void* d_out, void* stream) {
-  LAVB_CHECK_ARG(c % 8 == 0, "crop_bilinear: channels must be a multiple of 8 (got %d)", c);
-  LAVB_CHECK_ARG(crop >= 2 && b >= 1, "crop_bilinear: bad crop size / batch");
+  LAVB_CHECK_ARG(dtype == LAVB_F32 || dtype == LAVB_H16, "crop_bilinear: bad dtype %d", dtype);
+  const int vec = dtype == LAVB_F32 ? 4 : 8;       // channels per 16-byte vector
+  LAVB_CHECK_ARG(c >= vec && c % vec == 0, "crop_bilinear: channels must be a positive multiple of %d (got %d)", vec, c);
+  LAVB_CHECK_ARG(crop >= 2 && b >= 1 && h >= 1 && w >= 1, "crop_bilinear: bad crop size / map (%d; %d x %d x %d)", crop, b, h, w);
+  LAVB_CHECK_ARG(k >= 0, "crop_bilinear: negative crop count");
   if (k == 0) return 0;
   LAVB_CHECK_ARG(k <= 65535, "crop_bilinear: at most 65535 crops per call");
-  const int pw = (crop + 7) / 8, vec = dtype == LAVB_F32 ? 4 : 8;
+  LAVB_CHECK_ARG((uintptr_t)d_feat % 16 == 0 && (uintptr_t)d_out % 16 == 0, "crop_bilinear: feat and out must be 16-byte aligned");
+  const int pw = (crop + 7) / 8;
   const dim3 blocks(pw * pw, ceil_div(c, 4 * vec), k);
   cudaStream_t st = (cudaStream_t)stream;
   if (dtype == LAVB_F32)
     crop_kernel<float><<<blocks, 256, 0, st>>>((const float*)d_feat, b, h, w, c, d_frame_idx, d_theta, k, crop, (float*)d_out);
-  else if (dtype == LAVB_H16)
+  else
     crop_kernel<h16><<<blocks, 256, 0, st>>>((const h16*)d_feat, b, h, w, c, d_frame_idx, d_theta, k, crop,
                                                            (h16*)d_out);
-  else LAVB_CHECK_ARG(false, "crop_bilinear: bad dtype");
   LAVB_LAUNCH_OK();
   return 0;
 }
@@ -316,12 +330,15 @@ extern "C" int lavb_crop_bilinear_u8(const uint8_t* d_map, int b, int c, int h, 
 }
 
 // d(loss)/d(feat) of lavb_crop_bilinear for fp32 NHWC tensors: d_gout (k, crop, crop, c) -> d_gfeat (b, h, w, c), every element
-// written (zeros where no crop samples).  Replaces cudnn_grid_sampler_backward + the index_put of `features[frame]` in the
-// training forward of UniPlanner (lav/models/uniplanner.py:56-151).
+// written (zeros where no crop samples, every frame when k = 0).  Replaces cudnn_grid_sampler_backward + the index_put of
+// `features[frame]` in the training forward of UniPlanner (lav/models/uniplanner.py:56-151).
 extern "C" int lavb_crop_bilinear_bwd(const float* d_gout, int b, int h, int w, int c, const int* d_frame_idx, const float* d_theta,
                                       int k, int crop, float* d_gfeat, void* stream) {
-  LAVB_CHECK_ARG(c % 4 == 0, "crop_bilinear_bwd: channels must be a multiple of 4 (got %d)", c);
-  LAVB_CHECK_ARG(crop >= 2 && b >= 1 && b <= 65535, "crop_bilinear_bwd: bad crop size / batch");
+  LAVB_CHECK_ARG(c >= 4 && c % 4 == 0, "crop_bilinear_bwd: channels must be a positive multiple of 4 (got %d)", c);
+  LAVB_CHECK_ARG(crop >= 2 && b >= 1 && b <= 65535 && h >= 1 && w >= 1, "crop_bilinear_bwd: bad crop size / map (%d; %d x %d x %d)",
+                 crop, b, h, w);
+  LAVB_CHECK_ARG(k >= 0, "crop_bilinear_bwd: negative crop count");
+  LAVB_CHECK_ARG((uintptr_t)d_gout % 16 == 0 && (uintptr_t)d_gfeat % 16 == 0, "crop_bilinear_bwd: gout and gfeat must be 16-byte aligned");
   const dim3 blocks(((w + 7) / 8) * ((h + 7) / 8), b);
   crop_bwd_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(d_gout, b, h, w, c, d_frame_idx, d_theta, k, crop, d_gfeat);
   LAVB_LAUNCH_OK();

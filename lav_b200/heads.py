@@ -441,21 +441,23 @@ class UniPlanner(nn.Module):
     # -- crop: one CUDA kernel on channels-last features (or grid_sample for generic callers)
     def crop_feature(self, features, rel_locs, rel_oris, pixels_per_meter=4, crop_size=96, frame_idx=None):
         """features: logical (B,C,H,W).  With ``frame_idx`` (K,) the K crops read features[frame_idx[k]] without
-        materialising an expanded copy."""
+        materialising an expanded copy.  A map the crop kernel cannot take as it is (see ops.crop_supported) goes through
+        F.affine_grid + F.grid_sample."""
         B, C, H, W = features.size()
         theta = crop_theta(rel_locs, rel_oris, H, W, pixels_per_meter, crop_size, self.offset_x, self.offset_y)
         if features.is_cuda and not (torch.is_grad_enabled() and features.requires_grad):
             feats_nhwc = features.permute(0, 2, 3, 1)
-            if feats_nhwc.is_contiguous():
+            if ops.crop_supported(feats_nhwc):
                 if frame_idx is None:
                     frame_idx = torch.arange(theta.shape[0], device=features.device, dtype=torch.int32) % B
                 return ops.crop_bilinear(feats_nhwc, frame_idx, theta, crop_size).permute(0, 3, 1, 2)
-        if TRAIN_CROP_KERNEL and features.is_cuda and features.dtype == torch.float32 and C % 4 == 0:
+        if TRAIN_CROP_KERNEL and features.is_cuda and features.dtype == torch.float32:
             # training: same kernel forward, hand-written gather backward (ops.CropBilinear) instead of cudnn's atomics
             feats_nhwc = features.permute(0, 2, 3, 1).contiguous()           # no copy when `features` is channels-last
-            if frame_idx is None:
-                frame_idx = torch.arange(theta.shape[0], device=features.device, dtype=torch.int32) % B
-            return ops.CropBilinear.apply(feats_nhwc, frame_idx, theta, crop_size).permute(0, 3, 1, 2)
+            if ops.crop_supported(feats_nhwc):
+                if frame_idx is None:
+                    frame_idx = torch.arange(theta.shape[0], device=features.device, dtype=torch.int32) % B
+                return ops.CropBilinear.apply(feats_nhwc, frame_idx, theta, crop_size).permute(0, 3, 1, 2)
         if frame_idx is not None:
             features = features[frame_idx.long()]
         grids = F.affine_grid(theta, torch.Size((theta.shape[0], C, crop_size, crop_size)), align_corners=True)

@@ -286,14 +286,39 @@ def convert(src, dtype):
     return dst
 
 
-def crop_bilinear(feats_nhwc, frame_idx, theta, crop_size):
-    """feats_nhwc (B,H,W,C) contiguous fp32/f16; frame_idx (K,) int32; theta (K,2,3) fp32 -> (K,crop,crop,C)."""
-    _need_cuda(feats_nhwc, frame_idx, theta)
-    assert feats_nhwc.is_contiguous()
-    b, h, w, c = feats_nhwc.shape
+def crop_supported(feats_nhwc):
+    """True when lavb_crop_bilinear takes this (B,H,W,C) map as it is: contiguous and 16-byte aligned, fp32 with C a multiple
+    of 4 or the 16-bit type with C a multiple of 8 (a thread moves 16 bytes of channels)."""
+    vec = {torch.float32: 4, h16(): 8}.get(feats_nhwc.dtype)
+    return (vec is not None and feats_nhwc.dim() == 4 and feats_nhwc.is_contiguous() and feats_nhwc.data_ptr() % 16 == 0
+            and feats_nhwc.shape[3] > 0 and feats_nhwc.shape[3] % vec == 0)
+
+
+def _crop_poses(what, frame_idx, theta, b):
+    """the K crop poses as the kernels read them: frame_idx (K,) of any integer type -> int32 (values clamped to [0, B) first,
+    as the kernels clamp, so an int64 index past the int32 range still means the last frame), theta (K,2,3) -> fp32; both
+    contiguous.  Raises LavbError when they do not describe the same K crops."""
+    if theta.dim() != 3 or tuple(theta.shape[1:]) != (2, 3):
+        raise capi.LavbError(f"{what}: theta must be (K, 2, 3), got {tuple(theta.shape)}")
     k = theta.shape[0]
-    theta = theta.float().contiguous()
-    frame_idx = frame_idx.to(torch.int32).contiguous()
+    if frame_idx.dim() != 1 or frame_idx.numel() != k:
+        raise capi.LavbError(f"{what}: frame_idx {tuple(frame_idx.shape)} does not hold one frame per crop (K = {k})")
+    if frame_idx.dtype.is_floating_point or frame_idx.dtype.is_complex or frame_idx.dtype == torch.bool:
+        raise capi.LavbError(f"{what}: frame_idx must be an integer tensor, got {frame_idx.dtype}")
+    if frame_idx.dtype != torch.int32:
+        frame_idx = frame_idx.clamp(0, b - 1).to(torch.int32)
+    return k, frame_idx.contiguous(), theta.float().contiguous()
+
+
+def crop_bilinear(feats_nhwc, frame_idx, theta, crop_size):
+    """feats_nhwc (B,H,W,C) contiguous fp32 (C % 4 == 0) or h16 (C % 8 == 0); frame_idx (K,) integer; theta (K,2,3) ->
+    (K,crop,crop,C) in the feature dtype.  Frame indices outside [0, B) are clamped to the nearest frame."""
+    _need_cuda(feats_nhwc, frame_idx, theta)
+    if not crop_supported(feats_nhwc):
+        raise capi.LavbError(f"crop_bilinear: need a contiguous, 16-byte aligned (B,H,W,C) map, fp32 with C % 4 == 0 or "
+                             f"{h16()} with C % 8 == 0; got {feats_nhwc.dtype} {tuple(feats_nhwc.shape)}")
+    b, h, w, c = feats_nhwc.shape
+    k, frame_idx, theta = _crop_poses("crop_bilinear", frame_idx, theta, b)
     out = torch.empty((k, crop_size, crop_size, c), dtype=feats_nhwc.dtype, device=feats_nhwc.device)
     check(lib().lavb_crop_bilinear(_ptr(feats_nhwc), _DT[feats_nhwc.dtype], b, h, w, c, _ptr(frame_idx), _ptr(theta), k, crop_size,
                                    _ptr(out), _stream()), "lavb_crop_bilinear")
@@ -326,13 +351,27 @@ def crop_bilinear_u8(bev_u8, frame_idx, theta, crop_size, out=None):
     return out
 
 
-def crop_bilinear_bwd(gout_nhwc, frame_idx, theta, feat_shape):
-    """gout_nhwc (K,crop,crop,C) fp32 contiguous -> gradient of crop_bilinear w.r.t. the (B,H,W,C) fp32 feature map."""
+def crop_bilinear_bwd(gout_nhwc, frame_idx, theta, feat_shape, out=None):
+    """gout_nhwc (K,crop,crop,C) fp32 contiguous -> gradient of crop_bilinear w.r.t. the (B,H,W,C) fp32 feature map.
+    ``out`` (B,H,W,C) fp32 contiguous is written in full if given (zeros for every frame no crop samples)."""
     _need_cuda(gout_nhwc, frame_idx, theta)
-    assert gout_nhwc.is_contiguous() and gout_nhwc.dtype == torch.float32
-    b, h, w, c = feat_shape
-    k, crop = gout_nhwc.shape[0], gout_nhwc.shape[1]
-    gfeat = torch.empty((b, h, w, c), dtype=torch.float32, device=gout_nhwc.device)
+    if len(feat_shape) != 4:
+        raise capi.LavbError(f"crop_bilinear_bwd: feat_shape must be (B, H, W, C), got {tuple(feat_shape)}")
+    b, h, w, c = (int(v) for v in feat_shape)
+    if gout_nhwc.dtype != torch.float32 or gout_nhwc.dim() != 4 or not gout_nhwc.is_contiguous() or gout_nhwc.data_ptr() % 16:
+        raise capi.LavbError(f"crop_bilinear_bwd: gout must be a contiguous, 16-byte aligned fp32 (K, crop, crop, C) tensor, "
+                             f"got {gout_nhwc.dtype} {tuple(gout_nhwc.shape)}")
+    k, frame_idx, theta = _crop_poses("crop_bilinear_bwd", frame_idx, theta, b)
+    crop = gout_nhwc.shape[1]
+    if tuple(gout_nhwc.shape) != (k, crop, crop, c):
+        raise capi.LavbError(f"crop_bilinear_bwd: gout {tuple(gout_nhwc.shape)} does not match {k} square crops of the "
+                             f"{c}-channel map {tuple(feat_shape)}")
+    if out is None:
+        gfeat = torch.empty((b, h, w, c), dtype=torch.float32, device=gout_nhwc.device)
+    elif tuple(out.shape) != (b, h, w, c) or out.dtype != torch.float32 or not out.is_contiguous() or out.device != gout_nhwc.device:
+        raise capi.LavbError(f"crop_bilinear_bwd: out must be a contiguous fp32 ({b}, {h}, {w}, {c}) tensor on {gout_nhwc.device}")
+    else:
+        gfeat = out
     check(lib().lavb_crop_bilinear_bwd(_ptr(gout_nhwc), b, h, w, c, _ptr(frame_idx), _ptr(theta), k, crop, _ptr(gfeat), _stream()),
           "lavb_crop_bilinear_bwd")
     _COUNT[0] += 1
@@ -344,8 +383,8 @@ class CropBilinear(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, feats_nhwc, frame_idx, theta, crop_size):
-        frame_idx = frame_idx.to(torch.int32).contiguous()
-        theta = theta.detach().float().contiguous()
+        _need_cuda(frame_idx, theta)
+        _, frame_idx, theta = _crop_poses("CropBilinear", frame_idx, theta.detach(), feats_nhwc.shape[0])
         ctx.save_for_backward(frame_idx, theta)
         ctx.feat_shape = tuple(feats_nhwc.shape)
         return crop_bilinear(feats_nhwc, frame_idx, theta, crop_size)

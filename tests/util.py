@@ -52,6 +52,26 @@ def rel_err(a, b):
     return float((a - b).abs().max() / (b.abs().max() + 1e-12))
 
 
+def crop_ref64(feats_nchw, frame_idx, theta, S, padding="zeros"):
+    """lavb_crop_bilinear in float64: frame indices clamped to [0, B) as the kernel clamps them, then
+    F.affine_grid(theta, align_corners=True) + F.grid_sample(bilinear, align_corners=True).  feats (B,C,H,W), frame_idx (K,),
+    theta (K,2,3) -> (K,C,S,S) float64.  The bilinear weights are >= 0, so crop_ref64(|f|) is the per-element sum |w f| of
+    the forward.  ``padding`` other than the kernel's "zeros" is for error bounds (tests/test_gpu_crop_contract.py)."""
+    import torch.nn.functional as F
+    B, C = feats_nchw.shape[:2]
+    fi = frame_idx.long().cpu().clamp(0, B - 1)
+    grid = F.affine_grid(theta.double().cpu(), [theta.shape[0], C, S, S], align_corners=True)
+    return F.grid_sample(feats_nchw.double().cpu()[fi], grid, mode="bilinear", padding_mode=padding, align_corners=True)
+
+
+def crop_ref64_adjoint(gout_nchw, frame_idx, theta, feat_shape):
+    """the adjoint of crop_ref64 (the crop's gradient with respect to the (B,C,H,W) map) by float64 autograd through the same
+    call: gout (K,C,S,S) -> (B,C,H,W) float64.  Applied to |gout| it gives the per-element sum |w g| of the backward."""
+    f = torch.zeros(feat_shape, dtype=torch.float64, requires_grad=True)
+    out = crop_ref64(f, frame_idx, theta, gout_nchw.shape[-1])
+    return torch.autograd.grad(out, f, gout_nchw.double().cpu())[0]
+
+
 def seg_logit_err(got_prob, ref_feats, sd):
     """error of the seg head measured BEFORE its sigmoid, as a fraction of the logit scale: the reference module returns
     sigmoid(logits) with logits of O(30-90) on seeded weights, so a probability-space max-norm would measure the sigmoid's slope.
