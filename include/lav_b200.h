@@ -476,6 +476,21 @@ int lavb_conv_umma(const lavb_conv_desc* h_desc, void* stream);
 int lavb_conv7x7s2_umma(const void* d_in, int n, int h, int w, int cin, const void* d_w, const float* d_bias, void* d_out,
                         void* stream);
 
+/* ---------------------------------------------------------------- 3x3 convolution, output channels in M
+ * replaces (h16 path): the stride-1 and stride-2 Conv2d -> ReLU -> BatchNorm2d layers of ConvBackbone (lidar.py:57-131) and the
+ * fused 4-head 384->256 conv (lidar.py:152-154) where LiDARModel routes them here (layers.py).  The kernel of
+ * lavb_conv7x7s2_umma with a 3x3 / pad-1 tap set: 16 x 16 output-pixel tiles, one TMA box per kernel row (stride 1) or per
+ * kernel row and column parity (stride 2).
+ *   d_in : h16 NHWC (n, h, w, cin), dense; cin in {64, 128, 384}; h, w >= 1
+ *   d_w  : h16 [9 taps (ky*3 + kx)][cout][cin] (the lavb_conv_umma packing); cout in {64, 128, 256}; stride in {1, 2}
+ *   d_out: h16 NHWC (n, (h-1)/stride+1, (w-1)/stride+1, cout), dense, saturating:
+ *          out = max(conv + bias, 0) * scale + shift with pre_relu, (conv + bias) * scale + shift without it; d_bias,
+ *          d_scale / d_shift (fp32 [cout]) may be NULL (0, 1 / 0; scale and shift come together).  The fp32 operations are
+ *          those of lavb_conv_umma's epilogue; with cin <= 128 at stride 1, and cin = 64 at stride 2, the MMA order is too, so
+ *          the output equals lavb_conv_umma's bit for bit. */
+int lavb_conv3x3_umma(const void* d_in, int n, int h, int w, int cin, int stride, const void* d_w, int cout, const float* d_bias,
+                      const float* d_scale, const float* d_shift, int pre_relu, void* d_out, void* stream);
+
 /* ---------------------------------------------------------------- fused (3x1 -> 1x3) convolution pair
  * replaces: conv3x1_k -> ReLU -> conv1x3_k -> bn_k [-> + input] -> ReLU of non_bottleneck_1d (lav/models/erfnet.py:37-63) in
  * one wgmma kernel; the intermediate activation stays in shared memory.

@@ -141,6 +141,8 @@ _SIGS = {
     "lavb_conv_umma": (C.c_int, [C.POINTER(ConvDesc), C.c_void_p]),
     "lavb_conv7x7s2_umma": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
                                       C.c_void_p]),
+    "lavb_conv3x3_umma": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_int, C.c_void_p,
+                                    C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
 }
 
 _lib = None

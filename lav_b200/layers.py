@@ -31,6 +31,17 @@ def _pad_cout(w_tco):
     return out.contiguous()
 
 
+def cmajor_wins(hout, wout):
+    """whether a 3x3 / pad-1 layer runs faster on lavb_conv3x3_umma (output channels in M) than on lavb_conv_umma.
+    `scripts/conv_umma_ab.py`, B = 32, H100 SXM at 700 W, median of 5 rounds (conv_umma -> conv3x3_umma):
+      64->64 s1 160^2   0.218 -> 0.137 ms     64->64 s2 320->160   0.242 -> 0.197 ms     heads 384->256 160^2  2.58 -> 2.12 ms
+      64->128 s2 160->80  0.107 -> 0.085 ms   128->128 s1 80^2     0.146 -> 0.121 ms
+      128->128 s2 80->40  0.053 -> 0.061 ms   128->128 s1 40^2     0.049 -> 0.053 ms
+    At 40 x 40 the 16 x 16 tiles cover 48 x 48 and a B = 32 layer has 288 of them for 132 SMs (3 rounds, the last a fifth
+    full), against 8 x 16 tiles at two CTAs per SM; so maps of 80 x 80 and more go to the channel-major kernel."""
+    return hout >= 80 and wout >= 80
+
+
 class TapConv:
     def __init__(self, weight, transposed=False, stride=1, padding=0, dilation=1, output_padding=0, bias=None,
                  pre_relu=False, scale=None, shift=None, post_relu=False, sigmoid=False, cin_pad=None):
@@ -79,6 +90,10 @@ class TapConv:
         # wgmma path (f16 activations): weights [ntaps][cout][cin] f16, K contiguous
         # (cout that is a multiple of 8 but not of 32 is zero-padded to the MMA width; only the real channels are stored)
         self.umma_ok = USE_UMMA and self.cin_k % 64 == 0 and self.cout % 8 == 0 and self.cout <= 256
+        # the 3x3 / pad-1 convolutions lavb_conv3x3_umma takes (output channels in M, 16 x 16 pixel tiles)
+        self.cmajor_ok = (self.umma_ok and not transposed and (self.kh, self.kw) == (3, 3) and self.padding == (1, 1)
+                          and self.dilation == (1, 1) and self.stride in ((1, 1), (2, 2)) and self.cin_k in (64, 128, 384)
+                          and self.cout in (64, 128, 256) and not post_relu and not sigmoid)
         if self.umma_ok:
             cm = (self.cout + 31) // 32 * 32
             for ph in self.phases:
@@ -106,6 +121,12 @@ class TapConv:
         hout, wout = self.out_size(hin, win)
         if out is None:
             out = torch.empty((n, hout, wout, out_channels or self.cout), dtype=out_dtype or x.dtype, device=x.device)
+        if (self.cmajor_ok and cmajor_wins(hout, wout) and x.dtype == ops.h16()
+                and out.dtype == ops.h16() and x.shape[3] == self.cin_k and in_coff == 0 and out.shape[3] == self.cout
+                and out_coff == 0 and res is None):
+            ph = self.phases[0]
+            return ops.conv3x3_umma(x, ph["w_umma"], self.cout, self.stride[0], self.bias, self.scale, self.shift, self.pre_relu,
+                                    out=out)
         for ph in self.phases:
             osy, osx = ph["out_s"]
             ooy, oox = ph["out_o"]

@@ -1,8 +1,8 @@
 """LiDARModel / ConvBackbone / Head — drop-in mirrors of lav/models/lidar.py.
 
 Same constructors, forward signatures and ``state_dict`` keys; every conv / transposed conv
-(+ReLU+BatchNorm epilogue) runs in hand-written CUDA (csrc/conv_taps.cu; csrc/conv_umma.cu on the
-f16 path).  Tensors keep the reference's logical NCHW shapes but are stored channels-last.
+(+ReLU+BatchNorm epilogue) runs in hand-written CUDA (csrc/conv_taps.cu; csrc/conv_umma.cu and, for
+the large 3x3 layers, csrc/stem_umma.cu on the f16 path).  Tensors keep the reference's logical NCHW shapes but are stored channels-last.
 ``precision`` = 'fp32' (exact path, default) or 'f16' (tensor-core path).
 """
 import torch

@@ -1026,6 +1026,29 @@ def conv7x7s2_umma(x, w_packed, bias, out=None):
     return out
 
 
+def conv3x3_umma(x, w, cout, stride, bias=None, scale=None, shift=None, pre_relu=False, out=None):
+    """3x3 / pad 1 / stride 1 or 2 convolution with output channels in M (lavb_conv3x3_umma): x contiguous f16 NHWC (n, h, w, cin),
+    cin in (64, 128, 384); w (9, cout, cin) f16, the conv_umma packing; cout in (64, 128, 256); bias / scale / shift fp32 (cout,)
+    or None -> f16 NHWC (n, (h-1)//s+1, (w-1)//s+1, cout) = [relu](conv + bias) * scale + shift, written into `out` when given."""
+    _need_cuda(x, w)
+    assert x.dtype == h16() and x.is_contiguous() and x.dim() == 4
+    n, h, wd, cin = x.shape
+    assert w.dtype == h16() and w.is_contiguous() and tuple(w.shape) == (9, cout, cin), (tuple(w.shape), cout, cin)
+    for v in (bias, scale, shift):
+        assert v is None or (v.dtype == torch.float32 and v.is_contiguous() and v.numel() == cout)
+    ho, wo = (h - 1) // stride + 1, (wd - 1) // stride + 1
+    if out is None:
+        out = torch.empty((n, ho, wo, cout), dtype=h16(), device=x.device)
+    assert out.dtype == h16() and out.is_contiguous() and tuple(out.shape) == (n, ho, wo, cout)
+    e0 = _prof_begin()
+    check(lib().lavb_conv3x3_umma(_ptr(x), n, h, wd, cin, stride, _ptr(w), cout, _ptr(bias), _ptr(scale), _ptr(shift),
+                                  int(pre_relu), _ptr(out), _stream()), "lavb_conv3x3_umma")
+    # the label format of conv_taps' wgmma launches, so that bench.py's conv roofline keeps covering the same layers
+    _prof_end(f"umma:{cin}->{cout}x9taps@{ho}x{wo}", 2.0 * n * ho * wo * cout * cin * 9, e0)
+    _COUNT[0] += 1
+    return out
+
+
 def pack_conv7x7s2_weights(w):
     """(64, cin, 7, 7) conv weights -> (49, 64, cin) f16 [tap = ky*7 + kx][cout][cin], the layout conv7x7s2_umma reads."""
     assert w.dim() == 4 and tuple(w.shape[2:]) == (7, 7) and w.shape[0] == 64

@@ -1,7 +1,7 @@
 """A/B timing of the product's conv_umma layers (and the fused ERFNet pairs of conv_pair_umma) at bench shapes (B = 32 frames
-per agent group) for two builds of liblavb200.so.
+per agent group) for two builds of liblavb200.so, and of the two wgmma kernels of the 3x3 BEV convolutions in one build.
 
-    python scripts/conv_umma_ab.py --base-lib OTHER/liblavb200.so [--rounds 5] [--reps 10]
+    python scripts/conv_umma_ab.py [--base-lib OTHER/liblavb200.so] [--rounds 5] [--reps 10]
 
 Both libraries are loaded into one process; the rounds alternate base / this tree's build on the same inputs and weights.
 For every layer it prints the median kernel time (CUDA events over `reps` back-to-back launches), the GEMM rate and its
@@ -13,24 +13,42 @@ relative to the output's scale), and byte counts derived from the shapes:
   fill TB/s: all tiles' fill bytes of this tree over its median time
 The planner stem (conv7x7s2_umma, 128 and 9 crops of 96 x 96 x 384) is timed the same way, and so is every shape of the fused
 ERFNet pair a tick runs; the last line sums the pair times at their launch counts per tick.
+The base build runs every layer on the kernels it has (layers.cmajor_wins off), whatever this tree routes elsewhere.
+
+Kernel arm (this build only, always run): every 3x3 / pad-1 BEV layer on conv_umma_kernel (pixels in M, 8 x 16 tiles) and on
+lavb_conv3x3_umma (output channels in M, 16 x 16 tiles), alternating, with the same columns; fill KB/tile is per 256 output
+pixels for both (two conv_umma tiles, one conv3x3 tile per 128-channel CTA column).
 The card name, power limit and SM clocks are read in the same run.
 """
 import argparse
+import ctypes
 import os
 import subprocess
 import sys
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
-from lav_b200 import capi, ops
+from lav_b200 import capi, layers as L, ops
 from lav_b200.layers import TapConv
 
 PEAK = 989e12
 
 
 def load(path):
+    """capi.lib() of the library at `path`, binding only the entry points it exports (an older build lacks the newer ones)"""
+    saved = dict(capi._SIGS)
+    handle = ctypes.CDLL(path)
+    for name in [k for k in capi._SIGS if not hasattr(handle, k)]:
+        del capi._SIGS[name]
     capi._lib, capi.LIB_PATH = None, path
-    return capi.lib()
+    try:
+        return capi.lib()
+    finally:
+        capi._SIGS.clear()
+        capi._SIGS.update(saved)
+
+
+KERNEL_ARM = []   # (name, TapConv, input, GEMM flop) of the layers lavb_conv3x3_umma can run
 
 
 def layers(dev, B):
@@ -55,12 +73,17 @@ def layers(dev, B):
             -(-((wo - ph["out_o"][1] + ph["out_s"][1] - 1) // ph["out_s"][1]) // 16)
         out.append((name, lambda: layer(x, out=y), fl, (cout + 31) // 32 * 32,
                     [(cin, len(ph["taps"]), tiles(ph)) for ph in layer.phases]))
+        if layer.cmajor_ok:
+            KERNEL_ARM.append((name, layer, x, fl))
 
     bn = lambda c: dict(pre_relu=True, scale=rn(c).abs() + 0.5, shift=rn(c) * 0.1)
     tap("heads 384->256 160x160", B, 160, 160, 384, 256, 3, **bn(256))
     tap("bb 64->64 s1 160x160", B, 160, 160, 64, 64, 3, **bn(64))
     tap("bb 64->64 s2 320->160", B, 320, 320, 64, 64, 3, stride=2, **bn(64))
     tap("bb 128->128 s1 80x80", B, 80, 80, 128, 128, 3, **bn(128))
+    tap("bb 64->128 s2 160->80", B, 160, 160, 64, 128, 3, stride=2, **bn(128))
+    tap("bb 128->128 s2 80->40", B, 80, 80, 128, 128, 3, stride=2, **bn(128))
+    tap("bb 128->128 s1 40x40", B, 40, 40, 128, 128, 3, **bn(128))
     tap("erf down 64->64 s2 72x64", 3 * B, 72, 64, 64, 64, 3, stride=2, bias=rn(64) * 0.1, scale=rn(64).abs() + 0.5,
         shift=rn(64) * 0.1, post_relu=True)
     tap("erf up 128->64 36x32", 3 * B, 36, 32, 128, 64, 3, stride=2, transposed=True, opad=1, bias=rn(64) * 0.1,
@@ -141,6 +164,52 @@ def kblock_bytes(cout_mma, old_width=32):
     return old, 2 * 4 * a_per_wgmma + b, 128 * 128 + cout_mma * 128
 
 
+def cmajor_fill_bytes_per_tile(cin, cout, stride):
+    """TMA bytes from L2 into shared memory for one 16 x 16 tile of lavb_conv3x3_umma and one CTA column of min(cout, 128)
+    channels: per chunk and kernel row `stride` pixel boxes of 16 rows x (18 or 17) columns x 128 B, per tap and chunk one
+    weight box of that column's channels x 128 B"""
+    cols = 18 if stride == 1 else 17
+    return cin // 64 * (3 * stride * cols * 16 * 128 + 9 * min(cout, 128) * 128)
+
+
+def kernel_arm(rounds, reps):
+    """conv_umma_kernel against lavb_conv3x3_umma on every 3x3 BEV layer, in this build"""
+    med = lambda v: sorted(v)[len(v) // 2]
+    span = lambda v: f"{med(v):.3f} [{min(v):.3f}-{max(v):.3f}]"
+    print(f"\n{'layer (conv_umma vs conv3x3_umma)':34s} {'conv_umma ms':>24s} {'conv3x3 ms':>24s} {'TF/s':>7s} {'TF/s':>7s} "
+          f"{'/989':>5s} {'speedup':>7s} {'bitwise':>8s} {'fill KB/256px':>14s} {'fill TB/s':>10s}")
+    for name, layer, x, fl in KERNEL_ARM:
+        n, h, w, cin = x.shape
+        ho, wo = layer.out_size(h, w)
+        s = layer.stride[0]
+        ph = layer.phases[0]
+        ya = torch.empty(n, ho, wo, layer.cout, device=x.device, dtype=x.dtype)
+        yb = torch.empty_like(ya)
+        arms = {
+            "umma": lambda: ops.conv_taps(x, cin, 0, ya, layer.cout, 0, ho, wo, (s, s), (1, 1), (0, 0), ph["taps"], ph["w_umma"],
+                                          layer.bias, layer.scale, layer.shift, pre_relu=layer.pre_relu, umma=True),
+            "cmajor": lambda: ops.conv3x3_umma(x, ph["w_umma"], layer.cout, s, layer.bias, layer.scale, layer.shift, layer.pre_relu,
+                                               out=yb),
+        }
+        for f in arms.values():
+            f(); f()
+        torch.cuda.synchronize()
+        same = bool(torch.equal(ya, yb))
+        diff = "same" if same else f"{float((ya.float() - yb.float()).abs().max() / ya.float().abs().max()):.1e}"
+        t = {k: [] for k in arms}
+        for _ in range(rounds):
+            for k, f in arms.items():
+                t[k].append(time_ms(f, reps))
+        ncol = max(1, layer.cout // 128)
+        f_umma = 2 * fill_bytes_per_tile(cin, 9, layer.cout)
+        f_cm = ncol * cmajor_fill_bytes_per_tile(cin, layer.cout, s)
+        tiles_cm = n * -(-ho // 16) * -(-wo // 16)
+        rate = tiles_cm * f_cm / (med(t["cmajor"]) * 1e-3) / 1e12
+        print(f"{name:34s} {span(t['umma']):>24s} {span(t['cmajor']):>24s} {fl / med(t['umma']) / 1e9:7.1f} "
+              f"{fl / med(t['cmajor']) / 1e9:7.1f} {fl / (med(t['cmajor']) * 1e-3) / PEAK:5.2f} "
+              f"{med(t['umma']) / med(t['cmajor']):7.3f} {diff:>8s} {f'{f_umma // 1024}->{f_cm // 1024}':>14s} {rate:10.2f}")
+
+
 def time_ms(fn, reps):
     a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     a.record()
@@ -153,7 +222,7 @@ def time_ms(fn, reps):
 
 def main():
     ap = argparse.ArgumentParser()
-    ap.add_argument("--base-lib", required=True, help="liblavb200.so of the tree to compare against")
+    ap.add_argument("--base-lib", help="liblavb200.so of the tree to compare against (without it: the kernel arm only)")
     ap.add_argument("--batch", type=int, default=32)
     ap.add_argument("--rounds", type=int, default=5)
     ap.add_argument("--reps", type=int, default=10)
@@ -164,15 +233,23 @@ def main():
     q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.sm,clocks.max.sm", "--format=csv,noheader"],
                        capture_output=True, text=True).stdout.strip()
     print(f"device: {torch.cuda.get_device_name(dev)} | nvidia-smi name, power limit, SM clock, max SM clock: {q}")
+    ls = layers(dev, args.batch)
+    kernel_arm(args.rounds, args.reps)
+    if not args.base_lib:
+        return
     new_path = capi.LIB_PATH
     libs = {"base": load(os.path.abspath(args.base_lib)), "this": load(new_path)}
-    ls = layers(dev, args.batch)
+    wins = L.cmajor_wins
+
+    def use(k):                                   # the base build has no lavb_conv3x3_umma: keep its layers on conv_umma
+        capi._lib = libs[k]
+        L.cmajor_wins = wins if k == "this" else (lambda *a: False)
     times = {(n, k): [] for n, *_ in ls for k in libs}
     same = {}
     for name, run, *_ in ls:                      # warm up both builds on every shape; compare their outputs
         res = {}
-        for k, h in libs.items():
-            capi._lib = h
+        for k in libs:
+            use(k)
             for _ in range(2):
                 y = run()
             torch.cuda.synchronize()
@@ -181,10 +258,10 @@ def main():
                       float((res["base"].float() - res["this"].float()).abs().max() / res["base"].float().abs().max()))
     for _ in range(args.rounds):
         for name, run, *_ in ls:
-            for k, h in libs.items():
-                capi._lib = h
+            for k in libs:
+                use(k)
                 times[(name, k)].append(time_ms(run, args.reps))
-    capi._lib = libs["this"]
+    use("this")
     med = lambda v: sorted(v)[len(v) // 2]
     span = lambda v: f"{med(v):.3f} [{min(v):.3f}-{max(v):.3f}]"
     print(f"{'layer':34s} {'base ms [min-max]':>24s} {'this ms [min-max]':>24s} {'base TF/s':>9s} {'this TF/s':>9s} {'/989':>5s} "
