@@ -73,6 +73,23 @@ int lavb_paint_deconv_batched(const float* d_pts, int frames, int n, int pt_stri
                               const float* d_deconv, const float* h_cams, float* d_out, int out_stride,
                               long long out_frame_stride, int out_col0, int copy_cols, void* stream);
 
+/* ---------------------------------------------------------------- confusion counts of the segmentation model
+ * stands behind: an evaluation of RGBSegmentationModel (lav/models/rgb.py:35-45) against the recorded semantic camera images
+ *           (SegmentationDataset, lav/utils/datasets/seg_dataset.py:16-30, with filter_sem, lav/utils/__init__.py:3-8); the
+ *           reference has none.  The ERFNet logits are never materialised.
+ * One launch; one thread per feature pixel evaluates its 2 x 2 output pixels.  d_feat: NHWC (n, h/2, w/2, 16) fp32 or h16
+ *   (feat_dtype) = the input of output_conv, contiguous; d_deconv: lavb_paint_deconv_batched's 520-float table; d_labels:
+ *   uint8 (n, h, w) = the recorded CARLA tags; h_lut: HOST uint8[256] = the class of each tag (filter_sem as a table), read
+ *   during the call.
+ * Per output pixel (v, u): the logits of lavb_paint_deconv_batched before its softmax (bias[k], then fmaf over c = 0..15 in
+ *   order, weight phase [v&1][u&1]); the predicted class is the first index of the largest logit (ties to the lower class);
+ *   a pixel with a NaN logit counts as invalid and in no confusion entry.
+ * d_out: int32 (n, c_cls * c_cls + 1) = per image confusion[gt][pred], then the invalid count; integer sums, so the counts do
+ *   not depend on the schedule.  2 <= c_cls <= 8, h and w even, n <= 65535, every h_lut entry < c_cls; features 16-byte (fp32) /
+ *   8-byte (h16) and labels 2-byte aligned.  Every element of the n rows is written; a rejected call writes nothing. */
+int lavb_seg_confusion(const void* d_feat, int feat_dtype, const float* d_deconv, const uint8_t* d_labels, const uint8_t* h_lut,
+                       int n, int c_cls, int h, int w, int* d_out, void* stream);
+
 /* ---------------------------------------------------------------- sweep stacking
  * replaces: LAVAgent.get_stacked_lidar + move_lidar_points (team_code_v2/lav_agent_fast.py:363-383,547-565)
  * and the ego-roof filter LAVAgent.preprocess (lav_agent.py:448-457, roof_filter!=0 marks dropped rows x=NaN).

@@ -75,6 +75,28 @@ def infer_model(lidar_model, uniplanner, precision, camera_x, camera_z, device):
     return InferModel(lidar_model, up, camera_x, camera_z, device)
 
 
+def brake_model(bra_model, precision):
+    """The brake model the agent runs at ``precision``: a PRIVATE copy of ``bra_model`` (so a model object shared with a trainer /
+    checkpoint writer keeps its fp32 master weights) with its trunk and attention pools cast to the 16-bit type for "f16"."""
+    dt = ops.h16() if precision == "f16" else torch.float32
+    bra = copy.deepcopy(bra_model)
+    bra.conv_backbone.to(dt).to(memory_format=torch.channels_last)
+    bra.attn1.to(dt); bra.attn2.to(dt)
+    return bra
+
+
+def brake_probs(bra, rgbs_u8, tel_u8, u8=True):
+    """pred_bra (B,) of a brake_model copy on the camera bytes: rgbs_u8 (B, 3, H, W, 3) the three cameras side by side, tel_u8
+    (B, h, w, 3).  A 16-bit copy runs forward_u8 (the stem kernel on the raw bytes) when ``u8`` and STEM_U8; otherwise the float
+    call of lav_agent_fast.py:257-262,318-321 on the stitched wide view, which the caller runs under math_mode(precision)."""
+    if u8 and STEM_U8 and bra.conv_backbone.conv1.weight.dtype == ops.h16():
+        return bra.forward_u8(rgbs_u8, tel_u8)
+    B, n, H, W, _ = rgbs_u8.shape
+    wide = rgbs_u8.permute(0, 2, 1, 3, 4).reshape(B, H, n * W, 3).permute(0, 3, 1, 2).float()
+    tel = tel_u8.permute(0, 3, 1, 2).float()
+    return bra(wide.contiguous(memory_format=torch.channels_last), tel.contiguous(memory_format=torch.channels_last))
+
+
 @contextlib.contextmanager
 def math_mode(precision):
     """exact path: the cuDNN / cuBLAS heads must not drop to TF32 — scoped to the caller's block, the process-wide flags are
@@ -109,12 +131,8 @@ class FramePipeline:
         self.precision = precision
         self.seg_model.set_precision(precision)
         self.infer_model = infer_model(self._lidar_model, self._src_uniplanner, precision, self._cam[0], self._cam[1], self.device)
-        dt = ops.h16() if precision == "f16" else torch.float32
         if self._src_bra is not None:
-            bra = copy.deepcopy(self._src_bra)
-            bra.conv_backbone.to(dt).to(memory_format=torch.channels_last)
-            bra.attn1.to(dt); bra.attn2.to(dt)
-            self.bra_model = bra
+            self.bra_model = brake_model(self._src_bra, precision)
         return self
 
     def _math_mode(self):
@@ -165,10 +183,7 @@ class FramePipeline:
         out = im.forward_batch(stacked, counts, nxps, cmds)
         # (7) brake predictor on the stitched wide view + tele view (lav_agent_fast.py:257-262,318-321)
         if self.bra_model is not None and tel_u8 is not None:
-            wide = rgbs_u8.permute(0, 2, 1, 3, 4).reshape(B, 288, 768, 3).permute(0, 3, 1, 2).float()
-            tel = tel_u8.permute(0, 3, 1, 2).float()
-            out["pred_bra"] = self.bra_model(wide.contiguous(memory_format=torch.channels_last),
-                                             tel.contiguous(memory_format=torch.channels_last))
+            out["pred_bra"] = brake_probs(self.bra_model, rgbs_u8, tel_u8, u8=False)
         return out
 
 
@@ -301,12 +316,7 @@ class StaticFramePipeline(FramePipeline):
         return dict(features=feats, pred_bev=seg.permute(0, 3, 1, 2), packed=packed, pred_bra=bra, heat=heat)
 
     def _brake(self):
-        B = self.B
-        if STEM_U8 and self.bra_model.conv_backbone.conv1.weight.dtype == ops.h16():
-            return self.bra_model.forward_u8(self.rgbs, self.tels)
-        wide = self.rgbs.permute(0, 2, 1, 3, 4).reshape(B, 288, 768, 3).permute(0, 3, 1, 2).float()
-        tel = self.tels.permute(0, 3, 1, 2).float()
-        return self.bra_model(wide.contiguous(memory_format=torch.channels_last), tel.contiguous(memory_format=torch.channels_last))
+        return brake_probs(self.bra_model, self.rgbs, self.tels)
 
     def _g2_body(self, K, locs, oris, fidx):
         return self.infer_model.uniplanner.infer_device(self._o1["features"].permute(0, 3, 1, 2), locs, oris, fidx, K, self.nxps, self.cmds)

@@ -67,6 +67,8 @@ _SIGS = {
     "lavb_paint_deconv_batched": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_longlong, C.c_void_p, C.c_int, C.c_int, C.c_int,
                                             C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_longlong, C.c_int, C.c_int,
                                             C.c_void_p]),
+    "lavb_seg_confusion": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int,
+                                     C.c_void_p, C.c_void_p]),
     "lavb_stack_jobs": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p]),
     "lavb_bev_targets": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p]),
     "lavb_png_decode_gray8": (C.c_int, [C.c_void_p, C.c_longlong, C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_int,

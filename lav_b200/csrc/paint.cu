@@ -5,6 +5,7 @@
 // reference's fp32 operation order (k-sequential FMA chains, IEEE division, truncation toward
 // zero, bounds test on the truncated integers, later camera wins), then one gather.
 #include "common.cuh"
+#include "deconv_logits.cuh"
 
 namespace lavb {
 
@@ -239,8 +240,7 @@ extern "C" int lavb_paint_batched(const float* d_pts, int frames, int n, int pt_
 // frame).  So the last ERFNet layer — output_conv = ConvTranspose2d(16, C, 2, stride 2) (lav/models/erfnet.py:122-124,132) — is
 // evaluated inside the gather, for the hit pixel only: logits[k](v,u) = bias[k] + sum_c feat[v/2, u/2, c] * W[c][k][v%2][u%2],
 // followed by softmax and the background suppression of model_inference.py:45.  The (H x W x C) fp32 logit maps (141 MB per 32
-// frames) are never written, and the four launches of the transposed conv disappear.
-struct DeconvW { float w[2][2][16][8]; float bias[8]; };      // [v%2][u%2][c_in][k]  (k < c_cls <= 8)
+// frames) are never written, and the four launches of the transposed conv disappear.  The logits are deconv_logits.cuh's.
 
 template <typename TF>
 __global__ void __launch_bounds__(256) paint_deconv_kernel(const float* __restrict__ pts, int n, int pt_stride,
@@ -274,17 +274,9 @@ __global__ void __launch_bounds__(256) paint_deconv_kernel(const float* __restri
   const int hh = H >> 1, wh = W >> 1;
   const TF* f = feat + ((((long long)blockIdx.y * cams.ncam + hit_cam) * hh + (hit_v >> 1)) * wh + (hit_u >> 1)) * 16;
   float fv[16];
-#pragma unroll
-  for (int q = 0; q < 4; ++q) { const float4 t = load4<TF>(f + 4 * q); fv[4 * q] = t.x; fv[4 * q + 1] = t.y; fv[4 * q + 2] = t.z; fv[4 * q + 3] = t.w; }
-  const float (*wk)[8] = sw.w[hit_v & 1][hit_u & 1];
+  load_feat16<TF>(f, fv);
   float pr[8];
-#pragma unroll
-  for (int k = 0; k < 8; ++k) {
-    float acc = sw.bias[k];
-#pragma unroll
-    for (int c = 0; c < 16; ++c) acc = fmaf(fv[c], wk[c][k], acc);
-    pr[k] = acc;
-  }
+  deconv_logits<8>(sw, fv, hit_v & 1, hit_u & 1, pr);
   float mx = pr[0];
 #pragma unroll
   for (int k = 1; k < 8; ++k) if (k < c_cls) mx = fmaxf(mx, pr[k]);

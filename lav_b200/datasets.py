@@ -615,6 +615,108 @@ class TemporalBEVBatchLoader(TemporalBatchLoader):
                 torch.as_tensor(np.stack([h["typs"] for h in hs])).to(dev), ints("num_objs"))
 
 
+def load_img(env, tag, i):
+    """BasicDataset.load_img (basic_dataset.py:86-94) with the BGR -> RGB flip of the image datasets: key ``tag_%05d`` decoded by
+    cv2.imdecode, IMREAD_COLOR for an rgb tag (-> (h, w, 3) RGB), IMREAD_GRAYSCALE for a sem tag (-> (h, w))."""
+    import cv2
+    key = f"{tag}_{i:05d}"
+    data = env.get(key)
+    if data is None:
+        raise LavbError(f"record key {key} is missing")
+    img = cv2.imdecode(np.frombuffer(data, np.uint8), cv2.IMREAD_COLOR if "rgb" in tag else cv2.IMREAD_GRAYSCALE)
+    if img is None:
+        raise LavbError(f"record key {key} is not a decodable image")
+    return img[..., ::-1] if img.ndim == 3 else img
+
+
+class CameraDataset:
+    """The camera samples of a recording, for scoring the segmentation and brake models (lav_b200.evaluate_rgb): the frames of
+    BasicDataset (index_trajectories, the same YAML keys and ``overrides``), unaugmented.
+
+    Frame k holds, with ``seg``, every camera 0 .. len(camera_yaws) - 1 and its labels, SegmentationDataset's samples k * ncam + c
+    (seg_dataset.py:16-25); with ``brake``, the three middle cameras ncam//2 - 1 .. ncam//2 + 1, the telephoto view cut by
+    [:-crop_tel_bottom] and the brake label, BrakePredictionDataset's sample k (bra_dataset.py:17-31).  ``cams`` are the cameras
+    read (all with ``seg``, else the middle three) and ``brake_cams`` the positions of the middle three among them.  Images are
+    decoded on the host as BasicDataset.load_img decodes them, colour images flipped BGR -> RGB; no key a run does not need is
+    read.  The reference's augment(0.5) is training-only and not applied."""
+
+    def __init__(self, config_path, seg=True, brake=True, seed=2021, device=torch.device("cuda"), overrides=None):
+        if not (seg or brake):
+            raise LavbError("CameraDataset: nothing to load (neither seg nor brake)")
+        with open(config_path) as f:
+            cfg = yaml.safe_load(f)
+        cfg.update(overrides or {})
+        self.cfg = cfg
+        for k, v in cfg.items():
+            setattr(self, k, v)
+        self.device = torch.device(device)
+        self.seg, self.brake = seg, brake
+        ncam = len(self.camera_yaws)
+        mid = [ncam // 2 - 1, ncam // 2, ncam // 2 + 1]
+        if brake and (mid[0] < 0 or mid[2] >= ncam):
+            raise LavbError(f"CameraDataset: the brake model needs three middle cameras, the config has {ncam}")
+        self.cams = list(range(ncam)) if seg else mid
+        self.brake_cams = [self.cams.index(c) for c in mid] if brake else []
+        self.paths, self.index = index_trajectories(self.data_dir, self.percentage_data, self.all_towns, self.num_plan, seed)
+        self._envs, self._env_lock = {}, threading.Lock()
+
+    __len__ = TemporalLiDARPaintedDataset.__len__
+    env = TemporalLiDARPaintedDataset.env
+
+    def no_draw(self):
+        """no augmentation: nothing to draw."""
+        return ()
+
+    def prepare(self, idx):
+        """the decoded host images of frame ``idx``: rgbs (len(cams), h, w, 3), with seg labels (len(cams), h, w), with brake tel
+        (h_tel - crop_tel_bottom, w_tel, 3) and bra; uint8 numpy."""
+        traj, i = self.index[idx]
+        env = self.env(traj)
+        h = dict(rgbs=np.stack([load_img(env, f"rgb_{c}", i) for c in self.cams]))
+        if self.seg:
+            h["labels"] = np.stack([load_img(env, f"sem_{c}", i) for c in self.cams])
+        if self.brake:
+            h["tel"] = load_img(env, "tel_rgb", i)[:-self.crop_tel_bottom]
+            h["bra"] = int(_frame(env, "bra", i, np.uint8)[0])
+        return h
+
+    def stage_batch(self, hs):
+        """the prepared frames ``hs`` stacked into one host buffer per key (pinned on a CUDA dataset): rgbs (B, ncam, h, w, 3),
+        labels (B, ncam, h, w), tel (B, h_tel, w_tel, 3) uint8, bra (B,) int64."""
+        pin = self.device.type == "cuda"
+        st = {}
+        for key in ("rgbs", "labels", "tel"):
+            if key in hs[0]:
+                shapes = {h[key].shape for h in hs}
+                if len(shapes) != 1:
+                    raise LavbError(f"CameraDataset: the {key} images of a batch differ in size: {sorted(shapes)}")
+                buf = torch.empty((len(hs),) + hs[0][key].shape, dtype=torch.uint8, pin_memory=pin)
+                dst = buf.numpy()
+                for b, h in enumerate(hs):
+                    dst[b] = h[key]
+                st[key] = buf
+        if self.brake:
+            bra = torch.tensor([h["bra"] for h in hs], dtype=torch.int64)
+            st["bra"] = bra.pin_memory() if pin else bra
+        return st
+
+    def launch_batch(self, st):
+        """the staged host buffers copied to the device, one copy each."""
+        return {k: v.to(self.device, non_blocking=True) for k, v in st.items()}
+
+
+class CameraBatchLoader(TemporalBatchLoader):
+    """Batches of a CameraDataset in frame order, unaugmented, the last batch possibly short: TemporalBatchLoader's ordered mode,
+    with the record reads and image decodes of a batch on ``num_workers`` threads one batch ahead of the GPU.  A batch is the
+    dict of CameraDataset.launch_batch; staged_batches also yields the host buffers."""
+
+    def __init__(self, dataset, batch_size, num_workers=8):
+        super().__init__(dataset, batch_size, drop_last=False, num_workers=num_workers, ordered=True)
+
+    def _host(self, idxs, draws, gen, pool):
+        return self.ds.stage_batch(self._prepare(pool, idxs, draws))
+
+
 def get_data_loader(data_type, args):
     """lav.utils.datasets.get_data_loader for 'temporal_lidar_painted' and 'temporal_bev' (args: config_path, seed, batch_size;
     optional rank, world_size, device, num_workers).  The other dataset types are not provided."""

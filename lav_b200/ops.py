@@ -454,6 +454,46 @@ def paint_deconv_batched(points, feat, n_classes, deconv, cams, copy_cols, out, 
     return out
 
 
+def sem_class_table(seg_channels):
+    """filter_sem(sem, seg_channels) (lav/utils/__init__.py:3-8) as a lookup table: uint8 (256,) = the class of each CARLA tag, in
+    that loop's order: an unlisted tag is class 0 and a later duplicate of a tag wins."""
+    lut = np.zeros(256, np.uint8)
+    for i, tag in enumerate(seg_channels):
+        lut[int(tag)] = i + 1
+    return lut
+
+
+def seg_confusion(feat, table, labels, lut, n_classes, out=None):
+    """Per-image confusion counts of ERFNet's class map in one launch (see lavb_seg_confusion in include/lav_b200.h).  feat NHWC
+    (N, H/2, W/2, 16) fp32 / h16 = the input of output_conv (forward_features_nhwc); table = pack_deconv2x2 of output_conv; labels
+    (N, H, W) uint8 = the recorded tags; lut = sem_class_table(seg_channels) on the host.  -> int32 (N, C*C + 1) = confusion[gt][pred]
+    flattened, then the invalid (NaN-logit) pixels (written into ``out`` when given)."""
+    _need_cuda(feat, table, labels)
+    if feat.dtype not in (torch.float32, h16()) or feat.dim() != 4 or feat.shape[3] != 16 or not feat.is_contiguous():
+        raise capi.LavbError(f"seg_confusion: feat must be a contiguous (N, H/2, W/2, 16) fp32 or {h16()} tensor, got {feat.dtype} "
+                             f"{tuple(feat.shape)}")
+    n, hh, wh, _ = feat.shape
+    if labels.dtype != torch.uint8 or tuple(labels.shape) != (n, 2 * hh, 2 * wh) or not labels.is_contiguous():
+        raise capi.LavbError(f"seg_confusion: labels must be a contiguous ({n}, {2 * hh}, {2 * wh}) uint8 tensor, got {labels.dtype} "
+                             f"{tuple(labels.shape)}")
+    if table.dtype != torch.float32 or table.numel() != 520 or not table.is_contiguous():
+        raise capi.LavbError("seg_confusion: table must be the 520-float pack_deconv2x2 table")
+    lut = np.ascontiguousarray(lut)
+    if lut.dtype != np.uint8 or lut.shape != (256,):
+        raise capi.LavbError(f"seg_confusion: lut must be a host (256,) uint8 array, got {lut.dtype} {lut.shape}")
+    if len({feat.device, table.device, labels.device}) != 1:
+        raise capi.LavbError("seg_confusion: the inputs must be on one device")
+    c = int(n_classes)
+    if out is None:
+        out = torch.empty((n, c * c + 1), dtype=torch.int32, device=feat.device)
+    elif out.dtype != torch.int32 or tuple(out.shape) != (n, c * c + 1) or not out.is_contiguous() or out.device != feat.device:
+        raise capi.LavbError(f"seg_confusion: out must be a contiguous ({n}, {c * c + 1}) int32 tensor on {feat.device}")
+    check(lib().lavb_seg_confusion(_ptr(feat), _DT[feat.dtype], _ptr(table), _ptr(labels), lut.ctypes.data_as(C.c_void_p), n, c,
+                                   2 * hh, 2 * wh, _ptr(out), _stream()), "lavb_seg_confusion")
+    _COUNT[0] += n > 0
+    return out
+
+
 STACK_JOB_DTYPE = np.dtype([("src", np.uint64), ("dst", np.uint64), ("n", np.int32), ("time_idx", np.int32), ("R", np.float32, 9),
                             ("dx", np.float32), ("dy", np.float32), ("pad", np.int32)])
 assert STACK_JOB_DTYPE.itemsize == 72

@@ -270,13 +270,46 @@ def _road_planes(rs, h=320, w=320):
     return planes
 
 
+TEL_H, TEL_W = 288, 480          # the telephoto camera before crop_tel_bottom (team_code_v2/lav_agent.py:53-55)
+
+
+def _blobs(rs, h, w, n, values, base):
+    """(h, w) uint8: ``base`` with ``n`` axis-aligned rectangles, each filled with one draw from ``values``."""
+    img = np.full((h, w), base, np.uint8)
+    for _ in range(n):
+        y0, x0 = rs.randint(0, h), rs.randint(0, w)
+        img[y0:y0 + rs.randint(4, h // 3), x0:x0 + rs.randint(4, w // 3)] = rs.choice(values)
+    return img
+
+
+def _camera_images(rs, n_cameras, jpeg):
+    """the camera keys of one frame: rgb_{c} (288 x 256 colour, PNG or ``jpeg``), sem_{c} (grayscale PNG of tags 0..22 on a
+    background of 0, so listed tags, unlisted tags and background all occur) for each of ``n_cameras``, and tel_rgb (288 x 480)."""
+    import cv2
+    enc = (lambda im: cv2.imencode(".jpg", im, [cv2.IMWRITE_JPEG_QUALITY, 90])[1].tobytes()) if jpeg else \
+        (lambda im: cv2.imencode(".png", im)[1].tobytes())
+
+    def colour(h, w):
+        low = rs.randint(0, 256, (h // 16 + 1, w // 16 + 1, 3)).astype(np.uint8)
+        return cv2.resize(low, (w, h), interpolation=cv2.INTER_LINEAR)
+    keys = {}
+    for c in range(n_cameras):
+        keys[f"rgb_{c}"] = enc(colour(RGB_H, RGB_W))
+        keys[f"sem_{c}"] = encode_png(_blobs(rs, RGB_H, RGB_W, 12, np.arange(23), 0))
+    keys["tel_rgb"] = enc(colour(TEL_H, TEL_W))
+    return keys
+
+
 def record_trajectories(root, n_traj=2, n_frames=30, seed=SEED, n_points=600, n_actors=12, seg_channels=4,
-                        towns=("Town01", "Town03", "Town02", "Town04", "Town05", "Town06")):
+                        towns=("Town01", "Town03", "Town02", "Town04", "Town05", "Town06"), images=False, n_cameras=3):
     """Write ``n_traj`` seeded synthetic trajectories of ``n_frames`` frames under ``root`` in the reference's record layout
     (basic_dataset.py:52-53,82-157, temporal_lidar_painted_dataset.py:29-30), through data_paint.DirEnv (one file per key):
       len, town; lidar_%05d (n,4) f32; lidar_sem_%05d (n,C) f32; map_{0..11}_%05d grayscale PNG (0/255);
       id (int32, ego first), loc (f32 (n,2) metres), ori (f32 degrees), bbox (f32 (n,2)), type (uint8), cmd / bra (uint8),
       nxp (f32 (2,)) per frame.
+    With ``images`` every frame also holds the camera keys of the image datasets (seg_dataset.py, bra_dataset.py):
+      rgb_{c}_%05d for c < n_cameras (PNG; JPEG in trajectory 1), sem_{c}_%05d (grayscale PNG of CARLA tags), tel_rgb_%05d
+      (288 x 480, encoded as the rgb keys).  They come from a RandomState of their own, so every other key keeps its bytes.
     The ego drives a smooth arc; the other actors move smoothly, some leave before the last frame, some are out of range.
     Returns the trajectory directories."""
     import os
@@ -299,7 +332,11 @@ def record_trajectories(root, n_traj=2, n_frames=30, seed=SEED, n_points=600, n_
         a_ori = rs.uniform(-180, 180, n_actors)
         a_box = np.where(a_typ[:, None] == 1, rs.uniform(1.8, 2.6, (n_actors, 2)), rs.uniform(0.3, 0.5, (n_actors, 2)))
         a_last = np.where(rs.rand(n_actors) < 0.3, rs.randint(n_frames // 3, n_frames, n_actors), n_frames)   # leaves after a_last
+        rs_img = np.random.RandomState(int.from_bytes(hashlib.sha256(f"{seed}:img{k}".encode()).digest()[:4], "little"))
         for f in range(n_frames):
+            if images:
+                for key, data in _camera_images(rs_img, n_cameras, jpeg=k == 1).items():
+                    env.put(f"{key}_{f:05d}", data)
             yaw = yaw0 + yaw_rate * f
             heading = np.deg2rad(yaw0 + yaw_rate * f / 2)
             ego_loc = start + speed * f * np.array([np.cos(heading), np.sin(heading)])
