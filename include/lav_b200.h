@@ -311,6 +311,72 @@ int lavb_agent_control(const float* d_plan, const float* d_cast, int b, int t, i
                        const float* d_other_cmds, int k, const int* h_offsets, const float* d_pred_bra, const float* d_speed,
                        const int* h_cmd, const lavb_control_config* h_config, void* d_state, float* d_control, int* d_flags,
                        void* stream);
+/* The same with the commands on the DEVICE (d_cmd (b,) int32, e.g. lavb_agent_nav_front's output), in the same launch shape.  An
+ * agent whose command lies outside 0..c-1 gets NaN controls and flags LAVB_CTL_BAD_CMD, and its state is left as it was. */
+#define LAVB_CTL_BAD_CMD 64
+int lavb_agent_control_dcmd(const float* d_plan, const float* d_cast, int b, int t, int c, const float* d_other_locs,
+                            const float* d_other_cmds, int k, const int* h_offsets, const float* d_pred_bra, const float* d_speed,
+                            const int* d_cmd, const lavb_control_config* h_config, void* d_state, float* d_control, int* d_flags,
+                            void* stream);
+
+/* ---------------------------------------------------------------- agent localisation and route following
+ * replaces: the head of LAVAgent.run_step (team_code_v2/lav_agent_fast.py:215-226, 280-308, 314) and its EKF step (:338), with
+ *           EKF (team_code_v2/ekf.py), Waypointer (waypointer.py, pop_lane_change=True, pop_turning=False, default thresholds) and
+ *           RoutePlanner (planner.py, default thresholds), for b agents, one thread per agent.
+ * Routes: d_nodes (n_nodes, 2) fp64 holds every route's nodes as latlon_to_xy with the route's own scale cos(cos_0), cos_0 the mean
+ *   of the route latitudes in radians; d_node_cmd (n_nodes,) int32 their RoadOption values (-1..6).  d_route (b, 2) int32 =
+ *   (start, count) of agent i's route; an entry with start < 0, count < 1 or start + count > n_nodes is no route: the agent gets
+ *   flags LAVB_NAV_NO_ROUTE, cmds 3, NaN nxps and poses, and its state is left as it was.  The route table is device data, so
+ *   this check runs per agent in the kernel, not before the launch, and writes that agent's outputs; the node command values are
+ *   not checked here (lav_b200.navigation.set_routes checks them on the host).
+ * State: d_state holds b lavb_nav_state records (lavb_agent_nav_state_bytes() each, 8-byte aligned).  A new route is a record of
+ *   zeros with route_scale = cos(cos_0), ekf_scale = cos(1) (the agent's EKF is built with cos0 = 1) and lane_changed = -1.
+ * Front, per tick, before the planner (lavb_agent_nav_front): gnss (b, 2) fp64 = lat, lon; compass (b,) fp64 = imu[-1], raw.
+ *   compass' = 0 when NaN; on the route's first frame EKF.init(lat, lon, compass' - pi/2); poses (b, 3) fp64 = the EKF state
+ *   (x, y, theta).  The first frame stops there (flags LAVB_NAV_FIRST_FRAME, cmds 3, nxps 0), as run_step returns early.  On the
+ *   second frame the Waypointer (checkpoint = this frame's position, LANEFOLLOW) and the RoutePlanner are built; then every frame
+ *   runs Waypointer.tick and RoutePlanner.run_step in O(1), cmds = RoadOption value - 1 (VOID -> 3), the lane-change counter
+ *   and rule (a 4 / 5 held for more than 300 ticks becomes 3), and nxps (b, 2) fp32 = -(R(-compass + pi/2) @ (wx, wy)) with the
+ *   RAW compass, so a NaN compass gives NaN nxps.
+ * Update, per tick, after the controls (lavb_agent_nav_update): EKF.step(speed, steer, lat, lon, compass' - pi/2) of every agent
+ *   past its first frame; speed (b,) fp64 m/s, steer = d_control[3 i] (b, 3) fp32, lavb_agent_control's output.
+ * Arithmetic: fp64, correctly rounded, in numpy's order; cos, sin, tan and atan are CUDA's (within 2 ulp).  Every output of the
+ * b agents is written; a rejected call writes nothing. */
+#define LAVB_NAV_FIRST_FRAME 1   /* the route's first frame: pose only, no command, target or EKF step */
+#define LAVB_NAV_NO_ROUTE 2      /* d_route holds no route for the agent: nothing computed */
+#define LAVB_NAV_LANE_HELD 4     /* a lane change held past 300 ticks was replaced by 3 */
+
+typedef struct lavb_nav_state {
+  double ekf_x[3];           /* EKF.x: x, y, theta */
+  double ekf_p[3];           /* the diagonal of EKF.P (F = H = I, diagonal Q and R keep it diagonal) */
+  double wp_x, wp_y;         /* Waypointer.checkpoint */
+  double rp_x, rp_y;         /* RoutePlanner.checkpoint */
+  double route_scale;        /* cos(cos_0) of the route's Waypointer and RoutePlanner */
+  double ekf_scale;          /* cos(cos0) of the EKF, cos(1) */
+  int frames;                /* frames since the route was set (saturates at 2^30) */
+  int wp_idx, wp_cmd;        /* Waypointer.current_idx, the checkpoint's RoadOption value */
+  int rp_idx;                /* RoutePlanner.current_idx */
+  int lane_counter;          /* lane_change_counter */
+  int lane_changed;          /* lane_changed, -1 = None */
+  int pad[2];
+} lavb_nav_state;
+
+size_t lavb_agent_nav_state_bytes(void);
+int lavb_agent_nav_front(int b, const double* d_nodes, const int* d_node_cmd, int n_nodes, const int* d_route, const double* d_gnss,
+                         const double* d_compass, void* d_state, int* d_cmds, float* d_nxps, double* d_poses, int* d_flags,
+                         void* stream);
+int lavb_agent_nav_update(int b, const float* d_control, const double* d_speed, const double* d_gnss, const double* d_compass,
+                          void* d_state, void* stream);
+
+/* The pose fields (R, dx, dy) of lavb_stack_jobs' table, b agents x t sweeps (record (i, k) at d_jobs + (i * t + k) * 72), as
+ * StaticFramePipeline._fill_jobs computes them on the host.  d_ring_pose (b, keep, 3) fp64 holds each agent's pose (x, y, ori)
+ * per ring slot; when d_poses (b, 3) fp64 is given it is first written to slot tick % keep.  Job k reads slot
+ * (tick - k * gap) mod keep: R = [[cos d, sin d, 0], [-sin d, cos d, 0], [0, 0, 1]] with d = ori_k - ori_0, (dx, dy) =
+ * (dl.x cos ori_0 + dl.y sin ori_0, -dl.x sin ori_0 + dl.y cos ori_0) with dl = loc_k - loc_0, in fp64 rounded to fp32.  The
+ * other fields are not touched. */
+#define LAVB_STACK_JOB_BYTES 72
+int lavb_stack_job_poses(void* d_jobs, int b, int t, int gap, int keep, long long tick, double* d_ring_pose, const double* d_poses,
+                         void* stream);
 
 /* ---------------------------------------------------------------- PointPillars voxeliser + pillar encoder
  * replaces: PointPillarNet.forward (lav/models/point_pillar.py:92-116) incl. grid_locations :70-79,

@@ -204,9 +204,11 @@ class StaticFramePipeline(FramePipeline):
     COPY_STREAM = os.environ.get("LAVB_COPY_STREAM", "1") != "0"   # stage pinned host inputs on a copy stream (see begin())
 
     def __init__(self, seg_model, lidar_model, uniplanner, bra_model, batch, n_points, camera_x=1.5, camera_z=2.4,
-                 device=torch.device("cuda"), precision="f16", use_graphs=True, roof_filter=False):
+                 device=torch.device("cuda"), precision="f16", use_graphs=True, roof_filter=False, navigator=None):
         """roof_filter: the sweeps handed to step() are RAW sensor sweeps; the ego-roof drop of LAVAgent.preprocess
-        (lav_agent_fast.py:247) then runs on the device as the first kernel of G1 (order preserving, NaN-padded)."""
+        (lav_agent_fast.py:247) then runs on the device as the first kernel of G1 (order preserving, NaN-padded).
+        navigator: an AgentNavigator of the same B agents; begin(..., gnss=, compass=) then runs its front before G1 and feeds its
+        commands and targets to the planner and its poses to the sweep stack, all on the device."""
         super().__init__(seg_model, lidar_model, uniplanner, bra_model, camera_x, camera_z, device, precision)
         B, N, T = batch, n_points, NUM_FRAME_STACK + 1
         self.B, self.N, self.T, self.use_graphs = B, N, T, use_graphs
@@ -220,6 +222,14 @@ class StaticFramePipeline(FramePipeline):
         self.ring = torch.full((B, self.KEEP, N, 8), float("nan"), device=dev)
         self.ring_pose = np.zeros((B, self.KEEP, 3))                 # loc x, loc y, ori per slot
         self.ring_valid = np.zeros((B, self.KEEP), dtype=bool)
+        if navigator is not None and navigator.B != B:
+            raise ValueError(f"StaticFramePipeline: a navigator of {navigator.B} agents for {B}")
+        self.navigator = navigator
+        # with a navigator the poses the sweep stack reads live on the device (lavb_stack_job_poses); the host ring stays for the
+        # host-pose path.  Host ticks copy their pose into the device ring; the first host tick after navigator ticks copies the
+        # device ring back (one synchronising copy), so the two paths can alternate on one pipeline
+        self.ring_pose_dev = torch.zeros((B, self.KEEP, 3), dtype=torch.float64, device=dev) if navigator is not None else None
+        self._host_ring_stale = False
         self.stacked = torch.full((B, T * N, 8 + T), float("nan"), device=dev)
         self.jobs_host = torch.zeros(B * T * ops.STACK_JOB_DTYPE.itemsize, dtype=torch.uint8).pin_memory()
         self.jobs_dev = torch.zeros_like(self.jobs_host, device=dev)
@@ -239,12 +249,15 @@ class StaticFramePipeline(FramePipeline):
         self._cams = np.stack([c.packed() for c in self.infer_model.coord_converters])
 
     # ---- host-side state ------------------------------------------------------------------------------------
-    def _fill_jobs(self, poses):
-        """rewrite the (agent, sweep) job table for this tick — vectorised numpy, then one small H2D copy."""
+    def _fill_jobs(self, poses, device_poses=False):
+        """rewrite the (agent, sweep) job table for this tick — vectorised numpy, then one small H2D copy.  With device_poses the
+        pose fields (R, dx, dy) are left for lavb_stack_job_poses to write after the copy."""
         B, T, N, KEEP = self.B, self.T, self.N, self.KEEP
         jobs = self.jobs_host.numpy().view(ops.STACK_JOB_DTYPE).reshape(B, T)
         s0 = self.tick % KEEP
-        if poses is not None:
+        if device_poses:
+            pass
+        elif poses is not None:
             self.ring_pose[:, s0, :2] = np.asarray([p[0] for p in poses], dtype=np.float64)
             self.ring_pose[:, s0, 2] = np.asarray([p[1] for p in poses], dtype=np.float64)
         else:
@@ -252,17 +265,18 @@ class StaticFramePipeline(FramePipeline):
         self.ring_valid[:, s0] = True
         ticks = self.tick - np.arange(T) * GAP                                   # (T,)
         slots = ticks % KEEP
-        pose = self.ring_pose[:, slots]                                           # (B,T,3)
         valid = (ticks >= 0)[None] & self.ring_valid[:, slots]
-        loc0, ori0 = pose[:, :1, :2], pose[:, :1, 2]
-        d = pose[..., 2] - ori0                                                   # (B,T)
-        c0, si0 = np.cos(ori0), np.sin(ori0)
-        dl = pose[..., :2] - loc0
-        R = np.zeros((B, T, 9), dtype=np.float32)
-        R[..., 0], R[..., 1], R[..., 3], R[..., 4], R[..., 8] = np.cos(d), np.sin(d), -np.sin(d), np.cos(d), 1.0
-        jobs["R"] = R
-        jobs["dx"] = dl[..., 0] * c0 + dl[..., 1] * si0                           # dloc @ [[c,-s],[s,c]]
-        jobs["dy"] = -dl[..., 0] * si0 + dl[..., 1] * c0
+        if not device_poses:
+            pose = self.ring_pose[:, slots]                                       # (B,T,3)
+            loc0, ori0 = pose[:, :1, :2], pose[:, :1, 2]
+            d = pose[..., 2] - ori0                                               # (B,T)
+            c0, si0 = np.cos(ori0), np.sin(ori0)
+            dl = pose[..., :2] - loc0
+            R = np.zeros((B, T, 9), dtype=np.float32)
+            R[..., 0], R[..., 1], R[..., 3], R[..., 4], R[..., 8] = np.cos(d), np.sin(d), -np.sin(d), np.cos(d), 1.0
+            jobs["R"] = R
+            jobs["dx"] = dl[..., 0] * c0 + dl[..., 1] * si0                       # dloc @ [[c,-s],[s,c]]
+            jobs["dy"] = -dl[..., 0] * si0 + dl[..., 1] * c0
         jobs["n"] = np.where(valid, N, 0)
         jobs["time_idx"] = np.arange(T)[None]
         row_bytes = 4 * (8 + T)
@@ -282,6 +296,8 @@ class StaticFramePipeline(FramePipeline):
             self.ring[b, slot].fill_(float("nan"))
             self.ring[b, slot, :s.shape[0]] = s
             self.ring_pose[b, slot] = (loc[0], loc[1], ori)
+            if self.ring_pose_dev is not None:
+                self.ring_pose_dev[b, slot] = torch.from_numpy(self.ring_pose[b, slot].copy())
             self.ring_valid[b, slot] = True
 
     # ---- device work ----------------------------------------------------------------------------------------
@@ -337,23 +353,37 @@ class StaticFramePipeline(FramePipeline):
         return g, out
 
     @torch.no_grad()
-    def step(self, rgbs_u8, tel_u8, lidars, nxps, cmds, poses=None, fixed_dets=None):
+    def step(self, rgbs_u8, tel_u8, lidars, nxps=None, cmds=None, poses=None, fixed_dets=None, gnss=None, compass=None):
         """rgbs_u8 (B,3,288,256,3) u8 / tel_u8 (B,192,480,3) u8 on host (pinned) or device; lidars: (B,n,4) tensor or list of
-        (n_b,4) (n_b <= N); nxps (B,2); cmds (B,) ints.  Returns the dict of FramePipeline.step.
+        (n_b,4) (n_b <= N); nxps (B,2); cmds (B,) ints; or, with a navigator, gnss and compass instead (see begin).  Returns the
+        dict of FramePipeline.step.
         = begin() + finish(); call them separately to overlap the host-side decode of one pipeline with the GPU work of
         another (each StaticFramePipeline owns a stream)."""
-        self.begin(rgbs_u8, tel_u8, lidars, nxps, cmds, poses)
+        self.begin(rgbs_u8, tel_u8, lidars, nxps, cmds, poses, gnss=gnss, compass=compass)
         return self.finish(fixed_dets)
 
     @torch.no_grad()
-    def begin(self, rgbs_u8, tel_u8, lidars, nxps, cmds, poses=None):
-        """stage inputs and launch G1 (asynchronous)."""
+    def begin(self, rgbs_u8, tel_u8, lidars, nxps=None, cmds=None, poses=None, gnss=None, compass=None):
+        """stage inputs and launch G1 (asynchronous).  With gnss ((B, >=2) lat, lon) and compass ((B,) raw imu[-1]) the navigator's
+        front runs first, on the device: its cmds and nxps feed the planner, its poses the sweep stack, and nxps / cmds / poses
+        must be None.  Returns the front's dict (AgentNavigator.front) then, else None."""
+        nav = None
+        if gnss is not None or compass is not None:
+            if self.navigator is None or gnss is None or compass is None:
+                raise ValueError("StaticFramePipeline.begin: gnss and compass need a navigator and each other")
+            if nxps is not None or cmds is not None or poses is not None:
+                raise ValueError("StaticFramePipeline.begin: nxps, cmds and poses come from the navigator when gnss is given")
+        elif nxps is None or cmds is None:
+            raise ValueError("StaticFramePipeline.begin: nxps and cmds, or gnss and compass, are needed")
         rgbs_u8, tel_u8, lidars, used = self._stage_host(rgbs_u8, tel_u8, lidars)
         with torch.cuda.stream(self.stream), self._math_mode():
-            self._begin(rgbs_u8, tel_u8, lidars, nxps, cmds, poses)
+            if gnss is not None:
+                nav = self.navigator.front(gnss, compass, out=dict(nxps=self.nxps))
+            self._begin(rgbs_u8, tel_u8, lidars, nxps, cmds, poses, nav)
             if used is not None:
                 self._stage_free[used] = torch.cuda.Event()
                 self._stage_free[used].record(self.stream)
+        return nav
 
     def _stage_host(self, rgbs_u8, tel_u8, lidars):
         """pinned host tensors -> the staging set of this tick on the copy stream; returns device tensors (or the arguments
@@ -386,7 +416,7 @@ class StaticFramePipeline(FramePipeline):
         torch.cuda.current_stream().wait_stream(self.stream)
         return out
 
-    def _begin(self, rgbs_u8, tel_u8, lidars, nxps, cmds, poses):
+    def _begin(self, rgbs_u8, tel_u8, lidars, nxps, cmds, poses, nav=None):
         B, N = self.B, self.N
         self.rgbs.copy_(rgbs_u8, non_blocking=True)
         if tel_u8 is not None:
@@ -398,9 +428,21 @@ class StaticFramePipeline(FramePipeline):
                 self.lidar_raw[b, :l.shape[0]].copy_(l, non_blocking=True)
                 if l.shape[0] < N:
                     self.lidar_raw[b, l.shape[0]:].fill_(float("nan"))
-        self.nxps.copy_(torch.as_tensor(nxps, dtype=torch.float32), non_blocking=True)
-        self.cmds.copy_(torch.as_tensor(cmds, dtype=torch.long), non_blocking=True)
-        self._fill_jobs(poses)
+        if nav is None:
+            self.nxps.copy_(torch.as_tensor(nxps, dtype=torch.float32), non_blocking=True)
+            self.cmds.copy_(torch.as_tensor(cmds, dtype=torch.long), non_blocking=True)
+            if self._host_ring_stale:
+                self.ring_pose[:] = self.ring_pose_dev.cpu().numpy()
+                self._host_ring_stale = False
+            self._fill_jobs(poses)
+            if self.ring_pose_dev is not None:       # keep the device ring whole for later navigator ticks
+                s0 = self.tick % self.KEEP
+                self.ring_pose_dev[:, s0].copy_(torch.from_numpy(self.ring_pose[:, s0].copy()), non_blocking=True)
+        else:                                        # the front wrote self.nxps; its poses go to the ring and the job table
+            self.cmds.copy_(nav["cmds"])
+            self._fill_jobs(None, device_poses=True)
+            ops.stack_job_poses(self.jobs_dev, self.B, self.T, GAP, self.KEEP, self.tick, self.ring_pose_dev, nav["poses"])
+            self._host_ring_stale = True
         if self._g1 is None:
             self._g1, self._o1 = self._capture(self._g1_body)
         if self._g1 is not None:

@@ -94,6 +94,15 @@ _SIGS = {
     "lavb_agent_control": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p,
                                      C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(ControlConfig), C.c_void_p, C.c_void_p,
                                      C.c_void_p, C.c_void_p]),
+    "lavb_agent_control_dcmd": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_int,
+                                          C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(ControlConfig), C.c_void_p,
+                                          C.c_void_p, C.c_void_p, C.c_void_p]),
+    "lavb_agent_nav_state_bytes": (C.c_size_t, []),
+    "lavb_agent_nav_front": (C.c_int, [C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                       C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "lavb_agent_nav_update": (C.c_int, [C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "lavb_stack_job_poses": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_longlong, C.c_void_p, C.c_void_p,
+                                       C.c_void_p]),
     "lavb_roof_filter": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_longlong, C.c_void_p, C.c_longlong, C.c_void_p, C.c_int,
                                    C.c_void_p]),
     "lavb_stack_sweep": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_float, C.c_float, C.c_int, C.c_int, C.c_int,

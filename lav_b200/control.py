@@ -20,7 +20,7 @@ from . import capi, ops
 CONFIG_KEYS = ("aim_point", "speed_ratio", "turn_KP", "turn_KI", "turn_KD", "turn_n", "speed_KP", "speed_KI", "speed_KD",
                "speed_n", "brake_speed", "clip_delta", "max_throttle", "max_speed", "cmd_thresh", "pixels_per_meter")
 # LAVB_CTL_* of include/lav_b200.h
-FLAG_PLAN_INVALID, FLAG_PID_BRAKE, FLAG_BRAKE_MODEL, FLAG_COLLIDE, FLAG_SPEED_CAP, FLAG_CREEP = 1, 2, 4, 8, 16, 32
+FLAG_PLAN_INVALID, FLAG_PID_BRAKE, FLAG_BRAKE_MODEL, FLAG_COLLIDE, FLAG_SPEED_CAP, FLAG_CREEP, FLAG_BAD_CMD = 1, 2, 4, 8, 16, 32, 64
 MAX_CMDS = 8
 
 
@@ -69,7 +69,8 @@ class AgentController:
     def step(self, out, speeds, cmds):
         """One tick.  out: the dict FramePipeline.step / StaticFramePipeline.finish returns (ego_plan_locs, ego_cast_locs,
         other_cast_locs, other_cast_cmds, pred_bra; read, never changed); speeds (B,) m/s, host values or a device tensor; cmds
-        (B,) the commands the planner was given, host ints.  -> dict(control (B,3) fp32 = steer, throttle, brake; flags (B,)
+        (B,) the commands the planner was given, host ints or an int32 device tensor (AgentNavigator.front's "cmds"; an agent
+        whose command is outside the planner's branches gets NaN controls and FLAG_BAD_CMD).  -> dict(control (B,3) fp32 = steer, throttle, brake; flags (B,)
         int32), device tensors on the current stream."""
         B, dev = self.B, self.device
         ocl, occ = list(out["other_cast_locs"]), list(out["other_cast_cmds"])
@@ -80,7 +81,10 @@ class AgentController:
         locs, scores = torch.cat(ocl), torch.cat(occ)                  # the rows of all agents, concatenated on the device
         if locs.shape[1] != self.num_cmds:
             raise capi.LavbError(f"AgentController.step: {locs.shape[1]} forecast branches for {self.num_cmds} commands")
-        cmds = np.asarray(cmds.numpy() if torch.is_tensor(cmds) else cmds).astype(np.int32).reshape(-1)
+        if torch.is_tensor(cmds) and cmds.is_cuda:                      # AgentNavigator.front's commands, read on the device
+            cmds = cmds.to(torch.int32).reshape(-1).contiguous()
+        else:
+            cmds = np.asarray(cmds.numpy() if torch.is_tensor(cmds) else cmds).astype(np.int32).reshape(-1)
         if torch.is_tensor(speeds) and speeds.is_cuda:
             speed = speeds.to(torch.float32).reshape(B).contiguous()
         else:

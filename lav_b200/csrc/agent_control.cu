@@ -20,6 +20,7 @@ struct CtlArgs {
   const float2* plan; const float2* cast; const float2* locs; const float* scores; const float* pred_bra; const float* speed;
   unsigned char* state; long long state_bytes;
   float* control; int* flags;
+  const int* cmd;                        // the device commands of lavb_agent_control_dcmd; null when they travel in the Chunk
   int t, c;
 };
 
@@ -76,7 +77,15 @@ __global__ void __launch_bounds__(kWarps * 32) agent_control_kernel(const CtlArg
                                                                      const __grid_constant__ Chunk ch, int b0, int nb) {
   const int lane = threadIdx.x & 31, w = blockIdx.x * kWarps + (threadIdx.x >> 5);
   if (w >= nb) return;                                            // whole warps leave together
-  const int i = b0 + w, t = p.t, c = p.c, cmd = ch.cmd[w];
+  const int i = b0 + w, t = p.t, c = p.c, cmd = p.cmd ? __ldg(p.cmd + i) : ch.cmd[w];
+  if (cmd < 0 || cmd >= c) {                                      // only a device command can get here
+    if (lane == 0) {
+      const float nan = __int_as_float(0x7fc00000);
+      p.control[3LL * i] = nan; p.control[3LL * i + 1] = nan; p.control[3LL * i + 2] = nan;
+      p.flags[i] = LAVB_CTL_BAD_CMD;
+    }
+    return;
+  }
   const float2* plan = ((cmd == 4 || cmd == 5) ? p.cast : p.plan) + (long long)i * t;   // :325-326
   const float2 q = lane < t ? __ldg(plan + lane) : make_float2(0.f, 0.f);
   const bool valid = !__any_sync(0xffffffffu, isnan(q.x) || isnan(q.y));                 // :328
@@ -160,10 +169,10 @@ extern "C" size_t lavb_agent_control_state_bytes(int turn_n, int speed_n) {
   return (size_t)kHeader + sizeof(double) * (size_t)(turn_n + speed_n);
 }
 
-extern "C" int lavb_agent_control(const float* d_plan, const float* d_cast, int b, int t, int c, const float* d_other_locs,
-                                  const float* d_other_cmds, int k, const int* h_offsets, const float* d_pred_bra,
-                                  const float* d_speed, const int* h_cmd, const lavb_control_config* h_config, void* d_state,
-                                  float* d_control, int* d_flags, void* stream) {
+static int agent_control(const float* d_plan, const float* d_cast, int b, int t, int c, const float* d_other_locs,
+                         const float* d_other_cmds, int k, const int* h_offsets, const float* d_pred_bra, const float* d_speed,
+                         const int* h_cmd, const int* d_cmd, const lavb_control_config* h_config, void* d_state, float* d_control,
+                         int* d_flags, void* stream) {
   LAVB_CHECK_ARG(b >= 0 && k >= 0, "agent_control: bad sizes (b %d, k %d)", b, k);
   LAVB_CHECK_ARG(t >= 2 && t <= kMaxSteps, "agent_control: %d steps outside 2..%d", t, kMaxSteps);
   LAVB_CHECK_ARG(c >= 1 && c <= LAVB_CTL_MAX_CMDS, "agent_control: %d branches outside 1..%d", c, LAVB_CTL_MAX_CMDS);
@@ -181,10 +190,13 @@ extern "C" int lavb_agent_control(const float* d_plan, const float* d_cast, int 
   for (int i = 0; i < b; ++i)
     LAVB_CHECK_ARG(h_offsets[i] <= h_offsets[i + 1], "agent_control: row offsets of agent %d are not monotone (%d -> %d)", i,
                    h_offsets[i], h_offsets[i + 1]);
-  LAVB_CHECK_ARG(h_cmd || b == 0, "agent_control: missing host commands");
-  for (int i = 0; i < b; ++i)
-    LAVB_CHECK_ARG(h_cmd[i] >= 0 && h_cmd[i] < c, "agent_control: command %d of agent %d outside 0..%d", h_cmd[i], i, c - 1);
+  if (!d_cmd) {
+    LAVB_CHECK_ARG(h_cmd || b == 0, "agent_control: missing host commands");
+    for (int i = 0; i < b; ++i)
+      LAVB_CHECK_ARG(h_cmd[i] >= 0 && h_cmd[i] < c, "agent_control: command %d of agent %d outside 0..%d", h_cmd[i], i, c - 1);
+  }
   if (b == 0) return 0;
+  LAVB_CHECK_ARG((uintptr_t)d_cmd % 4 == 0, "agent_control: device commands must be 4-byte aligned");
   LAVB_CHECK_ARG(d_plan && d_cast && d_pred_bra && d_speed && d_state && d_control && d_flags &&
                  ((d_other_locs && d_other_cmds) || h_offsets[b] == h_offsets[0]), "agent_control: null pointer");
   LAVB_CHECK_ARG((uintptr_t)d_plan % 8 == 0 && (uintptr_t)d_cast % 8 == 0 && (uintptr_t)d_other_locs % 8 == 0 &&
@@ -198,14 +210,32 @@ extern "C" int lavb_agent_control(const float* d_plan, const float* d_cast, int 
   a.state = static_cast<unsigned char*>(d_state); a.state_bytes = (long long)lavb_agent_control_state_bytes(cfg.turn_n, cfg.speed_n);
   a.control = d_control; a.flags = d_flags;
   a.t = t; a.c = c;
+  a.cmd = d_cmd;
   cudaStream_t st = (cudaStream_t)stream;
   for (int b0 = 0; b0 < b; b0 += kChunk) {
     const int nb = b - b0 < kChunk ? b - b0 : kChunk;
     Chunk ch;
     for (int i = 0; i <= nb; ++i) ch.rows[i] = h_offsets[b0 + i];
-    for (int i = 0; i < nb; ++i) ch.cmd[i] = (signed char)h_cmd[b0 + i];
+    for (int i = 0; i < nb && !d_cmd; ++i) ch.cmd[i] = (signed char)h_cmd[b0 + i];
     agent_control_kernel<<<(nb + kWarps - 1) / kWarps, kWarps * 32, 0, st>>>(a, cfg, ch, b0, nb);
     LAVB_LAUNCH_OK();
   }
   return 0;
+}
+
+extern "C" int lavb_agent_control(const float* d_plan, const float* d_cast, int b, int t, int c, const float* d_other_locs,
+                                  const float* d_other_cmds, int k, const int* h_offsets, const float* d_pred_bra,
+                                  const float* d_speed, const int* h_cmd, const lavb_control_config* h_config, void* d_state,
+                                  float* d_control, int* d_flags, void* stream) {
+  return agent_control(d_plan, d_cast, b, t, c, d_other_locs, d_other_cmds, k, h_offsets, d_pred_bra, d_speed, h_cmd, nullptr,
+                       h_config, d_state, d_control, d_flags, stream);
+}
+
+extern "C" int lavb_agent_control_dcmd(const float* d_plan, const float* d_cast, int b, int t, int c, const float* d_other_locs,
+                                       const float* d_other_cmds, int k, const int* h_offsets, const float* d_pred_bra,
+                                       const float* d_speed, const int* d_cmd, const lavb_control_config* h_config, void* d_state,
+                                       float* d_control, int* d_flags, void* stream) {
+  LAVB_CHECK_ARG(d_cmd || b == 0, "agent_control: missing device commands");
+  return agent_control(d_plan, d_cast, b, t, c, d_other_locs, d_other_cmds, k, h_offsets, d_pred_bra, d_speed, nullptr, d_cmd,
+                       h_config, d_state, d_control, d_flags, stream);
 }

@@ -928,7 +928,8 @@ def agent_control(plan, cast, other_locs, other_cmds, offsets, pred_bra, speed, 
     """The agent's controls for B agents in one launch (see lavb_agent_control in include/lav_b200.h): plan / cast (B,T,2) fp32 =
     ego plan and ego cast under the command; other_locs (K,C,T,2) / other_cmds (K,C) fp32 = the forecast rows of all agents,
     agent i owning rows [offsets[i], offsets[i+1]) (offsets (B+1,) int32 on the HOST); pred_bra, speed (B,) fp32; cmds (B,)
-    int32 on the HOST; config a capi.ControlConfig; state the agents' controller state, a contiguous uint8 device tensor of
+    int32 on the HOST, or a (B,) int32 CUDA tensor (lavb_agent_control_dcmd: an agent whose command is outside 0..C-1 gets NaN
+    controls and LAVB_CTL_BAD_CMD); config a capi.ControlConfig; state the agents' controller state, a contiguous uint8 device tensor of
     B * agent_control_state_bytes(config.turn_n, config.speed_n) bytes, updated in place.
     -> (control (B,3) fp32 = steer, throttle, brake; flags (B,) int32 of LAVB_CTL_* bits), written into ``control`` / ``flags``
     when given."""
@@ -952,9 +953,15 @@ def agent_control(plan, cast, other_locs, other_cmds, offsets, pred_bra, speed, 
     offsets = np.ascontiguousarray(offsets.numpy() if torch.is_tensor(offsets) else offsets)
     if offsets.dtype != np.int32 or offsets.shape != (b + 1,):
         raise capi.LavbError(f"agent_control: offsets must be a host ({b + 1},) int32 array, got {offsets.dtype} {offsets.shape}")
-    cmds = np.ascontiguousarray(cmds.numpy() if torch.is_tensor(cmds) else cmds)
-    if cmds.dtype != np.int32 or cmds.shape != (b,):
-        raise capi.LavbError(f"agent_control: cmds must be a host ({b},) int32 array, got {cmds.dtype} {cmds.shape}")
+    dcmd = torch.is_tensor(cmds) and cmds.is_cuda
+    if dcmd:
+        if cmds.dtype != torch.int32 or tuple(cmds.shape) != (b,) or not cmds.is_contiguous() or cmds.device != plan.device:
+            raise capi.LavbError(f"agent_control: device cmds must be a contiguous ({b},) int32 tensor on {plan.device}, got "
+                                 f"{cmds.dtype} {tuple(cmds.shape)} on {cmds.device}")
+    else:
+        cmds = np.ascontiguousarray(cmds.numpy() if torch.is_tensor(cmds) else cmds)
+        if cmds.dtype != np.int32 or cmds.shape != (b,):
+            raise capi.LavbError(f"agent_control: cmds must be a host ({b},) int32 array, got {cmds.dtype} {cmds.shape}")
     if not isinstance(config, capi.ControlConfig):
         raise capi.LavbError("agent_control: config must be a capi.ControlConfig")
     nbytes = b * agent_control_state_bytes(config.turn_n, config.speed_n)
@@ -972,11 +979,111 @@ def agent_control(plan, cast, other_locs, other_cmds, offsets, pred_bra, speed, 
     elif flags.dtype != torch.int32 or tuple(flags.shape) != (b,) or not flags.is_contiguous() or flags.device != dev:
         raise capi.LavbError(f"agent_control: flags must be a contiguous ({b},) int32 tensor on {dev}")
     ip = lambda a: a.ctypes.data_as(C.c_void_p)
-    check(lib().lavb_agent_control(_ptr(plan), _ptr(cast), b, t, c, _ptr(other_locs), _ptr(other_cmds), k, ip(offsets),
-                                   _ptr(pred_bra), _ptr(speed), ip(cmds), C.byref(config), _ptr(state), _ptr(control),
-                                   _ptr(flags), _stream()), "lavb_agent_control")
+    if dcmd:
+        check(lib().lavb_agent_control_dcmd(_ptr(plan), _ptr(cast), b, t, c, _ptr(other_locs), _ptr(other_cmds), k, ip(offsets),
+                                            _ptr(pred_bra), _ptr(speed), _ptr(cmds), C.byref(config), _ptr(state), _ptr(control),
+                                            _ptr(flags), _stream()), "lavb_agent_control_dcmd")
+    else:
+        check(lib().lavb_agent_control(_ptr(plan), _ptr(cast), b, t, c, _ptr(other_locs), _ptr(other_cmds), k, ip(offsets),
+                                       _ptr(pred_bra), _ptr(speed), ip(cmds), C.byref(config), _ptr(state), _ptr(control),
+                                       _ptr(flags), _stream()), "lavb_agent_control")
     _COUNT[0] += -(-b // 512)
     return control, flags
+
+
+NAV_STATE_DTYPE = np.dtype([("ekf_x", np.float64, (3,)), ("ekf_p", np.float64, (3,)), ("wp_x", np.float64), ("wp_y", np.float64),
+                            ("rp_x", np.float64), ("rp_y", np.float64), ("route_scale", np.float64), ("ekf_scale", np.float64),
+                            ("frames", np.int32), ("wp_idx", np.int32), ("wp_cmd", np.int32), ("rp_idx", np.int32),
+                            ("lane_counter", np.int32), ("lane_changed", np.int32), ("pad", np.int32, (2,))])
+assert NAV_STATE_DTYPE.itemsize == 128         # lavb_nav_state of include/lav_b200.h
+
+
+def agent_nav_state_bytes():
+    """bytes of one agent's lavb_nav_state record (lavb_agent_nav_state_bytes)."""
+    n = int(lib().lavb_agent_nav_state_bytes())
+    if n != NAV_STATE_DTYPE.itemsize:
+        raise capi.LavbError(f"agent_nav: the library's state record has {n} bytes, NAV_STATE_DTYPE {NAV_STATE_DTYPE.itemsize}")
+    return n
+
+
+def _f64_rows(x, b, cols, what):
+    shape = (b, cols) if cols else (b,)
+    if x.dtype != torch.float64 or tuple(x.shape) != shape or not x.is_contiguous():
+        raise capi.LavbError(f"{what} must be a contiguous {shape} fp64 tensor, got {x.dtype} {tuple(x.shape)}")
+
+
+def agent_nav_front(nodes, node_cmd, route, gnss, compass, state, cmds=None, nxps=None, poses=None, flags=None):
+    """The front of B agents' tick in one launch (lavb_agent_nav_front in include/lav_b200.h): nodes (M, 2) fp64 and node_cmd (M,)
+    int32 = every route's nodes; route (B, 2) int32 = (start, count) per agent; gnss (B, 2) fp64 = lat, lon; compass (B,) fp64,
+    raw; state B lavb_nav_state records (uint8, updated in place).  -> (cmds (B,) int32, nxps (B, 2) fp32, poses (B, 3) fp64,
+    flags (B,) int32 of LAVB_NAV_* bits), written into the given tensors when given."""
+    _need_cuda(nodes, node_cmd, route, gnss, compass, state)
+    if route.dtype != torch.int32 or route.dim() != 2 or route.shape[1] != 2 or not route.is_contiguous():
+        raise capi.LavbError(f"agent_nav_front: route must be a contiguous (B, 2) int32 tensor, got {route.dtype} {tuple(route.shape)}")
+    b = route.shape[0]
+    if nodes.dtype != torch.float64 or nodes.dim() != 2 or nodes.shape[1] != 2 or not nodes.is_contiguous():
+        raise capi.LavbError(f"agent_nav_front: nodes must be a contiguous (M, 2) fp64 tensor, got {nodes.dtype} {tuple(nodes.shape)}")
+    m = nodes.shape[0]
+    if node_cmd.dtype != torch.int32 or tuple(node_cmd.shape) != (m,) or not node_cmd.is_contiguous():
+        raise capi.LavbError(f"agent_nav_front: node_cmd must be a contiguous ({m},) int32 tensor, got {node_cmd.dtype} "
+                             f"{tuple(node_cmd.shape)}")
+    _f64_rows(gnss, b, 2, "agent_nav_front: gnss")
+    _f64_rows(compass, b, 0, "agent_nav_front: compass")
+    nbytes = b * agent_nav_state_bytes()
+    if state.dtype != torch.uint8 or tuple(state.shape) != (nbytes,) or not state.is_contiguous():
+        raise capi.LavbError(f"agent_nav_front: state must be a contiguous ({nbytes},) uint8 tensor, got {state.dtype} "
+                             f"{tuple(state.shape)}")
+    dev = route.device
+    if len({dev, nodes.device, node_cmd.device, gnss.device, compass.device, state.device}) != 1:
+        raise capi.LavbError("agent_nav_front: the inputs must be on one device")
+
+    def out(x, shape, dt, name):
+        if x is None:
+            return torch.empty(shape, dtype=dt, device=dev)
+        if x.dtype != dt or tuple(x.shape) != shape or not x.is_contiguous() or x.device != dev:
+            raise capi.LavbError(f"agent_nav_front: {name} must be a contiguous {shape} {dt} tensor on {dev}")
+        return x
+    cmds, nxps = out(cmds, (b,), torch.int32, "cmds"), out(nxps, (b, 2), torch.float32, "nxps")
+    poses, flags = out(poses, (b, 3), torch.float64, "poses"), out(flags, (b,), torch.int32, "flags")
+    check(lib().lavb_agent_nav_front(b, _ptr(nodes), _ptr(node_cmd), m, _ptr(route), _ptr(gnss), _ptr(compass), _ptr(state),
+                                     _ptr(cmds), _ptr(nxps), _ptr(poses), _ptr(flags), _stream()), "lavb_agent_nav_front")
+    _COUNT[0] += 1 if b else 0
+    return cmds, nxps, poses, flags
+
+
+def agent_nav_update(control, speed, gnss, compass, state):
+    """EKF.step of B agents after the controls (lavb_agent_nav_update): control (B, 3) fp32 = agent_control's output (steer in
+    column 0); speed (B,) fp64 m/s; gnss (B, 2) fp64; compass (B,) fp64, raw; state as in agent_nav_front, updated in place."""
+    _need_cuda(control, speed, gnss, compass, state)
+    b = state.numel() // agent_nav_state_bytes()
+    if control.dtype != torch.float32 or tuple(control.shape) != (b, 3) or not control.is_contiguous():
+        raise capi.LavbError(f"agent_nav_update: control must be a contiguous ({b}, 3) fp32 tensor, got {control.dtype} "
+                             f"{tuple(control.shape)}")
+    _f64_rows(speed, b, 0, "agent_nav_update: speed")
+    _f64_rows(gnss, b, 2, "agent_nav_update: gnss")
+    _f64_rows(compass, b, 0, "agent_nav_update: compass")
+    if state.dtype != torch.uint8 or state.numel() != b * agent_nav_state_bytes() or not state.is_contiguous():
+        raise capi.LavbError("agent_nav_update: state must be a contiguous uint8 tensor of whole lavb_nav_state records")
+    if len({control.device, speed.device, gnss.device, compass.device, state.device}) != 1:
+        raise capi.LavbError("agent_nav_update: the inputs must be on one device")
+    check(lib().lavb_agent_nav_update(b, _ptr(control), _ptr(speed), _ptr(gnss), _ptr(compass), _ptr(state), _stream()),
+          "lavb_agent_nav_update")
+    _COUNT[0] += 1 if b else 0
+
+
+def stack_job_poses(d_jobs, b, t, gap, keep, tick, ring_pose, poses=None):
+    """the R / dx / dy fields of stack_jobs' table from the device pose ring (lavb_stack_job_poses): d_jobs the uint8 table of
+    b * t STACK_JOB_DTYPE records; ring_pose (b, keep, 3) fp64, ``poses`` (b, 3) fp64 written to slot tick % keep first."""
+    _need_cuda(d_jobs, ring_pose, poses)
+    if d_jobs.dtype != torch.uint8 or d_jobs.numel() != b * t * STACK_JOB_DTYPE.itemsize or not d_jobs.is_contiguous():
+        raise capi.LavbError(f"stack_job_poses: jobs must hold {b} x {t} contiguous records")
+    if ring_pose.dtype != torch.float64 or tuple(ring_pose.shape) != (b, keep, 3) or not ring_pose.is_contiguous():
+        raise capi.LavbError(f"stack_job_poses: ring_pose must be a contiguous ({b}, {keep}, 3) fp64 tensor")
+    if poses is not None:
+        _f64_rows(poses, b, 3, "stack_job_poses: poses")
+    check(lib().lavb_stack_job_poses(_ptr(d_jobs), b, t, gap, keep, int(tick), _ptr(ring_pose), _ptr(poses), _stream()),
+          "lavb_stack_job_poses")
+    _COUNT[0] += 1 if b else 0
 
 
 PILLAR_ENCODER ="sorted"    # name of the 16-bit pipeline's pillar encoder, reported by bench.py; it selects nothing
