@@ -90,6 +90,38 @@ int lavb_paint_deconv_batched(const float* d_pts, int frames, int n, int pt_stri
 int lavb_seg_confusion(const void* d_feat, int feat_dtype, const float* d_deconv, const uint8_t* d_labels, const uint8_t* h_lut,
                        int n, int c_cls, int h, int w, int* d_out, void* stream);
 
+/* ---------------------------------------------------------------- confusion counts of the point painting
+ * stands behind: the painting of the LiDAR points, online (lavb_paint_deconv_batched: InferModel.point_painting /
+ *           forward_paint, model_inference.py:44-50,75-93) and offline (lav/data_paint.py:44-107, lidar_sem_%05d), scored
+ *           against the recorded semantic cameras at the pixel each point hits; the reference has no such evaluation.
+ * One launch, one thread per point, grid (ceil(n / 256), frames).  d_pts: fp32 (frames, n, 4) (x, y, z, intensity), NaN-padded;
+ *   d_meta: NULL, or DEVICE int32 (frames, 2) = (rows of the frame, score its stored rows 0 / 1), rows clamped to 0..n (NULL:
+ *   every row, stored rows scored); d_feat: NULL, or NHWC (frames * ncam, h/2, w/2, 16) fp32 / h16 (feat_dtype) = the input of
+ *   output_conv, with d_deconv lavb_paint_deconv_batched's 520-float table; d_tags: uint8 (frames * ncam, h, w) = the recorded
+ *   CARLA tags; h_lut: HOST uint8[256], the class of each tag (filter_sem as a table); d_stored: NULL, or fp32 (frames, n,
+ *   c_cls - 1) = lidar_sem rows; h_cams as lavb_paint; the pillar grid window [min_x, max_x) x [min_y, max_y).  At least one of
+ *   d_feat and d_stored.
+ * Per row i < rows: a NaN x, y or z counts as nan and nowhere else.  Otherwise: roof = inside LAVAgent.preprocess's roof box
+ *   (lavb_roof_filter's fp32 test); in window = not roof and inside the grid window as the voxeliser tests it; the hit camera and
+ *   pixel (v, u) are lavb_paint's (the last camera whose truncated pixel lies inside h x w); a point no camera sees counts as
+ *   not_visible (and not_visible_in_window) and is scored nowhere.  gt = h_lut[tag at (v, u) of the hit camera]; range bin of
+ *   fp32 sqrt(x*x + y*y): [0, 10), [10, 20), [20, 40), [40, inf) m.  Online class: the logits of lavb_seg_confusion at (v, u),
+ *   first index of the largest, a NaN logit -> invalid.  Stored class: the row s_k = p_k (1 - p_0) decoded in fp64 without
+ *   contraction, q = sqrt(sum s_k), p_0 = 1 - q, p_k = s_k / q, first index of the largest of (p_0, p_1, ...); a row summing to 0
+ *   is class 0; a NaN entering the decode -> stored_invalid.
+ * d_out: int32 (frames, lavb_paint_confusion_ints(ncam, c_cls, online, stored)); per frame: 8 counters (points, nan, roof,
+ *   in_window, not_visible, not_visible_in_window, invalid, stored_invalid), then per scored source (online first, then stored)
+ *   confusion[cam][range][in window 0 / 1][gt][pred], then with both sources agreement[cam][online][stored] over the points both
+ *   score.  Integer sums, so the counts do not depend on the schedule.
+ * 2 <= c_cls <= 8, 1 <= ncam <= 4, h and w even, frames <= 65535, every h_lut entry < c_cls, min < max; points 16-byte,
+ *   features 16-byte (fp32) / 8-byte (h16), the other buffers 4-byte aligned.  Every element of the frames rows is written; a
+ *   rejected call writes nothing.  lavb_paint_confusion_ints returns -1 for arguments the kernel rejects. */
+int lavb_paint_confusion_ints(int ncam, int c_cls, int online, int stored);
+int lavb_paint_confusion(const float* d_pts, int frames, int n, const int* d_meta, const void* d_feat, int feat_dtype,
+                         const float* d_deconv, const uint8_t* d_tags, const uint8_t* h_lut, const float* d_stored,
+                         const float* h_cams, int ncam, int c_cls, int h, int w, float min_x, float max_x, float min_y,
+                         float max_y, int* d_out, void* stream);
+
 /* ---------------------------------------------------------------- sweep stacking
  * replaces: LAVAgent.get_stacked_lidar + move_lidar_points (team_code_v2/lav_agent_fast.py:363-383,547-565)
  * and the ego-roof filter LAVAgent.preprocess (lav_agent.py:448-457, roof_filter!=0 marks dropped rows x=NaN).

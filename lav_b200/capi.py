@@ -69,6 +69,10 @@ _SIGS = {
                                             C.c_void_p]),
     "lavb_seg_confusion": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int,
                                      C.c_void_p, C.c_void_p]),
+    "lavb_paint_confusion_ints": (C.c_int, [C.c_int, C.c_int, C.c_int, C.c_int]),
+    "lavb_paint_confusion": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p,
+                                       C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float, C.c_float,
+                                       C.c_float, C.c_float, C.c_void_p, C.c_void_p]),
     "lavb_stack_jobs": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p]),
     "lavb_bev_targets": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p]),
     "lavb_png_decode_gray8": (C.c_int, [C.c_void_p, C.c_longlong, C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_int,

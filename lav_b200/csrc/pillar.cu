@@ -3,6 +3,7 @@
 // decorates each point, runs the 2-layer point MLP and max-pools into the NHWC canvas.
 #include <stdlib.h>
 #include "common.cuh"
+#include "pillar_grid.cuh"
 
 namespace lavb {
 
@@ -14,11 +15,6 @@ struct Clouds {
   int batch;
 };
 
-struct Grid {
-  float min_x, max_x, min_y, max_y, ppm;
-  int nx, ny;
-};
-
 __device__ __forceinline__ int find_cloud(const Clouds& c, int i) {
   int lo = 0, hi = c.batch - 1;
   while (lo < hi) {
@@ -28,10 +24,10 @@ __device__ __forceinline__ int find_cloud(const Clouds& c, int i) {
   return lo;
 }
 
-// grid_locations, point_pillar.py:70-79: half-open window test on the raw fp32 coordinates, then
+// grid_locations, point_pillar.py:70-79: half-open window test on the raw fp32 coordinates (in_window), then
 // trunc((v - min) * ppm) in fp32.  Returns false for dropped points (NaN fails every comparison).
 __device__ __forceinline__ bool locate(const Grid& g, float x, float y, int& xi, int& yi) {
-  if (!(x >= g.min_x && x < g.max_x && y >= g.min_y && y < g.max_y)) return false;
+  if (!in_window(g, x, y)) return false;
   xi = (int)__fmul_rn(__fsub_rn(x, g.min_x), g.ppm);
   yi = (int)__fmul_rn(__fsub_rn(y, g.min_y), g.ppm);
   return true;

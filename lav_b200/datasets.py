@@ -705,6 +705,104 @@ class CameraDataset:
         return {k: v.to(self.device, non_blocking=True) for k, v in st.items()}
 
 
+class PaintDataset:
+    """The painted LiDAR samples of a recording, for scoring the point painting (lav_b200.evaluate_paint): the frames of
+    BasicDataset (index_trajectories, the same YAML keys and ``overrides``), unaugmented.
+
+    Frame k holds the recorded sweep lidar_%05d and the recorded tags sem_{c} of the painting cameras c = 0 .. 2
+    (point_painting.CAMERA_YAWS, the three cameras data_paint reads; not the config's camera_yaws, which lists five); with
+    ``online`` their colour images rgb_{c}, with ``stored`` the painted rows lidar_sem_%05d.  Images are decoded on the host as
+    BasicDataset.load_img decodes them; an image of another size than the painting geometry (288 x 256) is a LavbError.  A
+    lidar_sem key that is missing or whose size is not the sweep's rows x (len(seg_channels)) floats marks the frame
+    mismatched: its stored rows are not scored, and nothing is raised."""
+
+    def __init__(self, config_path, online=True, stored=False, seed=2021, device=torch.device("cuda"), overrides=None):
+        from . import point_painting
+        if not (online or stored):
+            raise LavbError("PaintDataset: nothing to score (neither online nor stored)")
+        with open(config_path) as f:
+            cfg = yaml.safe_load(f)
+        cfg.update(overrides or {})
+        self.cfg = cfg
+        for k, v in cfg.items():
+            setattr(self, k, v)
+        self.device = torch.device(device)
+        self.online, self.stored = online, stored
+        self.converters = point_painting.make_converters(self.camera_x, self.camera_z)
+        self.cams = list(range(len(self.converters)))
+        self.image_hw = (self.converters[0].rgb_h, self.converters[0].rgb_w)
+        self.window = (self.min_x, self.max_x, self.min_y, self.max_y)
+        self.n_classes = len(self.seg_channels) + 1
+        self.paths, self.index = index_trajectories(self.data_dir, self.percentage_data, self.all_towns, self.num_plan, seed)
+        self._envs, self._env_lock = {}, threading.Lock()
+
+    __len__ = TemporalLiDARPaintedDataset.__len__
+    env = TemporalLiDARPaintedDataset.env
+
+    def no_draw(self):
+        """no augmentation: nothing to draw."""
+        return ()
+
+    def _image(self, env, tag, i):
+        img = load_img(env, tag, i)
+        if img.shape[:2] != self.image_hw:
+            raise LavbError(f"record key {tag}_{i:05d} is {img.shape[1]} x {img.shape[0]}, the painting cameras' images are "
+                            f"{self.image_hw[1]} x {self.image_hw[0]}")
+        return img
+
+    def prepare(self, idx):
+        """the host record of frame ``idx``: lidar (n, 4) f32, labels (ncam, h, w) uint8, with online rgbs (ncam, h, w, 3) uint8,
+        with stored the lidar_sem rows (n, C - 1) f32 or None when the frame is mismatched."""
+        traj, i = self.index[idx]
+        env = self.env(traj)
+        key = f"lidar_{i:05d}"
+        raw = env.get(key)
+        if raw is None:
+            raise LavbError(f"record key {key} is missing")
+        h = dict(lidar=np.frombuffer(raw, np.float32).reshape(-1, 4))
+        h["labels"] = np.stack([self._image(env, f"sem_{c}", i) for c in self.cams])
+        if self.online:
+            h["rgbs"] = np.stack([self._image(env, f"rgb_{c}", i) for c in self.cams])
+        if self.stored:
+            sem = env.get(f"lidar_sem_{i:05d}")
+            w = self.n_classes - 1
+            ok = sem is not None and len(sem) == len(h["lidar"]) * w * 4
+            h["stored"] = np.frombuffer(sem, np.float32).reshape(-1, w) if ok else None
+        return h
+
+    def stage_batch(self, hs):
+        """the prepared frames ``hs`` in host buffers (pinned on a CUDA dataset): points (B, Nmax, 4) f32 NaN-padded (Nmax >= 1),
+        meta (B, 2) int32 = (rows, stored scored), labels (B, ncam, h, w) and rgbs (B, ncam, h, w, 3) uint8, stored (B, Nmax,
+        C - 1) f32 (zero where not scored)."""
+        pin = self.device.type == "cuda"
+        B, n_max = len(hs), max(1, max(len(h["lidar"]) for h in hs))
+        empty = lambda shape, dtype: torch.empty(shape, dtype=dtype, pin_memory=pin)
+        st = dict(points=empty((B, n_max, 4), torch.float32), meta=empty((B, 2), torch.int32))
+        pts, meta = st["points"].numpy(), st["meta"].numpy()
+        pts[:] = np.nan
+        for b, h in enumerate(hs):
+            pts[b, :len(h["lidar"])] = h["lidar"]
+            meta[b] = (len(h["lidar"]), int(h.get("stored") is not None))
+        for key in ("labels", "rgbs"):
+            if key in hs[0]:
+                st[key] = empty((B,) + hs[0][key].shape, torch.uint8)
+                dst = st[key].numpy()
+                for b, h in enumerate(hs):
+                    dst[b] = h[key]
+        if self.stored:
+            st["stored"] = empty((B, n_max, self.n_classes - 1), torch.float32)
+            dst = st["stored"].numpy()
+            dst[:] = 0
+            for b, h in enumerate(hs):
+                if h["stored"] is not None:
+                    dst[b, :len(h["stored"])] = h["stored"]
+        return st
+
+    def launch_batch(self, st):
+        """the staged host buffers copied to the device, one copy each."""
+        return {k: v.to(self.device, non_blocking=True) for k, v in st.items()}
+
+
 class CameraBatchLoader(TemporalBatchLoader):
     """Batches of a CameraDataset in frame order, unaugmented, the last batch possibly short: TemporalBatchLoader's ordered mode,
     with the record reads and image decodes of a batch on ``num_workers`` threads one batch ahead of the GPU.  A batch is the

@@ -494,6 +494,91 @@ def seg_confusion(feat, table, labels, lut, n_classes, out=None):
     return out
 
 
+PAINT_COUNTERS = ("points", "nan", "roof", "in_window", "not_visible", "not_visible_in_window", "invalid", "stored_invalid")
+PAINT_RANGES_M = (10.0, 20.0, 40.0)      # the range bins' edges (horizontal distance), the last bin open
+
+
+def paint_confusion_ints(ncam, n_classes, online, stored):
+    """length of one frame's lavb_paint_confusion row."""
+    per_src = ncam * (len(PAINT_RANGES_M) + 1) * 2 * n_classes * n_classes
+    return len(PAINT_COUNTERS) + (int(online) + int(stored)) * per_src + (ncam * n_classes * n_classes if online and stored else 0)
+
+
+def paint_confusion_views(counts, ncam, n_classes, online, stored):
+    """views of paint_confusion rows (F, L) (torch or numpy): counters (F, 8) in PAINT_COUNTERS order, "online" / "stored"
+    (F, ncam, 4, 2, C, C) = [camera][range bin][in window][recorded][predicted] for each scored source, and with both
+    "agreement" (F, ncam, C, C) = [camera][online][stored]."""
+    c, nr = n_classes, len(PAINT_RANGES_M) + 1
+    per_src = ncam * nr * 2 * c * c
+    views = dict(counters=counts[:, :len(PAINT_COUNTERS)])
+    o = len(PAINT_COUNTERS)
+    for name, on in (("online", online), ("stored", stored)):
+        if on:
+            views[name] = counts[:, o:o + per_src].reshape(-1, ncam, nr, 2, c, c)
+            o += per_src
+    if online and stored:
+        views["agreement"] = counts[:, o:o + ncam * c * c].reshape(-1, ncam, c, c)
+    return views
+
+
+def paint_confusion(points, tags, lut, cams, window, n_classes, feat=None, table=None, stored=None, meta=None, out=None):
+    """Per-frame confusion counts of the point painting against the recorded semantic cameras in one launch (see
+    lavb_paint_confusion in include/lav_b200.h).  points (F, N, 4) fp32 = the NaN-padded sweeps; tags (F * ncam, H, W) uint8 =
+    the recorded sem images; lut = sem_class_table(seg_channels) on the host; cams = the packed converters (ncam, 41); window =
+    (min_x, max_x, min_y, max_y) of the pillar grid; feat NHWC (F * ncam, H/2, W/2, 16) fp32 / h16 with table = pack_deconv2x2
+    (the online source) and / or stored (F, N, C - 1) fp32 = lidar_sem rows; meta (F, 2) int32 = (rows, stored scored) per frame
+    or None.  -> int32 (F, paint_confusion_ints(...)) (written into ``out`` when given); paint_confusion_views splits it."""
+    _need_cuda(points, tags, feat, table, stored, meta)
+    c = int(n_classes)
+    if points.dtype != torch.float32 or points.dim() != 3 or points.shape[2] != 4 or not points.is_contiguous():
+        raise capi.LavbError(f"paint_confusion: points must be a contiguous (F, N, 4) fp32 tensor, got {points.dtype} "
+                             f"{tuple(points.shape)}")
+    f, n, _ = points.shape
+    cams = np.ascontiguousarray(cams, dtype=np.float32)
+    if cams.ndim != 2 or cams.shape[1] != 41 or not 1 <= cams.shape[0] <= 4:
+        raise capi.LavbError(f"paint_confusion: cams must be (ncam, 41) with 1 <= ncam <= 4, got {cams.shape}")
+    ncam = cams.shape[0]
+    if tags.dtype != torch.uint8 or tags.dim() != 3 or tags.shape[0] != f * ncam or not tags.is_contiguous():
+        raise capi.LavbError(f"paint_confusion: tags must be a contiguous ({f * ncam}, H, W) uint8 tensor, got {tags.dtype} "
+                             f"{tuple(tags.shape)}")
+    h, w = tags.shape[1:]
+    if feat is None and stored is None:
+        raise capi.LavbError("paint_confusion: give feat (the online painting), stored (lidar_sem rows) or both")
+    if feat is not None:
+        if feat.dtype not in (torch.float32, h16()) or tuple(feat.shape) != (f * ncam, h // 2, w // 2, 16) or not feat.is_contiguous():
+            raise capi.LavbError(f"paint_confusion: feat must be a contiguous ({f * ncam}, {h // 2}, {w // 2}, 16) fp32 or {h16()} "
+                                 f"tensor, got {feat.dtype} {tuple(feat.shape)}")
+        if table is None or table.dtype != torch.float32 or table.numel() != 520 or not table.is_contiguous():
+            raise capi.LavbError("paint_confusion: table must be the 520-float pack_deconv2x2 table")
+    if stored is not None and (stored.dtype != torch.float32 or tuple(stored.shape) != (f, n, c - 1) or not stored.is_contiguous()):
+        raise capi.LavbError(f"paint_confusion: stored must be a contiguous ({f}, {n}, {c - 1}) fp32 tensor, got {stored.dtype} "
+                             f"{tuple(stored.shape)}")
+    if meta is not None and (meta.dtype != torch.int32 or tuple(meta.shape) != (f, 2) or not meta.is_contiguous()):
+        raise capi.LavbError(f"paint_confusion: meta must be a contiguous ({f}, 2) int32 tensor")
+    lut = np.ascontiguousarray(lut)
+    if lut.dtype != np.uint8 or lut.shape != (256,) or int(lut.max()) >= c:
+        raise capi.LavbError(f"paint_confusion: lut must be a host (256,) uint8 array of classes below {c}, got {lut.dtype} "
+                             f"{lut.shape}")
+    if len({t.device for t in (points, tags, feat, table, stored, meta) if t is not None}) != 1:
+        raise capi.LavbError("paint_confusion: the inputs must be on one device")
+    ints = lib().lavb_paint_confusion_ints(ncam, c, feat is not None, stored is not None)
+    if ints < 0:
+        raise capi.LavbError(f"paint_confusion: {c} classes outside 2..8")
+    if out is None:
+        out = torch.empty((f, ints), dtype=torch.int32, device=points.device)
+    elif out.dtype != torch.int32 or tuple(out.shape) != (f, ints) or not out.is_contiguous() or out.device != points.device:
+        raise capi.LavbError(f"paint_confusion: out must be a contiguous ({f}, {ints}) int32 tensor on {points.device}")
+    if n == 0:              # empty sweeps: every count is 0 (and an empty stored buffer has no device pointer to pass)
+        return out.zero_()
+    min_x, max_x, min_y, max_y = (float(v) for v in window)
+    check(lib().lavb_paint_confusion(_ptr(points), f, n, _ptr(meta), _ptr(feat), _DT[feat.dtype] if feat is not None else F32,
+                                     _ptr(table), _ptr(tags), lut.ctypes.data_as(C.c_void_p), _ptr(stored),
+                                     cams.ctypes.data_as(C.c_void_p), ncam, c, h, w, min_x, max_x, min_y, max_y, _ptr(out),
+                                     _stream()), "lavb_paint_confusion")
+    _COUNT[0] += f > 0
+    return out
+
+
 STACK_JOB_DTYPE = np.dtype([("src", np.uint64), ("dst", np.uint64), ("n", np.int32), ("time_idx", np.int32), ("R", np.float32, 9),
                             ("dx", np.float32), ("dy", np.float32), ("pad", np.int32)])
 assert STACK_JOB_DTYPE.itemsize == 72
