@@ -472,9 +472,22 @@ int lavb_pillar_scatter_max_bwd(const float* d_gcanvas, const int* d_argmax, con
  *        in[n, oy*in_sy+dy[t], ox*in_sx+dx[t], in_coff+ci] * w[t][ci][co] )   (zero outside the input)
  * epi(a): a += bias[co]; if pre_relu a=max(a,0); a = a*scale[co]+shift[co]; a += res[...]; if post_relu
  *         a=max(a,0); if sigmoid a=1/(1+exp(-a)).   Null pointers skip a step.
+ *         max(a,0) is fmaxf(a, 0.f): a NaN that reaches a ReLU leaves it as 0; without a ReLU a NaN accumulator stays NaN
+ *         through every step.  Every body follows this rule.
  * d_w: [ntaps][cin][cout_pad] fp32 with cout_pad = cout rounded up to 16.
+ * Accumulation is fp32.  One exception to "fp32 weights": a 16-bit input with cin == 16 and ntaps <= 9 runs on the
+ * tensor cores (mma.sync), which round each weight to the 16-bit type (round to nearest, saturating) before use; the
+ * same layer with 10..16 taps, or any fp32 input, multiplies by the fp32 weights.
  * A strided Conv2d uses in_s=stride, dy=ky*dil-pad; a ConvTranspose2d is issued once per output phase with
- * in_s=1, out_s=stride (lav_b200/layers.py builds the tap lists). */
+ * in_s=1, out_s=stride (lav_b200/layers.py builds the tap lists).
+ * Writes exactly the channels [out_coff, out_coff+cout) of the output pixels (oy*out_sy+out_oy, ox*out_sx+out_ox) with
+ * oy < hog, ox < wog that fall inside hout x wout, for the n images; nothing else.
+ * Checked (a rejected call writes nothing): 1 <= ntaps <= 16; cin >= 4 and cin, in_coff, in_cstride multiples of 4;
+ * 0 <= in_coff, in_coff+cin <= in_cstride; 0 <= out_coff, out_coff+cout <= out_cstride; with a residual 0 <= res_coff,
+ * res_coff+cout <= res_cstride and res_dtype == out_dtype; n, hog, wog, cout >= 1; hin, win, hout, wout >= 1;
+ * in_s, out_s >= 1, out_oy, out_ox >= 0; in, out, w non-null; scale and shift both or neither; in, out and res
+ * 4-element aligned (16 bytes fp32, 8 bytes 16-bit), w 16-byte aligned, bias / scale / shift 4-byte aligned.
+ * Not checked: that the buffers hold the extents the descriptor describes. */
 typedef struct {
   const void* in; int in_dtype; int n, hin, win, cin, in_cstride, in_coff;
   void* out; int out_dtype; int hout, wout, cout, out_cstride, out_coff;
@@ -495,18 +508,31 @@ int lavb_conv_taps(const lavb_conv_desc* h_desc, void* stream);
 /* grouped ConvTranspose2d(k3,s2,p1,op1) with <=4 output channels per group: the 4 head output layers in one launch.
  * replaces: Head.net[3] x4 (lav/models/lidar.py:155,159-164) incl. bias and the seg head's sigmoid.
  * d_in NHWC [n][h][w][in_cstride] (group g reads channels [g*cin_g,(g+1)*cin_g)); d_w fp32 [g][cin_g][9][4]
- * (tap = ky*3+kx, cout padded to 4); d_bias [g][4]; output g: fp32 NHWC [n][2h][2w][n_out[g]]. */
+ * (tap = ky*3+kx, cout padded to 4); d_bias [g][4]; output g: fp32 NHWC [n][2h][2w][n_out[g]], every element written,
+ * sigmoid applied when h_sigmoid[g] != 0.  dtype LAVB_F32 or the 16-bit type; fp32 weights and accumulation.
+ * Checked (a rejected call writes nothing): 1 <= groups <= 8; cin_g a multiple of 8 in 8..64; in_cstride a multiple
+ * of 8 with groups*cin_g <= in_cstride; n, h, w >= 0 (an empty map writes nothing); 1 <= n_out[g] <= 4; d_in 4-element
+ * aligned (16 bytes fp32, 8 bytes 16-bit); d_w, d_bias and the outputs non-null and 4-byte aligned. */
 int lavb_deconv3x3s2_small(const void* d_in, int dtype, int n, int h, int w, int in_cstride, int groups, int cin_g,
                            const float* d_w, const float* d_bias, const int* h_n_out, const int* h_sigmoid,
                            float* const* h_out_ptrs, void* stream);
 
-/* 2x2/2 max-pool -> y*scale[c]+shift[c] -> ReLU into a channel slice (ERFNet DownsamplerBlock, erfnet.py:20-23) */
+/* 2x2/2 max-pool -> y*scale[c]+shift[c] -> ReLU into a channel slice (ERFNet DownsamplerBlock, erfnet.py:20-23).
+ * out[n, y, x, out_coff+k] = fmaxf(fmaf(max of the 2x2 window of in[.., in_coff+k], scale[k], shift[k]), 0), k < c, in the
+ * input dtype (LAVB_F32 or the 16-bit type); nothing else is written.  A vector body runs when c, the offsets and the
+ * strides are multiples of 4, d_in / d_out are 4-element aligned and scale / shift 16-byte aligned; otherwise a scalar
+ * body computes the same values.  Checked (a rejected call writes nothing): n, hin, win >= 0 and even hin, win; c >= 1;
+ * 0 <= in_coff, in_coff+c <= in_cstride; 0 <= out_coff, out_coff+c <= out_cstride; when there is work, non-null
+ * pointers aligned to their element size. */
 int lavb_pool2_affine_relu(const void* d_in, int dtype, int n, int hin, int win, int c, int in_cstride, int in_coff,
                            const float* d_scale, const float* d_shift,
                            void* d_out, int out_cstride, int out_coff, void* stream);
 
 /* RGB ingest: uint8 NHWC (n,h,w,3) or float NCHW (n,3,h,w) in 0..255 -> (x/255-.5)*2 as NHWC with 4 channels
- * (4th = 0).  replaces RGBSegmentationModel.normalize (lav/models/rgb.py:41). */
+ * (4th = 0).  replaces RGBSegmentationModel.normalize (lav/models/rgb.py:41).  Computed as fp32 (x / 255 - 0.5) * 2 with
+ * three roundings, then stored in out_dtype (LAVB_F32 or the 16-bit type).  Checked: n, h, w >= 0 (an empty batch writes
+ * nothing); otherwise non-null pointers, d_out 4-element aligned (16 bytes fp32, 8 bytes 16-bit), a float source 4-byte
+ * aligned. */
 int lavb_rgb_normalize(const void* d_rgb, int src_is_u8_nhwc, int n, int h, int w, void* d_out, int out_dtype,
                        void* stream);
 
@@ -570,7 +596,10 @@ int lavb_crop_bilinear_u8(const uint8_t* d_map, int b, int c, int h, int w, cons
 int lavb_crop_bilinear_bwd(const float* d_gout, int b, int h, int w, int c, const int* d_frame_idx, const float* d_theta,
                            int k, int crop, float* d_gfeat, void* stream);
 
-/* dtype / layout helpers */
+/* dtype / layout helpers
+ * lavb_convert: count elements fp32 -> 16-bit (round to nearest, saturating to the finite range; NaN stays NaN) or 16-bit
+ * -> fp32 (exact).  count >= 0; pointers non-null and aligned to their element size.  Both 4-element aligned take the
+ * vector body, otherwise every element is converted one at a time; the results are the same. */
 int lavb_convert(const void* d_src, int src_dtype, void* d_dst, int dst_dtype, long long count, void* stream);
 
 /* ---------------------------------------------------------------- wgmma implicit-GEMM tap-list convolution

@@ -378,7 +378,6 @@ __global__ void __launch_bounds__(128) conv_c16_mma_kernel(const __grid_constant
       e_scale[nn][e] = (a.scale && in_range) ? __ldg(a.scale + c) : 1.f;
       e_shift[nn][e] = (a.shift && in_range) ? __ldg(a.shift + c) : 0.f;
     }
-  const float lo_pre = a.pre_relu ? 0.f : -INFINITY, lo_post = a.post_relu ? 0.f : -INFINITY;
   const bool pair_ok = (a.out_coff % 2 == 0) && (a.out_cstride % 2 == 0) && (a.res == nullptr || (a.res_coff % 2 == 0 && a.res_cstride % 2 == 0));
   const h16* in = reinterpret_cast<const h16*>(a.in) + (long long)img * a.hin * a.win * a.in_cstride + a.in_coff + 2 * tq;
   // the 4 pixels this lane touches: rows gq, gq+8 of both m-tiles
@@ -430,14 +429,15 @@ __global__ void __launch_bounds__(128) conv_c16_mma_kernel(const __grid_constant
       const int c = co0 + nn * 8 + 2 * tq;
       if (c >= a.cout) continue;
       float x0 = acc[r >> 1][nn][(r & 1) * 2] + e_bias[nn][0], x1 = acc[r >> 1][nn][(r & 1) * 2 + 1] + e_bias[nn][1];
-      x0 = fmaf(fmaxf(x0, lo_pre), e_scale[nn][0], e_shift[nn][0]);
-      x1 = fmaf(fmaxf(x1, lo_pre), e_scale[nn][1], e_shift[nn][1]);
+      // each step only when its flag / pointer is set, as in the other bodies: fmaxf(NaN, -inf) would turn a NaN into -inf
+      if (a.pre_relu) { x0 = fmaxf(x0, 0.f); x1 = fmaxf(x1, 0.f); }
+      if (a.scale) { x0 = fmaf(x0, e_scale[nn][0], e_shift[nn][0]); x1 = fmaf(x1, e_scale[nn][1], e_shift[nn][1]); }
       const bool pair = pair_ok && (c + 1 < a.cout);
       if (rp) {
         if (pair) { const float2 rr = load2<TOut>(rp + c); x0 += rr.x; x1 += rr.y; }
         else { x0 += to_f32<TOut>(rp[c]); if (c + 1 < a.cout) x1 += to_f32<TOut>(rp[c + 1]); }
       }
-      x0 = fmaxf(x0, lo_post); x1 = fmaxf(x1, lo_post);
+      if (a.post_relu) { x0 = fmaxf(x0, 0.f); x1 = fmaxf(x1, 0.f); }
       if (a.sigmoid) { x0 = 1.f / (1.f + expf(-x0)); x1 = 1.f / (1.f + expf(-x1)); }
       if (pair) store2<TOut>(op + c, x0, x1);
       else { op[c] = from_f32<TOut>(x0); if (c + 1 < a.cout) op[c + 1] = from_f32<TOut>(x1); }
@@ -490,9 +490,24 @@ extern "C" int lavb_conv_taps(const lavb_conv_desc* d, void* stream) {
   LAVB_CHECK_ARG(d->ntaps >= 1 && d->ntaps <= 16, "conv_taps: ntaps must be 1..16 (got %d)", d->ntaps);
   LAVB_CHECK_ARG(d->cin % 4 == 0 && d->in_coff % 4 == 0 && d->in_cstride % 4 == 0,
                  "conv_taps: cin/in_coff/in_cstride must be multiples of 4 (got %d/%d/%d)", d->cin, d->in_coff, d->in_cstride);
-  LAVB_CHECK_ARG(d->in_coff + d->cin <= d->in_cstride && d->out_coff + d->cout <= d->out_cstride, "conv_taps: channel slice out of range");
+  LAVB_CHECK_ARG(d->cin >= 4, "conv_taps: cin must be >= 4 (got %d)", d->cin);
+  LAVB_CHECK_ARG(d->in_coff >= 0 && d->out_coff >= 0 && d->in_coff + d->cin <= d->in_cstride && d->out_coff + d->cout <= d->out_cstride,
+                 "conv_taps: channel slice out of range");
+  LAVB_CHECK_ARG(d->res == nullptr || (d->res_coff >= 0 && d->res_coff + d->cout <= d->res_cstride),
+                 "conv_taps: residual channel slice out of range");
   LAVB_CHECK_ARG((d->scale == nullptr) == (d->shift == nullptr), "conv_taps: scale and shift come together");
   LAVB_CHECK_ARG(d->n > 0 && d->hog > 0 && d->wog > 0 && d->cout > 0, "conv_taps: empty problem");
+  LAVB_CHECK_ARG(d->hin >= 1 && d->win >= 1 && d->hout >= 1 && d->wout >= 1, "conv_taps: map sizes must be >= 1");
+  LAVB_CHECK_ARG(d->in_sy >= 1 && d->in_sx >= 1 && d->out_sy >= 1 && d->out_sx >= 1 && d->out_oy >= 0 && d->out_ox >= 0,
+                 "conv_taps: strides must be >= 1 and output offsets >= 0");
+  LAVB_CHECK_ARG(d->in != nullptr && d->out != nullptr && d->w != nullptr, "conv_taps: null in / out / w");
+  // the bodies move 4 channels at a time (float4 / 4 x h16) from these base pointers; bias / scale / shift are read per element
+  const uintptr_t in_al = d->in_dtype == LAVB_F32 ? 16 : 8, out_al = d->out_dtype == LAVB_F32 ? 16 : 8;
+  LAVB_CHECK_ARG(reinterpret_cast<uintptr_t>(d->in) % in_al == 0 && reinterpret_cast<uintptr_t>(d->out) % out_al == 0 &&
+                     reinterpret_cast<uintptr_t>(d->res) % out_al == 0 && reinterpret_cast<uintptr_t>(d->w) % 16 == 0 &&
+                     reinterpret_cast<uintptr_t>(d->bias) % 4 == 0 && reinterpret_cast<uintptr_t>(d->scale) % 4 == 0 &&
+                     reinterpret_cast<uintptr_t>(d->shift) % 4 == 0,
+                 "conv_taps: in / out / res must be 4-element aligned (16 B fp32, 8 B 16-bit), w 16-byte aligned");
   ConvArgs a;
   a.in = d->in; a.out = d->out; a.res = d->res; a.w = d->w; a.bias = d->bias; a.scale = d->scale; a.shift = d->shift;
   a.n = d->n; a.hin = d->hin; a.win = d->win; a.cin = d->cin; a.in_cstride = d->in_cstride; a.in_coff = d->in_coff;
@@ -515,11 +530,22 @@ extern "C" int lavb_conv_taps(const lavb_conv_desc* d, void* stream) {
 extern "C" int lavb_pool2_affine_relu(const void* d_in, int dtype, int n, int hin, int win, int c, int in_cstride, int in_coff,
                                       const float* d_scale, const float* d_shift, void* d_out, int out_cstride, int out_coff,
                                       void* stream) {
+  LAVB_CHECK_ARG(dtype == LAVB_F32 || dtype == LAVB_H16, "pool2: bad dtype");
+  LAVB_CHECK_ARG(n >= 0 && hin >= 0 && win >= 0 && c >= 1, "pool2: n, hin, win must be >= 0 and c >= 1");
   LAVB_CHECK_ARG(hin % 2 == 0 && win % 2 == 0, "pool2: odd input size");
+  LAVB_CHECK_ARG(in_coff >= 0 && in_coff + c <= in_cstride && out_coff >= 0 && out_coff + c <= out_cstride,
+                 "pool2: channel slice out of range");
   const long long total = (long long)n * (hin / 2) * (win / 2) * c;
   if (total == 0) return 0;
+  const uintptr_t esz = dtype == LAVB_F32 ? 4 : 2;
+  LAVB_CHECK_ARG(d_in != nullptr && d_out != nullptr && d_scale != nullptr && d_shift != nullptr, "pool2: null pointer");
+  LAVB_CHECK_ARG(reinterpret_cast<uintptr_t>(d_in) % esz == 0 && reinterpret_cast<uintptr_t>(d_out) % esz == 0 &&
+                     reinterpret_cast<uintptr_t>(d_scale) % 4 == 0 && reinterpret_cast<uintptr_t>(d_shift) % 4 == 0,
+                 "pool2: pointers must be aligned to their element size");
   cudaStream_t st = (cudaStream_t)stream;
+  // the vector body moves 4 channels at a time: it needs 4-element aligned maps and 16-byte aligned scale / shift
   const bool vec = c % 4 == 0 && in_cstride % 4 == 0 && in_coff % 4 == 0 && out_cstride % 4 == 0 && out_coff % 4 == 0 &&
+                   reinterpret_cast<uintptr_t>(d_in) % (4 * esz) == 0 && reinterpret_cast<uintptr_t>(d_out) % (4 * esz) == 0 &&
                    (reinterpret_cast<uintptr_t>(d_scale) % 16 == 0) && (reinterpret_cast<uintptr_t>(d_shift) % 16 == 0);
   if (vec && dtype == LAVB_F32) {
     pool2_vec4_kernel<float><<<ceil_div(total / 4, 256), 256, 0, st>>>((const float*)d_in, n, hin, win, c, in_cstride, in_coff, d_scale,
@@ -531,11 +557,10 @@ extern "C" int lavb_pool2_affine_relu(const void* d_in, int dtype, int n, int hi
   } else if (dtype == LAVB_F32)
     pool2_kernel<float><<<ceil_div(total, 256), 256, 0, st>>>((const float*)d_in, n, hin, win, c, in_cstride, in_coff, d_scale,
                                                                d_shift, (float*)d_out, out_cstride, out_coff);
-  else if (dtype == LAVB_H16)
+  else
     pool2_kernel<h16><<<ceil_div(total, 256), 256, 0, st>>>((const h16*)d_in, n, hin, win, c, in_cstride,
                                                                        in_coff, d_scale, d_shift, (h16*)d_out,
                                                                        out_cstride, out_coff);
-  else LAVB_CHECK_ARG(false, "pool2: bad dtype");
   LAVB_LAUNCH_OK();
   return 0;
 }

@@ -96,12 +96,24 @@ extern "C" int lavb_deconv3x3s2_small(const void* d_in, int dtype, int n, int h,
                                       const float* d_w, const float* d_bias, const int* h_n_out, const int* h_sigmoid,
                                       float* const* h_out_ptrs, void* stream) {
   LAVB_CHECK_ARG(groups >= 1 && groups <= kMaxGroups, "deconv_small: 1..8 groups");
-  LAVB_CHECK_ARG(cin_g % 8 == 0 && groups * cin_g <= in_cstride && in_cstride % 8 == 0, "deconv_small: channels must be multiples of 8");
+  LAVB_CHECK_ARG(dtype == LAVB_F32 || dtype == LAVB_H16, "deconv_small: bad dtype");
+  LAVB_CHECK_ARG(cin_g >= 8 && cin_g % 8 == 0 && groups * cin_g <= in_cstride && in_cstride % 8 == 0,
+                 "deconv_small: channels must be positive multiples of 8");
   LAVB_CHECK_ARG(cin_g <= 64, "deconv_small: at most 64 input channels per group (got %d)", cin_g);
+  LAVB_CHECK_ARG(n >= 0 && h >= 0 && w >= 0, "deconv_small: n, h, w must be >= 0");
+  LAVB_CHECK_ARG(h_n_out != nullptr && h_sigmoid != nullptr && h_out_ptrs != nullptr, "deconv_small: null host array");
+  // the input is staged 4 channels at a time; weights, bias and outputs are accessed per element
+  LAVB_CHECK_ARG((long long)n * h * w == 0 ||
+                     (d_in != nullptr && d_w != nullptr && d_bias != nullptr &&
+                      reinterpret_cast<uintptr_t>(d_in) % (dtype == LAVB_F32 ? 16 : 8) == 0 &&
+                      reinterpret_cast<uintptr_t>(d_w) % 4 == 0 && reinterpret_cast<uintptr_t>(d_bias) % 4 == 0),
+                 "deconv_small: d_in must be 4-element aligned (16 B fp32, 8 B 16-bit), d_w and d_bias non-null and 4-byte aligned");
   DeconvArgs a;
   a.in = d_in; a.n = n; a.h = h; a.w = w; a.in_cstride = in_cstride; a.cin_g = cin_g; a.groups = groups; a.wgt = d_w; a.bias = d_bias;
   for (int g = 0; g < groups; ++g) {
     LAVB_CHECK_ARG(h_n_out[g] >= 1 && h_n_out[g] <= 4, "deconv_small: 1..4 output channels per group");
+    LAVB_CHECK_ARG((long long)n * h * w == 0 || (h_out_ptrs[g] != nullptr && reinterpret_cast<uintptr_t>(h_out_ptrs[g]) % 4 == 0),
+                   "deconv_small: output %d null or not 4-byte aligned", g);
     a.out[g] = h_out_ptrs[g]; a.n_out[g] = h_n_out[g]; a.sigmoid[g] = h_sigmoid[g];
   }
   if ((long long)n * h * w == 0) return 0;
@@ -111,8 +123,7 @@ extern "C" int lavb_deconv3x3s2_small(const void* d_in, int dtype, int n, int h,
   LAVB_CUDA_OK(ensure_dyn_smem((const void*)deconv3x3s2_small_kernel<float>, 64 * 1024));
   LAVB_CUDA_OK(ensure_dyn_smem((const void*)deconv3x3s2_small_kernel<h16>, 64 * 1024));
   if (dtype == LAVB_F32) deconv3x3s2_small_kernel<float><<<grid, kTH * kTW, smem, st>>>(a);
-  else if (dtype == LAVB_H16) deconv3x3s2_small_kernel<h16><<<grid, kTH * kTW, smem, st>>>(a);
-  else LAVB_CHECK_ARG(false, "deconv_small: bad dtype");
+  else deconv3x3s2_small_kernel<h16><<<grid, kTH * kTW, smem, st>>>(a);
   LAVB_LAUNCH_OK();
   return 0;
 }

@@ -127,12 +127,13 @@ __global__ void __launch_bounds__(256) rgb_norm_kernel(const void* __restrict__ 
 }
 
 template <typename TS, typename TD>
-__global__ void __launch_bounds__(256) convert_kernel(const TS* __restrict__ s, TD* __restrict__ d, long long count) {
+__global__ void __launch_bounds__(256) convert_kernel(const TS* __restrict__ s, TD* __restrict__ d, long long count, int vec) {
   long long i = ((long long)blockIdx.x * blockDim.x + threadIdx.x) * 4;
-  if (i + 3 < count) {
+  const long long end = i + 4 < count ? i + 4 : count;
+  if (vec && end == i + 4) {
     store4<TD>(d + i, load4<TS>(s + i));
   } else {
-    for (; i < count; ++i) d[i] = from_f32<TD>(to_f32<TS>(s[i]));
+    for (; i < end; ++i) d[i] = from_f32<TD>(to_f32<TS>(s[i]));
   }
 }
 
@@ -458,27 +459,40 @@ extern "C" int lavb_stack_sweep(const float* d_src, int n, int src_cols, const f
 
 extern "C" int lavb_rgb_normalize(const void* d_rgb, int src_is_u8_nhwc, int n, int h, int w, void* d_out, int out_dtype,
                                   void* stream) {
+  LAVB_CHECK_ARG(n >= 0 && h >= 0 && w >= 0, "rgb_normalize: n, h, w must be >= 0");
+  LAVB_CHECK_ARG(out_dtype == LAVB_F32 || out_dtype == LAVB_H16, "rgb_normalize: bad dtype");
   const long long npix = (long long)n * h * w;
   if (npix == 0) return 0;
+  // one 4-channel pixel is stored at a time; the float source is read per element
+  LAVB_CHECK_ARG(d_rgb != nullptr && d_out != nullptr && (src_is_u8_nhwc || reinterpret_cast<uintptr_t>(d_rgb) % 4 == 0) &&
+                     reinterpret_cast<uintptr_t>(d_out) % (out_dtype == LAVB_F32 ? 16 : 8) == 0,
+                 "rgb_normalize: null pointer, or d_out not 4-element aligned (16 B fp32, 8 B 16-bit)");
   const int blocks = ceil_div(npix, 256);
   if (out_dtype == LAVB_F32)
     rgb_norm_kernel<float><<<blocks, 256, 0, (cudaStream_t)stream>>>(d_rgb, src_is_u8_nhwc, n, h, w, (float*)d_out);
   else if (out_dtype == LAVB_H16)
     rgb_norm_kernel<h16><<<blocks, 256, 0, (cudaStream_t)stream>>>(d_rgb, src_is_u8_nhwc, n, h, w, (h16*)d_out);
-  else LAVB_CHECK_ARG(false, "rgb_normalize: bad dtype");
   LAVB_LAUNCH_OK();
   return 0;
 }
 
 extern "C" int lavb_convert(const void* d_src, int src_dtype, void* d_dst, int dst_dtype, long long count, void* stream) {
+  LAVB_CHECK_ARG((src_dtype == LAVB_F32 && dst_dtype == LAVB_H16) || (src_dtype == LAVB_H16 && dst_dtype == LAVB_F32),
+                 "convert: unsupported dtype pair");
+  LAVB_CHECK_ARG(count >= 0, "convert: negative count");
   if (count == 0) return 0;
+  const uintptr_t ss = src_dtype == LAVB_F32 ? 4 : 2, ds = dst_dtype == LAVB_F32 ? 4 : 2;
+  const uintptr_t src = reinterpret_cast<uintptr_t>(d_src), dst = reinterpret_cast<uintptr_t>(d_dst);
+  LAVB_CHECK_ARG(d_src != nullptr && d_dst != nullptr && src % ss == 0 && dst % ds == 0,
+                 "convert: null pointer, or a pointer not aligned to its element size");
+  // 4 elements per thread: vector loads / stores when both pointers are 4-element aligned, element by element otherwise
+  const int vec = src % (4 * ss) == 0 && dst % (4 * ds) == 0;
   const int blocks = ceil_div(ceil_div(count, 4), 256);
   cudaStream_t st = (cudaStream_t)stream;
-  if (src_dtype == LAVB_F32 && dst_dtype == LAVB_H16)
-    convert_kernel<float, h16><<<blocks, 256, 0, st>>>((const float*)d_src, (h16*)d_dst, count);
-  else if (src_dtype == LAVB_H16 && dst_dtype == LAVB_F32)
-    convert_kernel<h16, float><<<blocks, 256, 0, st>>>((const h16*)d_src, (float*)d_dst, count);
-  else LAVB_CHECK_ARG(false, "convert: unsupported dtype pair");
+  if (src_dtype == LAVB_F32)
+    convert_kernel<float, h16><<<blocks, 256, 0, st>>>((const float*)d_src, (h16*)d_dst, count, vec);
+  else
+    convert_kernel<h16, float><<<blocks, 256, 0, st>>>((const h16*)d_src, (float*)d_dst, count, vec);
   LAVB_LAUNCH_OK();
   return 0;
 }
