@@ -418,7 +418,25 @@ int lavb_stack_job_poses(void* d_jobs, int b, int t, int gap, int keep, long lon
  * first `d` columns used).  MLP: Linear(d+5,h1) -> affine(s1,t1) -> ReLU -> Linear(h1,h2) -> affine -> ReLU
  * with d_w1 [h1][d+5], d_w2 [h2][h1] row-major (nn.Linear layout); the affine is BatchNorm1d expressed as
  * y*s+t (bias folded into t).  Output canvas NHWC [B][ny][nx][h2] (row = ny-1-xi, col = yi), fully written.
- * Workspace: lavb_pillar_workspace_bytes(B, nx, ny) bytes, contents irrelevant on entry. */
+ * Workspace: lavb_pillar_workspace_bytes(B, nx, ny) bytes, contents irrelevant on entry.
+ * Grid: a point is kept when min_x <= x < max_x and min_y <= y < max_y on the raw fp32 coordinates (NaN and +-inf are
+ *   dropped); xi = trunc(fp32(fp32(x - min_x) * ppm)), yi likewise.  A pillar is (b, xi, yi) before any clamp; its cell is
+ *   row = clamp(ny-1-xi, 0, ny-1), col = clamp(yi, 0, nx-1).  When two pillars clamp onto one cell (yi == nx by rounding, or
+ *   a grid with nx != ny), the cell holds the per-channel max over the rows of both.  The decorated row is [pt(d) | xyz -
+ *   centroid of its pillar | x - fp32(fp32(yi / ppm) + min_x) | y - fp32(fp32(xi / ppm) + min_y)].
+ * Values: each ReLU is max(a, 0) with NaN -> 0.  A NaN in any decorated column of a point (a NaN z or feature, or an inf z,
+ *   whose z - centroid is inf - inf) makes all its hidden units NaN, hence 0, so the point contributes relu(t2) to its
+ *   cell; a NaN z makes the centroid NaN, so every point of its pillar contributes relu(t2).  lavb_pillar_forward computes
+ *   in fp32 throughout: other infinities propagate as in IEEE arithmetic and may reach the canvas as +inf (never NaN).
+ *   With finite inputs whose fp32 sums stay finite it is accurate to fp32.
+ * The centroid sums are float atomics in an order that varies between calls, so neither encoder is bit-reproducible; results
+ *   differ by the rounding of those sums.
+ * Checked (a rejected call writes nothing): 1 <= batch <= 128, starts and counts >= 0, fewer than 2^31 points; d == 11,
+ *   h1 == h2 == 64, pt_stride >= d; ppm finite and > 0; finite window bounds with min < max; nx, ny >= 1, and the grid holds
+ *   the window: for v the largest fp32 below max_x (max_y), trunc(fp32(fp32(v - min) * ppm)) <= nx (ny); d_pts non-null
+ *   (unless there are no points) and 4-byte aligned; weights, canvas and workspace non-null; w2 8-byte aligned, the other
+ *   weights 4-byte aligned, the workspace 16-byte aligned; the fp32 canvas 4-byte aligned (lavb_pillar_forward) or the canvas
+ *   16-byte aligned (lavb_pillar_forward_sorted).  Not checked: that each cloud lies inside d_pts. */
 size_t lavb_pillar_workspace_bytes(int batch, int nx, int ny);
 int lavb_pillar_forward(const float* d_pts, int pt_stride, int d,
                         const long long* h_cloud_start, const int* h_cloud_count, int batch,
@@ -430,7 +448,12 @@ int lavb_pillar_forward(const float* d_pts, int pt_stride, int d,
 /* Sorted, atomic-free variant for the tensor-core pipeline (the product encoder): counting sort of the points by canvas cell,
  * layer 1 on hi/lo-split h16 operands (~ fp32), layer 2 on h16 operands with fp32 accumulation (mma.sync), one canvas row written
  * per pillar and the rows of empty cells zero-filled by the scan pass.  out_mode 0: fp32 canvas [B][ny][nx][h2]; 2: h16 canvas
- * [B][ny][nx][h2], saturating; any other out_mode is rejected.  Same semantics otherwise. */
+ * [B][ny][nx][h2], saturating; any other out_mode is rejected.  Same semantics otherwise.
+ * Precision: layer 1 splits each decorated value and each w1 weight into an h16 hi and lo part (saturating) and drops lo*lo;
+ *   this is close to fp32 only while the decorated values stay inside the h16 range (|v| < 65504): beyond it the split loses
+ *   the value silently (from 2 * 65504 on, v counts as +-131008), and an infinite decorated value that is not NaN saturates
+ *   the same way instead of propagating.  Layer 2 reads w2 and the hidden activations (after affine and ReLU) rounded to h16, saturating.  The
+ *   fp32 canvas is never NaN; the h16 canvas is the fp32 result rounded once, saturating, so it is always finite. */
 size_t lavb_pillar_sorted_workspace_bytes(int batch, int nx, int ny, long long total_points);
 int lavb_pillar_forward_sorted(const float* d_pts, int pt_stride, int d,
                                const long long* h_cloud_start, const int* h_cloud_count, int batch,
@@ -446,7 +469,7 @@ int lavb_pillar_forward_sorted(const float* d_pts, int pt_stride, int d,
  *          compaction of the in-window points).  A pillar is (b, xi, yi) before any clamp, so a y that rounds to yi == nx
  *          (SURVEY App. C.5) forms its own pillar for the centroid and cell-origin columns, while its cell clamps onto
  *          col nx-1 (an x that rounds up to the last index likewise clamps onto row 0).  pt_stride >= d, 1 <= batch <= 128,
- *          d == 11.
+ *          d == 11; the grid is checked as for lavb_pillar_forward.
  * The Linear/BN1d/ReLU stack then runs on d_feat with autograd; stage 1 max-pools rows into the canvas and
  * records the arg-max row per (cell, channel) for the backward:
  *   precondition: d_h >= 0 (post-ReLU) and 0 <= d_cell[r] < n_cells; m >= 0, c >= 1, n_cells >= 0.

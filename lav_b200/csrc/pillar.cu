@@ -1,6 +1,7 @@
 // PointPillars dynamic voxeliser + pillar encoder (lav/models/point_pillar.py:55-116) without sort/unique:
 // a pillar is addressed directly by (b, xi, yi); pass 1 accumulates the per-pillar centroid sums, pass 2
 // decorates each point, runs the 2-layer point MLP and max-pools into the NHWC canvas.
+#include <math.h>
 #include <stdlib.h>
 #include "common.cuh"
 #include "pillar_grid.cuh"
@@ -274,6 +275,34 @@ static int fill_clouds(Clouds& c, const long long* start, const int* count, int 
 }
 
 static size_t stats_bytes(int batch, int nx, int ny) { return (size_t)batch * (nx + 1) * (ny + 1) * sizeof(float4); }
+
+static bool aligned(const void* p, size_t a) { return (reinterpret_cast<uintptr_t>(p) & (a - 1)) == 0; }
+
+// The grid must hold every point the window keeps: pillar_key addresses xi in [0, nx] and yi in [0, ny].  The largest index is
+// reached by the largest fp32 coordinate below max, computed in the kernel's fp32 arithmetic (trunc(v) <= n  <=>  v < n + 1).
+static int check_grid(const char* who, float min_x, float max_x, float min_y, float max_y, float ppm, int nx, int ny) {
+  LAVB_CHECK_ARG(isfinite(ppm) && ppm > 0.f, "%s: ppm must be finite and > 0 (got %g)", who, ppm);
+  LAVB_CHECK_ARG(isfinite(min_x) && isfinite(max_x) && isfinite(min_y) && isfinite(max_y) && min_x < max_x && min_y < max_y,
+                 "%s: the window must be finite with min < max (got x [%g, %g), y [%g, %g))", who, min_x, max_x, min_y, max_y);
+  LAVB_CHECK_ARG(nx >= 1 && ny >= 1, "%s: nx, ny must be >= 1 (got %d, %d)", who, nx, ny);
+  const float top_x = (nextafterf(max_x, -INFINITY) - min_x) * ppm, top_y = (nextafterf(max_y, -INFINITY) - min_y) * ppm;
+  LAVB_CHECK_ARG((double)top_x < (double)nx + 1.0 && (double)top_y < (double)ny + 1.0,
+                 "%s: the window reaches index (%.0f, %.0f), beyond the grid's (%d, %d)", who, floor(top_x), floor(top_y), nx, ny);
+  return 0;
+}
+
+// pointer checks shared by both encoders: point rows are read as floats, the workspace holds float4 centroid sums
+static int check_encoder_ptrs(const char* who, const float* pts, int total, const float* w1, const float* s1, const float* t1,
+                              const float* w2, const float* s2, const float* t2, const void* canvas, size_t canvas_align,
+                              const void* ws) {
+  LAVB_CHECK_ARG(total == 0 || (pts != nullptr && aligned(pts, 4)), "%s: d_pts must be non-null and 4-byte aligned", who);
+  LAVB_CHECK_ARG(w1 && s1 && t1 && w2 && s2 && t2 && canvas && ws, "%s: null weight, canvas or workspace pointer", who);
+  LAVB_CHECK_ARG(aligned(w1, 4) && aligned(s1, 4) && aligned(t1, 4) && aligned(w2, 8) && aligned(s2, 4) && aligned(t2, 4),
+                 "%s: w2 must be 8-byte aligned, w1 / s1 / t1 / s2 / t2 4-byte aligned", who);
+  LAVB_CHECK_ARG(aligned(canvas, canvas_align) && aligned(ws, 16), "%s: the canvas must be %zu-byte and the workspace 16-byte "
+                 "aligned", who, canvas_align);
+  return 0;
+}
 
 // =====================================================================================================================
 // Sorted (atomic-free canvas) pillar encoder for the tensor-core pipeline.
@@ -650,6 +679,9 @@ extern "C" int lavb_pillar_forward(const float* d_pts, int pt_stride, int d, con
   LAVB_CHECK_ARG(d == 11 && h1 == 64 && h2 == 64, "pillar_forward: only the v2 configuration (D=11, features [64,64]) is built (got D=%d [%d,%d])", d, h1, h2);
   LAVB_CHECK_ARG(canvas_dtype == LAVB_F32, "pillar_forward: canvas must be fp32");
   LAVB_CHECK_ARG(pt_stride >= d, "pillar_forward: pt_stride < d");
+  if (check_grid("pillar_forward", min_x, max_x, min_y, max_y, ppm, nx, ny)) return 1;
+  if (check_encoder_ptrs("pillar_forward", d_pts, clouds.cum[batch], d_w1, d_s1, d_t1, d_w2, d_s2, d_t2, d_canvas, 4, d_workspace))
+    return 1;
   cudaStream_t st = (cudaStream_t)stream;
   Grid g{min_x, max_x, min_y, max_y, ppm, nx, ny};
   float4* stats = reinterpret_cast<float4*>(d_workspace);
@@ -675,6 +707,7 @@ extern "C" int lavb_pillar_decorate(const float* d_pts, int pt_stride, int d, co
   if (fill_clouds(clouds, h_cloud_start, h_cloud_count, batch)) return 1;
   LAVB_CHECK_ARG(d == 11, "pillar_decorate: only D=11 is built (got %d)", d);
   LAVB_CHECK_ARG(pt_stride >= d, "pillar_decorate: pt_stride < d");
+  if (check_grid("pillar_decorate", min_x, max_x, min_y, max_y, ppm, nx, ny)) return 1;
   cudaStream_t st = (cudaStream_t)stream;
   Grid g{min_x, max_x, min_y, max_y, ppm, nx, ny};
   float4* stats = reinterpret_cast<float4*>(d_workspace);
@@ -742,6 +775,10 @@ extern "C" int lavb_pillar_forward_sorted(const float* d_pts, int pt_stride, int
   LAVB_CHECK_ARG(d == 11 && h1 == 64 && h2 == 64, "pillar_forward_sorted: only the v2 configuration (D=11, features [64,64]) is built");
   LAVB_CHECK_ARG(out_mode == 0 || out_mode == 2, "pillar_forward_sorted: out_mode must be 0 (fp32) or 2 (h16) (got %d)", out_mode);
   LAVB_CHECK_ARG(pt_stride >= d, "pillar_forward_sorted: pt_stride < d");
+  if (check_grid("pillar_forward_sorted", min_x, max_x, min_y, max_y, ppm, nx, ny)) return 1;
+  if (check_encoder_ptrs("pillar_forward_sorted", d_pts, clouds.cum[batch], d_w1, d_s1, d_t1, d_w2, d_s2, d_t2, d_canvas, 16,
+                         d_workspace))
+    return 1;
   cudaStream_t st = (cudaStream_t)stream;
   Grid g{min_x, max_x, min_y, max_y, ppm, nx, ny};
   const int total = clouds.cum[batch];

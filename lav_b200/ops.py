@@ -121,11 +121,32 @@ def _workspace(device, nbytes):
     return torch.empty(int(nbytes), dtype=torch.uint8, device=device)
 
 
-def _clouds(starts, counts):
+def _clouds(starts, counts, pts, what):
+    """host arrays of the cloud table; raises LavbError when a cloud reaches past the last row of pts (the kernels read
+    rows start .. start + count - 1 without a bound)."""
     b = len(counts)
-    st = (C.c_longlong * b)(*[int(s) for s in starts])
-    ct = (C.c_int * b)(*[int(c) for c in counts])
+    starts, counts = [int(s) for s in starts], [int(c) for c in counts]
+    if len(starts) != b:
+        raise capi.LavbError(f"{what}: {len(starts)} starts for {b} counts")
+    for i, (s, c) in enumerate(zip(starts, counts)):
+        if c > 0 and s + c > pts.shape[0]:
+            raise capi.LavbError(f"{what}: cloud {i} = rows [{s}, {s + c}) lies past the {pts.shape[0]} rows of pts")
+    st = (C.c_longlong * b)(*starts)
+    ct = (C.c_int * b)(*counts)
     return b, st, ct
+
+
+def _check_point_mlp(what, pts, w1, s1, t1, w2, s2, t2):
+    """the encoders are built for the v2 point MLP only: w1 (64, 16), w2 (64, 64), s / t (64,), contiguous fp32 on pts' device,
+    and rows of pts at least 11 floats wide."""
+    for name, t, shape in (("w1", w1, (64, 16)), ("s1", s1, (64,)), ("t1", t1, (64,)), ("w2", w2, (64, 64)), ("s2", s2, (64,)),
+                           ("t2", t2, (64,))):
+        if (not torch.is_tensor(t) or tuple(t.shape) != shape or t.dtype != torch.float32 or not t.is_contiguous()
+                or t.device != pts.device):
+            got = f"{t.dtype} {tuple(t.shape)}" if torch.is_tensor(t) else type(t).__name__
+            raise capi.LavbError(f"{what}: {name} must be a contiguous fp32 {shape} tensor on {pts.device}, got {got}")
+    if pts.shape[1] < 11:
+        raise capi.LavbError(f"{what}: point rows must hold at least 11 floats, got {pts.shape[1]}")
 
 
 def pillar_forward(pts, starts, counts, grid, w1, s1, t1, w2, s2, t2):
@@ -133,9 +154,10 @@ def pillar_forward(pts, starts, counts, grid, w1, s1, t1, w2, s2, t2):
     Returns the NHWC canvas (B, ny, nx, H2) fp32."""
     _need_cuda(pts, w1, w2)
     assert pts.dtype == torch.float32 and pts.dim() == 2 and pts.stride(1) == 1
+    _check_point_mlp("pillar_forward", pts, w1, s1, t1, w2, s2, t2)
     min_x, max_x, min_y, max_y, ppm, nx, ny = grid
     d = w1.shape[1] - 5
-    b, st, ct = _clouds(starts, counts)
+    b, st, ct = _clouds(starts, counts, pts, "pillar_forward")
     canvas = torch.empty((b, ny, nx, w2.shape[0]), dtype=torch.float32, device=pts.device)
     ws = _workspace(pts.device, lib().lavb_pillar_workspace_bytes(b, nx, ny))
     e0 = _prof_begin()
@@ -153,7 +175,7 @@ def pillar_decorate(pts, starts, counts, grid, d):
     _need_cuda(pts)
     assert pts.dtype == torch.float32 and pts.dim() == 2 and pts.stride(1) == 1
     min_x, max_x, min_y, max_y, ppm, nx, ny = grid
-    b, st, ct = _clouds(starts, counts)
+    b, st, ct = _clouds(starts, counts, pts, "pillar_decorate")
     ws = _workspace(pts.device, lib().lavb_pillar_workspace_bytes(b, nx, ny))
     total = int(sum(int(c) for c in counts))
     feat = torch.empty((total, d + 5), dtype=torch.float32, device=pts.device)
@@ -1180,9 +1202,10 @@ def pillar_forward_sorted(pts, starts, counts, grid, w1, s1, t1, w2, s2, t2, can
     what the 16-bit pipeline feeds the backbone."""
     _need_cuda(pts, w1, w2)
     assert pts.dtype == torch.float32 and pts.dim() == 2 and pts.stride(1) == 1
+    _check_point_mlp("pillar_forward_sorted", pts, w1, s1, t1, w2, s2, t2)
     min_x, max_x, min_y, max_y, ppm, nx, ny = grid
     d = w1.shape[1] - 5
-    b, st, ct = _clouds(starts, counts)
+    b, st, ct = _clouds(starts, counts, pts, "pillar_forward_sorted")
     total = int(sum(int(c) for c in counts))
     h2 = w2.shape[0]
     canvas = torch.empty((b, ny, nx, h2), dtype=h16() if canvas16 else torch.float32, device=pts.device)

@@ -71,12 +71,13 @@ def fmax0(a):
     return torch.where(torch.isnan(a), torch.zeros_like(a), a.clamp_min(0))
 
 
-def kernels(fn, tmp_path):
-    """run fn under torch.profiler; the (name, grid) of every kernel it launched.  Every call traced here is idempotent (same
-    outputs, same elements written), so a capture in which the profiler recorded no kernel at all, which happens now and
-    then with short captures, is taken again.  A kernel record can also arrive in the capture after its own; kernels are
-    therefore kept only when their launch (matched by correlation id) was recorded in this capture."""
-    for _ in range(3):
+def kernels(fn, tmp_path, tries=5):
+    """run fn under torch.profiler; the (name, grid) of every kernel it launched, in launch order.  Every call traced here
+    is idempotent (same outputs, same elements written), so fn may be traced more than once.  The profiler's kernel
+    records can be missing from a short capture and arrive in a later one, so the kernel records of all captures are pooled
+    by correlation id, and the first capture in which every kernel launch has its kernel record is the answer."""
+    records, captures = {}, []
+    for _ in range(tries):
         torch.cuda.synchronize()
         with profile(activities=[ProfilerActivity.CPU, ProfilerActivity.CUDA]) as prof:
             fn()
@@ -86,13 +87,15 @@ def kernels(fn, tmp_path):
         with open(path) as f:
             events = json.load(f)["traceEvents"]
         os.remove(path)
-        launches = {e["args"]["correlation"] for e in events
-                    if e.get("cat") in ("cuda_runtime", "cuda_driver") and "correlation" in e.get("args", {})}
-        found = [(e["name"], e.get("args", {}).get("grid")) for e in events if e.get("cat") == "kernel"
-                 and (not launches or e.get("args", {}).get("correlation") in launches)]
-        if found:
-            break
-    return found
+        captures.append([e["args"]["correlation"] for e in events
+                         if e.get("cat") in ("cuda_runtime", "cuda_driver") and "Launch" in e.get("name", "")
+                         and "correlation" in e.get("args", {})])
+        records.update({e["args"]["correlation"]: (e["name"], e["args"].get("grid")) for e in events
+                        if e.get("cat") == "kernel" and "correlation" in e.get("args", {})})
+        for launches in captures:
+            if launches and all(c in records for c in launches):
+                return [records[c] for c in launches]
+    return []
 
 
 def num_sms():
