@@ -410,6 +410,47 @@ int lavb_agent_nav_update(int b, const float* d_control, const double* d_speed, 
 int lavb_stack_job_poses(void* d_jobs, int b, int t, int gap, int keep, long long tick, double* d_ring_pose, const double* d_poses,
                          void* stream);
 
+/* ---------------------------------------------------------------- the agent's debug view
+ * stands behind: LAVAgent.visualize (lav_agent_fast.py:459-518, lidar_to_bev :567-581) without its text, the frame run_step keeps
+ * every tick, for b agents in one memset and four launches (the points launch once per 256 agents, the boxes launch once per
+ * 96 drawn boxes).  Bit for bit with numpy and OpenCV's 8-bit arithmetic; oracle/view_ref.py states it.  Per agent i:
+ *   1. the LiDAR view: np.histogramdd of the (x, y) of d_points' rows over linspace(-10, 71, 321) x linspace(-40, 41, 321) (fp64
+ *      edges, a value on the last edge in the last bin, NaN / inf / outside rows dropped), clamped at 10, / 10 * 255 in fp64,
+ *      truncated; rows flipped; grey to RGB.
+ *   2. the drawing on it, later draws overwriting earlier ones: each plan point (d_cast when d_cmd[i] is 4 or 5, else d_plan) a
+ *      radius-1 dot (255, 0, 0); each step of each forecast branch scoring >= cmd_thresh a radius-1 dot in jet[row], row the
+ *      matplotlib Colormap row of the fp32 score (x 256, 256 -> 255, under 256, over 257, NaN 258); each box an outline of
+ *      thickness 2 (255, 0, 0) as cv2.drawContours draws it; the target a radius-2 dot (0, 255, 0) at clip(ego + tgt * ppm,
+ *      0, 255).  A point's pixel is (160, 280) + (float)(loc * (float)ppm) in fp64, truncated; a point or target that is NaN or
+ *      outside int32 is not drawn, nor a box whose corners are.
+ *   3. the predicted BEV: (255 * mean_c sigmoid(logit)) in fp32 (sigmoid = 1 / (1 + expf(-x)), channels summed in order,
+ *      divided by c), truncated; NaN -> 0.
+ *   4. cv2.resize INTER_LINEAR of the three cameras (288 x 768 -> 320 x 853) and of the tele view (192 x 480 -> 320 x 800),
+ *      the canvas [cameras | tele | LiDAR view | BEV] (320 x 2293) and its resize to 160 x 1146.
+ * Inputs: d_rgbs (b, 3, 288, 256, 3) uint8, the cameras in order; d_tels (b, 192, 480, 3) uint8; d_points (b, p, point_stride)
+ *   fp32, x and y in columns 0 and 1 (NaN rows are padding); d_bev the logits (b, c, 320, 320) fp32 (LAVB_F32) or the 16-bit
+ *   type, element strides h_bev_strides[4] = (b, c, y, x); d_plan / d_cast (b, t, 2) fp32; d_cmd (b,) int32; forecast rows
+ *   d_other_locs (k, m, t, 2) / d_other_cmds (k, m) fp32, agent i owning rows [h_offsets[i], h_offsets[i+1]); boxes h_boxes
+ *   (n_boxes, 6) HOST fp64 (x, y, w, h, cos, sin) in BEV pixels, agent i owning rows [h_box_offsets[i], h_box_offsets[i+1])
+ *   (HOST int32[b+1], monotone); d_target (b, 2) fp32 = [-wx, -wy]; *h_config read during the call.  1 <= t <= 64, 1 <= m <= 8,
+ *   1 <= c <= 64, b <= 65535; pixels_per_meter positive and exact in fp32.
+ * d_scratch: lavb_agent_view_scratch_bytes(b) bytes, 8-byte aligned, overwritten.  d_out (b, 160, 1146, 3) uint8, every byte of
+ * the b frames written.  A rejected call writes nothing.  The row offsets, the boxes' corners (computed here in fp64) and the
+ * config travel as kernel arguments: a captured graph replays those of the capture. */
+#define LAVB_VIEW_JET_ROWS 259
+typedef struct lavb_view_config {
+  double pixels_per_meter, cmd_thresh;
+  unsigned char jet[LAVB_VIEW_JET_ROWS * 3];   /* (int(r * 255), int(g * 255), int(b * 255)) of matplotlib's jet: 256 colours,
+                                                  then its under, over and bad rows */
+} lavb_view_config;
+
+size_t lavb_agent_view_scratch_bytes(int b);
+int lavb_agent_view(const unsigned char* d_rgbs, const unsigned char* d_tels, const float* d_points, int b, long long p,
+                    int point_stride, const void* d_bev, int bev_dtype, int bev_c, const long long* h_bev_strides, const float* d_plan,
+                    const float* d_cast, const int* d_cmd, int t, const float* d_other_locs, const float* d_other_cmds, int k, int m,
+                    const int* h_offsets, const double* h_boxes, int n_boxes, const int* h_box_offsets, const float* d_target,
+                    const lavb_view_config* h_config, void* d_scratch, size_t scratch_bytes, unsigned char* d_out, void* stream);
+
 /* ---------------------------------------------------------------- PointPillars voxeliser + pillar encoder
  * replaces: PointPillarNet.forward (lav/models/point_pillar.py:92-116) incl. grid_locations :70-79,
  *           pillar_generation/decorate :55-68,81-85, DynamicPointNet.forward :28-35 (torch_scatter

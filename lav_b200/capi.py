@@ -53,6 +53,11 @@ class ControlConfig(C.Structure):
     ]
 
 
+class ViewConfig(C.Structure):
+    """mirror of lavb_view_config"""
+    _fields_ = [("pixels_per_meter", C.c_double), ("cmd_thresh", C.c_double), ("jet", C.c_ubyte * (259 * 3))]
+
+
 _SIGS = {
     "lavb_abi_version": (C.c_int, []),
     "lavb_last_error": (C.c_char_p, []),
@@ -107,6 +112,11 @@ _SIGS = {
     "lavb_agent_nav_update": (C.c_int, [C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "lavb_stack_job_poses": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_longlong, C.c_void_p, C.c_void_p,
                                        C.c_void_p]),
+    "lavb_agent_view_scratch_bytes": (C.c_size_t, [C.c_int]),
+    "lavb_agent_view": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_longlong, C.c_int, C.c_void_p, C.c_int, C.c_int,
+                                  C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_int,
+                                  C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.POINTER(ViewConfig), C.c_void_p,
+                                  C.c_size_t, C.c_void_p, C.c_void_p]),
     "lavb_roof_filter": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_longlong, C.c_void_p, C.c_longlong, C.c_void_p, C.c_int,
                                    C.c_void_p]),
     "lavb_stack_sweep": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_float, C.c_float, C.c_int, C.c_int, C.c_int,

@@ -1406,3 +1406,78 @@ def cast_gru(embd, wih_t, whh_t, bih, bhh, wmlp, bmlp, steps):
                               _ptr(out), _stream()), "lavb_cast_gru")
     _COUNT[0] += 1
     return out
+
+
+def agent_view_scratch_bytes(b):
+    """bytes of agent_view's scratch for b agents (lavb_agent_view_scratch_bytes)."""
+    return int(lib().lavb_agent_view_scratch_bytes(int(b)))
+
+
+def agent_view(rgbs, tels, points, bev, plan, cast, cmds, other_locs, other_cmds, offsets, boxes, box_offsets, target, config,
+               scratch=None, out=None):
+    """The agents' debug frames, visualize's canvas before its text, in one memset and four launches (see lavb_agent_view in
+    include/lav_b200.h): rgbs (B, 3, 288, 256, 3) / tels (B, 192, 480, 3) uint8; points (B, P, S) fp32 rows with x, y first (NaN
+    rows are padding); bev (B, C, 320, 320) fp32 or 16-bit logits, any strides; plan / cast (B, T, 2) fp32; cmds (B,) int32;
+    other_locs (K, M, T, 2) / other_cmds (K, M) fp32 the forecast rows, agent i owning rows [offsets[i], offsets[i+1]) (offsets
+    (B+1,) int32 on the HOST); boxes (NB, 6) fp64 on the HOST, (x, y, w, h, cos, sin) in BEV pixels, agent i owning rows
+    [box_offsets[i], box_offsets[i+1]); target (B, 2) fp32; config a capi.ViewConfig; scratch a uint8 device tensor of at least
+    agent_view_scratch_bytes(B) bytes.  -> out (B, 160, 1146, 3) uint8, written into ``out`` when given."""
+    _need_cuda(rgbs, tels, points, bev, plan, cast, cmds, other_locs, other_cmds, target, scratch, out)
+    f32 = lambda x, shape: x.dtype == torch.float32 and tuple(x.shape) == shape and x.is_contiguous()
+    if rgbs.dtype != torch.uint8 or rgbs.dim() != 5 or tuple(rgbs.shape[1:]) != (3, 288, 256, 3) or not rgbs.is_contiguous():
+        raise capi.LavbError(f"agent_view: rgbs must be a contiguous (B, 3, 288, 256, 3) uint8 tensor, got {rgbs.dtype} {tuple(rgbs.shape)}")
+    b = rgbs.shape[0]
+    if tels.dtype != torch.uint8 or tuple(tels.shape) != (b, 192, 480, 3) or not tels.is_contiguous():
+        raise capi.LavbError(f"agent_view: tels must be a contiguous ({b}, 192, 480, 3) uint8 tensor, got {tels.dtype} {tuple(tels.shape)}")
+    if points.dtype != torch.float32 or points.dim() != 3 or points.shape[0] != b or points.shape[2] < 2 or not points.is_contiguous():
+        raise capi.LavbError(f"agent_view: points must be a contiguous ({b}, P, >= 2) fp32 tensor, got {points.dtype} {tuple(points.shape)}")
+    if bev.dtype not in (torch.float32, h16()) or bev.dim() != 4 or bev.shape[0] != b or tuple(bev.shape[2:]) != (320, 320):
+        raise capi.LavbError(f"agent_view: bev must be ({b}, C, 320, 320) fp32 or {h16()} logits, got {bev.dtype} {tuple(bev.shape)}")
+    if plan.dtype != torch.float32 or plan.dim() != 3 or plan.shape[0] != b or plan.shape[2] != 2 or not plan.is_contiguous():
+        raise capi.LavbError(f"agent_view: plan must be a contiguous ({b}, T, 2) fp32 tensor, got {plan.dtype} {tuple(plan.shape)}")
+    t = plan.shape[1]
+    if not f32(cast, (b, t, 2)) or not f32(target, (b, 2)):
+        raise capi.LavbError(f"agent_view: cast ({b}, {t}, 2) and target ({b}, 2) must be contiguous fp32 tensors, got "
+                             f"{tuple(cast.shape)} and {tuple(target.shape)}")
+    if cmds.dtype != torch.int32 or tuple(cmds.shape) != (b,) or not cmds.is_contiguous():
+        raise capi.LavbError(f"agent_view: cmds must be a contiguous ({b},) int32 tensor, got {cmds.dtype} {tuple(cmds.shape)}")
+    if other_locs.dim() != 4 or not f32(other_locs, (other_locs.shape[0], other_locs.shape[1], t, 2)):
+        raise capi.LavbError(f"agent_view: other_locs must be a contiguous (K, M, {t}, 2) fp32 tensor, got {other_locs.dtype} "
+                             f"{tuple(other_locs.shape)}")
+    k, m = other_locs.shape[:2]
+    if not f32(other_cmds, (k, m)):
+        raise capi.LavbError(f"agent_view: other_cmds must be a contiguous ({k}, {m}) fp32 tensor, got {other_cmds.dtype} "
+                             f"{tuple(other_cmds.shape)}")
+    offsets = np.ascontiguousarray(offsets.numpy() if torch.is_tensor(offsets) else offsets)
+    box_offsets = np.ascontiguousarray(box_offsets.numpy() if torch.is_tensor(box_offsets) else box_offsets)
+    for name, o in (("offsets", offsets), ("box_offsets", box_offsets)):
+        if o.dtype != np.int32 or o.shape != (b + 1,):
+            raise capi.LavbError(f"agent_view: {name} must be a host ({b + 1},) int32 array, got {o.dtype} {o.shape}")
+    boxes = np.ascontiguousarray(boxes.numpy() if torch.is_tensor(boxes) else boxes)
+    if boxes.dtype != np.float64 or boxes.ndim != 2 or boxes.shape[1] != 6:
+        raise capi.LavbError(f"agent_view: boxes must be a host (NB, 6) fp64 array, got {boxes.dtype} {boxes.shape}")
+    if not isinstance(config, capi.ViewConfig):
+        raise capi.LavbError("agent_view: config must be a capi.ViewConfig")
+    dev = rgbs.device
+    if len({dev, tels.device, points.device, bev.device, plan.device, cast.device, cmds.device, other_locs.device,
+            other_cmds.device, target.device}) != 1:
+        raise capi.LavbError("agent_view: the inputs must be on one device")
+    need = agent_view_scratch_bytes(b)
+    if scratch is None:
+        scratch = torch.empty((need,), dtype=torch.uint8, device=dev)
+    elif scratch.dtype != torch.uint8 or scratch.numel() < need or not scratch.is_contiguous() or scratch.device != dev:
+        raise capi.LavbError(f"agent_view: scratch must be a contiguous uint8 tensor of >= {need} bytes on {dev}")
+    if out is None:
+        out = torch.empty((b, 160, 1146, 3), dtype=torch.uint8, device=dev)
+    elif out.dtype != torch.uint8 or tuple(out.shape) != (b, 160, 1146, 3) or not out.is_contiguous() or out.device != dev:
+        raise capi.LavbError(f"agent_view: out must be a contiguous ({b}, 160, 1146, 3) uint8 tensor on {dev}")
+    strides = (C.c_longlong * 4)(*bev.stride())
+    ip = lambda a: a.ctypes.data_as(C.c_void_p)
+    code = F32 if bev.dtype == torch.float32 else capi.h16_code()
+    check(lib().lavb_agent_view(_ptr(rgbs), _ptr(tels), _ptr(points), b, points.shape[1], points.shape[2], _ptr(bev), code,
+                                bev.shape[1], strides, _ptr(plan), _ptr(cast), _ptr(cmds), t, _ptr(other_locs), _ptr(other_cmds),
+                                k, m, ip(offsets), ip(boxes) if boxes.size else None, boxes.shape[0], ip(box_offsets), _ptr(target),
+                                C.byref(config), _ptr(scratch), scratch.numel(), _ptr(out), _stream()), "lavb_agent_view")
+    if b:    # histogram, points per 256 agents, boxes per 96 (at most), compose
+        _COUNT[0] += int(points.shape[1] > 0) + -(-b // 256) + -(-int(box_offsets[b] - box_offsets[0]) // 96) + 1
+    return out
