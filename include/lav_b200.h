@@ -605,11 +605,27 @@ int lavb_rgb_normalize(const void* d_rgb, int src_is_u8_nhwc, int n, int h, int 
  * lav/models/resnet.py:178,235-238).  d_img: uint8 (batch, ncam, h, cam_w, 3) — the logical image is the ncam cameras side by
  * side (h x ncam*cam_w), ncam <= 4, cam_w % 4 == 0; d_w: BatchNorm-folded weights h16 [64][160] with
  * k = ky*22 + kx*3 + c (slot 21 of every window row and k >= 154 are zero); d_bias [64]; h_mean/h_std: the 3 ImageNet
- * constants; d_out: h16 NHWC (batch, h/2, ncam*cam_w/2, 64). */
+ * constants; d_out: h16 NHWC (batch, (h-1)/2+1, (ncam*cam_w-1)/2+1, 64), every element written.
+ * The staged operand is fmaf(u8, na, nb) in fp32 with na = 1.f / (255.f * std), nb = -mean / std computed in fp32 on the host,
+ * then rounded to h16; products with the h16 weights are summed in fp32 on the tensor cores; then + bias, ReLU = fmaxf(a, 0)
+ * and a saturating h16 store.  The fp32 operand differs from the reference's (x / 255 - mean) / std by at most a few fp32
+ * ulps, so an h16 operand can land one h16 ulp away from the reference's rounding.
+ * Checked before any launch (a rejected call writes nothing): batch >= 0 (0 writes nothing), 1 <= ncam <= 4, h >= 7,
+ * cam_w >= 8 and a multiple of 4; the grid fits (batch * ceil(ho / 8) < 2^31, ceil(wo / 128) <= 65535); otherwise non-null
+ * pointers, d_img / d_w / d_bias 4-byte and d_out 16-byte aligned, d_out not overlapping d_img, d_w or d_bias (every block
+ * reads them first), and mean / std giving a finite na, nb with std != 0. */
 int lavb_stem7x7s2_u8(const void* d_img, int batch, int ncam, int h, int cam_w, const void* d_w, const float* d_bias,
                       const float* h_mean, const float* h_std, void* d_out, void* stream);
 /* replaces: ResNet.maxpool = MaxPool2d(3, 2, 1) (lav/models/resnet.py:181,238) on h16 NHWC (n, h, w, c), c % 8 == 0
- * -> (n, (h-1)/2+1, (w-1)/2+1, c). */
+ * -> (n, (h-1)/2+1, (w-1)/2+1, c), every element written.  The result is the window's maximum, exactly; pixels off the map
+ * are skipped.  A NaN anywhere in the window gives a NaN, as MaxPool2d propagates NaN: the canonical 0x7FFF when the window
+ * holds two or more pixels; on a 1 x 1 map, whose windows hold one pixel, that pixel is copied, NaN payload and sign
+ * included.  One rule
+ * departs from MaxPool2d: when the maximum is zero and the window holds both -0 and +0 the result is +0, where MaxPool2d
+ * keeps whichever comes first in the window.
+ * Checked before any launch (a rejected call writes nothing): n >= 0 (0 writes nothing), h, w >= 1, c a positive multiple
+ * of 8, fewer than 2^31 blocks of 256 output vectors; otherwise non-null, 16-byte aligned d_in and d_out that do not
+ * overlap. */
 int lavb_maxpool3x3s2_nhwc(const void* d_in, int n, int h, int w, int c, void* d_out, void* stream);
 
 /* ---------------------------------------------------------------- detection decode (device part)
@@ -725,7 +741,14 @@ int lavb_conv_pair_set_trace(void* d_buf, int tiles_per_cta);
  * DownsamplerBlock(3, 16): relu(bn(cat[conv3x3 s2 p1 (13 ch), maxpool2x2 (3 ch)])) (lav/models/erfnet.py:12-23,67).
  * d_rgb_u8: uint8 NHWC (n, h, w, 3); h_w27x16: host fp32 [(ky*3+kx)*3+c][16] conv weights (columns >= 13 zero); h_scale16 /
  * h_shift16: host fp32 [16], epi(a) = relu(a * scale + shift) with the conv bias folded into the first 13 shifts; d_out: NHWC
- * (n, h/2, w/2, 16) fp32 or h16. */
+ * (n, h/2, w/2, 16) fp32 or h16, every element written.  Arithmetic: the normalised value is the fp32 (v / 255 - .5) * 2 of
+ * the reference (three roundings); each conv channel is a 27-term fp32 fmaf chain in (ky, kx, c) order over the zero-padded
+ * normalised image, then relu(fmaf(acc, scale, shift)); the pooled channels are relu(fmaf(max of 4, scale, shift)); the h16
+ * output is that fp32 value rounded once, saturating.  Weight columns 13..15 are never read.  ReLU is fmaxf(a, 0), so a NaN
+ * that reaches one (a NaN weight, scale or shift) comes out as 0.
+ * Checked before any launch (a rejected call writes nothing): n >= 0 (0 writes nothing), h, w even and >= 2, out_dtype
+ * LAVB_F32 or the 16-bit type, fewer than 2^31 blocks of 8 x 32 output pixels; otherwise non-null pointers, d_out 16-byte
+ * (fp32) or 8-byte (h16) aligned and not overlapping d_rgb_u8. */
 int lavb_erf_stem(const void* d_rgb_u8, int n, int h, int w, const float* h_w27x16, const float* h_scale16,
                   const float* h_shift16, void* d_out, int out_dtype, void* stream);
 
@@ -733,15 +756,29 @@ int lavb_erf_stem(const void* d_rgb_u8, int n, int h, int w, const float* h_w27x
  * replaces: Encoder.layers[0] = DownsamplerBlock(16, 64) (lav/models/erfnet.py:12-23,71): relu(bn(cat[conv3x3 s2 p1 (16 -> 48),
  * maxpool2x2 (16)])).  d_in: h16 NHWC (n, h, w, 16), h and w even, w <= 128; d_out: h16 NHWC (n, h/2, w/2, 64); d_w9: fp32
  * [9 taps (ky*3+kx)][16 cin][48 cout]; d_st: fp32 [64][2] = (scale, shift), epi(a) = relu(a * scale + shift) with the conv bias
- * folded into the first 48 shifts (the last 16 apply to the pooled channels, after the max). */
+ * folded into the first 48 shifts (the last 16 apply to the pooled channels, after the max).  Every output element is written.
+ * Arithmetic: the weights are rounded to h16; the conv channels sum the 144 products in fp32 on the tensor cores, then
+ * relu(fmaf(acc, scale, shift)) and a saturating h16 store; the pooled channels take the exact max of the four h16 inputs.
+ * NaN rules: ReLU is fmaxf(a, 0), so a conv channel whose window holds a NaN comes out as 0.  The pool starts from -inf and
+ * uses fmaxf, so it skips a NaN; a window of four NaNs gives -inf, which the affine and ReLU turn into 0 (scale > 0) or
+ * +inf, stored as 65504 (scale < 0).
+ * Checked before any launch (a rejected call writes nothing): n >= 0 (0 writes nothing), h, w even and >= 2, w <= 128,
+ * n * ceil(h / 8) < 2^31; otherwise non-null pointers, d_in / d_out 16-byte and d_w9 / d_st 4-byte aligned, d_out not
+ * overlapping d_in, d_w9 or d_st. */
 int lavb_erf_down16(const void* d_in, void* d_out, int n, int h, int w, const float* d_w9, const float* d_st, void* stream);
 
 /* ---------------------------------------------------------------- fused 16-channel non_bottleneck_1d block
  * replaces: non_bottleneck_1d(16, dropprob, dilated=1) of the ERFNet decoder (lav/models/erfnet.py:37-63, Decoder layers 4 and 5) —
  * conv3x1 -> ReLU -> conv1x3 -> bn1 -> ReLU -> conv3x1 -> ReLU -> conv1x3 -> bn2 -> (+ input) -> ReLU — in one kernel, all four
- * intermediates in shared memory.  d_in / d_out: h16 NHWC (n, h, w, 16), distinct buffers, w % 16 == 0; d_w4: fp32
+ * intermediates in shared memory.  d_in / d_out: h16 NHWC (n, h, w, 16), w % 16 == 0; d_w4: fp32
  * [4 convs][3 taps][16 cin][16 cout]; d_st: fp32 [4 convs][16 cout][2] = (scale, shift) with epi(a) = relu(a * scale + shift)
- * (conv bias folded into shift; scale = 1 for the two convs that have no BatchNorm). */
+ * (conv bias folded into shift; scale = 1 for the two convs that have no BatchNorm).  Every output element is written.
+ * Arithmetic: the weights are rounded to h16; each conv sums its 48 products in fp32 on the tensor cores, then fmaf(acc,
+ * scale, shift), [+ the input x for the last conv, one fp32 add], ReLU, and each intermediate is stored as saturating h16.
+ * NaN rule: every ReLU is fmaxf(a, 0), so a NaN that reaches one comes out as 0; an output is never NaN.
+ * Checked before any launch (a rejected call writes nothing): n >= 0 (0 writes nothing), h >= 1, 16 <= w <= 256,
+ * n * ceil(h / 8) < 2^31; otherwise non-null pointers, d_in / d_out 16-byte, d_w4 4-byte and d_st 8-byte aligned, and
+ * d_out not overlapping d_in (halo rows of neighbouring tiles are re-read), d_w4 or d_st (every block reads them first). */
 int lavb_erf_nb16(const void* d_in, void* d_out, int n, int h, int w, const float* d_w4, const float* d_st, void* stream);
 
 /* ---------------------------------------------------------------- motion-forecast ("cast") heads in one launch

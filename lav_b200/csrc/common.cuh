@@ -88,6 +88,13 @@ __device__ __forceinline__ float2 h1622float2(h162 v) { return unpack_h16(*reint
 
 static inline int ceil_div(long long a, long long b) { return (int)((a + b - 1) / b); }
 
+// host-side argument checks: pointer alignment, and whether the byte ranges [a, a + na) and [b, b + nb) share a byte
+static inline bool is_aligned(const void* p, size_t a) { return (reinterpret_cast<uintptr_t>(p) & (a - 1)) == 0; }
+static inline bool ranges_overlap(const void* a, size_t na, const void* b, size_t nb) {
+  const uintptr_t x = reinterpret_cast<uintptr_t>(a), y = reinterpret_cast<uintptr_t>(b);
+  return na > 0 && nb > 0 && x < y + nb && y < x + na;
+}
+
 template <typename T> __device__ __forceinline__ float to_f32(T v);
 template <> __device__ __forceinline__ float to_f32<float>(float v) { return v; }
 template <> __device__ __forceinline__ float to_f32<h16>(h16 v) { return h162float(v); }

@@ -11,6 +11,8 @@
 // Shared-memory row layout: (W + 2) pixels of 32 B (one zero guard pixel on each side = the horizontal zero padding); the two
 // 16-byte halves of a pixel are swapped when bit 2 of the pixel index is set, which makes both the ldmatrix row reads and the
 // fragment-layout epilogue stores bank-conflict free.
+#include <climits>
+
 #include "common.cuh"
 
 namespace lavb {
@@ -360,14 +362,21 @@ using namespace lavb;
 
 extern "C" int lavb_erf_nb16(const void* d_in, void* d_out, int n, int h, int w, const float* d_w4, const float* d_st, void* stream) {
   LAVB_CHECK_ARG(n >= 0 && h >= 1 && w >= 16 && w % 16 == 0 && w <= 256, "erf_nb16: width must be a multiple of 16, <= 256 (got %d)", w);
-  LAVB_CHECK_ARG(d_in != d_out, "erf_nb16: in-place is not supported (halo rows of neighbouring tiles are re-read)");
+  const int tiles_y = (h + kNbRowsOut - 1) / kNbRowsOut;
+  LAVB_CHECK_ARG((long long)n * tiles_y <= INT_MAX, "erf_nb16: %d images of %d rows need more than 2^31 - 1 blocks", n, h);
   if (n == 0) return 0;
+  LAVB_CHECK_ARG(d_in && d_out && d_w4 && d_st, "erf_nb16: null pointer");
+  LAVB_CHECK_ARG(is_aligned(d_in, 16) && is_aligned(d_out, 16) && is_aligned(d_w4, 4) && is_aligned(d_st, 8),
+                 "erf_nb16: d_in and d_out must be 16-byte, d_w4 4-byte and d_st 8-byte aligned");
+  const size_t bytes = (size_t)n * h * w * 16 * sizeof(h16);
+  LAVB_CHECK_ARG(!ranges_overlap(d_in, bytes, d_out, bytes), "erf_nb16: d_out overlaps d_in (halo rows of neighbouring tiles are re-read)");
+  LAVB_CHECK_ARG(!ranges_overlap(d_w4, 4 * 3 * 16 * 16 * sizeof(float), d_out, bytes) && !ranges_overlap(d_st, 4 * 16 * 2 * sizeof(float), d_out, bytes),
+                 "erf_nb16: d_out overlaps d_w4 or d_st (every block reads them at its start)");
   Nb16Args a;
   a.in = reinterpret_cast<const h16*>(d_in); a.out = reinterpret_cast<h16*>(d_out);
   a.n = n; a.h = h; a.w = w; a.w4 = d_w4; a.st = d_st;
   const int smem = 2 * kNbRows * (w + 2) * 32;
   LAVB_CUDA_OK(ensure_dyn_smem((const void*)erf_nb16_kernel, smem));
-  const int tiles_y = (h + kNbRowsOut - 1) / kNbRowsOut;
   erf_nb16_kernel<<<n * tiles_y, kNbThreads, smem, (cudaStream_t)stream>>>(a);
   LAVB_LAUNCH_OK();
   return 0;
@@ -376,29 +385,44 @@ extern "C" int lavb_erf_nb16(const void* d_in, void* d_out, int n, int h, int w,
 extern "C" int lavb_erf_stem(const void* d_rgb_u8, int n, int h, int w, const float* h_w27x16, const float* h_scale16,
                              const float* h_shift16, void* d_out, int out_dtype, void* stream) {
   LAVB_CHECK_ARG(n >= 0 && h >= 2 && w >= 2 && h % 2 == 0 && w % 2 == 0, "erf_stem: image size must be even");
+  LAVB_CHECK_ARG(out_dtype == LAVB_F32 || out_dtype == LAVB_H16, "erf_stem: output dtype must be fp32 or h16");
+  const long long blocks = (long long)n * ceil_div(h / 2, kSt_OH) * ceil_div(w / 2, kSt_OW);
+  LAVB_CHECK_ARG(blocks <= INT_MAX, "erf_stem: %d images of %d x %d need more than 2^31 - 1 blocks", n, h, w);
   if (n == 0) return 0;
+  LAVB_CHECK_ARG(d_rgb_u8 && d_out && h_w27x16 && h_scale16 && h_shift16, "erf_stem: null pointer");
+  const size_t esize = out_dtype == LAVB_F32 ? sizeof(float) : sizeof(h16);
+  LAVB_CHECK_ARG(is_aligned(d_out, 4 * esize), "erf_stem: d_out must be %d-byte aligned", (int)(4 * esize));
+  LAVB_CHECK_ARG(!ranges_overlap(d_rgb_u8, (size_t)n * h * w * 3, d_out, (size_t)n * (h / 2) * (w / 2) * 16 * esize),
+                 "erf_stem: d_out overlaps d_rgb_u8");
   StemW k;
   memcpy(k.w, h_w27x16, sizeof(k.w));
   memcpy(k.s, h_scale16, sizeof(k.s));
   memcpy(k.t, h_shift16, sizeof(k.t));
-  const int blocks = n * ceil_div(h / 2, kSt_OH) * ceil_div(w / 2, kSt_OW);
   const unsigned char* img = reinterpret_cast<const unsigned char*>(d_rgb_u8);
-  if (out_dtype == LAVB_F32) erf_stem_kernel<float><<<blocks, kSt_OH * kSt_OW, 0, (cudaStream_t)stream>>>(img, n, h, w, k, (float*)d_out);
-  else if (out_dtype == LAVB_H16) erf_stem_kernel<h16><<<blocks, kSt_OH * kSt_OW, 0, (cudaStream_t)stream>>>(img, n, h, w, k, (h16*)d_out);
-  else LAVB_CHECK_ARG(false, "erf_stem: output dtype must be fp32 or h16");
+  if (out_dtype == LAVB_F32) erf_stem_kernel<float><<<(int)blocks, kSt_OH * kSt_OW, 0, (cudaStream_t)stream>>>(img, n, h, w, k, (float*)d_out);
+  else erf_stem_kernel<h16><<<(int)blocks, kSt_OH * kSt_OW, 0, (cudaStream_t)stream>>>(img, n, h, w, k, (h16*)d_out);
   LAVB_LAUNCH_OK();
   return 0;
 }
 
 extern "C" int lavb_erf_down16(const void* d_in, void* d_out, int n, int h, int w, const float* d_w9, const float* d_st, void* stream) {
   LAVB_CHECK_ARG(n >= 0 && h >= 2 && w >= 2 && h % 2 == 0 && w % 2 == 0 && w <= 2 * kDnCols, "erf_down16: even input size, width <= %d (got %d x %d)", 2 * kDnCols, h, w);
+  const int tiles_y = ceil_div(h / 2, kDnRows);
+  LAVB_CHECK_ARG((long long)n * tiles_y <= INT_MAX, "erf_down16: %d images of %d rows need more than 2^31 - 1 blocks", n, h);
   if (n == 0) return 0;
+  LAVB_CHECK_ARG(d_in && d_out && d_w9 && d_st, "erf_down16: null pointer");
+  LAVB_CHECK_ARG(is_aligned(d_in, 16) && is_aligned(d_out, 16) && is_aligned(d_w9, 4) && is_aligned(d_st, 4),
+                 "erf_down16: d_in and d_out must be 16-byte, d_w9 and d_st 4-byte aligned");
+  const size_t out_bytes = (size_t)n * (h / 2) * (w / 2) * 64 * sizeof(h16);
+  LAVB_CHECK_ARG(!ranges_overlap(d_in, (size_t)n * h * w * 16 * sizeof(h16), d_out, out_bytes), "erf_down16: d_out overlaps d_in");
+  LAVB_CHECK_ARG(!ranges_overlap(d_w9, 9 * 16 * 48 * sizeof(float), d_out, out_bytes) && !ranges_overlap(d_st, 64 * 2 * sizeof(float), d_out, out_bytes),
+                 "erf_down16: d_out overlaps d_w9 or d_st (every block reads them at its start)");
   Dn16Args a;
   a.in = reinterpret_cast<const h16*>(d_in); a.out = reinterpret_cast<h16*>(d_out);
   a.n = n; a.h = h; a.w = w; a.w9 = d_w9; a.st = d_st;
   const int smem = kDnInRows * kDnRowPix * 32 + 9 * 48 * 16 * 2 + kDnRows * kDnCols * 128 + 128 * 4;
   LAVB_CUDA_OK(ensure_dyn_smem((const void*)erf_down16_kernel, smem));
-  erf_down16_kernel<<<n * ceil_div(h / 2, kDnRows), kDnThreads, smem, (cudaStream_t)stream>>>(a);
+  erf_down16_kernel<<<n * tiles_y, kDnThreads, smem, (cudaStream_t)stream>>>(a);
   LAVB_LAUNCH_OK();
   return 0;
 }

@@ -12,6 +12,9 @@
 //   * epilogue bias + ReLU -> h16, transposed through shared memory so every pixel's 128 B leave as full lines.
 // The "wide" image of the brake model is three cameras side by side (lav_agent_fast.py:257): `ncam`/`cam_w` index the
 // (B, ncam, H, cam_w, 3) camera tensor directly.
+#include <climits>
+#include <cmath>
+
 #include "common.cuh"
 
 namespace lavb {
@@ -140,6 +143,7 @@ __global__ void __launch_bounds__(128) stem7x7_u8_kernel(const __grid_constant__
 }
 
 // 3x3 stride-2 pad-1 max-pool on NHWC h16 (lav/models/resnet.py:181,238): one thread = one output pixel x 8 channels.
+// __hmax2_nan: a NaN in the window gives the canonical NaN, as MaxPool2d propagates NaN (__hmax2 would drop it).
 __global__ void __launch_bounds__(256) maxpool3x3s2_kernel(const h16* __restrict__ in, int n, int h, int w, int c8,
                                                            h16* __restrict__ out, int ho, int wo) {
   const long long gid = (long long)blockIdx.x * blockDim.x + threadIdx.x;
@@ -164,7 +168,7 @@ __global__ void __launch_bounds__(256) maxpool3x3s2_kernel(const h16* __restrict
       const uint4 v = __ldg(src + ((long long)iy * w + ix) * c8);
       const h162* pv = reinterpret_cast<const h162*>(&v);
       if (first) { m[0] = pv[0]; m[1] = pv[1]; m[2] = pv[2]; m[3] = pv[3]; first = false; }
-      else { m[0] = __hmax2(m[0], pv[0]); m[1] = __hmax2(m[1], pv[1]); m[2] = __hmax2(m[2], pv[2]); m[3] = __hmax2(m[3], pv[3]); }
+      else { m[0] = __hmax2_nan(m[0], pv[0]); m[1] = __hmax2_nan(m[1], pv[1]); m[2] = __hmax2_nan(m[2], pv[2]); m[3] = __hmax2_nan(m[3], pv[3]); }
     }
   }
   uint4 o;
@@ -181,14 +185,29 @@ extern "C" int lavb_stem7x7s2_u8(const void* d_img, int batch, int ncam, int h, 
                                  const float* h_mean, const float* h_std, void* d_out, void* stream) {
   LAVB_CHECK_ARG(batch >= 0 && ncam >= 1 && ncam <= 4 && h >= 7 && cam_w >= 8, "stem7x7s2_u8: bad shape");
   LAVB_CHECK_ARG(cam_w % 4 == 0, "stem7x7s2_u8: camera width must be a multiple of 4 (got %d)", cam_w);
+  LAVB_CHECK_ARG(cam_w <= INT_MAX / 12, "stem7x7s2_u8: camera width %d is too large", cam_w);
+  const int ho = (h + 6 - 7) / 2 + 1, wo = (ncam * cam_w + 6 - 7) / 2 + 1;
+  LAVB_CHECK_ARG((long long)batch * ceil_div(ho, kStemRows) <= INT_MAX && ceil_div(wo, 128) <= 65535,
+                 "stem7x7s2_u8: %d images of %d x %d need more blocks than a grid holds", batch, h, ncam * cam_w);
   if (batch == 0) return 0;
-  LAVB_CUDA_OK(ensure_dyn_smem((const void*)stem7x7_u8_kernel, kStemSmem));
+  LAVB_CHECK_ARG(d_img && d_w && d_bias && d_out && h_mean && h_std, "stem7x7s2_u8: null pointer");
+  LAVB_CHECK_ARG(is_aligned(d_img, 4) && is_aligned(d_w, 4) && is_aligned(d_bias, 4) && is_aligned(d_out, 16),
+                 "stem7x7s2_u8: d_img, d_w and d_bias must be 4-byte and d_out 16-byte aligned");
+  const size_t out_bytes = (size_t)batch * ho * wo * 64 * sizeof(h16);
+  LAVB_CHECK_ARG(!ranges_overlap(d_img, (size_t)batch * ncam * h * cam_w * 3, d_out, out_bytes), "stem7x7s2_u8: d_out overlaps d_img");
+  LAVB_CHECK_ARG(!ranges_overlap(d_w, 64 * 160 * sizeof(h16), d_out, out_bytes) && !ranges_overlap(d_bias, 64 * sizeof(float), d_out, out_bytes),
+                 "stem7x7s2_u8: d_out overlaps d_w or d_bias (every block reads them at its start)");
   StemArgs a;
+  for (int c = 0; c < 3; ++c) {
+    a.na[c] = 1.f / (255.f * h_std[c]); a.nb[c] = -h_mean[c] / h_std[c];
+    LAVB_CHECK_ARG(std::isfinite(a.na[c]) && std::isfinite(a.nb[c]) && h_std[c] != 0.f,
+                   "stem7x7s2_u8: mean[%d] = %g and std[%d] = %g give a non-finite normalisation", c, h_mean[c], c, h_std[c]);
+  }
+  LAVB_CUDA_OK(ensure_dyn_smem((const void*)stem7x7_u8_kernel, kStemSmem));
   a.img = reinterpret_cast<const unsigned char*>(d_img); a.batch = batch; a.ncam = ncam; a.h = h; a.cam_w = cam_w;
   a.w = reinterpret_cast<const h16*>(d_w); a.bias = d_bias;
-  for (int c = 0; c < 3; ++c) { a.na[c] = 1.f / (255.f * h_std[c]); a.nb[c] = -h_mean[c] / h_std[c]; }
   a.out = reinterpret_cast<h16*>(d_out);
-  a.ho = (h + 6 - 7) / 2 + 1; a.wo = (ncam * cam_w + 6 - 7) / 2 + 1;
+  a.ho = ho; a.wo = wo;
   dim3 grid(batch * ceil_div(a.ho, kStemRows), ceil_div(a.wo, 128));
   stem7x7_u8_kernel<<<grid, 128, kStemSmem, (cudaStream_t)stream>>>(a);
   LAVB_LAUNCH_OK();
@@ -197,9 +216,14 @@ extern "C" int lavb_stem7x7s2_u8(const void* d_img, int batch, int ncam, int h, 
 
 extern "C" int lavb_maxpool3x3s2_nhwc(const void* d_in, int n, int h, int w, int c, void* d_out, void* stream) {
   LAVB_CHECK_ARG(n >= 0 && h >= 1 && w >= 1 && c >= 8 && c % 8 == 0, "maxpool3x3s2_nhwc: bad shape (channels must be a multiple of 8)");
-  if (n == 0) return 0;
   const int ho = (h - 1) / 2 + 1, wo = (w - 1) / 2 + 1;
   const long long total = (long long)n * ho * wo * (c / 8);
+  LAVB_CHECK_ARG((total + 255) / 256 <= INT_MAX, "maxpool3x3s2_nhwc: %lld output vectors need more than 2^31 - 1 blocks", total);
+  if (n == 0) return 0;
+  LAVB_CHECK_ARG(d_in && d_out, "maxpool3x3s2_nhwc: null pointer");
+  LAVB_CHECK_ARG(is_aligned(d_in, 16) && is_aligned(d_out, 16), "maxpool3x3s2_nhwc: d_in and d_out must be 16-byte aligned");
+  LAVB_CHECK_ARG(!ranges_overlap(d_in, (size_t)n * h * w * c * sizeof(h16), d_out, (size_t)total * 8 * sizeof(h16)),
+                 "maxpool3x3s2_nhwc: d_out overlaps d_in");
   maxpool3x3s2_kernel<<<ceil_div(total, 256), 256, 0, (cudaStream_t)stream>>>(reinterpret_cast<const h16*>(d_in), n, h, w, c / 8,
                                                                               reinterpret_cast<h16*>(d_out), ho, wo);
   LAVB_LAUNCH_OK();

@@ -36,6 +36,12 @@ def _need_cuda(*ts):
             raise capi.LavbError("lav_b200 kernels need CUDA tensors (there is no CPU fallback)")
 
 
+def _require(ok, msg):
+    """argument checks that protect memory: a LavbError, never an assert (python -O strips asserts)."""
+    if not ok:
+        raise capi.LavbError(msg)
+
+
 def launches():
     """number of kernel launches issued through this module (bench.py reports it)."""
     return _COUNT[0]
@@ -1238,8 +1244,13 @@ def stem7x7s2_u8(img_u8, w_h16, bias, mean, std):
     """img_u8 (B, ncam, H, cam_w, 3) uint8 contiguous; w_h16 (64,160) packed by pack_stem_weights; bias (64,)
     -> f16 NHWC (B, H/2, ncam*cam_w/2, 64)."""
     _need_cuda(img_u8, w_h16, bias)
-    assert img_u8.dtype == torch.uint8 and img_u8.is_contiguous() and img_u8.dim() == 5 and img_u8.shape[4] == 3
-    assert w_h16.dtype == h16() and tuple(w_h16.shape) == (64, 160) and w_h16.is_contiguous()
+    _require(img_u8.dtype == torch.uint8 and img_u8.is_contiguous() and img_u8.dim() == 5 and img_u8.shape[4] == 3,
+             "stem7x7s2_u8: img_u8 must be a contiguous uint8 (B, ncam, H, cam_w, 3) tensor")
+    _require(w_h16.dtype == h16() and tuple(w_h16.shape) == (64, 160) and w_h16.is_contiguous(),
+             "stem7x7s2_u8: w_h16 must be the contiguous (64, 160) 16-bit packing of pack_stem_weights")
+    _require(bias.dtype == torch.float32 and tuple(bias.shape) == (64,) and bias.is_contiguous(),
+             "stem7x7s2_u8: bias must be a contiguous fp32 (64,) tensor")
+    _require(len(mean) == 3 and len(std) == 3, "stem7x7s2_u8: mean and std hold 3 values")
     b, ncam, h, cw, _ = img_u8.shape
     out = torch.empty((b, (h - 1) // 2 + 1, (ncam * cw - 1) // 2 + 1, 64), dtype=h16(), device=img_u8.device)
     m = (C.c_float * 3)(*[float(v) for v in mean])
@@ -1313,7 +1324,8 @@ def pack_conv7x7s2_weights(w):
 def maxpool3x3s2_nhwc(x):
     """MaxPool2d(3, 2, 1) on a contiguous f16 NHWC tensor."""
     _need_cuda(x)
-    assert x.dtype == h16() and x.is_contiguous() and x.dim() == 4 and x.shape[3] % 8 == 0
+    _require(x.dtype == h16() and x.is_contiguous() and x.dim() == 4 and x.shape[3] % 8 == 0,
+             "maxpool3x3s2_nhwc: x must be a contiguous 16-bit NHWC tensor with channels a multiple of 8")
     n, h, w, c = x.shape
     out = torch.empty((n, (h - 1) // 2 + 1, (w - 1) // 2 + 1, c), dtype=h16(), device=x.device)
     check(lib().lavb_maxpool3x3s2_nhwc(_ptr(x), n, h, w, c, _ptr(out), _stream()), "lavb_maxpool3x3s2_nhwc")
@@ -1354,11 +1366,13 @@ def erf_stem(rgb_u8, w27, scale, shift, out_dtype):
     """fused normalize + ERFNet initial block: rgb_u8 (N,H,W,3) uint8 -> NHWC (N,H/2,W/2,16).  w27 (27,16), scale/shift (16,)
     are HOST float32 numpy arrays (kernel parameters)."""
     _need_cuda(rgb_u8)
-    assert rgb_u8.dtype == torch.uint8 and rgb_u8.is_contiguous() and rgb_u8.dim() == 4 and rgb_u8.shape[3] == 3
+    _require(rgb_u8.dtype == torch.uint8 and rgb_u8.is_contiguous() and rgb_u8.dim() == 4 and rgb_u8.shape[3] == 3,
+             "erf_stem: rgb_u8 must be a contiguous uint8 (N, H, W, 3) tensor")
+    _require(out_dtype in (torch.float32, h16()), f"erf_stem: out_dtype must be float32 or {h16()}, got {out_dtype}")
     n, h, w, _ = rgb_u8.shape
-    out = torch.empty((n, h // 2, w // 2, 16), dtype=out_dtype, device=rgb_u8.device)
     a, b, c = (np.ascontiguousarray(t, dtype=np.float32) for t in (w27, scale, shift))
-    assert a.shape == (27, 16) and b.shape == (16,) and c.shape == (16,)
+    _require(a.shape == (27, 16) and b.shape == (16,) and c.shape == (16,), "erf_stem: w27 must be (27, 16), scale and shift (16,)")
+    out = torch.empty((n, h // 2, w // 2, 16), dtype=out_dtype, device=rgb_u8.device)
     check(lib().lavb_erf_stem(_ptr(rgb_u8), n, h, w, a.ctypes.data_as(C.c_void_p), b.ctypes.data_as(C.c_void_p), c.ctypes.data_as(C.c_void_p),
                               _ptr(out), _DT[out_dtype], _stream()), "lavb_erf_stem")
     _COUNT[0] += 1
@@ -1368,9 +1382,12 @@ def erf_stem(rgb_u8, w27, scale, shift, out_dtype):
 def erf_down16(x, w9, st):
     """fused DownsamplerBlock(16, 64): x h16 NHWC (n,h,w,16) -> (n,h/2,w/2,64) (lavb_erf_down16)."""
     _need_cuda(x, w9, st)
-    assert x.dtype == h16() and x.is_contiguous() and x.dim() == 4 and x.shape[3] == 16
-    assert w9.dtype == torch.float32 and tuple(w9.shape) == (9, 16, 48) and w9.is_contiguous()
-    assert st.dtype == torch.float32 and tuple(st.shape) == (64, 2) and st.is_contiguous()
+    _require(x.dtype == h16() and x.is_contiguous() and x.dim() == 4 and x.shape[3] == 16,
+             "erf_down16: x must be a contiguous 16-bit NHWC tensor of 16 channels")
+    _require(w9.dtype == torch.float32 and tuple(w9.shape) == (9, 16, 48) and w9.is_contiguous(),
+             "erf_down16: w9 must be a contiguous fp32 (9, 16, 48) tensor")
+    _require(st.dtype == torch.float32 and tuple(st.shape) == (64, 2) and st.is_contiguous(),
+             "erf_down16: st must be a contiguous fp32 (64, 2) tensor")
     n, h, w, _ = x.shape
     out = torch.empty((n, h // 2, w // 2, 64), dtype=x.dtype, device=x.device)
     check(lib().lavb_erf_down16(_ptr(x), _ptr(out), n, h, w, _ptr(w9), _ptr(st), _stream()), "lavb_erf_down16")
@@ -1378,15 +1395,17 @@ def erf_down16(x, w9, st):
     return out
 
 
-def erf_nb16(x, w4, st, out=None):
+def erf_nb16(x, w4, st):
     """fused non_bottleneck_1d(16, dilation 1) block: x h16 NHWC (n,h,w,16) -> same shape (lavb_erf_nb16)."""
     _need_cuda(x, w4, st)
-    assert x.dtype == h16() and x.is_contiguous() and x.dim() == 4 and x.shape[3] == 16
-    assert w4.dtype == torch.float32 and tuple(w4.shape) == (4, 3, 16, 16) and w4.is_contiguous()
-    assert st.dtype == torch.float32 and tuple(st.shape) == (4, 16, 2) and st.is_contiguous()
+    _require(x.dtype == h16() and x.is_contiguous() and x.dim() == 4 and x.shape[3] == 16,
+             "erf_nb16: x must be a contiguous 16-bit NHWC tensor of 16 channels")
+    _require(w4.dtype == torch.float32 and tuple(w4.shape) == (4, 3, 16, 16) and w4.is_contiguous(),
+             "erf_nb16: w4 must be a contiguous fp32 (4, 3, 16, 16) tensor")
+    _require(st.dtype == torch.float32 and tuple(st.shape) == (4, 16, 2) and st.is_contiguous(),
+             "erf_nb16: st must be a contiguous fp32 (4, 16, 2) tensor")
     n, h, w, _ = x.shape
-    if out is None:
-        out = torch.empty_like(x)
+    out = torch.empty_like(x)
     check(lib().lavb_erf_nb16(_ptr(x), _ptr(out), n, h, w, _ptr(w4), _ptr(st), _stream()), "lavb_erf_nb16")
     _COUNT[0] += 1
     return out

@@ -15,39 +15,24 @@ Misaligned or out-of-range arguments appear only in cases the entry points refus
 convert) route to their element-wise bodies.
 """
 import ctypes as C
-import itertools
-import json
 import math
 import os
 
 import pytest
 import torch
 import torch.nn.functional as F
-from torch.profiler import ProfilerActivity, profile
 
 from lav_b200 import capi, ops, synth
+from tests.util import INT, canary, is_canary, kernels
 
 pytestmark = pytest.mark.gpu
 
-CANARY = {torch.float32: 0x7FC0DEAD, torch.float16: 0x7E5A, torch.bfloat16: 0x7FDA}
-INT = {torch.float32: torch.int32, torch.float16: torch.int16, torch.bfloat16: torch.int16}
 CNAME = {torch.float32: "float", torch.float16: "__half", torch.bfloat16: "__nv_bfloat16"}
 TOL = {torch.float32: 2e-5, torch.float16: 1e-3, torch.bfloat16: 1e-2}
-_TRACES = itertools.count()
 
 
 def dt(code):
     return torch.float32 if code == "f" else ops.h16()
-
-
-def canary(shape, dtype, device):
-    t = torch.empty(shape, dtype=dtype, device=device)
-    t.view(INT[dtype]).fill_(CANARY[dtype])
-    return t
-
-
-def is_canary(t):
-    return t.contiguous().view(INT[t.dtype]) == CANARY[t.dtype]
 
 
 def bits(t):
@@ -69,33 +54,6 @@ def nchw(t):
 def fmax0(a):
     """fmaxf(a, 0.f): a NaN comes out as 0 (torch.relu would keep it)"""
     return torch.where(torch.isnan(a), torch.zeros_like(a), a.clamp_min(0))
-
-
-def kernels(fn, tmp_path, tries=5):
-    """run fn under torch.profiler; the (name, grid) of every kernel it launched, in launch order.  Every call traced here
-    is idempotent (same outputs, same elements written), so fn may be traced more than once.  The profiler's kernel
-    records can be missing from a short capture and arrive in a later one, so the kernel records of all captures are pooled
-    by correlation id, and the first capture in which every kernel launch has its kernel record is the answer."""
-    records, captures = {}, []
-    for _ in range(tries):
-        torch.cuda.synchronize()
-        with profile(activities=[ProfilerActivity.CPU, ProfilerActivity.CUDA]) as prof:
-            fn()
-            torch.cuda.synchronize()
-        path = os.path.join(str(tmp_path), f"trace{next(_TRACES)}.json")
-        prof.export_chrome_trace(path)
-        with open(path) as f:
-            events = json.load(f)["traceEvents"]
-        os.remove(path)
-        captures.append([e["args"]["correlation"] for e in events
-                         if e.get("cat") in ("cuda_runtime", "cuda_driver") and "Launch" in e.get("name", "")
-                         and "correlation" in e.get("args", {})])
-        records.update({e["args"]["correlation"]: (e["name"], e["args"].get("grid")) for e in events
-                        if e.get("cat") == "kernel" and "correlation" in e.get("args", {})})
-        for launches in captures:
-            if launches and all(c in records for c in launches):
-                return [records[c] for c in launches]
-    return []
 
 
 def num_sms():

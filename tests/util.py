@@ -1,4 +1,7 @@
 """Shared builders for the tests: seeded weights (identical in the pin script) and inputs."""
+import itertools
+import json
+import math
 import os
 
 import numpy as np
@@ -222,3 +225,246 @@ def pillar_forward_ref64(pts, starts, counts, grid, w1, s1, t1, w2, s2, t2, mode
         bound = bound + torch.where(occupied & ((bound > 0) | (parts == "all")), flip, torch.zeros_like(bound))
         canvas = round_h16(canvas)
     return canvas.view(B, ny, nx, 64), bound.view(B, ny, nx, 64)
+
+
+# ----------------------------------------------------------------------------------------------------- output canaries
+CANARY = {torch.float32: 0x7FC0DEAD, torch.float16: 0x7E5A, torch.bfloat16: 0x7FDA}    # NaN bit patterns no kernel writes
+INT = {torch.float32: torch.int32, torch.float16: torch.int16, torch.bfloat16: torch.int16}
+_TRACES = itertools.count()
+
+
+def canary(shape, dtype, device):
+    t = torch.empty(shape, dtype=dtype, device=device)
+    t.view(INT[dtype]).fill_(CANARY[dtype])
+    return t
+
+
+def is_canary(t):
+    return t.contiguous().view(INT[t.dtype]) == CANARY[t.dtype]
+
+
+def kernels(fn, tmp_path, tries=5):
+    """run fn under torch.profiler; the (name, grid) of every kernel it launched, in launch order.  Every call traced here
+    is idempotent (same outputs, same elements written), so fn may be traced more than once.  The profiler's kernel
+    records can be missing from a short capture and arrive in a later one, so the kernel records of all captures are pooled
+    by correlation id, and the first capture in which every kernel launch has its kernel record is the answer."""
+    from torch.profiler import ProfilerActivity, profile
+    records, captures = {}, []
+    for _ in range(tries):
+        torch.cuda.synchronize()
+        with profile(activities=[ProfilerActivity.CPU, ProfilerActivity.CUDA]) as prof:
+            fn()
+            torch.cuda.synchronize()
+        path = os.path.join(str(tmp_path), f"trace{next(_TRACES)}.json")
+        prof.export_chrome_trace(path)
+        with open(path) as f:
+            events = json.load(f)["traceEvents"]
+        os.remove(path)
+        captures.append([e["args"]["correlation"] for e in events
+                         if e.get("cat") in ("cuda_runtime", "cuda_driver") and "Launch" in e.get("name", "")
+                         and "correlation" in e.get("args", {})])
+        records.update({e["args"]["correlation"]: (e["name"], e["args"].get("grid")) for e in events
+                        if e.get("cat") == "kernel" and "correlation" in e.get("args", {})})
+        for launches in captures:
+            if launches and all(c in records for c in launches):
+                return [records[c] for c in launches]
+    return []
+
+
+# ----------------------------------------------------------------------------------------------------- camera kernels
+# fp64 statements of lavb_erf_stem, lavb_erf_down16, lavb_erf_nb16, lavb_stem7x7s2_u8 and lavb_maxpool3x3s2_nhwc
+# (include/lav_b200.h), on the operands as each kernel reads them.  Each returns (expected, bound) as float64 NHWC on the
+# input's device: every correct kernel output c satisfies |c - expected| <= bound element-wise (bound 0 = bit-exact value).
+U_MMA = 2.0 ** -23          # fp32 accumulation on the tensor cores: mma.sync is not guaranteed to round to nearest
+
+
+def _store_h16(v, e):
+    """the final saturating h16 store of a value known within e: both the kernel and the statement round their own value,
+    so they can land one h16 ulp apart, 2^-10 (|v| + e) for normal values and 2^-24 (the subnormal spacing) below.  A
+    non-finite v (an exact -inf / +inf of the pool branch) is stored exactly."""
+    fin = torch.isfinite(v)
+    e = torch.where(fin, e + 2.0 ** -10 * (v.abs() + e) + 2.0 ** -24, torch.zeros_like(e))
+    return round_h16(v), e
+
+
+def _store_h16_interval(v, e):
+    """the same store, bounded exactly: the kernel's fp32 value lies in [v - e, v + e] and rounding is monotonic, so its h16
+    value lies between the roundings of the two ends.  Where both ends round to round_h16(v) the kernel's stored value IS
+    the statement's, bit for bit (bound 0); elsewhere the bound is the distance to the farther end's rounding."""
+    r = round_h16(v)
+    b = torch.maximum(round_h16(v + e) - r, r - round_h16(v - e))
+    return r, torch.where(torch.isfinite(v), b, torch.zeros_like(b))
+
+
+def _affine(a, ea, s, t):
+    """relu(fmaf(a, s, t)) for a known within ea: |s| ea from the input, one fp32 rounding of the result.  A NaN (from a NaN
+    operand) comes out as exactly 0 with bound 0, as fmaxf(NaN, 0) = 0."""
+    v = a * s + t
+    e = s.abs() * ea + U32 * (s.abs() * (a.abs() + ea) + t.abs())
+    nan = torch.isnan(v)
+    return _relu(v), torch.where(nan | ~torch.isfinite(e), torch.zeros_like(e), e)
+
+
+def erf_stem_lut():
+    """(v / 255 - .5) * 2 in fp32 for the 256 byte values, three roundings (rgb.py:41) -> float64 (256,).  numpy's fp32
+    division, subtraction and product round to nearest, as the kernel's __fdiv_rn and fp32 ops do."""
+    v = np.arange(256, dtype=np.float32)
+    return torch.from_numpy(((v / np.float32(255) - np.float32(0.5)) * np.float32(2)).astype(np.float64))
+
+
+def erf_stem_ref64(rgb_u8, w27, scale, shift, out_dtype):
+    """lavb_erf_stem in float64.  rgb_u8 (N, H, W, 3) uint8; w27 (27, 16) [(ky*3+kx)*3+c][co] (only co < 13 read);
+    scale / shift (16,); out_dtype float32 or the 16-bit type -> (N, H/2, W/2, 16) float64 expected and bound.
+
+    The statement: x = erf_stem_lut()[rgb] (bit for bit the kernel's normalised image); channels 0..12 = relu(fmaf(conv3x3
+    s2 p1 (x, w), s, t)) with zero padding in the normalised domain; channels 13..15 = relu(fmaf(maxpool2x2(x), s, t)).
+    The bound (u = 2^-24, gamma_n = n u / (1 - n u)):
+      * conv: the kernel's 27-term fp32 fmaf chain, gamma_27 sum |x w| (the exact fp64 sum of fp32 products adds < 2^-50
+        sum |x w|, inside gamma_28, which is used);
+      * pool: the max of four fp32 values is exact;
+      * fmaf(a, s, t): |s| times the propagated error plus u (|s| (|a| + e) + |t|); ReLU is 1-Lipschitz;
+      * h16 output: the final rounding (_store_h16)."""
+    import torch.nn.functional as F
+    dev = rgb_u8.device
+    x = erf_stem_lut().to(dev)[rgb_u8.long()].permute(0, 3, 1, 2)
+    w = torch.as_tensor(np.asarray(w27, dtype=np.float32)).double().to(dev)
+    s = torch.as_tensor(np.asarray(scale, dtype=np.float32)).double().to(dev)[None, :, None, None]
+    t = torch.as_tensor(np.asarray(shift, dtype=np.float32)).double().to(dev)[None, :, None, None]
+    W = w[:, :13].reshape(3, 3, 3, 13).permute(3, 2, 0, 1)                 # [co][c][ky][kx]
+    a = F.conv2d(x, W, stride=2, padding=1)
+    ea = gamma(28) * F.conv2d(x.abs(), W.abs(), stride=2, padding=1)
+    vc, ec = _affine(a, ea, s[:, :13], t[:, :13])
+    m = F.max_pool2d(x, 2, 2)
+    vp, ep = _affine(m, torch.zeros_like(m), s[:, 13:], t[:, 13:])
+    v, e = torch.cat([vc, vp], 1).permute(0, 2, 3, 1), torch.cat([ec, ep], 1).permute(0, 2, 3, 1)
+    if out_dtype != torch.float32:
+        v, e = _store_h16(v, e)
+    return v.contiguous(), e.contiguous()
+
+
+def erf_down16_ref64(x_h16, w9, st):
+    """lavb_erf_down16 in float64.  x_h16 (N, H, W, 16) 16-bit; w9 (9, 16, 48) fp32 [ky*3+kx][cin][cout]; st (64, 2) fp32
+    (scale, shift) -> (N, H/2, W/2, 64) float64 expected and bound.
+
+    The statement: channels 0..47 = relu(fmaf(conv3x3 s2 p1 (x, h16(w9)), s, t)); channels 48..63 = relu(fmaf(m, s, t)) with
+    m the max of the 2x2 window that skips NaN and starts from -inf (so four NaNs give -inf); h16 store.
+    The bound: the 144 products are exact in fp32 and summed on the tensor cores, bounded as gamma_144 with u = 2^-23 per
+    add (U_MMA) on sum |x w|; the pool's max is exact; then _affine and _store_h16.  A conv channel whose window holds a NaN
+    is exactly 0 (fmaxf(NaN, 0)), bound 0."""
+    import torch.nn.functional as F
+    x = x_h16.double().permute(0, 3, 1, 2)
+    W = round_h16(w9.double()).to(x.device).reshape(3, 3, 16, 48).permute(3, 2, 0, 1)
+    s, t = (st[:, i].double().to(x.device)[None, :, None, None] for i in (0, 1))
+    a = F.conv2d(x, W, stride=2, padding=1)
+    ea = gamma(144, U_MMA) * F.conv2d(x.abs(), W.abs(), stride=2, padding=1)
+    vc, ec = _affine(a, ea, s[:, :48], t[:, :48])
+    m = F.max_pool2d(torch.where(torch.isnan(x), torch.full_like(x, -math.inf), x), 2, 2)
+    vp, ep = _affine(m, torch.zeros_like(m), s[:, 48:], t[:, 48:])
+    v, e = torch.cat([vc, vp], 1).permute(0, 2, 3, 1), torch.cat([ec, ep], 1).permute(0, 2, 3, 1)
+    return tuple(r.contiguous() for r in _store_h16(v, e))
+
+
+def erf_nb16_ref64(x_h16, w4, st):
+    """lavb_erf_nb16 in float64.  x_h16 (N, H, W, 16) 16-bit; w4 (4, 3, 16, 16) fp32 [conv][tap][cin][cout]; st (4, 16, 2)
+    fp32 (scale, shift) -> (N, H, W, 16) float64 expected and bound.
+
+    The statement: four stages, 3x1 / 1x3 / 3x1 / 1x3 with zero padding, each relu(fmaf(conv(in, h16(w)), s, t)) [+ x before
+    the last ReLU, one fp32 add] stored as h16 for the next stage.
+    The bound carries each stage's error e_in into the next: sum |w| e_in through the conv, plus the tensor-core sum of 48
+    products, gamma_48 (u = 2^-23) on sum |w| (|in| + e_in); then _affine; the residual add rounds once more, u (|v| + e);
+    ReLU is 1-Lipschitz.  Each h16 store is bounded exactly by _store_h16_interval: the fp32 error before a store is far
+    below an h16 ulp, so almost every intermediate is bit-exact (bound 0) and only values within that error of a rounding
+    boundary carry a one-ulp bound into the next stage, which amplifies it by its sum |w| |s|.  A NaN that reaches a ReLU
+    gives exactly 0 (bound 0) in both."""
+    import torch.nn.functional as F
+    x = x_h16.double().permute(0, 3, 1, 2)
+    W = round_h16(w4.double()).to(x.device)
+    S = st.double().to(x.device)
+    v, e = x, torch.zeros_like(x)
+    for k in range(4):
+        Wk = W[k].permute(2, 1, 0)                                              # [cout][cin][tap]
+        Wk, pad = (Wk[..., None], (1, 0)) if k % 2 == 0 else (Wk[:, :, None, :], (0, 1))
+        a = F.conv2d(v, Wk, padding=pad)
+        ep = F.conv2d(e, Wk.abs(), padding=pad)
+        ea = ep + gamma(48, U_MMA) * (F.conv2d(v.abs(), Wk.abs(), padding=pad) + ep)
+        s, t = S[k, :, 0][None, :, None, None], S[k, :, 1][None, :, None, None]
+        pre = a * s + t
+        epre = s.abs() * ea + U32 * (s.abs() * (a.abs() + ea) + t.abs())
+        if k == 3:
+            pre = pre + x
+            epre = epre + U32 * (pre.abs() + epre)
+        nan = torch.isnan(pre)
+        v = _relu(pre)
+        e = torch.where(nan | ~torch.isfinite(epre), torch.zeros_like(epre), epre)
+        v, e = _store_h16_interval(v, e)
+    return v.permute(0, 2, 3, 1).contiguous(), e.permute(0, 2, 3, 1).contiguous()
+
+
+def nb16_test_params(seed, weight_scale=0.03):
+    """seeded erf_nb16 operands for the tests: w4 (4, 3, 16, 16) randn * weight_scale and st (4, 16, 2) fp32.  The default
+    scale keeps sum |w| |s| of every stage below 2, so a one-ulp h16 difference is not amplified into a bound as large as the
+    values: the statement's bound then tells an h16 kernel from a bf16 one (tests/test_camera_kernels_ref_cpu.py).  The
+    scales of the two convs without BatchNorm are 1; the shifts of stages 1..3 are positive, so every channel is alive
+    after their ReLUs; the last shift takes both signs."""
+    g = torch.Generator().manual_seed(seed)
+    w4 = torch.randn(4, 3, 16, 16, generator=g) * weight_scale
+    s = torch.rand(4, 16, generator=g) + 0.5
+    s[0], s[2] = 1.0, 1.0
+    t = torch.randn(4, 16, generator=g) * 0.2
+    t[:3] = t[:3].abs() + 0.05
+    return w4, torch.stack([s, t], 2)
+
+
+def stem_u8_operand(mean, std):
+    """the staged operand of lavb_stem7x7s2_u8 for every byte value and channel, bit for bit -> (256, 3) float64 of h16
+    values: na = 1.f / (255.f * std), nb = -mean / std in fp32 as the host computes them; fmaf(u8, na, nb), whose fp64
+    product and sum are exact here (at most 40 significant bits), rounded once to fp32; then rounded to h16."""
+    m, s = np.asarray(mean, dtype=np.float32), np.asarray(std, dtype=np.float32)
+    na = np.float32(1) / (np.float32(255) * s)
+    nb = -m / s
+    u = np.arange(256, dtype=np.float64)[:, None]
+    f32 = (u * na.astype(np.float64) + nb.astype(np.float64)).astype(np.float32)
+    return torch.from_numpy(f32).half().double()
+
+
+def stem_unpack_weights(w_h16):
+    """(64, 160) in the stem kernel's K order k = ky*22 + kx*3 + c -> (64, 3, 7, 7) float64; slot 21 of each window row and
+    k >= 154 are zero by the header's contract and are not part of the statement."""
+    return w_h16.double()[:, :154].reshape(64, 7, 22)[:, :, :21].reshape(64, 7, 7, 3).permute(0, 3, 1, 2)
+
+
+def stem7x7s2_u8_ref64(img_u8, w_h16, bias, mean, std):
+    """lavb_stem7x7s2_u8 in float64.  img_u8 (B, ncam, H, cam_w, 3) uint8; w_h16 (64, 160) 16-bit from pack_stem_weights;
+    bias (64,) fp32 -> (B, (H-1)//2+1, (ncam*cam_w-1)//2+1, 64) float64 expected and bound.
+
+    The statement: the side-by-side image of the cameras, each byte replaced by stem_u8_operand (zero padding in the
+    normalised domain), conv 7x7 s2 p3 with the h16 weights (exact products), + bias, ReLU, h16 store.
+    The bound: the 147 live products (154 slots) are summed in fp32 on the tensor cores over 10 k-steps of 16, bounded as
+    gamma_160 with u = 2^-23 per add on sum |x w|; the bias add rounds once, u (|a| + e + |b|); then _store_h16."""
+    import torch.nn.functional as F
+    B, ncam, H, cw, _ = img_u8.shape
+    dev = img_u8.device
+    op = stem_u8_operand(mean, std).to(dev)
+    wide = img_u8.permute(0, 2, 1, 3, 4).reshape(B, H, ncam * cw, 3).long()
+    x = torch.stack([op[wide[..., c], c] for c in range(3)], 1)
+    W = stem_unpack_weights(w_h16).to(dev)
+    b = bias.double().to(dev)[None, :, None, None]
+    a = F.conv2d(x, W, stride=2, padding=3)
+    ea = gamma(160, U_MMA) * F.conv2d(x.abs(), W.abs(), stride=2, padding=3)
+    v = a + b
+    e = ea + U32 * (a.abs() + ea + b.abs())
+    v, e = _store_h16(_relu(v).permute(0, 2, 3, 1), e.permute(0, 2, 3, 1))
+    return v.contiguous(), e.contiguous()
+
+
+def maxpool3x3s2_ref64(x_h16):
+    """lavb_maxpool3x3s2_nhwc in float64, exact: (N, H, W, C) 16-bit -> (N, (H-1)//2+1, (W-1)//2+1, C) float64.  Pixels off
+    the map are skipped, a NaN anywhere in the window gives NaN (MaxPool2d's rule), and -0 ranks below +0 (the header's
+    rule; MaxPool2d would keep whichever zero comes first)."""
+    import torch.nn.functional as F
+    x = x_h16.double().permute(0, 3, 1, 2)
+    neg0 = (x == 0) & torch.signbit(x)
+    tiny = -1e-300                                  # -0 -> a value between every negative h16 (<= -2^-24) and +0
+    m = F.max_pool2d(torch.where(neg0, torch.full_like(x, tiny), x), 3, 2, 1)
+    m = torch.where(m == tiny, torch.full_like(m, -0.0), m)
+    return m.permute(0, 2, 3, 1).contiguous()
