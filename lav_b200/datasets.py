@@ -413,8 +413,9 @@ class TemporalBatchLoader:
     uint8, ego_locs (B,T+1,2) f32, cmds (B,) int64, nxps (B,2) f32, bras (B,) int64, locs (B,max_objs,T+1,2) f32, oris
     (B,max_objs) f32, typs (B,max_objs) int32, num_objs (B,) int64; train_lidar takes the first 13.
 
-    With ``ordered`` (evaluation) the samples come in index order with no augmentation: every draw is dataset.no_draw(), and the
-    LiDAR shuffles still come from the generator of (seed, epoch, rank).  With ``plan_safety`` (ordered only) every sample is
+    With ``ordered`` (evaluation) the samples come in index order with no augmentation, rank r taking the contiguous range
+    [r * n // world, (r + 1) * n // world): every draw is dataset.no_draw(), and the LiDAR shuffles still come from the
+    generator of (seed, epoch, rank).  With ``plan_safety`` (ordered only) every sample is
     prepared with its plan_safety_table, and the staged tables carry them packed under "plan_safety" (stage_plan_safety)."""
 
     def __init__(self, dataset, batch_size, seed=2021, rank=0, world=1, drop_last=True, num_workers=8, ordered=False,
@@ -432,11 +433,16 @@ class TemporalBatchLoader:
         return list(pool.map(lambda a: self.ds.prepare(int(a[0]), *a[1], **kw), zip(idxs, draws)))
 
     def shard(self, epoch):
-        perm = np.arange(len(self.ds)) if self.ordered else np.random.RandomState([self.seed, epoch]).permutation(len(self.ds))
-        return perm[self.rank::self.world][:len(self.ds) // self.world]
+        """this rank's sample indices of ``epoch``: training takes every world-th entry of the epoch's shuffle (the remainder
+        dropped, so every rank runs as many steps); ordered mode takes the contiguous range [rank * n // world,
+        (rank + 1) * n // world), so the ranks together score every sample once, in index order."""
+        n = len(self.ds)
+        if self.ordered:
+            return np.arange(self.rank * n // self.world, (self.rank + 1) * n // self.world)
+        return np.random.RandomState([self.seed, epoch]).permutation(n)[self.rank::self.world][:n // self.world]
 
     def __len__(self):
-        n = len(self.ds) // self.world
+        n = len(self.shard(0)) if self.ordered else len(self.ds) // self.world
         return n // self.B if self.drop_last else -(-n // self.B)
 
     def generators(self, epoch):

@@ -5,10 +5,23 @@ against the expert's future — as numbers over every sample of the recording, t
     python -m lav_b200.evaluate --config-path config_v2.yaml --data-dir VALDIR --lidar-weights lidar_7.th \
         --uniplanner-weights uniplanner_7.th [--batch-size 32] [--precision f16|fp32] [--num-workers 16] [--json out.json] \
         [--forecast] [--forecast-detected] [--plan-safety]
+    python -m lav_b200.evaluate ... --lidar-weights lidar_8.th lidar_16.th --uniplanner-weights uniplanner_8.th uniplanner_16.th
+    python -m lav_b200.evaluate ... --run-dir RUN [--epochs 1,8,16-64]
+    torchrun --nproc-per-node N -m lav_b200.evaluate ...
 
 Every sample is taken once, in index order, unaugmented (TemporalBatchLoader's ordered mode); the last batch may be short.  Per
 batch, InferModel.forward_batch runs the models and one ops.eval_batch launch scores its outputs; the one device-to-host copy
 is that launch's result buffer.  The host sums the counts and computes AP over the whole recording.
+
+Several checkpoints (weight paths paired by position, or train_full's lidar_{e}.th / uniplanner_{e}.th pairs found by --run-dir)
+are scored in one pass, each batch loaded once and run through every checkpoint (evaluate_checkpoints, lav_b200.eval_sweep);
+each checkpoint's result is exactly what a run of it alone reports.  One checkpoint prints and writes what a single run always
+has; a sweep prints one row of headline numbers per checkpoint and writes {samples, ranks, checkpoints: [{epoch, weights,
+result}]}.  Under torchrun each rank scores a contiguous range of the recording on GPU LOCAL_RANK % device_count and rank 0
+merges the per-sample records over gloo, so the result is the one a single process computes from the same per-sample values;
+rank 0 alone prints and writes --json.  The model outputs themselves are not bit-reproducible across runs (the pillar encoder
+sums with float atomics), and a rank's LiDAR shuffle stream starts at its own first sample, so a sample's point order differs
+from a single process's, and which points are kept differs when its sweep stack exceeds max_lidar_points.
 
 Metrics:
   bev_iou[c]      intersection / union of (pred > 0.5, gt != 0) over all pixels of BEV channel c (null without any union)
@@ -127,6 +140,8 @@ from . import ops
 from .agent import infer_model, math_mode
 from .capi import LavbError
 from .datasets import TemporalBatchLoader, TemporalLiDARPaintedDataset
+from .eval_sweep import (ResidentMeter, add_checkpoint_args, check_sweep_fits, eval_device, gather_merged, init_ranks,
+                         rank_and_world, select_checkpoints, sweep_json, sweep_table)
 from .heads import off_centre
 from .model_inference import peak_filter
 
@@ -168,6 +183,16 @@ class Scores:
         self.ade += pe[:, 0].tolist()
         self.fde += pe[:, 1].tolist()
         self.cmd += [int(c) for c in cmds]
+
+    def extend(self, other):
+        """append the records of ``other``, which follow this one's in sample order (a later rank's shard)."""
+        self.iou += other.iou
+        self.ngt += other.ngt
+        for c in range(len(CLASSES)):
+            self.det[c] += other.det[c]
+        self.ade += other.ade
+        self.fde += other.fde
+        self.cmd += other.cmd
 
     def summary(self):
         inter, union = self.iou[:, 0], self.iou[:, 1]
@@ -219,6 +244,11 @@ class ForecastScores:
         if self.plan:
             self.ego_plan.append(err[n_other + b:n_other + 2 * b])
         self.cmd.append(np.asarray(cmds, np.int64))
+
+    def extend(self, other):
+        """append the records of ``other``, which follow this one's in sample order."""
+        for k in ("other", "ego", "top", "ego_plan", "cmd"):
+            getattr(self, k).extend(getattr(other, k))
 
     def summary(self):
         mean = lambda a: float(np.mean(a)) if len(a) else None
@@ -301,6 +331,13 @@ class DetectedForecastScores:
         self.err.append(v["err"].numpy()[:, :4].copy())
         self.gt += int(v["ngt"].numpy()[:, 0].sum())
 
+    def extend(self, other):
+        """append the records of ``other``, which follow this one's in sample order."""
+        self.score += other.score
+        self.flag += other.flag
+        self.err += other.err
+        self.gt += other.gt
+
     def summary(self):
         mean = lambda a: float(np.mean(a)) if len(a) else None
         s = np.concatenate(self.score) if self.score else np.zeros(0, np.float32)
@@ -341,6 +378,11 @@ class PlanSafetyScores:
         self.res.append(np.asarray(res, np.int32).copy())
         self.cmd.append(np.asarray(cmds, np.int64))
 
+    def extend(self, other):
+        """append the records of ``other``, which follow this one's in sample order."""
+        self.res += other.res
+        self.cmd += other.cmd
+
     def summary(self, t):
         """per trajectory: the rates over all samples and per recorded command (``t`` steps per trajectory)."""
         res = np.concatenate(self.res) if self.res else np.zeros((0, len(self.names), 8), np.int32)
@@ -375,42 +417,54 @@ def format_plan_safety(s):
     return lines
 
 
-@torch.no_grad()
 def evaluate(lidar_model, uniplanner, dataset, batch_size=32, precision="f16", num_workers=16, forecast=False,
              forecast_detected=False, plan_safety=False):
     """Scores of ``lidar_model`` and ``uniplanner`` over every sample of ``dataset`` (a TemporalLiDARPaintedDataset), the models
     run as the agent runs them at ``precision``; with ``forecast`` also the UniPlanner's forecast scores on the recorded poses,
     with ``forecast_detected`` those on the detected vehicles, with ``plan_safety`` the collision and off-road rates of the ego
-    plan and of the expert.  -> dict (see the module docstring)."""
+    plan and of the expert.  -> dict (see the module docstring); None on a rank other than 0 of a process group."""
+    results = evaluate_checkpoints([(lidar_model, uniplanner)], dataset, batch_size, precision, num_workers, forecast,
+                                   forecast_detected, plan_safety)
+    return None if results is None else results[0]
+
+
+@torch.no_grad()
+def evaluate_checkpoints(pairs, dataset, batch_size=32, precision="f16", num_workers=16, forecast=False, forecast_detected=False,
+                         plan_safety=False):
+    """evaluate() of every (lidar_model, uniplanner) of ``pairs`` in one pass over ``dataset``: each batch is loaded and staged
+    once, then every pair runs its own InferModel and scoring launches on it into its own accumulators.  All pairs stay
+    resident; a sweep that would not fit on the device is refused before any data is loaded.  In a process group each rank
+    scores its contiguous shard of the recording and rank 0 merges the ranks' records (eval_sweep.gather_merged).  -> one
+    evaluate() result per pair on rank 0, None on the other ranks."""
     dev = dataset.device
-    lidar_model.to(dev).eval()
-    uniplanner.to(dev).eval()
-    im = infer_model(lidar_model, uniplanner, precision, dataset.camera_x, dataset.camera_z, dev)
+    rank, world = rank_and_world()
+    models = []
+    for i, (lid, uni) in enumerate(pairs):
+        meter = ResidentMeter(dev, lid, uni) if i == 0 and len(pairs) > 1 else None
+        lid.to(dev).eval()
+        uni.to(dev).eval()
+        models.append(infer_model(lid, uni, precision, dataset.camera_x, dataset.camera_z, dev))
+        if meter is not None:
+            check_sweep_fits(len(pairs), meter.resident(), meter.available, batch_size, "LiDAR + UniPlanner pairs")
     grid = dict(min_x=dataset.min_x, max_x=dataset.max_x, min_y=dataset.min_y, max_y=dataset.max_y,
                 pixels_per_meter=dataset.pixels_per_meter)
-    loader = TemporalBatchLoader(dataset, batch_size, drop_last=False, num_workers=num_workers, ordered=True, plan_safety=plan_safety)
-    scores, forecasts, detected, safety = Scores(), ForecastScores(), DetectedForecastScores(), PlanSafetyScores()
+    loader = TemporalBatchLoader(dataset, batch_size, rank=rank, world=world, drop_last=False, num_workers=num_workers, ordered=True,
+                                 plan_safety=plan_safety)
+    accs = [(Scores(), ForecastScores(), DetectedForecastScores(), PlanSafetyScores()) for _ in models]
     with math_mode(precision):
         for batch, staged in loader.staged_batches():
-            lidars, num_points, bev, ego_locs, cmds, nxps = batch[0], batch[1], batch[5], batch[6], batch[7], batch[8]
-            out = im.forward_batch(lidars, num_points, nxps, cmds)
-            res = ops.eval_batch(out["pred_bev"].permute(0, 2, 3, 1), bev, out["packed"], staged["actors"].to(dev, non_blocking=True),
-                                 staged["offsets"], out["ego_plan_locs"].float().contiguous(), ego_locs, grid)
-            host_cmds = staged["labels"]["cmd"].numpy()
-            scores.add(ops.eval_views(res.cpu(), len(num_points), out["packed"].shape[2]), host_cmds)
-            if forecast:
-                fc = im.uniplanner.forecast_recorded(out["features"].permute(0, 3, 1, 2), ego_locs, batch[10], batch[11], batch[12])
-                k = fc["cast"].shape[0]
-                forecasts.add(ops.forecast_views(score_forecasts(fc, cmds).cpu(), k + len(num_points)), k, host_cmds)
-            if forecast_detected:
-                h, w = out["features"].shape[1:3]                   # forward_batch's features are NHWC at half the map size
-                rows = detected_rows(out["packed"].cpu().numpy(), im.pixels_per_meter, im.uniplanner.crop_centre(2 * h, 2 * w))
-                res = score_detected(out, rows, staged["actors"].to(dev, non_blocking=True), staged["offsets"], batch[10], ego_locs,
-                                     batch[13], grid)
-                detected.add(ops.det_match_views(res.cpu(), len(num_points), len(rows["col"]), batch[10].shape[2] - 1), rows["score"])
-            if plan_safety:
-                res = score_plan_safety(out["ego_plan_locs"], ego_locs, staged["plan_safety"], bev, grid)
-                safety.add(res.cpu().numpy(), host_cmds)
+            actors = staged["actors"].to(dev, non_blocking=True)
+            for im, acc in zip(models, accs):
+                score_batch(im, batch, staged, actors, grid, acc, forecast, forecast_detected, plan_safety)
+    accs = gather_merged(accs)
+    if accs is None:
+        return None
+    return [summarize(acc, precision, forecast, forecast_detected, plan_safety, dataset.num_plan) for acc in accs]
+
+
+def summarize(acc, precision, forecast, forecast_detected, plan_safety, num_plan):
+    """the evaluate() result of one checkpoint's accumulators ``acc`` (score_batch's tuple)."""
+    scores, forecasts, detected, safety = acc
     result = scores.summary()
     result["precision"] = precision
     if forecast:
@@ -418,16 +472,41 @@ def evaluate(lidar_model, uniplanner, dataset, batch_size=32, precision="f16", n
     if forecast_detected:
         result["forecast_detected"] = detected.summary()
     if plan_safety:
-        result["plan_safety"] = safety.summary(dataset.num_plan)
+        result["plan_safety"] = safety.summary(num_plan)
     return result
+
+
+def score_batch(im, batch, staged, actors, grid, acc, forecast, forecast_detected, plan_safety):
+    """one checkpoint's InferModel ``im`` on one loader batch (its 14-tuple, staged tables and the actor table on the device),
+    scored into ``acc`` = (Scores, ForecastScores, DetectedForecastScores, PlanSafetyScores)."""
+    scores, forecasts, detected, safety = acc
+    dev = actors.device
+    lidars, num_points, bev, ego_locs, cmds, nxps = batch[0], batch[1], batch[5], batch[6], batch[7], batch[8]
+    out = im.forward_batch(lidars, num_points, nxps, cmds)
+    res = ops.eval_batch(out["pred_bev"].permute(0, 2, 3, 1), bev, out["packed"], actors, staged["offsets"],
+                         out["ego_plan_locs"].float().contiguous(), ego_locs, grid)
+    host_cmds = staged["labels"]["cmd"].numpy()
+    scores.add(ops.eval_views(res.cpu(), len(num_points), out["packed"].shape[2]), host_cmds)
+    if forecast:
+        fc = im.uniplanner.forecast_recorded(out["features"].permute(0, 3, 1, 2), ego_locs, batch[10], batch[11], batch[12])
+        k = fc["cast"].shape[0]
+        forecasts.add(ops.forecast_views(score_forecasts(fc, cmds).cpu(), k + len(num_points)), k, host_cmds)
+    if forecast_detected:
+        h, w = out["features"].shape[1:3]                   # forward_batch's features are NHWC at half the map size
+        rows = detected_rows(out["packed"].cpu().numpy(), im.pixels_per_meter, im.uniplanner.crop_centre(2 * h, 2 * w))
+        res = score_detected(out, rows, actors, staged["offsets"], batch[10], ego_locs, batch[13], grid)
+        detected.add(ops.det_match_views(res.cpu(), len(num_points), len(rows["col"]), batch[10].shape[2] - 1), rows["score"])
+    if plan_safety:
+        res = score_plan_safety(out["ego_plan_locs"], ego_locs, staged["plan_safety"], bev, grid)
+        safety.add(res.cpu().numpy(), host_cmds)
 
 
 def parse_args(argv=None):
     ap = argparse.ArgumentParser(description=__doc__.split("\n")[0])
     ap.add_argument("--config-path", default="config_v2.yaml")
     ap.add_argument("--data-dir", required=True, help="the held-out recording (replaces the YAML's data_dir)")
-    ap.add_argument("--lidar-weights", required=True)
-    ap.add_argument("--uniplanner-weights", required=True)
+    add_checkpoint_args(ap, ("lidar", "uniplanner"), dict(lidar="a LiDARModel state_dict (train_full's lidar_{epoch}.th)",
+                                                          uniplanner="a UniPlanner state_dict (train_full's uniplanner_{epoch}.th)"))
     ap.add_argument("--batch-size", type=int, default=32)
     ap.add_argument("--precision", default="f16", choices=["f16", "fp32"])
     ap.add_argument("--num-workers", type=int, default=16, help="host threads of the loader (record reads, PNG chunk walks)")
@@ -462,25 +541,62 @@ def format_result(r):
     return "\n".join(lines)
 
 
+def headline(r):
+    """the (column, value) pairs of a result in a sweep's table."""
+    cols = [(f"IoU{c}", v) for c, v in enumerate(r["bev_iou"])]
+    cols += [("ped mAP", r["det"]["pedestrian"]["ap"]["mean"]), ("veh mAP", r["det"]["vehicle"]["ap"]["mean"]),
+             ("ADE", r["plan"]["ade"]), ("FDE", r["plan"]["fde"])]
+    if "forecast" in r:
+        cols += [("fc minADE", r["forecast"]["other"]["min_ade"]), ("fc minFDE", r["forecast"]["other"]["min_fde"])]
+    if "forecast_detected" in r:
+        cols.append(("det fc AP", r["forecast_detected"]["ap"]))
+    if "plan_safety" in r:
+        cols += [("collision", r["plan_safety"]["plan"]["collision_rate"]), ("off-road", r["plan_safety"]["plan"]["off_road_rate"])]
+    return cols
+
+
+def report(checkpoints, results, world):
+    """(printout, --json document) of an evaluation: one checkpoint's as format_result and its result dict; a sweep's as one
+    table row per checkpoint and sweep_json."""
+    if len(results) == 1:
+        return format_result(results[0]), results[0]
+    r0 = results[0]
+    text = (f"{r0['samples']} samples, precision {r0['precision']}, {len(results)} checkpoints, {world} rank(s)\n" +
+            sweep_table(checkpoints, [headline(r) for r in results]))
+    return text, sweep_json(checkpoints, results, r0["samples"], world)
+
+
 def main(argv=None):
+    import torch.distributed as dist
     import yaml
     from .train_full import make_models
     args = parse_args(argv)
+    checkpoints = select_checkpoints(args, ("lidar", "uniplanner"))
     with open(args.config_path) as f:
         cfg = yaml.safe_load(f)
-    dev = torch.device("cuda")
-    # inference never runs the nested BEVPlanner: a freshly initialised one fills its place, and no bev_model_dir is read
-    lid, _, uni = make_models(cfg)
-    lid.load_state_dict(torch.load(args.lidar_weights, map_location="cpu"))
-    uni.load_state_dict(torch.load(args.uniplanner_weights, map_location="cpu"))
+    own_group = init_ranks()
+    dev = eval_device()
+    torch.cuda.set_device(dev)
+    pairs = []
+    for _, paths in checkpoints:
+        # inference never runs the nested BEVPlanner: a freshly initialised one fills its place, and no bev_model_dir is read
+        lid, _, uni = make_models(cfg)
+        lid.load_state_dict(torch.load(paths["lidar"], map_location="cpu"))
+        uni.load_state_dict(torch.load(paths["uniplanner"], map_location="cpu"))
+        pairs.append((lid, uni))
     ds = TemporalLiDARPaintedDataset(args.config_path, device=dev, overrides=dict(data_dir=args.data_dir))
-    result = evaluate(lid, uni, ds, args.batch_size, args.precision, args.num_workers, args.forecast, args.forecast_detected,
-                      args.plan_safety)
-    print(format_result(result))
-    if args.json:
-        with open(args.json, "w") as f:
-            json.dump(result, f, indent=1)
-    return result
+    results = evaluate_checkpoints(pairs, ds, args.batch_size, args.precision, args.num_workers, args.forecast,
+                                   args.forecast_detected, args.plan_safety)
+    out = None
+    if results is not None:
+        text, out = report(checkpoints, results, rank_and_world()[1])
+        print(text)
+        if args.json:
+            with open(args.json, "w") as f:
+                json.dump(out, f, indent=1)
+    if own_group:
+        dist.destroy_process_group()
+    return out
 
 
 if __name__ == "__main__":
