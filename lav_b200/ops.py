@@ -2,6 +2,10 @@
 
 PyTorch is plumbing here: allocation, streams, views.  Every function launches hand-written
 sm_90a kernels through lav_b200.capi; nothing falls back to torch math.
+
+Each wrapper checks what it hands to the kernels with _tensor / _out / _host, plus one _require per rule those cannot state,
+so that every pointer it passes covers what the kernel reads or writes; a bad call raises LavbError, never an assert (python -O
+strips asserts).  The checks read tensor metadata only, never device data, so the wrappers can be captured into CUDA graphs.
 """
 import ctypes as C
 import math
@@ -30,6 +34,10 @@ def _ptr(t):
     return C.c_void_p(t.data_ptr()) if t is not None else C.c_void_p(0)
 
 
+def _hptr(a):
+    return a.ctypes.data_as(C.c_void_p)
+
+
 def _need_cuda(*ts):
     for t in ts:
         if t is not None and not t.is_cuda:
@@ -37,9 +45,48 @@ def _need_cuda(*ts):
 
 
 def _require(ok, msg):
-    """argument checks that protect memory: a LavbError, never an assert (python -O strips asserts)."""
     if not ok:
         raise capi.LavbError(msg)
+
+
+def _shape_ok(got, shape):
+    return shape is None or (len(got) == len(shape) and all(s is None or s == g for s, g in zip(shape, got)))
+
+
+def _want(shape, dtypes):
+    """'(*, 2) torch.float32 ' for shape (None, 2) and dtypes (torch.float32,); None / () leave their part out"""
+    s = "" if shape is None else "(" + ", ".join("*" if v is None else str(v) for v in shape) + ("," if len(shape) == 1 else "") + ") "
+    return s + (" or ".join(str(d) for d in dtypes) + " " if dtypes else "")
+
+
+def _tensor(what, name, t, dtype, shape, device=None, contiguous=True):
+    """-> t's shape when t is a CUDA tensor of dtype (one or a tuple; None: any) and shape (an int entry must match, a None entry
+    matches any size; None: any shape), contiguous unless told otherwise, and on ``device`` when one is given; else LavbError
+    (for None too)."""
+    dts = dtype if isinstance(dtype, tuple) else () if dtype is None else (dtype,)
+    if not (torch.is_tensor(t) and t.is_cuda and (not dts or t.dtype in dts) and _shape_ok(t.shape, shape)
+            and (not contiguous or t.is_contiguous()) and (device is None or t.device == device)):
+        got = f"{t.dtype} {tuple(t.shape)} on {t.device}" if torch.is_tensor(t) else type(t).__name__
+        raise capi.LavbError(f"{what}: {name} must be a {'contiguous ' if contiguous else ''}{_want(shape, dts)}tensor on "
+                             f"{device or 'a CUDA device'}, got {got}")
+    return tuple(t.shape)
+
+
+def _out(what, name, out, dtype, shape, device):
+    """a new tensor when ``out`` is None, else ``out`` once _tensor has accepted it."""
+    if out is None:
+        return torch.empty(shape, dtype=dtype, device=device)
+    _tensor(what, name, out, dtype, shape, device)
+    return out
+
+
+def _host(what, name, a, dtype, shape, cast=False):
+    """a host array a kernel reads (numpy or a CPU tensor) -> it as contiguous numpy, converted to dtype with cast=True; raises
+    LavbError unless it has dtype and shape (as _tensor's)."""
+    a = np.ascontiguousarray(a.numpy() if torch.is_tensor(a) else a, dtype=dtype if cast else None)
+    if a.dtype != dtype or not _shape_ok(a.shape, shape):
+        raise capi.LavbError(f"{what}: {name} must be a host {_want(shape, (np.dtype(dtype),))}array, got {a.dtype} {a.shape}")
+    return a
 
 
 def launches():
@@ -51,71 +98,64 @@ _COUNT = [0]
 PROFILE = None     # bench.py sets this to a list to collect (kind, work, start_event, end_event) per launch
 
 
-def _prof_begin():
-    if PROFILE is None:
-        return None
-    e = torch.cuda.Event(enable_timing=True)
-    e.record()
-    return e
-
-
-def _prof_end(kind, work, e0):
+def _launch(fn, *args, launches=1, prof=None):
+    """lib().fn(*args, current stream), its status checked, counted as ``launches`` kernels; with prof = (kind, work) and
+    PROFILE set, timed into PROFILE."""
+    e0 = None
+    if prof is not None and PROFILE is not None:
+        e0 = torch.cuda.Event(enable_timing=True)
+        e0.record()
+    check(getattr(lib(), fn)(*args, _stream()), fn)
     if e0 is not None:
         e1 = torch.cuda.Event(enable_timing=True)
         e1.record()
-        PROFILE.append((kind, work, e0, e1))
+        PROFILE.append((*prof, e0, e1))
+    _COUNT[0] += launches
 
 
 # ----------------------------------------------------------------------------- painting
 def paint(points, sem, cams, mode, copy_cols=0, out=None, out_col0=None):
     """points (N,>=3) fp32; sem (ncam,C,H,W)-shaped tensor with ANY strides (NCHW or channels-last);
     cams (ncam,41) float32 numpy (K|lidar_to_world|world_to_cam).  See lavb_paint in include/lav_b200.h."""
-    _need_cuda(points, sem)
-    assert points.dtype == torch.float32 and sem.dtype == torch.float32 and points.dim() == 2
-    assert points.stride(1) == 1
-    ncam, c_in, h, w = sem.shape
+    n, _ = _tensor("paint", "points", points, torch.float32, (None, None), contiguous=False)
+    _require(points.stride(1) == 1, "paint: points must have unit stride along a row")
+    ncam, c_in, h, w = _tensor("paint", "sem", sem, torch.float32, (None,) * 4, contiguous=False)
     c_out = c_in if mode == 0 else c_in - 1
-    n = points.shape[0]
     if out_col0 is None:
         out_col0 = copy_cols
     if out is None:
         out = torch.empty((n, out_col0 + c_out), dtype=torch.float32, device=points.device)
-    assert out.stride(1) == 1
-    cams = np.ascontiguousarray(cams, dtype=np.float32)
-    assert cams.shape == (ncam, 41)
+    _require(out.stride(1) == 1, "paint: out must have unit stride along a row")
+    cams = _host("paint", "cams", cams, np.float32, (ncam, 41), cast=True)
     s = sem.stride()
-    check(lib().lavb_paint(_ptr(points), n, points.stride(0), _ptr(sem), ncam, c_in, h, w, s[0], s[1], s[2], s[3],
-                           cams.ctypes.data_as(C.c_void_p), mode, _ptr(out), out.stride(0), out_col0, copy_cols, _stream()),
-          "lavb_paint")
-    _COUNT[0] += 1
+    _launch("lavb_paint", _ptr(points), n, points.stride(0), _ptr(sem), ncam, c_in, h, w, s[0], s[1], s[2], s[3], _hptr(cams), mode,
+            _ptr(out), out.stride(0), out_col0, copy_cols)
     return out
 
 
 def stack_sweep(src, R, dx, dy, time_idx, n_time, dst, roof_filter=False):
     """dst (n, src_cols+n_time) <- [src[:, :3] @ R + (dx,dy,0) | src[:,3:] | one_hot(time_idx)]"""
-    _need_cuda(src, dst)
-    assert src.is_contiguous() and dst.is_contiguous() and dst.shape == (src.shape[0], src.shape[1] + n_time)
+    _tensor("stack_sweep", "src", src, None, None)
+    _tensor("stack_sweep", "dst", dst, None, (src.shape[0], src.shape[1] + n_time))
     R = np.ascontiguousarray(R, dtype=np.float32)
-    check(lib().lavb_stack_sweep(_ptr(src), src.shape[0], src.shape[1], R.ctypes.data_as(C.c_void_p), float(dx), float(dy),
-                                 time_idx, n_time, int(roof_filter), _ptr(dst), _stream()), "lavb_stack_sweep")
-    _COUNT[0] += 1
+    _launch("lavb_stack_sweep", _ptr(src), src.shape[0], src.shape[1], _hptr(R), float(dx), float(dy), time_idx, n_time,
+            int(roof_filter), _ptr(dst))
     return dst
 
 
 def roof_filter(sweeps, pad_nan=False, out=None):
     """LAVAgent.preprocess (lav_agent.py:448-457) on the device, order preserving.  sweeps: (n, cols) or (F, n, cols) fp32
     contiguous -> (out like sweeps with the kept rows first, counts (F,) int32).  pad_nan fills rows past the count with NaN."""
-    _need_cuda(sweeps)
-    assert sweeps.dtype == torch.float32 and sweeps.is_contiguous() and sweeps.dim() in (2, 3)
+    _tensor("roof_filter", "sweeps", sweeps, torch.float32, None)
+    _require(sweeps.dim() in (2, 3), f"roof_filter: sweeps must be (n, cols) or (F, n, cols), got {tuple(sweeps.shape)}")
     x = sweeps if sweeps.dim() == 3 else sweeps[None]
     f, n, cols = x.shape
     if out is None:
         out = torch.empty_like(x)
-    assert out.is_contiguous() and out.shape == x.shape and out.data_ptr() != x.data_ptr()
+    _tensor("roof_filter", "out", out, None, x.shape)
+    _require(out.data_ptr() != x.data_ptr(), "roof_filter: out must not be the sweeps' storage")
     counts = torch.empty((f,), dtype=torch.int32, device=x.device)
-    check(lib().lavb_roof_filter(_ptr(x), f, n, cols, n * cols, _ptr(out), n * cols, _ptr(counts), int(pad_nan), _stream()),
-          "lavb_roof_filter")
-    _COUNT[0] += 1
+    _launch("lavb_roof_filter", _ptr(x), f, n, cols, n * cols, _ptr(out), n * cols, _ptr(counts), int(pad_nan))
     return (out if sweeps.dim() == 3 else out[0]), counts
 
 
@@ -142,44 +182,34 @@ def _clouds(starts, counts, pts, what):
     return b, st, ct
 
 
-def _check_point_mlp(what, pts, w1, s1, t1, w2, s2, t2):
-    """the encoders are built for the v2 point MLP only: w1 (64, 16), w2 (64, 64), s / t (64,), contiguous fp32 on pts' device,
-    and rows of pts at least 11 floats wide."""
-    for name, t, shape in (("w1", w1, (64, 16)), ("s1", s1, (64,)), ("t1", t1, (64,)), ("w2", w2, (64, 64)), ("s2", s2, (64,)),
-                           ("t2", t2, (64,))):
-        if (not torch.is_tensor(t) or tuple(t.shape) != shape or t.dtype != torch.float32 or not t.is_contiguous()
-                or t.device != pts.device):
-            got = f"{t.dtype} {tuple(t.shape)}" if torch.is_tensor(t) else type(t).__name__
-            raise capi.LavbError(f"{what}: {name} must be a contiguous fp32 {shape} tensor on {pts.device}, got {got}")
-    if pts.shape[1] < 11:
-        raise capi.LavbError(f"{what}: point rows must hold at least 11 floats, got {pts.shape[1]}")
+# the encoders are built for the v2 point MLP only: these fp32 parameters, and point rows of at least 11 floats
+_POINT_MLP = (("w1", (64, 16)), ("s1", (64,)), ("t1", (64,)), ("w2", (64, 64)), ("s2", (64,)), ("t2", (64,)))
 
 
 def pillar_forward(pts, starts, counts, grid, w1, s1, t1, w2, s2, t2):
     """pts: 2-D fp32 row buffer (rows of >= D floats); cloud b = rows [starts[b], starts[b]+counts[b]).
     Returns the NHWC canvas (B, ny, nx, H2) fp32."""
-    _need_cuda(pts, w1, w2)
-    assert pts.dtype == torch.float32 and pts.dim() == 2 and pts.stride(1) == 1
-    _check_point_mlp("pillar_forward", pts, w1, s1, t1, w2, s2, t2)
+    _tensor("pillar_forward", "pts", pts, torch.float32, (None, None), contiguous=False)
+    _require(pts.stride(1) == 1 and pts.shape[1] >= 11, f"pillar_forward: point rows must be unit-stride and hold at least 11 "
+             f"floats, got {tuple(pts.shape)} with strides {pts.stride()}")
+    for (name, shape), t in zip(_POINT_MLP, (w1, s1, t1, w2, s2, t2)):
+        _tensor("pillar_forward", name, t, torch.float32, shape, pts.device)
     min_x, max_x, min_y, max_y, ppm, nx, ny = grid
     d = w1.shape[1] - 5
     b, st, ct = _clouds(starts, counts, pts, "pillar_forward")
     canvas = torch.empty((b, ny, nx, w2.shape[0]), dtype=torch.float32, device=pts.device)
     ws = _workspace(pts.device, lib().lavb_pillar_workspace_bytes(b, nx, ny))
-    e0 = _prof_begin()
-    check(lib().lavb_pillar_forward(_ptr(pts), pts.stride(0), d, st, ct, b, min_x, max_x, min_y, max_y, ppm, nx, ny,
-                                    _ptr(w1), _ptr(s1), _ptr(t1), w1.shape[0], _ptr(w2), _ptr(s2), _ptr(t2), w2.shape[0],
-                                    _ptr(canvas), F32, _ptr(ws), _stream()), "lavb_pillar_forward")
     # algorithmic bytes (SURVEY 8d): read P x D fp32 points once + write the canvas once
-    _prof_end("pillar", float(sum(int(c) for c in counts)) * d * 4 + canvas.numel() * 4, e0)
-    _COUNT[0] += 4
+    _launch("lavb_pillar_forward", _ptr(pts), pts.stride(0), d, st, ct, b, min_x, max_x, min_y, max_y, ppm, nx, ny, _ptr(w1),
+            _ptr(s1), _ptr(t1), w1.shape[0], _ptr(w2), _ptr(s2), _ptr(t2), w2.shape[0], _ptr(canvas), F32, _ptr(ws), launches=4,
+            prof=("pillar", float(sum(int(c) for c in counts)) * d * 4 + canvas.numel() * 4))
     return canvas
 
 
 def pillar_decorate(pts, starts, counts, grid, d):
     """training stage 0: returns (feat (M,d+5) fp32, cell (M,) int32), rows in input order (clouds in batch order)."""
-    _need_cuda(pts)
-    assert pts.dtype == torch.float32 and pts.dim() == 2 and pts.stride(1) == 1
+    _tensor("pillar_decorate", "pts", pts, torch.float32, (None, None), contiguous=False)
+    _require(pts.stride(1) == 1, "pillar_decorate: pts must have unit stride along a row")
     min_x, max_x, min_y, max_y, ppm, nx, ny = grid
     b, st, ct = _clouds(starts, counts, pts, "pillar_decorate")
     ws = _workspace(pts.device, lib().lavb_pillar_workspace_bytes(b, nx, ny))
@@ -187,42 +217,33 @@ def pillar_decorate(pts, starts, counts, grid, d):
     feat = torch.empty((total, d + 5), dtype=torch.float32, device=pts.device)
     cell = torch.empty((total,), dtype=torch.int32, device=pts.device)
     m = C.c_int(0)
-    check(lib().lavb_pillar_decorate(_ptr(pts), pts.stride(0), d, st, ct, b, min_x, max_x, min_y, max_y, ppm, nx, ny,
-                                     _ptr(feat), _ptr(cell), C.byref(m), _ptr(ws), _stream()), "lavb_pillar_decorate")
-    _COUNT[0] += 4
+    _launch("lavb_pillar_decorate", _ptr(pts), pts.stride(0), d, st, ct, b, min_x, max_x, min_y, max_y, ppm, nx, ny, _ptr(feat),
+            _ptr(cell), C.byref(m), _ptr(ws), launches=4)
     return feat[:m.value], cell[:m.value]
 
 
 def pillar_scatter_max(h, cell, n_cells, want_argmax=True):
     """training stage 1: h (M,C) fp32 >= 0, cell (M,) int32 in [0, n_cells) -> (canvas (n_cells,C) fp32, arg (n_cells,C) int32
     or None).  See lavb_pillar_scatter_max in include/lav_b200.h for the tie rule and the empty-cell values."""
-    _need_cuda(h, cell)
-    assert h.dtype == torch.float32 and h.dim() == 2, "h must be (M, C) fp32"
-    assert cell.dtype == torch.int32 and cell.shape == (h.shape[0],) and cell.is_contiguous(), "cell must be (M,) int32"
-    assert cell.device == h.device and int(n_cells) >= 0
+    m, c = _tensor("pillar_scatter_max", "h", h, torch.float32, (None, None), contiguous=False)
+    _tensor("pillar_scatter_max", "cell", cell, torch.int32, (m,), h.device)
+    _require(int(n_cells) >= 0, f"pillar_scatter_max: n_cells = {n_cells} < 0")
     h = h.contiguous()
-    m, c = h.shape
     canvas = torch.empty((n_cells, c), dtype=torch.float32, device=h.device)
     arg = torch.empty((n_cells, c), dtype=torch.int32, device=h.device) if want_argmax else None
-    check(lib().lavb_pillar_scatter_max(_ptr(h), _ptr(cell), m, c, n_cells, _ptr(canvas), _ptr(arg), _stream()),
-          "lavb_pillar_scatter_max")
-    _COUNT[0] += 2
+    _launch("lavb_pillar_scatter_max", _ptr(h), _ptr(cell), m, c, n_cells, _ptr(canvas), _ptr(arg), launches=2)
     return canvas, arg
 
 
 def pillar_scatter_max_bwd(gcanvas, arg, cell, m):
     """gh (m,C) fp32: gh[r, c] = gcanvas[cell[r], c] where arg[cell[r], c] == r, else 0.  gcanvas may have any strides."""
-    _need_cuda(gcanvas, arg, cell)
-    assert gcanvas.dtype == torch.float32 and gcanvas.dim() == 2, "gcanvas must be (n_cells, C) fp32"
-    assert arg.dtype == torch.int32 and arg.shape == gcanvas.shape and arg.is_contiguous(), "arg must be (n_cells, C) int32"
-    assert cell.dtype == torch.int32 and cell.shape == (m,) and cell.is_contiguous(), "cell must be (m,) int32"
-    assert gcanvas.device == arg.device == cell.device
+    shape = _tensor("pillar_scatter_max_bwd", "gcanvas", gcanvas, torch.float32, (None, None), contiguous=False)
+    _tensor("pillar_scatter_max_bwd", "arg", arg, torch.int32, shape, gcanvas.device)
+    _tensor("pillar_scatter_max_bwd", "cell", cell, torch.int32, (m,), gcanvas.device)
     gcanvas = gcanvas.contiguous()
     c = gcanvas.shape[-1]
     gh = torch.empty((m, c), dtype=torch.float32, device=gcanvas.device)
-    check(lib().lavb_pillar_scatter_max_bwd(_ptr(gcanvas), _ptr(arg), _ptr(cell), m, c, _ptr(gh), _stream()),
-          "lavb_pillar_scatter_max_bwd")
-    _COUNT[0] += 1
+    _launch("lavb_pillar_scatter_max_bwd", _ptr(gcanvas), _ptr(arg), _ptr(cell), m, c, _ptr(gh))
     return gh
 
 
@@ -232,29 +253,27 @@ def conv_taps(x, cin, in_coff, out, cout, out_coff, hog, wog, in_s, out_s, out_o
     """x, out, res: contiguous NHWC buffers (N,H,W,Ctot).  taps: list of (dy,dx).
     umma=False: CUDA-core kernel, w (ntaps,cin,cout_pad16) fp32.
     umma=True : wgmma kernel, x f16, w (ntaps,cout,cin) f16."""
-    _need_cuda(x, out, w)
-    assert x.is_contiguous() and out.is_contiguous() and w.is_contiguous()
+    _tensor("conv_taps", "x", x, h16() if umma else None, (None,) * 4)
+    _tensor("conv_taps", "out", out, torch.float32 if d2s_nout else None, (x.shape[0], None, None, d2s_nout or None))
+    _tensor("conv_taps", "w", w, h16() if umma else torch.float32,
+            (len(taps), (cout + 31) // 32 * 32, cin) if umma else (len(taps), cin, (cout + 15) // 16 * 16))
+    _require(not d2s_nout or (umma and cout == 32 and 4 * d2s_nout <= 32),
+             f"conv_taps: d2s_nout = {d2s_nout} needs the wgmma kernel, cout 32 and 4 * d2s_nout <= 32")
     d = ConvDesc()
     d.inp, d.in_dtype = x.data_ptr(), _DT[x.dtype]
     d.n, d.hin, d.win, d.in_cstride = x.shape
     d.cin, d.in_coff = cin, in_coff
     d.out, d.out_dtype = out.data_ptr(), _DT[out.dtype]
-    assert out.shape[0] == x.shape[0]
     _, d.hout, d.wout, d.out_cstride = out.shape
     d.cout, d.out_coff = cout, out_coff
     d.d2s_nout = d2s_nout
     if d2s_nout:
-        assert umma and out.dtype == torch.float32 and out.shape[3] == d2s_nout and cout == 32 and 4 * d2s_nout <= 32
         d.out_cstride, d.out_coff = 32, 0        # (validated as a 32-column GEMM; addressing is done by the d2s epilogue)
     d.hog, d.wog = hog, wog
     d.in_sy, d.in_sx = in_s
     d.out_sy, d.out_sx = out_s
     d.out_oy, d.out_ox = out_o
     d.ntaps = len(taps)
-    if umma:
-        assert w.dtype == h16() and tuple(w.shape) == (len(taps), (cout + 31) // 32 * 32, cin) and x.dtype == h16()
-    else:
-        assert w.dtype == torch.float32 and tuple(w.shape) == (len(taps), cin, (cout + 15) // 16 * 16)
     for i, (dy, dx) in enumerate(taps):
         d.dy[i], d.dx[i] = dy, dx
     d.w = w.data_ptr()
@@ -262,44 +281,33 @@ def conv_taps(x, cin, in_coff, out, cout, out_coff, hog, wog, in_s, out_s, out_o
     d.scale = scale.data_ptr() if scale is not None else None
     d.shift = shift.data_ptr() if shift is not None else None
     if res is not None:
-        assert res.is_contiguous() and res.shape[:3] == out.shape[:3]
+        _tensor("conv_taps", "res", res, None, (*out.shape[:3], None))
         d.res, d.res_dtype, d.res_cstride, d.res_coff = res.data_ptr(), _DT[res.dtype], res.shape[3], res_coff
     d.pre_relu, d.post_relu, d.sigmoid = int(pre_relu), int(post_relu), int(sigmoid)
-    if umma:
-        e0 = _prof_begin()
-        check(lib().lavb_conv_umma(C.byref(d), _stream()), "lavb_conv_umma")
-        _prof_end(f"umma:{cin}->{cout}x{len(taps)}taps@{hog}x{wog}", 2.0 * x.shape[0] * hog * wog * cout * cin * len(taps), e0)
-    else:
-        check(lib().lavb_conv_taps(C.byref(d), _stream()), "lavb_conv_taps")
-    _COUNT[0] += 1
+    _launch("lavb_conv_umma" if umma else "lavb_conv_taps", C.byref(d),
+            prof=(f"umma:{cin}->{cout}x{len(taps)}taps@{hog}x{wog}", 2.0 * x.shape[0] * hog * wog * cout * cin * len(taps))
+            if umma else None)
     return out
 
 
 def pool2_affine_relu(x, c, in_coff, scale, shift, out, out_coff):
     _need_cuda(x, out)
     n, h, w, cs = x.shape
-    check(lib().lavb_pool2_affine_relu(_ptr(x), _DT[x.dtype], n, h, w, c, cs, in_coff, _ptr(scale), _ptr(shift), _ptr(out),
-                                       out.shape[3], out_coff, _stream()), "lavb_pool2_affine_relu")
-    _COUNT[0] += 1
+    _launch("lavb_pool2_affine_relu", _ptr(x), _DT[x.dtype], n, h, w, c, cs, in_coff, _ptr(scale), _ptr(shift), _ptr(out),
+            out.shape[3], out_coff)
     return out
 
 
 def rgb_normalize(rgb, out_dtype=torch.float32):
     """uint8 (N,H,W,3) or float (N,3,H,W) in 0..255 -> NHWC4 normalised ((x/255-.5)*2, 4th channel 0)."""
-    _need_cuda(rgb)
-    if rgb.dtype == torch.uint8:
-        assert rgb.dim() == 4 and rgb.shape[3] == 3
-        n, h, w, _ = rgb.shape
-        u8 = 1
-        rgb = rgb.contiguous()
+    if torch.is_tensor(rgb) and rgb.dtype == torch.uint8:
+        n, h, w, _ = _tensor("rgb_normalize", "rgb", rgb, None, (None, None, None, 3), contiguous=False)
+        rgb, u8 = rgb.contiguous(), 1
     else:
-        assert rgb.dim() == 4 and rgb.shape[1] == 3
-        n, _, h, w = rgb.shape
-        u8 = 0
-        rgb = rgb.float().contiguous()
+        n, _, h, w = _tensor("rgb_normalize", "rgb", rgb, None, (None, 3, None, None), contiguous=False)
+        rgb, u8 = rgb.float().contiguous(), 0
     out = torch.empty((n, h, w, 4), dtype=out_dtype, device=rgb.device)
-    check(lib().lavb_rgb_normalize(_ptr(rgb), u8, n, h, w, _ptr(out), _DT[out_dtype], _stream()), "lavb_rgb_normalize")
-    _COUNT[0] += 1
+    _launch("lavb_rgb_normalize", _ptr(rgb), u8, n, h, w, _ptr(out), _DT[out_dtype])
     return out
 
 
@@ -309,8 +317,7 @@ def convert(src, dtype):
     if src.dtype == dtype:
         return src
     dst = torch.empty(src.shape, dtype=dtype, device=src.device)
-    check(lib().lavb_convert(_ptr(src), _DT[src.dtype], _ptr(dst), _DT[dtype], src.numel(), _stream()), "lavb_convert")
-    _COUNT[0] += 1
+    _launch("lavb_convert", _ptr(src), _DT[src.dtype], _ptr(dst), _DT[dtype], src.numel())
     return dst
 
 
@@ -326,13 +333,10 @@ def _crop_poses(what, frame_idx, theta, b):
     """the K crop poses as the kernels read them: frame_idx (K,) of any integer type -> int32 (values clamped to [0, B) first,
     as the kernels clamp, so an int64 index past the int32 range still means the last frame), theta (K,2,3) -> fp32; both
     contiguous.  Raises LavbError when they do not describe the same K crops."""
-    if theta.dim() != 3 or tuple(theta.shape[1:]) != (2, 3):
-        raise capi.LavbError(f"{what}: theta must be (K, 2, 3), got {tuple(theta.shape)}")
-    k = theta.shape[0]
-    if frame_idx.dim() != 1 or frame_idx.numel() != k:
-        raise capi.LavbError(f"{what}: frame_idx {tuple(frame_idx.shape)} does not hold one frame per crop (K = {k})")
-    if frame_idx.dtype.is_floating_point or frame_idx.dtype.is_complex or frame_idx.dtype == torch.bool:
-        raise capi.LavbError(f"{what}: frame_idx must be an integer tensor, got {frame_idx.dtype}")
+    k, _, _ = _tensor(what, "theta", theta, None, (None, 2, 3), contiguous=False)
+    _tensor(what, "frame_idx", frame_idx, None, (k,), contiguous=False)
+    _require(not (frame_idx.dtype.is_floating_point or frame_idx.dtype.is_complex or frame_idx.dtype == torch.bool),
+             f"{what}: frame_idx must be an integer tensor, got {frame_idx.dtype}")
     if frame_idx.dtype != torch.int32:
         frame_idx = frame_idx.clamp(0, b - 1).to(torch.int32)
     return k, frame_idx.contiguous(), theta.float().contiguous()
@@ -341,16 +345,14 @@ def _crop_poses(what, frame_idx, theta, b):
 def crop_bilinear(feats_nhwc, frame_idx, theta, crop_size):
     """feats_nhwc (B,H,W,C) contiguous fp32 (C % 4 == 0) or h16 (C % 8 == 0); frame_idx (K,) integer; theta (K,2,3) ->
     (K,crop,crop,C) in the feature dtype.  Frame indices outside [0, B) are clamped to the nearest frame."""
-    _need_cuda(feats_nhwc, frame_idx, theta)
-    if not crop_supported(feats_nhwc):
-        raise capi.LavbError(f"crop_bilinear: need a contiguous, 16-byte aligned (B,H,W,C) map, fp32 with C % 4 == 0 or "
-                             f"{h16()} with C % 8 == 0; got {feats_nhwc.dtype} {tuple(feats_nhwc.shape)}")
+    _need_cuda(feats_nhwc)
+    _require(crop_supported(feats_nhwc), f"crop_bilinear: need a contiguous, 16-byte aligned (B,H,W,C) map, fp32 with C % 4 == 0 "
+             f"or {h16()} with C % 8 == 0; got {feats_nhwc.dtype} {tuple(feats_nhwc.shape)}")
     b, h, w, c = feats_nhwc.shape
     k, frame_idx, theta = _crop_poses("crop_bilinear", frame_idx, theta, b)
     out = torch.empty((k, crop_size, crop_size, c), dtype=feats_nhwc.dtype, device=feats_nhwc.device)
-    check(lib().lavb_crop_bilinear(_ptr(feats_nhwc), _DT[feats_nhwc.dtype], b, h, w, c, _ptr(frame_idx), _ptr(theta), k, crop_size,
-                                   _ptr(out), _stream()), "lavb_crop_bilinear")
-    _COUNT[0] += 1
+    _launch("lavb_crop_bilinear", _ptr(feats_nhwc), _DT[feats_nhwc.dtype], b, h, w, c, _ptr(frame_idx), _ptr(theta), k, crop_size,
+            _ptr(out))
     return out
 
 
@@ -358,51 +360,30 @@ def crop_bilinear_u8(bev_u8, frame_idx, theta, crop_size, out=None):
     """bev_u8 (B,C,H,W) contiguous uint8; frame_idx (K,) int32; theta (K,2,3) fp32 -> fp32 NCHW (K,C,crop,crop): the crops of
     crop_bilinear read straight from a uint8 planar map (bit-identical to crop_bilinear on its float copy).  Frame indices
     outside [0, B) are clamped to the nearest frame.  ``out`` (K,C,crop,crop) fp32 contiguous is written in full if given."""
-    _need_cuda(bev_u8, frame_idx, theta)
-    if bev_u8.dtype != torch.uint8 or bev_u8.dim() != 4:
-        raise capi.LavbError(f"crop_bilinear_u8: need a 4-d uint8 map, got {bev_u8.dtype} {tuple(bev_u8.shape)}")
-    if not bev_u8.is_contiguous():
-        raise capi.LavbError("crop_bilinear_u8: the map must be contiguous (B,C,H,W)")
-    b, c, h, w = bev_u8.shape
-    k = theta.shape[0]
-    if tuple(theta.shape) != (k, 2, 3) or frame_idx.numel() != k:
-        raise capi.LavbError(f"crop_bilinear_u8: theta {tuple(theta.shape)} / frame_idx {tuple(frame_idx.shape)} do not describe K crops")
+    _need_cuda(frame_idx)
+    b, c, h, w = _tensor("crop_bilinear_u8", "bev_u8", bev_u8, torch.uint8, (None,) * 4)
+    k, _, _ = _tensor("crop_bilinear_u8", "theta", theta, None, (None, 2, 3), contiguous=False)
+    _require(frame_idx.numel() == k, f"crop_bilinear_u8: frame_idx {tuple(frame_idx.shape)} does not hold one frame per crop (K = {k})")
     theta = theta.float().contiguous()
     frame_idx = frame_idx.to(torch.int32).contiguous()
-    if out is None:
-        out = torch.empty((k, c, crop_size, crop_size), dtype=torch.float32, device=bev_u8.device)
-    elif tuple(out.shape) != (k, c, crop_size, crop_size) or out.dtype != torch.float32 or not out.is_contiguous():
-        raise capi.LavbError(f"crop_bilinear_u8: out must be a contiguous fp32 ({k}, {c}, {crop_size}, {crop_size}) tensor")
-    check(lib().lavb_crop_bilinear_u8(_ptr(bev_u8), b, c, h, w, _ptr(frame_idx), _ptr(theta), k, crop_size, _ptr(out), _stream()),
-          "lavb_crop_bilinear_u8")
-    _COUNT[0] += 1
+    out = _out("crop_bilinear_u8", "out", out, torch.float32, (k, c, crop_size, crop_size), bev_u8.device)
+    _launch("lavb_crop_bilinear_u8", _ptr(bev_u8), b, c, h, w, _ptr(frame_idx), _ptr(theta), k, crop_size, _ptr(out))
     return out
 
 
 def crop_bilinear_bwd(gout_nhwc, frame_idx, theta, feat_shape, out=None):
     """gout_nhwc (K,crop,crop,C) fp32 contiguous -> gradient of crop_bilinear w.r.t. the (B,H,W,C) fp32 feature map.
     ``out`` (B,H,W,C) fp32 contiguous is written in full if given (zeros for every frame no crop samples)."""
-    _need_cuda(gout_nhwc, frame_idx, theta)
-    if len(feat_shape) != 4:
-        raise capi.LavbError(f"crop_bilinear_bwd: feat_shape must be (B, H, W, C), got {tuple(feat_shape)}")
+    _require(len(feat_shape) == 4, f"crop_bilinear_bwd: feat_shape must be (B, H, W, C), got {tuple(feat_shape)}")
     b, h, w, c = (int(v) for v in feat_shape)
-    if gout_nhwc.dtype != torch.float32 or gout_nhwc.dim() != 4 or not gout_nhwc.is_contiguous() or gout_nhwc.data_ptr() % 16:
-        raise capi.LavbError(f"crop_bilinear_bwd: gout must be a contiguous, 16-byte aligned fp32 (K, crop, crop, C) tensor, "
-                             f"got {gout_nhwc.dtype} {tuple(gout_nhwc.shape)}")
+    _tensor("crop_bilinear_bwd", "gout", gout_nhwc, torch.float32, (None,) * 4)
+    _require(gout_nhwc.data_ptr() % 16 == 0, "crop_bilinear_bwd: gout must be 16-byte aligned")
     k, frame_idx, theta = _crop_poses("crop_bilinear_bwd", frame_idx, theta, b)
     crop = gout_nhwc.shape[1]
-    if tuple(gout_nhwc.shape) != (k, crop, crop, c):
-        raise capi.LavbError(f"crop_bilinear_bwd: gout {tuple(gout_nhwc.shape)} does not match {k} square crops of the "
-                             f"{c}-channel map {tuple(feat_shape)}")
-    if out is None:
-        gfeat = torch.empty((b, h, w, c), dtype=torch.float32, device=gout_nhwc.device)
-    elif tuple(out.shape) != (b, h, w, c) or out.dtype != torch.float32 or not out.is_contiguous() or out.device != gout_nhwc.device:
-        raise capi.LavbError(f"crop_bilinear_bwd: out must be a contiguous fp32 ({b}, {h}, {w}, {c}) tensor on {gout_nhwc.device}")
-    else:
-        gfeat = out
-    check(lib().lavb_crop_bilinear_bwd(_ptr(gout_nhwc), b, h, w, c, _ptr(frame_idx), _ptr(theta), k, crop, _ptr(gfeat), _stream()),
-          "lavb_crop_bilinear_bwd")
-    _COUNT[0] += 1
+    _require(tuple(gout_nhwc.shape) == (k, crop, crop, c), f"crop_bilinear_bwd: gout {tuple(gout_nhwc.shape)} does not match {k} "
+             f"square crops of the {c}-channel map {tuple(feat_shape)}")
+    gfeat = _out("crop_bilinear_bwd", "out", out, torch.float32, (b, h, w, c), gout_nhwc.device)
+    _launch("lavb_crop_bilinear_bwd", _ptr(gout_nhwc), b, h, w, c, _ptr(frame_idx), _ptr(theta), k, crop, _ptr(gfeat))
     return gfeat
 
 
@@ -411,7 +392,6 @@ class CropBilinear(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, feats_nhwc, frame_idx, theta, crop_size):
-        _need_cuda(frame_idx, theta)
         _, frame_idx, theta = _crop_poses("CropBilinear", frame_idx, theta.detach(), feats_nhwc.shape[0])
         ctx.save_for_backward(frame_idx, theta)
         ctx.feat_shape = tuple(feats_nhwc.shape)
@@ -425,31 +405,26 @@ class CropBilinear(torch.autograd.Function):
 
 def deconv3x3s2_small(x, groups, cin_g, w, bias, n_outs, sigmoids):
     """x NHWC (N,H,W,Ctot); w fp32 (G,cin_g,9,4); bias (G,4) -> list of fp32 NHWC (N,2H,2W,n_out[g])."""
-    _need_cuda(x, w, bias)
-    assert x.is_contiguous() and w.is_contiguous() and bias.is_contiguous()
-    n, h, wd, cs = x.shape
+    n, h, wd, cs = _tensor("deconv3x3s2_small", "x", x, None, (None,) * 4)
+    _tensor("deconv3x3s2_small", "w", w, None, None)
+    _tensor("deconv3x3s2_small", "bias", bias, None, None)
     outs = [torch.empty((n, 2 * h, 2 * wd, no), dtype=torch.float32, device=x.device) for no in n_outs]
     ptrs = (C.c_void_p * groups)(*[o.data_ptr() for o in outs])
     no = (C.c_int * groups)(*n_outs)
     sg = (C.c_int * groups)(*[int(s) for s in sigmoids])
-    check(lib().lavb_deconv3x3s2_small(_ptr(x), _DT[x.dtype], n, h, wd, cs, groups, cin_g, _ptr(w), _ptr(bias), no, sg, ptrs,
-                                       _stream()), "lavb_deconv3x3s2_small")
-    _COUNT[0] += 1
+    _launch("lavb_deconv3x3s2_small", _ptr(x), _DT[x.dtype], n, h, wd, cs, groups, cin_g, _ptr(w), _ptr(bias), no, sg, ptrs)
     return outs
 
 
 def paint_batched(points, sem, cams, mode, copy_cols, out):
     """points (F,N,>=3) fp32 contiguous; sem logical (F,ncam,C,H,W) any strides; out (F,N,copy_cols+c_out) contiguous."""
-    _need_cuda(points, sem, out)
-    assert points.is_contiguous() and out.is_contiguous() and points.dtype == torch.float32 and sem.dtype == torch.float32
-    f, n, ps = points.shape
-    _, ncam, c_in, h, w = sem.shape
-    cams = np.ascontiguousarray(cams, dtype=np.float32)
+    f, n, ps = _tensor("paint_batched", "points", points, torch.float32, (None,) * 3)
+    _, ncam, c_in, h, w = _tensor("paint_batched", "sem", sem, torch.float32, (None,) * 5, contiguous=False)
+    _tensor("paint_batched", "out", out, None, None)
+    cams = _host("paint_batched", "cams", cams, np.float32, None, cast=True)
     s = sem.stride()
-    check(lib().lavb_paint_batched(_ptr(points), f, n, ps, n * ps, _ptr(sem), ncam, c_in, h, w, s[0], s[1], s[2], s[3], s[4],
-                                   cams.ctypes.data_as(C.c_void_p), mode, _ptr(out), out.shape[2], n * out.shape[2], copy_cols,
-                                   copy_cols, _stream()), "lavb_paint_batched")
-    _COUNT[0] += 1
+    _launch("lavb_paint_batched", _ptr(points), f, n, ps, n * ps, _ptr(sem), ncam, c_in, h, w, s[0], s[1], s[2], s[3], s[4],
+            _hptr(cams), mode, _ptr(out), out.shape[2], n * out.shape[2], copy_cols, copy_cols)
     return out
 
 
@@ -457,7 +432,7 @@ def pack_deconv2x2(weight, bias):
     """ConvTranspose2d(16, C, 2, stride=2) parameters (weight (16,C,2,2), bias (C,)) -> the 520-float table
     lavb_paint_deconv_batched reads: w[v%2][u%2][c_in][8] | bias[8]."""
     cin, c, kh, kw = weight.shape
-    assert cin == 16 and kh == 2 and kw == 2 and c <= 8
+    _require(cin == 16 and kh == 2 and kw == 2 and c <= 8, f"pack_deconv2x2: weight must be (16, C <= 8, 2, 2), got {tuple(weight.shape)}")
     w = torch.zeros((2, 2, 16, 8), dtype=torch.float32, device=weight.device)
     w[:, :, :, :c] = weight.detach().float().permute(2, 3, 0, 1)
     b = torch.zeros((8,), dtype=torch.float32, device=weight.device)
@@ -468,17 +443,16 @@ def pack_deconv2x2(weight, bias):
 def paint_deconv_batched(points, feat, n_classes, deconv, cams, copy_cols, out, image_hw):
     """points (F,N,>=3) fp32; feat NHWC (F*ncam, H/2, W/2, 16) fp32 / h16 = ERFNet decoder output before output_conv;
     deconv = pack_deconv2x2(...); out (F,N,copy_cols + n_classes-1)."""
-    _need_cuda(points, feat, out, deconv)
-    assert points.is_contiguous() and out.is_contiguous() and feat.is_contiguous() and points.dtype == torch.float32
-    f, n, ps = points.shape
+    _need_cuda(deconv)
+    f, n, ps = _tensor("paint_deconv_batched", "points", points, torch.float32, (None,) * 3)
+    _tensor("paint_deconv_batched", "out", out, None, None)
     h, w = image_hw
-    cams = np.ascontiguousarray(cams, dtype=np.float32)
+    cams = _host("paint_deconv_batched", "cams", cams, np.float32, None, cast=True)
     ncam = cams.shape[0]
-    assert feat.shape == (f * ncam, h // 2, w // 2, 16) and deconv.numel() == 520
-    check(lib().lavb_paint_deconv_batched(_ptr(points), f, n, ps, n * ps, _ptr(feat), _DT[feat.dtype], ncam, n_classes, h, w,
-                                          _ptr(deconv), cams.ctypes.data_as(C.c_void_p), _ptr(out), out.shape[2], n * out.shape[2],
-                                          copy_cols, copy_cols, _stream()), "lavb_paint_deconv_batched")
-    _COUNT[0] += 1
+    _tensor("paint_deconv_batched", "feat", feat, None, (f * ncam, h // 2, w // 2, 16))
+    _require(deconv.numel() == 520, "paint_deconv_batched: deconv must be the 520-float pack_deconv2x2 table")
+    _launch("lavb_paint_deconv_batched", _ptr(points), f, n, ps, n * ps, _ptr(feat), _DT[feat.dtype], ncam, n_classes, h, w,
+            _ptr(deconv), _hptr(cams), _ptr(out), out.shape[2], n * out.shape[2], copy_cols, copy_cols)
     return out
 
 
@@ -496,29 +470,15 @@ def seg_confusion(feat, table, labels, lut, n_classes, out=None):
     (N, H/2, W/2, 16) fp32 / h16 = the input of output_conv (forward_features_nhwc); table = pack_deconv2x2 of output_conv; labels
     (N, H, W) uint8 = the recorded tags; lut = sem_class_table(seg_channels) on the host.  -> int32 (N, C*C + 1) = confusion[gt][pred]
     flattened, then the invalid (NaN-logit) pixels (written into ``out`` when given)."""
-    _need_cuda(feat, table, labels)
-    if feat.dtype not in (torch.float32, h16()) or feat.dim() != 4 or feat.shape[3] != 16 or not feat.is_contiguous():
-        raise capi.LavbError(f"seg_confusion: feat must be a contiguous (N, H/2, W/2, 16) fp32 or {h16()} tensor, got {feat.dtype} "
-                             f"{tuple(feat.shape)}")
-    n, hh, wh, _ = feat.shape
-    if labels.dtype != torch.uint8 or tuple(labels.shape) != (n, 2 * hh, 2 * wh) or not labels.is_contiguous():
-        raise capi.LavbError(f"seg_confusion: labels must be a contiguous ({n}, {2 * hh}, {2 * wh}) uint8 tensor, got {labels.dtype} "
-                             f"{tuple(labels.shape)}")
-    if table.dtype != torch.float32 or table.numel() != 520 or not table.is_contiguous():
-        raise capi.LavbError("seg_confusion: table must be the 520-float pack_deconv2x2 table")
-    lut = np.ascontiguousarray(lut)
-    if lut.dtype != np.uint8 or lut.shape != (256,):
-        raise capi.LavbError(f"seg_confusion: lut must be a host (256,) uint8 array, got {lut.dtype} {lut.shape}")
-    if len({feat.device, table.device, labels.device}) != 1:
-        raise capi.LavbError("seg_confusion: the inputs must be on one device")
+    n, hh, wh, _ = _tensor("seg_confusion", "feat", feat, (torch.float32, h16()), (None, None, None, 16))
+    _tensor("seg_confusion", "labels", labels, torch.uint8, (n, 2 * hh, 2 * wh), feat.device)
+    _tensor("seg_confusion", "table", table, torch.float32, None, feat.device)
+    _require(table.numel() == 520, "seg_confusion: table must be the 520-float pack_deconv2x2 table")
+    lut = _host("seg_confusion", "lut", lut, np.uint8, (256,))
     c = int(n_classes)
-    if out is None:
-        out = torch.empty((n, c * c + 1), dtype=torch.int32, device=feat.device)
-    elif out.dtype != torch.int32 or tuple(out.shape) != (n, c * c + 1) or not out.is_contiguous() or out.device != feat.device:
-        raise capi.LavbError(f"seg_confusion: out must be a contiguous ({n}, {c * c + 1}) int32 tensor on {feat.device}")
-    check(lib().lavb_seg_confusion(_ptr(feat), _DT[feat.dtype], _ptr(table), _ptr(labels), lut.ctypes.data_as(C.c_void_p), n, c,
-                                   2 * hh, 2 * wh, _ptr(out), _stream()), "lavb_seg_confusion")
-    _COUNT[0] += n > 0
+    out = _out("seg_confusion", "out", out, torch.int32, (n, c * c + 1), feat.device)
+    _launch("lavb_seg_confusion", _ptr(feat), _DT[feat.dtype], _ptr(table), _ptr(labels), _hptr(lut), n, c, 2 * hh, 2 * wh, _ptr(out),
+            launches=n > 0)
     return out
 
 
@@ -556,73 +516,51 @@ def paint_confusion(points, tags, lut, cams, window, n_classes, feat=None, table
     (min_x, max_x, min_y, max_y) of the pillar grid; feat NHWC (F * ncam, H/2, W/2, 16) fp32 / h16 with table = pack_deconv2x2
     (the online source) and / or stored (F, N, C - 1) fp32 = lidar_sem rows; meta (F, 2) int32 = (rows, stored scored) per frame
     or None.  -> int32 (F, paint_confusion_ints(...)) (written into ``out`` when given); paint_confusion_views splits it."""
-    _need_cuda(points, tags, feat, table, stored, meta)
     c = int(n_classes)
-    if points.dtype != torch.float32 or points.dim() != 3 or points.shape[2] != 4 or not points.is_contiguous():
-        raise capi.LavbError(f"paint_confusion: points must be a contiguous (F, N, 4) fp32 tensor, got {points.dtype} "
-                             f"{tuple(points.shape)}")
-    f, n, _ = points.shape
-    cams = np.ascontiguousarray(cams, dtype=np.float32)
-    if cams.ndim != 2 or cams.shape[1] != 41 or not 1 <= cams.shape[0] <= 4:
-        raise capi.LavbError(f"paint_confusion: cams must be (ncam, 41) with 1 <= ncam <= 4, got {cams.shape}")
+    f, n, _ = _tensor("paint_confusion", "points", points, torch.float32, (None, None, 4))
+    dev = points.device
+    cams = _host("paint_confusion", "cams", cams, np.float32, (None, 41), cast=True)
     ncam = cams.shape[0]
-    if tags.dtype != torch.uint8 or tags.dim() != 3 or tags.shape[0] != f * ncam or not tags.is_contiguous():
-        raise capi.LavbError(f"paint_confusion: tags must be a contiguous ({f * ncam}, H, W) uint8 tensor, got {tags.dtype} "
-                             f"{tuple(tags.shape)}")
-    h, w = tags.shape[1:]
-    if feat is None and stored is None:
-        raise capi.LavbError("paint_confusion: give feat (the online painting), stored (lidar_sem rows) or both")
+    _require(1 <= ncam <= 4, f"paint_confusion: cams must be (ncam, 41) with 1 <= ncam <= 4, got {cams.shape}")
+    _, h, w = _tensor("paint_confusion", "tags", tags, torch.uint8, (f * ncam, None, None), dev)
+    _require(feat is not None or stored is not None, "paint_confusion: give feat (the online painting), stored (lidar_sem rows) or both")
     if feat is not None:
-        if feat.dtype not in (torch.float32, h16()) or tuple(feat.shape) != (f * ncam, h // 2, w // 2, 16) or not feat.is_contiguous():
-            raise capi.LavbError(f"paint_confusion: feat must be a contiguous ({f * ncam}, {h // 2}, {w // 2}, 16) fp32 or {h16()} "
-                                 f"tensor, got {feat.dtype} {tuple(feat.shape)}")
-        if table is None or table.dtype != torch.float32 or table.numel() != 520 or not table.is_contiguous():
-            raise capi.LavbError("paint_confusion: table must be the 520-float pack_deconv2x2 table")
-    if stored is not None and (stored.dtype != torch.float32 or tuple(stored.shape) != (f, n, c - 1) or not stored.is_contiguous()):
-        raise capi.LavbError(f"paint_confusion: stored must be a contiguous ({f}, {n}, {c - 1}) fp32 tensor, got {stored.dtype} "
-                             f"{tuple(stored.shape)}")
-    if meta is not None and (meta.dtype != torch.int32 or tuple(meta.shape) != (f, 2) or not meta.is_contiguous()):
-        raise capi.LavbError(f"paint_confusion: meta must be a contiguous ({f}, 2) int32 tensor")
-    lut = np.ascontiguousarray(lut)
-    if lut.dtype != np.uint8 or lut.shape != (256,) or int(lut.max()) >= c:
-        raise capi.LavbError(f"paint_confusion: lut must be a host (256,) uint8 array of classes below {c}, got {lut.dtype} "
-                             f"{lut.shape}")
-    if len({t.device for t in (points, tags, feat, table, stored, meta) if t is not None}) != 1:
-        raise capi.LavbError("paint_confusion: the inputs must be on one device")
+        _tensor("paint_confusion", "feat", feat, (torch.float32, h16()), (f * ncam, h // 2, w // 2, 16), dev)
+        _tensor("paint_confusion", "table", table, torch.float32, None, dev)
+        _require(table.numel() == 520, "paint_confusion: table must be the 520-float pack_deconv2x2 table")
+    elif table is not None:      # unused without feat, but held to the inputs' device all the same
+        _tensor("paint_confusion", "table", table, None, None, dev, contiguous=False)
+    if stored is not None:
+        _tensor("paint_confusion", "stored", stored, torch.float32, (f, n, c - 1), dev)
+    if meta is not None:
+        _tensor("paint_confusion", "meta", meta, torch.int32, (f, 2), dev)
+    lut = _host("paint_confusion", "lut", lut, np.uint8, (256,))
+    _require(int(lut.max()) < c, f"paint_confusion: lut must hold classes below {c}")
     ints = lib().lavb_paint_confusion_ints(ncam, c, feat is not None, stored is not None)
-    if ints < 0:
-        raise capi.LavbError(f"paint_confusion: {c} classes outside 2..8")
-    if out is None:
-        out = torch.empty((f, ints), dtype=torch.int32, device=points.device)
-    elif out.dtype != torch.int32 or tuple(out.shape) != (f, ints) or not out.is_contiguous() or out.device != points.device:
-        raise capi.LavbError(f"paint_confusion: out must be a contiguous ({f}, {ints}) int32 tensor on {points.device}")
+    _require(ints >= 0, f"paint_confusion: {c} classes outside 2..8")
+    out = _out("paint_confusion", "out", out, torch.int32, (f, ints), dev)
     if n == 0:              # empty sweeps: every count is 0 (and an empty stored buffer has no device pointer to pass)
         return out.zero_()
     min_x, max_x, min_y, max_y = (float(v) for v in window)
-    check(lib().lavb_paint_confusion(_ptr(points), f, n, _ptr(meta), _ptr(feat), _DT[feat.dtype] if feat is not None else F32,
-                                     _ptr(table), _ptr(tags), lut.ctypes.data_as(C.c_void_p), _ptr(stored),
-                                     cams.ctypes.data_as(C.c_void_p), ncam, c, h, w, min_x, max_x, min_y, max_y, _ptr(out),
-                                     _stream()), "lavb_paint_confusion")
-    _COUNT[0] += f > 0
+    _launch("lavb_paint_confusion", _ptr(points), f, n, _ptr(meta), _ptr(feat), _DT[feat.dtype] if feat is not None else F32,
+            _ptr(table), _ptr(tags), _hptr(lut), _ptr(stored), _hptr(cams), ncam, c, h, w, min_x, max_x, min_y, max_y, _ptr(out),
+            launches=f > 0)
     return out
 
 
 STACK_JOB_DTYPE = np.dtype([("src", np.uint64), ("dst", np.uint64), ("n", np.int32), ("time_idx", np.int32), ("R", np.float32, 9),
                             ("dx", np.float32), ("dy", np.float32), ("pad", np.int32)])
-assert STACK_JOB_DTYPE.itemsize == 72
 
 
 def stack_jobs(d_jobs, n_jobs, max_n, src_cols, n_time, roof_filter=False):
     """d_jobs: uint8 device tensor holding n_jobs STACK_JOB_DTYPE records."""
     _need_cuda(d_jobs)
-    check(lib().lavb_stack_jobs(_ptr(d_jobs), n_jobs, max_n, src_cols, n_time, int(roof_filter), _stream()), "lavb_stack_jobs")
-    _COUNT[0] += 1
+    _launch("lavb_stack_jobs", _ptr(d_jobs), n_jobs, max_n, src_cols, n_time, int(roof_filter))
 
 
 # ----------------------------------------------------------------------------- temporal BEV targets
 BEV_JOB_DTYPE = np.dtype([("src", np.int64), ("dst", np.int64), ("m1", np.float64, 6), ("m2", np.float64, 6), ("dx", np.int32),
                           ("dy", np.int32), ("pad", np.int32, 2)])
-assert BEV_JOB_DTYPE.itemsize == 128
 BEV_MARGIN = 32                  # TemporalLiDARPaintedDataset.margin (lidar_painted_dataset.py:19)
 
 
@@ -653,31 +591,26 @@ def bev_targets(src_planes, jobs, out=None):
     src_planes (P, h, w) uint8 CUDA; jobs: BEV_JOB_DTYPE records (see bev_jobs); out: uint8 CUDA tensor of (..., h, w) planes
     (default (max dst + 1, h, w)).  Every plane a job names is overwritten with 0/1; a missing source (src < 0) gives zeros.
     Raises LavbError for a shift beyond the 32-pixel margin, where the reference's crop fails."""
-    _need_cuda(src_planes)
-    assert src_planes.dtype == torch.uint8 and src_planes.dim() == 3 and src_planes.is_contiguous()
+    P, h, w = _tensor("bev_targets", "src_planes", src_planes, torch.uint8, (None,) * 3)
     jobs = np.ascontiguousarray(jobs, dtype=BEV_JOB_DTYPE)
-    P, h, w = src_planes.shape
-    if len(jobs) and (np.abs(jobs["dx"]).max() > BEV_MARGIN or np.abs(jobs["dy"]).max() > BEV_MARGIN):
-        raise capi.LavbError(f"bev_targets: shift beyond the {BEV_MARGIN}-pixel margin "
-                             f"(dx {jobs['dx'].tolist()}, dy {jobs['dy'].tolist()})")
+    _require(not len(jobs) or (np.abs(jobs["dx"]).max() <= BEV_MARGIN and np.abs(jobs["dy"]).max() <= BEV_MARGIN),
+             f"bev_targets: a job shifts beyond the {BEV_MARGIN}-pixel margin")
     if out is None:
         out = torch.empty((int(jobs["dst"].max()) + 1 if len(jobs) else 0, h, w), dtype=torch.uint8, device=src_planes.device)
-    _need_cuda(out)
-    assert out.dtype == torch.uint8 and out.is_contiguous() and tuple(out.shape[-2:]) == (h, w)
+    _tensor("bev_targets", "out", out, torch.uint8, None)
+    _require(tuple(out.shape[-2:]) == (h, w), f"bev_targets: out must hold ({h}, {w}) planes, got {tuple(out.shape)}")
     n_out = out.numel() // (h * w)
-    if len(jobs) and (jobs["src"].max() >= P or jobs["dst"].min() < 0 or jobs["dst"].max() >= n_out):
-        raise capi.LavbError(f"bev_targets: job plane index out of range ({P} source planes, {n_out} output planes)")
+    _require(not len(jobs) or (jobs["src"].max() < P and jobs["dst"].min() >= 0 and jobs["dst"].max() < n_out),
+             f"bev_targets: job plane index out of range ({P} source planes, {n_out} output planes)")
     if len(jobs) == 0:
         return out
     d_jobs = _to_device(jobs.view(np.uint8), src_planes.device)
-    check(lib().lavb_bev_targets(_ptr(d_jobs), len(jobs), _ptr(src_planes), _ptr(out), h, w, _stream()), "lavb_bev_targets")
-    _COUNT[0] += 1
+    _launch("lavb_bev_targets", _ptr(d_jobs), len(jobs), _ptr(src_planes), _ptr(out), h, w)
     return out
 
 
 PNG_JOB_DTYPE = np.dtype([("off", np.int64), ("len", np.int64), ("dst", np.int32), ("h", np.int32), ("w", np.int32),
                           ("pad", np.int32)])
-assert PNG_JOB_DTYPE.itemsize == 32
 
 
 def png_decode_gray8(src, jobs, out, status=None):
@@ -686,31 +619,24 @@ def png_decode_gray8(src, jobs, out, status=None):
     concatenated); jobs: PNG_JOB_DTYPE records (off, len, dst, h, w); out: contiguous (P, h, w) uint8 CUDA tensor, every job's (h, w)
     equal to its planes'.  -> status (n_jobs,) int32 on the device, 0 where the image decoded; a nonzero entry marks a malformed
     stream whose plane holds garbage.  The other planes of out are not written."""
-    _need_cuda(src, out, status)
-    if src.dtype != torch.uint8 or src.dim() != 1 or not src.is_contiguous():
-        raise capi.LavbError(f"png_decode_gray8: src must be a contiguous 1-D uint8 tensor, got {src.dtype} {tuple(src.shape)}")
-    if out.dtype != torch.uint8 or out.dim() != 3 or not out.is_contiguous() or out.device != src.device:
-        raise capi.LavbError(f"png_decode_gray8: out must be a contiguous (P, h, w) uint8 tensor on {src.device}")
+    _tensor("png_decode_gray8", "src", src, torch.uint8, (None,))
+    P, h, w = _tensor("png_decode_gray8", "out", out, torch.uint8, (None,) * 3, src.device)
     jobs = np.ascontiguousarray(jobs, dtype=PNG_JOB_DTYPE)
-    P, h, w = out.shape
-    if not (0 < h <= 4096 and 0 < w <= 4096):
-        raise capi.LavbError(f"png_decode_gray8: plane size {h}x{w} outside 1..4096")
-    if len(jobs) and ((jobs["h"] != h).any() or (jobs["w"] != w).any()):
-        raise capi.LavbError(f"png_decode_gray8: a job's size differs from the {h}x{w} planes")
-    if len(jobs) and ((jobs["dst"] < 0).any() or (jobs["dst"] >= P).any() or len(np.unique(jobs["dst"])) != len(jobs)):
-        raise capi.LavbError(f"png_decode_gray8: job planes must be distinct and in 0..{P - 1}")
-    if len(jobs) and ((jobs["off"] < 0).any() or (jobs["len"] < 0).any() or (jobs["off"] + jobs["len"] > src.numel()).any()):
-        raise capi.LavbError(f"png_decode_gray8: a job's stream lies outside the {src.numel()}-byte source")
+    _require(0 < h <= 4096 and 0 < w <= 4096, f"png_decode_gray8: plane size {h}x{w} outside 1..4096")
+    if len(jobs):
+        _require(not ((jobs["h"] != h).any() or (jobs["w"] != w).any()), f"png_decode_gray8: a job's size differs from the {h}x{w} planes")
+        _require(not ((jobs["dst"] < 0).any() or (jobs["dst"] >= P).any() or len(np.unique(jobs["dst"])) != len(jobs)),
+                 f"png_decode_gray8: job planes must be distinct and in 0..{P - 1}")
+        _require(not ((jobs["off"] < 0).any() or (jobs["len"] < 0).any() or (jobs["off"] + jobs["len"] > src.numel()).any()),
+                 f"png_decode_gray8: a job's stream lies outside the {src.numel()}-byte source")
     if status is None:
         status = torch.empty(len(jobs), dtype=torch.int32, device=src.device)
-    elif status.dtype != torch.int32 or status.numel() != len(jobs) or not status.is_contiguous() or status.device != src.device:
-        raise capi.LavbError(f"png_decode_gray8: status must be a contiguous ({len(jobs)},) int32 tensor on {src.device}")
+    _tensor("png_decode_gray8", "status", status, torch.int32, None, src.device)
+    _require(status.numel() == len(jobs), f"png_decode_gray8: status must hold {len(jobs)} entries, got {tuple(status.shape)}")
     if len(jobs) == 0:
         return status
     d_jobs = _to_device(jobs.view(np.uint8), src.device)
-    check(lib().lavb_png_decode_gray8(_ptr(src), src.numel(), _ptr(d_jobs), len(jobs), _ptr(out), P, h, w, _ptr(status), _stream()),
-          "lavb_png_decode_gray8")
-    _COUNT[0] += 1
+    _launch("lavb_png_decode_gray8", _ptr(src), src.numel(), _ptr(d_jobs), len(jobs), _ptr(out), P, h, w, _ptr(status))
     return status
 
 
@@ -723,7 +649,6 @@ def _to_device(a, device):
 # ----------------------------------------------------------------------------- training batches
 LIDAR_SWEEP_DTYPE = np.dtype([("R_aug", np.float32, 9), ("R_mv", np.float32, 9), ("dx", np.float32), ("dy", np.float32),
                               ("time_idx", np.int32), ("row0", np.int32)])
-assert LIDAR_SWEEP_DTYPE.itemsize == 88
 
 
 def lidar_batch(raw, rows, sweeps, cams, image_hw, n_time, out=None):
@@ -731,29 +656,16 @@ def lidar_batch(raw, rows, sweeps, cams, image_hw, n_time, out=None):
     sweep's rows [xyzr | painted]; rows (B, P) int32: the raw row of each output row, -1 for a zero row; sweeps: uint8 CUDA tensor
     of LIDAR_SWEEP_DTYPE records sorted by row0; cams (ncam, 41) float32 numpy; image_hw = the camera image size.
     -> (B, P, 4+C+n_time) fp32, bit-identical to GpuLidarStacker on each sample for the same shuffle."""
-    _need_cuda(raw, rows, sweeps)
-    if raw.dtype != torch.float32 or raw.dim() != 2 or not raw.is_contiguous() or raw.shape[1] < 4:
-        raise capi.LavbError(f"lidar_batch: raw must be a contiguous (N, 4+C) fp32 tensor, got {raw.dtype} {tuple(raw.shape)}")
-    if rows.dtype != torch.int32 or rows.dim() != 2 or not rows.is_contiguous():
-        raise capi.LavbError(f"lidar_batch: rows must be a contiguous (B, P) int32 tensor, got {rows.dtype} {tuple(rows.shape)}")
-    if sweeps.dtype != torch.uint8 or not sweeps.is_contiguous() or sweeps.numel() % LIDAR_SWEEP_DTYPE.itemsize:
-        raise capi.LavbError("lidar_batch: sweeps must be a contiguous uint8 tensor of 88-byte LIDAR_SWEEP_DTYPE records")
-    if not raw.device == rows.device == sweeps.device:
-        raise capi.LavbError("lidar_batch: raw, rows and sweeps must be on one device")
-    cams = np.ascontiguousarray(cams, dtype=np.float32)
-    if cams.ndim != 2 or cams.shape[1] != 41:
-        raise capi.LavbError(f"lidar_batch: cams must be (ncam, 41), got {cams.shape}")
-    b, p = rows.shape
-    c = raw.shape[1] - 4
-    if out is None:
-        out = torch.empty((b, p, 4 + c + n_time), dtype=torch.float32, device=raw.device)
-    elif out.dtype != torch.float32 or tuple(out.shape) != (b, p, 4 + c + n_time) or not out.is_contiguous() \
-            or out.device != raw.device:
-        raise capi.LavbError(f"lidar_batch: out must be a contiguous fp32 ({b}, {p}, {4 + c + n_time}) tensor on {raw.device}")
-    check(lib().lavb_lidar_batch(_ptr(raw), raw.shape[0], c, _ptr(rows), b * p, _ptr(sweeps),
-                                 sweeps.numel() // LIDAR_SWEEP_DTYPE.itemsize, cams.ctypes.data_as(C.c_void_p), cams.shape[0],
-                                 image_hw[0], image_hw[1], n_time, _ptr(out), _stream()), "lavb_lidar_batch")
-    _COUNT[0] += 1
+    _, cols = _tensor("lidar_batch", "raw", raw, torch.float32, (None, None))
+    _require(cols >= 4, f"lidar_batch: raw must be (N, 4+C), got {tuple(raw.shape)}")
+    b, p = _tensor("lidar_batch", "rows", rows, torch.int32, (None, None), raw.device)
+    _tensor("lidar_batch", "sweeps", sweeps, torch.uint8, None, raw.device)
+    _require(sweeps.numel() % LIDAR_SWEEP_DTYPE.itemsize == 0, "lidar_batch: sweeps must hold whole 88-byte LIDAR_SWEEP_DTYPE records")
+    cams = _host("lidar_batch", "cams", cams, np.float32, (None, 41), cast=True)
+    c = cols - 4
+    out = _out("lidar_batch", "out", out, torch.float32, (b, p, 4 + c + n_time), raw.device)
+    _launch("lavb_lidar_batch", _ptr(raw), raw.shape[0], c, _ptr(rows), b * p, _ptr(sweeps), sweeps.numel() // LIDAR_SWEEP_DTYPE.itemsize,
+            _hptr(cams), cams.shape[0], image_hw[0], image_hw[1], n_time, _ptr(out))
     return out
 
 
@@ -768,46 +680,45 @@ def det_heatmaps(actors, offsets, grid=None, out=None):
     """Heat, size and orientation maps of a batch in one launch (see lavb_det_heatmaps in include/lav_b200.h).  actors (A, 6)
     fp32 rows [x, y, ori, bx, by, typ]; offsets (B+1,) int32: sample i owns actors[offsets[i]:offsets[i+1]]; grid: the
     keyword arguments of det_grid.  -> (heat, size, orim), each (B, 2, h, w) fp32, bit-identical to detections_to_heatmap."""
-    _need_cuda(actors, offsets)
-    if actors.dtype != torch.float32 or actors.dim() != 2 or actors.shape[1] != 6 or not actors.is_contiguous():
-        raise capi.LavbError(f"det_heatmaps: actors must be a contiguous (A, 6) fp32 tensor, got {actors.dtype} {tuple(actors.shape)}")
-    if offsets.dtype != torch.int32 or offsets.dim() != 1 or offsets.numel() < 1 or not offsets.is_contiguous():
-        raise capi.LavbError(f"det_heatmaps: offsets must be a contiguous (B+1,) int32 tensor, got {offsets.dtype} "
-                             f"{tuple(offsets.shape)}")
-    if actors.device != offsets.device:
-        raise capi.LavbError("det_heatmaps: actors and offsets must be on one device")
+    _tensor("det_heatmaps", "actors", actors, torch.float32, (None, 6))
+    b1, = _tensor("det_heatmaps", "offsets", offsets, torch.int32, (None,), actors.device)
+    _require(b1 >= 1, "det_heatmaps: offsets must hold B+1 >= 1 entries")
     h, w, (ppm, cx0, cy0, cy1, inv_r) = det_grid(**(grid or {}))
-    b = offsets.numel() - 1
+    b = b1 - 1
     if out is None:
-        out = tuple(torch.empty((b, 2, h, w), dtype=torch.float32, device=actors.device) for _ in range(3))
-    elif any(t.dtype != torch.float32 or tuple(t.shape) != (b, 2, h, w) or not t.is_contiguous() or t.device != actors.device
-             for t in out):
-        raise capi.LavbError(f"det_heatmaps: out must be three contiguous fp32 ({b}, 2, {h}, {w}) tensors on {actors.device}")
+        out = [torch.empty((b, 2, h, w), dtype=torch.float32, device=actors.device) for _ in range(3)]
+    for o in out:
+        _tensor("det_heatmaps", "out", o, torch.float32, (b, 2, h, w), actors.device)
     heat, size, orim = out
-    check(lib().lavb_det_heatmaps(_ptr(actors), _ptr(offsets), b, h, w, ppm, cx0, cy0, cy1, inv_r, _ptr(heat), _ptr(size),
-                                  _ptr(orim), _stream()), "lavb_det_heatmaps")
-    _COUNT[0] += 1
+    _launch("lavb_det_heatmaps", _ptr(actors), _ptr(offsets), b, h, w, ppm, cx0, cy0, cy1, inv_r, _ptr(heat), _ptr(size), _ptr(orim))
     return heat, size, orim
 
 
-def _eval_layout(b, ncols):
-    """(name, dtype, shape, byte offset) of the parts of eval_batch's result buffer, 8-byte parts first, and its size."""
-    parts = [("iou", torch.int64, (b, 3, 2)), ("plan_err", torch.float64, (b, 2)), ("ngt", torch.int32, (b, 2)),
-             ("score", torch.float32, (b, ncols)), ("flags", torch.int32, (b, ncols))]
+def _layout(parts):
+    """(name, dtype, shape, byte offset) of each of a packed result buffer's parts (name, dtype, shape), laid end to end in
+    order, and the buffer's size."""
     out, pos = [], 0
     for name, dt, shape in parts:
         out.append((name, dt, shape, pos))
-        pos += int(np.prod(shape)) * torch.empty((), dtype=dt).element_size()
+        pos += math.prod(shape) * dt.itemsize
     return out, pos
+
+
+def _views(buf, parts):
+    """the named parts of a packed result buffer (uint8, on the device or a host copy), as _layout places them."""
+    return {name: buf[pos:pos + math.prod(shape) * dt.itemsize].view(dt).view(shape) for name, dt, shape, pos in _layout(parts)[0]}
+
+
+def _eval_parts(b, ncols):     # 8-byte parts first
+    return [("iou", torch.int64, (b, 3, 2)), ("plan_err", torch.float64, (b, 2)), ("ngt", torch.int32, (b, 2)),
+            ("score", torch.float32, (b, ncols)), ("flags", torch.int32, (b, ncols))]
 
 
 def eval_views(buf, b, ncols):
     """the named parts of an eval_batch result buffer (on the device or a host copy of it): iou (b,3,2) int64 = per BEV channel
     (intersection, union); plan_err (b,2) fp64 = (ADE, FDE); ngt (b,2) int32 = actors per class in the window; score / flags
     (b, ncols) = the packed scores and, per column, bit 4 for a surviving peak and bit k for a match at EVAL_THRESHOLDS_M[k]."""
-    layout, _ = _eval_layout(b, ncols)
-    return {name: buf[pos:pos + int(np.prod(shape)) * torch.empty((), dtype=dt).element_size()].view(dt).view(shape)
-            for name, dt, shape, pos in layout}
+    return _views(buf, _eval_parts(b, ncols))
 
 
 EVAL_THRESHOLDS_M = (0.5, 1.0, 2.0, 4.0)      # centre-distance thresholds of the detection matching (evaluate.cu)
@@ -819,92 +730,58 @@ def eval_batch(seg, gt, packed, actors, offsets, plan, ego_locs, grid=None, min_
     det_heatmaps table, on the device); offsets (B+1,) int32 on the HOST; plan (B,T,2) and ego_locs (B,T+1,2) fp32; grid: the
     keyword arguments of det_grid.  -> the uint8 result buffer (written into ``out`` when given), to be read through eval_views,
     usually after one copy to the host."""
-    _need_cuda(seg, gt, packed, actors, plan, ego_locs)
-    if seg.dim() != 4 or seg.shape[3] != 3 or seg.dtype not in (torch.float32, h16()) or not seg.is_contiguous():
-        raise capi.LavbError(f"eval_batch: seg must be a contiguous (B,H,W,3) fp32 or {h16()} tensor, got {seg.dtype} {tuple(seg.shape)}")
-    b, h, w, _ = seg.shape
-    if gt.dtype != torch.uint8 or gt.dim() != 4 or gt.shape[0] != b or tuple(gt.shape[2:]) != (h, w) or not gt.is_contiguous():
-        raise capi.LavbError(f"eval_batch: gt must be a contiguous ({b}, P, {h}, {w}) uint8 tensor, got {gt.dtype} {tuple(gt.shape)}")
-    if packed.dtype != torch.float32 or packed.dim() != 3 or packed.shape[:2] != (b, 7) or packed.shape[2] % 2 \
-            or not packed.is_contiguous():
-        raise capi.LavbError(f"eval_batch: packed must be a contiguous ({b}, 7, 2*n_det) fp32 tensor, got {tuple(packed.shape)}")
-    if actors.dtype != torch.float32 or actors.dim() != 2 or actors.shape[1] != 6 or not actors.is_contiguous():
-        raise capi.LavbError(f"eval_batch: actors must be a contiguous (A, 6) fp32 tensor, got {actors.dtype} {tuple(actors.shape)}")
-    offsets = np.ascontiguousarray(offsets.numpy() if torch.is_tensor(offsets) else offsets)
-    if offsets.dtype != np.int32 or offsets.shape != (b + 1,):
-        raise capi.LavbError(f"eval_batch: offsets must be a host ({b + 1},) int32 array, got {offsets.dtype} {offsets.shape}")
-    t = plan.shape[1] if plan.dim() == 3 else -1
-    if plan.dtype != torch.float32 or tuple(plan.shape) != (b, t, 2) or not plan.is_contiguous() or ego_locs.dtype != torch.float32 \
-            or tuple(ego_locs.shape) != (b, t + 1, 2) or not ego_locs.is_contiguous():
-        raise capi.LavbError(f"eval_batch: plan ({b}, T, 2) and ego_locs ({b}, T+1, 2) must be contiguous fp32, got "
-                             f"{plan.dtype} {tuple(plan.shape)} / {ego_locs.dtype} {tuple(ego_locs.shape)}")
-    if len({seg.device, gt.device, packed.device, actors.device, plan.device, ego_locs.device}) != 1:
-        raise capi.LavbError("eval_batch: the inputs must be on one device")
-    ncols = packed.shape[2]
-    _, nbytes = _eval_layout(b, ncols)
-    if out is None:
-        out = torch.empty((nbytes,), dtype=torch.uint8, device=seg.device)
-    elif out.dtype != torch.uint8 or tuple(out.shape) != (nbytes,) or out.device != seg.device:
-        raise capi.LavbError(f"eval_batch: out must be a ({nbytes},) uint8 tensor on {seg.device}")
-    v = eval_views(out, b, ncols)
+    b, h, w, _ = _tensor("eval_batch", "seg", seg, (torch.float32, h16()), (None, None, None, 3))
+    dev = seg.device
+    _tensor("eval_batch", "gt", gt, torch.uint8, (b, None, h, w), dev)
+    _, _, ncols = _tensor("eval_batch", "packed", packed, torch.float32, (b, 7, None), dev)
+    _require(ncols % 2 == 0, f"eval_batch: packed must be (B, 7, 2*n_det), got {tuple(packed.shape)}")
+    _tensor("eval_batch", "actors", actors, torch.float32, (None, 6), dev)
+    offsets = _host("eval_batch", "offsets", offsets, np.int32, (b + 1,))
+    _, t, _ = _tensor("eval_batch", "plan", plan, torch.float32, (b, None, 2), dev)
+    _tensor("eval_batch", "ego_locs", ego_locs, torch.float32, (b, t + 1, 2), dev)
+    parts = _eval_parts(b, ncols)
+    out = _out("eval_batch", "out", out, torch.uint8, (_layout(parts)[1],), dev)
+    v = _views(out, parts)
     _, _, (ppm, cx0, cy0, cy1, _) = det_grid(**(grid or {}))
-    check(lib().lavb_eval_batch(_ptr(seg), _DT[seg.dtype], _ptr(gt), gt.shape[1], b, h, w, _ptr(packed), ncols // 2, _ptr(actors),
-                                actors.shape[0], offsets.ctypes.data_as(C.c_void_p), ppm, cx0, cy0, cy1, float(min_score), _ptr(plan),
-                                _ptr(ego_locs), t, _ptr(v["iou"]), _ptr(v["ngt"]), _ptr(v["score"]), _ptr(v["flags"]),
-                                _ptr(v["plan_err"]), _stream()), "lavb_eval_batch")
-    _COUNT[0] += -(-b // 256)
+    _launch("lavb_eval_batch", _ptr(seg), _DT[seg.dtype], _ptr(gt), gt.shape[1], b, h, w, _ptr(packed), ncols // 2, _ptr(actors),
+            actors.shape[0], _hptr(offsets), ppm, cx0, cy0, cy1, float(min_score), _ptr(plan), _ptr(ego_locs), t, _ptr(v["iou"]),
+            _ptr(v["ngt"]), _ptr(v["score"]), _ptr(v["flags"]), _ptr(v["plan_err"]), launches=-(-b // 256))
     return out
+
+
+def _forecast_parts(k):
+    return [("err", torch.float64, (k, 6)), ("branch", torch.int32, (k, 2))]
 
 
 def forecast_views(buf, k):
     """the named parts of a forecast_eval result buffer (on the device or a host copy of it): err (k,6) fp64 = (min ADE, min FDE,
     top-branch ADE, top-branch FDE, ADE and FDE under the recorded command or NaN); branch (k,2) int32 = (argmin-ADE branch, top
     branch)."""
-    return dict(err=buf[:k * 48].view(torch.float64).view(k, 6), branch=buf[k * 48:k * 56].view(torch.int32).view(k, 2))
+    return _views(buf, _forecast_parts(k))
 
 
 def forecast_eval(cast, score, target, cmd, out=None):
     """The forecast scores of k rows in one launch (see lavb_forecast_eval in include/lav_b200.h).  cast (k,C,T,2), score (k,C)
     and target (k,T,2) fp32; cmd (k,) int32, -1 where the row has no recorded command.  -> the uint8 result buffer (written into
     ``out`` when given), to be read through forecast_views, usually after one copy to the host."""
-    _need_cuda(cast, score, target, cmd)
-    if cast.dtype != torch.float32 or cast.dim() != 4 or cast.shape[3] != 2 or not cast.is_contiguous():
-        raise capi.LavbError(f"forecast_eval: cast must be a contiguous (k, C, T, 2) fp32 tensor, got {cast.dtype} {tuple(cast.shape)}")
-    k, c, t, _ = cast.shape
-    if score.dtype != torch.float32 or tuple(score.shape) != (k, c) or not score.is_contiguous():
-        raise capi.LavbError(f"forecast_eval: score must be a contiguous ({k}, {c}) fp32 tensor, got {score.dtype} {tuple(score.shape)}")
-    if target.dtype != torch.float32 or tuple(target.shape) != (k, t, 2) or not target.is_contiguous():
-        raise capi.LavbError(f"forecast_eval: target must be a contiguous ({k}, {t}, 2) fp32 tensor, got {target.dtype} "
-                             f"{tuple(target.shape)}")
-    if cmd.dtype != torch.int32 or tuple(cmd.shape) != (k,) or not cmd.is_contiguous():
-        raise capi.LavbError(f"forecast_eval: cmd must be a contiguous ({k},) int32 tensor, got {cmd.dtype} {tuple(cmd.shape)}")
-    if len({cast.device, score.device, target.device, cmd.device}) != 1:
-        raise capi.LavbError("forecast_eval: the inputs must be on one device")
-    if out is None:
-        out = torch.empty((k * 56,), dtype=torch.uint8, device=cast.device)
-    elif out.dtype != torch.uint8 or tuple(out.shape) != (k * 56,) or out.device != cast.device:
-        raise capi.LavbError(f"forecast_eval: out must be a ({k * 56},) uint8 tensor on {cast.device}")
+    k, c, t, _ = _tensor("forecast_eval", "cast", cast, torch.float32, (None, None, None, 2))
+    dev = cast.device
+    _tensor("forecast_eval", "score", score, torch.float32, (k, c), dev)
+    _tensor("forecast_eval", "target", target, torch.float32, (k, t, 2), dev)
+    _tensor("forecast_eval", "cmd", cmd, torch.int32, (k,), dev)
+    out = _out("forecast_eval", "out", out, torch.uint8, (_layout(_forecast_parts(k))[1],), dev)
     v = forecast_views(out, k)
-    check(lib().lavb_forecast_eval(_ptr(cast), _ptr(score), _ptr(target), _ptr(cmd), k, c, t, _ptr(v["err"]), _ptr(v["branch"]),
-                                   _stream()), "lavb_forecast_eval")
-    _COUNT[0] += k > 0
+    _launch("lavb_forecast_eval", _ptr(cast), _ptr(score), _ptr(target), _ptr(cmd), k, c, t, _ptr(v["err"]), _ptr(v["branch"]),
+            launches=k > 0)
     return out
 
 
 DET_MATCH_M = 2.0       # centre-distance radius of the detected-forecast match (det_forecast.cu)
 
 
-def _det_match_layout(b, k, t):
-    """(name, dtype, shape, byte offset) of the parts of det_forecast_match's result buffer and its size: forecast_eval's result
-    of the k rows first (err, branch: its ``out`` is buf[:56 * k]), then the match's."""
-    parts = [("err", torch.float64, (k, 6)), ("branch", torch.int32, (k, 2)), ("dist", torch.float64, (k,)),
-             ("target", torch.float32, (k, t, 2)), ("actor", torch.int32, (k,)), ("flag", torch.int32, (k,)),
-             ("ngt", torch.int32, (b, 2))]
-    out, pos = [], 0
-    for name, dt, shape in parts:
-        out.append((name, dt, shape, pos))
-        pos += int(np.prod(shape)) * torch.empty((), dtype=dt).element_size()
-    return out, pos
+def _det_match_parts(b, k, t):  # forecast_eval's result of the k rows first (its ``out`` is buf[:56 * k]), then the match's
+    return _forecast_parts(k) + [("dist", torch.float64, (k,)), ("target", torch.float32, (k, t, 2)), ("actor", torch.int32, (k,)),
+                                 ("flag", torch.int32, (k,)), ("ngt", torch.int32, (b, 2))]
 
 
 def det_match_views(buf, b, k, t):
@@ -913,9 +790,7 @@ def det_match_views(buf, b, k, t):
     match distance in metres, NaN when unmatched; target (k,t,2) fp32 = the matched track's future in the ego frame, NaN unless
     matched to a tracked actor; actor (k,) int32 = the actor row within its sample, or -1; flag (k,) int32 = bit 0 matched, bit 1
     matched to a tracked actor; ngt (b,2) int32 = vehicles in the window with and without a track."""
-    layout, _ = _det_match_layout(b, k, t)
-    return {name: buf[pos:pos + int(np.prod(shape)) * torch.empty((), dtype=dt).element_size()].view(dt).view(shape)
-            for name, dt, shape, pos in layout}
+    return _views(buf, _det_match_parts(b, k, t))
 
 
 def det_forecast_match(packed, actors, offsets, row_offsets, cols, num_objs, locs, ego_locs, grid=None, match_m=DET_MATCH_M,
@@ -926,51 +801,31 @@ def det_forecast_match(packed, actors, offsets, row_offsets, cols, num_objs, loc
     columns; num_objs (B,) on the HOST = the recorded tracks; locs (B,max_objs,T+1,2) and ego_locs (B,T+1,2) fp32 = the labels;
     grid: the keyword arguments of det_grid.  -> the uint8 result buffer (written into ``out`` when given), read through
     det_match_views; forecast_eval(..., out=buf[:56 * K]) puts the rows' scores in the same buffer."""
-    _need_cuda(packed, actors, locs, ego_locs)
-    if packed.dtype != torch.float32 or packed.dim() != 3 or packed.shape[1] != 7 or packed.shape[2] % 2 or not packed.is_contiguous():
-        raise capi.LavbError(f"det_forecast_match: packed must be a contiguous (B, 7, 2*n_det) fp32 tensor, got {packed.dtype} "
-                             f"{tuple(packed.shape)}")
-    b = packed.shape[0]
-    if actors.dtype != torch.float32 or actors.dim() != 2 or actors.shape[1] != 6 or not actors.is_contiguous():
-        raise capi.LavbError(f"det_forecast_match: actors must be a contiguous (A, 6) fp32 tensor, got {actors.dtype} "
-                             f"{tuple(actors.shape)}")
-    host = lambda a: np.ascontiguousarray(a.numpy() if torch.is_tensor(a) else a)
-    offsets, row_offsets, cols, num_objs = host(offsets), host(row_offsets), host(cols), host(num_objs).astype(np.int32)
-    for name, a, shape in (("offsets", offsets, (b + 1,)), ("row_offsets", row_offsets, (b + 1,)), ("num_objs", num_objs, (b,))):
-        if a.dtype != np.int32 or a.shape != shape:
-            raise capi.LavbError(f"det_forecast_match: {name} must be a host {shape} int32 array, got {a.dtype} {a.shape}")
+    b, _, ncols = _tensor("det_forecast_match", "packed", packed, torch.float32, (None, 7, None))
+    _require(ncols % 2 == 0, f"det_forecast_match: packed must be (B, 7, 2*n_det), got {tuple(packed.shape)}")
+    dev = packed.device
+    _tensor("det_forecast_match", "actors", actors, torch.float32, (None, 6), dev)
+    offsets = _host("det_forecast_match", "offsets", offsets, np.int32, (b + 1,))
+    row_offsets = _host("det_forecast_match", "row_offsets", row_offsets, np.int32, (b + 1,))
+    num_objs = _host("det_forecast_match", "num_objs", num_objs, np.int32, (b,), cast=True)
     k = int(row_offsets[-1])
-    if cols.dtype != np.int32 or cols.shape != (k,):
-        raise capi.LavbError(f"det_forecast_match: cols must be a host ({k},) int32 array, got {cols.dtype} {cols.shape}")
-    if locs.dtype != torch.float32 or locs.dim() != 4 or locs.shape[0] != b or locs.shape[3] != 2 or not locs.is_contiguous():
-        raise capi.LavbError(f"det_forecast_match: locs must be a contiguous ({b}, max_objs, T+1, 2) fp32 tensor, got {locs.dtype} "
-                             f"{tuple(locs.shape)}")
-    t = locs.shape[2] - 1
-    if ego_locs.dtype != torch.float32 or tuple(ego_locs.shape) != (b, t + 1, 2) or not ego_locs.is_contiguous():
-        raise capi.LavbError(f"det_forecast_match: ego_locs must be a contiguous ({b}, {t + 1}, 2) fp32 tensor, got {ego_locs.dtype} "
-                             f"{tuple(ego_locs.shape)}")
-    if len({packed.device, actors.device, locs.device, ego_locs.device}) != 1:
-        raise capi.LavbError("det_forecast_match: the inputs must be on one device")
-    _, nbytes = _det_match_layout(b, k, t)
-    if out is None:
-        out = torch.empty((nbytes,), dtype=torch.uint8, device=packed.device)
-    elif out.dtype != torch.uint8 or tuple(out.shape) != (nbytes,) or out.device != packed.device:
-        raise capi.LavbError(f"det_forecast_match: out must be a ({nbytes},) uint8 tensor on {packed.device}")
-    v = det_match_views(out, b, k, t)
+    cols = _host("det_forecast_match", "cols", cols, np.int32, (k,))
+    _, max_objs, t1, _ = _tensor("det_forecast_match", "locs", locs, torch.float32, (b, None, None, 2), dev)
+    t = t1 - 1
+    _tensor("det_forecast_match", "ego_locs", ego_locs, torch.float32, (b, t + 1, 2), dev)
+    parts = _det_match_parts(b, k, t)
+    out = _out("det_forecast_match", "out", out, torch.uint8, (_layout(parts)[1],), dev)
+    v = _views(out, parts)
     h, w, (ppm, cx0, cy0, cy1, _) = det_grid(**(grid or {}))
-    ip = lambda a: a.ctypes.data_as(C.c_void_p)
-    check(lib().lavb_det_forecast_match(_ptr(packed), b, w, packed.shape[2] // 2, _ptr(actors), actors.shape[0], ip(offsets),
-                                        ip(row_offsets), ip(cols), ip(num_objs), _ptr(locs), _ptr(ego_locs), locs.shape[1], t, ppm,
-                                        cx0, cy0, cy1, float(match_m), _ptr(v["actor"]), _ptr(v["flag"]), _ptr(v["dist"]),
-                                        _ptr(v["target"]), _ptr(v["ngt"]), _stream()), "lavb_det_forecast_match")
-    _COUNT[0] += -(-b // 128)
+    _launch("lavb_det_forecast_match", _ptr(packed), b, w, ncols // 2, _ptr(actors), actors.shape[0], _hptr(offsets), _hptr(row_offsets),
+            _hptr(cols), _hptr(num_objs), _ptr(locs), _ptr(ego_locs), max_objs, t, ppm, cx0, cy0, cy1, float(match_m), _ptr(v["actor"]),
+            _ptr(v["flag"]), _ptr(v["dist"]), _ptr(v["target"]), _ptr(v["ngt"]), launches=-(-b // 128))
     return out
 
 
 # one (actor, step) record of plan_safety's actor table (lavb_plan_safety in include/lav_b200.h)
 PLAN_SAFETY_ACTOR_DTYPE = np.dtype([("x", np.float64), ("y", np.float64), ("cos", np.float64), ("sin", np.float64),
                                     ("e1", np.float64), ("e2", np.float64), ("typ", np.int32), ("present", np.int32)])
-assert PLAN_SAFETY_ACTOR_DTYPE.itemsize == 56
 PLAN_SAFETY_FIELDS = ("veh_step", "veh_row", "ped_step", "ped_row", "off_road_step", "off_map_steps", "invalid_steps", "first_step")
 
 
@@ -988,41 +843,25 @@ def plan_safety(traj, actors, offsets, ego_ext, bev, grid=None, out=None):
     tensor on the device, sample i owning rows [offsets[i], offsets[i+1]) (offsets (B+1,) int32 on the HOST), row a's step s at
     record a * T + s - 1; ego_ext (B,2) fp64 = the ego's half extents; bev (B,P,H,W) uint8, plane 0 the road; grid: the keyword
     arguments of det_grid.  -> (B,n,8) int32, read through plan_safety_views (written into ``out`` when given)."""
-    _need_cuda(traj, actors, ego_ext, bev)
-    if traj.dtype != torch.float32 or traj.dim() != 4 or traj.shape[3] != 2 or not traj.is_contiguous():
-        raise capi.LavbError(f"plan_safety: traj must be a contiguous (B, n, T, 2) fp32 tensor, got {traj.dtype} {tuple(traj.shape)}")
-    b, n, t, _ = traj.shape
-    offsets = np.ascontiguousarray(offsets.numpy() if torch.is_tensor(offsets) else offsets)
-    if offsets.dtype != np.int32 or offsets.shape != (b + 1,):
-        raise capi.LavbError(f"plan_safety: offsets must be a host ({b + 1},) int32 array, got {offsets.dtype} {offsets.shape}")
+    b, n, t, _ = _tensor("plan_safety", "traj", traj, torch.float32, (None, None, None, 2))
+    dev = traj.device
+    offsets = _host("plan_safety", "offsets", offsets, np.int32, (b + 1,))
     rec = PLAN_SAFETY_ACTOR_DTYPE.itemsize
-    if actors.dtype != torch.uint8 or actors.dim() != 1 or actors.numel() % (rec * t) or not actors.is_contiguous():
-        raise capi.LavbError(f"plan_safety: actors must be a contiguous 1-D uint8 tensor of {rec}-byte records, {t} per actor row, "
-                             f"got {actors.dtype} {tuple(actors.shape)}")
-    if ego_ext.dtype != torch.float64 or tuple(ego_ext.shape) != (b, 2) or not ego_ext.is_contiguous():
-        raise capi.LavbError(f"plan_safety: ego_ext must be a contiguous ({b}, 2) fp64 tensor, got {ego_ext.dtype} {tuple(ego_ext.shape)}")
-    if bev.dtype != torch.uint8 or bev.dim() != 4 or bev.shape[0] != b or not bev.is_contiguous():
-        raise capi.LavbError(f"plan_safety: bev must be a contiguous ({b}, P, H, W) uint8 tensor, got {bev.dtype} {tuple(bev.shape)}")
-    if len({traj.device, actors.device, ego_ext.device, bev.device}) != 1:
-        raise capi.LavbError("plan_safety: the inputs must be on one device")
-    if out is None:
-        out = torch.empty((b, n, 8), dtype=torch.int32, device=traj.device)
-    elif out.dtype != torch.int32 or tuple(out.shape) != (b, n, 8) or not out.is_contiguous() or out.device != traj.device:
-        raise capi.LavbError(f"plan_safety: out must be a contiguous ({b}, {n}, 8) int32 tensor on {traj.device}")
-    _, _, h, w = bev.shape
+    _tensor("plan_safety", "actors", actors, torch.uint8, (None,), dev)
+    _require(actors.numel() % (rec * t) == 0, f"plan_safety: actors must hold {rec}-byte records, {t} per actor row, got {actors.numel()} bytes")
+    _tensor("plan_safety", "ego_ext", ego_ext, torch.float64, (b, 2), dev)
+    _, _, h, w = _tensor("plan_safety", "bev", bev, torch.uint8, (b, None, None, None), dev)
+    out = _out("plan_safety", "out", out, torch.int32, (b, n, 8), dev)
     _, _, (ppm, cx0, cy0, cy1, _) = det_grid(**(grid or {}))
-    check(lib().lavb_plan_safety(_ptr(traj), b, n, t, _ptr(actors), actors.numel() // (rec * t), offsets.ctypes.data_as(C.c_void_p),
-                                 _ptr(ego_ext), _ptr(bev), bev[0].numel() if b else h * w, h, w, ppm, cx0, cy0, cy1, _ptr(out),
-                                 _stream()), "lavb_plan_safety")
-    _COUNT[0] += -(-b // 512)
+    _launch("lavb_plan_safety", _ptr(traj), b, n, t, _ptr(actors), actors.numel() // (rec * t), _hptr(offsets), _ptr(ego_ext), _ptr(bev),
+            bev[0].numel() if b else h * w, h, w, ppm, cx0, cy0, cy1, _ptr(out), launches=-(-b // 512))
     return out
 
 
 def agent_control_state_bytes(turn_n, speed_n):
     """bytes of one agent's controller state (lavb_agent_control_state_bytes); all-zero bytes are a new route."""
     n = int(lib().lavb_agent_control_state_bytes(int(turn_n), int(speed_n)))
-    if n == 0:
-        raise capi.LavbError(f"agent_control: PID windows {turn_n}, {speed_n} outside 1..64")
+    _require(n != 0, f"agent_control: PID windows {turn_n}, {speed_n} outside 1..64")
     return n
 
 
@@ -1046,83 +885,40 @@ def agent_control(plan, cast, other_locs, other_cmds, offsets, pred_bra, speed, 
     B * agent_control_state_bytes(config.turn_n, config.speed_n) bytes, updated in place.
     -> (control (B,3) fp32 = steer, throttle, brake; flags (B,) int32 of LAVB_CTL_* bits), written into ``control`` / ``flags``
     when given."""
-    _need_cuda(plan, cast, other_locs, other_cmds, pred_bra, speed, state)
-    f32 = lambda x, shape: x.dtype == torch.float32 and tuple(x.shape) == shape and x.is_contiguous()
-    if plan.dtype != torch.float32 or plan.dim() != 3 or plan.shape[2] != 2 or not plan.is_contiguous():
-        raise capi.LavbError(f"agent_control: plan must be a contiguous (B, T, 2) fp32 tensor, got {plan.dtype} {tuple(plan.shape)}")
-    b, t, _ = plan.shape
-    if not f32(cast, (b, t, 2)):
-        raise capi.LavbError(f"agent_control: cast must be a contiguous ({b}, {t}, 2) fp32 tensor, got {cast.dtype} {tuple(cast.shape)}")
-    if other_locs.dim() != 4 or not f32(other_locs, (other_locs.shape[0], other_locs.shape[1], t, 2)):
-        raise capi.LavbError(f"agent_control: other_locs must be a contiguous (K, C, {t}, 2) fp32 tensor, got {other_locs.dtype} "
-                             f"{tuple(other_locs.shape)}")
-    k, c = other_locs.shape[:2]
-    if not f32(other_cmds, (k, c)):
-        raise capi.LavbError(f"agent_control: other_cmds must be a contiguous ({k}, {c}) fp32 tensor, got {other_cmds.dtype} "
-                             f"{tuple(other_cmds.shape)}")
-    if not f32(pred_bra, (b,)) or not f32(speed, (b,)):
-        raise capi.LavbError(f"agent_control: pred_bra and speed must be contiguous ({b},) fp32 tensors, got "
-                             f"{tuple(pred_bra.shape)} and {tuple(speed.shape)}")
-    offsets = np.ascontiguousarray(offsets.numpy() if torch.is_tensor(offsets) else offsets)
-    if offsets.dtype != np.int32 or offsets.shape != (b + 1,):
-        raise capi.LavbError(f"agent_control: offsets must be a host ({b + 1},) int32 array, got {offsets.dtype} {offsets.shape}")
+    b, t, _ = _tensor("agent_control", "plan", plan, torch.float32, (None, None, 2))
+    dev = plan.device
+    _tensor("agent_control", "cast", cast, torch.float32, (b, t, 2), dev)
+    k, c, _, _ = _tensor("agent_control", "other_locs", other_locs, torch.float32, (None, None, t, 2), dev)
+    _tensor("agent_control", "other_cmds", other_cmds, torch.float32, (k, c), dev)
+    _tensor("agent_control", "pred_bra", pred_bra, torch.float32, (b,), dev)
+    _tensor("agent_control", "speed", speed, torch.float32, (b,), dev)
+    offsets = _host("agent_control", "offsets", offsets, np.int32, (b + 1,))
     dcmd = torch.is_tensor(cmds) and cmds.is_cuda
     if dcmd:
-        if cmds.dtype != torch.int32 or tuple(cmds.shape) != (b,) or not cmds.is_contiguous() or cmds.device != plan.device:
-            raise capi.LavbError(f"agent_control: device cmds must be a contiguous ({b},) int32 tensor on {plan.device}, got "
-                                 f"{cmds.dtype} {tuple(cmds.shape)} on {cmds.device}")
+        _tensor("agent_control", "device cmds", cmds, torch.int32, (b,), dev)
     else:
-        cmds = np.ascontiguousarray(cmds.numpy() if torch.is_tensor(cmds) else cmds)
-        if cmds.dtype != np.int32 or cmds.shape != (b,):
-            raise capi.LavbError(f"agent_control: cmds must be a host ({b},) int32 array, got {cmds.dtype} {cmds.shape}")
-    if not isinstance(config, capi.ControlConfig):
-        raise capi.LavbError("agent_control: config must be a capi.ControlConfig")
-    nbytes = b * agent_control_state_bytes(config.turn_n, config.speed_n)
-    if state.dtype != torch.uint8 or tuple(state.shape) != (nbytes,) or not state.is_contiguous():
-        raise capi.LavbError(f"agent_control: state must be a contiguous ({nbytes},) uint8 tensor, got {state.dtype} {tuple(state.shape)}")
-    dev = plan.device
-    if len({dev, cast.device, other_locs.device, other_cmds.device, pred_bra.device, speed.device, state.device}) != 1:
-        raise capi.LavbError("agent_control: the inputs must be on one device")
-    if control is None:
-        control = torch.empty((b, 3), dtype=torch.float32, device=dev)
-    elif not f32(control, (b, 3)) or control.device != dev:
-        raise capi.LavbError(f"agent_control: control must be a contiguous ({b}, 3) fp32 tensor on {dev}")
-    if flags is None:
-        flags = torch.empty((b,), dtype=torch.int32, device=dev)
-    elif flags.dtype != torch.int32 or tuple(flags.shape) != (b,) or not flags.is_contiguous() or flags.device != dev:
-        raise capi.LavbError(f"agent_control: flags must be a contiguous ({b},) int32 tensor on {dev}")
-    ip = lambda a: a.ctypes.data_as(C.c_void_p)
-    if dcmd:
-        check(lib().lavb_agent_control_dcmd(_ptr(plan), _ptr(cast), b, t, c, _ptr(other_locs), _ptr(other_cmds), k, ip(offsets),
-                                            _ptr(pred_bra), _ptr(speed), _ptr(cmds), C.byref(config), _ptr(state), _ptr(control),
-                                            _ptr(flags), _stream()), "lavb_agent_control_dcmd")
-    else:
-        check(lib().lavb_agent_control(_ptr(plan), _ptr(cast), b, t, c, _ptr(other_locs), _ptr(other_cmds), k, ip(offsets),
-                                       _ptr(pred_bra), _ptr(speed), ip(cmds), C.byref(config), _ptr(state), _ptr(control),
-                                       _ptr(flags), _stream()), "lavb_agent_control")
-    _COUNT[0] += -(-b // 512)
+        cmds = _host("agent_control", "cmds", cmds, np.int32, (b,))
+    _require(isinstance(config, capi.ControlConfig), "agent_control: config must be a capi.ControlConfig")
+    _tensor("agent_control", "state", state, torch.uint8, (b * agent_control_state_bytes(config.turn_n, config.speed_n),), dev)
+    control = _out("agent_control", "control", control, torch.float32, (b, 3), dev)
+    flags = _out("agent_control", "flags", flags, torch.int32, (b,), dev)
+    _launch("lavb_agent_control_dcmd" if dcmd else "lavb_agent_control", _ptr(plan), _ptr(cast), b, t, c, _ptr(other_locs),
+            _ptr(other_cmds), k, _hptr(offsets), _ptr(pred_bra), _ptr(speed), _ptr(cmds) if dcmd else _hptr(cmds), C.byref(config),
+            _ptr(state), _ptr(control), _ptr(flags), launches=-(-b // 512))
     return control, flags
 
 
 NAV_STATE_DTYPE = np.dtype([("ekf_x", np.float64, (3,)), ("ekf_p", np.float64, (3,)), ("wp_x", np.float64), ("wp_y", np.float64),
                             ("rp_x", np.float64), ("rp_y", np.float64), ("route_scale", np.float64), ("ekf_scale", np.float64),
                             ("frames", np.int32), ("wp_idx", np.int32), ("wp_cmd", np.int32), ("rp_idx", np.int32),
-                            ("lane_counter", np.int32), ("lane_changed", np.int32), ("pad", np.int32, (2,))])
-assert NAV_STATE_DTYPE.itemsize == 128         # lavb_nav_state of include/lav_b200.h
+                            ("lane_counter", np.int32), ("lane_changed", np.int32), ("pad", np.int32, (2,))])   # lavb_nav_state
 
 
 def agent_nav_state_bytes():
     """bytes of one agent's lavb_nav_state record (lavb_agent_nav_state_bytes)."""
     n = int(lib().lavb_agent_nav_state_bytes())
-    if n != NAV_STATE_DTYPE.itemsize:
-        raise capi.LavbError(f"agent_nav: the library's state record has {n} bytes, NAV_STATE_DTYPE {NAV_STATE_DTYPE.itemsize}")
+    _require(n == NAV_STATE_DTYPE.itemsize, f"agent_nav: the library's state record has {n} bytes, NAV_STATE_DTYPE {NAV_STATE_DTYPE.itemsize}")
     return n
-
-
-def _f64_rows(x, b, cols, what):
-    shape = (b, cols) if cols else (b,)
-    if x.dtype != torch.float64 or tuple(x.shape) != shape or not x.is_contiguous():
-        raise capi.LavbError(f"{what} must be a contiguous {shape} fp64 tensor, got {x.dtype} {tuple(x.shape)}")
 
 
 def agent_nav_front(nodes, node_cmd, route, gnss, compass, state, cmds=None, nxps=None, poses=None, flags=None):
@@ -1130,73 +926,46 @@ def agent_nav_front(nodes, node_cmd, route, gnss, compass, state, cmds=None, nxp
     int32 = every route's nodes; route (B, 2) int32 = (start, count) per agent; gnss (B, 2) fp64 = lat, lon; compass (B,) fp64,
     raw; state B lavb_nav_state records (uint8, updated in place).  -> (cmds (B,) int32, nxps (B, 2) fp32, poses (B, 3) fp64,
     flags (B,) int32 of LAVB_NAV_* bits), written into the given tensors when given."""
-    _need_cuda(nodes, node_cmd, route, gnss, compass, state)
-    if route.dtype != torch.int32 or route.dim() != 2 or route.shape[1] != 2 or not route.is_contiguous():
-        raise capi.LavbError(f"agent_nav_front: route must be a contiguous (B, 2) int32 tensor, got {route.dtype} {tuple(route.shape)}")
-    b = route.shape[0]
-    if nodes.dtype != torch.float64 or nodes.dim() != 2 or nodes.shape[1] != 2 or not nodes.is_contiguous():
-        raise capi.LavbError(f"agent_nav_front: nodes must be a contiguous (M, 2) fp64 tensor, got {nodes.dtype} {tuple(nodes.shape)}")
-    m = nodes.shape[0]
-    if node_cmd.dtype != torch.int32 or tuple(node_cmd.shape) != (m,) or not node_cmd.is_contiguous():
-        raise capi.LavbError(f"agent_nav_front: node_cmd must be a contiguous ({m},) int32 tensor, got {node_cmd.dtype} "
-                             f"{tuple(node_cmd.shape)}")
-    _f64_rows(gnss, b, 2, "agent_nav_front: gnss")
-    _f64_rows(compass, b, 0, "agent_nav_front: compass")
-    nbytes = b * agent_nav_state_bytes()
-    if state.dtype != torch.uint8 or tuple(state.shape) != (nbytes,) or not state.is_contiguous():
-        raise capi.LavbError(f"agent_nav_front: state must be a contiguous ({nbytes},) uint8 tensor, got {state.dtype} "
-                             f"{tuple(state.shape)}")
+    b, _ = _tensor("agent_nav_front", "route", route, torch.int32, (None, 2))
     dev = route.device
-    if len({dev, nodes.device, node_cmd.device, gnss.device, compass.device, state.device}) != 1:
-        raise capi.LavbError("agent_nav_front: the inputs must be on one device")
-
-    def out(x, shape, dt, name):
-        if x is None:
-            return torch.empty(shape, dtype=dt, device=dev)
-        if x.dtype != dt or tuple(x.shape) != shape or not x.is_contiguous() or x.device != dev:
-            raise capi.LavbError(f"agent_nav_front: {name} must be a contiguous {shape} {dt} tensor on {dev}")
-        return x
-    cmds, nxps = out(cmds, (b,), torch.int32, "cmds"), out(nxps, (b, 2), torch.float32, "nxps")
-    poses, flags = out(poses, (b, 3), torch.float64, "poses"), out(flags, (b,), torch.int32, "flags")
-    check(lib().lavb_agent_nav_front(b, _ptr(nodes), _ptr(node_cmd), m, _ptr(route), _ptr(gnss), _ptr(compass), _ptr(state),
-                                     _ptr(cmds), _ptr(nxps), _ptr(poses), _ptr(flags), _stream()), "lavb_agent_nav_front")
-    _COUNT[0] += 1 if b else 0
+    m, _ = _tensor("agent_nav_front", "nodes", nodes, torch.float64, (None, 2), dev)
+    _tensor("agent_nav_front", "node_cmd", node_cmd, torch.int32, (m,), dev)
+    _tensor("agent_nav_front", "gnss", gnss, torch.float64, (b, 2), dev)
+    _tensor("agent_nav_front", "compass", compass, torch.float64, (b,), dev)
+    _tensor("agent_nav_front", "state", state, torch.uint8, (b * agent_nav_state_bytes(),), dev)
+    cmds = _out("agent_nav_front", "cmds", cmds, torch.int32, (b,), dev)
+    nxps = _out("agent_nav_front", "nxps", nxps, torch.float32, (b, 2), dev)
+    poses = _out("agent_nav_front", "poses", poses, torch.float64, (b, 3), dev)
+    flags = _out("agent_nav_front", "flags", flags, torch.int32, (b,), dev)
+    _launch("lavb_agent_nav_front", b, _ptr(nodes), _ptr(node_cmd), m, _ptr(route), _ptr(gnss), _ptr(compass), _ptr(state), _ptr(cmds),
+            _ptr(nxps), _ptr(poses), _ptr(flags), launches=1 if b else 0)
     return cmds, nxps, poses, flags
 
 
 def agent_nav_update(control, speed, gnss, compass, state):
     """EKF.step of B agents after the controls (lavb_agent_nav_update): control (B, 3) fp32 = agent_control's output (steer in
     column 0); speed (B,) fp64 m/s; gnss (B, 2) fp64; compass (B,) fp64, raw; state as in agent_nav_front, updated in place."""
-    _need_cuda(control, speed, gnss, compass, state)
+    _need_cuda(state)
     b = state.numel() // agent_nav_state_bytes()
-    if control.dtype != torch.float32 or tuple(control.shape) != (b, 3) or not control.is_contiguous():
-        raise capi.LavbError(f"agent_nav_update: control must be a contiguous ({b}, 3) fp32 tensor, got {control.dtype} "
-                             f"{tuple(control.shape)}")
-    _f64_rows(speed, b, 0, "agent_nav_update: speed")
-    _f64_rows(gnss, b, 2, "agent_nav_update: gnss")
-    _f64_rows(compass, b, 0, "agent_nav_update: compass")
-    if state.dtype != torch.uint8 or state.numel() != b * agent_nav_state_bytes() or not state.is_contiguous():
-        raise capi.LavbError("agent_nav_update: state must be a contiguous uint8 tensor of whole lavb_nav_state records")
-    if len({control.device, speed.device, gnss.device, compass.device, state.device}) != 1:
-        raise capi.LavbError("agent_nav_update: the inputs must be on one device")
-    check(lib().lavb_agent_nav_update(b, _ptr(control), _ptr(speed), _ptr(gnss), _ptr(compass), _ptr(state), _stream()),
-          "lavb_agent_nav_update")
-    _COUNT[0] += 1 if b else 0
+    _tensor("agent_nav_update", "control", control, torch.float32, (b, 3))
+    dev = control.device
+    _tensor("agent_nav_update", "speed", speed, torch.float64, (b,), dev)
+    _tensor("agent_nav_update", "gnss", gnss, torch.float64, (b, 2), dev)
+    _tensor("agent_nav_update", "compass", compass, torch.float64, (b,), dev)
+    _tensor("agent_nav_update", "state", state, torch.uint8, None, dev)
+    _require(state.numel() == b * agent_nav_state_bytes(), "agent_nav_update: state must hold whole lavb_nav_state records")
+    _launch("lavb_agent_nav_update", b, _ptr(control), _ptr(speed), _ptr(gnss), _ptr(compass), _ptr(state), launches=1 if b else 0)
 
 
 def stack_job_poses(d_jobs, b, t, gap, keep, tick, ring_pose, poses=None):
     """the R / dx / dy fields of stack_jobs' table from the device pose ring (lavb_stack_job_poses): d_jobs the uint8 table of
     b * t STACK_JOB_DTYPE records; ring_pose (b, keep, 3) fp64, ``poses`` (b, 3) fp64 written to slot tick % keep first."""
-    _need_cuda(d_jobs, ring_pose, poses)
-    if d_jobs.dtype != torch.uint8 or d_jobs.numel() != b * t * STACK_JOB_DTYPE.itemsize or not d_jobs.is_contiguous():
-        raise capi.LavbError(f"stack_job_poses: jobs must hold {b} x {t} contiguous records")
-    if ring_pose.dtype != torch.float64 or tuple(ring_pose.shape) != (b, keep, 3) or not ring_pose.is_contiguous():
-        raise capi.LavbError(f"stack_job_poses: ring_pose must be a contiguous ({b}, {keep}, 3) fp64 tensor")
+    _tensor("stack_job_poses", "jobs", d_jobs, torch.uint8, None)
+    _require(d_jobs.numel() == b * t * STACK_JOB_DTYPE.itemsize, f"stack_job_poses: jobs must hold {b} x {t} records")
+    _tensor("stack_job_poses", "ring_pose", ring_pose, torch.float64, (b, keep, 3))
     if poses is not None:
-        _f64_rows(poses, b, 3, "stack_job_poses: poses")
-    check(lib().lavb_stack_job_poses(_ptr(d_jobs), b, t, gap, keep, int(tick), _ptr(ring_pose), _ptr(poses), _stream()),
-          "lavb_stack_job_poses")
-    _COUNT[0] += 1 if b else 0
+        _tensor("stack_job_poses", "poses", poses, torch.float64, (b, 3))
+    _launch("lavb_stack_job_poses", _ptr(d_jobs), b, t, gap, keep, int(tick), _ptr(ring_pose), _ptr(poses), launches=1 if b else 0)
 
 
 PILLAR_ENCODER ="sorted"    # name of the 16-bit pipeline's pillar encoder, reported by bench.py; it selects nothing
@@ -1206,9 +975,11 @@ def pillar_forward_sorted(pts, starts, counts, grid, w1, s1, t1, w2, s2, t2, can
     """tensor-core pillar encoder of the 16-bit pipeline: counting sort by canvas cell + persistent mma.sync encoder
     (lavb_pillar_forward_sorted).  Returns the NHWC canvas: fp32 (B,ny,nx,H2); with canvas16, h16 (B,ny,nx,H2), saturating —
     what the 16-bit pipeline feeds the backbone."""
-    _need_cuda(pts, w1, w2)
-    assert pts.dtype == torch.float32 and pts.dim() == 2 and pts.stride(1) == 1
-    _check_point_mlp("pillar_forward_sorted", pts, w1, s1, t1, w2, s2, t2)
+    _tensor("pillar_forward_sorted", "pts", pts, torch.float32, (None, None), contiguous=False)
+    _require(pts.stride(1) == 1 and pts.shape[1] >= 11, f"pillar_forward_sorted: point rows must be unit-stride and hold at least "
+             f"11 floats, got {tuple(pts.shape)} with strides {pts.stride()}")
+    for (name, shape), t in zip(_POINT_MLP, (w1, s1, t1, w2, s2, t2)):
+        _tensor("pillar_forward_sorted", name, t, torch.float32, shape, pts.device)
     min_x, max_x, min_y, max_y, ppm, nx, ny = grid
     d = w1.shape[1] - 5
     b, st, ct = _clouds(starts, counts, pts, "pillar_forward_sorted")
@@ -1216,48 +987,35 @@ def pillar_forward_sorted(pts, starts, counts, grid, w1, s1, t1, w2, s2, t2, can
     h2 = w2.shape[0]
     canvas = torch.empty((b, ny, nx, h2), dtype=h16() if canvas16 else torch.float32, device=pts.device)
     ws = _workspace(pts.device, lib().lavb_pillar_sorted_workspace_bytes(b, nx, ny, total))
-    e0 = _prof_begin()
-    check(lib().lavb_pillar_forward_sorted(_ptr(pts), pts.stride(0), d, st, ct, b, min_x, max_x, min_y, max_y, ppm, nx, ny,
-                                           _ptr(w1), _ptr(s1), _ptr(t1), w1.shape[0], _ptr(w2), _ptr(s2), _ptr(t2), h2,
-                                           _ptr(canvas), 2 if canvas16 else 0, _ptr(ws), _stream()), "lavb_pillar_forward_sorted")
-    _prof_end("pillar", float(total) * d * 4 + float(b) * ny * nx * h2 * (2 if canvas16 else 4), e0)
-    _COUNT[0] += 6
+    _launch("lavb_pillar_forward_sorted", _ptr(pts), pts.stride(0), d, st, ct, b, min_x, max_x, min_y, max_y, ppm, nx, ny, _ptr(w1),
+            _ptr(s1), _ptr(t1), w1.shape[0], _ptr(w2), _ptr(s2), _ptr(t2), h2, _ptr(canvas), 2 if canvas16 else 0, _ptr(ws),
+            launches=6, prof=("pillar", float(total) * d * 4 + float(b) * ny * nx * h2 * (2 if canvas16 else 4)))
     return canvas
 
 
 def det_peaks(center, box, ori, min_score=0.2, max_det=15):
     """center (LOGITS) fp32 NHWC (B,H,W,ncls), box, ori: fp32 NHWC (B,H,W,2), all contiguous -> packed (B,7,ncls*max_det)
     (see lavb_det_peaks)."""
-    _need_cuda(center, box, ori)
-    assert center.dim() == 4 and all(t.is_contiguous() and t.dtype == torch.float32 for t in (center, box, ori))
-    b, h, w, ncls = center.shape
-    assert tuple(box.shape) == tuple(ori.shape) == (b, h, w, 2), "det_peaks: box and ori must be (B, H, W, 2)"
+    b, h, w, ncls = _tensor("det_peaks", "center", center, torch.float32, (None,) * 4)
+    _tensor("det_peaks", "box", box, torch.float32, (b, h, w, 2))
+    _tensor("det_peaks", "ori", ori, torch.float32, (b, h, w, 2))
     packed = torch.empty((b, 7, ncls * max_det), dtype=torch.float32, device=center.device)
     ws = _workspace(center.device, lib().lavb_det_peaks_workspace_bytes(b, ncls))
-    check(lib().lavb_det_peaks(_ptr(center), _ptr(box), _ptr(ori), b, h, w, ncls, min_score, max_det, _ptr(packed), _ptr(ws), _stream()),
-          "lavb_det_peaks")
-    _COUNT[0] += 2
+    _launch("lavb_det_peaks", _ptr(center), _ptr(box), _ptr(ori), b, h, w, ncls, min_score, max_det, _ptr(packed), _ptr(ws), launches=2)
     return packed
 
 
 def stem7x7s2_u8(img_u8, w_h16, bias, mean, std):
     """img_u8 (B, ncam, H, cam_w, 3) uint8 contiguous; w_h16 (64,160) packed by pack_stem_weights; bias (64,)
     -> f16 NHWC (B, H/2, ncam*cam_w/2, 64)."""
-    _need_cuda(img_u8, w_h16, bias)
-    _require(img_u8.dtype == torch.uint8 and img_u8.is_contiguous() and img_u8.dim() == 5 and img_u8.shape[4] == 3,
-             "stem7x7s2_u8: img_u8 must be a contiguous uint8 (B, ncam, H, cam_w, 3) tensor")
-    _require(w_h16.dtype == h16() and tuple(w_h16.shape) == (64, 160) and w_h16.is_contiguous(),
-             "stem7x7s2_u8: w_h16 must be the contiguous (64, 160) 16-bit packing of pack_stem_weights")
-    _require(bias.dtype == torch.float32 and tuple(bias.shape) == (64,) and bias.is_contiguous(),
-             "stem7x7s2_u8: bias must be a contiguous fp32 (64,) tensor")
+    b, ncam, h, cw, _ = _tensor("stem7x7s2_u8", "img_u8", img_u8, torch.uint8, (None, None, None, None, 3))
+    _tensor("stem7x7s2_u8", "w_h16", w_h16, h16(), (64, 160))
+    _tensor("stem7x7s2_u8", "bias", bias, torch.float32, (64,))
     _require(len(mean) == 3 and len(std) == 3, "stem7x7s2_u8: mean and std hold 3 values")
-    b, ncam, h, cw, _ = img_u8.shape
     out = torch.empty((b, (h - 1) // 2 + 1, (ncam * cw - 1) // 2 + 1, 64), dtype=h16(), device=img_u8.device)
     m = (C.c_float * 3)(*[float(v) for v in mean])
     sd = (C.c_float * 3)(*[float(v) for v in std])
-    check(lib().lavb_stem7x7s2_u8(_ptr(img_u8), b, ncam, h, cw, _ptr(w_h16), _ptr(bias), m, sd, _ptr(out), _stream()),
-          "lavb_stem7x7s2_u8")
-    _COUNT[0] += 1
+    _launch("lavb_stem7x7s2_u8", _ptr(img_u8), b, ncam, h, cw, _ptr(w_h16), _ptr(bias), m, sd, _ptr(out))
     return out
 
 
@@ -1274,21 +1032,15 @@ def conv7x7s2_umma(x, w_packed, bias, out=None):
     """relu(conv 7x7 / stride 2 / pad 3 + bias) to 64 channels: x contiguous f16 NHWC (n, h, w, cin), cin % 64 == 0;
     w_packed (49, 64, cin) f16 from pack_conv7x7s2_weights; bias fp32 (64,) -> f16 NHWC (n, (h-1)//2+1, (w-1)//2+1, 64),
     written into `out` when given (contiguous, that shape)."""
-    _need_cuda(x, w_packed, bias)
-    assert x.dtype == h16() and x.is_contiguous() and x.dim() == 4
-    n, h, w, cin = x.shape
-    assert cin % 64 == 0 and h >= 7 and w >= 7, x.shape
-    assert w_packed.dtype == h16() and w_packed.is_contiguous() and tuple(w_packed.shape) == (49, 64, cin)
-    assert bias.dtype == torch.float32 and bias.is_contiguous() and bias.numel() == 64
+    n, h, w, cin = _tensor("conv7x7s2_umma", "x", x, h16(), (None,) * 4)
+    _require(cin % 64 == 0 and h >= 7 and w >= 7, f"conv7x7s2_umma: x must have cin % 64 == 0 and h, w >= 7, got {tuple(x.shape)}")
+    _tensor("conv7x7s2_umma", "w_packed", w_packed, h16(), (49, 64, cin))
+    _tensor("conv7x7s2_umma", "bias", bias, torch.float32, None)
+    _require(bias.numel() == 64, f"conv7x7s2_umma: bias must hold 64 values, got {bias.numel()}")
     ho, wo = (h - 1) // 2 + 1, (w - 1) // 2 + 1
-    if out is None:
-        out = torch.empty((n, ho, wo, 64), dtype=h16(), device=x.device)
-    assert out.dtype == h16() and out.is_contiguous() and tuple(out.shape) == (n, ho, wo, 64)
-    e0 = _prof_begin()
-    check(lib().lavb_conv7x7s2_umma(_ptr(x), n, h, w, cin, _ptr(w_packed), _ptr(bias), _ptr(out), _stream()),
-          "lavb_conv7x7s2_umma")
-    _prof_end(f"stem7x7s2:{cin}->64@{h}x{w}", 2.0 * n * ho * wo * 64 * cin * 49, e0)
-    _COUNT[0] += 1
+    out = _out("conv7x7s2_umma", "out", out, h16(), (n, ho, wo, 64), x.device)
+    _launch("lavb_conv7x7s2_umma", _ptr(x), n, h, w, cin, _ptr(w_packed), _ptr(bias), _ptr(out),
+            prof=(f"stem7x7s2:{cin}->64@{h}x{w}", 2.0 * n * ho * wo * 64 * cin * 49))
     return out
 
 
@@ -1296,40 +1048,33 @@ def conv3x3_umma(x, w, cout, stride, bias=None, scale=None, shift=None, pre_relu
     """3x3 / pad 1 / stride 1 or 2 convolution with output channels in M (lavb_conv3x3_umma): x contiguous f16 NHWC (n, h, w, cin),
     cin in (64, 128, 384); w (9, cout, cin) f16, the conv_umma packing; cout in (64, 128, 256); bias / scale / shift fp32 (cout,)
     or None -> f16 NHWC (n, (h-1)//s+1, (w-1)//s+1, cout) = [relu](conv + bias) * scale + shift, written into `out` when given."""
-    _need_cuda(x, w)
-    assert x.dtype == h16() and x.is_contiguous() and x.dim() == 4
-    n, h, wd, cin = x.shape
-    assert w.dtype == h16() and w.is_contiguous() and tuple(w.shape) == (9, cout, cin), (tuple(w.shape), cout, cin)
-    for v in (bias, scale, shift):
-        assert v is None or (v.dtype == torch.float32 and v.is_contiguous() and v.numel() == cout)
+    n, h, wd, cin = _tensor("conv3x3_umma", "x", x, h16(), (None,) * 4)
+    _tensor("conv3x3_umma", "w", w, h16(), (9, cout, cin))
+    for name, v in (("bias", bias), ("scale", scale), ("shift", shift)):
+        if v is not None:
+            _tensor("conv3x3_umma", name, v, torch.float32, None)
+            _require(v.numel() == cout, f"conv3x3_umma: {name} must hold {cout} values, got {v.numel()}")
     ho, wo = (h - 1) // stride + 1, (wd - 1) // stride + 1
-    if out is None:
-        out = torch.empty((n, ho, wo, cout), dtype=h16(), device=x.device)
-    assert out.dtype == h16() and out.is_contiguous() and tuple(out.shape) == (n, ho, wo, cout)
-    e0 = _prof_begin()
-    check(lib().lavb_conv3x3_umma(_ptr(x), n, h, wd, cin, stride, _ptr(w), cout, _ptr(bias), _ptr(scale), _ptr(shift),
-                                  int(pre_relu), _ptr(out), _stream()), "lavb_conv3x3_umma")
+    out = _out("conv3x3_umma", "out", out, h16(), (n, ho, wo, cout), x.device)
     # the label format of conv_taps' wgmma launches, so that bench.py's conv roofline keeps covering the same layers
-    _prof_end(f"umma:{cin}->{cout}x9taps@{ho}x{wo}", 2.0 * n * ho * wo * cout * cin * 9, e0)
-    _COUNT[0] += 1
+    _launch("lavb_conv3x3_umma", _ptr(x), n, h, wd, cin, stride, _ptr(w), cout, _ptr(bias), _ptr(scale), _ptr(shift), int(pre_relu),
+            _ptr(out), prof=(f"umma:{cin}->{cout}x9taps@{ho}x{wo}", 2.0 * n * ho * wo * cout * cin * 9))
     return out
 
 
 def pack_conv7x7s2_weights(w):
     """(64, cin, 7, 7) conv weights -> (49, 64, cin) f16 [tap = ky*7 + kx][cout][cin], the layout conv7x7s2_umma reads."""
-    assert w.dim() == 4 and tuple(w.shape[2:]) == (7, 7) and w.shape[0] == 64
+    _require(w.dim() == 4 and tuple(w.shape[2:]) == (7, 7) and w.shape[0] == 64,
+             f"pack_conv7x7s2_weights: w must be (64, cin, 7, 7), got {tuple(w.shape)}")
     return w.permute(2, 3, 0, 1).reshape(49, 64, w.shape[1]).to(h16()).contiguous()
 
 
 def maxpool3x3s2_nhwc(x):
     """MaxPool2d(3, 2, 1) on a contiguous f16 NHWC tensor."""
-    _need_cuda(x)
-    _require(x.dtype == h16() and x.is_contiguous() and x.dim() == 4 and x.shape[3] % 8 == 0,
-             "maxpool3x3s2_nhwc: x must be a contiguous 16-bit NHWC tensor with channels a multiple of 8")
-    n, h, w, c = x.shape
+    n, h, w, c = _tensor("maxpool3x3s2_nhwc", "x", x, h16(), (None,) * 4)
+    _require(c % 8 == 0, f"maxpool3x3s2_nhwc: x must have channels a multiple of 8, got {c}")
     out = torch.empty((n, (h - 1) // 2 + 1, (w - 1) // 2 + 1, c), dtype=h16(), device=x.device)
-    check(lib().lavb_maxpool3x3s2_nhwc(_ptr(x), n, h, w, c, _ptr(out), _stream()), "lavb_maxpool3x3s2_nhwc")
-    _COUNT[0] += 1
+    _launch("lavb_maxpool3x3s2_nhwc", _ptr(x), n, h, w, c, _ptr(out))
     return out
 
 
@@ -1339,91 +1084,68 @@ def conv_pair_umma(x, w1, bias1, w2, shift2, dil, res=None, post_relu=True, out=
     x / res: contiguous f16 NHWC (n, h, w, c), c in {64, 128}, w in {32, 64, 128}; w1 / w2: (3, c, c) f16 [tap][cout][cin];
     bias1 / shift2: fp32 (c,).  The result goes to `out` when given (contiguous, the shape of x)."""
     from .capi import ConvPairDesc
-    _need_cuda(x, w1, w2, bias1, shift2)
-    n, h, w, c = x.shape
-    assert x.dtype == h16() and x.is_contiguous() and w1.is_contiguous() and w2.is_contiguous()
-    assert tuple(w1.shape) == (3, c, c) and tuple(w2.shape) == (3, c, c) and w1.dtype == w2.dtype == h16()
-    assert bias1.dtype == shift2.dtype == torch.float32 and bias1.numel() == shift2.numel() == c
-    if out is None:
-        out = torch.empty_like(x)
-    assert out.dtype == h16() and out.is_contiguous() and out.shape == x.shape
+    n, h, w, c = _tensor("conv_pair_umma", "x", x, h16(), (None,) * 4)
+    _tensor("conv_pair_umma", "w1", w1, h16(), (3, c, c))
+    _tensor("conv_pair_umma", "w2", w2, h16(), (3, c, c))
+    for name, v in (("bias1", bias1), ("shift2", shift2)):
+        _tensor("conv_pair_umma", name, v, torch.float32, None, contiguous=False)
+        _require(v.numel() == c, f"conv_pair_umma: {name} must hold {c} values, got {v.numel()}")
+    out = _out("conv_pair_umma", "out", out, h16(), x.shape, x.device)
     d = ConvPairDesc()
     d.inp, d.out = x.data_ptr(), out.data_ptr()
     d.n, d.h, d.w, d.c, d.dil, d.post_relu = n, h, w, c, int(dil), int(post_relu)
     d.w1, d.bias1 = w1.data_ptr(), bias1.data_ptr()
     d.w2, d.shift2 = w2.data_ptr(), shift2.data_ptr()
     if res is not None:
-        assert res.is_contiguous() and res.shape == x.shape and res.dtype == h16()
+        _tensor("conv_pair_umma", "res", res, h16(), x.shape)
         d.res = res.data_ptr()
-    e0 = _prof_begin()
-    check(lib().lavb_conv_pair_umma(C.byref(d), _stream()), "lavb_conv_pair_umma")
-    _prof_end(f"umma_pair:{c}x{h}x{w}", 2.0 * n * h * w * c * c * 6, e0)
-    _COUNT[0] += 1
+    _launch("lavb_conv_pair_umma", C.byref(d), prof=(f"umma_pair:{c}x{h}x{w}", 2.0 * n * h * w * c * c * 6))
     return out
 
 
 def erf_stem(rgb_u8, w27, scale, shift, out_dtype):
     """fused normalize + ERFNet initial block: rgb_u8 (N,H,W,3) uint8 -> NHWC (N,H/2,W/2,16).  w27 (27,16), scale/shift (16,)
     are HOST float32 numpy arrays (kernel parameters)."""
-    _need_cuda(rgb_u8)
-    _require(rgb_u8.dtype == torch.uint8 and rgb_u8.is_contiguous() and rgb_u8.dim() == 4 and rgb_u8.shape[3] == 3,
-             "erf_stem: rgb_u8 must be a contiguous uint8 (N, H, W, 3) tensor")
+    n, h, w, _ = _tensor("erf_stem", "rgb_u8", rgb_u8, torch.uint8, (None, None, None, 3))
     _require(out_dtype in (torch.float32, h16()), f"erf_stem: out_dtype must be float32 or {h16()}, got {out_dtype}")
-    n, h, w, _ = rgb_u8.shape
-    a, b, c = (np.ascontiguousarray(t, dtype=np.float32) for t in (w27, scale, shift))
-    _require(a.shape == (27, 16) and b.shape == (16,) and c.shape == (16,), "erf_stem: w27 must be (27, 16), scale and shift (16,)")
+    a = _host("erf_stem", "w27", w27, np.float32, (27, 16), cast=True)
+    b = _host("erf_stem", "scale", scale, np.float32, (16,), cast=True)
+    c = _host("erf_stem", "shift", shift, np.float32, (16,), cast=True)
     out = torch.empty((n, h // 2, w // 2, 16), dtype=out_dtype, device=rgb_u8.device)
-    check(lib().lavb_erf_stem(_ptr(rgb_u8), n, h, w, a.ctypes.data_as(C.c_void_p), b.ctypes.data_as(C.c_void_p), c.ctypes.data_as(C.c_void_p),
-                              _ptr(out), _DT[out_dtype], _stream()), "lavb_erf_stem")
-    _COUNT[0] += 1
+    _launch("lavb_erf_stem", _ptr(rgb_u8), n, h, w, _hptr(a), _hptr(b), _hptr(c), _ptr(out), _DT[out_dtype])
     return out
 
 
 def erf_down16(x, w9, st):
     """fused DownsamplerBlock(16, 64): x h16 NHWC (n,h,w,16) -> (n,h/2,w/2,64) (lavb_erf_down16)."""
-    _need_cuda(x, w9, st)
-    _require(x.dtype == h16() and x.is_contiguous() and x.dim() == 4 and x.shape[3] == 16,
-             "erf_down16: x must be a contiguous 16-bit NHWC tensor of 16 channels")
-    _require(w9.dtype == torch.float32 and tuple(w9.shape) == (9, 16, 48) and w9.is_contiguous(),
-             "erf_down16: w9 must be a contiguous fp32 (9, 16, 48) tensor")
-    _require(st.dtype == torch.float32 and tuple(st.shape) == (64, 2) and st.is_contiguous(),
-             "erf_down16: st must be a contiguous fp32 (64, 2) tensor")
-    n, h, w, _ = x.shape
+    n, h, w, _ = _tensor("erf_down16", "x", x, h16(), (None, None, None, 16))
+    _tensor("erf_down16", "w9", w9, torch.float32, (9, 16, 48))
+    _tensor("erf_down16", "st", st, torch.float32, (64, 2))
     out = torch.empty((n, h // 2, w // 2, 64), dtype=x.dtype, device=x.device)
-    check(lib().lavb_erf_down16(_ptr(x), _ptr(out), n, h, w, _ptr(w9), _ptr(st), _stream()), "lavb_erf_down16")
-    _COUNT[0] += 1
+    _launch("lavb_erf_down16", _ptr(x), _ptr(out), n, h, w, _ptr(w9), _ptr(st))
     return out
 
 
 def erf_nb16(x, w4, st):
     """fused non_bottleneck_1d(16, dilation 1) block: x h16 NHWC (n,h,w,16) -> same shape (lavb_erf_nb16)."""
-    _need_cuda(x, w4, st)
-    _require(x.dtype == h16() and x.is_contiguous() and x.dim() == 4 and x.shape[3] == 16,
-             "erf_nb16: x must be a contiguous 16-bit NHWC tensor of 16 channels")
-    _require(w4.dtype == torch.float32 and tuple(w4.shape) == (4, 3, 16, 16) and w4.is_contiguous(),
-             "erf_nb16: w4 must be a contiguous fp32 (4, 3, 16, 16) tensor")
-    _require(st.dtype == torch.float32 and tuple(st.shape) == (4, 16, 2) and st.is_contiguous(),
-             "erf_nb16: st must be a contiguous fp32 (4, 16, 2) tensor")
-    n, h, w, _ = x.shape
+    n, h, w, _ = _tensor("erf_nb16", "x", x, h16(), (None, None, None, 16))
+    _tensor("erf_nb16", "w4", w4, torch.float32, (4, 3, 16, 16))
+    _tensor("erf_nb16", "st", st, torch.float32, (4, 16, 2))
     out = torch.empty_like(x)
-    check(lib().lavb_erf_nb16(_ptr(x), _ptr(out), n, h, w, _ptr(w4), _ptr(st), _stream()), "lavb_erf_nb16")
-    _COUNT[0] += 1
+    _launch("lavb_erf_nb16", _ptr(x), _ptr(out), n, h, w, _ptr(w4), _ptr(st))
     return out
 
 
 def cast_gru(embd, wih_t, whh_t, bih, bhh, wmlp, bmlp, steps):
     """the 6 cast branches in one launch (csrc/cast_gru.cu).  embd (N, 512) fp32; wih_t (ncmd, 512, 192), whh_t (ncmd, 64, 192) the
     TRANSPOSED GRU weights; bih / bhh (ncmd, 192); wmlp (ncmd, 2, 64); bmlp (ncmd, 2) -> (N, ncmd, steps, 2) fp32 cumulative waypoints."""
-    _need_cuda(embd, wih_t, whh_t)
-    n, ncmd = embd.shape[0], wih_t.shape[0]
-    assert tuple(embd.shape) == (n, 512) and tuple(wih_t.shape) == (ncmd, 512, 192) and tuple(whh_t.shape) == (ncmd, 64, 192)
-    assert tuple(bih.shape) == tuple(bhh.shape) == (ncmd, 192) and tuple(wmlp.shape) == (ncmd, 2, 64) and tuple(bmlp.shape) == (ncmd, 2)
-    for t in (embd, wih_t, whh_t, bih, bhh, wmlp, bmlp):
-        assert t.dtype == torch.float32 and t.is_contiguous()
+    n, _ = _tensor("cast_gru", "embd", embd, torch.float32, (None, 512))
+    ncmd, _, _ = _tensor("cast_gru", "wih_t", wih_t, torch.float32, (None, 512, 192))
+    for name, t, shape in (("whh_t", whh_t, (ncmd, 64, 192)), ("bih", bih, (ncmd, 192)), ("bhh", bhh, (ncmd, 192)),
+                           ("wmlp", wmlp, (ncmd, 2, 64)), ("bmlp", bmlp, (ncmd, 2))):
+        _tensor("cast_gru", name, t, torch.float32, shape)
     out = torch.empty((n, ncmd, steps, 2), dtype=torch.float32, device=embd.device)
-    check(lib().lavb_cast_gru(_ptr(embd), n, _ptr(wih_t), _ptr(whh_t), _ptr(bih), _ptr(bhh), _ptr(wmlp), _ptr(bmlp), ncmd, steps,
-                              _ptr(out), _stream()), "lavb_cast_gru")
-    _COUNT[0] += 1
+    _launch("lavb_cast_gru", _ptr(embd), n, _ptr(wih_t), _ptr(whh_t), _ptr(bih), _ptr(bhh), _ptr(wmlp), _ptr(bmlp), ncmd, steps, _ptr(out))
     return out
 
 
@@ -1441,62 +1163,33 @@ def agent_view(rgbs, tels, points, bev, plan, cast, cmds, other_locs, other_cmds
     (B+1,) int32 on the HOST); boxes (NB, 6) fp64 on the HOST, (x, y, w, h, cos, sin) in BEV pixels, agent i owning rows
     [box_offsets[i], box_offsets[i+1]); target (B, 2) fp32; config a capi.ViewConfig; scratch a uint8 device tensor of at least
     agent_view_scratch_bytes(B) bytes.  -> out (B, 160, 1146, 3) uint8, written into ``out`` when given."""
-    _need_cuda(rgbs, tels, points, bev, plan, cast, cmds, other_locs, other_cmds, target, scratch, out)
-    f32 = lambda x, shape: x.dtype == torch.float32 and tuple(x.shape) == shape and x.is_contiguous()
-    if rgbs.dtype != torch.uint8 or rgbs.dim() != 5 or tuple(rgbs.shape[1:]) != (3, 288, 256, 3) or not rgbs.is_contiguous():
-        raise capi.LavbError(f"agent_view: rgbs must be a contiguous (B, 3, 288, 256, 3) uint8 tensor, got {rgbs.dtype} {tuple(rgbs.shape)}")
-    b = rgbs.shape[0]
-    if tels.dtype != torch.uint8 or tuple(tels.shape) != (b, 192, 480, 3) or not tels.is_contiguous():
-        raise capi.LavbError(f"agent_view: tels must be a contiguous ({b}, 192, 480, 3) uint8 tensor, got {tels.dtype} {tuple(tels.shape)}")
-    if points.dtype != torch.float32 or points.dim() != 3 or points.shape[0] != b or points.shape[2] < 2 or not points.is_contiguous():
-        raise capi.LavbError(f"agent_view: points must be a contiguous ({b}, P, >= 2) fp32 tensor, got {points.dtype} {tuple(points.shape)}")
-    if bev.dtype not in (torch.float32, h16()) or bev.dim() != 4 or bev.shape[0] != b or tuple(bev.shape[2:]) != (320, 320):
-        raise capi.LavbError(f"agent_view: bev must be ({b}, C, 320, 320) fp32 or {h16()} logits, got {bev.dtype} {tuple(bev.shape)}")
-    if plan.dtype != torch.float32 or plan.dim() != 3 or plan.shape[0] != b or plan.shape[2] != 2 or not plan.is_contiguous():
-        raise capi.LavbError(f"agent_view: plan must be a contiguous ({b}, T, 2) fp32 tensor, got {plan.dtype} {tuple(plan.shape)}")
-    t = plan.shape[1]
-    if not f32(cast, (b, t, 2)) or not f32(target, (b, 2)):
-        raise capi.LavbError(f"agent_view: cast ({b}, {t}, 2) and target ({b}, 2) must be contiguous fp32 tensors, got "
-                             f"{tuple(cast.shape)} and {tuple(target.shape)}")
-    if cmds.dtype != torch.int32 or tuple(cmds.shape) != (b,) or not cmds.is_contiguous():
-        raise capi.LavbError(f"agent_view: cmds must be a contiguous ({b},) int32 tensor, got {cmds.dtype} {tuple(cmds.shape)}")
-    if other_locs.dim() != 4 or not f32(other_locs, (other_locs.shape[0], other_locs.shape[1], t, 2)):
-        raise capi.LavbError(f"agent_view: other_locs must be a contiguous (K, M, {t}, 2) fp32 tensor, got {other_locs.dtype} "
-                             f"{tuple(other_locs.shape)}")
-    k, m = other_locs.shape[:2]
-    if not f32(other_cmds, (k, m)):
-        raise capi.LavbError(f"agent_view: other_cmds must be a contiguous ({k}, {m}) fp32 tensor, got {other_cmds.dtype} "
-                             f"{tuple(other_cmds.shape)}")
-    offsets = np.ascontiguousarray(offsets.numpy() if torch.is_tensor(offsets) else offsets)
-    box_offsets = np.ascontiguousarray(box_offsets.numpy() if torch.is_tensor(box_offsets) else box_offsets)
-    for name, o in (("offsets", offsets), ("box_offsets", box_offsets)):
-        if o.dtype != np.int32 or o.shape != (b + 1,):
-            raise capi.LavbError(f"agent_view: {name} must be a host ({b + 1},) int32 array, got {o.dtype} {o.shape}")
-    boxes = np.ascontiguousarray(boxes.numpy() if torch.is_tensor(boxes) else boxes)
-    if boxes.dtype != np.float64 or boxes.ndim != 2 or boxes.shape[1] != 6:
-        raise capi.LavbError(f"agent_view: boxes must be a host (NB, 6) fp64 array, got {boxes.dtype} {boxes.shape}")
-    if not isinstance(config, capi.ViewConfig):
-        raise capi.LavbError("agent_view: config must be a capi.ViewConfig")
+    b, _, _, _, _ = _tensor("agent_view", "rgbs", rgbs, torch.uint8, (None, 3, 288, 256, 3))
     dev = rgbs.device
-    if len({dev, tels.device, points.device, bev.device, plan.device, cast.device, cmds.device, other_locs.device,
-            other_cmds.device, target.device}) != 1:
-        raise capi.LavbError("agent_view: the inputs must be on one device")
+    _tensor("agent_view", "tels", tels, torch.uint8, (b, 192, 480, 3), dev)
+    _, p, s = _tensor("agent_view", "points", points, torch.float32, (b, None, None), dev)
+    _require(s >= 2, f"agent_view: points rows must hold x, y, got {tuple(points.shape)}")
+    _tensor("agent_view", "bev", bev, (torch.float32, h16()), (b, None, 320, 320), dev, contiguous=False)
+    _, t, _ = _tensor("agent_view", "plan", plan, torch.float32, (b, None, 2), dev)
+    _tensor("agent_view", "cast", cast, torch.float32, (b, t, 2), dev)
+    _tensor("agent_view", "target", target, torch.float32, (b, 2), dev)
+    _tensor("agent_view", "cmds", cmds, torch.int32, (b,), dev)
+    k, m, _, _ = _tensor("agent_view", "other_locs", other_locs, torch.float32, (None, None, t, 2), dev)
+    _tensor("agent_view", "other_cmds", other_cmds, torch.float32, (k, m), dev)
+    offsets = _host("agent_view", "offsets", offsets, np.int32, (b + 1,))
+    box_offsets = _host("agent_view", "box_offsets", box_offsets, np.int32, (b + 1,))
+    boxes = _host("agent_view", "boxes", boxes, np.float64, (None, 6))
+    _require(isinstance(config, capi.ViewConfig), "agent_view: config must be a capi.ViewConfig")
     need = agent_view_scratch_bytes(b)
     if scratch is None:
         scratch = torch.empty((need,), dtype=torch.uint8, device=dev)
-    elif scratch.dtype != torch.uint8 or scratch.numel() < need or not scratch.is_contiguous() or scratch.device != dev:
-        raise capi.LavbError(f"agent_view: scratch must be a contiguous uint8 tensor of >= {need} bytes on {dev}")
-    if out is None:
-        out = torch.empty((b, 160, 1146, 3), dtype=torch.uint8, device=dev)
-    elif out.dtype != torch.uint8 or tuple(out.shape) != (b, 160, 1146, 3) or not out.is_contiguous() or out.device != dev:
-        raise capi.LavbError(f"agent_view: out must be a contiguous ({b}, 160, 1146, 3) uint8 tensor on {dev}")
+    _tensor("agent_view", "scratch", scratch, torch.uint8, None, dev)
+    _require(scratch.numel() >= need, f"agent_view: scratch must hold >= {need} bytes, got {scratch.numel()}")
+    out = _out("agent_view", "out", out, torch.uint8, (b, 160, 1146, 3), dev)
     strides = (C.c_longlong * 4)(*bev.stride())
-    ip = lambda a: a.ctypes.data_as(C.c_void_p)
     code = F32 if bev.dtype == torch.float32 else capi.h16_code()
-    check(lib().lavb_agent_view(_ptr(rgbs), _ptr(tels), _ptr(points), b, points.shape[1], points.shape[2], _ptr(bev), code,
-                                bev.shape[1], strides, _ptr(plan), _ptr(cast), _ptr(cmds), t, _ptr(other_locs), _ptr(other_cmds),
-                                k, m, ip(offsets), ip(boxes) if boxes.size else None, boxes.shape[0], ip(box_offsets), _ptr(target),
-                                C.byref(config), _ptr(scratch), scratch.numel(), _ptr(out), _stream()), "lavb_agent_view")
-    if b:    # histogram, points per 256 agents, boxes per 96 (at most), compose
-        _COUNT[0] += int(points.shape[1] > 0) + -(-b // 256) + -(-int(box_offsets[b] - box_offsets[0]) // 96) + 1
+    # histogram, points per 256 agents, boxes per 96 (at most), compose
+    n = int(p > 0) + -(-b // 256) + -(-int(box_offsets[b] - box_offsets[0]) // 96) + 1 if b else 0
+    _launch("lavb_agent_view", _ptr(rgbs), _ptr(tels), _ptr(points), b, p, s, _ptr(bev), code, bev.shape[1], strides, _ptr(plan),
+            _ptr(cast), _ptr(cmds), t, _ptr(other_locs), _ptr(other_cmds), k, m, _hptr(offsets), _hptr(boxes) if boxes.size else None,
+            boxes.shape[0], _hptr(box_offsets), _ptr(target), C.byref(config), _ptr(scratch), scratch.numel(), _ptr(out), launches=n)
     return out

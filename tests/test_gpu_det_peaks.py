@@ -204,7 +204,7 @@ def test_eval_batch_survivors_equal_peak_filter(cuda):
     assert keep[:4].sum() == sum(len(k) for k in D.KEPT) and keep[5:].any()
 
 
-def test_det_peaks_rejects_bad_arguments_and_writes_nothing(cuda):
+def test_det_peaks_rejects_bad_arguments_with_lavb_error_and_writes_nothing(cuda):
     """Rejected calls (checked on the host, before any launch) return non-zero and leave the output as it was; batch = 0
     succeeds and writes nothing."""
     lib = capi.lib()
@@ -231,5 +231,5 @@ def test_det_peaks_rejects_bad_arguments_and_writes_nothing(cuda):
     assert ok.shape == (1, 7, 15)
     for b, o in ((box[:, :16, :15].contiguous(), ori[:, :16, :16].contiguous()),
                  (box[:, :16, :16].contiguous(), torch.zeros((1, 16, 16, 3), device=cuda))):
-        with pytest.raises(AssertionError):
+        with pytest.raises(capi.LavbError):
             ops.det_peaks(center[:, :16, :16].contiguous(), b, o)
