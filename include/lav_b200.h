@@ -228,6 +228,42 @@ int lavb_eval_batch(const void* d_seg, int seg_dtype, const uint8_t* d_gt, int g
                     double min_score, const float* d_plan, const float* d_ego_locs, int n_plan, long long* d_iou, int* d_ngt,
                     float* d_score, int* d_flags, double* d_plan_err, void* stream);
 
+/* ---------------------------------------------------------------- box scores of the decoded detections
+ * stands behind: the boxes LAVAgent.visualize draws (lav_agent_fast.py:485-490) and UniPlanner.infer crops at; the reference
+ *           scores detections by centre only.  Rotated-box IoU matches and the position, size and heading errors of the
+ *           detections lavb_eval_batch matches at 2 m.
+ * One block per sample (batches of more than 256 samples take one launch per 256).  d_packed (b, 7, 2 * n_det), w, d_actors /
+ *   n_actors / h_offsets (at most 1024 rows per sample), ppm, cx0, cy0, cy1 and min_score exactly as lavb_eval_batch takes them;
+ *   the survivors (its decode_packed filters), their rank order and the ground truth (class 0 / 1 in the window) are its own, and
+ *   d_ngt (b, 2) int32 equals its d_ngt.
+ * Boxes in map pixels, fp64.  A survivor in column j: centre (x, y) = its peak pixel, half extents (ww, hh) = packed rows 2, 3,
+ *   heading (c, s) = packed rows 4, 5.  An actor: centre = (cx, cy) placed as lavb_det_heatmaps places it, half extents (bx * ppm,
+ *   by * ppm) (exact in fp64), (c, s) = (cos, sin)(ori) in fp64.  Corners: u = (-(s * ww), c * ww), v = (-(c * hh), -(s * hh)),
+ *   corner k = (x + (a_k * u.x + b_k * v.x), y + (a_k * u.y + b_k * v.y)) for (a, b) = (-1, -1), (-1, 1), (1, 1), (1, -1) (the
+ *   reference's drawing without its int cast).  Area = |s| / 2 with s the shoelace sum over i ascending of (x_i * y_{i+1} -
+ *   x_{i+1} * y_i).  A box is degenerate when an extent is not finite and > 0, c, s or the centre is not finite, or its area is 0.
+ * IoU of survivor box P and actor box Q: 0 when either is degenerate or when the corner bounding boxes are apart (P's largest x <
+ *   Q's smallest x, or the same the other way or in y); else P is clipped by each edge e = 0..3 of Q in turn (Sutherland-Hodgman):
+ *   with (x0, y0) = corner e, (ex, ey) = corner e+1 - corner e, side(p) = ex * (p.y - y0) - ey * (p.x - x0), a vertex is inside
+ *   when side <= 0; the vertices q in order, each with its predecessor p (the last vertex before the first): when exactly one of
+ *   p, q is inside, p + t * (q - p) with t = side(p) / (side(p) - side(q)) is emitted, then q when inside (at most 16 vertices
+ *   kept; a convex polygon has at most 8).  I = the area of the result (0 below 3 vertices), IoU = I / ((A + B) - I), 0 when
+ *   that union is not > 0.  Every fp64 operation is correctly rounded and none is contracted.
+ * IoU match, per class and threshold k (0.3, 0.5, 0.7): the survivors in rank order each take the actor of their class not yet
+ *   taken at k with the highest IoU >= the threshold; equal IoUs go to the lower actor row.  2 m match: lavb_eval_batch's match at
+ *   2 m (the same search, the same result).
+ * Outputs per column, (b, 2 * n_det) row-major: d_score fp32 = the packed score; d_flags int32 = bit 4 survivor, bit k (0..2) IoU
+ *   match at threshold k, bit 3 the 2 m match; d_actor (.., 4) int32 = the actor row within the sample of the matches at the three
+ *   thresholds and at 2 m, -1 for none; d_err (.., 5) fp64, for a column with a 2 m match (NaN otherwise): the IoU of its box
+ *   with the actor's; the translation error sqrt(d2) / ppm in metres; the scale error 1 - i / ((ww * hh + wa * ha) - i), i =
+ *   min(ww, wa) * min(hh, ha), with (wa, ha) the actor's half extents (1 when an extent is not finite and > 0); the heading error
+ *   min(r, 2 pi - r) with r = fmod(|atan2(s, c) - ori|, 2 pi) (NaN when the heading or ori is not finite); the actor's distance
+ *   from the window centre in metres.  Every output element of the b samples is written; a rejected call writes nothing.
+ *   1 <= n_det <= 64; err 8-byte aligned, the other arrays 4-byte aligned. */
+int lavb_det_box_eval(const float* d_packed, int b, int w, int n_det, const void* d_actors, int n_actors, const int* h_offsets,
+                      float ppm, float cx0, float cy0, float cy1, double min_score, float* d_score, int* d_flags, int* d_actor,
+                      double* d_err, int* d_ngt, void* stream);
+
 /* ---------------------------------------------------------------- scores of the planners' motion forecasts
  * replaces: the forecast terms of the planners' training losses (other_cast_loss, ego_cast_loss, cmd_loss in lav_b200.train) as
  *           displacement errors and branch choices per forecast row, for an evaluation over a recording.

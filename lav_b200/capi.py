@@ -96,6 +96,9 @@ _SIGS = {
                                           C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_float, C.c_float,
                                           C.c_float, C.c_float, C.c_double, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                           C.c_void_p, C.c_void_p]),
+    "lavb_det_box_eval": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_float, C.c_float,
+                                    C.c_float, C.c_float, C.c_double, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                    C.c_void_p]),
     "lavb_plan_safety": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
                                    C.c_longlong, C.c_int, C.c_int, C.c_float, C.c_float, C.c_float, C.c_float, C.c_void_p,
                                    C.c_void_p]),

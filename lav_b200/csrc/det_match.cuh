@@ -1,6 +1,6 @@
-// The matching of decoded detections to the recorded actors, shared by the evaluation kernel (evaluate.cu) and the match of the
-// detected-forecast rows (det_forecast.cu): the order detections are taken in, the ego window and the greedy nearest-unmatched
-// search, so a detection takes the same actor in both.
+// The matching of decoded detections to the recorded actors, shared by the evaluation kernel (evaluate.cu), the match of the
+// detected-forecast rows (det_forecast.cu) and the box scores (det_box_eval.cu): the peak filters, the order detections are
+// taken in, the ego window and the greedy nearest-unmatched search, so a detection takes the same actor in all three.
 #pragma once
 #include "det_grid.cuh"
 
@@ -29,6 +29,29 @@ __device__ __forceinline__ void peak_pixel(float flat, int w, long long& loc, lo
   if (x < 0) x += w;
   y = (loc - x) / w;
 }
+
+// The constants of InferModel.decode_packed's filters on a map of ppm pixels per metre: score > float32(min_score) in fp32, the
+// class-1 size filter and the ego window 2 < d < 30 m, in pixels.
+struct DetFilter {
+  float min_score;                   // the reference compares fp32 scores in fp32
+  float size_thr;                    // class 1: dropped when both box sides are below it (pixels)
+  double win_lo, win_hi;
+};
+
+inline DetFilter det_filter(float ppm, double min_score) {
+  DetFilter f;
+  f.min_score = (float)min_score;
+  f.size_thr = (float)(0.1 * (double)ppm);                        // numpy compares the float32 sizes with float32(0.1 * ppm)
+  f.win_lo = 2.0;                                                 // decode_packed's `dist <= 2 | dist >= 30 * ppm` (pixels)
+  f.win_hi = 30.0 * (double)ppm;
+  return f;
+}
+
+// Whether a packed peak of class cls with score sc and box sides (bw, bh), at window_dist d, survives decode_packed's filters;
+// a NaN score never survives.  f is any struct with DetFilter's four fields (the kernels' argument structs).  A macro rather
+// than a function: a function boundary here changes the code nvcc emits for eval_batch_kernel, the expression in place does not.
+#define LAVB_PEAK_SURVIVES(sc, bw, bh, d, cls, f) \
+  ((sc) > (f).min_score && !((cls) == 1 && (bw) < (f).size_thr && (bh) < (f).size_thr) && (d) > (f).win_lo && (d) < (f).win_hi)
 
 // One warp, every lane calling with the same arguments: the nearest of actors [0, n) with ok(i) whose squared distance from
 // (px, py) is at most thr2; equal distances go to the lower row.  -> the row, or -1 with *d2 = +inf, on every lane.

@@ -106,7 +106,7 @@ __global__ void __launch_bounds__(kThreads) eval_batch_kernel(const EvalArgs p, 
     lavb::peak_pixel(pk[ncols], p.w, loc, x, y);
     const double d = lavb::window_dist((double)x, (double)y, p.g);
     const int cls = tid / p.n_det;
-    const bool keep = sc > p.min_score && !(cls == 1 && bw < p.size_thr && bh < p.size_thr) && d > p.win_lo && d < p.win_hi;
+    const bool keep = LAVB_PEAK_SURVIVES(sc, bw, bh, d, cls, p);
     s_score[tid] = sc; s_loc[tid] = loc; s_x[tid] = (int)x; s_y[tid] = (int)y; s_keep[tid] = keep; s_flags[tid] = keep ? 16 : 0;
   }
   const int a0 = off.a[bl], a1 = off.a[bl + 1];
@@ -209,10 +209,8 @@ extern "C" int lavb_eval_batch(const void* d_seg, int seg_dtype, const uint8_t* 
   a.plan = d_plan; a.ego_locs = d_ego_locs;
   a.h = h; a.w = w; a.gt_planes = gt_planes; a.n_det = n_det; a.n_plan = n_plan;
   a.g = DetGrid{ppm, cx0, cy0, cy1, 0.f};
-  a.min_score = (float)min_score;
-  a.win_lo = 2.0;                                                 // decode_packed's `dist <= 2 | dist >= 30 * ppm` (pixels)
-  a.win_hi = 30.0 * (double)ppm;
-  a.size_thr = (float)(0.1 * (double)ppm);                        // numpy compares the float32 sizes with float32(0.1 * ppm)
+  const lavb::DetFilter f = lavb::det_filter(ppm, min_score);
+  a.min_score = f.min_score; a.win_lo = f.win_lo; a.win_hi = f.win_hi; a.size_thr = f.size_thr;
   a.iou = d_iou; a.ngt = d_ngt; a.score = d_score; a.flags = d_flags; a.plan_err = d_plan_err;
   cudaStream_t st = (cudaStream_t)stream;
   for (int b0 = 0; b0 < b; b0 += kChunk) {

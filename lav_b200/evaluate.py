@@ -4,7 +4,7 @@ against the expert's future — as numbers over every sample of the recording, t
 
     python -m lav_b200.evaluate --config-path config_v2.yaml --data-dir VALDIR --lidar-weights lidar_7.th \
         --uniplanner-weights uniplanner_7.th [--batch-size 32] [--precision f16|fp32] [--num-workers 16] [--json out.json] \
-        [--forecast] [--forecast-detected] [--plan-safety]
+        [--forecast] [--forecast-detected] [--plan-safety] [--det-boxes]
     python -m lav_b200.evaluate ... --lidar-weights lidar_8.th lidar_16.th --uniplanner-weights uniplanner_8.th uniplanner_16.th
     python -m lav_b200.evaluate ... --run-dir RUN [--epochs 1,8,16-64]
     torchrun --nproc-per-node N -m lav_b200.evaluate ...
@@ -129,6 +129,29 @@ the batch's bev; no extra model call.  The protocol:
     class), vehicle_collision_rate, pedestrian_collision_rate, off_road_rate, collision_rate_by_step (T values: the share of
     samples whose first collision is at or before that step), and the summed off_map_steps and invalid_steps.  A rate over no
     sample is null.
+
+With --det-boxes (``det_boxes=True``) the result also holds ``det_boxes``: the detections scored as boxes, by rotated-box IoU
+and by the position, size and heading errors of the detections matched at 2 m.  Per batch: one ops.det_box_eval launch on the
+packed peaks and the actor table eval_batch reads, and one copy of its result buffer; no extra model call.  The protocol
+(lavb_det_box_eval in include/lav_b200.h states every operation):
+
+  Survivors and ground truth.  Those of eval_batch: the same filters, rank order and window, per class.
+  Boxes, in map pixels, fp64.  A detection: centre at its peak pixel, half extents packed rows 2-3 (ww, hh), heading (cos, sin)
+    = packed rows 4-5, corners centre + (+-ww (-sin, cos) +- hh (-cos, -sin)), the boxes LAVAgent.visualize draws.  An actor:
+    centre at det_centre, half extents (bx, by) * ppm, heading (cos, sin)(ori), the targets detections_to_heatmap writes.  A box
+    with an extent not finite and > 0, a non-finite heading or centre, or zero area is degenerate: IoU 0 with every box.
+  IoU.  The exact intersection area of the two quadrilaterals (the detection's clipped by the actor's, Sutherland-Hodgman, then
+    the shoelace formula), I / (A + B - I).
+  IoU match.  Per class and threshold 0.3 / 0.5 / 0.7: the survivors in rank order each take the untaken actor of their class
+    with the highest IoU >= the threshold, ties to the lower actor row.
+  Errors of the 2 m match (eval_batch's, the same pairs): the IoU of the pair; translation = the pixel distance / ppm; scale =
+    1 - the IoU of the two boxes with centres and headings aligned (nuScenes' ASE), from the half extents; heading = min(r, 2 pi -
+    r), r = fmod(|atan2(sin, cos) - ori|, 2 pi), in [0, pi]; range = the actor's distance from the ego in metres.
+  Host reduction (DetBoxScores), per class: n_gt, n_det, ap_iou[t] = average_precision of the survivors at IoU threshold t
+    (det[cls].ap's tie rule), matched = the 2 m matches, recall = matched / n_gt, and over the matches the mean IoU,
+    translation_m, scale, heading_rad and flipped_rate (the share with a heading error > pi / 2); the same errors per range band
+    of the actor's distance, [0, 10), [10, 20) and [20, 30) m.  Heading means skip a non-finite heading error.  A mean over no
+    row, and recall and AP with n_gt = 0, are null.
 """
 import argparse
 import json
@@ -353,6 +376,74 @@ class DetectedForecastScores:
                     ap=average_precision(s[~untracked], tp[~untracked], self.gt), match_m=self.match_m)
 
 
+DET_BOX_RANGES_M = ((0, 10), (10, 20), (20, 30))      # range bands of the box errors, by the matched actor's distance
+
+
+class DetBoxScores:
+    """host accumulation of ops.det_box_eval results over a recording."""
+
+    def __init__(self):
+        self.score, self.flags, self.err = [[] for _ in CLASSES], [[] for _ in CLASSES], [[] for _ in CLASSES]
+        self.ngt = np.zeros(len(CLASSES), np.int64)
+
+    def add(self, v):
+        """v = ops.det_box_views of a host copy of one batch's result buffer."""
+        score, flags, err = v["score"].numpy(), v["flags"].numpy(), v["err"].numpy()
+        n_det = score.shape[1] // 2
+        for c in range(len(CLASSES)):
+            s, f, e = (a[:, c * n_det:(c + 1) * n_det] for a in (score, flags, err))
+            keep = (f & 16) != 0
+            self.score[c].append(s[keep].copy())
+            self.flags[c].append(f[keep].copy())
+            self.err[c].append(e[keep].copy())
+        self.ngt += v["ngt"].numpy().sum(0)
+
+    def extend(self, other):
+        """append the records of ``other``, which follow this one's in sample order."""
+        for c in range(len(CLASSES)):
+            self.score[c] += other.score[c]
+            self.flags[c] += other.flags[c]
+            self.err[c] += other.err[c]
+        self.ngt += other.ngt
+
+    @staticmethod
+    def errors(e):
+        """the means over the matched rows ``e`` (k, 5) of ops.DET_BOX_ERRORS; the heading's over its finite values."""
+        mean = lambda a: float(np.mean(a)) if len(a) else None
+        h = e[:, 3][np.isfinite(e[:, 3])]
+        return dict(matched=len(e), mean_iou=mean(e[:, 0]), translation_m=mean(e[:, 1]), scale=mean(e[:, 2]), heading_rad=mean(h),
+                    flipped_rate=mean(h > np.pi / 2))
+
+    def summary(self):
+        out = {}
+        for c, name in enumerate(CLASSES):
+            s = np.concatenate(self.score[c]) if self.score[c] else np.zeros(0, np.float32)
+            f = np.concatenate(self.flags[c]) if self.flags[c] else np.zeros(0, np.int32)
+            e = np.concatenate(self.err[c]) if self.err[c] else np.zeros((0, len(ops.DET_BOX_ERRORS)))
+            n_gt = int(self.ngt[c])
+            m = e[(f & 8) != 0]
+            d = dict(n_gt=n_gt, n_det=len(s),
+                     ap_iou={f"{t:g}": average_precision(s, (f >> k) & 1, n_gt) for k, t in enumerate(ops.DET_BOX_IOU_THRESHOLDS)},
+                     recall=len(m) / n_gt if n_gt else None, **self.errors(m))
+            d["by_range"] = {f"{lo}-{hi}": self.errors(m[(m[:, 4] >= lo) & (m[:, 4] < hi)]) for lo, hi in DET_BOX_RANGES_M}
+            out[name] = d
+        return out
+
+
+def format_det_boxes(r):
+    """the printout lines of a DetBoxScores summary."""
+    fmt = lambda v: "n/a" if v is None else f"{v:.4f}"
+    errs = lambda d: (f"IoU {fmt(d['mean_iou'])}, translation {fmt(d['translation_m'])} m, scale {fmt(d['scale'])}, heading "
+                      f"{fmt(d['heading_rad'])} rad, flipped {fmt(d['flipped_rate'])}")
+    lines = []
+    for name, d in r.items():
+        lines.append(f"det boxes, {name} ({d['n_gt']} GT, {d['n_det']} detections): AP at IoU " +
+                     " ".join(f"{k}={fmt(v)}" for k, v in d["ap_iou"].items()) +
+                     f"; {d['matched']} matched at 2 m, recall {fmt(d['recall'])}: " + errs(d))
+        lines += [f"  {band} m: {e['matched']} matched, " + errs(e) for band, e in d["by_range"].items()]
+    return lines
+
+
 PLAN_SAFETY_TRAJECTORIES = ("plan", "expert")
 
 
@@ -418,19 +509,19 @@ def format_plan_safety(s):
 
 
 def evaluate(lidar_model, uniplanner, dataset, batch_size=32, precision="f16", num_workers=16, forecast=False,
-             forecast_detected=False, plan_safety=False):
+             forecast_detected=False, plan_safety=False, det_boxes=False):
     """Scores of ``lidar_model`` and ``uniplanner`` over every sample of ``dataset`` (a TemporalLiDARPaintedDataset), the models
     run as the agent runs them at ``precision``; with ``forecast`` also the UniPlanner's forecast scores on the recorded poses,
     with ``forecast_detected`` those on the detected vehicles, with ``plan_safety`` the collision and off-road rates of the ego
-    plan and of the expert.  -> dict (see the module docstring); None on a rank other than 0 of a process group."""
+    plan and of the expert, with ``det_boxes`` the detections' box scores.  -> dict (see the module docstring); None on a rank other than 0 of a process group."""
     results = evaluate_checkpoints([(lidar_model, uniplanner)], dataset, batch_size, precision, num_workers, forecast,
-                                   forecast_detected, plan_safety)
+                                   forecast_detected, plan_safety, det_boxes)
     return None if results is None else results[0]
 
 
 @torch.no_grad()
 def evaluate_checkpoints(pairs, dataset, batch_size=32, precision="f16", num_workers=16, forecast=False, forecast_detected=False,
-                         plan_safety=False):
+                         plan_safety=False, det_boxes=False):
     """evaluate() of every (lidar_model, uniplanner) of ``pairs`` in one pass over ``dataset``: each batch is loaded and staged
     once, then every pair runs its own InferModel and scoring launches on it into its own accumulators.  All pairs stay
     resident; a sweep that would not fit on the device is refused before any data is loaded.  In a process group each rank
@@ -450,21 +541,22 @@ def evaluate_checkpoints(pairs, dataset, batch_size=32, precision="f16", num_wor
                 pixels_per_meter=dataset.pixels_per_meter)
     loader = TemporalBatchLoader(dataset, batch_size, rank=rank, world=world, drop_last=False, num_workers=num_workers, ordered=True,
                                  plan_safety=plan_safety)
-    accs = [(Scores(), ForecastScores(), DetectedForecastScores(), PlanSafetyScores()) for _ in models]
+    accs = [(Scores(), ForecastScores(), DetectedForecastScores(), PlanSafetyScores(), DetBoxScores()) for _ in models]
     with math_mode(precision):
         for batch, staged in loader.staged_batches():
             actors = staged["actors"].to(dev, non_blocking=True)
             for im, acc in zip(models, accs):
-                score_batch(im, batch, staged, actors, grid, acc, forecast, forecast_detected, plan_safety)
+                score_batch(im, batch, staged, actors, grid, acc, forecast, forecast_detected, plan_safety, det_boxes)
     accs = gather_merged(accs)
     if accs is None:
         return None
-    return [summarize(acc, precision, forecast, forecast_detected, plan_safety, dataset.num_plan) for acc in accs]
+    return [summarize(acc, precision, forecast, forecast_detected, plan_safety, dataset.num_plan, det_boxes) for acc in accs]
 
 
-def summarize(acc, precision, forecast, forecast_detected, plan_safety, num_plan):
-    """the evaluate() result of one checkpoint's accumulators ``acc`` (score_batch's tuple)."""
-    scores, forecasts, detected, safety = acc
+def summarize(acc, precision, forecast, forecast_detected, plan_safety, num_plan, det_boxes=False):
+    """the evaluate() result of one checkpoint's accumulators ``acc`` (score_batch's tuple; its DetBoxScores is read only with
+    ``det_boxes``)."""
+    scores, forecasts, detected, safety = acc[:4]
     result = scores.summary()
     result["precision"] = precision
     if forecast:
@@ -473,13 +565,16 @@ def summarize(acc, precision, forecast, forecast_detected, plan_safety, num_plan
         result["forecast_detected"] = detected.summary()
     if plan_safety:
         result["plan_safety"] = safety.summary(num_plan)
+    if det_boxes:
+        result["det_boxes"] = acc[4].summary()
     return result
 
 
-def score_batch(im, batch, staged, actors, grid, acc, forecast, forecast_detected, plan_safety):
+def score_batch(im, batch, staged, actors, grid, acc, forecast, forecast_detected, plan_safety, det_boxes=False):
     """one checkpoint's InferModel ``im`` on one loader batch (its 14-tuple, staged tables and the actor table on the device),
-    scored into ``acc`` = (Scores, ForecastScores, DetectedForecastScores, PlanSafetyScores)."""
-    scores, forecasts, detected, safety = acc
+    scored into ``acc`` = (Scores, ForecastScores, DetectedForecastScores, PlanSafetyScores, DetBoxScores); the last is used
+    only with ``det_boxes``."""
+    scores, forecasts, detected, safety = acc[:4]
     dev = actors.device
     lidars, num_points, bev, ego_locs, cmds, nxps = batch[0], batch[1], batch[5], batch[6], batch[7], batch[8]
     out = im.forward_batch(lidars, num_points, nxps, cmds)
@@ -499,6 +594,9 @@ def score_batch(im, batch, staged, actors, grid, acc, forecast, forecast_detecte
     if plan_safety:
         res = score_plan_safety(out["ego_plan_locs"], ego_locs, staged["plan_safety"], bev, grid)
         safety.add(res.cpu().numpy(), host_cmds)
+    if det_boxes:
+        res = ops.det_box_eval(out["packed"], actors, staged["offsets"], grid)
+        acc[4].add(ops.det_box_views(res.cpu(), len(num_points), out["packed"].shape[2]))
 
 
 def parse_args(argv=None):
@@ -516,6 +614,8 @@ def parse_args(argv=None):
                     help="also score the forecasts the agent makes for the vehicles it detects, matched to the recorded tracks")
     ap.add_argument("--plan-safety", action="store_true",
                     help="also score the ego plan and the expert for collisions with the recorded traffic and for leaving the road")
+    ap.add_argument("--det-boxes", action="store_true",
+                    help="also score the detections as rotated boxes: IoU AP and the position, size and heading errors of the 2 m matches")
     return ap.parse_args(argv)
 
 
@@ -538,6 +638,8 @@ def format_result(r):
                      f"FDE {fmt(d['top_fde'])} m, miss rate {fmt(d['miss_rate'])}, AP {fmt(d['ap'])}")
     if "plan_safety" in r:
         lines += format_plan_safety(r["plan_safety"])
+    if "det_boxes" in r:
+        lines += format_det_boxes(r["det_boxes"])
     return "\n".join(lines)
 
 
@@ -552,6 +654,9 @@ def headline(r):
         cols.append(("det fc AP", r["forecast_detected"]["ap"]))
     if "plan_safety" in r:
         cols += [("collision", r["plan_safety"]["plan"]["collision_rate"]), ("off-road", r["plan_safety"]["plan"]["off_road_rate"])]
+    if "det_boxes" in r:
+        veh = r["det_boxes"]["vehicle"]
+        cols += [("veh AP@IoU.5", veh["ap_iou"]["0.5"]), ("veh heading", veh["heading_rad"])]
     return cols
 
 
@@ -586,7 +691,7 @@ def main(argv=None):
         pairs.append((lid, uni))
     ds = TemporalLiDARPaintedDataset(args.config_path, device=dev, overrides=dict(data_dir=args.data_dir))
     results = evaluate_checkpoints(pairs, ds, args.batch_size, args.precision, args.num_workers, args.forecast,
-                                   args.forecast_detected, args.plan_safety)
+                                   args.forecast_detected, args.plan_safety, args.det_boxes)
     out = None
     if results is not None:
         text, out = report(checkpoints, results, rank_and_world()[1])

@@ -749,6 +749,45 @@ def eval_batch(seg, gt, packed, actors, offsets, plan, ego_locs, grid=None, min_
     return out
 
 
+DET_BOX_IOU_THRESHOLDS = (0.3, 0.5, 0.7)      # rotated-box IoU thresholds of the box match (det_box_eval.cu)
+DET_BOX_ERRORS = ("iou", "translation_m", "scale", "heading_rad", "range_m")
+
+
+def _det_box_parts(b, ncols):  # 8-byte parts first
+    return [("err", torch.float64, (b, ncols, len(DET_BOX_ERRORS))), ("score", torch.float32, (b, ncols)),
+            ("flags", torch.int32, (b, ncols)), ("actor", torch.int32, (b, ncols, len(DET_BOX_IOU_THRESHOLDS) + 1)),
+            ("ngt", torch.int32, (b, 2))]
+
+
+def det_box_views(buf, b, ncols):
+    """the named parts of a det_box_eval result buffer (on the device or a host copy of it): err (b, ncols, 5) fp64 = per column
+    with a 2 m match the DET_BOX_ERRORS (the IoU with the matched actor's box, translation in metres, scale error, heading error in
+    radians, the actor's distance from the ego in metres), NaN otherwise; score (b, ncols) fp32 = the packed scores; flags (b,
+    ncols) int32 = bit 4 survivor, bit k an IoU match at DET_BOX_IOU_THRESHOLDS[k], bit 3 the 2 m match; actor (b, ncols, 4)
+    int32 = the actor row of each of those four matches, -1 for none; ngt (b, 2) int32 = actors per class in the window."""
+    return _views(buf, _det_box_parts(b, ncols))
+
+
+def det_box_eval(packed, actors, offsets, grid=None, min_score=0.2, out=None):
+    """The box scores of one batch's detections in one launch (see lavb_det_box_eval in include/lav_b200.h).  packed (B,7,2*n_det)
+    fp32 from det_peaks, actors (A,6) fp32 on the device and offsets (B+1,) int32 on the HOST (eval_batch's actor table); grid:
+    the keyword arguments of det_grid; min_score as eval_batch's.  -> the uint8 result buffer (written into ``out`` when given),
+    read through det_box_views, usually after one copy to the host."""
+    b, _, ncols = _tensor("det_box_eval", "packed", packed, torch.float32, (None, 7, None))
+    _require(ncols % 2 == 0, f"det_box_eval: packed must be (B, 7, 2*n_det), got {tuple(packed.shape)}")
+    dev = packed.device
+    _tensor("det_box_eval", "actors", actors, torch.float32, (None, 6), dev)
+    offsets = _host("det_box_eval", "offsets", offsets, np.int32, (b + 1,))
+    parts = _det_box_parts(b, ncols)
+    out = _out("det_box_eval", "out", out, torch.uint8, (_layout(parts)[1],), dev)
+    v = _views(out, parts)
+    h, w, (ppm, cx0, cy0, cy1, _) = det_grid(**(grid or {}))
+    _launch("lavb_det_box_eval", _ptr(packed), b, w, ncols // 2, _ptr(actors), actors.shape[0], _hptr(offsets), ppm, cx0, cy0, cy1,
+            float(min_score), _ptr(v["score"]), _ptr(v["flags"]), _ptr(v["actor"]), _ptr(v["err"]), _ptr(v["ngt"]),
+            launches=-(-b // 256))
+    return out
+
+
 def _forecast_parts(k):
     return [("err", torch.float64, (k, 6)), ("branch", torch.int32, (k, 2))]
 
