@@ -47,7 +47,21 @@ int lavb_h16_dtype(void);
  * mode 1: d_sem holds softmax probabilities (c_in>=2) -> c_in-1 outputs p[1+j]*(1-p[0])
  * mode 2: d_sem holds logits; softmax over c_in then as mode 1
  * Row i of the output receives `copy_cols` leading columns of point i, then the painted
- * channels at column `out_col0`; later cameras overwrite earlier ones; unseen points get 0. */
+ * channels at column `out_col0`; later cameras overwrite earlier ones; unseen points get 0.
+ * Projection, bit for bit (project_hit.cuh): per camera, k-sequential fp32 FMA chains lidar_to_world, world_to_cam, the axis
+ *   swap (y, -z, x) and K; u = q0 / (1e-5f + q2), v = q1 / (1e-5f + q2) (IEEE division), each and q2 truncated toward zero to
+ *   int64, where NaN, +-inf and |value| >= 2^63 give INT64_MIN; a camera sees the point when q2' >= 0, 0 <= u < w, 0 <= v < h.
+ * Values: mode 0 copies the sem bits (NaN payloads included); mode 1 computes bg = 1 - p0 and p[k] * bg in fp32; mode 2 first
+ *   p = expf(x - max) / sum in fp32 (fmaxf max, so a NaN logit is skipped by the max; sum in class order; IEEE division), so any
+ *   NaN or +inf logit, or all logits -inf, gives NaN in every painted channel of that point.  Copied columns keep their bits.
+ * Written: per row the copy_cols leading columns and the c_out channels at out_col0, nothing else (columns between them and
+ *   past out_col0 + c_out keep their values).
+ * Checked before any launch (a rejected call writes nothing): n >= 0, pt_stride >= 3, ncam 1..4, mode 0..2, c_in 1..8 (mode
+ *   0) or 2..8, copy_cols <= pt_stride, copy_cols <= out_col0, out_col0 + c_out <= out_stride, frames 0..65535; then, unless n
+ *   or frames is 0 (nothing written), non-null pointers and d_pts / d_sem / d_out 4-byte aligned.  h_cams must hold 41 * ncam
+ *   floats.  Any alignment above that is optional: the point row is read as one 16-byte vector when pt_stride is 4 and every
+ *   frame's rows are 16-byte aligned, and the copied columns stored as one when copy_cols is 4, out_col0 >= 4 and every output
+ *   row is 16-byte aligned; other layouts are read and written element by element. */
 int lavb_paint(const float* d_pts, int n, int pt_stride,
                const float* d_sem, int ncam, int c_in, int h, int w,
                long long s_cam, long long s_c, long long s_y, long long s_x,
@@ -67,7 +81,11 @@ int lavb_paint_batched(const float* d_pts, int frames, int n, int pt_stride, lon
  * evaluated for the hit pixel only, so the (h x w x c_cls) logit maps are never materialised.
  * d_feat: NHWC (frames*ncam, h/2, w/2, 16) fp32 or h16 = input of output_conv; d_deconv: 2*2*16*8 + 8 = 520 floats =
  * w[v%2][u%2][c_in][k] (k >= c_cls zero) | bias[8].  Output row as lavb_paint mode 2: copy_cols point columns, then c_cls-1
- * painted channels at out_col0. */
+ * painted channels at out_col0.  The hit pixel (v, u) of camera c in frame f reads feature pixel (v/2, u/2) of image f*ncam + c;
+ * logit k = bias[k], then fmaf(feat[ch], w[v&1][u&1][ch][k], .) over ch = 0..15 in order (h16 features widened exactly), then
+ * lavb_paint's mode-2 softmax, NaN rule and suppression.  Projection, written columns and layout checks as lavb_paint; also
+ * checked: c_cls 2..8, h and w even, feat_dtype LAVB_F32 or the 16-bit type, and (n, frames > 0) non-null pointers, d_feat 16-byte
+ * (fp32) / 8-byte (h16) aligned, d_pts / d_deconv / d_out 4-byte aligned. */
 int lavb_paint_deconv_batched(const float* d_pts, int frames, int n, int pt_stride, long long pts_frame_stride,
                               const void* d_feat, int feat_dtype, int ncam, int c_cls, int h, int w,
                               const float* d_deconv, const float* h_cams, float* d_out, int out_stride,
@@ -125,7 +143,13 @@ int lavb_paint_confusion(const float* d_pts, int frames, int n, const int* d_met
 /* ---------------------------------------------------------------- sweep stacking
  * replaces: LAVAgent.get_stacked_lidar + move_lidar_points (team_code_v2/lav_agent_fast.py:363-383,547-565)
  * and the ego-roof filter LAVAgent.preprocess (lav_agent.py:448-457, roof_filter!=0 marks dropped rows x=NaN).
- * dst row = [xyz @ R + (dx,dy,0) | src cols 3..src_cols | one_hot(time_idx, n_time)];  h_R is 3x3 row-major. */
+ * dst row = [xyz @ R + (dx,dy,0) | src cols 3..src_cols | one_hot(time_idx, n_time)];  h_R is 3x3 row-major (9 floats).
+ * Arithmetic, bit for bit: x' = fp32(fmaf(z, R[6], fmaf(y, R[3], x * R[0])) + dx), y' likewise with R[1], R[4], R[7] and dy (real
+ * adds: a -0 sum becomes +0), z' = fmaf(z, R[8], fmaf(y, R[5], x * R[2])) (no add: a -0 z' stays -0).  With roof_filter, x' of a
+ * row inside lavb_roof_filter's box (tested on the input x, y, z) is the canonical NaN.  Copied columns keep their bits.  Every
+ * element of the n dst rows is written, nothing else.
+ * Checked before any launch (a rejected call writes nothing): n >= 0, src_cols >= 3, n_time >= 0, time_idx >= 0 and, when
+ * n_time > 0, time_idx < n_time; then, unless n is 0, non-null pointers, d_src / d_dst 4-byte aligned and not overlapping. */
 int lavb_stack_sweep(const float* d_src, int n, int src_cols, const float* h_R, float dx, float dy,
                      int time_idx, int n_time, int roof_filter, float* d_dst, void* stream);
 
@@ -134,14 +158,25 @@ int lavb_stack_sweep(const float* d_src, int n, int src_cols, const float* h_R, 
  *           lav_agent_fast.py:247): rows with x in (-2.4,0), y in (-0.8,0.8), z in (-1.5,-1) are removed, the others keep their order.
  * `frames` independent sweeps of n rows x cols floats (frame f at d_src + f*src_frame_stride); the kept rows of frame f are written
  * to d_dst + f*dst_frame_stride, their number to d_counts[f] (may be NULL); with pad_nan the remaining rows [count, n) are filled
- * with NaN (the fixed-shape pipeline's padding — every kernel drops NaN rows).  d_dst must not alias d_src. */
+ * with NaN (the fixed-shape pipeline's padding — every kernel drops NaN rows).  The box test is the fp32 comparisons above on the
+ * raw x, y, z, so a row with a NaN coordinate is kept; kept rows are copied bit for bit.  Written: the kept rows and, with
+ * pad_nan, rows [count, n) of each frame (canonical NaN); without pad_nan those rows keep their values.
+ * Checked before any launch (a rejected call writes nothing): frames, n >= 0, cols >= 3, src_frame_stride >= 0; then, unless
+ * frames is 0, dst_frame_stride >= n * cols when frames > 1 (output frames must not overlap), non-null d_src / d_dst, 4-byte
+ * aligned pointers, and the dst extent ((frames - 1) * dst_frame_stride + n * cols floats) not overlapping the src extent. */
 int lavb_roof_filter(const float* d_src, int frames, int n, int cols, long long src_frame_stride, float* d_dst,
                      long long dst_frame_stride, int* d_counts, int pad_nan, void* stream);
 
 /* table-driven variant: d_jobs is a DEVICE array of n_jobs 72-byte records
  *   { const float* src; float* dst; int n; int time_idx; float R[9]; float dx, dy; int pad; }
  * (one per (agent, sweep)); all jobs run in one launch and the table can be rewritten between replays of a captured
- * CUDA graph (new poses, new ring-buffer slots) without touching kernel arguments. max_n = largest job. */
+ * CUDA graph (new poses, new ring-buffer slots) without touching kernel arguments.  Each job is lavb_stack_sweep's row
+ * arithmetic on its n rows (src_cols in, src_cols + n_time out); a time_idx outside [0, n_time) sets no one-hot column; a job
+ * with n <= 0 writes nothing.  max_n only sizes the grid: a job longer than max_n is still done in full.  A job's src and dst
+ * must be 4-byte aligned and not overlap; with src_cols 8, a 16-byte aligned src is read as two 16-byte vectors (the kernel
+ * tests each job's src, since the table is device data the call never sees).
+ * Checked before any launch (a rejected call writes nothing): 0 <= n_jobs <= 65535, max_n >= 0, src_cols >= 3, n_time >= 0,
+ * src_cols + n_time <= 16; then, unless n_jobs or max_n is 0, d_jobs non-null and 8-byte aligned. */
 int lavb_stack_jobs(const void* d_jobs, int n_jobs, int max_n, int src_cols, int n_time, int roof_filter, void* stream);
 
 /* ---------------------------------------------------------------- temporal BEV training targets
@@ -183,11 +218,15 @@ int lavb_png_decode_gray8(const uint8_t* d_src, long long src_bytes, const void*
  * d_sweeps: DEVICE array of n_sweeps 88-byte records, sorted by row0,
  *   { float R_aug[9]; float R_mv[9]; float dx, dy; int time_idx; int row0; }
  *   (3x3 row-major matrices).  Each output row = [xyz' @ R_mv + (dx, dy, 0) | r | painted * vis | one_hot(time_idx, n_time)] with
- *   xyz' = xyz @ R_aug + (0, 0, 0) (a real fp32 add: -0 becomes +0) and vis = 1 if lavb_paint's projection through the ncam
+ *   xyz' = xyz @ R_aug + (0, 0, 0) (lavb_stack_sweep's arithmetic: x' and y' take a real fp32 add, so a -0 there becomes +0;
+ *   z' has no add, so a -0 z' stays -0) and vis = 1 if lavb_paint's projection through the ncam
  *   cameras of h_cams (host, as lavb_paint) lands inside an h x w image, else 0, multiplied in as one fp32 multiply (NaN * 0 stays
  *   NaN).  Bit-identical to lavb_roof_filter + lavb_stack_sweep + lavb_paint (mode 0, a ones map) + multiply + lavb_stack_sweep.
  *   A row index outside [0, n_raw) or below the first row0 gives a zero row.
- * d_out: n_rows x (4 + c + n_time) fp32, every element written.  4 + c + n_time <= 16, ncam 1..4. */
+ *   The sweep of row src is the last one with row0 <= src.
+ * d_out: n_rows x (4 + c + n_time) fp32, every element written.  4 + c + n_time <= 16, ncam 1..4.
+ * Checked before any launch (a rejected call writes nothing): the sizes >= 0, n_raw < 2^31, fewer than 2^31 blocks of 256 rows,
+ *   non-null h_cams, row table and output (n_rows > 0), raw rows and sweeps (n_raw > 0), every device pointer 4-byte aligned. */
 int lavb_lidar_batch(const float* d_raw, long long n_raw, int c, const int* d_rows, long long n_rows, const void* d_sweeps,
                      int n_sweeps, const float* h_cams, int ncam, int h, int w, int n_time, float* d_out, void* stream);
 

@@ -17,7 +17,7 @@ __global__ void __launch_bounds__(256) paint_kernel(const float* __restrict__ pt
                                                     const __grid_constant__ CamSet cams, float* __restrict__ out,
                                                     int out_stride, int out_col0, int copy_cols,
                                                     long long pts_frame_stride, long long sem_frame_stride,
-                                                    long long out_frame_stride) {
+                                                    long long out_frame_stride, int vec_in, int vec_out) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
   // blockIdx.y = frame of a batch of independent agents (each with its own sweep and semantic maps)
@@ -27,8 +27,7 @@ __global__ void __launch_bounds__(256) paint_kernel(const float* __restrict__ pt
   const float* p = pts + (size_t)i * pt_stride;
   float x, y, z;
   float4 p4;
-  const bool vec = (pt_stride == 4);
-  if (vec) {
+  if (vec_in) {
     p4 = __ldg(reinterpret_cast<const float4*>(p));
     x = p4.x; y = p4.y; z = p4.z;
   } else {
@@ -37,7 +36,7 @@ __global__ void __launch_bounds__(256) paint_kernel(const float* __restrict__ pt
   int hit_u = 0, hit_v = 0;
   const int hit_cam = project_hit(cams, x, y, z, H, W, hit_u, hit_v);
   float* o = out + (size_t)i * out_stride;
-  if (copy_cols == 4 && vec && out_col0 >= 4 && (out_stride % 4) == 0) {
+  if (vec_out) {
     *reinterpret_cast<float4*>(o) = p4;
   } else {
     for (int k = 0; k < copy_cols; ++k) o[k] = __ldg(p + k);
@@ -141,6 +140,16 @@ __global__ void __launch_bounds__(256) convert_kernel(const TS* __restrict__ s, 
 
 using namespace lavb;
 
+// The float4 paths of the painting kernels, decided here from the pointers and strides: a point row is loaded as one float4
+// when every frame's rows are 4 floats and 16-byte aligned; its 4 copied columns are stored as one float4 when, in addition,
+// every output row is 16-byte aligned and the painted channels start past them.  Any other layout takes the per-element path.
+static void paint_vec(const float* d_pts, int pt_stride, long long pts_fs, const float* d_out, int out_stride, long long out_fs,
+                      int out_col0, int copy_cols, int frames, int& vec_in, int& vec_out) {
+  vec_in = pt_stride == 4 && is_aligned(d_pts, 16) && (frames <= 1 || pts_fs % 4 == 0);
+  vec_out = vec_in && copy_cols == 4 && out_col0 >= 4 && out_stride % 4 == 0 && is_aligned(d_out, 16) &&
+            (frames <= 1 || out_fs % 4 == 0);
+}
+
 static int paint_impl(const float* d_pts, int n, int pt_stride, const float* d_sem, int ncam, int c_in, int h, int w,
                       long long s_cam, long long s_c, long long s_y, long long s_x, const float* h_cams, int mode,
                       float* d_out, int out_stride, int out_col0, int copy_cols, int frames, long long pts_fs, long long sem_fs,
@@ -153,13 +162,17 @@ static int paint_impl(const float* d_pts, int n, int pt_stride, const float* d_s
   LAVB_CHECK_ARG(copy_cols >= 0 && copy_cols <= pt_stride && out_col0 >= copy_cols && out_col0 + c_out <= out_stride,
                  "paint: output row layout inconsistent");
   if (n == 0 || frames == 0) return 0;
+  LAVB_CHECK_ARG(d_pts && d_sem && d_out && h_cams, "paint: null pointer");
+  LAVB_CHECK_ARG(is_aligned(d_pts, 4) && is_aligned(d_sem, 4) && is_aligned(d_out, 4), "paint: d_pts, d_sem and d_out must be 4-byte aligned");
   CamSet cs;
   memcpy(cs.m, h_cams, sizeof(float) * 41 * ncam);
   cs.ncam = ncam;
+  int vec_in, vec_out;
+  paint_vec(d_pts, pt_stride, pts_fs, d_out, out_stride, out_fs, out_col0, copy_cols, frames, vec_in, vec_out);
   cudaStream_t st = (cudaStream_t)stream;
   const dim3 blocks(ceil_div(n, 256), frames);
 #define LAUNCH(M) paint_kernel<M><<<blocks, 256, 0, st>>>(d_pts, n, pt_stride, d_sem, c_in, h, w, s_cam, s_c, s_y, s_x, cs, \
-                                                           d_out, out_stride, out_col0, copy_cols, pts_fs, sem_fs, out_fs)
+                                                           d_out, out_stride, out_col0, copy_cols, pts_fs, sem_fs, out_fs, vec_in, vec_out)
   if (mode == 0) LAUNCH(0); else if (mode == 1) LAUNCH(1); else LAUNCH(2);
 #undef LAUNCH
   LAVB_LAUNCH_OK();
@@ -194,7 +207,8 @@ __global__ void __launch_bounds__(256) paint_deconv_kernel(const float* __restri
                                                            const TF* __restrict__ feat, int c_cls, int H, int W,
                                                            const __grid_constant__ CamSet cams, const DeconvW* __restrict__ dw,
                                                            float* __restrict__ out, int out_stride, int out_col0, int copy_cols,
-                                                           long long pts_frame_stride, long long out_frame_stride) {
+                                                           long long pts_frame_stride, long long out_frame_stride, int vec_in,
+                                                           int vec_out) {
   __shared__ DeconvW sw;
   for (int i = threadIdx.x; i < (int)(sizeof(DeconvW) / 4); i += blockDim.x) reinterpret_cast<float*>(&sw)[i] = __ldg(reinterpret_cast<const float*>(dw) + i);
   __syncthreads();
@@ -205,13 +219,12 @@ __global__ void __launch_bounds__(256) paint_deconv_kernel(const float* __restri
   const float* p = pts + (size_t)i * pt_stride;
   float x, y, z;
   float4 p4;
-  const bool vec = (pt_stride == 4);
-  if (vec) { p4 = __ldg(reinterpret_cast<const float4*>(p)); x = p4.x; y = p4.y; z = p4.z; }
+  if (vec_in) { p4 = __ldg(reinterpret_cast<const float4*>(p)); x = p4.x; y = p4.y; z = p4.z; }
   else { x = __ldg(p); y = __ldg(p + 1); z = __ldg(p + 2); }
   int hit_u = 0, hit_v = 0;
   const int hit_cam = project_hit(cams, x, y, z, H, W, hit_u, hit_v);
   float* o = out + (size_t)i * out_stride;
-  if (copy_cols == 4 && vec && out_col0 >= 4 && (out_stride % 4) == 0) *reinterpret_cast<float4*>(o) = p4;
+  if (vec_out) *reinterpret_cast<float4*>(o) = p4;
   else for (int k = 0; k < copy_cols; ++k) o[k] = __ldg(p + k);
   o += out_col0;
   if (hit_cam < 0) {
@@ -246,20 +259,26 @@ extern "C" int lavb_paint_deconv_batched(const float* d_pts, int frames, int n, 
   LAVB_CHECK_ARG(h % 2 == 0 && w % 2 == 0, "paint_deconv: image size must be even (the feature map is h/2 x w/2)");
   LAVB_CHECK_ARG(copy_cols >= 0 && copy_cols <= pt_stride && out_col0 >= copy_cols && out_col0 + c_cls - 1 <= out_stride,
                  "paint_deconv: output row layout inconsistent");
+  LAVB_CHECK_ARG(feat_dtype == LAVB_F32 || feat_dtype == LAVB_H16, "paint_deconv: feature dtype must be fp32 or h16");
   if (n == 0 || frames == 0) return 0;
+  LAVB_CHECK_ARG(d_pts && d_feat && d_deconv && h_cams && d_out, "paint_deconv: null pointer");
+  LAVB_CHECK_ARG(is_aligned(d_pts, 4) && is_aligned(d_deconv, 4) && is_aligned(d_out, 4) &&
+                     is_aligned(d_feat, feat_dtype == LAVB_F32 ? 16 : 8),
+                 "paint_deconv: d_feat must be 16-byte (fp32) / 8-byte (h16) aligned, d_pts, d_deconv and d_out 4-byte aligned");
   CamSet cs;
   memcpy(cs.m, h_cams, sizeof(float) * 41 * ncam);
   cs.ncam = ncam;
+  int vec_in, vec_out;
+  paint_vec(d_pts, pt_stride, pts_frame_stride, d_out, out_stride, out_frame_stride, out_col0, copy_cols, frames, vec_in, vec_out);
   const dim3 blocks(ceil_div(n, 256), frames);
   cudaStream_t st = (cudaStream_t)stream;
   const DeconvW* dw = reinterpret_cast<const DeconvW*>(d_deconv);
   if (feat_dtype == LAVB_F32)
     paint_deconv_kernel<float><<<blocks, 256, 0, st>>>(d_pts, n, pt_stride, (const float*)d_feat, c_cls, h, w, cs, dw, d_out, out_stride,
-                                                       out_col0, copy_cols, pts_frame_stride, out_frame_stride);
-  else if (feat_dtype == LAVB_H16)
+                                                       out_col0, copy_cols, pts_frame_stride, out_frame_stride, vec_in, vec_out);
+  else
     paint_deconv_kernel<h16><<<blocks, 256, 0, st>>>(d_pts, n, pt_stride, (const h16*)d_feat, c_cls, h, w, cs, dw, d_out, out_stride,
-                                                     out_col0, copy_cols, pts_frame_stride, out_frame_stride);
-  else LAVB_CHECK_ARG(false, "paint_deconv: feature dtype must be fp32 or h16");
+                                                     out_col0, copy_cols, pts_frame_stride, out_frame_stride, vec_in, vec_out);
   LAVB_LAUNCH_OK();
   return 0;
 }
@@ -279,6 +298,9 @@ __global__ void __launch_bounds__(256) stack_jobs_kernel(const StackJob* __restr
                                                          int roof_filter) {
   __shared__ float rows[256 * kStackMaxCols];
   const StackJob j = jobs[blockIdx.y];
+  // the table is rewritten between graph replays without the host seeing it, so the vector path is chosen here, per job (one
+  // branch, uniform across the block)
+  const bool src16 = (reinterpret_cast<uintptr_t>(j.src) & 15) == 0;
   const int dcols = src_cols + n_time;
   for (int i0 = blockIdx.x * 256; i0 < j.n; i0 += gridDim.x * 256) {
     const int i = i0 + threadIdx.x;
@@ -286,7 +308,7 @@ __global__ void __launch_bounds__(256) stack_jobs_kernel(const StackJob* __restr
       const float* s = j.src + (size_t)i * src_cols;
       float* d = rows + threadIdx.x * dcols;
       float x, y, z;
-      if (src_cols == 8) {            // fused sweeps: two aligned 16-byte loads per row
+      if (src_cols == 8 && src16) {   // fused sweeps: two 16-byte loads per row
         const float4 a = __ldg(reinterpret_cast<const float4*>(s)), b = __ldg(reinterpret_cast<const float4*>(s) + 1);
         x = a.x; y = a.y; z = a.z;
         d[3] = a.w; d[4] = b.x; d[5] = b.y; d[6] = b.z; d[7] = b.w;
@@ -309,9 +331,11 @@ __global__ void __launch_bounds__(256) stack_jobs_kernel(const StackJob* __restr
 }
 
 extern "C" int lavb_stack_jobs(const void* d_jobs, int n_jobs, int max_n, int src_cols, int n_time, int roof_filter, void* stream) {
-  LAVB_CHECK_ARG(n_jobs >= 0 && n_jobs <= 65535 && src_cols >= 3 && n_time >= 0, "stack_jobs: bad arguments");
+  LAVB_CHECK_ARG(n_jobs >= 0 && n_jobs <= 65535 && max_n >= 0 && src_cols >= 3 && n_time >= 0,
+                 "stack_jobs: bad arguments (n_jobs %d, max_n %d, src_cols %d, n_time %d)", n_jobs, max_n, src_cols, n_time);
   LAVB_CHECK_ARG(src_cols + n_time <= kStackMaxCols, "stack_jobs: rows wider than %d floats", kStackMaxCols);
   if (n_jobs == 0 || max_n == 0) return 0;
+  LAVB_CHECK_ARG(d_jobs != nullptr && is_aligned(d_jobs, 8), "stack_jobs: d_jobs null or not 8-byte aligned");
   dim3 grid(min(ceil_div(max_n, 256), 64), n_jobs);
   stack_jobs_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(reinterpret_cast<const StackJob*>(d_jobs), src_cols, n_time, roof_filter);
   LAVB_LAUNCH_OK();
@@ -379,6 +403,9 @@ extern "C" int lavb_lidar_batch(const float* d_raw, long long n_raw, int c, cons
                  ncam, h, w);
   LAVB_CHECK_ARG(n_rows == 0 || (d_rows != nullptr && d_out != nullptr), "lidar_batch: null row table or output");
   LAVB_CHECK_ARG(n_raw == 0 || (d_raw != nullptr && d_sweeps != nullptr && n_sweeps > 0), "lidar_batch: null raw rows or sweeps");
+  LAVB_CHECK_ARG((n_rows + 255) / 256 <= 0x7fffffffLL, "lidar_batch: n_rows %lld needs 2^31 or more blocks", n_rows);
+  LAVB_CHECK_ARG(is_aligned(d_raw, 4) && is_aligned(d_rows, 4) && is_aligned(d_sweeps, 4) && is_aligned(d_out, 4),
+                 "lidar_batch: d_raw, d_rows, d_sweeps and d_out must be 4-byte aligned");
   if (n_rows == 0) return 0;
   CamSet cs;
   memcpy(cs.m, h_cams, sizeof(float) * 41 * ncam);
@@ -435,9 +462,16 @@ __global__ void __launch_bounds__(1024) roof_filter_kernel(const float* __restri
 
 extern "C" int lavb_roof_filter(const float* d_src, int frames, int n, int cols, long long src_frame_stride, float* d_dst,
                                 long long dst_frame_stride, int* d_counts, int pad_nan, void* stream) {
-  LAVB_CHECK_ARG(frames >= 0 && n >= 0 && cols >= 3, "roof_filter: bad arguments");
-  LAVB_CHECK_ARG(d_src != d_dst, "roof_filter: in-place compaction is not supported");
+  LAVB_CHECK_ARG(frames >= 0 && n >= 0 && cols >= 3 && src_frame_stride >= 0, "roof_filter: bad arguments");
   if (frames == 0) return 0;
+  const long long frame = (long long)n * cols;
+  LAVB_CHECK_ARG(frames == 1 || dst_frame_stride >= frame, "roof_filter: output frames overlap (dst_frame_stride %lld < n * cols %lld)",
+                 dst_frame_stride, frame);
+  LAVB_CHECK_ARG(d_src && d_dst, "roof_filter: null pointer");
+  LAVB_CHECK_ARG(is_aligned(d_src, 4) && is_aligned(d_dst, 4) && is_aligned(d_counts, 4), "roof_filter: pointers must be 4-byte aligned");
+  LAVB_CHECK_ARG(!ranges_overlap(d_src, 4 * (size_t)((frames - 1) * src_frame_stride + frame), d_dst,
+                                 4 * (size_t)((frames - 1) * (frames > 1 ? dst_frame_stride : 0) + frame)),
+                 "roof_filter: d_dst overlaps d_src (in-place compaction is not supported)");
   roof_filter_kernel<<<frames, 1024, 0, (cudaStream_t)stream>>>(d_src, n, cols, src_frame_stride, d_dst, dst_frame_stride, d_counts,
                                                                   pad_nan);
   LAVB_LAUNCH_OK();
@@ -449,6 +483,10 @@ extern "C" int lavb_stack_sweep(const float* d_src, int n, int src_cols, const f
   LAVB_CHECK_ARG(n >= 0 && src_cols >= 3 && n_time >= 0 && time_idx >= 0 && (n_time == 0 || time_idx < n_time),
                  "stack_sweep: bad arguments");
   if (n == 0) return 0;
+  LAVB_CHECK_ARG(d_src && d_dst && h_R, "stack_sweep: null pointer");
+  LAVB_CHECK_ARG(is_aligned(d_src, 4) && is_aligned(d_dst, 4), "stack_sweep: d_src and d_dst must be 4-byte aligned");
+  LAVB_CHECK_ARG(!ranges_overlap(d_src, 4 * (size_t)n * src_cols, d_dst, 4 * (size_t)n * (src_cols + n_time)),
+                 "stack_sweep: d_dst overlaps d_src");
   StackParams P;
   memcpy(P.R, h_R, sizeof(float) * 9);
   P.dx = dx; P.dy = dy;

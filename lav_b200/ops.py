@@ -119,13 +119,15 @@ def paint(points, sem, cams, mode, copy_cols=0, out=None, out_col0=None):
     cams (ncam,41) float32 numpy (K|lidar_to_world|world_to_cam).  See lavb_paint in include/lav_b200.h."""
     n, _ = _tensor("paint", "points", points, torch.float32, (None, None), contiguous=False)
     _require(points.stride(1) == 1, "paint: points must have unit stride along a row")
-    ncam, c_in, h, w = _tensor("paint", "sem", sem, torch.float32, (None,) * 4, contiguous=False)
+    ncam, c_in, h, w = _tensor("paint", "sem", sem, torch.float32, (None,) * 4, points.device, contiguous=False)
     c_out = c_in if mode == 0 else c_in - 1
     if out_col0 is None:
         out_col0 = copy_cols
     if out is None:
         out = torch.empty((n, out_col0 + c_out), dtype=torch.float32, device=points.device)
-    _require(out.stride(1) == 1, "paint: out must have unit stride along a row")
+    _, oc = _tensor("paint", "out", out, torch.float32, (n, None), points.device, contiguous=False)
+    _require(out.stride(1) == 1 and oc >= out_col0 + c_out, f"paint: out must have unit stride along a row and hold "
+             f"{out_col0 + c_out} columns, got {tuple(out.shape)} with strides {out.stride()}")
     cams = _host("paint", "cams", cams, np.float32, (ncam, 41), cast=True)
     s = sem.stride()
     _launch("lavb_paint", _ptr(points), n, points.stride(0), _ptr(sem), ncam, c_in, h, w, s[0], s[1], s[2], s[3], _hptr(cams), mode,
@@ -135,9 +137,9 @@ def paint(points, sem, cams, mode, copy_cols=0, out=None, out_col0=None):
 
 def stack_sweep(src, R, dx, dy, time_idx, n_time, dst, roof_filter=False):
     """dst (n, src_cols+n_time) <- [src[:, :3] @ R + (dx,dy,0) | src[:,3:] | one_hot(time_idx)]"""
-    _tensor("stack_sweep", "src", src, None, None)
-    _tensor("stack_sweep", "dst", dst, None, (src.shape[0], src.shape[1] + n_time))
-    R = np.ascontiguousarray(R, dtype=np.float32)
+    _tensor("stack_sweep", "src", src, torch.float32, (None, None))
+    _tensor("stack_sweep", "dst", dst, torch.float32, (src.shape[0], src.shape[1] + n_time), src.device)
+    R = _host("stack_sweep", "R", R, np.float32, (3, 3), cast=True)
     _launch("lavb_stack_sweep", _ptr(src), src.shape[0], src.shape[1], _hptr(R), float(dx), float(dy), time_idx, n_time,
             int(roof_filter), _ptr(dst))
     return dst
@@ -152,8 +154,7 @@ def roof_filter(sweeps, pad_nan=False, out=None):
     f, n, cols = x.shape
     if out is None:
         out = torch.empty_like(x)
-    _tensor("roof_filter", "out", out, None, x.shape)
-    _require(out.data_ptr() != x.data_ptr(), "roof_filter: out must not be the sweeps' storage")
+    _tensor("roof_filter", "out", out, torch.float32, x.shape, x.device)
     counts = torch.empty((f,), dtype=torch.int32, device=x.device)
     _launch("lavb_roof_filter", _ptr(x), f, n, cols, n * cols, _ptr(out), n * cols, _ptr(counts), int(pad_nan))
     return (out if sweeps.dim() == 3 else out[0]), counts
@@ -419,9 +420,10 @@ def deconv3x3s2_small(x, groups, cin_g, w, bias, n_outs, sigmoids):
 def paint_batched(points, sem, cams, mode, copy_cols, out):
     """points (F,N,>=3) fp32 contiguous; sem logical (F,ncam,C,H,W) any strides; out (F,N,copy_cols+c_out) contiguous."""
     f, n, ps = _tensor("paint_batched", "points", points, torch.float32, (None,) * 3)
-    _, ncam, c_in, h, w = _tensor("paint_batched", "sem", sem, torch.float32, (None,) * 5, contiguous=False)
-    _tensor("paint_batched", "out", out, None, None)
-    cams = _host("paint_batched", "cams", cams, np.float32, None, cast=True)
+    _, ncam, c_in, h, w = _tensor("paint_batched", "sem", sem, torch.float32, (f, None, None, None, None), points.device,
+                                  contiguous=False)
+    _tensor("paint_batched", "out", out, torch.float32, (f, n, copy_cols + (c_in if mode == 0 else c_in - 1)), points.device)
+    cams = _host("paint_batched", "cams", cams, np.float32, (ncam, 41), cast=True)
     s = sem.stride()
     _launch("lavb_paint_batched", _ptr(points), f, n, ps, n * ps, _ptr(sem), ncam, c_in, h, w, s[0], s[1], s[2], s[3], s[4],
             _hptr(cams), mode, _ptr(out), out.shape[2], n * out.shape[2], copy_cols, copy_cols)
@@ -443,14 +445,13 @@ def pack_deconv2x2(weight, bias):
 def paint_deconv_batched(points, feat, n_classes, deconv, cams, copy_cols, out, image_hw):
     """points (F,N,>=3) fp32; feat NHWC (F*ncam, H/2, W/2, 16) fp32 / h16 = ERFNet decoder output before output_conv;
     deconv = pack_deconv2x2(...); out (F,N,copy_cols + n_classes-1)."""
-    _need_cuda(deconv)
     f, n, ps = _tensor("paint_deconv_batched", "points", points, torch.float32, (None,) * 3)
-    _tensor("paint_deconv_batched", "out", out, None, None)
+    _tensor("paint_deconv_batched", "out", out, torch.float32, (f, n, copy_cols + n_classes - 1), points.device)
     h, w = image_hw
-    cams = _host("paint_deconv_batched", "cams", cams, np.float32, None, cast=True)
+    cams = _host("paint_deconv_batched", "cams", cams, np.float32, (None, 41), cast=True)
     ncam = cams.shape[0]
-    _tensor("paint_deconv_batched", "feat", feat, None, (f * ncam, h // 2, w // 2, 16))
-    _require(deconv.numel() == 520, "paint_deconv_batched: deconv must be the 520-float pack_deconv2x2 table")
+    _tensor("paint_deconv_batched", "feat", feat, (torch.float32, h16()), (f * ncam, h // 2, w // 2, 16), points.device)
+    _tensor("paint_deconv_batched", "deconv", deconv, torch.float32, (520,), points.device)
     _launch("lavb_paint_deconv_batched", _ptr(points), f, n, ps, n * ps, _ptr(feat), _DT[feat.dtype], ncam, n_classes, h, w,
             _ptr(deconv), _hptr(cams), _ptr(out), out.shape[2], n * out.shape[2], copy_cols, copy_cols)
     return out
@@ -554,7 +555,9 @@ STACK_JOB_DTYPE = np.dtype([("src", np.uint64), ("dst", np.uint64), ("n", np.int
 
 def stack_jobs(d_jobs, n_jobs, max_n, src_cols, n_time, roof_filter=False):
     """d_jobs: uint8 device tensor holding n_jobs STACK_JOB_DTYPE records."""
-    _need_cuda(d_jobs)
+    _tensor("stack_jobs", "d_jobs", d_jobs, torch.uint8, (None,))
+    _require(d_jobs.numel() >= n_jobs * STACK_JOB_DTYPE.itemsize,
+             f"stack_jobs: d_jobs holds {d_jobs.numel()} bytes, fewer than {n_jobs} 72-byte STACK_JOB_DTYPE records")
     _launch("lavb_stack_jobs", _ptr(d_jobs), n_jobs, max_n, src_cols, n_time, int(roof_filter))
 
 

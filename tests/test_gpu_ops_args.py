@@ -20,7 +20,9 @@ def nc(t):
 
 
 def _cases(dev):
-    """(wrapper, valid keyword arguments, name of the output argument or None, bad overrides of those arguments)"""
+    """(wrapper, valid keyword arguments, output, bad overrides of those arguments).  The output is the name of the argument the
+    wrapper writes, None, or the tensor itself when the call reaches it only through a device table (stack_jobs): the case then
+    holds the tensor, so it outlives every call that writes through the table."""
     g = torch.Generator().manual_seed(7)
     r = lambda *s, dt=torch.float32: torch.rand(s, generator=g).to(dt).to(dev)             # noqa: E731
     z = lambda *s, dt=torch.float32: torch.zeros(s, dtype=dt, device=dev)                 # noqa: E731
@@ -42,15 +44,21 @@ def _cases(dev):
     c33 = r(1, 8, 8, 64, dt=h)
     xp = r(1, 8, 32, 64, dt=h)
     gru = [r(2, 512), r(6, 512, 192), r(6, 64, 192), r(6, 192), r(6, 192), r(6, 2, 64), r(6, 2)]
+    dst7 = z(64, 7)
+    job = np.zeros(1, ops.STACK_JOB_DTYPE)
+    job[0] = (pts.data_ptr(), dst7.data_ptr(), 64, 0, np.eye(3, dtype=np.float32).ravel(), 0.0, 0.0, 0)   # pts: held by the cases
+    jobs = torch.from_numpy(job.view(np.uint8)).to(dev)
     return [
         (ops.paint, dict(points=pts, sem=sem, cams=cams, mode=0, out=z(64, 5)), "out",
          [dict(points=pts.double()), dict(points=pts[None]), dict(points=pts.t()), dict(points=pts.cpu()), dict(sem=sem.half()),
-          dict(sem=sem[0]), dict(sem=sem.cpu()), dict(cams=cams[:2]), dict(out=z(64, 5).t())]),
+          dict(sem=sem[0]), dict(sem=sem.cpu()), dict(cams=cams[:2]), dict(out=z(64, 5).t()), dict(out=z(64, 5).double()),
+          dict(out=z(63, 5)), dict(out=z(64, 4)), dict(cams=cams[:, :40])]),
         (ops.stack_sweep, dict(src=pts, R=np.eye(3), dx=1.0, dy=2.0, time_idx=1, n_time=3, dst=z(64, 7)), "dst",
-         [dict(src=nc(pts)), dict(src=pts.cpu()), dict(dst=nc(z(64, 7))), dict(dst=z(64, 6)), dict(dst=z(63, 7))]),
+         [dict(src=nc(pts)), dict(src=pts.cpu()), dict(dst=nc(z(64, 7))), dict(dst=z(64, 6)), dict(dst=z(63, 7)),
+          dict(src=pts.half()), dict(dst=z(64, 7).double()), dict(R=np.eye(2)), dict(R=np.ones(8))]),
         (ops.roof_filter, dict(sweeps=sw, out=z(1, 64, 4)), "out",
          [dict(sweeps=pts.double()), dict(sweeps=nc(pts)), dict(sweeps=pts.flatten()), dict(sweeps=pts.cpu()), dict(out=z(1, 64, 5)),
-          dict(out=nc(z(1, 64, 4))), dict(out=sw[None])]),
+          dict(out=nc(z(1, 64, 4))), dict(out=sw[None]), dict(out=z(1, 64, 4).double())]),
         (ops.pillar_forward, pill, None, pill_bad),
         (ops.pillar_forward_sorted, pill, None, pill_bad),
         (ops.pillar_decorate, dict(pts=p11, starts=[0], counts=[64], grid=GRID, d=11), None,
@@ -72,13 +80,18 @@ def _cases(dev):
          [dict(x=nc(tx)), dict(x=tx[0]), dict(x=tx.cpu()), dict(w=nc(r(1, 16, 9, 4))), dict(bias=nc(r(1, 4)))]),
         (ops.paint_batched, dict(points=pts[None], sem=sem[None], cams=cams, mode=1, copy_cols=4, out=z(1, 64, 8)), "out",
          [dict(points=pts[None].double()), dict(points=nc(pts[None])), dict(points=pts), dict(points=pts[None].cpu()),
-          dict(sem=sem[None].half()), dict(sem=sem), dict(out=nc(z(1, 64, 8)))]),
+          dict(sem=sem[None].half()), dict(sem=sem), dict(out=nc(z(1, 64, 8))), dict(out=z(1, 64, 7)), dict(out=z(1, 64, 8).double()),
+          dict(out=z(1, 63, 8)), dict(sem=sem[None].expand(2, -1, -1, -1, -1)), dict(cams=cams[:2]), dict(cams=cams[:, :40])]),
         (ops.pack_deconv2x2, dict(weight=r(16, 5, 2, 2), bias=r(5)), None,
          [dict(weight=r(16, 9, 2, 2), bias=r(9)), dict(weight=r(8, 5, 2, 2)), dict(weight=r(16, 5, 3, 3))]),
         (ops.paint_deconv_batched, dict(points=pts[None], feat=r(3, 16, 16, 16), n_classes=5, deconv=deconv, cams=cams, copy_cols=4,
                                         out=z(1, 64, 8), image_hw=(32, 32)), "out",
          [dict(points=pts[None].double()), dict(points=nc(pts[None])), dict(points=pts[None].cpu()), dict(feat=r(3, 16, 16, 8)),
-          dict(feat=nc(r(3, 16, 16, 16))), dict(deconv=deconv[:519]), dict(out=nc(z(1, 64, 8)))]),
+          dict(feat=nc(r(3, 16, 16, 16))), dict(deconv=deconv[:519]), dict(out=nc(z(1, 64, 8))), dict(deconv=deconv.half()),
+          dict(feat=r(3, 16, 16, 16).double()), dict(out=z(1, 64, 7)), dict(out=z(1, 64, 8).double()), dict(cams=cams[:, :40]),
+          dict(n_classes=9)]),
+        (ops.stack_jobs, dict(d_jobs=jobs, n_jobs=1, max_n=64, src_cols=4, n_time=3), dst7,
+         [dict(d_jobs=jobs[:71]), dict(n_jobs=2), dict(d_jobs=jobs.cpu()), dict(d_jobs=jobs.view(torch.int32)), dict(max_n=-1)]),
         (ops.bev_targets, dict(src_planes=r(2, 320, 320, dt=u8), jobs=ops.bev_jobs([(0, 0, 10.0, -5.0, 3, 2), (1, 1, 0.0, 0.0, 0, 0)]),
                                out=z(2, 320, 320, dt=u8)), "out",
          [dict(src_planes=r(2, 320, 320, dt=i32)), dict(src_planes=r(320, 320, dt=u8)), dict(src_planes=nc(r(2, 320, 320, dt=u8))),
@@ -113,7 +126,7 @@ def test_wrappers_refuse_bad_arguments_with_lavb_error(cuda):
         fn(**kw)
         for over in bad:
             call = {**kw, **over}
-            out = call.get(out_key)
+            out = out_key if torch.is_tensor(out_key) else call.get(out_key)
             if out is not None:
                 out.fill_(7)
             before = ops.launches()

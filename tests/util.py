@@ -468,3 +468,218 @@ def maxpool3x3s2_ref64(x_h16):
     m = F.max_pool2d(torch.where(neg0, torch.full_like(x, tiny), x), 3, 2, 1)
     m = torch.where(m == tiny, torch.full_like(m, -0.0), m)
     return m.permute(0, 2, 3, 1).contiguous()
+
+
+# ----------------------------------------------------------------------------------------------------- painting and stacking
+# Bit-exact fp32 statements of lavb_paint / _batched / lavb_paint_deconv_batched, lavb_stack_sweep / lavb_stack_jobs,
+# lavb_roof_filter and lavb_lidar_batch (include/lav_b200.h), in numpy.  numpy's fp32 +, -, *, / round to nearest as the
+# kernels' __fadd_rn, __fsub_rn, __fmul_rn, __fdiv_rn do; fma32 is a correctly rounded fmaf.  The one operation that is not
+# correctly rounded, expf, is bounded instead (paint_softmax32).
+F32 = np.float32
+INT64_MIN = np.int64(-2 ** 63)
+
+
+def fma32(a, b, c):
+    """fmaf(a, b, c) element-wise, correctly rounded: a*b is exact in fp64 (48 significant bits); s = a*b + c rounded to fp64
+    with its exact error from TwoSum; where the error is nonzero s is moved to the odd fp64 neighbour of the exact sum (round to
+    odd, 53 >= 24 + 2 bits), so the final fp64 -> fp32 rounding cannot double-round."""
+    a, b, c = (np.asarray(v, dtype=F32) for v in (a, b, c))
+    with np.errstate(all="ignore"):
+        p = a.astype(np.float64) * b.astype(np.float64)
+        c64 = c.astype(np.float64)
+        s = p + c64
+        bb = s - p
+        err = (p - (s - bb)) + (c64 - bb)
+        fix = np.isfinite(s) & (err != 0) & ((s.view(np.int64) & 1) == 0)
+        s = np.where(fix, np.nextafter(s, np.where(err > 0, np.inf, -np.inf)), s)
+        return s.astype(F32)
+
+
+def trunc_i64(v):
+    """cvttss2si as project_hit.cuh restates it: toward zero, NaN / +-inf / |v| >= 2^63 -> INT64_MIN"""
+    v = np.asarray(v, dtype=F32)
+    ok = np.abs(v) < F32(2.0 ** 63)
+    with np.errstate(all="ignore"):
+        return np.where(ok, np.where(ok, v, 0).astype(np.int64), INT64_MIN)
+
+
+def _dot(r, xs):
+    acc = (F32(r[0]) * xs[0]).astype(F32)
+    for k in range(1, len(xs)):
+        acc = fma32(F32(r[k]), xs[k], acc)
+    return acc
+
+
+def project_hit32(cams, x, y, z, H, W):
+    """project_hit.cuh: -> (camera (int64, -1 = unseen), u, v) for fp32 points; the last camera whose truncated pixel lies in
+    the W x H image wins."""
+    cams = np.asarray(cams, dtype=F32)
+    x, y, z = (np.asarray(t, dtype=F32) for t in (x, y, z))
+    one = np.ones_like(x)
+    cam, hu, hv = np.full(x.shape, -1, np.int64), np.zeros(x.shape, np.int64), np.zeros(x.shape, np.int64)
+    with np.errstate(all="ignore"):
+        for c in range(len(cams)):
+            K, L, Wc = cams[c, :9], cams[c, 9:25], cams[c, 25:41]
+            w = [_dot(L[4 * i:4 * i + 4], (x, y, z, one)) for i in range(4)]
+            c0, c1, c2 = (_dot(Wc[4 * i:4 * i + 4], w) for i in range(3))
+            a = (c1, -c2, c0)
+            q0, q1, q2 = (_dot(K[3 * i:3 * i + 3], a) for i in range(3))
+            den = (F32(1e-5) + q2).astype(F32)
+            u, v, zi = trunc_i64((q0 / den).astype(F32)), trunc_i64((q1 / den).astype(F32)), trunc_i64(q2)
+            hit = (zi >= 0) & (u >= 0) & (u < W) & (v >= 0) & (v < H)
+            cam, hu, hv = np.where(hit, c, cam), np.where(hit, u, hu), np.where(hit, v, hv)
+    return cam, hu, hv
+
+
+def paint_softmax32(x):
+    """lavb_paint mode 2's softmax and suppression on fp32 logits x (..., C) -> (want (..., C-1) float64, bound float64, nan
+    (...,) bool: every painted channel NaN).
+
+    Bit-exact parts: mx = fmaxf over the classes in order (NaN skipped), d_k = fp32(x_k - mx).  E_k = exp(d_k) in fp64; the
+    statement is want_k = P_k (1 - P_0), P_k = E_k / S, S = sum E_k.  The bound (u = 2^-24, gamma_n = n u / (1 - n u)):
+      * expf is within 2 ulp (CUDA C Programming Guide, full range): |e_k - E_k| <= dl_k = 2^-22 E_k + 2^-148 (the ulp of a
+        value is at most 2^-23 of it, or the subnormal spacing 2^-149);
+      * the sequential fp32 sum of C terms: |s - S| <= dS = sum dl_k + gamma_(C-1) sum (E_k + dl_k); S >= 1 (the max's term is
+        expf(0) = 1 exactly), so S - dS > 0 here;
+      * p_k = fp32(e_k / s): |e_k / s - P_k| <= (dl_k S + E_k dS) / (S (S - dS)) = r_k, plus the rounding u (P_k + r_k): eta_k;
+      * bg = fp32(1 - p_0): 1 - P_0 cancels, so its error is absolute: ebg = eta_0 + u (B + eta_0), B = 1 - P_0;
+      * o_k = fp32(p_k bg): |p_k bg - P_k B| <= eta_k (B + ebg) + P_k ebg, plus u times the magnitude.
+    The bound is on the absolute error of each output, with a 2^-40 relative margin for the fp64 evaluation of the statement.
+    NaN rule: any NaN or +inf logit, or all logits -inf, makes every output NaN (the sum is NaN)."""
+    x = np.asarray(x, dtype=F32)
+    C = x.shape[-1]
+    with np.errstate(all="ignore"):
+        mx = x[..., 0]
+        for k in range(1, C):
+            mx = np.fmax(mx, x[..., k])
+        d = (x - mx[..., None]).astype(F32)
+        nan = np.isnan(d).any(-1)
+        E = np.exp(d.astype(np.float64))
+        dl = 2.0 ** -22 * E + 2.0 ** -148
+        S = E.sum(-1, keepdims=True)
+        dS = dl.sum(-1, keepdims=True) + gamma(C - 1) * (E + dl).sum(-1, keepdims=True)
+        P = E / S
+        r = (dl * S + E * dS) / (S * (S - dS))
+        eta = r + U32 * (P + r)
+        B = 1.0 - P[..., :1]
+        ebg = eta[..., :1] + U32 * (B + eta[..., :1])
+        want = P[..., 1:] * B
+        e = eta[..., 1:] * (B + ebg) + P[..., 1:] * ebg
+        bound = (e + U32 * (want + e)) * (1 + 2.0 ** -40)
+    want = np.where(nan[..., None], np.nan, want)
+    return want, np.where(nan[..., None], 0.0, bound), nan
+
+
+def paint32(pts, sem, cams, mode, H, W):
+    """the painted channels of lavb_paint for fp32 points pts (..., >=3) and one frame's semantic maps sem (ncam, C, H, W) as a
+    numpy array (any strides) -> (want (..., c_out), bound or None, nan (...,) or None): mode 0 / 1 are bit-exact fp32 (bound
+    None), mode 2 is paint_softmax32's statement.  Unseen points are exact zeros."""
+    pts = np.asarray(pts, dtype=F32)
+    cam, u, v = project_hit32(cams, pts[..., 0], pts[..., 1], pts[..., 2], H, W)
+    seen = cam >= 0
+    g = np.asarray(sem, dtype=F32)[np.where(seen, cam, 0), :, np.where(seen, v, 0), np.where(seen, u, 0)]   # (..., C)
+    return _paint_values(g, seen, mode)
+
+
+def _paint_values(g, seen, mode):
+    C = g.shape[-1]
+    c_out = C if mode == 0 else C - 1
+    if mode == 0:
+        return np.where(seen[..., None], g, F32(0)), None, None
+    if mode == 1:
+        with np.errstate(all="ignore"):
+            bg = (F32(1) - g[..., 0]).astype(F32)
+            want = (g[..., 1:] * bg[..., None]).astype(F32)
+        return np.where(seen[..., None], want, F32(0)), None, None
+    want, bound, nan = paint_softmax32(g)
+    return np.where(seen[..., None], want, 0.0), np.where(seen[..., None], bound, 0.0), nan & seen
+
+
+def deconv_logits32(fv, table, pv, pu, C):
+    """deconv_logits.cuh: fv (..., 16) fp32 (h16 features widened exactly), table the 520-float pack_deconv2x2 table,
+    phases pv, pu (...) -> logits (..., C) fp32, bias then fmaf over the 16 channels in order"""
+    t = np.asarray(table, dtype=F32)
+    w, bias = t[:512].reshape(2, 2, 16, 8), t[512:]
+    out = []
+    for k in range(C):
+        acc = np.broadcast_to(bias[k], fv.shape[:-1]).astype(F32)
+        for c in range(16):
+            acc = fma32(fv[..., c], w[pv, pu, c, k], acc)
+        out.append(acc)
+    return np.stack(out, -1)
+
+
+def paint_deconv32(pts, feat, table, cams, C, H, W):
+    """lavb_paint_deconv_batched's painted channels: pts (F, N, >=3) fp32, feat (F * ncam, H/2, W/2, 16) as float32 (the h16
+    features widened) -> as paint32 mode 2"""
+    pts = np.asarray(pts, dtype=F32)
+    ncam = len(cams)
+    cam, u, v = project_hit32(cams, pts[..., 0], pts[..., 1], pts[..., 2], H, W)
+    seen = cam >= 0
+    f = np.arange(pts.shape[0])[:, None] * ncam + np.where(seen, cam, 0)
+    vv, uu = np.where(seen, v, 0), np.where(seen, u, 0)
+    fv = np.asarray(feat, dtype=F32)[f, vv >> 1, uu >> 1]
+    g = deconv_logits32(fv, table, vv & 1, uu & 1, C)
+    return _paint_values(g, seen, 2)
+
+
+def move_point32(R, dx, dy, x, y, z):
+    """paint.cu move_point: [x y z] @ R as k-sequential fmaf chains, then x + dx, y + dy as fp32 adds (z has no add)"""
+    R = np.asarray(R, dtype=F32).ravel()
+    with np.errstate(all="ignore"):
+        nx = (fma32(z, R[6], fma32(y, R[3], (x * R[0]).astype(F32))) + F32(dx)).astype(F32)
+        ny = (fma32(z, R[7], fma32(y, R[4], (x * R[1]).astype(F32))) + F32(dy)).astype(F32)
+        nz = fma32(z, R[8], fma32(y, R[5], (x * R[2]).astype(F32)))
+    return nx, ny, nz
+
+
+ROOF = tuple(F32(v) for v in (-2.4, 0, -0.8, 0.8, -1.5, -1))
+
+
+def roof_keep32(rows):
+    """lavb_roof_filter's keep predicate on (n, >=3) fp32 rows: not strictly inside the box (a NaN coordinate keeps the row)"""
+    x, y, z = (np.asarray(rows, dtype=F32)[:, k] for k in range(3))
+    x0, x1, y0, y1, z0, z1 = ROOF
+    return ~((x > x0) & (x < x1) & (y > y0) & (y < y1) & (z > z0) & (z < z1))
+
+
+def stack32(src, R, dx, dy, time_idx, n_time, roof=False):
+    """lavb_stack_sweep's rows: src (n, cols) fp32 -> (n, cols + n_time) fp32"""
+    src = np.asarray(src, dtype=F32)
+    out = np.zeros((src.shape[0], src.shape[1] + n_time), F32)
+    nx, ny, nz = move_point32(R, dx, dy, src[:, 0], src[:, 1], src[:, 2])
+    if roof:
+        nx = np.where(roof_keep32(src), nx, np.array([0x7FC00000], np.uint32).view(F32)[0])
+    out[:, 0], out[:, 1], out[:, 2] = nx, ny, nz
+    out[:, 3:src.shape[1]] = src[:, 3:]
+    if 0 <= time_idx < n_time:
+        out[:, src.shape[1] + time_idx] = 1
+    return out
+
+
+def lidar_batch32(raw, rows, sweeps, cams, H, W, n_time):
+    """lavb_lidar_batch: raw (n_raw, 4 + c) fp32, rows (n_rows,) int, sweeps LIDAR_SWEEP_DTYPE records sorted by row0 ->
+    (n_rows, 4 + c + n_time) fp32"""
+    raw = np.asarray(raw, dtype=F32)
+    rows = np.asarray(rows, dtype=np.int64).ravel()
+    cols = raw.shape[1]
+    out = np.zeros((len(rows), cols + n_time), F32)
+    valid = (rows >= 0) & (rows < len(raw))
+    s = np.searchsorted(sweeps["row0"].astype(np.int64), np.where(valid, rows, 0), side="right") - 1 if len(sweeps) else \
+        np.full(len(rows), -1)
+    live = valid & (s >= 0)
+    for k in np.unique(s[live]):
+        m = live & (s == k)
+        sw = sweeps[k]
+        p = raw[rows[m]]
+        ax, ay, az = move_point32(sw["R_aug"], 0.0, 0.0, p[:, 0], p[:, 1], p[:, 2])
+        vis = (project_hit32(cams, ax, ay, az, H, W)[0] >= 0).astype(F32)
+        o = out[m]
+        o[:, 0], o[:, 1], o[:, 2] = move_point32(sw["R_mv"], sw["dx"], sw["dy"], ax, ay, az)
+        o[:, 3] = p[:, 3]
+        with np.errstate(all="ignore"):
+            o[:, 4:cols] = (p[:, 4:] * vis[:, None]).astype(F32)
+        if 0 <= sw["time_idx"] < n_time:
+            o[:, cols + sw["time_idx"]] = 1
+        out[m] = o
+    return out
