@@ -216,11 +216,14 @@ class TemporalLiDARPaintedDataset:
         return 0.0, [(np.zeros(2), 0.0)] * (self.num_frame_stack + 1)
 
     # ---- host part: record reads, PNG chunk walks, labels, BEV job rows
-    def prepare(self, idx, angle, jitters, plan_safety=False):
+    def prepare(self, idx, angle, jitters, plan_safety=False, cameras=False):
         """the host record of sample ``idx``; with ``plan_safety`` (unaugmented samples only) it also holds the sample's
-        plan_safety_table, from the same record reads."""
+        plan_safety_table, from the same record reads; with ``cameras``, under "cameras", what CameraDataset reads for the brake
+        model (read_cameras: the three middle cameras of camera_yaws and tel_rgb[:-crop_tel_bottom])."""
         traj, index = self.index[idx]
         env = self.env(traj)
+        cams = read_cameras(env, index, brake_cameras(len(self.camera_yaws), "TemporalLiDARPaintedDataset"),
+                            self.crop_tel_bottom) if cameras else None
         T, nseg = self.num_plan, len(self.seg_channels)
         radii = (self.max_pedestrian_radius, self.max_vehicle_radius)
         frames = [i for i in range(index, index - self.num_frame_stack - 1, -1) if i >= 0]
@@ -260,6 +263,8 @@ class TemporalLiDARPaintedDataset:
                  locs=-p_locs, oris=p_oris, typs=p_typs, num_objs=n_obj)
         if table is not None:
             h["plan_safety"] = table
+        if cams is not None:
+            h["cameras"] = cams
         return h
 
     # ---- device part
@@ -350,6 +355,8 @@ class TemporalLiDARPaintedDataset:
                   labels={k: pinned(v) for k, v in labels.items()}, num_objs=[h["num_objs"] for h in hs])
         if hs and "plan_safety" in hs[0]:                                       # prepared with plan_safety (the evaluator)
             st["plan_safety"] = stage_plan_safety([h["plan_safety"] for h in hs], pin)
+        if hs and "cameras" in hs[0]:                                           # prepared with cameras (the brake evaluation)
+            st["cameras"] = stage_images([h["cameras"] for h in hs], ("rgbs", "tel"), pin, "TemporalLiDARPaintedDataset")
         return st
 
     @torch.no_grad()
@@ -416,20 +423,25 @@ class TemporalBatchLoader:
     With ``ordered`` (evaluation) the samples come in index order with no augmentation, rank r taking the contiguous range
     [r * n // world, (r + 1) * n // world): every draw is dataset.no_draw(), and the LiDAR shuffles still come from the
     generator of (seed, epoch, rank).  With ``plan_safety`` (ordered only) every sample is
-    prepared with its plan_safety_table, and the staged tables carry them packed under "plan_safety" (stage_plan_safety)."""
+    prepared with its plan_safety_table, and the staged tables carry them packed under "plan_safety" (stage_plan_safety).  With
+    ``cameras`` every sample is prepared with the brake model's camera images, and the staged tables carry them under "cameras"
+    as one pinned uint8 buffer per key: rgbs (B, 3, h, w, 3), tel (B, h_tel, w_tel, 3)."""
 
     def __init__(self, dataset, batch_size, seed=2021, rank=0, world=1, drop_last=True, num_workers=8, ordered=False,
-                 plan_safety=False):
+                 plan_safety=False, cameras=False):
         self.ds, self.B, self.seed, self.rank, self.world, self.drop_last = dataset, batch_size, seed, rank, world, drop_last
         self.num_workers = max(1, int(num_workers))
         self.ordered = ordered
         self.plan_safety = plan_safety
+        self.cameras = cameras
         if plan_safety and not ordered:
             raise LavbError("plan_safety tables need the ordered, unaugmented loader")
         self.epoch = 0
 
     def _prepare(self, pool, idxs, draws):
         kw = dict(plan_safety=True) if self.plan_safety else {}
+        if self.cameras:
+            kw["cameras"] = True
         return list(pool.map(lambda a: self.ds.prepare(int(a[0]), *a[1], **kw), zip(idxs, draws)))
 
     def shard(self, epoch):
@@ -635,6 +647,41 @@ def load_img(env, tag, i):
     return img[..., ::-1] if img.ndim == 3 else img
 
 
+def brake_cameras(ncam, what):
+    """the three middle cameras ncam//2 - 1 .. ncam//2 + 1 of ``ncam`` (BrakePredictionDataset's, bra_dataset.py:17-31), the
+    ones the brake model sees side by side; fewer than three cameras is a LavbError of ``what``."""
+    mid = [ncam // 2 - 1, ncam // 2, ncam // 2 + 1]
+    if mid[0] < 0 or mid[2] >= ncam:
+        raise LavbError(f"{what}: the brake model needs three middle cameras, the config has {ncam}")
+    return mid
+
+
+def read_cameras(env, i, cams, crop_tel_bottom=None):
+    """the colour images of frame ``i``, decoded by load_img: rgbs (len(cams), h, w, 3) of the cameras ``cams``, and with
+    ``crop_tel_bottom`` tel = tel_rgb[:-crop_tel_bottom] (h_tel - crop_tel_bottom, w_tel, 3); uint8 numpy."""
+    h = dict(rgbs=np.stack([load_img(env, f"rgb_{c}", i) for c in cams]))
+    if crop_tel_bottom is not None:
+        h["tel"] = load_img(env, "tel_rgb", i)[:-crop_tel_bottom]
+    return h
+
+
+def stage_images(hs, keys, pin, what):
+    """the images under ``keys`` of the prepared records ``hs`` stacked into one uint8 host buffer per key (pinned on ``pin``),
+    record b at index b; a key missing from the first record is skipped, images of different sizes are a LavbError of ``what``."""
+    st = {}
+    for key in keys:
+        if key in hs[0]:
+            shapes = {h[key].shape for h in hs}
+            if len(shapes) != 1:
+                raise LavbError(f"{what}: the {key} images of a batch differ in size: {sorted(shapes)}")
+            buf = torch.empty((len(hs),) + hs[0][key].shape, dtype=torch.uint8, pin_memory=pin)
+            dst = buf.numpy()
+            for b, h in enumerate(hs):
+                dst[b] = h[key]
+            st[key] = buf
+    return st
+
+
 class CameraDataset:
     """The camera samples of a recording, for scoring the segmentation and brake models (lav_b200.evaluate_rgb): the frames of
     BasicDataset (index_trajectories, the same YAML keys and ``overrides``), unaugmented.
@@ -658,9 +705,7 @@ class CameraDataset:
         self.device = torch.device(device)
         self.seg, self.brake = seg, brake
         ncam = len(self.camera_yaws)
-        mid = [ncam // 2 - 1, ncam // 2, ncam // 2 + 1]
-        if brake and (mid[0] < 0 or mid[2] >= ncam):
-            raise LavbError(f"CameraDataset: the brake model needs three middle cameras, the config has {ncam}")
+        mid = brake_cameras(ncam, "CameraDataset") if brake else [ncam // 2 - 1, ncam // 2, ncam // 2 + 1]
         self.cams = list(range(ncam)) if seg else mid
         self.brake_cams = [self.cams.index(c) for c in mid] if brake else []
         self.paths, self.index = index_trajectories(self.data_dir, self.percentage_data, self.all_towns, self.num_plan, seed)
@@ -678,11 +723,10 @@ class CameraDataset:
         (h_tel - crop_tel_bottom, w_tel, 3) and bra; uint8 numpy."""
         traj, i = self.index[idx]
         env = self.env(traj)
-        h = dict(rgbs=np.stack([load_img(env, f"rgb_{c}", i) for c in self.cams]))
+        h = read_cameras(env, i, self.cams, self.crop_tel_bottom if self.brake else None)
         if self.seg:
             h["labels"] = np.stack([load_img(env, f"sem_{c}", i) for c in self.cams])
         if self.brake:
-            h["tel"] = load_img(env, "tel_rgb", i)[:-self.crop_tel_bottom]
             h["bra"] = int(_frame(env, "bra", i, np.uint8)[0])
         return h
 
@@ -690,17 +734,7 @@ class CameraDataset:
         """the prepared frames ``hs`` stacked into one host buffer per key (pinned on a CUDA dataset): rgbs (B, ncam, h, w, 3),
         labels (B, ncam, h, w), tel (B, h_tel, w_tel, 3) uint8, bra (B,) int64."""
         pin = self.device.type == "cuda"
-        st = {}
-        for key in ("rgbs", "labels", "tel"):
-            if key in hs[0]:
-                shapes = {h[key].shape for h in hs}
-                if len(shapes) != 1:
-                    raise LavbError(f"CameraDataset: the {key} images of a batch differ in size: {sorted(shapes)}")
-                buf = torch.empty((len(hs),) + hs[0][key].shape, dtype=torch.uint8, pin_memory=pin)
-                dst = buf.numpy()
-                for b, h in enumerate(hs):
-                    dst[b] = h[key]
-                st[key] = buf
+        st = stage_images(hs, ("rgbs", "labels", "tel"), pin, "CameraDataset")
         if self.brake:
             bra = torch.tensor([h["bra"] for h in hs], dtype=torch.int64)
             st["bra"] = bra.pin_memory() if pin else bra

@@ -4,7 +4,7 @@ against the expert's future — as numbers over every sample of the recording, t
 
     python -m lav_b200.evaluate --config-path config_v2.yaml --data-dir VALDIR --lidar-weights lidar_7.th \
         --uniplanner-weights uniplanner_7.th [--batch-size 32] [--precision f16|fp32] [--num-workers 16] [--json out.json] \
-        [--forecast] [--forecast-detected] [--plan-safety] [--det-boxes]
+        [--forecast] [--forecast-detected] [--plan-safety] [--det-boxes] [--brake --bra-weights bra.th [--agent-config AGENT.yaml]]
     python -m lav_b200.evaluate ... --lidar-weights lidar_8.th lidar_16.th --uniplanner-weights uniplanner_8.th uniplanner_16.th
     python -m lav_b200.evaluate ... --run-dir RUN [--epochs 1,8,16-64]
     torchrun --nproc-per-node N -m lav_b200.evaluate ...
@@ -152,6 +152,40 @@ packed peaks and the actor table eval_batch reads, and one copy of its result bu
     translation_m, scale, heading_rad and flipped_rate (the share with a heading error > pi / 2); the same errors per range band
     of the actor's distance, [0, 10), [10, 20) and [20, 30) m.  Heading means skip a non-finite heading error.  A mean over no
     row, and recall and AP with n_gt = 0, are null.
+
+With --brake --bra-weights PATH (``brake=True, bra_model=...``) the result also holds ``brake``: the agent's brake-or-drive
+decision (lav_agent_fast.run_step) against the recorded brake flag bra, and each of its three rules on its own.  The decision is
+the verdict of the agent's own kernel (lavb_agent_control, control.AgentController's launch); nothing restates it.  The loader
+also reads the brake model's camera images (TemporalBatchLoader ``cameras``).  Per batch: one brake-model call for all
+checkpoints, then per checkpoint two ops.agent_control launches and one copy of their (B, 3) int32 result.  The protocol:
+
+  Brake model.  agent.brake_model's private copy of bra_model at ``precision`` (the agent's), called through agent.brake_probs
+    on the batch's camera bytes: the three middle cameras of camera_yaws side by side and tel_rgb[:-crop_tel_bottom], decoded by
+    datasets.load_img (what datasets.CameraDataset reads for evaluate_rgb).  One call per batch, shared by every checkpoint.
+  Controls.  ops.agent_control on forward_batch's ego_plan_locs and ego_cast_locs (commands 4 and 5 take the cast in the kernel,
+    as in the agent), the brake probabilities, the recorded commands, speeds of 0 and a freshly zeroed controller state per
+    launch; the agent's YAML (``agent_config``, --agent-config; default the dataset's config) gives the CONTROLLER keys,
+    cmd_thresh and pixels_per_meter (control.control_config).  Rows of the first launch: forward_batch's other_cast_locs /
+    other_cast_cmds, the forecasts the agent makes for the vehicles it detects.  Rows of the second (expert_track_rows): the
+    recorded futures of the sample's tracked vehicles, label slots 1 <= a < num_objs with typ 1, branch 0 = locs[f, a, 1:] -
+    ego_locs[f, 0] (the ego frame of other_cast_locs, as in the --forecast-detected protocol) with score 1, every other branch
+    NaN with score 0, so it never collides; built on the device from the batch's label tensors.  The labels are capped at
+    max_objs, and pedestrians are not rows: the agent forecasts vehicles only.
+  Speed.  Speed enters only the throttle, the speed cap and the creep, none of which is scored; with speed 0 and a fresh state
+    the stop counter is 1, far below the 600 ticks that start the creep, so the brake output is exactly the three rules.
+  Verdicts per sample.  agent: the control's brake output is 1; brake_model: LAVB_CTL_BRAKE_MODEL (pred_bra > 0.1); plan_stop:
+    LAVB_CTL_PID_BRAKE (pid_control's desired speed below brake_speed * ppm; never set on a plan with a NaN, which skips the PID
+    step); collide: LAVB_CTL_COLLIDE of the first launch (plan_collide on the detected vehicles' forecasts); collide_expert_tracks:
+    LAVB_CTL_COLLIDE of the second (the collision rule with perfect detection and forecasts: its difference from collide is the
+    perception and forecast error, not the rule).
+  Host reduction (BrakeScores), against the recorded bra (positive when non-zero): per verdict tp, fp, fn, tn, precision =
+    tp / (tp + fp), recall = tp / (tp + fn), false_brake_rate = fp / (fp + tn) (the agent brakes, the expert drives: phantom
+    braking), missed_brake_rate = fn / (tp + fn) (the expert brakes, the agent drives on); the same per recorded command, for
+    every command 0 .. C - 1 the planner has; samples, positives, invalid_plans (LAVB_CTL_PLAN_INVALID); by_reason: for every
+    combination of the three rules that fired alone together (brake_model, plan_stop, collide, their pairs and all three) the
+    agent brakes it triggered and how many of them were false.  A rate over no sample is null.
+  Not scored: the throttle, the steer, the speed cap and the creep (they depend on the speed, which the recording holds only as
+    the expert's).
 """
 import argparse
 import json
@@ -160,8 +194,9 @@ import numpy as np
 import torch
 
 from . import ops
-from .agent import infer_model, math_mode
+from .agent import brake_model, brake_probs, infer_model, math_mode
 from .capi import LavbError
+from .control import FLAG_BRAKE_MODEL, FLAG_COLLIDE, FLAG_PID_BRAKE, FLAG_PLAN_INVALID, control_config
 from .datasets import TemporalBatchLoader, TemporalLiDARPaintedDataset
 from .eval_sweep import (ResidentMeter, add_checkpoint_args, check_sweep_fits, eval_device, gather_merged, init_ranks,
                          rank_and_world, select_checkpoints, sweep_json, sweep_table)
@@ -508,27 +543,161 @@ def format_plan_safety(s):
     return lines
 
 
+BRAKE_VERDICTS = ("agent", "brake_model", "plan_stop", "collide", "collide_expert_tracks")
+BRAKE_REASONS = (("brake_model", FLAG_BRAKE_MODEL), ("plan_stop", FLAG_PID_BRAKE), ("collide", FLAG_COLLIDE))
+
+
+def expert_track_rows(locs, ego_locs, typs, num_objs, num_cmds):
+    """The recorded futures of a batch's tracked vehicles as forecast rows of ops.agent_control, built on the device of the label
+    tensors locs (B, M, T+1, 2), ego_locs (B, T+1, 2) and typs (B, M) from num_objs (B,) with no host loop.  Every label slot
+    1 .. M - 1 of a sample is a row, sample b owning rows [b (M - 1), (b + 1)(M - 1)); a slot a < num_objs[b] with typs[b, a] ==
+    1 has branch 0 = locs[b, a, 1:] - ego_locs[b, 0] with score 1, and every other branch, and every branch of any other slot,
+    NaN points with score 0, which never collide.  -> (rows (B (M - 1), num_cmds, T, 2) fp32, scores (B (M - 1), num_cmds) fp32,
+    offsets (B + 1,) int32 on the host)."""
+    B, M = typs.shape
+    dev = locs.device
+    n = torch.as_tensor(num_objs).to(dev).reshape(B, 1)
+    live = (typs[:, 1:] == 1) & (torch.arange(1, M, device=dev)[None] < n)                   # (B, M - 1)
+    track = (locs[:, 1:, 1:] - ego_locs[:, None, :1]).float()                                  # (B, M - 1, T, 2)
+    T = track.shape[2]
+    rows = torch.full((B, M - 1, num_cmds, T, 2), float("nan"), device=dev)
+    rows[:, :, 0] = torch.where(live[..., None, None], track, rows[:, :, 0])
+    scores = torch.zeros((B, M - 1, num_cmds), device=dev)
+    scores[:, :, 0] = live.float()
+    return rows.reshape(-1, num_cmds, T, 2), scores.reshape(-1, num_cmds), np.arange(B + 1, dtype=np.int32) * (M - 1)
+
+
+def score_brake(out, pred_bra, expert, cmds, config):
+    """The agent's brake decision on one batch: two ops.agent_control launches on forward_batch's ``out`` and the brake
+    probabilities ``pred_bra`` (B,), each from a freshly zeroed controller state, with speeds 0 and the recorded commands
+    ``cmds`` (B,) on the host; the first with the detected vehicles' forecasts as rows, the second with ``expert`` (the
+    expert_track_rows triple).  ``config`` is a capi.ControlConfig.  -> (B, 3) int32 on the device: the flags, the flags on the
+    recorded tracks, and the agent's brake (control[:, 2] == 1)."""
+    plan, cast = out["ego_plan_locs"].float().contiguous(), out["ego_cast_locs"].float().contiguous()
+    B, dev = plan.shape[0], plan.device
+    offsets = np.concatenate([[0], np.cumsum([len(o) for o in out["other_cast_locs"]])]).astype(np.int32)
+    detected = (torch.cat(list(out["other_cast_locs"])).float().contiguous(),
+                torch.cat(list(out["other_cast_cmds"])).float().contiguous(), offsets)
+    speed = torch.zeros(B, device=dev)
+    pred = pred_bra.reshape(B).float().contiguous()
+    record = ops.agent_control_state_bytes(config.turn_n, config.speed_n)
+    controls, flags = [], []
+    for rows, scores, offs in (detected, expert):
+        state = torch.zeros(B * record, dtype=torch.uint8, device=dev)
+        control, f = ops.agent_control(plan, cast, rows, scores, offs, pred, speed, cmds, config, state)
+        controls.append(control)
+        flags.append(f)
+    return torch.stack([flags[0], flags[1], (controls[0][:, 2] == 1).to(torch.int32)], 1)
+
+
+def brake_verdicts(res):
+    """the (n, 5) bool verdicts of BRAKE_VERDICTS of score_brake results ``res`` (n, 3) on the host."""
+    res = np.asarray(res).reshape(-1, 3)
+    f, fe = res[:, 0], res[:, 1]
+    return np.stack([res[:, 2] != 0, (f & FLAG_BRAKE_MODEL) != 0, (f & FLAG_PID_BRAKE) != 0, (f & FLAG_COLLIDE) != 0,
+                     (fe & FLAG_COLLIDE) != 0], 1)
+
+
+def brake_table(fire, y):
+    """the counts and rates of brake verdicts ``fire`` (n,) against the recorded brakes ``y`` (n,), both bool."""
+    tp, fp = int((fire & y).sum()), int((fire & ~y).sum())
+    fn, tn = int((~fire & y).sum()), int((~fire & ~y).sum())
+    div = lambda a, b: a / b if b else None
+    return dict(tp=tp, fp=fp, fn=fn, tn=tn, precision=div(tp, tp + fp), recall=div(tp, tp + fn), false_brake_rate=div(fp, fp + tn),
+                missed_brake_rate=div(fn, tp + fn))
+
+
+class BrakeScores:
+    """host accumulation of score_brake results over a recording, for a planner of ``num_cmds`` command branches."""
+
+    def __init__(self, num_cmds=6):
+        self.num_cmds = num_cmds
+        self.res, self.cmd, self.bra = [], [], []
+
+    def add(self, res, cmds, bras):
+        """res (B, 3) int32, a host copy of one batch's score_brake result; cmds (B,) the recorded commands; bras (B,) the
+        recorded brake flags."""
+        self.res.append(np.asarray(res, np.int32).reshape(-1, 3).copy())
+        self.cmd.append(np.asarray(cmds, np.int64).reshape(-1))
+        self.bra.append(np.asarray(bras, np.int64).reshape(-1))
+
+    def extend(self, other):
+        """append the records of ``other``, which follow this one's in sample order."""
+        self.res += other.res
+        self.cmd += other.cmd
+        self.bra += other.bra
+
+    def summary(self):
+        res = np.concatenate(self.res) if self.res else np.zeros((0, 3), np.int32)
+        cmd = np.concatenate(self.cmd) if self.cmd else np.zeros(0, np.int64)
+        y = (np.concatenate(self.bra) if self.bra else np.zeros(0, np.int64)) != 0
+        v = brake_verdicts(res)
+        tables = lambda m: {name: brake_table(v[m, j], y[m]) for j, name in enumerate(BRAKE_VERDICTS)}
+        cmds = sorted(set(range(self.num_cmds)) | set(cmd.tolist()))
+        agent = v[:, 0]
+        fired = np.stack([(res[:, 0] & bit) != 0 for _, bit in BRAKE_REASONS], 1)
+        by_reason = {}
+        for mask in range(1, 1 << len(BRAKE_REASONS)):
+            want = np.array([(mask >> k) & 1 for k in range(len(BRAKE_REASONS))], bool)
+            hit = agent & (fired == want[None]).all(1)
+            by_reason["+".join(n for (n, _), w in zip(BRAKE_REASONS, want) if w)] = dict(brakes=int(hit.sum()),
+                                                                                          false_brakes=int((hit & ~y).sum()))
+        return dict(samples=len(res), positives=int(y.sum()), invalid_plans=int(((res[:, 0] & FLAG_PLAN_INVALID) != 0).sum()),
+                    verdicts=tables(np.ones(len(res), bool)), per_cmd={str(c): dict(samples=int((cmd == c).sum()), verdicts=tables(cmd == c))
+                                                                      for c in cmds},
+                    by_reason=by_reason)
+
+
+def format_brake(b):
+    """the printout lines of a BrakeScores summary."""
+    fmt = lambda v: "n/a" if v is None else f"{v:.4f}"
+    line = lambda d: (f"tp {d['tp']} fp {d['fp']} fn {d['fn']} tn {d['tn']}, precision {fmt(d['precision'])}, recall "
+                      f"{fmt(d['recall'])}, false brake rate {fmt(d['false_brake_rate'])}, missed brake rate "
+                      f"{fmt(d['missed_brake_rate'])}")
+    lines = [f"brake decision ({b['samples']} samples, {b['positives']} recorded brakes, {b['invalid_plans']} invalid plans):"]
+    lines += [f"  {name}: " + line(d) for name, d in b["verdicts"].items()]
+    lines += [f"  cmd {c} ({d['samples']} samples), agent: " + line(d["verdicts"]["agent"]) for c, d in b["per_cmd"].items()]
+    lines.append("  agent brakes by the rules that fired: " +
+                 ", ".join(f"{k} {d['brakes']} ({d['false_brakes']} false)" for k, d in b["by_reason"].items()))
+    return lines
+
+
 def evaluate(lidar_model, uniplanner, dataset, batch_size=32, precision="f16", num_workers=16, forecast=False,
-             forecast_detected=False, plan_safety=False, det_boxes=False):
+             forecast_detected=False, plan_safety=False, det_boxes=False, brake=False, bra_model=None, agent_config=None):
     """Scores of ``lidar_model`` and ``uniplanner`` over every sample of ``dataset`` (a TemporalLiDARPaintedDataset), the models
     run as the agent runs them at ``precision``; with ``forecast`` also the UniPlanner's forecast scores on the recorded poses,
     with ``forecast_detected`` those on the detected vehicles, with ``plan_safety`` the collision and off-road rates of the ego
-    plan and of the expert, with ``det_boxes`` the detections' box scores.  -> dict (see the module docstring); None on a rank other than 0 of a process group."""
+    plan and of the expert, with ``det_boxes`` the detections' box scores, with ``brake`` the agent's brake decision with the
+    brake model ``bra_model`` under the controls of ``agent_config`` (the agent's YAML dict; default the dataset's config).
+    -> dict (see the module docstring); None on a rank other than 0 of a process group."""
     results = evaluate_checkpoints([(lidar_model, uniplanner)], dataset, batch_size, precision, num_workers, forecast,
-                                   forecast_detected, plan_safety, det_boxes)
+                                   forecast_detected, plan_safety, det_boxes, brake, bra_model, agent_config)
     return None if results is None else results[0]
 
 
 @torch.no_grad()
 def evaluate_checkpoints(pairs, dataset, batch_size=32, precision="f16", num_workers=16, forecast=False, forecast_detected=False,
-                         plan_safety=False, det_boxes=False):
+                         plan_safety=False, det_boxes=False, brake=False, bra_model=None, agent_config=None):
     """evaluate() of every (lidar_model, uniplanner) of ``pairs`` in one pass over ``dataset``: each batch is loaded and staged
     once, then every pair runs its own InferModel and scoring launches on it into its own accumulators.  All pairs stay
-    resident; a sweep that would not fit on the device is refused before any data is loaded.  In a process group each rank
-    scores its contiguous shard of the recording and rank 0 merges the ranks' records (eval_sweep.gather_merged).  -> one
-    evaluate() result per pair on rank 0, None on the other ranks."""
+    resident; a sweep that would not fit on the device is refused before any data is loaded.  With ``brake`` the one brake
+    model ``bra_model`` is resident once, before the pairs are measured, and runs once per batch for all pairs.  In a process
+    group each rank scores its contiguous shard of the recording and rank 0 merges the ranks' records
+    (eval_sweep.gather_merged).  -> one evaluate() result per pair on rank 0, None on the other ranks."""
     dev = dataset.device
     rank, world = rank_and_world()
+    bra = ctl = None
+    if brake:
+        if bra_model is None or not pairs:
+            raise LavbError("evaluate: brake=True needs the brake model (bra_model) and a checkpoint")
+        num_cmds = pairs[0][1].num_cmds
+        agent_config = dataset.cfg if agent_config is None else agent_config
+        aim = agent_config.get("aim_point")
+        if not isinstance(aim, (list, tuple)) or len(aim) != num_cmds:       # config_v2.yaml's aim_point is the trainer's scalar
+            raise LavbError(f"evaluate: brake needs the agent's config, whose aim_point has one entry per command of the planner "
+                            f"({num_cmds}); this one has {aim!r} (--agent-config)")
+        ctl = control_config(agent_config)
+        bra = brake_model(bra_model.to(dev).eval(), precision)
     models = []
     for i, (lid, uni) in enumerate(pairs):
         meter = ResidentMeter(dev, lid, uni) if i == 0 and len(pairs) > 1 else None
@@ -540,22 +709,28 @@ def evaluate_checkpoints(pairs, dataset, batch_size=32, precision="f16", num_wor
     grid = dict(min_x=dataset.min_x, max_x=dataset.max_x, min_y=dataset.min_y, max_y=dataset.max_y,
                 pixels_per_meter=dataset.pixels_per_meter)
     loader = TemporalBatchLoader(dataset, batch_size, rank=rank, world=world, drop_last=False, num_workers=num_workers, ordered=True,
-                                 plan_safety=plan_safety)
-    accs = [(Scores(), ForecastScores(), DetectedForecastScores(), PlanSafetyScores(), DetBoxScores()) for _ in models]
+                                 plan_safety=plan_safety, cameras=brake)
+    accs = [(Scores(), ForecastScores(), DetectedForecastScores(), PlanSafetyScores(), DetBoxScores(), BrakeScores(uni.num_cmds))
+            for _, uni in pairs]
     with math_mode(precision):
         for batch, staged in loader.staged_batches():
             actors = staged["actors"].to(dev, non_blocking=True)
+            brake_in = None
+            if brake:
+                cams = staged["cameras"]
+                pred_bra = brake_probs(bra, cams["rgbs"].to(dev, non_blocking=True), cams["tel"].to(dev, non_blocking=True))
+                brake_in = (pred_bra, expert_track_rows(batch[10], batch[6], batch[12], batch[13], num_cmds), ctl)
             for im, acc in zip(models, accs):
-                score_batch(im, batch, staged, actors, grid, acc, forecast, forecast_detected, plan_safety, det_boxes)
+                score_batch(im, batch, staged, actors, grid, acc, forecast, forecast_detected, plan_safety, det_boxes, brake_in)
     accs = gather_merged(accs)
     if accs is None:
         return None
-    return [summarize(acc, precision, forecast, forecast_detected, plan_safety, dataset.num_plan, det_boxes) for acc in accs]
+    return [summarize(acc, precision, forecast, forecast_detected, plan_safety, dataset.num_plan, det_boxes, brake) for acc in accs]
 
 
-def summarize(acc, precision, forecast, forecast_detected, plan_safety, num_plan, det_boxes=False):
+def summarize(acc, precision, forecast, forecast_detected, plan_safety, num_plan, det_boxes=False, brake=False):
     """the evaluate() result of one checkpoint's accumulators ``acc`` (score_batch's tuple; its DetBoxScores is read only with
-    ``det_boxes``)."""
+    ``det_boxes``, its BrakeScores only with ``brake``)."""
     scores, forecasts, detected, safety = acc[:4]
     result = scores.summary()
     result["precision"] = precision
@@ -567,13 +742,16 @@ def summarize(acc, precision, forecast, forecast_detected, plan_safety, num_plan
         result["plan_safety"] = safety.summary(num_plan)
     if det_boxes:
         result["det_boxes"] = acc[4].summary()
+    if brake:
+        result["brake"] = acc[5].summary()
     return result
 
 
-def score_batch(im, batch, staged, actors, grid, acc, forecast, forecast_detected, plan_safety, det_boxes=False):
+def score_batch(im, batch, staged, actors, grid, acc, forecast, forecast_detected, plan_safety, det_boxes=False, brake=None):
     """one checkpoint's InferModel ``im`` on one loader batch (its 14-tuple, staged tables and the actor table on the device),
-    scored into ``acc`` = (Scores, ForecastScores, DetectedForecastScores, PlanSafetyScores, DetBoxScores); the last is used
-    only with ``det_boxes``."""
+    scored into ``acc`` = (Scores, ForecastScores, DetectedForecastScores, PlanSafetyScores, DetBoxScores, BrakeScores); the
+    DetBoxScores is used only with ``det_boxes``, the BrakeScores only with ``brake`` = (the batch's brake probabilities, its
+    expert_track_rows, the capi.ControlConfig)."""
     scores, forecasts, detected, safety = acc[:4]
     dev = actors.device
     lidars, num_points, bev, ego_locs, cmds, nxps = batch[0], batch[1], batch[5], batch[6], batch[7], batch[8]
@@ -597,6 +775,10 @@ def score_batch(im, batch, staged, actors, grid, acc, forecast, forecast_detecte
     if det_boxes:
         res = ops.det_box_eval(out["packed"], actors, staged["offsets"], grid)
         acc[4].add(ops.det_box_views(res.cpu(), len(num_points), out["packed"].shape[2]))
+    if brake is not None:
+        pred_bra, expert, ctl = brake
+        res = score_brake(out, pred_bra, expert, host_cmds.astype(np.int32), ctl)
+        acc[5].add(res.cpu().numpy(), host_cmds, staged["labels"]["bra"].numpy())
 
 
 def parse_args(argv=None):
@@ -616,7 +798,16 @@ def parse_args(argv=None):
                     help="also score the ego plan and the expert for collisions with the recorded traffic and for leaving the road")
     ap.add_argument("--det-boxes", action="store_true",
                     help="also score the detections as rotated boxes: IoU AP and the position, size and heading errors of the 2 m matches")
-    return ap.parse_args(argv)
+    ap.add_argument("--brake", action="store_true",
+                    help="also score the agent's brake decision (brake model, plan stop, collision brake) against the recorded brake flag")
+    ap.add_argument("--bra-weights", default=None, help="with --brake: the RGBBrakePredictionModel state_dict (bra_v2_9.th)")
+    ap.add_argument("--agent-config", default=None,
+                    help="with --brake: the agent's YAML (team_code_v2/config.yaml), for its CONTROLLER keys, cmd_thresh and "
+                         "pixels_per_meter (default: --config-path)")
+    args = ap.parse_args(argv)
+    if args.brake and args.bra_weights is None:
+        ap.error("--brake needs --bra-weights")
+    return args
 
 
 def format_result(r):
@@ -640,6 +831,8 @@ def format_result(r):
         lines += format_plan_safety(r["plan_safety"])
     if "det_boxes" in r:
         lines += format_det_boxes(r["det_boxes"])
+    if "brake" in r:
+        lines += format_brake(r["brake"])
     return "\n".join(lines)
 
 
@@ -657,6 +850,9 @@ def headline(r):
     if "det_boxes" in r:
         veh = r["det_boxes"]["vehicle"]
         cols += [("veh AP@IoU.5", veh["ap_iou"]["0.5"]), ("veh heading", veh["heading_rad"])]
+    if "brake" in r:
+        agent = r["brake"]["verdicts"]["agent"]
+        cols += [("false brake", agent["false_brake_rate"]), ("missed brake", agent["missed_brake_rate"])]
     return cols
 
 
@@ -689,9 +885,17 @@ def main(argv=None):
         lid.load_state_dict(torch.load(paths["lidar"], map_location="cpu"))
         uni.load_state_dict(torch.load(paths["uniplanner"], map_location="cpu"))
         pairs.append((lid, uni))
+    bra = agent_cfg = None
+    if args.brake:
+        from .heads import RGBBrakePredictionModel
+        bra = RGBBrakePredictionModel(cfg["seg_channels"])
+        bra.load_state_dict(torch.load(args.bra_weights, map_location="cpu"))
+        if args.agent_config is not None:
+            with open(args.agent_config) as f:
+                agent_cfg = yaml.safe_load(f)
     ds = TemporalLiDARPaintedDataset(args.config_path, device=dev, overrides=dict(data_dir=args.data_dir))
     results = evaluate_checkpoints(pairs, ds, args.batch_size, args.precision, args.num_workers, args.forecast,
-                                   args.forecast_detected, args.plan_safety, args.det_boxes)
+                                   args.forecast_detected, args.plan_safety, args.det_boxes, args.brake, bra, agent_cfg)
     out = None
     if results is not None:
         text, out = report(checkpoints, results, rank_and_world()[1])
