@@ -728,17 +728,30 @@ int lavb_det_peaks(const float* d_center, const float* d_box, const float* d_ori
  * [k][crop][crop][c] in the feature dtype.  d_frame_idx: int32 [k]; d_theta: fp32 [k][2][3].
  * dtype LAVB_F32 (c a positive multiple of 4) or the library's 16-bit type (c a positive multiple of 8): a thread moves
  * 16 bytes of channels, so d_feat and d_out must be 16-byte aligned.  b, h, w >= 1 (maps one pixel wide or high included),
- * crop >= 2, 0 <= k <= 65535; k = 0 launches nothing and writes nothing.  Frame indices outside [0, b) are clamped to the
- * nearest frame.  Every element of d_out is written (zeros where a sample leaves the map).  Accumulation is fp32 in the same
- * fmaf order for both dtypes; the 16-bit output is the fp32 result rounded once to nearest. */
+ * 2 <= crop <= 65535, 0 <= k <= 65535; k = 0 launches nothing and writes nothing.  Frame indices outside [0, b) are clamped
+ * to the nearest frame.  Every element of d_out is written (zeros where a sample leaves the map).  Accumulation is fp32 in
+ * the same fmaf order for both dtypes; the 16-bit output is the fp32 result rounded once to nearest.
+ * Sample position of crop pixel (i, j), in fp32: x_i = torch.linspace(-1, 1, crop)[i] as start + step i for i < crop / 2
+ * and end - step (crop - 1 - i) after (one fmaf each, step = 2 / (crop - 1)), y_j likewise; gx = fmaf(t00, x_i, fmaf(t01,
+ * y_j, t02)), gy with t1.; ix = (gx + 1) * 0.5 * (w - 1), iy = (gy + 1) * 0.5 * (h - 1).  Taps at floor(ix), floor(iy) and
+ * +1 with the weights (1 - ax) (1 - ay), ax (1 - ay), (1 - ax) ay, ax ay, ax = ix - floor(ix), summed as fmaf(w, f, acc)
+ * in the order 00, 01, 10, 11 over the taps on the map.
+ * Non-finite and far positions: a sample with a NaN coordinate (a NaN theta, or inf * 0) is NaN in every channel, whatever
+ * its other coordinate; a sample with an infinite coordinate, or one past +-2^31, is off the map and gives 0.  The same
+ * rule holds for lavb_crop_bilinear_u8. */
 int lavb_crop_bilinear(const void* d_feat, int dtype, int b, int h, int w, int c, const int* d_frame_idx,
                        const float* d_theta, int k, int crop, void* d_out, void* stream);
 /* the same crop from a uint8 PLANAR map (the ground-truth BEV): d_map [b][c][h][w] uint8 -> d_out NCHW [k][c][crop][crop] fp32.
  * replaces: BEVPlanner.forward's `bev.float()`, `bev.expand(N,...).permute(...).contiguous()[typs]`, F.affine_grid and
  *           F.grid_sample (lav/models/bev_planner_v2.py:92,104,146,222-264).
- * Bit-identical to lavb_crop_bilinear (fp32) on the float copy of the map.  Frame indices outside [0, b) are clamped to the
- * nearest frame, as in lavb_crop_bilinear.  Every output element is written (zeros where a sample leaves the map).
- * c >= 1, crop >= 2, k <= 65535; no backward (the map is data). */
+ * Bit-identical to lavb_crop_bilinear (fp32) on the float copy of the map: the same sample positions, taps and fmaf order,
+ * and the same rule for non-finite and far positions (NaN coordinate: NaN in every channel; infinite or past +-2^31: 0).
+ * Frame indices outside [0, b) are clamped to the nearest frame, as in lavb_crop_bilinear.  Written: every element of
+ * d_out [k][c][crop][crop] (zeros where a sample leaves the map), nothing else.  No backward (the map is data).
+ * Checked before any launch (a rejected call writes nothing): c >= 1, 2 <= crop <= 65535 (a crop's grid of
+ * ceil(crop / 32) * ceil(crop / 8) blocks of 32 x 8 pixels then stays below 2^24), b, h, w >= 1, 0 <= k <= 65535 (0 writes
+ * nothing); otherwise non-null pointers, d_frame_idx / d_theta / d_out 4-byte aligned, and d_out not overlapping d_map,
+ * d_frame_idx or d_theta. */
 int lavb_crop_bilinear_u8(const uint8_t* d_map, int b, int c, int h, int w, const int* d_frame_idx, const float* d_theta,
                           int k, int crop, float* d_out, void* stream);
 /* gradient of lavb_crop_bilinear with respect to d_feat (fp32 NHWC; training, lav/models/uniplanner.py:56-151 through F.grid_sample):
@@ -861,7 +874,21 @@ int lavb_erf_nb16(const void* d_in, void* d_out, int n, int h, int w, const floa
  * for each of ncmd branches, nn.GRU(512, 64, batch_first=True) over the embedding repeated `steps` times, nn.Linear(64, 2) and the
  * cumulative sum over the steps — 6 x (GRU + Linear + cumsum) calls in the reference.  fp32 FFMA.
  * d_embd (n, 512); d_wih_t (ncmd, 512, 192) = weight_ih_l0 TRANSPOSED; d_whh_t (ncmd, 64, 192) = weight_hh_l0 transposed;
- * d_bih / d_bhh (ncmd, 192); d_wmlp (ncmd, 2, 64); d_bmlp (ncmd, 2); d_out (n, ncmd, steps, 2) fp32. */
+ * d_bih / d_bhh (ncmd, 192); d_wmlp (ncmd, 2, 64); d_bmlp (ncmd, 2); d_out (n, ncmd, steps, 2) fp32, all dense.
+ * Arithmetic, per row and branch, in fp32 (PyTorch's gate order r, z, n in the 192 columns; h starts at 0):
+ *   gi = b_ih + x . W_ih^T            (one fmaf chain over the 512 inputs in order, once: the input is the same every step)
+ *   gh = b_hh + h . W_hh^T            (one fmaf chain over the 64 hidden units in order, every step)
+ *   r = sigmoid(gi_r + gh_r), z = sigmoid(gi_z + gh_z), sigmoid(v) = 1 / (1 + expf(-v));
+ *   n = tanhf(fmaf(r, gh_n, gi_n))    (b_hn inside the reset gate, as nn.GRU);  h' = fmaf(z, h - n, n) = (1 - z) n + z h;
+ *   loc_t = loc_(t-1) + (b_mlp + W_mlp . h'), the Linear an fmaf chain over the 64 units from the bias; d_out[., ., t] = loc_t
+ *   (the cumsum is inclusive: step 0 holds the first increment).
+ * NaN / inf: a NaN anywhere in a row's embedding makes every output of that row NaN.  An infinite embedding element makes
+ * that row's input projections infinite, and the formula then runs in IEEE arithmetic: sigmoid(+-inf) = 1 / 0 and
+ * tanh(+-inf) = +-1 exactly, so the gates saturate and the outputs stay finite (unless a weight of that element is 0:
+ * inf * 0 = NaN).  Rows are independent: a row's outputs never depend on the other rows.
+ * Written: d_out rows 0..n-1, every element; nothing else (the padding rows of the last 16-row block write nothing).
+ * Checked before any launch (a rejected call writes nothing): n >= 0 (0 writes nothing), 1 <= ncmd <= 65535, steps >= 1;
+ * otherwise non-null pointers, every pointer 4-byte aligned, and d_out not overlapping any of the seven inputs. */
 int lavb_cast_gru(const float* d_embd, int n, const float* d_wih_t, const float* d_whh_t, const float* d_bih, const float* d_bhh,
                   const float* d_wmlp, const float* d_bmlp, int ncmd, int steps, float* d_out, void* stream);
 

@@ -110,8 +110,19 @@ using namespace lavb;
 extern "C" int lavb_cast_gru(const float* d_embd, int n, const float* d_wih_t, const float* d_whh_t, const float* d_bih,
                              const float* d_bhh, const float* d_wmlp, const float* d_bmlp, int ncmd, int steps, float* d_out,
                              void* stream) {
-  LAVB_CHECK_ARG(n >= 0 && ncmd >= 1 && ncmd <= 65535 && steps >= 1, "cast_gru: bad shape");
+  LAVB_CHECK_ARG(n >= 0 && ncmd >= 1 && ncmd <= 65535 && steps >= 1, "cast_gru: bad shape (n %d, ncmd %d, steps %d)", n, ncmd, steps);
   if (n == 0) return 0;
+  const float* ins[7] = {d_embd, d_wih_t, d_whh_t, d_bih, d_bhh, d_wmlp, d_bmlp};
+  const size_t in_floats[7] = {(size_t)n * kCgIn, (size_t)ncmd * kCgIn * kCgCols, (size_t)ncmd * kCgH * kCgCols, (size_t)ncmd * kCgCols,
+                               (size_t)ncmd * kCgCols, (size_t)ncmd * 2 * kCgH, (size_t)ncmd * 2};
+  LAVB_CHECK_ARG(d_out != nullptr, "cast_gru: null pointer (out)");
+  LAVB_CHECK_ARG(is_aligned(d_out, 4), "cast_gru: out must be 4-byte aligned");
+  const size_t out_bytes = (size_t)n * ncmd * steps * 2 * sizeof(float);
+  for (int a = 0; a < 7; ++a) {
+    LAVB_CHECK_ARG(ins[a] != nullptr, "cast_gru: null pointer (input %d)", a);
+    LAVB_CHECK_ARG(is_aligned(ins[a], 4), "cast_gru: input %d must be 4-byte aligned", a);
+    LAVB_CHECK_ARG(!ranges_overlap(d_out, out_bytes, ins[a], in_floats[a] * sizeof(float)), "cast_gru: out overlaps input %d", a);
+  }
   LAVB_CUDA_OK(ensure_dyn_smem((const void*)cast_gru_kernel, (int)sizeof(CastSmem)));
   const dim3 grid(ceil_div(n, kCgSeq), ncmd);
   cast_gru_kernel<<<grid, kCgCols, sizeof(CastSmem), (cudaStream_t)stream>>>(d_embd, n, d_wih_t, d_whh_t, d_bih, d_bhh, d_wmlp, d_bmlp, ncmd,

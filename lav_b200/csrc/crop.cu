@@ -50,6 +50,29 @@ __device__ __forceinline__ void crop_sample_pos(int i, int j, int S, const float
   iy = (gy + 1.f) * 0.5f * (float)(H - 1);
 }
 
+// the four bilinear taps of sample position (ix, iy) on an H x W map, shared by both forward kernels so that they agree on
+// every position.  x0 = floor(ix) through the saturating conversion (a position past +-2^31 or infinite gives INT_MAX / INT_MIN)
+// and the on-map tests never form x0 + 1, so no int overflows.  A NaN coordinate reads pixel (0, 0) with its NaN weights, so
+// every channel of the sample is NaN, whatever the other coordinate; a tap off the map is skipped (zero padding).
+struct CropTaps {
+  int x0, y0;
+  float w00, w01, w10, w11;
+  bool v00, v01, v10, v11;
+};
+
+__device__ __forceinline__ CropTaps crop_taps(float ix, float iy, int H, int W) {
+  CropTaps t;
+  const bool nan = isnan(ix) || isnan(iy);
+  t.x0 = nan ? 0 : __float2int_rd(ix);
+  t.y0 = nan ? 0 : __float2int_rd(iy);
+  const float ax = ix - floorf(ix), ay = iy - floorf(iy);
+  t.w00 = (1.f - ax) * (1.f - ay); t.w01 = ax * (1.f - ay); t.w10 = (1.f - ax) * ay; t.w11 = ax * ay;
+  const bool vx0 = t.x0 >= 0 && t.x0 < W, vx1 = t.x0 >= -1 && t.x0 < W - 1;
+  const bool vy0 = t.y0 >= 0 && t.y0 < H, vy1 = t.y0 >= -1 && t.y0 < H - 1;
+  t.v00 = vx0 && vy0; t.v01 = vx1 && vy0; t.v10 = vx0 && vy1; t.v11 = vx1 && vy1;
+  return t;
+}
+
 // block = one 8x8 patch of output pixels x one 64 B channel slice (4 threads of 16 B per pixel): neighbouring output
 // pixels sample overlapping 2x2 input neighbourhoods, so a compact patch lets L1 serve the ~4x re-reads that a row-major
 // pixel order sent to L2.  grid = (patches per crop, channel slices, crops).
@@ -70,14 +93,10 @@ __global__ void __launch_bounds__(256) crop_kernel(const T* __restrict__ feat, i
   for (int e = 0; e < 6; ++e) th[e] = __ldg(theta + k * 6 + e);
   float ix, iy;
   crop_sample_pos(i, j, S, th, H, W, ix, iy);
-  const float fx = floorf(ix), fy = floorf(iy);
-  const int x0 = (int)fx, y0 = (int)fy;
-  const float ax = ix - fx, ay = iy - fy;
-  const float w00 = (1.f - ax) * (1.f - ay), w01 = ax * (1.f - ay), w10 = (1.f - ax) * ay, w11 = ax * ay;
-  const bool vx0 = x0 >= 0 && x0 < W, vx1 = x0 + 1 >= 0 && x0 + 1 < W, vy0 = y0 >= 0 && y0 < H, vy1 = y0 + 1 >= 0 && y0 + 1 < H;
+  const CropTaps tp = crop_taps(ix, iy, H, W);
   int b = __ldg(frame_idx + k);
   b = b < 0 ? 0 : (b >= B ? B - 1 : b);
-  const T* p00 = feat + (long long)b * H * W * C + ((long long)y0 * W + x0) * C + c;
+  const T* p00 = feat + (long long)b * H * W * C + ((long long)tp.y0 * W + tp.x0) * C + c;
   float acc[VEC];
 #pragma unroll
   for (int e = 0; e < VEC; ++e) acc[e] = 0.f;
@@ -88,8 +107,8 @@ __global__ void __launch_bounds__(256) crop_kernel(const T* __restrict__ feat, i
 #pragma unroll
     for (int e = 0; e < VEC; ++e) acc[e] = fmaf(wgt, v[e], acc[e]);
   };
-  add(p00, w00, vx0 && vy0); add(p00 + C, w01, vx1 && vy0);
-  add(p00 + (long long)W * C, w10, vx0 && vy1); add(p00 + (long long)W * C + C, w11, vx1 && vy1);
+  add(p00, tp.w00, tp.v00); add(p00 + C, tp.w01, tp.v01);
+  add(p00 + (long long)W * C, tp.w10, tp.v10); add(p00 + (long long)W * C + C, tp.w11, tp.v11);
   Vec16<T>::store(out + pix * C + c, acc);
 }
 
@@ -115,25 +134,20 @@ __global__ void __launch_bounds__(256) crop_u8_kernel(const uint8_t* __restrict_
   for (int e = 0; e < 6; ++e) th[e] = __ldg(theta + k * 6 + e);
   float ix, iy;
   crop_sample_pos(i, j, S, th, H, W, ix, iy);
-  const float fx = floorf(ix), fy = floorf(iy);
-  const int x0 = (int)fx, y0 = (int)fy;
-  const float ax = ix - fx, ay = iy - fy;
-  const float w00 = (1.f - ax) * (1.f - ay), w01 = ax * (1.f - ay), w10 = (1.f - ax) * ay, w11 = ax * ay;
-  const bool vx0 = x0 >= 0 && x0 < W, vx1 = x0 + 1 >= 0 && x0 + 1 < W, vy0 = y0 >= 0 && y0 < H, vy1 = y0 + 1 >= 0 && y0 + 1 < H;
-  const bool v00 = vx0 && vy0, v01 = vx1 && vy0, v10 = vx0 && vy1, v11 = vx1 && vy1;
+  const CropTaps tp = crop_taps(ix, iy, H, W);
   int b = __ldg(frame_idx + k);
   b = b < 0 ? 0 : (b >= B ? B - 1 : b);
   const long long plane = (long long)H * W;
-  // offsets of the taps inside a plane, formed only for taps that lie on the map
-  const long long o00 = (long long)y0 * W + x0;
+  // offset of tap 00 inside a plane; a tap is read only when it lies on the map
+  const long long o00 = (long long)tp.y0 * W + tp.x0;
   const uint8_t* src = map + (long long)b * C * plane;
   float* dst = out + (long long)k * C * S * S + (long long)j * S + i;
   for (int c = 0; c < C; ++c, src += plane, dst += (long long)S * S) {
     float acc = 0.f;
-    if (v00) acc = fmaf(w00, (float)__ldg(src + o00), acc);
-    if (v01) acc = fmaf(w01, (float)__ldg(src + o00 + 1), acc);
-    if (v10) acc = fmaf(w10, (float)__ldg(src + o00 + W), acc);
-    if (v11) acc = fmaf(w11, (float)__ldg(src + o00 + W + 1), acc);
+    if (tp.v00) acc = fmaf(tp.w00, (float)__ldg(src + o00), acc);
+    if (tp.v01) acc = fmaf(tp.w01, (float)__ldg(src + o00 + 1), acc);
+    if (tp.v10) acc = fmaf(tp.w10, (float)__ldg(src + o00 + W), acc);
+    if (tp.v11) acc = fmaf(tp.w11, (float)__ldg(src + o00 + W + 1), acc);
     *dst = acc;
   }
 }
@@ -296,7 +310,8 @@ extern "C" int lavb_crop_bilinear(const void* d_feat, int dtype, int b, int h, i
   LAVB_CHECK_ARG(dtype == LAVB_F32 || dtype == LAVB_H16, "crop_bilinear: bad dtype %d", dtype);
   const int vec = dtype == LAVB_F32 ? 4 : 8;       // channels per 16-byte vector
   LAVB_CHECK_ARG(c >= vec && c % vec == 0, "crop_bilinear: channels must be a positive multiple of %d (got %d)", vec, c);
-  LAVB_CHECK_ARG(crop >= 2 && b >= 1 && h >= 1 && w >= 1, "crop_bilinear: bad crop size / map (%d; %d x %d x %d)", crop, b, h, w);
+  LAVB_CHECK_ARG(crop >= 2 && crop <= 65535 && b >= 1 && h >= 1 && w >= 1, "crop_bilinear: bad crop size / map (%d; %d x %d x %d)", crop,
+                 b, h, w);
   LAVB_CHECK_ARG(k >= 0, "crop_bilinear: negative crop count");
   if (k == 0) return 0;
   LAVB_CHECK_ARG(k <= 65535, "crop_bilinear: at most 65535 crops per call");
@@ -318,11 +333,19 @@ extern "C" int lavb_crop_bilinear(const void* d_feat, int dtype, int b, int h, i
 extern "C" int lavb_crop_bilinear_u8(const uint8_t* d_map, int b, int c, int h, int w, const int* d_frame_idx, const float* d_theta,
                                      int k, int crop, float* d_out, void* stream) {
   LAVB_CHECK_ARG(c >= 1, "crop_bilinear_u8: need at least one channel (got %d)", c);
-  LAVB_CHECK_ARG(crop >= 2, "crop_bilinear_u8: crop size must be >= 2 (got %d)", crop);
+  LAVB_CHECK_ARG(crop >= 2 && crop <= 65535, "crop_bilinear_u8: crop size must be in [2, 65535] (got %d)", crop);
   LAVB_CHECK_ARG(b >= 1 && h >= 1 && w >= 1, "crop_bilinear_u8: empty map (%d x %d x %d)", b, h, w);
   LAVB_CHECK_ARG(k >= 0, "crop_bilinear_u8: negative crop count");
   if (k == 0) return 0;
   LAVB_CHECK_ARG(k <= 65535, "crop_bilinear_u8: at most 65535 crops per call");
+  LAVB_CHECK_ARG(d_map && d_frame_idx && d_theta && d_out, "crop_bilinear_u8: null pointer");
+  LAVB_CHECK_ARG(is_aligned(d_frame_idx, 4) && is_aligned(d_theta, 4) && is_aligned(d_out, 4),
+                 "crop_bilinear_u8: frame_idx, theta and out must be 4-byte aligned");
+  const size_t out_bytes = (size_t)k * c * crop * crop * sizeof(float);
+  LAVB_CHECK_ARG(!ranges_overlap(d_out, out_bytes, d_map, (size_t)b * c * h * w) &&
+                     !ranges_overlap(d_out, out_bytes, d_frame_idx, (size_t)k * sizeof(int)) &&
+                     !ranges_overlap(d_out, out_bytes, d_theta, (size_t)k * 6 * sizeof(float)),
+                 "crop_bilinear_u8: out overlaps map, frame_idx or theta");
   const dim3 blocks(((crop + 31) / 32) * ((crop + 7) / 8), k);
   crop_u8_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(d_map, b, c, h, w, d_frame_idx, d_theta, crop, d_out);
   LAVB_LAUNCH_OK();

@@ -80,6 +80,16 @@ def _out(what, name, out, dtype, shape, device):
     return out
 
 
+def _apart(what, name, out, **inputs):
+    """LavbError unless the bytes of ``out`` share none with those of each named input tensor (the kernels read their inputs
+    while they write out)."""
+    o0, o1 = out.data_ptr(), out.data_ptr() + out.numel() * out.element_size()
+    for k, t in inputs.items():
+        t0 = t.data_ptr()
+        _require(o0 == o1 or t.numel() == 0 or not (o0 < t0 + t.numel() * t.element_size() and t0 < o1),
+                 f"{what}: {name} must not overlap {k}")
+
+
 def _host(what, name, a, dtype, shape, cast=False):
     """a host array a kernel reads (numpy or a CPU tensor) -> it as contiguous numpy, converted to dtype with cast=True; raises
     LavbError unless it has dtype and shape (as _tensor's)."""
@@ -360,14 +370,19 @@ def crop_bilinear(feats_nhwc, frame_idx, theta, crop_size):
 def crop_bilinear_u8(bev_u8, frame_idx, theta, crop_size, out=None):
     """bev_u8 (B,C,H,W) contiguous uint8; frame_idx (K,) int32; theta (K,2,3) fp32 -> fp32 NCHW (K,C,crop,crop): the crops of
     crop_bilinear read straight from a uint8 planar map (bit-identical to crop_bilinear on its float copy).  Frame indices
-    outside [0, B) are clamped to the nearest frame.  ``out`` (K,C,crop,crop) fp32 contiguous is written in full if given."""
-    _need_cuda(frame_idx)
-    b, c, h, w = _tensor("crop_bilinear_u8", "bev_u8", bev_u8, torch.uint8, (None,) * 4)
-    k, _, _ = _tensor("crop_bilinear_u8", "theta", theta, None, (None, 2, 3), contiguous=False)
-    _require(frame_idx.numel() == k, f"crop_bilinear_u8: frame_idx {tuple(frame_idx.shape)} does not hold one frame per crop (K = {k})")
-    theta = theta.float().contiguous()
-    frame_idx = frame_idx.to(torch.int32).contiguous()
-    out = _out("crop_bilinear_u8", "out", out, torch.float32, (k, c, crop_size, crop_size), bev_u8.device)
+    outside [0, B) are clamped to the nearest frame.  ``out`` (K,C,crop,crop) fp32 contiguous is written in full if given; it
+    must not overlap the map or the poses."""
+    what = "crop_bilinear_u8"
+    b, c, h, w = _tensor(what, "bev_u8", bev_u8, torch.uint8, (None,) * 4)
+    dev = bev_u8.device
+    _tensor(what, "theta", theta, None, (None, 2, 3), dev, contiguous=False)
+    _tensor(what, "frame_idx", frame_idx, None, None, dev, contiguous=False)
+    _require(c >= 1 and h >= 1 and w >= 1 and b >= 1, f"{what}: bev_u8 must be a non-empty (B,C,H,W) map, got {tuple(bev_u8.shape)}")
+    _require(2 <= crop_size <= 65535, f"{what}: crop_size must be in [2, 65535], got {crop_size}")
+    k, frame_idx, theta = _crop_poses(what, frame_idx, theta, b)
+    _require(k <= 65535, f"{what}: at most 65535 crops per call, got {k}")
+    out = _out(what, "out", out, torch.float32, (k, c, crop_size, crop_size), dev)
+    _apart(what, "out", out, bev_u8=bev_u8, frame_idx=frame_idx, theta=theta)
     _launch("lavb_crop_bilinear_u8", _ptr(bev_u8), b, c, h, w, _ptr(frame_idx), _ptr(theta), k, crop_size, _ptr(out))
     return out
 
@@ -1178,15 +1193,20 @@ def erf_nb16(x, w4, st):
     return out
 
 
-def cast_gru(embd, wih_t, whh_t, bih, bhh, wmlp, bmlp, steps):
+def cast_gru(embd, wih_t, whh_t, bih, bhh, wmlp, bmlp, steps, out=None):
     """the 6 cast branches in one launch (csrc/cast_gru.cu).  embd (N, 512) fp32; wih_t (ncmd, 512, 192), whh_t (ncmd, 64, 192) the
-    TRANSPOSED GRU weights; bih / bhh (ncmd, 192); wmlp (ncmd, 2, 64); bmlp (ncmd, 2) -> (N, ncmd, steps, 2) fp32 cumulative waypoints."""
+    TRANSPOSED GRU weights; bih / bhh (ncmd, 192); wmlp (ncmd, 2, 64); bmlp (ncmd, 2) -> (N, ncmd, steps, 2) fp32 cumulative waypoints,
+    written into ``out`` (contiguous, not overlapping an input) when given."""
     n, _ = _tensor("cast_gru", "embd", embd, torch.float32, (None, 512))
-    ncmd, _, _ = _tensor("cast_gru", "wih_t", wih_t, torch.float32, (None, 512, 192))
-    for name, t, shape in (("whh_t", whh_t, (ncmd, 64, 192)), ("bih", bih, (ncmd, 192)), ("bhh", bhh, (ncmd, 192)),
-                           ("wmlp", wmlp, (ncmd, 2, 64)), ("bmlp", bmlp, (ncmd, 2))):
-        _tensor("cast_gru", name, t, torch.float32, shape)
-    out = torch.empty((n, ncmd, steps, 2), dtype=torch.float32, device=embd.device)
+    dev = embd.device
+    ncmd, _, _ = _tensor("cast_gru", "wih_t", wih_t, torch.float32, (None, 512, 192), dev)
+    ins = dict(embd=embd, wih_t=wih_t, whh_t=whh_t, bih=bih, bhh=bhh, wmlp=wmlp, bmlp=bmlp)
+    for name, shape in (("whh_t", (ncmd, 64, 192)), ("bih", (ncmd, 192)), ("bhh", (ncmd, 192)), ("wmlp", (ncmd, 2, 64)), ("bmlp", (ncmd, 2))):
+        _tensor("cast_gru", name, ins[name], torch.float32, shape, dev)
+    _require(1 <= ncmd <= 65535 and steps >= 1,
+             f"cast_gru: need 1 <= ncmd <= 65535 and steps >= 1, got ncmd {ncmd}, steps {steps}")
+    out = _out("cast_gru", "out", out, torch.float32, (n, ncmd, steps, 2), dev)
+    _apart("cast_gru", "out", out, **ins)
     _launch("lavb_cast_gru", _ptr(embd), n, _ptr(wih_t), _ptr(whh_t), _ptr(bih), _ptr(bhh), _ptr(wmlp), _ptr(bmlp), ncmd, steps, _ptr(out))
     return out
 

@@ -44,6 +44,11 @@ def _cases(dev):
     c33 = r(1, 8, 8, 64, dt=h)
     xp = r(1, 8, 32, 64, dt=h)
     gru = [r(2, 512), r(6, 512, 192), r(6, 64, 192), r(6, 192), r(6, 192), r(6, 2, 64), r(6, 2)]
+    e2 = r(2, 512)
+    bev8 = r(2, 3, 16, 16, dt=u8)
+    fi = torch.tensor([0, 1, 5], dtype=i32, device=dev)
+    th = (r(3, 2, 3) - 0.5).contiguous()
+    buf8 = z(3, 3, 8, 8)                                                      # an output whose first bytes are the poses
     dst7 = z(64, 7)
     job = np.zeros(1, ops.STACK_JOB_DTYPE)
     job[0] = (pts.data_ptr(), dst7.data_ptr(), 64, 0, np.eye(3, dtype=np.float32).ravel(), 0.0, 0.0, 0)   # pts: held by the cases
@@ -114,9 +119,18 @@ def _cases(dev):
          [dict(x=xp.float()), dict(x=nc(xp)), dict(x=xp.cpu()), dict(w1=r(3, 64, 32, dt=h)), dict(w2=r(3, 64, 64)),
           dict(w1=nc(r(3, 64, 64, dt=h))), dict(bias1=r(32)), dict(shift2=r(64).double()), dict(res=r(1, 8, 16, 64, dt=h)),
           dict(res=nc(r(1, 8, 32, 64, dt=h))), dict(out=nc(z(1, 8, 32, 64, dt=h))), dict(out=z(1, 8, 32, 64))]),
-        (ops.cast_gru, dict(embd=gru[0], wih_t=gru[1], whh_t=gru[2], bih=gru[3], bhh=gru[4], wmlp=gru[5], bmlp=gru[6], steps=4), None,
+        (ops.cast_gru, dict(embd=gru[0], wih_t=gru[1], whh_t=gru[2], bih=gru[3], bhh=gru[4], wmlp=gru[5], bmlp=gru[6], steps=4,
+                            out=z(2, 6, 4, 2)), "out",
          [dict(embd=gru[0].double()), dict(embd=r(2, 256)), dict(embd=nc(gru[0])), dict(embd=gru[0].cpu()), dict(whh_t=r(6, 64, 96)),
-          dict(bih=r(5, 192)), dict(wmlp=nc(gru[5])), dict(bmlp=gru[6].double())]),
+          dict(bih=r(5, 192)), dict(wmlp=nc(gru[5])), dict(bmlp=gru[6].double()), dict(bhh=gru[4].cpu()), dict(steps=0),
+          dict(out=z(2, 6, 4, 2).double()), dict(out=z(2, 6, 5, 2)), dict(out=z(3, 6, 4, 2)), dict(out=nc(z(2, 6, 4, 2))),
+          dict(out=z(2, 6, 4, 2).cpu()), dict(embd=e2, out=e2.view(-1)[100:196].view(2, 6, 4, 2))]),
+        (ops.crop_bilinear_u8, dict(bev_u8=bev8, frame_idx=fi, theta=th, crop_size=8, out=z(3, 3, 8, 8)), "out",
+         [dict(bev_u8=bev8.float()), dict(bev_u8=bev8[0]), dict(bev_u8=nc(bev8)), dict(bev_u8=bev8.cpu()), dict(bev_u8=bev8[:, :0]),
+          dict(frame_idx=fi.float()), dict(frame_idx=fi[:2]), dict(frame_idx=fi.cpu()), dict(theta=th.view(3, 6)), dict(theta=th[:2]),
+          dict(theta=th.cpu()), dict(crop_size=1), dict(crop_size=65536), dict(out=z(3, 3, 8, 9)), dict(out=z(3, 3, 8, 8).double()),
+          dict(out=nc(z(3, 3, 8, 8))), dict(out=z(3, 3, 8, 8).cpu()),
+          dict(theta=buf8.view(-1)[:18].view(3, 2, 3), out=buf8)]),
     ]
 
 

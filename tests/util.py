@@ -683,3 +683,184 @@ def lidar_batch32(raw, rows, sweeps, cams, H, W, n_time):
             o[:, cols + sw["time_idx"]] = 1
         out[m] = o
     return out
+
+
+# ----------------------------------------------------------------------------------------------------- cast GRU and u8 crop
+# fp64 statements of lavb_cast_gru and lavb_crop_bilinear_u8 (include/lav_b200.h), pinned to torch's float64 nn.GRU and
+# F.affine_grid + F.grid_sample by tests/test_cast_crop_ref_cpu.py and held against the kernels by
+# tests/test_gpu_cast_crop_contract.py.
+CAST_MUTANTS = ("bhn_outside_r", "r_z_swapped", "h_update_swapped", "cumsum_shifted", "branches_swapped")
+# largest |kernel - cast_gru_ref| / mag allowed on the H100, mag being cast_gru_ref's per-element magnitude
+# (tests/test_gpu_cast_crop_contract.py states the measured value and the margin)
+CAST_TOL = 4e-5
+
+
+def cast_gru_ref(embd, wih_t, whh_t, bih, bhh, wmlp, bmlp, steps, mutant=None):
+    """lavb_cast_gru in float64 on embd's device, from the packed operands the kernel reads (embd (n, 512), wih_t (ncmd, 512,
+    192), whh_t (ncmd, 64, 192), bih / bhh (ncmd, 192), wmlp (ncmd, 2, 64), bmlp (ncmd, 2)) -> (out, mag), both
+    (n, ncmd, steps, 2) float64.
+
+    out: nn.GRU(512, 64) over the embedding repeated ``steps`` times from h = 0 (gate order r, z, n; n = tanh(gi_n +
+    r (W_hn h + b_hn)); h' = (1 - z) n + z h), then Linear(64, 2) and the inclusive cumsum over the steps.
+    mag: the cumsum of |b_mlp| + sum_j |W_mlp,j| |h'_j| over the same steps, the size of the terms that make up each output:
+    an error measured in units of mag is measured against that step's own waypoint, not the largest one.
+    mutant: one of CAST_MUTANTS states a plausible wrong kernel instead: b_hn added outside the reset gate, the r and z
+    columns swapped, h' = (1 - z) h + z n, the cumsum shifted by one step (exclusive), or branches 0 and 1 swapped."""
+    assert mutant is None or mutant in CAST_MUTANTS
+    dev = embd.device
+    x = embd.double()
+    wi, wh, bi, bh, wm, bm = (t.to(dev).double() for t in (wih_t, whh_t, bih, bhh, wmlp, bmlp))
+    if mutant == "branches_swapped":
+        perm = torch.arange(wi.shape[0], device=dev)
+        perm[[0, 1]] = perm[[1, 0]]
+        wi, wh, bi, bh, wm, bm = (t[perm] for t in (wi, wh, bi, bh, wm, bm))
+    ncmd, n = wi.shape[0], x.shape[0]
+    gi = torch.einsum("nk,ckg->cng", x, wi) + bi[:, None]                  # (ncmd, n, 192)
+    h = torch.zeros((ncmd, n, 64), dtype=torch.float64, device=dev)
+    loc, mg = torch.zeros((ncmd, n, 2), dtype=torch.float64, device=dev), torch.zeros((ncmd, n, 2), dtype=torch.float64, device=dev)
+    outs, mags = [], []
+    for _ in range(steps):
+        ghw = torch.bmm(h, wh)                                                 # W_hh h, (ncmd, n, 192)
+        gh = ghw + bh[:, None]
+        r = torch.sigmoid(gi[..., :64] + gh[..., :64])
+        z = torch.sigmoid(gi[..., 64:128] + gh[..., 64:128])
+        if mutant == "r_z_swapped":
+            r, z = z, r
+        if mutant == "bhn_outside_r":
+            nn_ = torch.tanh(gi[..., 128:] + r * ghw[..., 128:] + bh[:, None, 128:])
+        else:
+            nn_ = torch.tanh(gi[..., 128:] + r * gh[..., 128:])
+        h = (1 - z) * h + z * nn_ if mutant == "h_update_swapped" else (1 - z) * nn_ + z * h
+        loc = loc + torch.einsum("cnj,coj->cno", h, wm) + bm[:, None]
+        mg = mg + torch.einsum("cnj,coj->cno", h.abs(), wm.abs()) + bm.abs()[:, None]
+        outs.append(loc)
+        mags.append(mg)
+    out, mag = torch.stack(outs, 2).permute(1, 0, 2, 3), torch.stack(mags, 2).permute(1, 0, 2, 3)
+    if mutant == "cumsum_shifted":
+        out = torch.cat([torch.zeros_like(out[:, :, :1]), out[:, :, :-1]], 2)
+    return out.contiguous(), mag.contiguous()
+
+
+def cast_rel_err(got, want, mag):
+    """max over the elements where want is finite of |got - want| / mag (cast_gru_ref's units); inf if got is not finite there"""
+    fin = torch.isfinite(want)
+    if not bool(fin.any()):
+        return 0.0
+    g, w, m = got.double().to(want.device)[fin], want[fin], mag[fin]
+    if not bool(torch.isfinite(g).all()):
+        return math.inf
+    return float(((g - w).abs() / m).max())
+
+
+def cast_inputs(n, ncmd, scale="product", seed=0):
+    """seeded fp32 CPU operands of lavb_cast_gru, packed as the kernel reads them: (embd, wih_t, whh_t, bih, bhh, wmlp, bmlp).
+    Every branch has its own weights; the biases are N(0, 1), eight times nn.GRU's default init, so that where a bias enters
+    the gate formula shows in the output.  scale "product": non-negative embeddings of the embedder's ReLU + average-pool
+    output, about 0.5 on average; "saturating": N(0, 150) embeddings, whose input projections reach +-100 and beyond, so that
+    most gates round to exactly 0 or 1 in fp32 (expf(100) overflows; tanhf(17) is 1)."""
+    g = torch.Generator().manual_seed(seed)
+    r = lambda *s: torch.randn(s, generator=g)                                 # noqa: E731
+    embd = r(n, 512).abs() * 0.6 if scale == "product" else r(n, 512) * 150.0
+    wih = r(ncmd, 192, 512) / 512 ** 0.5
+    whh = r(ncmd, 192, 64) / 64 ** 0.5
+    bih, bhh = r(ncmd, 192), r(ncmd, 192)
+    wmlp, bmlp = r(ncmd, 2, 64) / 8, r(ncmd, 2)
+    return (embd.contiguous(), wih.transpose(1, 2).contiguous(), whh.transpose(1, 2).contiguous(), bih, bhh, wmlp.contiguous(), bmlp)
+
+
+def cast_planner_inputs(n, seed=0):
+    """the ego cast branches of the benchmarked UniPlanner (6 x GRU(512, 64) + Linear(64, 2)) with synth.fill_state_dict_
+    weights, packed as heads._cast_branches packs them, and n product-scale embeddings -> as cast_inputs"""
+    import torch.nn as nn
+
+    class Branches(nn.Module):                         # the state_dict keys of UniPlanner's ego branches
+        def __init__(self):
+            super().__init__()
+            self.cast_grus_ego = nn.ModuleList([nn.GRU(512, 64, batch_first=True) for _ in range(6)])
+            self.cast_mlps_ego = nn.ModuleList([nn.Linear(64, 2) for _ in range(6)])
+
+    m = Branches()
+    m.load_state_dict(synth.fill_state_dict_(m.state_dict()))
+    grus, mlps = m.cast_grus_ego, m.cast_mlps_ego
+    with torch.no_grad():
+        pack = (torch.stack([q.weight_ih_l0.t() for q in grus]).contiguous(), torch.stack([q.weight_hh_l0.t() for q in grus]).contiguous(),
+                torch.stack([q.bias_ih_l0 for q in grus]).contiguous(), torch.stack([q.bias_hh_l0 for q in grus]).contiguous(),
+                torch.stack([q.weight for q in mlps]).contiguous(), torch.stack([q.bias for q in mlps]).contiguous())
+    return (cast_inputs(n, 1, "product", seed)[0], *pack)
+
+
+def crop_linspace32(S):
+    """torch.linspace(-1, 1, S) in fp32 as the crop kernels form it (start + step i for i < S // 2, end - step (S - 1 - i)
+    after, one fmaf each: i * step is exact in float64, so one rounding to fp32 is the fmaf) -> float32 numpy (S,)"""
+    step = np.float32(2) / np.float32(S - 1)
+    i = np.arange(S, dtype=np.float64)
+    lo = (i * np.float64(step) - 1.0).astype(np.float32)
+    hi = (1.0 - (S - 1 - i) * np.float64(step)).astype(np.float32)
+    return np.where(np.arange(S) < S // 2, lo, hi)
+
+
+def crop_positions(theta, S, H, W, fp32=False):
+    """sample positions of the crops of theta (K, 2, 3) on an H x W map -> (ix, iy), each (K, S, S) float64 CPU, [k, j, i].
+    fp32=False: the affine map in float64 from the fp32 grid values x_i, y_j (crop_linspace32) and the fp32 theta.
+    fp32=True: the kernels' own fp32 positions, bit for bit: gx = fmaf(t00, x_i, fmaf(t01, y_j, t02)), ix = (gx + 1) * 0.5 *
+    (W - 1), each operation rounded to fp32 (fma32 is a correctly rounded fmaf)."""
+    lin = crop_linspace32(S)
+    if fp32:
+        t = theta.detach().float().cpu().numpy()
+        X, Y = lin[None, None, :], lin[None, :, None]
+        out = []
+        for row, n in ((0, W), (1, H)):
+            g = fma32(t[:, row, 0, None, None], X, fma32(t[:, row, 1, None, None], Y, t[:, row, 2, None, None]))
+            with np.errstate(all="ignore"):
+                out.append(torch.from_numpy((((g + F32(1)) * F32(0.5)) * F32(n - 1)).astype(np.float64)))
+        return out[0], out[1]
+    t = theta.detach().float().cpu().double()
+    x = torch.from_numpy(lin.astype(np.float64))
+    X, Y = x[None, None, :], x[None, :, None]
+    gx = t[:, 0, 0, None, None] * X + t[:, 0, 1, None, None] * Y + t[:, 0, 2, None, None]
+    gy = t[:, 1, 0, None, None] * X + t[:, 1, 1, None, None] * Y + t[:, 1, 2, None, None]
+    return (gx + 1) / 2 * (W - 1), (gy + 1) / 2 * (H - 1)
+
+
+def crop_u8_ref(bev_u8, frame_idx, theta, S, fp32_positions=False):
+    """lavb_crop_bilinear_u8 in float64 on bev_u8's device: bev_u8 (B, C, H, W) uint8, frame_idx (K,) clamped to [0, B),
+    theta (K, 2, 3) -> (K, C, S, S) float64.  Bilinear with zero padding at crop_positions(theta, S, H, W, fp32_positions):
+    taps floor(ix) + {0, 1}, floor(iy) + {0, 1} with weights (1 - ax)(1 - ay), ax (1 - ay), (1 - ax) ay, ax ay; a tap off
+    the map adds nothing.  The header's rule for non-finite positions: a NaN coordinate gives NaN in every channel; an
+    infinite one reads no tap (0)."""
+    B, C, H, W = bev_u8.shape
+    dev = bev_u8.device
+    fi = frame_idx.long().to(dev).clamp(0, B - 1)
+    ix, iy = (p.to(dev) for p in crop_positions(theta, S, H, W, fp32_positions))
+    x0, y0 = ix.floor(), iy.floor()
+    ax, ay = ix - x0, iy - y0
+    flat = bev_u8.reshape(-1)
+    chan = (torch.arange(C, device=dev) * (H * W))[None, :, None, None]
+    out = torch.zeros((fi.numel(), C, S, S), dtype=torch.float64, device=dev)
+    for dy, dx, wgt in ((0, 0, (1 - ax) * (1 - ay)), (0, 1, ax * (1 - ay)), (1, 0, (1 - ax) * ay), (1, 1, ax * ay)):
+        x, y = x0 + dx, y0 + dy
+        ok = (x >= 0) & (x < W) & (y >= 0) & (y < H)
+        base = fi[:, None, None] * (C * H * W) + torch.where(ok, y, 0).long() * W + torch.where(ok, x, 0).long()
+        out += torch.where(ok, wgt, 0.0)[:, None] * flat[base[:, None] + chan].double()
+    nan = (torch.isnan(ix) | torch.isnan(iy))[:, None].expand_as(out)
+    return torch.where(nan, torch.full_like(out, math.nan), out)
+
+
+def cast_case(n, ncmd, steps, scale, rows=None):
+    """the operands of one case of tests/test_gpu_cast_crop_contract.py, seeded by the case itself -> (operands, steps).
+    scale "product" / "saturating": cast_inputs; "planner": cast_planner_inputs (ncmd must be 6).  rows: keep only the first
+    rows embeddings (the cases' rows are independent, so these are still the GPU test's inputs)."""
+    seed = n * 1000 + ncmd * 100 + steps + {"product": 0, "saturating": 1, "planner": 2}[scale]
+    if scale == "planner":
+        assert ncmd == 6
+        ops_ = cast_planner_inputs(n, seed)
+    else:
+        ops_ = cast_inputs(n, ncmd, scale, seed)
+    if rows is not None:
+        ops_ = (ops_[0][:rows].contiguous(), *ops_[1:])
+    return ops_, steps
+
+
+# (n, ncmd, steps, scale) cases of the GPU test at which the CPU test shows every mutant far outside CAST_TOL; the last is the
+# frame path at the benchmark's batch: 2 pipelines x 32 agents, 3 detected vehicles each -> 96 + 32 rows, 20 steps
+CAST_MUTANT_CASES = {"product": (37, 7, 20, "product"), "saturating": (37, 7, 20, "saturating"), "frame_path": (128, 6, 20, "planner")}
