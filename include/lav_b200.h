@@ -230,6 +230,32 @@ int lavb_png_decode_gray8(const uint8_t* d_src, long long src_bytes, const void*
 int lavb_lidar_batch(const float* d_raw, long long n_raw, int c, const int* d_rows, long long n_rows, const void* d_sweeps,
                      int n_sweeps, const float* h_cams, int ncam, int h, int w, int n_time, float* d_out, void* stream);
 
+/* the same batch with its sweeps painted online, as the agent paints each sweep when it arrives
+ * replaces: InferModel.forward_paint + point_painting (team_code_v2/model_inference.py:44-50,75-93) with the segmentation head's
+ *           output_conv, softmax and background suppression (lav/models/erfnet.py:122-124,132, lav_agent_fast.py:264) on each
+ *           stacked sweep, then lavb_lidar_batch; the reference paints offline instead (lav/data_paint.py:44-107, lidar_sem_%05d).
+ * d_raw: n_raw rows of 4 floats [x y z r], 16-byte aligned, every sweep of the batch; d_rows, d_sweeps (LidarSweep records, its
+ *   layout unchanged) and n_sweeps as lavb_lidar_batch; d_slots: DEVICE int32[n_sweeps], the frame slot of each sweep.
+ * d_feat: NHWC (n_frames * ncam, h/2, w/2, 16) fp32 or h16 (feat_dtype) = the input of output_conv for the ncam images of each
+ *   frame slot, image f * ncam + c; d_deconv: lavb_paint_deconv_batched's 520-float table of c_cls classes; h_cams as lavb_paint,
+ *   the cameras of both the painting and the re-mask.
+ * Each output row is lavb_lidar_batch's row of c = c_cls - 1 painted columns, the painted columns of raw row i being those
+ *   lavb_paint_deconv_batched (copy_cols 4) computes for point i from frame slot slots[s] of its sweep s: the projection of the
+ *   raw, unrotated point; at a hit, the logits at (v/2, u/2) of image slots[s] * ncam + hit camera, softmax and suppression;
+ *   zeros where no camera sees it.  Then the rotation, the re-mask of the rotated point, the move and the one-hot of
+ *   lavb_lidar_batch.  Bit-identical to lavb_paint_deconv_batched on each sweep followed by lavb_lidar_batch on the painted rows.
+ * The frame slots are device data the call never sees: a slot outside [0, n_frames) reads no feature and gives every row of
+ *   that sweep NaN painted columns (NaN after the re-mask too), so such a row cannot pass for an unseen point.
+ * d_out: n_rows x (3 + c_cls + n_time) fp32, every element written.  3 + c_cls + n_time <= 16.
+ * Checked before any launch (a rejected call writes nothing): the sizes >= 0, n_raw < 2^31, c_cls 2..8, ncam 1..4, h and w even
+ *   and > 0, feat_dtype LAVB_F32 or the 16-bit type, fewer than 2^31 blocks of 256 rows; non-null h_cams, row table, output and
+ *   deconv table (n_rows > 0), raw rows, sweeps and slots (n_raw > 0), features (n_raw and n_frames > 0); d_raw 16-byte, d_feat
+ *   16-byte (fp32) / 8-byte (h16), every other device pointer 4-byte aligned. */
+int lavb_lidar_batch_paint(const float* d_raw, long long n_raw, const int* d_rows, long long n_rows, const void* d_sweeps,
+                           const int* d_slots, int n_sweeps, const void* d_feat, int feat_dtype, int n_frames, int c_cls,
+                           const float* d_deconv, const float* h_cams, int ncam, int h, int w, int n_time, float* d_out,
+                           void* stream);
+
 /* ---------------------------------------------------------------- detection targets of a training batch
  * replaces: LiDARDataset.detections_to_heatmap (lav/utils/datasets/lidar_dataset.py:92-127), once per sample.
  * d_actors: DEVICE array of 24-byte records { float x, y, ori, bx, by, typ; } (ego-frame metres, radians, box extents, class:

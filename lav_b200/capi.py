@@ -84,6 +84,9 @@ _SIGS = {
                                         C.c_void_p, C.c_void_p]),
     "lavb_lidar_batch": (C.c_int, [C.c_void_p, C.c_longlong, C.c_int, C.c_void_p, C.c_longlong, C.c_void_p, C.c_int, C.c_void_p,
                                    C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
+    "lavb_lidar_batch_paint": (C.c_int, [C.c_void_p, C.c_longlong, C.c_void_p, C.c_longlong, C.c_void_p, C.c_void_p, C.c_int,
+                                         C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int,
+                                         C.c_int, C.c_void_p, C.c_void_p]),
     "lavb_det_heatmaps": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_float, C.c_float, C.c_float, C.c_float,
                                     C.c_float, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "lavb_eval_batch": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_int,

@@ -30,4 +30,21 @@ __device__ __forceinline__ void deconv_logits(const DeconvW& dw, const float (&f
   }
 }
 
+// torch.softmax over the c_cls logits pr[0 .. c_cls) (expf(x - max) / sum: fmaxf max, so a NaN logit is skipped by the max; sum
+// in class order; IEEE division), then the background suppression of forward_paint (model_inference.py:45): o[k - 1] = p_k *
+// (1 - p_0) for k = 1 .. c_cls - 1.  The one tail every kernel that paints from the logits uses, so their columns agree bit for bit.
+__device__ __forceinline__ void softmax_suppress(float (&pr)[8], int c_cls, float* o) {
+  float mx = pr[0];
+#pragma unroll
+  for (int k = 1; k < 8; ++k) if (k < c_cls) mx = fmaxf(mx, pr[k]);
+  float sum = 0.f;
+#pragma unroll
+  for (int k = 0; k < 8; ++k) if (k < c_cls) { pr[k] = expf(pr[k] - mx); sum += pr[k]; }
+#pragma unroll
+  for (int k = 0; k < 8; ++k) if (k < c_cls) pr[k] = __fdiv_rn(pr[k], sum);
+  const float bg = __fsub_rn(1.f, pr[0]);
+#pragma unroll
+  for (int k = 1; k < 8; ++k) if (k < c_cls) o[k - 1] = __fmul_rn(pr[k], bg);
+}
+
 }  // namespace lavb

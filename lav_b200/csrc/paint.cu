@@ -237,17 +237,7 @@ __global__ void __launch_bounds__(256) paint_deconv_kernel(const float* __restri
   load_feat16<TF>(f, fv);
   float pr[8];
   deconv_logits<8>(sw, fv, hit_v & 1, hit_u & 1, pr);
-  float mx = pr[0];
-#pragma unroll
-  for (int k = 1; k < 8; ++k) if (k < c_cls) mx = fmaxf(mx, pr[k]);
-  float sum = 0.f;
-#pragma unroll
-  for (int k = 0; k < 8; ++k) if (k < c_cls) { pr[k] = expf(pr[k] - mx); sum += pr[k]; }
-#pragma unroll
-  for (int k = 0; k < 8; ++k) if (k < c_cls) pr[k] = __fdiv_rn(pr[k], sum);
-  const float bg = __fsub_rn(1.f, pr[0]);
-#pragma unroll
-  for (int k = 1; k < 8; ++k) if (k < c_cls) o[k - 1] = __fmul_rn(pr[k], bg);
+  softmax_suppress(pr, c_cls, o);
 }
 
 extern "C" int lavb_paint_deconv_batched(const float* d_pts, int frames, int n, int pt_stride, long long pts_frame_stride,
@@ -412,6 +402,113 @@ extern "C" int lavb_lidar_batch(const float* d_raw, long long n_raw, int c, cons
   cs.ncam = ncam;
   lidar_batch_kernel<<<(unsigned)((n_rows + 255) / 256), 256, 0, (cudaStream_t)stream>>>(
       d_raw, n_raw, 4 + c, d_rows, n_rows, reinterpret_cast<const LidarSweep*>(d_sweeps), n_sweeps, cs, h, w, n_time, d_out);
+  LAVB_LAUNCH_OK();
+  return 0;
+}
+
+// ---- the same batch painted online: lidar_batch_kernel with the painted columns computed from the ERFNet decoder's features
+// instead of read from raw.  Per row: project_hit of the raw, unrotated point; at a hit, the 16 features of the sweep's frame slot
+// and camera at (v/2, u/2), deconv_logits and softmax_suppress, exactly paint_deconv_kernel's chain; then lidar_batch_kernel's
+// rotation, re-mask, move and one-hot.  Bit-identical to lavb_paint_deconv_batched on each sweep followed by lavb_lidar_batch on
+// the painted rows, without the painted intermediate: a row reads 16 B of raw point and, when a camera sees it, 32 B (h16) or
+// 64 B (fp32) of features.
+template <typename TF>
+__global__ void __launch_bounds__(256) lidar_batch_paint_kernel(const float* __restrict__ raw, long long n_raw,
+                                                                const int* __restrict__ rows, long long n_rows,
+                                                                const LidarSweep* __restrict__ sweeps,
+                                                                const int* __restrict__ slots, int n_sweeps,
+                                                                const TF* __restrict__ feat, int n_frames, int c_cls,
+                                                                const DeconvW* __restrict__ dw, const __grid_constant__ CamSet cams,
+                                                                int H, int W, int n_time, float* __restrict__ out) {
+  __shared__ float tile[256 * kStackMaxCols];
+  __shared__ DeconvW sdw;
+  for (int i = threadIdx.x; i < (int)(sizeof(DeconvW) / 4); i += blockDim.x) reinterpret_cast<float*>(&sdw)[i] = __ldg(reinterpret_cast<const float*>(dw) + i);
+  __syncthreads();
+  const int npaint = c_cls - 1, dcols = 4 + npaint + n_time;
+  const long long r0 = (long long)blockIdx.x * 256, r = r0 + threadIdx.x;
+  if (r < n_rows) {
+    float* d = tile + threadIdx.x * dcols;
+    const int src = __ldg(rows + r);
+    int s = -1;
+    if (src >= 0 && src < n_raw) {
+      int lo = 0, hi = n_sweeps;
+      while (lo < hi) {
+        const int mid = (lo + hi) >> 1;
+        if (__ldg(&sweeps[mid].row0) <= src) lo = mid + 1; else hi = mid;
+      }
+      s = lo - 1;
+    }
+    if (s < 0) {
+      for (int k = 0; k < dcols; ++k) d[k] = 0.f;
+    } else {
+      const LidarSweep& sw = sweeps[s];
+      const float4 p = __ldg(reinterpret_cast<const float4*>(raw) + src);
+      float* pc = d + 4;
+      const int f = __ldg(slots + s);
+      int u = 0, v = 0;
+      const int cam = project_hit(cams, p.x, p.y, p.z, H, W, u, v);
+      if (f < 0 || f >= n_frames) {          // a frame slot outside the feature buffer: NaN, never an unseen point's zeros
+        for (int k = 0; k < npaint; ++k) pc[k] = __int_as_float(0x7fc00000);
+      } else if (cam < 0) {
+        for (int k = 0; k < npaint; ++k) pc[k] = 0.f;
+      } else {
+        const TF* fp = feat + ((((long long)f * cams.ncam + cam) * (H >> 1) + (v >> 1)) * (W >> 1) + (u >> 1)) * 16;
+        float fv[16];
+        load_feat16<TF>(fp, fv);
+        float pr[8];
+        deconv_logits<8>(sdw, fv, v & 1, u & 1, pr);
+        softmax_suppress(pr, c_cls, pc);
+      }
+      float ax, ay, az;
+      move_point(sw.R_aug, 0.f, 0.f, p.x, p.y, p.z, ax, ay, az);
+      const float vis = project_hit(cams, ax, ay, az, H, W, u, v) >= 0 ? 1.f : 0.f;
+      move_point(sw.R_mv, sw.dx, sw.dy, ax, ay, az, d[0], d[1], d[2]);
+      d[3] = p.w;
+      for (int k = 0; k < npaint; ++k) pc[k] = __fmul_rn(pc[k], vis);
+      for (int k = 0; k < n_time; ++k) d[4 + npaint + k] = (k == sw.time_idx) ? 1.f : 0.f;
+    }
+  }
+  __syncthreads();
+  const int nrow = (int)min(256LL, n_rows - r0);
+  float* o = out + r0 * dcols;
+  for (int e = threadIdx.x; e < nrow * dcols; e += 256) o[e] = tile[e];
+}
+
+extern "C" int lavb_lidar_batch_paint(const float* d_raw, long long n_raw, const int* d_rows, long long n_rows, const void* d_sweeps,
+                                      const int* d_slots, int n_sweeps, const void* d_feat, int feat_dtype, int n_frames, int c_cls,
+                                      const float* d_deconv, const float* h_cams, int ncam, int h, int w, int n_time, float* d_out,
+                                      void* stream) {
+  LAVB_CHECK_ARG(n_raw >= 0 && n_raw <= 0x7fffffffLL && n_rows >= 0 && n_sweeps >= 0 && n_frames >= 0 && n_time >= 0,
+                 "lidar_batch_paint: bad sizes (n_raw %lld, n_rows %lld, n_sweeps %d, n_frames %d, n_time %d)", n_raw, n_rows,
+                 n_sweeps, n_frames, n_time);
+  LAVB_CHECK_ARG(c_cls >= 2 && c_cls <= 8, "lidar_batch_paint: c_cls must be 2..8 (got %d)", c_cls);
+  LAVB_CHECK_ARG(3 + c_cls + n_time <= kStackMaxCols, "lidar_batch_paint: rows wider than %d floats", kStackMaxCols);
+  LAVB_CHECK_ARG(h_cams != nullptr && ncam >= 1 && ncam <= 4 && h > 0 && w > 0 && h % 2 == 0 && w % 2 == 0,
+                 "lidar_batch_paint: bad cameras (ncam %d, %d x %d; the image size must be even)", ncam, h, w);
+  LAVB_CHECK_ARG(feat_dtype == LAVB_F32 || feat_dtype == LAVB_H16, "lidar_batch_paint: feature dtype must be fp32 or h16");
+  LAVB_CHECK_ARG(n_rows == 0 || (d_rows != nullptr && d_out != nullptr && d_deconv != nullptr),
+                 "lidar_batch_paint: null row table, output or deconv table");
+  LAVB_CHECK_ARG(n_raw == 0 || (d_raw != nullptr && d_sweeps != nullptr && d_slots != nullptr && n_sweeps > 0),
+                 "lidar_batch_paint: null raw rows, sweeps or frame slots");
+  LAVB_CHECK_ARG(n_raw == 0 || n_frames == 0 || d_feat != nullptr, "lidar_batch_paint: null features");
+  LAVB_CHECK_ARG((n_rows + 255) / 256 <= 0x7fffffffLL, "lidar_batch_paint: n_rows %lld needs 2^31 or more blocks", n_rows);
+  LAVB_CHECK_ARG(is_aligned(d_raw, 16) && is_aligned(d_feat, feat_dtype == LAVB_F32 ? 16 : 8) && is_aligned(d_rows, 4) &&
+                     is_aligned(d_sweeps, 4) && is_aligned(d_slots, 4) && is_aligned(d_deconv, 4) && is_aligned(d_out, 4),
+                 "lidar_batch_paint: d_raw must be 16-byte aligned, d_feat 16-byte (fp32) / 8-byte (h16), the others 4-byte");
+  if (n_rows == 0) return 0;
+  CamSet cs;
+  memcpy(cs.m, h_cams, sizeof(float) * 41 * ncam);
+  cs.ncam = ncam;
+  const unsigned blocks = (unsigned)((n_rows + 255) / 256);
+  cudaStream_t st = (cudaStream_t)stream;
+  const LidarSweep* sw = reinterpret_cast<const LidarSweep*>(d_sweeps);
+  const DeconvW* dw = reinterpret_cast<const DeconvW*>(d_deconv);
+  if (feat_dtype == LAVB_F32)
+    lidar_batch_paint_kernel<float><<<blocks, 256, 0, st>>>(d_raw, n_raw, d_rows, n_rows, sw, d_slots, n_sweeps, (const float*)d_feat,
+                                                            n_frames, c_cls, dw, cs, h, w, n_time, d_out);
+  else
+    lidar_batch_paint_kernel<h16><<<blocks, 256, 0, st>>>(d_raw, n_raw, d_rows, n_rows, sw, d_slots, n_sweeps, (const h16*)d_feat,
+                                                          n_frames, c_cls, dw, cs, h, w, n_time, d_out);
   LAVB_LAUNCH_OK();
   return 0;
 }

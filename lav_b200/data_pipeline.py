@@ -66,25 +66,30 @@ class GpuLidarStacker:
         padded[:num] = lidar[:num]
         return padded, num
 
-    def batch_tables(self, samples, generator=None):
+    def batch_tables(self, samples, generator=None, paint=False):
         """The host half of a batch: samples = [(sweeps, angle_deg, jitters)] as __call__ takes them, sweeps numpy.  Draws each
         sample's permutation from ``generator`` (a CPU torch.Generator; None = torch's default CPU generator) with the sizes and in
         the order of one __call__ per sample, and composes it with the kept rows of the roof filter.  No device work.
         -> dict(raw (N, 4+C) fp32, rows (B, P) int32, sweeps LIDAR_SWEEP_DTYPE records, nums list): raw and rows are pinned
-        CPU tensors when the stacker's device is CUDA."""
+        CPU tensors when the stacker's device is CUDA.  With ``paint`` (online painting) the second entry of each sweep is its
+        frame slot instead of its painted rows: raw is (N, 4) and the dict also holds slots (n_sweeps,) int32, pinned likewise."""
         pin = torch.device(self.device).type == "cuda"
         n_raw = sum(len(sw[0]) for sweeps, _, _ in samples for sw in sweeps)
-        raw = torch.empty((n_raw, 4 + self.C), dtype=torch.float32, pin_memory=pin)
+        raw = torch.empty((n_raw, 4 if paint else 4 + self.C), dtype=torch.float32, pin_memory=pin)
         rows = torch.full((len(samples), self.max_points), -1, dtype=torch.int32, pin_memory=pin)
         a, r = raw.numpy(), rows.numpy()
         table = np.zeros(sum(len(sweeps) for sweeps, _, _ in samples), ops.LIDAR_SWEEP_DTYPE)
+        slots = torch.zeros(len(table), dtype=torch.int32, pin_memory=pin) if paint else None
         r0, s, nums = 0, 0, []
         for b, (sweeps, angle_deg, jitters) in enumerate(samples):
             R_aug, moves = sweep_transforms(sweeps, angle_deg, jitters)
             kept = []
             for i, (xyzr, painted, _, _) in enumerate(sweeps):
                 n = len(xyzr)
-                a[r0:r0 + n, :4], a[r0:r0 + n, 4:] = xyzr, painted
+                if paint:
+                    a[r0:r0 + n], slots[s] = xyzr, int(painted)
+                else:
+                    a[r0:r0 + n, :4], a[r0:r0 + n, 4:] = xyzr, painted
                 kept.append(r0 + np.flatnonzero(roof_keep(a[r0:r0 + n])))
                 R_mv, dloc = moves[i]
                 table[s] = (R_aug.ravel(), R_mv.ravel(), dloc[0], dloc[1], i, r0)
@@ -94,14 +99,23 @@ class GpuLidarStacker:
             num = min(self.max_points, len(kept))
             r[b, :num] = kept[perm[:num]]
             nums.append(num)
-        return dict(raw=raw, rows=rows, sweeps=table, nums=nums)
+        out = dict(raw=raw, rows=rows, sweeps=table, nums=nums)
+        if paint:
+            out["slots"] = slots
+        return out
 
     @torch.no_grad()
-    def batch_launch(self, t):
-        """The device half: H2D copies of the tables and one lavb_lidar_batch launch -> (B, P, 4+C+T) fp32."""
+    def batch_launch(self, t, painting=None):
+        """The device half: H2D copies of the tables and one lavb_lidar_batch launch -> (B, P, 4+C+T) fp32.  Tables made with
+        ``paint`` take painting = (features of the frame slots' images, their deconv table, n_classes) of forward_features_nhwc
+        and one lavb_lidar_batch_paint launch instead."""
         dev = self.device
         raw, rows = t["raw"].to(dev, non_blocking=True), t["rows"].to(dev, non_blocking=True)
         sweeps = ops._to_device(t["sweeps"].view(np.uint8), dev)
+        if "slots" in t:
+            feat, table, n_classes = painting
+            return ops.lidar_batch_paint(raw, rows, sweeps, t["slots"].to(dev, non_blocking=True), feat, n_classes, table,
+                                         self.cams, self.rgb_hw, self.T)
         return ops.lidar_batch(raw, rows, sweeps, self.cams, self.rgb_hw, self.T)
 
     def batch(self, samples, generator=None):

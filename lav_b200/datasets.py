@@ -216,10 +216,12 @@ class TemporalLiDARPaintedDataset:
         return 0.0, [(np.zeros(2), 0.0)] * (self.num_frame_stack + 1)
 
     # ---- host part: record reads, PNG chunk walks, labels, BEV job rows
-    def prepare(self, idx, angle, jitters, plan_safety=False, cameras=False):
+    def prepare(self, idx, angle, jitters, plan_safety=False, cameras=False, paint=False):
         """the host record of sample ``idx``; with ``plan_safety`` (unaugmented samples only) it also holds the sample's
         plan_safety_table, from the same record reads; with ``cameras``, under "cameras", what CameraDataset reads for the brake
-        model (read_cameras: the three middle cameras of camera_yaws and tel_rgb[:-crop_tel_bottom])."""
+        model (read_cameras: the three middle cameras of camera_yaws and tel_rgb[:-crop_tel_bottom]).  With ``paint`` (online
+        painting) no lidar_sem key is read: each sweep carries its frame index where the painted rows would be, and "traj" the
+        trajectory, for stage_batch's frame table."""
         traj, index = self.index[idx]
         env = self.env(traj)
         cams = read_cameras(env, index, brake_cameras(len(self.camera_yaws), "TemporalLiDARPaintedDataset"),
@@ -232,8 +234,8 @@ class TemporalLiDARPaintedDataset:
         ego_locs, locs, oris, bbox, typs = _label_tracks(tracks, *radii)
         poses = {i: ego_pose(env, i) for i in frames}
         loc0, ori0 = poses[index]
-        sweeps = [(_frame(env, "lidar", i).reshape(-1, 4), _frame(env, "lidar_sem", i).reshape(-1, nseg), poses[i][0], poses[i][1])
-                  for i in frames]
+        sweeps = [(_frame(env, "lidar", i).reshape(-1, 4), i if paint else _frame(env, "lidar_sem", i).reshape(-1, nseg), poses[i][0],
+                   poses[i][1]) for i in frames]
         pngs = [self.map_png(traj, env, c, index) for c in (0, 9, 10)]
         rows = [(c, c, 0.0, angle, 0, 0) for c in range(3)]                                   # load_bev_channels(angle=0, loc=0)
         ppm = self.pixels_per_meter
@@ -265,7 +267,51 @@ class TemporalLiDARPaintedDataset:
             h["plan_safety"] = table
         if cams is not None:
             h["cameras"] = cams
+        if paint:
+            h["traj"] = traj
         return h
+
+    def paint_images(self, traj, i):
+        """the painting cameras' images of frame ``i`` of trajectory ``traj``: rgb_0 .. rgb_2 (point_painting.CAMERA_YAWS, the
+        cameras data_paint reads) decoded by load_img -> (3, 288, 256, 3) uint8 RGB.  A missing key or an image of another size is
+        a LavbError naming the trajectory and the key."""
+        env, what = self.env(traj), self.paths[traj]
+        h, w = self.stacker.rgb_hw
+        imgs = []
+        for c in range(len(self.stacker.cams)):
+            key = f"rgb_{c}_{i:05d}"
+            try:
+                img = load_img(env, f"rgb_{c}", i)
+            except LavbError as e:
+                raise LavbError(f"{what}: {e}") from None
+            if img.shape != (h, w, 3):
+                raise LavbError(f"{what}: record key {key} is {img.shape[1]} x {img.shape[0]}, the painting cameras' images are "
+                                f"{w} x {h}")
+            imgs.append(img)
+        return np.stack(imgs)
+
+    def stage_paint(self, hs, pin, pool=None):
+        """the frame table of a batch prepared with ``paint``: its distinct (trajectory, frame) pairs in first-use order (sample
+        order, each sample's sweeps newest first), each pair's images decoded once by paint_images (on ``pool`` when given) into
+        one (F, 3, 288, 256, 3) uint8 buffer (pinned on ``pin``), and the samples' sweeps with each frame index replaced by its
+        slot.  -> (dict(images, pairs), [sweeps of each sample])."""
+        slot, pairs, sweeps = {}, [], []
+        for h in hs:
+            mine = []
+            for xyzr, i, loc, ori in h["sweeps"]:
+                key = (h["traj"], int(i))
+                if key not in slot:
+                    slot[key] = len(pairs)
+                    pairs.append(key)
+                mine.append((xyzr, slot[key], loc, ori))
+            sweeps.append(mine)
+        imgs = list((pool.map if pool is not None else map)(lambda k: self.paint_images(*k), pairs))
+        h, w = self.stacker.rgb_hw
+        buf = torch.empty((len(pairs), len(self.stacker.cams), h, w, 3), dtype=torch.uint8, pin_memory=pin)
+        dst = buf.numpy()
+        for f, img in enumerate(imgs):
+            dst[f] = img
+        return dict(images=buf, pairs=pairs), sweeps
 
     # ---- device part
     def lidar_and_maps(self, h, generator=None):
@@ -336,12 +382,16 @@ class TemporalLiDARPaintedDataset:
         return self.sample(idx, angle, jit, self.gen)
 
     # ---- a whole batch: host tables (any thread), then a fixed number of launches and H2D copies (the caller's thread)
-    def stage_batch(self, hs, generator=None):
+    def stage_batch(self, hs, generator=None, pool=None):
         """the host tables of a batch of prepared samples ``hs``, in pinned memory on a CUDA dataset.  Draws the LiDAR
-        shuffles from ``generator`` (CPU) in sample order, as one sample() per entry of ``hs`` would."""
+        shuffles from ``generator`` (CPU) in sample order, as one sample() per entry of ``hs`` would.  Samples prepared with
+        ``paint`` also stage their frame table and images under "paint" (stage_paint, the decodes on ``pool``), and the LiDAR
+        tables carry raw (N, 4) rows and a frame slot per sweep."""
         pin = self.device.type == "cuda"
         pinned = lambda a: torch.from_numpy(np.ascontiguousarray(a)).pin_memory() if pin else torch.from_numpy(np.ascontiguousarray(a))
-        lidar = self.stacker.batch_tables([(h["sweeps"], h["angle"], h["jitters"]) for h in hs], generator)
+        paint = bool(hs) and "traj" in hs[0]
+        painting, sweeps = self.stage_paint(hs, pin, pool) if paint else (None, [h["sweeps"] for h in hs])
+        lidar = self.stacker.batch_tables([(sw, h["angle"], h["jitters"]) for sw, h in zip(sweeps, hs)], generator, paint=paint)
         dets = [np.column_stack([np.reshape(locs, (-1, 2)), oris, np.reshape(bbox, (-1, 2)), typs]) for locs, oris, bbox, typs in
                 (h["det"] for h in hs)]
         offsets = np.concatenate([[0], np.cumsum([len(d) for d in dets])]).astype(np.int32)
@@ -357,16 +407,29 @@ class TemporalLiDARPaintedDataset:
             st["plan_safety"] = stage_plan_safety([h["plan_safety"] for h in hs], pin)
         if hs and "cameras" in hs[0]:                                           # prepared with cameras (the brake evaluation)
             st["cameras"] = stage_images([h["cameras"] for h in hs], ("rgbs", "tel"), pin, "TemporalLiDARPaintedDataset")
+        if painting is not None:
+            st["paint"] = painting
         return st
 
+    def paint_features(self, st, seg_model):
+        """forward_features_nhwc of ``seg_model`` over the F x 3 staged images of a batch staged with "paint", in one call ->
+        (features, deconv table, n_classes)."""
+        if seg_model is None:
+            raise LavbError("the batch was prepared for online painting: launch_batch needs the segmentation model")
+        imgs = st["paint"]["images"]
+        F_, ncam, h, w, _ = imgs.shape
+        return seg_model.forward_features_nhwc(imgs.to(self.device, non_blocking=True).view(F_ * ncam, h, w, 3))
+
     @torch.no_grad()
-    def launch_batch(self, st):
+    def launch_batch(self, st, seg_model=None):
         """the device half of a batch staged by stage_batch: the map decode (unless decode_maps ran ahead), lidar_batch,
         det_heatmaps and bev_targets, and the H2D copies; the only device-to-host read is the decode's status, on its own stream
-        -> the loader's 14-tuple."""
+        -> the loader's 14-tuple.  A batch staged with "paint" runs ``seg_model`` once over its frame table's images
+        (paint_features) and takes lidar_batch_paint's one launch instead of lidar_batch."""
         dev = self.device
         to = lambda t: t.to(dev, non_blocking=True)
-        lidar = self.stacker.batch_launch(st["lidar"])
+        painting = self.paint_features(st, seg_model) if "paint" in st else None
+        lidar = self.stacker.batch_launch(st["lidar"], painting)
         grid = dict(min_x=self.min_x, max_x=self.max_x, min_y=self.min_y, max_y=self.max_y, pixels_per_meter=self.pixels_per_meter)
         heat, size, orim = ops.det_heatmaps(to(st["actors"]), to(st["offsets"]), grid)
         planes = self.planes_on_stream(st.get("decoded") or self.decode_maps(st["maps"]))
@@ -425,15 +488,21 @@ class TemporalBatchLoader:
     generator of (seed, epoch, rank).  With ``plan_safety`` (ordered only) every sample is
     prepared with its plan_safety_table, and the staged tables carry them packed under "plan_safety" (stage_plan_safety).  With
     ``cameras`` every sample is prepared with the brake model's camera images, and the staged tables carry them under "cameras"
-    as one pinned uint8 buffer per key: rgbs (B, 3, h, w, 3), tel (B, h_tel, w_tel, 3)."""
+    as one pinned uint8 buffer per key: rgbs (B, 3, h, w, 3), tel (B, h_tel, w_tel, 3).
+
+    With ``seg_model`` (an RGBSegmentationModel, set to the caller's precision) the sweeps are painted online instead of read
+    from lidar_sem: every sample is prepared with ``paint``, the batch's distinct (trajectory, frame) pairs are decoded once each
+    on the ``num_workers`` threads (stage_paint; in ordered mode a batch of 32 consecutive samples has about 34 of them), and
+    launch_batch runs the model once over their images and lidar_batch_paint once; the staged tables carry them under "paint"."""
 
     def __init__(self, dataset, batch_size, seed=2021, rank=0, world=1, drop_last=True, num_workers=8, ordered=False,
-                 plan_safety=False, cameras=False):
+                 plan_safety=False, cameras=False, seg_model=None):
         self.ds, self.B, self.seed, self.rank, self.world, self.drop_last = dataset, batch_size, seed, rank, world, drop_last
         self.num_workers = max(1, int(num_workers))
         self.ordered = ordered
         self.plan_safety = plan_safety
         self.cameras = cameras
+        self.seg_model = seg_model
         if plan_safety and not ordered:
             raise LavbError("plan_safety tables need the ordered, unaugmented loader")
         self.epoch = 0
@@ -442,6 +511,8 @@ class TemporalBatchLoader:
         kw = dict(plan_safety=True) if self.plan_safety else {}
         if self.cameras:
             kw["cameras"] = True
+        if self.seg_model is not None:
+            kw["paint"] = True
         return list(pool.map(lambda a: self.ds.prepare(int(a[0]), *a[1], **kw), zip(idxs, draws)))
 
     def shard(self, epoch):
@@ -464,7 +535,7 @@ class TemporalBatchLoader:
 
     def _host(self, idxs, draws, gen, pool):
         hs = self._prepare(pool, idxs, draws)
-        st = self.ds.stage_batch(hs, gen)
+        st = self.ds.stage_batch(hs, gen, **(dict(pool=pool) if self.seg_model is not None else {}))
         st["decoded"] = self.ds.decode_maps(st["maps"])
         return st
 
@@ -483,13 +554,14 @@ class TemporalBatchLoader:
             return
         draw = self.ds.no_draw if self.ordered else lambda: self.ds.draw(rng)
         draws = lambda idxs: [draw() for _ in idxs]                             # on this thread, in sample order
+        launch = self.ds.launch_batch if self.seg_model is None else lambda st: self.ds.launch_batch(st, self.seg_model)
         with ThreadPoolExecutor(1) as ahead, ThreadPoolExecutor(self.num_workers) as pool:
             nxt = ahead.submit(self._host, batches[0], draws(batches[0]), gen, pool)
             for k in range(len(batches)):
                 staged = nxt.result()
                 if k + 1 < len(batches):
                     nxt = ahead.submit(self._host, batches[k + 1], draws(batches[k + 1]), gen, pool)
-                yield self.ds.launch_batch(staged), staged
+                yield launch(staged), staged
 
 
 class TemporalBEVDataset:

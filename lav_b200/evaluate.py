@@ -4,7 +4,8 @@ against the expert's future — as numbers over every sample of the recording, t
 
     python -m lav_b200.evaluate --config-path config_v2.yaml --data-dir VALDIR --lidar-weights lidar_7.th \
         --uniplanner-weights uniplanner_7.th [--batch-size 32] [--precision f16|fp32] [--num-workers 16] [--json out.json] \
-        [--forecast] [--forecast-detected] [--plan-safety] [--det-boxes] [--brake --bra-weights bra.th [--agent-config AGENT.yaml]]
+        [--forecast] [--forecast-detected] [--plan-safety] [--det-boxes] [--brake --bra-weights bra.th [--agent-config AGENT.yaml]] \
+        [--seg-weights seg_1.th]
     python -m lav_b200.evaluate ... --lidar-weights lidar_8.th lidar_16.th --uniplanner-weights uniplanner_8.th uniplanner_16.th
     python -m lav_b200.evaluate ... --run-dir RUN [--epochs 1,8,16-64]
     torchrun --nproc-per-node N -m lav_b200.evaluate ...
@@ -186,6 +187,27 @@ checkpoints, then per checkpoint two ops.agent_control launches and one copy of 
     agent brakes it triggered and how many of them were false.  A rate over no sample is null.
   Not scored: the throttle, the steer, the speed cap and the creep (they depend on the speed, which the recording holds only as
     the expert's).
+
+With --seg-weights PATH (``seg_model=...``) the LiDAR rows are painted online by that RGBSegmentationModel, as the agent paints
+each sweep when it arrives, instead of read from the recording's lidar_sem keys, which are then never read: a recording that was
+never painted can be scored, two segmentation checkpoints can be scored side by side, and the effect of the painting on every
+score above can be seen.  The model is loaded strictly, as data_paint and evaluate_paint load it, and runs at ``precision``.
+Per batch: the batch's distinct frames decoded once each on the loader's threads, one forward_features_nhwc call over their
+images (shared by every checkpoint of a sweep) and one ops.lidar_batch_paint launch in place of ops.lidar_batch.  The result
+gains painting = {frames: F, images: 3F}, F the frames segmented over the recording.  The protocol:
+
+  What is painted.  The sample at frame i stacks the sweeps of frames i, i - 1, ..., i - num_frame_stack (those >= 0); each
+    sweep is painted with its own frame's images.  That is what data_paint stored for that frame and what the agent painted
+    when that sweep arrived.
+  Cameras.  Those of data_paint and evaluate_paint: point_painting.make_converters(camera_x, camera_z) with CAMERA_YAWS (-60,
+    0, 60), records rgb_0 .. rgb_2 decoded by datasets.load_img (BGR -> RGB), each 288 x 256.  The config's five camera_yaws
+    are not the painting cameras.
+  Order of operations.  Each row is painted on its raw, unrotated point, before the rotation jitter and the field-of-view
+    re-mask of the stored path, so online painting followed by the batch construction equals data_paint followed by the
+    stored path, row for row.
+  Errors.  A missing rgb_{c} key, or an image of another size, raises LavbError naming the trajectory and the key, before the
+    batch is built.
+With --brake the brake model's camera reads are unchanged.
 """
 import argparse
 import json
@@ -662,26 +684,42 @@ def format_brake(b):
     return lines
 
 
+class PaintingCount:
+    """the frames segmented for online painting over a recording."""
+
+    def __init__(self):
+        self.frames = 0
+
+    def extend(self, other):
+        self.frames += other.frames
+
+    def summary(self, ncam=3):
+        return dict(frames=self.frames, images=ncam * self.frames)
+
+
 def evaluate(lidar_model, uniplanner, dataset, batch_size=32, precision="f16", num_workers=16, forecast=False,
-             forecast_detected=False, plan_safety=False, det_boxes=False, brake=False, bra_model=None, agent_config=None):
+             forecast_detected=False, plan_safety=False, det_boxes=False, brake=False, bra_model=None, agent_config=None,
+             seg_model=None):
     """Scores of ``lidar_model`` and ``uniplanner`` over every sample of ``dataset`` (a TemporalLiDARPaintedDataset), the models
     run as the agent runs them at ``precision``; with ``forecast`` also the UniPlanner's forecast scores on the recorded poses,
     with ``forecast_detected`` those on the detected vehicles, with ``plan_safety`` the collision and off-road rates of the ego
     plan and of the expert, with ``det_boxes`` the detections' box scores, with ``brake`` the agent's brake decision with the
-    brake model ``bra_model`` under the controls of ``agent_config`` (the agent's YAML dict; default the dataset's config).
+    brake model ``bra_model`` under the controls of ``agent_config`` (the agent's YAML dict; default the dataset's config); with
+    ``seg_model`` (an RGBSegmentationModel) the sweeps painted online by it instead of read from lidar_sem.
     -> dict (see the module docstring); None on a rank other than 0 of a process group."""
     results = evaluate_checkpoints([(lidar_model, uniplanner)], dataset, batch_size, precision, num_workers, forecast,
-                                   forecast_detected, plan_safety, det_boxes, brake, bra_model, agent_config)
+                                   forecast_detected, plan_safety, det_boxes, brake, bra_model, agent_config, seg_model)
     return None if results is None else results[0]
 
 
 @torch.no_grad()
 def evaluate_checkpoints(pairs, dataset, batch_size=32, precision="f16", num_workers=16, forecast=False, forecast_detected=False,
-                         plan_safety=False, det_boxes=False, brake=False, bra_model=None, agent_config=None):
+                         plan_safety=False, det_boxes=False, brake=False, bra_model=None, agent_config=None, seg_model=None):
     """evaluate() of every (lidar_model, uniplanner) of ``pairs`` in one pass over ``dataset``: each batch is loaded and staged
     once, then every pair runs its own InferModel and scoring launches on it into its own accumulators.  All pairs stay
     resident; a sweep that would not fit on the device is refused before any data is loaded.  With ``brake`` the one brake
-    model ``bra_model`` is resident once, before the pairs are measured, and runs once per batch for all pairs.  In a process
+    model ``bra_model`` is resident once, before the pairs are measured, and runs once per batch for all pairs; so is the
+    segmentation model ``seg_model``, whose painting of each batch all pairs share.  In a process
     group each rank scores its contiguous shard of the recording and rank 0 merges the ranks' records
     (eval_sweep.gather_merged).  -> one evaluate() result per pair on rank 0, None on the other ranks."""
     dev = dataset.device
@@ -698,6 +736,11 @@ def evaluate_checkpoints(pairs, dataset, batch_size=32, precision="f16", num_wor
                             f"({num_cmds}); this one has {aim!r} (--agent-config)")
         ctl = control_config(agent_config)
         bra = brake_model(bra_model.to(dev).eval(), precision)
+    if seg_model is not None:
+        n_cls = seg_model.erfnet.decoder.output_conv.out_channels
+        if n_cls != len(dataset.seg_channels) + 1:
+            raise LavbError(f"evaluate: the seg model has {n_cls} classes, seg_channels gives {len(dataset.seg_channels) + 1}")
+        seg_model.to(dev).eval().set_precision(precision)
     models = []
     for i, (lid, uni) in enumerate(pairs):
         meter = ResidentMeter(dev, lid, uni) if i == 0 and len(pairs) > 1 else None
@@ -709,12 +752,15 @@ def evaluate_checkpoints(pairs, dataset, batch_size=32, precision="f16", num_wor
     grid = dict(min_x=dataset.min_x, max_x=dataset.max_x, min_y=dataset.min_y, max_y=dataset.max_y,
                 pixels_per_meter=dataset.pixels_per_meter)
     loader = TemporalBatchLoader(dataset, batch_size, rank=rank, world=world, drop_last=False, num_workers=num_workers, ordered=True,
-                                 plan_safety=plan_safety, cameras=brake)
-    accs = [(Scores(), ForecastScores(), DetectedForecastScores(), PlanSafetyScores(), DetBoxScores(), BrakeScores(uni.num_cmds))
-            for _, uni in pairs]
+                                 plan_safety=plan_safety, cameras=brake, seg_model=seg_model)
+    accs = [(Scores(), ForecastScores(), DetectedForecastScores(), PlanSafetyScores(), DetBoxScores(), BrakeScores(uni.num_cmds),
+             PaintingCount()) for _, uni in pairs]
     with math_mode(precision):
         for batch, staged in loader.staged_batches():
             actors = staged["actors"].to(dev, non_blocking=True)
+            if "paint" in staged:
+                for acc in accs:
+                    acc[6].frames += len(staged["paint"]["pairs"])
             brake_in = None
             if brake:
                 cams = staged["cameras"]
@@ -725,12 +771,14 @@ def evaluate_checkpoints(pairs, dataset, batch_size=32, precision="f16", num_wor
     accs = gather_merged(accs)
     if accs is None:
         return None
-    return [summarize(acc, precision, forecast, forecast_detected, plan_safety, dataset.num_plan, det_boxes, brake) for acc in accs]
+    return [summarize(acc, precision, forecast, forecast_detected, plan_safety, dataset.num_plan, det_boxes, brake,
+                      seg_model is not None) for acc in accs]
 
 
-def summarize(acc, precision, forecast, forecast_detected, plan_safety, num_plan, det_boxes=False, brake=False):
-    """the evaluate() result of one checkpoint's accumulators ``acc`` (score_batch's tuple; its DetBoxScores is read only with
-    ``det_boxes``, its BrakeScores only with ``brake``)."""
+def summarize(acc, precision, forecast, forecast_detected, plan_safety, num_plan, det_boxes=False, brake=False, painting=False):
+    """the evaluate() result of one checkpoint's accumulators ``acc`` (score_batch's tuple, then its PaintingCount; its
+    DetBoxScores is read only with ``det_boxes``, its BrakeScores only with ``brake``, its PaintingCount only with
+    ``painting``)."""
     scores, forecasts, detected, safety = acc[:4]
     result = scores.summary()
     result["precision"] = precision
@@ -744,6 +792,8 @@ def summarize(acc, precision, forecast, forecast_detected, plan_safety, num_plan
         result["det_boxes"] = acc[4].summary()
     if brake:
         result["brake"] = acc[5].summary()
+    if painting:
+        result["painting"] = acc[6].summary()
     return result
 
 
@@ -804,6 +854,9 @@ def parse_args(argv=None):
     ap.add_argument("--agent-config", default=None,
                     help="with --brake: the agent's YAML (team_code_v2/config.yaml), for its CONTROLLER keys, cmd_thresh and "
                          "pixels_per_meter (default: --config-path)")
+    ap.add_argument("--seg-weights", default=None,
+                    help="paint every stacked sweep online with this RGBSegmentationModel state_dict (seg_1.th) instead of "
+                         "reading the recording's lidar_sem")
     args = ap.parse_args(argv)
     if args.brake and args.bra_weights is None:
         ap.error("--brake needs --bra-weights")
@@ -833,6 +886,8 @@ def format_result(r):
         lines += format_det_boxes(r["det_boxes"])
     if "brake" in r:
         lines += format_brake(r["brake"])
+    if "painting" in r:
+        lines.append(f"painted online: {r['painting']['frames']} frames, {r['painting']['images']} images segmented")
     return "\n".join(lines)
 
 
@@ -893,12 +948,19 @@ def main(argv=None):
         if args.agent_config is not None:
             with open(args.agent_config) as f:
                 agent_cfg = yaml.safe_load(f)
+    seg = None
+    if args.seg_weights is not None:
+        from .rgb import RGBSegmentationModel
+        seg = RGBSegmentationModel(cfg["seg_channels"])
+        seg.load_state_dict(torch.load(args.seg_weights, map_location="cpu"))
     ds = TemporalLiDARPaintedDataset(args.config_path, device=dev, overrides=dict(data_dir=args.data_dir))
     results = evaluate_checkpoints(pairs, ds, args.batch_size, args.precision, args.num_workers, args.forecast,
-                                   args.forecast_detected, args.plan_safety, args.det_boxes, args.brake, bra, agent_cfg)
+                                   args.forecast_detected, args.plan_safety, args.det_boxes, args.brake, bra, agent_cfg, seg)
     out = None
     if results is not None:
         text, out = report(checkpoints, results, rank_and_world()[1])
+        if args.seg_weights is not None:
+            out = dict(out, seg_weights=args.seg_weights)
         print(text)
         if args.json:
             with open(args.json, "w") as f:

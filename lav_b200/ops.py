@@ -687,6 +687,38 @@ def lidar_batch(raw, rows, sweeps, cams, image_hw, n_time, out=None):
     return out
 
 
+def lidar_batch_paint(raw, rows, sweeps, slots, feat, n_classes, deconv, cams, image_hw, n_time, out=None):
+    """lidar_batch with every sweep painted online (see lavb_lidar_batch_paint in include/lav_b200.h).  raw (N, 4) fp32, 16-byte
+    aligned: every sweep's [xyzr] rows; rows and sweeps as lidar_batch; slots (n_sweeps,) int32 on the device: the frame slot of
+    each sweep; feat NHWC (F * ncam, H/2, W/2, 16) fp32 / h16 = forward_features_nhwc of the ncam images of each of F frames;
+    deconv = its pack_deconv2x2 table of ``n_classes``; cams (ncam, 41) float32 numpy, the painting cameras; image_hw = their
+    image size.  -> (B, P, 3 + n_classes + n_time) fp32, bit-identical to paint_deconv_batched on each sweep followed by
+    lidar_batch."""
+    what = "lidar_batch_paint"
+    n_raw, _ = _tensor(what, "raw", raw, torch.float32, (None, 4))
+    _require(raw.data_ptr() % 16 == 0, f"{what}: raw must be 16-byte aligned")
+    b, p = _tensor(what, "rows", rows, torch.int32, (None, None), raw.device)
+    _tensor(what, "sweeps", sweeps, torch.uint8, None, raw.device)
+    _require(sweeps.numel() % LIDAR_SWEEP_DTYPE.itemsize == 0, f"{what}: sweeps must hold whole 88-byte LIDAR_SWEEP_DTYPE records")
+    n_sweeps = sweeps.numel() // LIDAR_SWEEP_DTYPE.itemsize
+    _tensor(what, "slots", slots, torch.int32, (n_sweeps,), raw.device)
+    cams = _host(what, "cams", cams, np.float32, (None, 41), cast=True)
+    ncam, (h, w) = cams.shape[0], image_hw
+    _require(1 <= ncam <= 4 and h > 0 and w > 0 and h % 2 == 0 and w % 2 == 0,
+             f"{what}: 1..4 cameras and an even image size, got {ncam} cameras of {h} x {w}")
+    nf, _, _, _ = _tensor(what, "feat", feat, (torch.float32, h16()), (None, h // 2, w // 2, 16), raw.device)
+    _require(nf % ncam == 0, f"{what}: feat holds {nf} images, not a whole number of frames of {ncam} cameras")
+    _require(feat.data_ptr() % (16 if feat.dtype == torch.float32 else 8) == 0, f"{what}: feat must be 16-byte (fp32) / 8-byte aligned")
+    c = int(n_classes)
+    _require(2 <= c <= 8, f"{what}: n_classes must be 2..8, got {c}")
+    _tensor(what, "deconv", deconv, torch.float32, (520,), raw.device)
+    out = _out(what, "out", out, torch.float32, (b, p, 3 + c + n_time), raw.device)
+    _apart(what, "out", out, raw=raw, rows=rows, sweeps=sweeps, slots=slots, feat=feat, deconv=deconv)
+    _launch("lavb_lidar_batch_paint", _ptr(raw), n_raw, _ptr(rows), b * p, _ptr(sweeps), _ptr(slots), n_sweeps, _ptr(feat),
+            _DT[feat.dtype], nf // ncam, c, _ptr(deconv), _hptr(cams), ncam, h, w, n_time, _ptr(out))
+    return out
+
+
 def det_grid(min_x=-10, max_x=70, min_y=-40, max_y=40, pixels_per_meter=4, radius=1):
     """(h, w, scalars) of the heat-map grid, each scalar computed as detections_to_heatmap's torch ops see it."""
     h, w = (max_y - min_y) * pixels_per_meter, (max_x - min_x) * pixels_per_meter
