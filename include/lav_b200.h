@@ -395,6 +395,42 @@ int lavb_plan_safety(const float* d_traj, int b, int n, int t, const void* d_act
                      const double* d_ego_ext, const uint8_t* d_map, long long map_stride, int h, int w, float ppm, float cx0,
                      float cy0, float cy1, int* d_out, void* stream);
 
+/* ---------------------------------------------------------------- the terms of a PDM-style driving score of planned ego trajectories
+ * stands behind: nothing in the reference, which drives its plans in CARLA; the open-loop stand-in of nuPlan / NAVSIM (no at-fault
+ *   collision, drivable area, time to collision, ego progress, comfort) against the recorded, non-reactive traffic.
+ * One block of n warps per sample, a warp per trajectory (batches of more than 512 samples take one launch per 512).  d_traj,
+ *   d_ego_ext, the map and the grid as lavb_plan_safety's, with its ego boxes, validity, separating-axis test and road-corner rule;
+ *   step 0 is the origin box, heading (0, -1).  d_expert (b, t, 2) fp32 = the polyline the progress is measured along (the
+ *   origin, then its t points).  dt = the step period in seconds; K = floor(1 / dt + 1e-9) <= 64 projections (computed in double
+ *   on the host).
+ * Actors: lavb_plan_safety's 56-byte records, but t + 1 per actor row: row a's record of step s (0..t) at index a * (t + 1) + s.
+ *   Classes 0 and 1 take part, others are ignored.
+ * Kinematics, fp64, correctly rounded, no contraction: v_s = (p_s - p_{s-1}) / dt, speed |v_s| = sqrt(v . v); an actor's
+ *   velocity at s is (q_s - q_{s-1}) / dt when it is present at s - 1 and s, else 0.  The ego is stopped when |v_s| < 0.05.
+ * Collisions: a new collision at step s with a present actor: its box overlaps the ego's at s and did not at s - 1 (at s = 1 the
+ *   origin box against the actor's step-0 box; an actor absent at s - 1 did not overlap).  Exempt when the ego is stopped or the
+ *   actor's centre is behind the ego's rear face, (q_s - p_s) . h_s < -e1; at fault otherwise.
+ * Time to collision: at a step s where the ego is not stopped, for each present actor not overlapping the ego at s: both boxes
+ *   moved to centre + (k * dt) v (ego) and q_s + (k * dt) u (actor), headings held, k = 1..K; at the first k whose boxes
+ *   overlap, a hit unless the projected actor's centre is behind the projected ego's rear face (a rear collision).
+ * Comfort at steps s >= 2 (jerk and yaw acceleration s >= 3), psi_s = atan2(h_s.y, h_s.x) (device atan2, within 2 ulp):
+ *   a_s = (|v_s| - |v_{s-1}|) / dt outside [-4.05, 2.40]; jerk (a_s - a_{s-1}) / dt, |.| > 4.13; yaw rate w_s = wrap(psi_s -
+ *   psi_{s-1}) / dt, wrap to (-pi, pi], |.| > 0.95; yaw acceleration (w_s - w_{s-1}) / dt, |.| > 1.93; lateral |v_s| w_s, |.| > 4.89.
+ * Progress: L = the expert's arc length, segment lengths summed in order; the trajectory's last point P projected on each segment
+ *   [q_{k-1}, q_k], d = q_k - q_{k-1}: u = ((P - q_{k-1}) . d) / (d . d), 0 when d . d = 0, clamped to [0, 1]; distance^2 |P -
+ *   (q_{k-1} + u d)|^2; the first segment of least distance gives s = (length of the segments before it) + u |d|.
+ * A trajectory with an invalid step is scored for the road only (at its valid steps); every other field is -1 (the comfort mask
+ *   0) and s is NaN.
+ * d_out (b, n, 16) int32 per trajectory: [0..2] first at-fault collision step, actor row, class; [3..5] the same for the first
+ *   exempt collision; [6..7] first time-to-collision step and actor row (the lowest (step, row) of each kind); [8] first off-road
+ *   step; [9] comfort mask, bit q set when term q (acceleration, jerk, yaw rate, yaw acceleration, lateral) fails at some step;
+ *   [10..14] each term's first failing step; [15] first invalid step; -1 for none.  d_ep (b, n, 2) fp64 = (s, L).
+ * 1 <= n <= 8, 1 <= t <= 32; traj, expert, actors, ego_ext and ep 8-byte aligned.  Every output element of the b samples is
+ *   written; a rejected call writes nothing. */
+int lavb_driving_score(const float* d_traj, const float* d_expert, int b, int n, int t, const void* d_actors, int n_actors,
+                       const int* h_offsets, const double* d_ego_ext, const uint8_t* d_map, long long map_stride, int h, int w,
+                       float ppm, float cx0, float cy0, float cy1, double dt, double* d_ep, int* d_out, void* stream);
+
 /* ---------------------------------------------------------------- the agent's controls: collision brake, PIDs, brake rules
  * stands behind: lav_agent_fast.py:228-231 and 325-352 (the stop counter, the 4/5 plan swap, pid_control called twice, the
  *           brake model, plan_collide, the speed cap and the creep), pid_control :404-426, plan_collide :385-401 and

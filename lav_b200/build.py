@@ -11,7 +11,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIBDIR = os.path.join(HERE, "_lib")
 LIB = os.path.join(LIBDIR, "liblavb200.so")
-SOURCES = ["capi.cu", "paint.cu", "pillar.cu", "conv_taps.cu", "conv_umma.cu", "stem_umma.cu", "crop.cu", "deconv_small.cu", "peaks.cu", "stem.cu", "conv_pair_umma.cu", "cast_gru.cu", "erf16.cu", "bev_warp.cu", "heatmap.cu", "png.cu", "evaluate.cu", "forecast_eval.cu", "det_forecast.cu", "det_box_eval.cu", "plan_safety.cu", "agent_control.cu", "seg_eval.cu", "agent_nav.cu", "paint_eval.cu", "agent_view.cu"]
+SOURCES = ["capi.cu", "paint.cu", "pillar.cu", "conv_taps.cu", "conv_umma.cu", "stem_umma.cu", "crop.cu", "deconv_small.cu", "peaks.cu", "stem.cu", "conv_pair_umma.cu", "cast_gru.cu", "erf16.cu", "bev_warp.cu", "heatmap.cu", "png.cu", "evaluate.cu", "forecast_eval.cu", "det_forecast.cu", "det_box_eval.cu", "plan_safety.cu", "driving_score.cu", "agent_control.cu", "seg_eval.cu", "agent_nav.cu", "paint_eval.cu", "agent_view.cu"]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 FLAGS = [*ARCH, "-O3", "-std=c++17", "-lineinfo", "-Xcompiler", "-fPIC",

@@ -105,6 +105,9 @@ _SIGS = {
     "lavb_plan_safety": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
                                    C.c_longlong, C.c_int, C.c_int, C.c_float, C.c_float, C.c_float, C.c_float, C.c_void_p,
                                    C.c_void_p]),
+    "lavb_driving_score": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p,
+                                     C.c_void_p, C.c_longlong, C.c_int, C.c_int, C.c_float, C.c_float, C.c_float, C.c_float,
+                                     C.c_double, C.c_void_p, C.c_void_p, C.c_void_p]),
     "lavb_agent_control_state_bytes": (C.c_size_t, [C.c_int, C.c_int]),
     "lavb_agent_control": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p,
                                      C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(ControlConfig), C.c_void_p, C.c_void_p,

@@ -113,15 +113,16 @@ def actor_tracks(env, index, T, max_pedestrian_radius, max_vehicle_radius):
     return _label_tracks(_read_tracks(env, index, T), max_pedestrian_radius, max_vehicle_radius)
 
 
-def _safety_table(tracks):
+def _safety_table(tracks, first=1):
+    """the actor table of steps first .. T of ``tracks`` (plan_safety_table: first = 1, driving_score_table: first = 0)."""
     seen, locs, oris, bbox, typs, e = tracks
     origin, R, ego_ori = _ego_transform(locs, oris, e)
     others = np.arange(len(seen)) != e
-    present = seen[others, 1:]
-    yaw = oris[others, 1:] - ego_ori
+    present = seen[others, first:]
+    yaw = oris[others, first:] - ego_ori
     only = lambda a: np.where(present.reshape(present.shape + (1,) * (a.ndim - 2)), a, 0)
-    return dict(locs=only(-((locs[others, 1:] - origin) @ R)), cos=only(np.cos(yaw)), sin=only(np.sin(yaw)),
-                bbox=only(bbox[others, 1:]), typ=only(typs[others, 1:]).astype(np.int32), present=present,
+    return dict(locs=only(-((locs[others, first:] - origin) @ R)), cos=only(np.cos(yaw)), sin=only(np.sin(yaw)),
+                bbox=only(bbox[others, first:]), typ=only(typs[others, first:]).astype(np.int32), present=present,
                 ego_bbox=bbox[e, 0].copy())
 
 
@@ -144,10 +145,26 @@ def _plan_safety_of(tracks, wanted, augmented):
     return _safety_table(tracks)
 
 
+def driving_score_table(env, index, T):
+    """The actors an ego plan of sample ``index`` is scored against by the driving score (lav_b200.evaluate, --driving-score):
+    plan_safety_table's actors, records and layout, at steps 0..T (frames index .. index + T), so that step 0 gives each actor's
+    pose before the plan's first step.  -> the dict of plan_safety_table with T + 1 steps per actor."""
+    return _safety_table(_read_tracks(env, index, T), first=0)
+
+
+def _driving_score_of(tracks, wanted, augmented):
+    """the driving_score_table of a prepared sample when ``wanted``; its label frame is the unaugmented one."""
+    if not wanted:
+        return None
+    if augmented:
+        raise LavbError("driving_score_table: the table is in the unaugmented label frame; the sample is rotated or shifted")
+    return _safety_table(tracks, first=0)
+
+
 def stage_plan_safety(tables, pin):
-    """the plan_safety_table of each sample of a batch packed for ops.plan_safety: actors = PLAN_SAFETY_ACTOR_DTYPE records as a
-    1-D uint8 tensor (sample i's rows, then within a row its steps), offsets (B+1,) int32 = the actor rows of each sample, ego_ext
-    (B,2) fp64; pinned on ``pin``."""
+    """the plan_safety_table (or driving_score_table) of each sample of a batch packed for ops.plan_safety (ops.driving_score):
+    actors = PLAN_SAFETY_ACTOR_DTYPE records as a 1-D uint8 tensor (sample i's rows, then within a row its steps), offsets (B+1,)
+    int32 = the actor rows of each sample, ego_ext (B,2) fp64; pinned on ``pin``."""
     T = tables[0]["locs"].shape[1] if tables else 0
     rec = np.zeros((sum(len(s["locs"]) for s in tables), T), ops.PLAN_SAFETY_ACTOR_DTYPE)
     offsets = np.concatenate([[0], np.cumsum([len(s["locs"]) for s in tables])]).astype(np.int32)
@@ -216,9 +233,9 @@ class TemporalLiDARPaintedDataset:
         return 0.0, [(np.zeros(2), 0.0)] * (self.num_frame_stack + 1)
 
     # ---- host part: record reads, PNG chunk walks, labels, BEV job rows
-    def prepare(self, idx, angle, jitters, plan_safety=False, cameras=False, paint=False):
+    def prepare(self, idx, angle, jitters, plan_safety=False, cameras=False, paint=False, driving_score=False):
         """the host record of sample ``idx``; with ``plan_safety`` (unaugmented samples only) it also holds the sample's
-        plan_safety_table, from the same record reads; with ``cameras``, under "cameras", what CameraDataset reads for the brake
+        plan_safety_table, from the same record reads, and with ``driving_score`` its driving_score_table; with ``cameras``, under "cameras", what CameraDataset reads for the brake
         model (read_cameras: the three middle cameras of camera_yaws and tel_rgb[:-crop_tel_bottom]).  With ``paint`` (online
         painting) no lidar_sem key is read: each sweep carries its frame index where the painted rows would be, and "traj" the
         trajectory, for stage_batch's frame table."""
@@ -231,6 +248,7 @@ class TemporalLiDARPaintedDataset:
         frames = [i for i in range(index, index - self.num_frame_stack - 1, -1) if i >= 0]
         tracks = _read_tracks(env, index, T)
         table = _plan_safety_of(tracks, plan_safety, angle != 0)
+        driving = _driving_score_of(tracks, driving_score, angle != 0)
         ego_locs, locs, oris, bbox, typs = _label_tracks(tracks, *radii)
         poses = {i: ego_pose(env, i) for i in frames}
         loc0, ori0 = poses[index]
@@ -265,6 +283,8 @@ class TemporalLiDARPaintedDataset:
                  locs=-p_locs, oris=p_oris, typs=p_typs, num_objs=n_obj)
         if table is not None:
             h["plan_safety"] = table
+        if driving is not None:
+            h["driving_score"] = driving
         if cams is not None:
             h["cameras"] = cams
         if paint:
@@ -405,6 +425,8 @@ class TemporalLiDARPaintedDataset:
                   labels={k: pinned(v) for k, v in labels.items()}, num_objs=[h["num_objs"] for h in hs])
         if hs and "plan_safety" in hs[0]:                                       # prepared with plan_safety (the evaluator)
             st["plan_safety"] = stage_plan_safety([h["plan_safety"] for h in hs], pin)
+        if hs and "driving_score" in hs[0]:                                     # prepared with driving_score (the evaluator)
+            st["driving_score"] = stage_plan_safety([h["driving_score"] for h in hs], pin)
         if hs and "cameras" in hs[0]:                                           # prepared with cameras (the brake evaluation)
             st["cameras"] = stage_images([h["cameras"] for h in hs], ("rgbs", "tel"), pin, "TemporalLiDARPaintedDataset")
         if painting is not None:
@@ -486,7 +508,8 @@ class TemporalBatchLoader:
     With ``ordered`` (evaluation) the samples come in index order with no augmentation, rank r taking the contiguous range
     [r * n // world, (r + 1) * n // world): every draw is dataset.no_draw(), and the LiDAR shuffles still come from the
     generator of (seed, epoch, rank).  With ``plan_safety`` (ordered only) every sample is
-    prepared with its plan_safety_table, and the staged tables carry them packed under "plan_safety" (stage_plan_safety).  With
+    prepared with its plan_safety_table, and the staged tables carry them packed under "plan_safety" (stage_plan_safety); with
+    ``driving_score`` (ordered only) the same with its driving_score_table, under "driving_score".  With
     ``cameras`` every sample is prepared with the brake model's camera images, and the staged tables carry them under "cameras"
     as one pinned uint8 buffer per key: rgbs (B, 3, h, w, 3), tel (B, h_tel, w_tel, 3).
 
@@ -496,19 +519,24 @@ class TemporalBatchLoader:
     launch_batch runs the model once over their images and lidar_batch_paint once; the staged tables carry them under "paint"."""
 
     def __init__(self, dataset, batch_size, seed=2021, rank=0, world=1, drop_last=True, num_workers=8, ordered=False,
-                 plan_safety=False, cameras=False, seg_model=None):
+                 plan_safety=False, cameras=False, seg_model=None, driving_score=False):
         self.ds, self.B, self.seed, self.rank, self.world, self.drop_last = dataset, batch_size, seed, rank, world, drop_last
         self.num_workers = max(1, int(num_workers))
         self.ordered = ordered
         self.plan_safety = plan_safety
+        self.driving_score = driving_score
         self.cameras = cameras
         self.seg_model = seg_model
         if plan_safety and not ordered:
             raise LavbError("plan_safety tables need the ordered, unaugmented loader")
+        if driving_score and not ordered:
+            raise LavbError("driving_score tables need the ordered, unaugmented loader")
         self.epoch = 0
 
     def _prepare(self, pool, idxs, draws):
         kw = dict(plan_safety=True) if self.plan_safety else {}
+        if self.driving_score:
+            kw["driving_score"] = True
         if self.cameras:
             kw["cameras"] = True
         if self.seg_model is not None:
@@ -609,14 +637,15 @@ class TemporalBEVDataset:
         return 0, 0.0
 
     # ---- host part: record reads, PNG chunk walks, labels, BEV job rows
-    def prepare(self, idx, offset, angle, plan_safety=False):
+    def prepare(self, idx, offset, angle, plan_safety=False, driving_score=False):
         """the host record of sample ``idx``; with ``plan_safety`` (unaugmented samples only) it also holds the sample's
-        plan_safety_table, from the same record reads."""
+        plan_safety_table, from the same record reads, and with ``driving_score`` its driving_score_table."""
         traj, index = self.index[idx]
         env = self.env(traj)
         T = self.num_plan
         tracks = _read_tracks(env, index, T)
         table = _plan_safety_of(tracks, plan_safety, offset != 0 or angle != 0)
+        driving = _driving_score_of(tracks, driving_score, offset != 0 or angle != 0)
         ego_locs, locs, oris, _, typs = _label_tracks(tracks, self.max_pedestrian_radius, self.max_vehicle_radius)
         frames = [i for i in range(index, index - self.num_frame_stack - 1, -1) if i >= 0]
         poses = {i: ego_pose(env, i) for i in frames}
@@ -650,6 +679,8 @@ class TemporalBEVDataset:
                  bra=int(_frame(env, "bra", index, np.uint8)[0]), locs=-p_locs, oris=p_oris, typs=p_typs, num_objs=n_obj)
         if table is not None:
             h["plan_safety"] = table
+        if driving is not None:
+            h["driving_score"] = driving
         return h
 
     def sample(self, idx, offset, angle):
@@ -671,7 +702,8 @@ class TemporalBEVBatchLoader(TemporalBatchLoader):
     decoded in one launch on a side stream, one batch ahead of the GPU.  A batch is the 9-tuple bev (B,9,320,320) uint8, ego_locs (B,T+1,2) f32, cmds (B,) int64, nxps (B,2) f32,
     bras (B,) int64, locs (B,max_objs,T+1,2) f32, oris (B,max_objs) f32, typs (B,max_objs) int32, num_objs (B,) int64 (host),
     with one bev_targets launch per batch.  With ``ordered`` (evaluation) the samples come in index order and every draw is
-    dataset.no_draw(); with ``plan_safety`` as well, every host record holds its plan_safety_table under "plan_safety"."""
+    dataset.no_draw(); with ``plan_safety`` as well, every host record holds its plan_safety_table under "plan_safety", and with
+    ``driving_score`` its driving_score_table under "driving_score"."""
 
     def _host_bev(self, idxs, draws, pool):
         hs = self._prepare(pool, idxs, draws)

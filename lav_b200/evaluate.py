@@ -5,7 +5,7 @@ against the expert's future — as numbers over every sample of the recording, t
     python -m lav_b200.evaluate --config-path config_v2.yaml --data-dir VALDIR --lidar-weights lidar_7.th \
         --uniplanner-weights uniplanner_7.th [--batch-size 32] [--precision f16|fp32] [--num-workers 16] [--json out.json] \
         [--forecast] [--forecast-detected] [--plan-safety] [--det-boxes] [--brake --bra-weights bra.th [--agent-config AGENT.yaml]] \
-        [--seg-weights seg_1.th]
+        [--seg-weights seg_1.th] [--driving-score [--step-seconds 0.25]]
     python -m lav_b200.evaluate ... --lidar-weights lidar_8.th lidar_16.th --uniplanner-weights uniplanner_8.th uniplanner_16.th
     python -m lav_b200.evaluate ... --run-dir RUN [--epochs 1,8,16-64]
     torchrun --nproc-per-node N -m lav_b200.evaluate ...
@@ -130,6 +130,60 @@ the batch's bev; no extra model call.  The protocol:
     class), vehicle_collision_rate, pedestrian_collision_rate, off_road_rate, collision_rate_by_step (T values: the share of
     samples whose first collision is at or before that step), and the summed off_map_steps and invalid_steps.  A rate over no
     sample is null.
+
+With --driving-score (``driving_score=True``, also lav_b200.evaluate_bev) the result also holds ``driving_score``: a PDM-style
+score of the same two trajectories, the open-loop stand-in for closed-loop driving that nuPlan and NAVSIM use, built from no
+at-fault collision (NC), drivable-area compliance (DAC), time to collision (TTC), ego progress (EP) and comfort (C), against the
+recorded, non-reactive traffic.  It ranks plans that plan ADE / FDE cannot: a plan that stops for a car that then runs into it
+from behind keeps NC, and a plan that never moves loses EP.  Per batch: one ops.driving_score launch and one copy of its result
+buffer; the actor table comes from the loader (datasets.driving_score_table, built only when asked), the road from the batch's
+bev; no extra model call.  It works with or without --plan-safety.  The protocol:
+
+  Trajectories, ego boxes, validity, actors, the collision test and the road rule are the plan-safety protocol's, unchanged
+    (the plan under the recorded command and the expert ego_locs[:, 1:]; step 0 is the origin with heading (0, -1), headings
+    carried over steps shorter than 0.1 m).  The actor table has one more step: step 0, the actors at the sample's own frame.
+  Step period.  dt = --step-seconds (``step_seconds``), default 0.25 s.  The recordings carry no timestamps, so the default is
+    inferred from the reference agent, not measured on a recording: the agent stacks sweeps GAP = NUM_REPEAT + 1 = 5 sensor
+    ticks apart (team_code_v2/lav_agent_fast.py:32-33,150,368), its sensor tick is 0.05 s (:44), and training stacks
+    consecutive recorded frames, so one recorded frame stands for 5 x 0.05 s.
+  Velocities, t = 1..T, fp64.  Ego v_t = (p_t - p_{t-1}) / dt; the ego is stopped at t when |v_t| < 0.05 m/s.  An actor's
+    velocity at t is (q_t - q_{t-1}) / dt from its step t - 1 and step t positions when it is present at both, else 0.
+  NC.  A collision with actor a is new at step t when the boxes overlap at t and did not at t - 1 (at t = 1 the origin box
+    against the actor's step-0 box; an actor absent at t - 1 did not overlap).  A new collision is not at fault when the ego is
+    stopped or it is a rear collision, (q_t - p_t) . h_t < -e1 (the actor's centre behind the ego's rear face); every other
+    new collision is at fault: front, lateral, or against a stopped actor.  nuPlan also exempts lateral collisions by the lanes
+    the two agents occupy; the recordings have no lanes, so every lateral collision here is at fault.  NC = 0 if any at-fault
+    collision with a vehicle or a pedestrian occurs, else 1.  An overlap already present at step 0 is never new.
+  DAC.  0 if any valid step is off-road under the plan-safety corner rule, else 1: per sample the plan-safety off-road verdict.
+  TTC.  At each step t where the ego is not stopped, every present actor that does not overlap the ego at t: both boxes are
+    moved at constant velocity, headings held, to t + k dt, k = 1..K, K = floor(1.0 s / dt + 1e-9) (4 at 0.25 s); the ego to
+    p_t + (k dt) v_t, the actor to q_t + (k dt) u_t.  The projected collision is judged at the first k whose boxes overlap,
+    where it would begin: the step violates TTC unless the projected actor's centre is behind the projected ego's rear face
+    there (the at-fault rule's rear exemption; the ego is moving).  TTC = 0
+    if any step violates it, else 1.
+  EP.  L = the arc length of the expert polyline, origin -> expert points, segment lengths summed in order; s = the arc-length
+    position of the plan's last point projected onto that polyline: on each segment the closest point (the projection
+    parameter clamped to [0, 1], 0 on a zero-length segment), the first segment of least distance, s = the segments before it +
+    the parameter x its length.  EP = clamp(s / L, 0, 1), 0 when s / L is not a number; EP = 1 when L < 5 m (NAVSIM's
+    minimum-progress rule).
+  C.  Finite differences at dt, with no smoothing: nuPlan first smooths the trajectory with a Savitzky-Golay filter, this score
+    does not, so a jagged plan fails more often than it would there; each term's failure rate is reported for that reason.
+    Speed |v_t| (t >= 1); yaw psi_t = atan2 of h_t; yaw differences wrapped to (-pi, pi].  Bounds (nuPlan's): longitudinal
+    acceleration (|v_t| - |v_{t-1}|) / dt in [-4.05, 2.40] m/s^2 (t >= 2); jerk, its difference / dt, |.| <= 4.13 m/s^3 (t >= 3);
+    yaw rate w_t = wrap(psi_t - psi_{t-1}) / dt, |.| <= 0.95 rad/s (t >= 2); yaw acceleration (w_t - w_{t-1}) / dt, |.| <= 1.93
+    rad/s^2 (t >= 3); lateral acceleration |v_t| w_t, |.| <= 4.89 m/s^2 (t >= 2).  C = 1 when every term stays within its bound.
+  Score.  PDMS = NC x DAC x (5 TTC + 5 EP + 2 C) / 12, NAVSIM's weights, so a trajectory that passes every term and makes
+    full progress scores 1.  A trajectory with an invalid step (a non-finite centre or heading)
+    scores 0 and is counted in ``invalid``; its terms are not computed and it is left out of the term rates.
+  Per sample and trajectory (ops.driving_score_views): the first at-fault and the first exempt collision (step, actor row,
+    class), the first TTC violation (step, row), the first off-road step, the comfort mask with each term's first failing step,
+    s and L in fp64, and the first invalid step.
+  Host reduction (DrivingScores), for plan and for expert, overall and per recorded command: samples, pdms (the mean over every
+    sample, invalid ones counting 0), over the valid samples the nc / dac / ttc / comfort pass rates, the mean ep and each
+    comfort term's failure rate, the samples with an at-fault and with an exempt collision, invalid, and step_seconds.  A rate
+    over no sample is null.
+  Not modelled: reactive agents (the recorded traffic does not respond to the plan), lane and driving-direction compliance,
+    static objects other than the recorded actors, smoothing, and lane-based at-fault logic for lateral collisions.
 
 With --det-boxes (``det_boxes=True``) the result also holds ``det_boxes``: the detections scored as boxes, by rotated-box IoU
 and by the position, size and heading errors of the detections matched at 2 m.  Per batch: one ops.det_box_eval launch on the
@@ -502,6 +556,8 @@ def format_det_boxes(r):
 
 
 PLAN_SAFETY_TRAJECTORIES = ("plan", "expert")
+DRIVING_SCORE_WEIGHTS = (5.0, 5.0, 2.0)      # TTC, EP and C in the PDMS (NAVSIM's), over their sum 12
+DRIVING_SCORE_MIN_LENGTH_M = 5.0             # an expert shorter than this gives EP 1
 
 
 def score_plan_safety(plan, ego_locs, table, bev, grid):
@@ -550,6 +606,102 @@ class PlanSafetyScores:
             r = res[:, j]
             out[name] = dict(rates(r), per_cmd={str(c): rates(r[cmd == c]) for c in sorted(set(cmd.tolist()))})
         return out
+
+
+def score_driving(plan, ego_locs, table, bev, grid, dt=ops.DRIVING_SCORE_STEP_S):
+    """one ops.driving_score launch over a batch's ego plans ``plan`` (B,T,2) and experts ego_locs[:, 1:], against the batch's
+    packed driving_score tables (stage_plan_safety, on the host) and the road plane of its ``bev``, at step period ``dt``.  -> the
+    result buffer on the device (ops.driving_score_views with n = 2), trajectory 0 the plan, 1 the expert."""
+    dev = bev.device
+    expert = ego_locs[:, 1:].float().contiguous()
+    traj = torch.stack([plan.float(), expert], 1).contiguous()
+    return ops.driving_score(traj, expert, table["actors"].to(dev, non_blocking=True), table["offsets"],
+                             table["ego_ext"].to(dev, non_blocking=True), bev, grid, dt)
+
+
+def driving_terms(v):
+    """the per-trajectory terms of driving_score_views ``v`` (numpy arrays): dict of invalid, nc, dac, ttc, comfort, at_fault,
+    exempt (bool), ep and pdms (fp64), and comfort_fail (..., 5) bool, one entry per ops.DRIVING_SCORE_COMFORT term."""
+    invalid = v["invalid_step"] > 0
+    nc, dac, ttc = v["fault_step"] < 0, v["off_road_step"] < 0, v["ttc_step"] < 0
+    mask = v["comfort_mask"]
+    comfort = mask == 0
+    s, length = v["progress"], v["length"]
+    with np.errstate(invalid="ignore", divide="ignore"):
+        ratio = s / length
+        ep = np.where(length < DRIVING_SCORE_MIN_LENGTH_M, 1.0, np.where(np.isnan(ratio), 0.0, np.clip(ratio, 0.0, 1.0)))
+    w_ttc, w_ep, w_c = DRIVING_SCORE_WEIGHTS
+    pdms = np.where(invalid, 0.0, nc * dac * (w_ttc * ttc + w_ep * ep + w_c * comfort) / (w_ttc + w_ep + w_c))
+    fail = np.stack([(mask >> q) & 1 for q in range(len(ops.DRIVING_SCORE_COMFORT))], -1) != 0
+    return dict(invalid=invalid, nc=nc, dac=dac, ttc=ttc, comfort=comfort, at_fault=~nc, exempt=v["exempt_step"] > 0, ep=ep,
+                pdms=pdms, comfort_fail=fail)
+
+
+class DrivingScores:
+    """host accumulation of score_driving results over a recording."""
+
+    def __init__(self, names=PLAN_SAFETY_TRAJECTORIES, dt=ops.DRIVING_SCORE_STEP_S):
+        self.names, self.dt = names, dt
+        self.res, self.ep, self.cmd = [], [], []
+
+    def add(self, buf, cmds):
+        """buf = a host copy of one batch's result buffer; cmds (B,) the recorded commands."""
+        b = len(cmds)
+        v = ops.driving_score_views(buf, b, len(self.names))
+        self.res.append(torch.stack([v[k] for k in ops.DRIVING_SCORE_FIELDS], -1).numpy().copy())
+        self.ep.append(torch.stack([v["progress"], v["length"]], -1).numpy().copy())
+        self.cmd.append(np.asarray(cmds, np.int64).reshape(-1))
+
+    def extend(self, other):
+        """append the records of ``other``, which follow this one's in sample order."""
+        self.res += other.res
+        self.ep += other.ep
+        self.cmd += other.cmd
+
+    def terms(self):
+        """driving_terms of every record, (samples, trajectories) each, and the recorded commands."""
+        n, f = len(self.names), len(ops.DRIVING_SCORE_FIELDS)
+        res = np.concatenate(self.res) if self.res else np.zeros((0, n, f), np.int32)
+        ep = np.concatenate(self.ep) if self.ep else np.zeros((0, n, 2))
+        v = {k: res[..., i] for i, k in enumerate(ops.DRIVING_SCORE_FIELDS)}
+        v["progress"], v["length"] = ep[..., 0], ep[..., 1]
+        return driving_terms(v), np.concatenate(self.cmd) if self.cmd else np.zeros(0, np.int64)
+
+    def summary(self):
+        """per trajectory: the score and its terms over all samples and per recorded command."""
+        d, cmd = self.terms()
+
+        def stats(m, j):
+            mean = lambda a: float(np.mean(a)) if len(a) else None
+            ok = m & ~d["invalid"][:, j]
+            fail = d["comfort_fail"][ok, j]
+            return dict(samples=int(m.sum()), pdms=mean(d["pdms"][m, j]), nc=mean(d["nc"][ok, j]), dac=mean(d["dac"][ok, j]),
+                        ttc=mean(d["ttc"][ok, j]), comfort=mean(d["comfort"][ok, j]), ep=mean(d["ep"][ok, j]),
+                        comfort_failure_rate={name: mean(fail[:, q]) for q, name in enumerate(ops.DRIVING_SCORE_COMFORT)},
+                        at_fault_collisions=int(d["at_fault"][ok, j].sum()), exempt_collisions=int(d["exempt"][ok, j].sum()),
+                        invalid=int(d["invalid"][m, j].sum()))
+
+        out = {}
+        every = np.ones(len(cmd), bool)
+        for j, name in enumerate(self.names):
+            out[name] = dict(stats(every, j), per_cmd={str(c): stats(cmd == c, j) for c in sorted(set(cmd.tolist()))})
+        out["step_seconds"] = self.dt
+        return out
+
+
+def format_driving_score(s):
+    """the printout lines of a DrivingScores summary."""
+    fmt = lambda v: "n/a" if v is None else f"{v:.4f}"
+    line = lambda d: (f"{d['samples']} samples, PDMS {fmt(d['pdms'])}: NC {fmt(d['nc'])}, DAC {fmt(d['dac'])}, TTC {fmt(d['ttc'])}, "
+                      f"EP {fmt(d['ep'])}, comfort {fmt(d['comfort'])}; {d['at_fault_collisions']} at-fault and "
+                      f"{d['exempt_collisions']} exempt collisions, {d['invalid']} invalid")
+    lines = []
+    for name in (k for k in s if k != "step_seconds"):
+        d = s[name]
+        lines.append(f"driving score, {name} (dt {s['step_seconds']:g} s): " + line(d))
+        lines.append("  comfort failures: " + ", ".join(f"{k} {fmt(v)}" for k, v in d["comfort_failure_rate"].items()))
+        lines += [f"  cmd {c}: " + line(e) for c, e in d["per_cmd"].items()]
+    return lines
 
 
 def format_plan_safety(s):
@@ -699,22 +851,25 @@ class PaintingCount:
 
 def evaluate(lidar_model, uniplanner, dataset, batch_size=32, precision="f16", num_workers=16, forecast=False,
              forecast_detected=False, plan_safety=False, det_boxes=False, brake=False, bra_model=None, agent_config=None,
-             seg_model=None):
+             seg_model=None, driving_score=False, step_seconds=ops.DRIVING_SCORE_STEP_S):
     """Scores of ``lidar_model`` and ``uniplanner`` over every sample of ``dataset`` (a TemporalLiDARPaintedDataset), the models
     run as the agent runs them at ``precision``; with ``forecast`` also the UniPlanner's forecast scores on the recorded poses,
     with ``forecast_detected`` those on the detected vehicles, with ``plan_safety`` the collision and off-road rates of the ego
     plan and of the expert, with ``det_boxes`` the detections' box scores, with ``brake`` the agent's brake decision with the
     brake model ``bra_model`` under the controls of ``agent_config`` (the agent's YAML dict; default the dataset's config); with
-    ``seg_model`` (an RGBSegmentationModel) the sweeps painted online by it instead of read from lidar_sem.
+    ``seg_model`` (an RGBSegmentationModel) the sweeps painted online by it instead of read from lidar_sem; with ``driving_score``
+    the driving score of the ego plan and of the expert at a step period of ``step_seconds``.
     -> dict (see the module docstring); None on a rank other than 0 of a process group."""
     results = evaluate_checkpoints([(lidar_model, uniplanner)], dataset, batch_size, precision, num_workers, forecast,
-                                   forecast_detected, plan_safety, det_boxes, brake, bra_model, agent_config, seg_model)
+                                   forecast_detected, plan_safety, det_boxes, brake, bra_model, agent_config, seg_model,
+                                   driving_score, step_seconds)
     return None if results is None else results[0]
 
 
 @torch.no_grad()
 def evaluate_checkpoints(pairs, dataset, batch_size=32, precision="f16", num_workers=16, forecast=False, forecast_detected=False,
-                         plan_safety=False, det_boxes=False, brake=False, bra_model=None, agent_config=None, seg_model=None):
+                         plan_safety=False, det_boxes=False, brake=False, bra_model=None, agent_config=None, seg_model=None,
+                         driving_score=False, step_seconds=ops.DRIVING_SCORE_STEP_S):
     """evaluate() of every (lidar_model, uniplanner) of ``pairs`` in one pass over ``dataset``: each batch is loaded and staged
     once, then every pair runs its own InferModel and scoring launches on it into its own accumulators.  All pairs stay
     resident; a sweep that would not fit on the device is refused before any data is loaded.  With ``brake`` the one brake
@@ -752,9 +907,9 @@ def evaluate_checkpoints(pairs, dataset, batch_size=32, precision="f16", num_wor
     grid = dict(min_x=dataset.min_x, max_x=dataset.max_x, min_y=dataset.min_y, max_y=dataset.max_y,
                 pixels_per_meter=dataset.pixels_per_meter)
     loader = TemporalBatchLoader(dataset, batch_size, rank=rank, world=world, drop_last=False, num_workers=num_workers, ordered=True,
-                                 plan_safety=plan_safety, cameras=brake, seg_model=seg_model)
+                                 plan_safety=plan_safety, cameras=brake, seg_model=seg_model, driving_score=driving_score)
     accs = [(Scores(), ForecastScores(), DetectedForecastScores(), PlanSafetyScores(), DetBoxScores(), BrakeScores(uni.num_cmds),
-             PaintingCount()) for _, uni in pairs]
+             PaintingCount(), DrivingScores(dt=step_seconds)) for _, uni in pairs]
     with math_mode(precision):
         for batch, staged in loader.staged_batches():
             actors = staged["actors"].to(dev, non_blocking=True)
@@ -767,18 +922,20 @@ def evaluate_checkpoints(pairs, dataset, batch_size=32, precision="f16", num_wor
                 pred_bra = brake_probs(bra, cams["rgbs"].to(dev, non_blocking=True), cams["tel"].to(dev, non_blocking=True))
                 brake_in = (pred_bra, expert_track_rows(batch[10], batch[6], batch[12], batch[13], num_cmds), ctl)
             for im, acc in zip(models, accs):
-                score_batch(im, batch, staged, actors, grid, acc, forecast, forecast_detected, plan_safety, det_boxes, brake_in)
+                score_batch(im, batch, staged, actors, grid, acc, forecast, forecast_detected, plan_safety, det_boxes, brake_in,
+                            step_seconds if driving_score else None)
     accs = gather_merged(accs)
     if accs is None:
         return None
     return [summarize(acc, precision, forecast, forecast_detected, plan_safety, dataset.num_plan, det_boxes, brake,
-                      seg_model is not None) for acc in accs]
+                      seg_model is not None, driving_score) for acc in accs]
 
 
-def summarize(acc, precision, forecast, forecast_detected, plan_safety, num_plan, det_boxes=False, brake=False, painting=False):
-    """the evaluate() result of one checkpoint's accumulators ``acc`` (score_batch's tuple, then its PaintingCount; its
-    DetBoxScores is read only with ``det_boxes``, its BrakeScores only with ``brake``, its PaintingCount only with
-    ``painting``)."""
+def summarize(acc, precision, forecast, forecast_detected, plan_safety, num_plan, det_boxes=False, brake=False, painting=False,
+              driving_score=False):
+    """the evaluate() result of one checkpoint's accumulators ``acc`` (score_batch's tuple, then its PaintingCount and its
+    DrivingScores; its DetBoxScores is read only with ``det_boxes``, its BrakeScores only with ``brake``, its PaintingCount only
+    with ``painting``, its DrivingScores only with ``driving_score``)."""
     scores, forecasts, detected, safety = acc[:4]
     result = scores.summary()
     result["precision"] = precision
@@ -794,14 +951,18 @@ def summarize(acc, precision, forecast, forecast_detected, plan_safety, num_plan
         result["brake"] = acc[5].summary()
     if painting:
         result["painting"] = acc[6].summary()
+    if driving_score:
+        result["driving_score"] = acc[7].summary()
     return result
 
 
-def score_batch(im, batch, staged, actors, grid, acc, forecast, forecast_detected, plan_safety, det_boxes=False, brake=None):
+def score_batch(im, batch, staged, actors, grid, acc, forecast, forecast_detected, plan_safety, det_boxes=False, brake=None,
+                driving_dt=None):
     """one checkpoint's InferModel ``im`` on one loader batch (its 14-tuple, staged tables and the actor table on the device),
-    scored into ``acc`` = (Scores, ForecastScores, DetectedForecastScores, PlanSafetyScores, DetBoxScores, BrakeScores); the
-    DetBoxScores is used only with ``det_boxes``, the BrakeScores only with ``brake`` = (the batch's brake probabilities, its
-    expert_track_rows, the capi.ControlConfig)."""
+    scored into ``acc`` = (Scores, ForecastScores, DetectedForecastScores, PlanSafetyScores, DetBoxScores, BrakeScores,
+    PaintingCount, DrivingScores); the DetBoxScores is used only with ``det_boxes``, the BrakeScores only with ``brake`` = (the
+    batch's brake probabilities, its expert_track_rows, the capi.ControlConfig), the DrivingScores only with a step period
+    ``driving_dt``."""
     scores, forecasts, detected, safety = acc[:4]
     dev = actors.device
     lidars, num_points, bev, ego_locs, cmds, nxps = batch[0], batch[1], batch[5], batch[6], batch[7], batch[8]
@@ -829,6 +990,17 @@ def score_batch(im, batch, staged, actors, grid, acc, forecast, forecast_detecte
         pred_bra, expert, ctl = brake
         res = score_brake(out, pred_bra, expert, host_cmds.astype(np.int32), ctl)
         acc[5].add(res.cpu().numpy(), host_cmds, staged["labels"]["bra"].numpy())
+    if driving_dt is not None:
+        res = score_driving(out["ego_plan_locs"], ego_locs, staged["driving_score"], bev, grid, driving_dt)
+        acc[7].add(res.cpu(), host_cmds)
+
+
+def add_driving_score_args(ap):
+    ap.add_argument("--driving-score", action="store_true",
+                    help="also score the ego plan and the expert with a PDM-style driving score: at-fault collisions, drivable "
+                         "area, time to collision, progress and comfort")
+    ap.add_argument("--step-seconds", type=float, default=ops.DRIVING_SCORE_STEP_S,
+                    help="with --driving-score: seconds between recorded frames (default %(default)s)")
 
 
 def parse_args(argv=None):
@@ -857,6 +1029,7 @@ def parse_args(argv=None):
     ap.add_argument("--seg-weights", default=None,
                     help="paint every stacked sweep online with this RGBSegmentationModel state_dict (seg_1.th) instead of "
                          "reading the recording's lidar_sem")
+    add_driving_score_args(ap)
     args = ap.parse_args(argv)
     if args.brake and args.bra_weights is None:
         ap.error("--brake needs --bra-weights")
@@ -888,6 +1061,8 @@ def format_result(r):
         lines += format_brake(r["brake"])
     if "painting" in r:
         lines.append(f"painted online: {r['painting']['frames']} frames, {r['painting']['images']} images segmented")
+    if "driving_score" in r:
+        lines += format_driving_score(r["driving_score"])
     return "\n".join(lines)
 
 
@@ -908,6 +1083,8 @@ def headline(r):
     if "brake" in r:
         agent = r["brake"]["verdicts"]["agent"]
         cols += [("false brake", agent["false_brake_rate"]), ("missed brake", agent["missed_brake_rate"])]
+    if "driving_score" in r:
+        cols.append(("PDMS", r["driving_score"]["plan"]["pdms"]))
     return cols
 
 
@@ -955,7 +1132,8 @@ def main(argv=None):
         seg.load_state_dict(torch.load(args.seg_weights, map_location="cpu"))
     ds = TemporalLiDARPaintedDataset(args.config_path, device=dev, overrides=dict(data_dir=args.data_dir))
     results = evaluate_checkpoints(pairs, ds, args.batch_size, args.precision, args.num_workers, args.forecast,
-                                   args.forecast_detected, args.plan_safety, args.det_boxes, args.brake, bra, agent_cfg, seg)
+                                   args.forecast_detected, args.plan_safety, args.det_boxes, args.brake, bra, agent_cfg, seg,
+                                   args.driving_score, args.step_seconds)
     out = None
     if results is not None:
         text, out = report(checkpoints, results, rank_and_world()[1])

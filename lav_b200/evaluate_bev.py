@@ -2,7 +2,7 @@
 recorded vehicles and of the ego, its command scores and its ego plan, under the protocol of lav_b200.evaluate --forecast.
 
     python -m lav_b200.evaluate_bev --config-path config_v2.yaml --data-dir VALDIR --bev-weights bev_7.th [--batch-size 64] \
-        [--num-workers 16] [--json out.json] [--plan-safety]
+        [--num-workers 16] [--json out.json] [--plan-safety] [--driving-score [--step-seconds 0.25]]
     python -m lav_b200.evaluate_bev ... --bev-weights bev_40.th bev_80.th bev_160.th
     python -m lav_b200.evaluate_bev ... --run-dir RUN [--epochs 40-160]
     torchrun --nproc-per-node N -m lav_b200.evaluate_bev ...
@@ -13,7 +13,9 @@ ops.forecast_eval launch scores the vehicle rows, the ego casts and the ego plan
 result buffer.  The result is dict(samples, forecast) with ``forecast`` as ForecastScores.summary(plan=True) gives it; a student
 UniPlanner scored by lav_b200.evaluate --forecast on the same recording is comparable row for row.  With --plan-safety the result
 also holds ``plan_safety``: the recorded command's branch of the ego plan and the expert, checked against the recorded traffic and
-the road plane by one ops.plan_safety launch per batch, under lav_b200.evaluate's plan-safety protocol.
+the road plane by one ops.plan_safety launch per batch, under lav_b200.evaluate's plan-safety protocol.  With --driving-score it
+holds ``driving_score``: the same two trajectories scored by one ops.driving_score launch per batch, under lav_b200.evaluate's
+driving-score protocol.
 
 Sweeps of several planners (paths, or train_bev's bev_{e}.th found by --run-dir) and torchrun ranks work as in
 lav_b200.evaluate (lav_b200.eval_sweep): each batch is loaded once for every planner, and rank 0 merges the ranks' records.
@@ -28,7 +30,8 @@ from .agent import math_mode
 from .datasets import TemporalBEVBatchLoader, TemporalBEVDataset, stage_plan_safety
 from .eval_sweep import (ResidentMeter, add_checkpoint_args, check_sweep_fits, eval_device, gather_merged, init_ranks,
                          rank_and_world, select_checkpoints, sweep_json, sweep_table)
-from .evaluate import ForecastScores, PlanSafetyScores, format_forecast, format_plan_safety, score_forecasts, score_plan_safety
+from .evaluate import (DrivingScores, ForecastScores, PlanSafetyScores, add_driving_score_args, format_driving_score, format_forecast,
+                       format_plan_safety, score_driving, score_forecasts, score_plan_safety)
 
 
 def recorded_branch(ego_plan, cmds):
@@ -40,16 +43,19 @@ def recorded_branch(ego_plan, cmds):
     return torch.where(ok[:, None, None], picked, torch.full_like(picked, float("nan")))
 
 
-def evaluate_bev(bev_planner, dataset, batch_size=64, num_workers=16, plan_safety=False):
+def evaluate_bev(bev_planner, dataset, batch_size=64, num_workers=16, plan_safety=False, driving_score=False,
+                 step_seconds=ops.DRIVING_SCORE_STEP_S):
     """Forecast scores of ``bev_planner`` over every sample of ``dataset`` (a TemporalBEVDataset); with ``plan_safety`` also the
-    collision and off-road rates of its ego plan and of the expert.  -> dict(samples, forecast[, plan_safety]); None on a rank
-    other than 0 of a process group."""
-    results = evaluate_bev_checkpoints([bev_planner], dataset, batch_size, num_workers, plan_safety)
+    collision and off-road rates of its ego plan and of the expert, with ``driving_score`` their driving score at a step period
+    of ``step_seconds``.  -> dict(samples, forecast[, plan_safety][, driving_score]); None on a rank other than 0 of a process
+    group."""
+    results = evaluate_bev_checkpoints([bev_planner], dataset, batch_size, num_workers, plan_safety, driving_score, step_seconds)
     return None if results is None else results[0]
 
 
 @torch.no_grad()
-def evaluate_bev_checkpoints(planners, dataset, batch_size=64, num_workers=16, plan_safety=False):
+def evaluate_bev_checkpoints(planners, dataset, batch_size=64, num_workers=16, plan_safety=False, driving_score=False,
+                             step_seconds=ops.DRIVING_SCORE_STEP_S):
     """evaluate_bev() of every BEVPlanner of ``planners`` in one pass over ``dataset``: each batch is loaded once, then every
     planner runs forecast_recorded and its scoring launches on it into its own accumulators.  All planners stay resident; a
     sweep that would not fit on the device is refused before any data is loaded.  In a process group each rank scores its
@@ -63,33 +69,40 @@ def evaluate_bev_checkpoints(planners, dataset, batch_size=64, num_workers=16, p
         if meter is not None:
             check_sweep_fits(len(planners), meter.resident(), meter.available, batch_size, "BEV planners")
     loader = TemporalBEVBatchLoader(dataset, batch_size, rank=rank, world=world, drop_last=False, num_workers=num_workers,
-                                    ordered=True, plan_safety=plan_safety)
-    accs = [(ForecastScores(plan=True), PlanSafetyScores()) for _ in planners]
+                                    ordered=True, plan_safety=plan_safety, driving_score=driving_score)
+    accs = [(ForecastScores(plan=True), PlanSafetyScores(), DrivingScores(dt=step_seconds)) for _ in planners]
     grid = dict(min_x=dataset.min_x, max_x=dataset.max_x, min_y=dataset.min_y, max_y=dataset.max_y,
                 pixels_per_meter=dataset.pixels_per_meter)
     with math_mode("fp32"):
         for (bev, ego_locs, cmds, nxps, _, locs, oris, typs, _), hs in loader.staged_batches():
             host_cmds = [h["cmd"] for h in hs]
             table = stage_plan_safety([h["plan_safety"] for h in hs], dev.type == "cuda") if plan_safety else None
-            for planner, (scores, safety) in zip(planners, accs):
+            driving = stage_plan_safety([h["driving_score"] for h in hs], dev.type == "cuda") if driving_score else None
+            for planner, (scores, safety, drive) in zip(planners, accs):
                 fc = planner.forecast_recorded(bev, ego_locs, locs, oris, typs, nxps)
                 k, b = fc["cast"].shape[0], len(hs)
                 scores.add(ops.forecast_views(score_forecasts(fc, cmds, plan=True).cpu(), k + 2 * b), k, host_cmds)
                 if plan_safety:
                     res = score_plan_safety(recorded_branch(fc["ego_plan"], cmds), ego_locs, table, bev, grid)
                     safety.add(res.cpu().numpy(), host_cmds)
+                if driving_score:
+                    res = score_driving(recorded_branch(fc["ego_plan"], cmds), ego_locs, driving, bev, grid, step_seconds)
+                    drive.add(res.cpu(), host_cmds)
     accs = gather_merged(accs)
     if accs is None:
         return None
-    return [summarize(acc, len(dataset), plan_safety, dataset.num_plan) for acc in accs]
+    return [summarize(acc, len(dataset), plan_safety, dataset.num_plan, driving_score) for acc in accs]
 
 
-def summarize(acc, samples, plan_safety, num_plan):
-    """the evaluate_bev() result of one planner's accumulators ``acc`` = (ForecastScores, PlanSafetyScores)."""
-    scores, safety = acc
+def summarize(acc, samples, plan_safety, num_plan, driving_score=False):
+    """the evaluate_bev() result of one planner's accumulators ``acc`` = (ForecastScores, PlanSafetyScores[, DrivingScores]); the
+    DrivingScores is read only with ``driving_score``."""
+    scores, safety = acc[:2]
     result = dict(samples=samples, forecast=scores.summary())
     if plan_safety:
         result["plan_safety"] = safety.summary(num_plan)
+    if driving_score:
+        result["driving_score"] = acc[2].summary()
     return result
 
 
@@ -103,12 +116,14 @@ def parse_args(argv=None):
     ap.add_argument("--json", default=None, help="also write the result here")
     ap.add_argument("--plan-safety", action="store_true",
                     help="also score the ego plan and the expert for collisions with the recorded traffic and for leaving the road")
+    add_driving_score_args(ap)
     return ap.parse_args(argv)
 
 
 def format_result(r):
     return "\n".join([f"{r['samples']} samples"] + format_forecast(r["forecast"]) +
-                     (format_plan_safety(r["plan_safety"]) if "plan_safety" in r else []))
+                     (format_plan_safety(r["plan_safety"]) if "plan_safety" in r else []) +
+                     (format_driving_score(r["driving_score"]) if "driving_score" in r else []))
 
 
 def headline(r):
@@ -118,6 +133,8 @@ def headline(r):
             ("cmd acc", f["ego_cast"]["cmd_accuracy"]), ("plan ADE", f["ego_plan"]["ade"]), ("plan FDE", f["ego_plan"]["fde"])]
     if "plan_safety" in r:
         cols += [("collision", r["plan_safety"]["plan"]["collision_rate"]), ("off-road", r["plan_safety"]["plan"]["off_road_rate"])]
+    if "driving_score" in r:
+        cols.append(("PDMS", r["driving_score"]["plan"]["pdms"]))
     return cols
 
 
@@ -147,7 +164,8 @@ def main(argv=None):
         planner.load_state_dict(torch.load(paths["bev"], map_location="cpu"))
         planners.append(planner)
     ds = TemporalBEVDataset(args.config_path, device=dev, overrides=dict(data_dir=args.data_dir))
-    results = evaluate_bev_checkpoints(planners, ds, args.batch_size, args.num_workers, args.plan_safety)
+    results = evaluate_bev_checkpoints(planners, ds, args.batch_size, args.num_workers, args.plan_safety, args.driving_score,
+                                       args.step_seconds)
     out = None
     if results is not None:
         text, out = report(checkpoints, results, rank_and_world()[1])

@@ -947,6 +947,56 @@ def plan_safety(traj, actors, offsets, ego_ext, bev, grid=None, out=None):
     return out
 
 
+DRIVING_SCORE_STEP_S = 0.25       # default step period of the recordings (lav_b200.evaluate's driving-score protocol)
+DRIVING_SCORE_COMFORT = ("lon_acceleration", "lon_jerk", "yaw_rate", "yaw_acceleration", "lat_acceleration")
+DRIVING_SCORE_FIELDS = ("fault_step", "fault_row", "fault_class", "exempt_step", "exempt_row", "exempt_class", "ttc_step", "ttc_row",
+                        "off_road_step", "comfort_mask") + tuple(f"{c}_step" for c in DRIVING_SCORE_COMFORT) + ("invalid_step",)
+
+
+def _driving_parts(b, n):     # 8-byte part first
+    return [("ep", torch.float64, (b, n, 2)), ("res", torch.int32, (b, n, len(DRIVING_SCORE_FIELDS)))]
+
+
+def driving_score_views(buf, b, n):
+    """the named parts of a driving_score result buffer of b samples and n trajectories (on the device or a host copy), each
+    (b, n): fault_step / fault_row / fault_class = the first at-fault collision's step (1..T), actor row and class; exempt_* the
+    same for the first exempt collision; ttc_step / ttc_row = the first time-to-collision violation; off_road_step; comfort_mask =
+    bit q set when DRIVING_SCORE_COMFORT[q] fails, {term}_step its first failing step; invalid_step = the first invalid step;
+    -1 for none.  progress / length (fp64) = the arc-length position s of the last point on the expert polyline and its length L."""
+    v = _views(buf, _driving_parts(b, n))
+    out = {name: v["res"][..., i] for i, name in enumerate(DRIVING_SCORE_FIELDS)}
+    out["progress"], out["length"] = v["ep"][..., 0], v["ep"][..., 1]
+    return out
+
+
+def driving_score(traj, expert, actors, offsets, ego_ext, bev, grid=None, dt=DRIVING_SCORE_STEP_S, out=None):
+    """The driving-score terms of n ego trajectories per sample in one launch (see lavb_driving_score in include/lav_b200.h).
+    traj (B,n,T,2) fp32 in the label frame; expert (B,T,2) fp32 = the polyline progress is measured along; actors =
+    PLAN_SAFETY_ACTOR_DTYPE records as a 1-D uint8 tensor on the device, T + 1 per actor row (steps 0..T), sample i owning rows
+    [offsets[i], offsets[i+1]) (offsets (B+1,) int32 on the HOST); ego_ext (B,2) fp64; bev (B,P,H,W) uint8, plane 0 the road; grid:
+    the keyword arguments of det_grid; dt the step period in seconds.  -> the uint8 result buffer (written into ``out`` when
+    given), read through driving_score_views, usually after one copy to the host."""
+    b, n, t, _ = _tensor("driving_score", "traj", traj, torch.float32, (None, None, None, 2))
+    dev = traj.device
+    _tensor("driving_score", "expert", expert, torch.float32, (b, t, 2), dev)
+    offsets = _host("driving_score", "offsets", offsets, np.int32, (b + 1,))
+    rec = PLAN_SAFETY_ACTOR_DTYPE.itemsize * (t + 1)
+    _tensor("driving_score", "actors", actors, torch.uint8, (None,), dev)
+    _require(actors.numel() % rec == 0, f"driving_score: actors must hold {t + 1} 56-byte records per actor row, got {actors.numel()} bytes")
+    _tensor("driving_score", "ego_ext", ego_ext, torch.float64, (b, 2), dev)
+    _, _, h, w = _tensor("driving_score", "bev", bev, torch.uint8, (b, None, None, None), dev)
+    _require(isinstance(dt, (int, float)) and math.isfinite(dt) and dt > 0, f"driving_score: dt must be a finite period > 0, got {dt!r}")
+    parts = _driving_parts(b, n)
+    out = _out("driving_score", "out", out, torch.uint8, (_layout(parts)[1],), dev)
+    _apart("driving_score", "out", out, traj=traj, expert=expert, actors=actors, ego_ext=ego_ext, bev=bev)
+    v = _views(out, parts)
+    _, _, (ppm, cx0, cy0, cy1, _) = det_grid(**(grid or {}))
+    _launch("lavb_driving_score", _ptr(traj), _ptr(expert), b, n, t, _ptr(actors), actors.numel() // rec, _hptr(offsets), _ptr(ego_ext),
+            _ptr(bev), bev[0].numel() if b else h * w, h, w, ppm, cx0, cy0, cy1, float(dt), _ptr(v["ep"]), _ptr(v["res"]),
+            launches=-(-b // 512))
+    return out
+
+
 def agent_control_state_bytes(turn_n, speed_n):
     """bytes of one agent's controller state (lavb_agent_control_state_bytes); all-zero bytes are a new route."""
     n = int(lib().lavb_agent_control_state_bytes(int(turn_n), int(speed_n)))
