@@ -835,10 +835,34 @@ int lavb_convert(const void* d_src, int src_dtype, void* d_dst, int dst_dtype, l
 /* ---------------------------------------------------------------- wgmma implicit-GEMM tap-list convolution
  * replaces (h16 path): the Conv2d -> ReLU -> BatchNorm2d layers of ConvBackbone (lidar.py:57-131), the fused 4-head
  *           384->256 conv (lidar.py:152-154) and the 64/128-channel factorised convs of ERFNet (erfnet.py:31-61).
- * Same descriptor and epilogue semantics as lavb_conv_taps, with these differences: input is h16 NHWC, cin % 64 == 0,
- * cout % 32 == 0 and <= 256, channel offsets/strides multiples of 8; d->w points to h16 weights laid out
- * [ntaps][cout][cin] (K contiguous).  Tiles are 8 x 16 output-grid pixels; operands are fetched by TMA
- * (cuTensorMapEncodeTiled through cudaGetDriverEntryPoint), accumulators live in registers. */
+ * The descriptor, tap sum and epilogue steps of lavb_conv_taps, with these differences: input and weights are h16 (in NHWC,
+ * d->w h16 [ntaps][cout_mma][cin], K contiguous, cout_mma = cout rounded up to 32; rows past cout are never stored, whatever
+ * they hold); a residual is h16 even with fp32 output; cin % 64 == 0, cout % 8 == 0 and <= 256, channel offsets and strides
+ * multiples of 8; in_s <= 8; with d2s_nout the output is addressed by the depth-to-space rule below, not by out_cstride /
+ * out_coff.  Tiles are 8 x 16 output-grid pixels; operands are fetched by TMA (cuTensorMapEncodeTiled through
+ * cudaGetDriverEntryPoint), accumulators live in registers.
+ * Arithmetic: the products of h16 operands are exact in fp32 and accumulate in fp32 on the tensor cores in an unspecified
+ *   order (lavb_conv3x3_umma states where its order is this kernel's).  The epilogue then runs in fp32, in order: with
+ *   pre_relu, a = fmaxf(a + bias, 0) and a = fmaf(a, scale, shift); without it the bias folds into the shift,
+ *   a = fmaf(a, scale, fmaf(bias, scale, shift)) (a missing bias is 0, missing scale / shift 1 / 0); a += res; post_relu:
+ *   a = fmaxf(a, 0); sigmoid: 1 / (1 + expf(-a)); h16 output: one saturating rounding (cvt.rn.satfinite).
+ * NaN / inf: a ReLU is fmaxf(a, 0) and turns a NaN into 0; without a ReLU a NaN stays NaN through every step; an infinity
+ *   follows IEEE fp32 arithmetic; h16 stores saturate at +-65504 and keep NaN.
+ * Written: the channels [out_coff, out_coff + cout) of the output pixels (oy*out_sy+out_oy, ox*out_sx+out_ox) with oy < hog,
+ *   ox < wog that fall inside hout x wout, for the n images; nothing else.  d2s_nout: each lattice pixel's four positions
+ *   (oy + pos/2, ox + pos%2), each clipped to hout x wout on its own, channels [0, d2s_nout) of the fp32 [n][hout][wout][d2s_nout]
+ *   output.
+ * Checked before any launch (a rejected call writes nothing): 1 <= ntaps <= 16; in_dtype h16, out_dtype fp32 or h16; cin a
+ *   positive multiple of 64; 8 <= cout <= 256, a multiple of 8, and of 32 with a residual; 0 <= in_coff, in_coff + cin <=
+ *   in_cstride; 0 <= out_coff, out_coff + cout <= out_cstride; with a residual res_dtype h16, 0 <= res_coff, res_coff + cout
+ *   <= res_cstride; every channel offset and stride a multiple of 8; scale and shift both or neither; n, hog, wog, hin, win,
+ *   hout, wout >= 1; 1 <= in_sy, in_sx <= 8, out_sy, out_sx >= 1, out_oy, out_ox >= 0; (hog - 1) * out_sy + out_oy and the
+ *   same along x below 2^31, and fewer than 2^31 tiles; in, out and w non-null; in, out, w and res 16-byte aligned, bias /
+ *   scale / shift 4-byte aligned; out not overlapping in or w (the whole extents the descriptor gives them), and out not
+ *   overlapping res unless out IS res element for element (same pointer, h16 output, equal channel stride and offset: each
+ *   thread reads a residual pair before it stores the same output pair); d2s_nout: 1 <= d2s_nout <= 8, cout 32, fp32
+ *   output, out_s 2, no residual.
+ * Not checked: that the buffers hold the extents the descriptor describes. */
 int lavb_conv_umma(const lavb_conv_desc* h_desc, void* stream);
 
 /* ---------------------------------------------------------------- planner embedder stem
@@ -846,7 +870,13 @@ int lavb_conv_umma(const lavb_conv_desc* h_desc, void* stream);
  * (team_code_v2/models/uniplanner.py:36-40, lav/models/resnet.py:178,235-238) on the h16 path.  d_in: h16 NHWC (n, h, w, cin),
  * cin % 64 == 0, h, w >= 7; d_w: BatchNorm-folded h16 weights laid out [49 taps (ky*7 + kx)][64 cout][cin]; d_bias: fp32 [64];
  * d_out: h16 NHWC (n, (h-1)/2+1, (w-1)/2+1, 64) = relu(conv + bias), saturating.  wgmma implicit GEMM with output channels
- * in M and 16 x 16 output-pixel tiles in N; operands fetched by TMA, whose out-of-bounds zero fill is the padding. */
+ * in M and 16 x 16 output-pixel tiles in N; operands fetched by TMA, whose out-of-bounds zero fill is the padding.
+ * Arithmetic, NaN / inf: lavb_conv3x3_umma's with pre_relu and no scale / shift: fp32 accumulation of exact products in an
+ *   unspecified order, then fmaxf(a + bias, 0) (a NaN becomes 0) and the saturating h16 store.  Written: every element of
+ *   d_out, nothing else.
+ * Checked before any launch (a rejected call writes nothing): non-null d_in, d_w, d_bias, d_out; n >= 0 (0 writes nothing),
+ *   h, w >= 7; cin a positive multiple of 64; d_in, d_w, d_out 16-byte aligned, d_bias 4-byte aligned; d_out not overlapping
+ *   d_in, d_w or d_bias; fewer than 2^31 tiles. */
 int lavb_conv7x7s2_umma(const void* d_in, int n, int h, int w, int cin, const void* d_w, const float* d_bias, void* d_out,
                         void* stream);
 
@@ -861,7 +891,14 @@ int lavb_conv7x7s2_umma(const void* d_in, int n, int h, int w, int cin, const vo
  *          out = max(conv + bias, 0) * scale + shift with pre_relu, (conv + bias) * scale + shift without it; d_bias,
  *          d_scale / d_shift (fp32 [cout]) may be NULL (0, 1 / 0; scale and shift come together).  The fp32 operations are
  *          those of lavb_conv_umma's epilogue; with cin <= 128 at stride 1, and cin = 64 at stride 2, the MMA order is too, so
- *          the output equals lavb_conv_umma's bit for bit. */
+ *          the output equals lavb_conv_umma's bit for bit.
+ * Arithmetic: h16 products exact in fp32, fp32 accumulation in an unspecified order except where the bit-equality above is
+ *   stated; then the epilogue's fp32 operations in lavb_conv_umma's order and the saturating h16 store.
+ * NaN / inf: the pre-ReLU is fmaxf(a, 0) and turns a NaN into 0; without it a NaN stays NaN (stored as an h16 NaN); h16 stores
+ *   saturate at +-65504.  Written: every element of d_out, nothing else.
+ * Checked before any launch (a rejected call writes nothing): non-null d_in, d_w, d_out; n >= 0 (0 writes nothing), h, w >= 1;
+ *   stride, cin, cout as above; scale and shift both or neither; d_in, d_w, d_out 16-byte aligned, bias / scale / shift
+ *   4-byte aligned; d_out not overlapping d_in, d_w, bias, scale or shift; fewer than 2^31 tiles. */
 int lavb_conv3x3_umma(const void* d_in, int n, int h, int w, int cin, int stride, const void* d_w, int cout, const float* d_bias,
                       const float* d_scale, const float* d_shift, int pre_relu, void* d_out, void* stream);
 
@@ -870,11 +907,18 @@ int lavb_conv3x3_umma(const void* d_in, int n, int h, int w, int cin, int stride
  * one wgmma kernel; the intermediate activation stays in shared memory.
  *   mid = relu(conv3x1_dil(in) + bias1);  out = [relu](conv1x3_dil(mid) + shift2 [+ res])
  * The BatchNorm affine (conv + b2) * s + t is folded by the caller: w2 <- w2 * s per output channel, shift2 <- b2 * s + t.
- * bias1 / shift2 (fp32 [c]) are added to the register accumulators in the epilogues, which then pack, clamp and add the residual
- * (16-bit packed arithmetic: the residual add rounds once more than an fp32 add would, and its sum saturates at +-65504).
+ * Arithmetic: h16 products exact in fp32 with fp32 accumulation in an unspecified order; mid = the h16 rounding (saturating)
+ * of acc1 + bias1, then fmaxf(mid, 0); acc2 + shift2 (shift2 NULL: 0) is rounded to h16 (saturating); the residual is added in
+ * packed 16-bit arithmetic (one more rounding than an fp32 add would make), and the sum saturates at +-65504 (bf16 build: at
+ * bf16's largest finite value).
+ * NaN / inf: every ReLU is max(a, 0) with a NaN turned into 0, with or without the residual; without post_relu a NaN stays NaN
+ * through the residual add.  Written: every element of out, nothing else.
  * in / out / res: h16 NHWC (n, h, w, c) contiguous, c in {64, 128}, w in {32, 64, 128}; w1 / w2: h16 [3 taps][c out][c in];
- * res may be NULL.  out must not overlap in or res (rejected): the kernel reads a tile's residual while earlier tiles are
- * still being stored. */
+ * res may be NULL.
+ * Checked before any launch (a rejected call writes nothing): c in {64, 128}; w in {32, 64, 128}; 1 <= dil < w; n >= 0 (0
+ * writes nothing), h >= 1; non-null in, out, w1, w2, bias1; bias1 / shift2 4-byte aligned; in, out, res, w1, w2 16-byte
+ * aligned (their tensor maps refuse anything else); out not overlapping in or res: the kernel reads a tile's residual while
+ * earlier tiles are still being stored; fewer than 2^31 tiles. */
 typedef struct lavb_conv_pair_desc {
   const void* in; void* out; const void* res;
   int n, h, w, c, dil, post_relu;

@@ -10,7 +10,7 @@
 //               shifted by +d, 0, -d pixels inside each image row (rows that fall off the image border stay zero), i.e. the
 //               three A operands of the horizontal taps
 //   stage 2: wgmma over the 3 horizontal taps (A = those copies, B = W2 blocks through the same TMA ring)
-//   epilogue 2: acc2 + shift2 -> h16 (+ residual, ReLU as one packed fma.relu), written in place over the residual tile in a
+//   epilogue 2: acc2 + shift2 -> h16 (+ residual, saturating) -> ReLU = max(a, 0) with NaN -> 0, written in place over the residual tile in a
 //               ring slot and stored to NHWC by one TMA store per 64 channels.  The BatchNorm scale is folded into W2 by the caller.
 // Warp roles: warps 0-3 and 4-7 are two consumer warpgroups (tile pixels 0-63 / 64-127), warp 8 is the TMA producer; persistent
 // over tiles.  Ring order per tile: stage-1 fills (A + W1), stage-2 fills (W2 only), then the tile's output slot, which the
@@ -43,20 +43,25 @@ struct PairArgs {
 
 using namespace sm90;
 
+// ReLU as fmaxf(a, 0): __hmax2 returns the operand that is not NaN, so a NaN comes out as 0
+__device__ __forceinline__ h162 relu2(h162 v) { return __hmax2(v, floats2h162(0.f, 0.f)); }
 __device__ __forceinline__ uint32_t relu2(uint32_t x) {
-  const h162 v = __hmax2(*reinterpret_cast<const h162*>(&x), floats2h162(0.f, 0.f));
+  const h162 v = relu2(*reinterpret_cast<const h162*>(&x));
   return *reinterpret_cast<const uint32_t*>(&v);
 }
-// residual add in packed h16 arithmetic.  A packed add rounds a sum past the finite range to inf, so the sum is clamped to
-// +-65504 afterwards: the same saturating store as every cvt.rn.satfinite in the library (in-range sums are unchanged).
+// residual add in packed 16-bit arithmetic.  A packed add rounds a sum past the finite range to inf, so the sum is clamped to
+// the largest finite value (+-65504; +-bf16's maximum in the bf16 build) afterwards: the same saturating store as every
+// cvt.rn.satfinite in the library (in-range sums are unchanged).  The clamp keeps a NaN (the _nan forms), and the ReLU then
+// turns it into 0, so the residual paths follow the same NaN rule as the residual-free ones.
 __device__ __forceinline__ uint32_t add2(uint32_t x, uint32_t r, bool relu) {
   const h162 a = *reinterpret_cast<const h162*>(&x), b = *reinterpret_cast<const h162*>(&r);
-  h162 v = relu ? __hfma2_relu(a, floats2h162(1.f, 1.f), b) : __hadd2(a, b);
 #ifndef LAVB_H16_BF16
   const uint32_t hi = 0x7BFF7BFFu, lo = 0xFBFFFBFFu;           // +65504 / -65504 in both halves
-  v = __hmin2(v, *reinterpret_cast<const h162*>(&hi));
-  if (!relu) v = __hmax2(v, *reinterpret_cast<const h162*>(&lo));
+#else
+  const uint32_t hi = 0x7F7F7F7Fu, lo = 0xFF7FFF7Fu;           // +-bf16's largest finite value in both halves
 #endif
+  h162 v = __hmin2_nan(__hadd2(a, b), *reinterpret_cast<const h162*>(&hi));
+  v = relu ? relu2(v) : __hmax2_nan(v, *reinterpret_cast<const h162*>(&lo));
   return *reinterpret_cast<const uint32_t*>(&v);
 }
 
@@ -280,6 +285,9 @@ extern "C" int lavb_conv_pair_umma(const lavb_conv_pair_desc* d, void* stream) {
   LAVB_CHECK_ARG(d->dil >= 1 && d->dil < d->w, "conv_pair_umma: dilation must be in [1, width)");
   LAVB_CHECK_ARG(d->n >= 0 && d->h >= 1, "conv_pair_umma: bad shape");
   LAVB_CHECK_ARG(d->w1 && d->w2 && d->bias1 && d->in && d->out, "conv_pair_umma: null operand");
+  LAVB_CHECK_ARG((long long)d->n * ceil_div(d->h, kBlockM / d->w) < (1LL << 31), "conv_pair_umma: more than 2^31 tiles");
+  LAVB_CHECK_ARG(reinterpret_cast<uintptr_t>(d->bias1) % 4 == 0 && reinterpret_cast<uintptr_t>(d->shift2) % 4 == 0,
+                 "conv_pair_umma: bias1 and shift2 must be 4 B aligned");
   {  // the residual tile is prefetched while earlier tiles are stored: `out` must not overlap `in` or `res`
     const size_t bytes = (size_t)d->n * d->h * d->w * d->c * 2;
     const auto overlap = [&](const void* x) {

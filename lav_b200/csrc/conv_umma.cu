@@ -63,7 +63,7 @@ __global__ void __launch_bounds__(kConvThreads, kNC <= 4 ? 2 : 1) conv_umma_kern
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   for (int c = threadIdx.x; c < kN; c += blockDim.x) {
-    // epi(a) = max(a + b, lo) * s + t.  Without the pre-ReLU the bias folds into the shift: (a + b) s + t = a s + (b s + t)
+    // epi(a) = max(a + b, 0) * s + t with the pre-ReLU.  Without it the bias folds into the shift: (a + b) s + t = a s + (b s + t)
     const bool real = c < p.cout_store;      // columns past cout_store are MMA padding (never stored)
     const float b = (p.bias && real) ? __ldg(p.bias + c) : 0.f;
     const float sc = (p.scale && real) ? __ldg(p.scale + c) : 1.f;
@@ -98,7 +98,6 @@ __global__ void __launch_bounds__(kConvThreads, kNC <= 4 ? 2 : 1) conv_umma_kern
   }
 
   const int wg = warp >> 2;                        // tile rows [64 wg, 64 wg + 64)
-  const float lo_pre = p.pre_relu ? 0.f : -INFINITY, lo_post = p.post_relu ? 0.f : -INFINITY;
   int stage = 0; uint32_t phase = 0;
   float acc[16 * kNC];                             // 32-column chunk c: acc[16c .. 16c+15]
   for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
@@ -144,13 +143,15 @@ __global__ void __launch_bounds__(kConvThreads, kNC <= 4 ? 2 : 1) conv_umma_kern
         float x0 = acc[4 * j + 2 * h], x1 = acc[4 * j + 2 * h + 1];
         if (p.pre_bias) { x0 += bias_at[g]; x1 += bias_at[g + 1]; }
         const float4 st = *reinterpret_cast<const float4*>(st_at + 2 * g);   // (s0, t0, s1, t1)
-        x0 = fmaf(fmaxf(x0, lo_pre), st.x, st.y);
-        x1 = fmaf(fmaxf(x1, lo_pre), st.z, st.w);
+        // each max only when its flag is set, as in conv_taps.cu: fmaxf(NaN, -inf) would turn a NaN into -inf
+        if (p.pre_relu) { x0 = fmaxf(x0, 0.f); x1 = fmaxf(x1, 0.f); }
+        x0 = fmaf(x0, st.x, st.y);
+        x1 = fmaf(x1, st.z, st.w);
         if (res_at) {
           const float2 rv = unpack_h16(__ldg(reinterpret_cast<const uint32_t*>(res_at + g)));
           x0 += rv.x; x1 += rv.y;
         }
-        x0 = fmaxf(x0, lo_post); x1 = fmaxf(x1, lo_post);
+        if (p.post_relu) { x0 = fmaxf(x0, 0.f); x1 = fmaxf(x1, 0.f); }
         if (p.sigmoid) { x0 = 1.f / (1.f + expf(-x0)); x1 = 1.f / (1.f + expf(-x1)); }
         if (kNC == 1 && p.d2s_nout) {   // depth-to-space (cout 32 only): column q = pos*nout + k -> pixel (oy + pos/2, ox + pos%2), channel k
           float* ob = reinterpret_cast<float*>(p.out);
@@ -160,7 +161,9 @@ __global__ void __launch_bounds__(kConvThreads, kNC <= 4 ? 2 : 1) conv_umma_kern
             const int q = g + c0 + e;
             if (q < 4 * no) {
               const int pos = q / no, k = q - pos * no;
-              ob[(pix + (long long)(pos >> 1) * p.wout + (pos & 1)) * no + k] = e ? x1 : x0;
+              // each of the four pixels is clipped to hout x wout on its own (oy < hout, ox < wout hold already)
+              if (oy + (pos >> 1) < p.hout && ox + (pos & 1) < p.wout)
+                ob[(pix + (long long)(pos >> 1) * p.wout + (pos & 1)) * no + k] = e ? x1 : x0;
             }
           }
         } else if (g < store_lim) {                  // g + c0 < cout_store
@@ -187,11 +190,41 @@ extern "C" int lavb_conv_umma(const lavb_conv_desc* d, void* stream) {
   LAVB_CHECK_ARG(d->cout % 8 == 0 && d->cout >= 8 && d->cout <= 256, "conv_umma: cout must be 8..256, multiple of 8 (got %d)", d->cout);
   const int cout_mma = (d->cout + 31) / 32 * 32;      // MMA width; d->w holds cout_mma rows per tap (zero rows past cout)
   LAVB_CHECK_ARG(d->res == nullptr || cout_mma == d->cout, "conv_umma: residual needs cout %% 32 == 0");
-  LAVB_CHECK_ARG(d->in_cstride % 8 == 0 && d->in_coff % 8 == 0 && d->in_coff + d->cin <= d->in_cstride, "conv_umma: input slice misaligned");
-  LAVB_CHECK_ARG(d->out_cstride % 8 == 0 && d->out_coff % 8 == 0 && d->out_coff + d->cout <= d->out_cstride, "conv_umma: output slice misaligned");
-  LAVB_CHECK_ARG(d->res == nullptr || (d->res_dtype == LAVB_H16 && d->res_cstride % 8 == 0 && d->res_coff % 8 == 0), "conv_umma: residual must be h16, 16 B aligned");
+  LAVB_CHECK_ARG(d->in_cstride % 8 == 0 && d->in_coff % 8 == 0 && d->in_coff >= 0 && d->in_coff + d->cin <= d->in_cstride,
+                 "conv_umma: input slice misaligned or out of range");
+  LAVB_CHECK_ARG(d->out_cstride % 8 == 0 && d->out_coff % 8 == 0 && d->out_coff >= 0 && d->out_coff + d->cout <= d->out_cstride,
+                 "conv_umma: output slice misaligned or out of range");
+  LAVB_CHECK_ARG(d->res == nullptr || (d->res_dtype == LAVB_H16 && d->res_cstride % 8 == 0 && d->res_coff % 8 == 0 && d->res_coff >= 0 &&
+                                       d->res_coff + d->cout <= d->res_cstride),
+                 "conv_umma: residual must be h16, its slice 16 B aligned and inside res_cstride");
   LAVB_CHECK_ARG((d->scale == nullptr) == (d->shift == nullptr), "conv_umma: scale and shift come together");
+  LAVB_CHECK_ARG(d->n >= 1 && d->hog >= 1 && d->wog >= 1, "conv_umma: empty problem");
+  LAVB_CHECK_ARG(d->hin >= 1 && d->win >= 1 && d->hout >= 1 && d->wout >= 1, "conv_umma: map sizes must be >= 1");
   LAVB_CHECK_ARG(d->in_sy >= 1 && d->in_sy <= 8 && d->in_sx >= 1 && d->in_sx <= 8, "conv_umma: bad input stride");
+  LAVB_CHECK_ARG(d->out_sy >= 1 && d->out_sx >= 1 && d->out_oy >= 0 && d->out_ox >= 0, "conv_umma: bad output stride or offset");
+  // the output lattice's coordinates and the tile count are ints in the kernel
+  LAVB_CHECK_ARG((long long)(d->hog - 1) * d->out_sy + d->out_oy < (1LL << 31) && (long long)(d->wog - 1) * d->out_sx + d->out_ox < (1LL << 31),
+                 "conv_umma: output lattice past 2^31");
+  LAVB_CHECK_ARG((long long)d->n * ceil_div(d->hog, kTileH) * ceil_div(d->wog, kTileW) < (1LL << 31), "conv_umma: more than 2^31 tiles");
+  LAVB_CHECK_ARG(d->in != nullptr && d->out != nullptr && d->w != nullptr, "conv_umma: null in / out / w");
+  // TMA reads in and w; the epilogue stores up to 8 B (fp32 pairs) and reads 4 B residual pairs and 4 B bias / scale / shift
+  const auto al = [](const void* q, int a) { return reinterpret_cast<uintptr_t>(q) % a == 0; };
+  LAVB_CHECK_ARG(al(d->in, 16) && al(d->out, 16) && al(d->w, 16) && al(d->res, 16), "conv_umma: in, out, w and res must be 16 B aligned");
+  LAVB_CHECK_ARG(al(d->bias, 4) && al(d->scale, 4) && al(d->shift, 4), "conv_umma: bias, scale and shift must be 4 B aligned");
+  {  // every tile reads in and w while others store: out must not overlap them.  out may be res itself, element for element
+     // (each thread reads a residual pair before it stores the same output pair); any other overlap with res is refused
+    const long long px = (long long)d->n * d->hout * d->wout;
+    const long long out_bytes = px * (d->d2s_nout ? 4LL * d->d2s_nout : (long long)d->out_cstride * (d->out_dtype == LAVB_F32 ? 4 : 2));
+    const auto overlap = [&](const void* q, long long bytes) {
+      const char *o = static_cast<const char*>(d->out), *c = static_cast<const char*>(q);
+      return q && o < c + bytes && c < o + out_bytes;
+    };
+    LAVB_CHECK_ARG(!overlap(d->in, (long long)d->n * d->hin * d->win * d->in_cstride * 2) &&
+                   !overlap(d->w, (long long)d->ntaps * ((d->cout + 31) / 32 * 32) * d->cin * 2),
+                   "conv_umma: out must not overlap in or w");
+    const bool same = d->res == d->out && d->out_dtype == LAVB_H16 && d->res_cstride == d->out_cstride && d->res_coff == d->out_coff;
+    LAVB_CHECK_ARG(same || !overlap(d->res, px * d->res_cstride * 2), "conv_umma: out may only overlap res element for element");
+  }
   auto encode = get_encode();
   LAVB_CHECK_ARG(encode != nullptr, "conv_umma: cuTensorMapEncodeTiled not available from the driver");
 

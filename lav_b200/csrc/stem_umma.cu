@@ -30,7 +30,7 @@
 //   more channels run as CTA columns of CO channels each (the 256-channel heads conv: two), adjacent in the tile order so
 //   that both columns of a tile read its input window from L2 at about the same time.
 // Warp roles (288 threads, 1 CTA per SM, persistent over tiles):
-//   warps 0-7: two consumer warpgroups; one K-block of MMAs in flight; epilogue max(acc [+ b], lo) * s + t -> h16 (conv_umma's
+//   warps 0-7: two consumer warpgroups; one K-block of MMAs in flight; epilogue [max](acc [+ b], 0) * s + t -> h16 (conv_umma's
 //              fp32 operations and saturating conversion), transposed through shared memory (the accumulator holds
 //              D[cout][pixel], NHWC wants the channels of a pixel contiguous) -> 16 B stores
 //   warp 8   : TMA producer (one lane): a pixel ring of kPStages slots of one kernel row's boxes (SC chunks) and a weight ring of
@@ -72,7 +72,7 @@ struct Cfg {
 struct Args {
   int ho, wo, cout, kchunks, tiles_x, tiles_per_img, ncol, num_tiles;
   int pre_bias;           // bias added before the ReLU (else folded into the shift)
-  float lo_pre;           // 0 with the pre-ReLU, -inf without
+  int pre_relu;           // max(a [+ b], 0) before the affine (fmaxf: a NaN becomes 0); without it a NaN stays NaN
   float shift0;           // the shift where none is given
   h16* out;
   const float* bias; const float* scale; const float* shift;
@@ -106,7 +106,7 @@ __global__ void __launch_bounds__(kThreads, 1) conv_cmajor_kernel(const __grid_c
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   for (int c = threadIdx.x; c < p.cout; c += blockDim.x) {
-    // epi(a) = max(a + b, lo) * s + t.  Without the pre-ReLU the bias folds into the shift: (a + b) s + t = a s + (b s + t)
+    // epi(a) = max(a + b, 0) * s + t with the pre-ReLU.  Without it the bias folds into the shift: (a + b) s + t = a s + (b s + t)
     const float b = p.bias ? __ldg(p.bias + c) : 0.f;
     const float sc = p.scale ? __ldg(p.scale + c) : 1.f;
     const float sh = p.shift ? __ldg(p.shift + c) : p.shift0;
@@ -197,7 +197,7 @@ __global__ void __launch_bounds__(kThreads, 1) conv_cmajor_kernel(const __grid_c
       mbar_arrive(p_empty + 8 * (ps ? ps - 1 : kPStages - 1));
     }
 
-    // ---- epilogue: max(acc [+ b], lo) * s + t -> h16 -> [pixel][64 cout] in shared memory -> 16 B NHWC stores, 64 pixels
+    // ---- epilogue: [max](acc [+ b], 0) * s + t -> h16 -> [pixel][64 cout] in shared memory -> 16 B NHWC stores, 64 pixels
     // per pass.  acc[4 i + 2 h + e] = D[co + 8 h][8 i + 2 (lane % 4) + e]
     const int col = tile % p.ncol, sp = tile / p.ncol;
     const int img = sp / p.tiles_per_img, r = sp - img * p.tiles_per_img;
@@ -217,8 +217,9 @@ __global__ void __launch_bounds__(kThreads, 1) conv_cmajor_kernel(const __grid_c
           uint8_t* row = ep + px * kEpiPitch;
           float x0 = acc[4 * i + e], x1 = acc[4 * i + 2 + e];
           if (p.pre_bias) { x0 += b0; x1 += b1; }
-          x0 = fmaf(fmaxf(x0, p.lo_pre), s0, t0);
-          x1 = fmaf(fmaxf(x1, p.lo_pre), s1, t1);
+          if (p.pre_relu) { x0 = fmaxf(x0, 0.f); x1 = fmaxf(x1, 0.f); }   // only when set: fmaxf(NaN, -inf) would be -inf
+          x0 = fmaf(x0, s0, t0);
+          x1 = fmaf(x1, s1, t1);
           *reinterpret_cast<h16*>(row + 2 * co) = float2h16(x0);
           *reinterpret_cast<h16*>(row + 2 * (co + 8)) = float2h16(x1);
         }
@@ -274,6 +275,26 @@ static int launch(const CUtensorMap& tmap_x, const CUtensorMap& tmap_w, const Ar
   return 0;
 }
 
+// The checks both entries make once their sizes are valid: alignment (TMA reads d_in / d_w, the epilogue stores d_out in 16 B
+// vectors and reads bias / scale / shift as floats), d_out apart from every operand (each CTA reads them while others store),
+// and the tile count, an int in the kernel.
+static int check_operands(const char* who, const void* d_in, int n, int h, int w, int cin, int taps, const void* d_w, int cout,
+                          const float* bias, const float* scale, const float* shift, const void* d_out, int ho, int wo, int co) {
+  const auto al = [](const void* q, int a) { return reinterpret_cast<uintptr_t>(q) % a == 0; };
+  LAVB_CHECK_ARG(al(d_in, 16) && al(d_w, 16) && al(d_out, 16), "%s: d_in, d_w and d_out must be 16 B aligned", who);
+  LAVB_CHECK_ARG(al(bias, 4) && al(scale, 4) && al(shift, 4), "%s: bias, scale and shift must be 4 B aligned", who);
+  LAVB_CHECK_ARG((long long)n * ceil_div(ho, kTile) * ceil_div(wo, kTile) * (cout / co) < (1LL << 31), "%s: more than 2^31 tiles", who);
+  const long long out_bytes = (long long)n * ho * wo * cout * 2;
+  const auto overlap = [&](const void* q, long long bytes) {
+    const char *o = static_cast<const char*>(d_out), *c = static_cast<const char*>(q);
+    return q && o < c + bytes && c < o + out_bytes;
+  };
+  LAVB_CHECK_ARG(!overlap(d_in, (long long)n * h * w * cin * 2) && !overlap(d_w, (long long)taps * cout * cin * 2) &&
+                 !overlap(bias, 4LL * cout) && !overlap(scale, 4LL * cout) && !overlap(shift, 4LL * cout),
+                 "%s: d_out must not overlap d_in, d_w, bias, scale or shift", who);
+  return 0;
+}
+
 static void tiles(Args& a, int n, int ho, int wo, int cout, int co) {
   a.ho = ho; a.wo = wo; a.cout = cout; a.ncol = cout / co;
   a.tiles_x = ceil_div(wo, kTile);
@@ -293,6 +314,8 @@ extern "C" int lavb_conv7x7s2_umma(const void* d_in, int n, int h, int w, int ci
   LAVB_CHECK_ARG(n >= 0 && h >= 7 && w >= 7, "conv7x7s2_umma: bad shape n=%d h=%d w=%d (h, w >= 7)", n, h, w);
   LAVB_CHECK_ARG(cin > 0 && cin % 64 == 0, "conv7x7s2_umma: cin must be a multiple of 64 (got %d)", cin);
   if (n == 0) return 0;
+  if (int e = check_operands("conv7x7s2_umma", d_in, n, h, w, cin, 49, d_w, 64, d_bias, nullptr, nullptr, d_out, (h - 1) / 2 + 1,
+                             (w - 1) / 2 + 1, 64)) return e;
   CUtensorMap tmap_x, tmap_w;
   if (int e = encode_maps("conv7x7s2_umma", d_in, n, h, w, cin, 7, 2, d_w, 64, 64, &tmap_x, &tmap_w)) return e;
   Args a;
@@ -300,7 +323,7 @@ extern "C" int lavb_conv7x7s2_umma(const void* d_in, int n, int h, int w, int ci
   tiles(a, n, (h - 1) / 2 + 1, (w - 1) / 2 + 1, 64, 64);
   a.kchunks = cin / kBlockK;
   // relu(acc + b) as max(acc + b, 0) * 1 + (-0): adding -0 leaves every value, a -0 from fmaxf included, as it is
-  a.pre_bias = 1; a.lo_pre = 0.f; a.shift0 = -0.f;
+  a.pre_bias = 1; a.pre_relu = 1; a.shift0 = -0.f;
   a.out = reinterpret_cast<h16*>(d_out); a.bias = d_bias;
   return launch<7, 2, 64, 1>(tmap_x, tmap_w, a, stream);
 }
@@ -316,6 +339,8 @@ extern "C" int lavb_conv3x3_umma(const void* d_in, int n, int h, int w, int cin,
   LAVB_CHECK_ARG((d_scale == nullptr) == (d_shift == nullptr), "conv3x3_umma: scale and shift come together");
   if (n == 0) return 0;
   const int co = cout == 64 ? 64 : 128;
+  if (int e = check_operands("conv3x3_umma", d_in, n, h, w, cin, 9, d_w, cout, d_bias, d_scale, d_shift, d_out, (h - 1) / stride + 1,
+                             (w - 1) / stride + 1, co)) return e;
   CUtensorMap tmap_x, tmap_w;
   if (int e = encode_maps("conv3x3_umma", d_in, n, h, w, cin, 3, stride, d_w, cout, co, &tmap_x, &tmap_w)) return e;
   Args a;
@@ -323,7 +348,7 @@ extern "C" int lavb_conv3x3_umma(const void* d_in, int n, int h, int w, int cin,
   tiles(a, n, (h - 1) / stride + 1, (w - 1) / stride + 1, cout, co);
   a.kchunks = cin / kBlockK;
   a.pre_bias = pre_relu && d_bias != nullptr;
-  a.lo_pre = pre_relu ? 0.f : -INFINITY;
+  a.pre_relu = pre_relu != 0;
   a.shift0 = 0.f;
   a.out = reinterpret_cast<h16*>(d_out); a.bias = d_bias; a.scale = d_scale; a.shift = d_shift;
   // cin = 128 at stride 1: both chunks of a kernel row per pixel slot (tap-major K, as conv_umma_kernel); otherwise chunk-major

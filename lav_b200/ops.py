@@ -1227,7 +1227,7 @@ def conv_pair_umma(x, w1, bias1, w2, shift2, dil, res=None, post_relu=True, out=
     _tensor("conv_pair_umma", "w1", w1, h16(), (3, c, c))
     _tensor("conv_pair_umma", "w2", w2, h16(), (3, c, c))
     for name, v in (("bias1", bias1), ("shift2", shift2)):
-        _tensor("conv_pair_umma", name, v, torch.float32, None, contiguous=False)
+        _tensor("conv_pair_umma", name, v, torch.float32, None)
         _require(v.numel() == c, f"conv_pair_umma: {name} must hold {c} values, got {v.numel()}")
     out = _out("conv_pair_umma", "out", out, h16(), x.shape, x.device)
     d = ConvPairDesc()

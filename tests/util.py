@@ -864,3 +864,290 @@ def cast_case(n, ncmd, steps, scale, rows=None):
 # (n, ncmd, steps, scale) cases of the GPU test at which the CPU test shows every mutant far outside CAST_TOL; the last is the
 # frame path at the benchmark's batch: 2 pipelines x 32 agents, 3 detected vehicles each -> 96 + 32 rows, 20 steps
 CAST_MUTANT_CASES = {"product": (37, 7, 20, "product"), "saturating": (37, 7, 20, "saturating"), "frame_path": (128, 6, 20, "planner")}
+
+
+# ----------------------------------------------------------------------------------------------------- wgmma convolutions
+# fp64 statements of lavb_conv_umma, lavb_conv3x3_umma, lavb_conv7x7s2_umma and lavb_conv_pair_umma (include/lav_b200.h) on
+# the operands as the kernels read them, tied to F.conv2d / F.conv_transpose2d by tests/test_wgmma_ref_cpu.py and held against
+# the kernels by tests/test_gpu_wgmma_contract.py.  The tolerances are max-norm errors as a fraction of the output scale (the
+# largest finite |expected|), bounds the kernels must meet: fp32 output, h16 output, the pair (two h16 roundings and a packed
+# h16 residual add).
+WGMMA_TOL = {"f32": 2e-5, "h16": 1e-3, "pair": 1e-2}
+WGMMA_MUTANTS = ("k_chunk_dropped", "tap_shifted", "phase_out_o_swapped", "bias_after_pre_relu", "res_slice_off8", "nan_to_neg_inf")
+
+
+def fmax0(a):
+    """fmaxf(a, 0.f): a NaN comes out as 0 (torch.relu would keep it)"""
+    return torch.where(torch.isnan(a), torch.zeros_like(a), a.clamp_min(0))
+
+
+def tap_conv64(x, taps, w, in_s, hog, wog, mutant=None):
+    """the tap sum of the wgmma convolutions in float64: x (n, H, W, cin) (the channel slice the kernel reads), taps [(dy, dx)],
+    w (ntaps, cout, cin), in_s (sy, sx) -> (n, hog, wog, cout) with
+    acc[n, oy, ox, co] = sum_t sum_ci x[n, oy*sy + dy_t, ox*sx + dx_t, ci] w[t, co, ci]   (zero outside the input).
+    NaN rule: an output whose receptive field (the pixels its taps read) holds a NaN is NaN, whatever the weights; that set is
+    computed from the NaN mask apart from the sum, so that the fp64 algorithm cannot spread a NaN.  Infinities enter the
+    sum as they are (one infinite pixel reaches an output through one tap, so the sum is +-inf, never inf - inf).
+    mutant "k_chunk_dropped": the last 64-channel chunk of every tap left out; "tap_shifted": tap 0 reads one pixel to the
+    right."""
+    n, H, W, cin = x.shape
+    sy, sx = in_s
+    dev = x.device
+    nan_px = torch.isnan(x).any(-1)
+    xz = torch.where(torch.isnan(x), torch.zeros_like(x), x)
+    if mutant == "k_chunk_dropped":
+        xz = xz.clone()
+        xz[..., cin - 64:] = 0
+    acc = torch.zeros((n, hog, wog, w.shape[1]), dtype=torch.float64, device=dev)
+    hit = torch.zeros((n, hog, wog), dtype=torch.bool, device=dev)
+    for t, (dy, dx) in enumerate(taps):
+        if mutant == "tap_shifted" and t == 0:
+            dx += 1
+        ry = torch.arange(hog, device=dev) * sy + dy
+        rx = torch.arange(wog, device=dev) * sx + dx
+        oky, okx = (ry >= 0) & (ry < H), (rx >= 0) & (rx < W)
+        ok = oky[:, None] & okx[None, :]
+        g = xz[:, ry.clamp(0, H - 1)][:, :, rx.clamp(0, W - 1)]
+        g = torch.where(ok[None, :, :, None], g, torch.zeros_like(g))
+        acc += torch.einsum("nhwc,oc->nhwo", g, w[t].double().to(dev))
+        hit |= nan_px[:, ry.clamp(0, H - 1)][:, :, rx.clamp(0, W - 1)] & ok[None]
+    return torch.where(hit[..., None], torch.full_like(acc, math.nan), acc)
+
+
+def wgmma_epilogue64(a, bias=None, scale=None, shift=None, res=None, pre=False, post=False, sig=False, mutant=None):
+    """the epilogue of lavb_conv_umma / lavb_conv3x3_umma in float64: a += bias; pre: fmax0; a * scale + shift; a += res; post:
+    fmax0; sigmoid.  A missing operand skips its step.  mutant "bias_after_pre_relu": fmax0(a) + bias; "nan_to_neg_inf": each
+    ReLU that is off is fmaxf(a, -inf), which turns a NaN into -inf (the rule before it was fixed)."""
+    ninf = torch.full_like(a, -math.inf)
+    if mutant == "nan_to_neg_inf" and not pre:
+        a = torch.where(torch.isnan(a), ninf, a)
+    if bias is not None and mutant != "bias_after_pre_relu":
+        a = a + bias.double().to(a.device)
+    if pre:
+        a = fmax0(a)
+    if bias is not None and mutant == "bias_after_pre_relu":
+        a = a + bias.double().to(a.device)
+    if scale is not None:
+        a = a * scale.double().to(a.device) + shift.double().to(a.device)
+    if res is not None:
+        a = a + res.double().to(a.device)
+    if mutant == "nan_to_neg_inf" and not post:
+        a = torch.where(torch.isnan(a), ninf, a)
+    if post:
+        a = fmax0(a)
+    if sig:
+        a = torch.sigmoid(a)
+    return a
+
+
+def store64(v, out):
+    """the output store: "f32" keeps the value (fp32 NaN / inf as they are); "h16" saturates at +-65504 and keeps NaN.  The
+    statement is not rounded further: the tolerances cover the roundings."""
+    return v.clamp(-65504, 65504) if out == "h16" else v
+
+
+def convT_phases(wt, k=3, s=2, p=1):
+    """ConvTranspose2d(k, stride s, padding p) with weight wt (cin, cout, k, k) as s * s output phases, the way
+    lav_b200/layers.py issues it: [(out_o, taps, w (ntaps, cout, cin))], phase (py, px) writing pixels (s oy + py, s ox + px)"""
+    phases = []
+    for py in range(s):
+        for px in range(s):
+            taps, blocks = [], []
+            for ky in range(k):
+                if (py + p - ky) % s:
+                    continue
+                for kx in range(k):
+                    if (px + p - kx) % s:
+                        continue
+                    taps.append(((py + p - ky) // s, (px + p - kx) // s))
+                    blocks.append(wt[:, :, ky, kx].t())
+            phases.append(((py, px), taps, torch.stack(blocks)))
+    return phases
+
+
+def convT_assemble64(x, phases, hout, wout, epi, mutant=None):
+    """every phase's tap sum and epilogue placed on its lattice of an (n, hout, wout, cout) float64 map (the pixels of
+    hout x wout that the phase's lattice reaches; a phase is called on the input's h x w grid).  mutant
+    "phase_out_o_swapped": phases (0, 1) and (1, 0) write each other's lattice."""
+    n, h, w, _ = x.shape
+    out = torch.zeros((n, hout, wout, phases[0][2].shape[1]), dtype=torch.float64, device=x.device)
+    for (py, px), taps, wp in phases:
+        if mutant == "phase_out_o_swapped" and (py, px) in ((0, 1), (1, 0)):
+            py, px = px, py
+        v = epi(tap_conv64(x, taps, wp, (1, 1), h, w))
+        ly, lx = len(range(py, hout, 2)), len(range(px, wout, 2))
+        out[:, py::2, px::2] = v[:, :ly, :lx]
+    return out
+
+
+def d2s_scatter64(v, no, hout, wout, out_o=(0, 0)):
+    """the depth-to-space store: v (n, hog, wog, 32) columns q = pos * no + k -> pixel (2 gy + oy0 + pos // 2, 2 gx + ox0 +
+    pos % 2), channel k, each position clipped to hout x wout -> (values, written mask), both (n, hout, wout, no)"""
+    n, hog, wog, _ = v.shape
+    out = torch.zeros((n, hout, wout, no), dtype=torch.float64, device=v.device)
+    written = torch.zeros(out.shape, dtype=torch.bool, device=v.device)
+    for pos in range(4):
+        y0, x0 = out_o[0] + pos // 2, out_o[1] + pos % 2
+        ys, xs = list(range(y0, hout, 2))[:hog], list(range(x0, wout, 2))[:wog]
+        if ys and xs:
+            blk = v[:, :len(ys), :len(xs), pos * no:(pos + 1) * no]
+            out[:, y0:y0 + 2 * len(ys):2, x0:x0 + 2 * len(xs):2] = blk
+            written[:, y0:y0 + 2 * len(ys):2, x0:x0 + 2 * len(xs):2] = True
+    return out, written
+
+
+def pair_ref64(x, w1, b1, w2, t2, dil, res=None, relu=True, h16=torch.float16):
+    """lavb_conv_pair_umma in float64: x (n, h, w, c) 16-bit values, w1 / w2 (3, c, c) [tap][cout][cin] -> (n, h, w, c).
+    mid = fmax0(h16(conv3x1_dil(x) + b1)); a = h16(conv1x3_dil(mid) + shift2); with a residual h16(a + res) saturating;
+    relu: fmax0.  The NaN rule is tap_conv64's, and every ReLU turns a NaN into 0."""
+    rnd = lambda v: v.clamp(-65504, 65504).to(h16).double() if h16 == torch.float16 else v.to(h16).double()  # noqa: E731
+    a = tap_conv64(x, [((t - 1) * dil, 0) for t in range(3)], w1, (1, 1), x.shape[1], x.shape[2])
+    mid = fmax0(rnd(a + b1.double().to(x.device)))
+    a = rnd(tap_conv64(mid, [(0, (t - 1) * dil) for t in range(3)], w2, (1, 1), x.shape[1], x.shape[2]) + t2.double().to(x.device))
+    if res is not None:
+        a = rnd(a + res.double())
+    return fmax0(a) if relu else a
+
+
+def wgmma_err(got, want):
+    """max |got - want| over the finite expected values as a fraction of their largest magnitude, after the NaN pattern,
+    every infinite expected value and every saturated h16 one (+-65504) are matched exactly (inf when they are not)"""
+    g, w = got.double().to(want.device), want
+    if not torch.equal(torch.isnan(g), torch.isnan(w)):
+        return math.inf
+    inf = torch.isinf(w) | (w.abs() == 65504)          # infinities, and h16 stores the statement saturates: exact
+    if not torch.equal(g[inf], w[inf]):
+        return math.inf
+    fin = ~inf & ~torch.isnan(w)
+    if not bool(fin.any()):
+        return 0.0
+    if not bool(torch.isfinite(g[fin]).all()):
+        return math.inf
+    return float((g - w)[fin].abs().max() / (w[fin].abs().max() or 1.0))
+
+
+def _taps(k, pad, dil=1):
+    kh, kw = (k, k) if isinstance(k, int) else k
+    ph, pw = (pad, pad) if isinstance(pad, int) else pad
+    return [(ky * dil - ph, kx * dil - pw) for ky in range(kh) for kx in range(kw)]
+
+
+# lavb_conv_umma cases of tests/test_gpu_wgmma_contract.py (one call each; the transposed phases are UMMA_CONVT).  Defaults:
+# n 2, 13 x 21 input, cin 64 -> cout 64, 3 x 3 taps with padding 1, stride 1, bias + affine, pre-ReLU, fp32 output.
+UMMA_CASES = {
+    # input strides the product does not use: asymmetric, and the entry's maximum 8 (a 1 x 1 and a 3 x 3 tap set)
+    "in_s21": dict(in_s=(2, 1), hin=17, win=19, cin=128, out="h16"),
+    "in_s13": dict(in_s=(1, 3), hin=11, win=40, res=True, post=True),
+    "in_s8_1x1": dict(in_s=(8, 8), k=1, pad=0, hin=41, win=70, cout=96),
+    "in_s8_3x3": dict(in_s=(8, 8), hin=35, win=131, cin=128, cout=32, out="h16", res=True),
+    # weight rows past cout (cout_mma = 32, 32, 64, 256) hold NaN, which must never reach a stored channel
+    "pad_rows_cout8": dict(cout=8, pad_nan=True),
+    "pad_rows_cout16": dict(cout=16, pad_nan=True, out="h16", pre=False, post=True),
+    "pad_rows_cout40": dict(cout=40, pad_nan=True, out_cs=56, out_off=8),
+    "pad_rows_cout248": dict(cout=248, pad_nan=True, cin=128, out="h16"),
+    # a residual slice (the mutant reads it 8 channels further on) and the sigmoid
+    "res_slice": dict(cout=96, res=True, res_cs=120, res_off=16, post=True, out="h16"),
+    "sigmoid": dict(cout=32, pre=False, sig=True),
+    # one NaN pixel and one +-inf pixel, without / with the ReLUs, both outputs; a negative scale on some channels
+    "nan_plain_f32": dict(nan=True, pre=False, neg_scale=True),
+    "nan_plain_h16": dict(nan=True, pre=False, neg_scale=True, out="h16", res=True),
+    "nan_pre": dict(nan=True, neg_scale=True),
+    "nan_post": dict(nan=True, pre=False, post=True, res=True, out="h16"),
+    "inf_plain_h16": dict(inf=True, pre=False, out="h16"),
+    "inf_pre_post": dict(inf=True, post=True, neg_scale=True),
+    "nan_inf_sigmoid": dict(nan=True, inf=True, pre=False, sig=True, cout=32),
+}
+
+
+class UmmaCase:
+    """the seeded CPU operands of one lavb_conv_umma call, h16 values as the kernel reads them (float32 tensors holding
+    16-bit values of the type ``h16``), and its statement"""
+
+    def __init__(self, name, h16=torch.float16, n=2, hin=13, win=21, cin=64, cout=64, k=3, pad=1, in_s=(1, 1), in_cs=None, in_off=0,
+                 out_cs=None, out_off=0, res=False, res_cs=None, res_off=0, bias=True, affine=True, neg_scale=False, pre=True,
+                 post=False, sig=False, out="f32", nan=False, inf=False, pad_nan=False):
+        g = synth._gen(57, f"umma:{name}")
+        self.name, self.n, self.cin, self.cout, self.in_s, self.out = name, n, cin, cout, in_s, out
+        self.in_off, self.out_off, self.res_off = in_off, out_off, res_off
+        self.in_cs, self.out_cs, self.res_cs = in_cs or cin, out_cs or cout, res_cs or cout
+        self.pre, self.post, self.sig = pre, post, sig
+        self.taps = _taps(k, pad)
+        kh = kw = k
+        self.hog = (hin + 2 * pad - kh) // in_s[0] + 1
+        self.wog = (win + 2 * pad - kw) // in_s[1] + 1
+        rnd = lambda t: t.to(h16).float()                                      # noqa: E731
+        x = torch.randn(n, hin, win, self.in_cs, generator=g)
+        if nan:
+            x[1, hin // 2, win // 3, in_off + 5] = math.nan
+        if inf:
+            x[0, 1, win - 2, in_off + 7] = math.inf
+            x[1, hin - 1, 2, in_off + 60] = -math.inf
+        self.x = rnd(x)
+        cm = (cout + 31) // 32 * 32
+        w = torch.full((len(self.taps), cm, cin), math.nan if pad_nan else 0.0)
+        w[:, :cout] = torch.randn(len(self.taps), cout, cin, generator=g) / (cin * len(self.taps)) ** 0.5
+        self.w = rnd(w)
+        self.bias = torch.randn(cout, generator=g) if bias else None
+        self.scale = torch.rand(cout, generator=g) + 0.5 if affine else None
+        if affine and neg_scale:
+            self.scale[::3] *= -1
+        self.shift = torch.randn(cout, generator=g) if affine else None
+        self.res = rnd(torch.randn(n, self.hog, self.wog, self.res_cs, generator=g)) if res else None
+
+    def want(self, mutant=None):
+        """(n, hog, wog, cout) float64: the statement on the output lattice (out_s 1 here: the whole hog x wog map)"""
+        a = tap_conv64(self.x[..., self.in_off:self.in_off + self.cin].double(), self.taps, self.w[:, :self.cout], self.in_s,
+                       self.hog, self.wog, mutant)
+        ro = self.res_off + (8 if mutant == "res_slice_off8" else 0)
+        r = None if self.res is None else self.res[..., ro:ro + self.cout]
+        v = wgmma_epilogue64(a, self.bias, self.scale, self.shift, r, self.pre, self.post, self.sig, mutant)
+        return store64(v, self.out)
+
+
+# the two UpsamplerBlocks of ERFNet's decoder at the agent's 288 x 256 frames (ConvTranspose2d(k3, s2, p1, op1) + BatchNorm +
+# ReLU: bias, affine and post-ReLU), and the 64 -> 16 one on an odd output (output_padding 0: hout = 2h - 1, wout = 2w - 1),
+# where the odd phases' last row / column falls outside the map
+UMMA_CONVT = {"erf_up128_64": dict(cin=128, cout=64, h=36, w=32, op=1), "erf_up64_16": dict(cin=64, cout=16, h=72, w=64, op=1),
+              "erf_up64_16_odd": dict(cin=64, cout=16, h=9, w=13, op=0)}
+
+
+class ConvTCase:
+    """the seeded CPU operands of one transposed convolution run as four lavb_conv_umma phase calls"""
+
+    def __init__(self, name, h16=torch.float16, cin=64, cout=16, h=9, w=13, op=1, n=2):
+        g = synth._gen(58, f"convT:{name}")
+        rnd = lambda t: t.to(h16).float()                                      # noqa: E731
+        self.n, self.cin, self.cout, self.h, self.w = n, cin, cout, h, w
+        self.hout, self.wout = 2 * h - 1 + op, 2 * w - 1 + op
+        self.x = rnd(torch.randn(n, h, w, cin, generator=g))
+        self.wt = rnd(torch.randn(cin, cout, 3, 3, generator=g) / (cin * 2.25) ** 0.5)
+        self.bias = torch.randn(cout, generator=g)
+        self.scale, self.shift = torch.rand(cout, generator=g) + 0.5, torch.randn(cout, generator=g)
+        self.phases = convT_phases(self.wt)
+
+    def epi(self, a, mutant=None):
+        return wgmma_epilogue64(a, self.bias, self.scale, self.shift, None, False, True, False, mutant)
+
+    def want(self, mutant=None):
+        """(n, hout, wout, cout) float64, fp32 output"""
+        return convT_assemble64(self.x.double(), self.phases, self.hout, self.wout, lambda a: self.epi(a, mutant), mutant)
+
+
+# the mutant each statement must tell apart, and the case it is shown at (the GPU test's inputs)
+WGMMA_MUTANT_CASES = {"k_chunk_dropped": ("umma", "in_s21"), "tap_shifted": ("umma", "pad_rows_cout40"),
+                      "phase_out_o_swapped": ("convT", "erf_up64_16_odd"), "bias_after_pre_relu": ("umma", "in_s13"),
+                      "res_slice_off8": ("umma", "res_slice"), "nan_to_neg_inf": ("umma", "nan_plain_h16")}
+
+
+def pack_d2s(wt, no):
+    """ConvTranspose2d(cin, no, 3, stride 2, padding 1, output_padding 1) weight (cin, no, 3, 3) -> the 2 x 2-tap GEMM operand
+    [tap = dy*2 + dx][column = pos*no + k][cin] of lavb_conv_umma's depth-to-space epilogue (taps (0,0), (0,1), (1,0), (1,1)),
+    zero in the columns past 4 no"""
+    wu = torch.zeros((4, 32, wt.shape[0]), dtype=wt.dtype, device=wt.device)
+    opts = {0: [(0, 1)], 1: [(0, 2), (1, 0)]}
+    for pa in (0, 1):
+        for pb in (0, 1):
+            for dy, ky in opts[pa]:
+                for dx, kx in opts[pb]:
+                    wu[dy * 2 + dx, (pa * 2 + pb) * no:(pa * 2 + pb + 1) * no] = wt[:, :, ky, kx].t()
+    return wu
